@@ -1,8 +1,9 @@
 #!/usr/bin/env python3
-"""bench.py -- megapixels/s of the JPEG encode hot path on N B200s.
+"""bench.py -- megapixels/s of the JPEG encode hot path on N H100s.
 
     python bench.py --gpus N --steps K --warmup W            (ours)
     python bench.py --impl reference --gpus N --steps K --warmup W   (the reference's CPU encoder)
+    python bench.py ... --dump-outputs DIR                   (also write the last timed step's files, see dump_outputs)
 
 A "step" is one pass of the hot path over one batch of synthetic images.
 Default workload = BASELINE.json configs[1]: a batch of 256 synthetic
@@ -64,7 +65,12 @@ def parse():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-parity-gate", action="store_true", help="development only: skip the untimed byte comparison with the reference")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the JPEG files of the last timed end-to-end step (a seeded sample, at most 64 MB) as DIR/*.npy "
+                         "(with --no-e2e: of the untimed end-to-end call the parity gate reads)")
     a = ap.parse_args()
+    if a.steps < 1 or a.warmup < 0:
+        ap.error("--steps must be at least 1 and --warmup at least 0")
     w = WORKLOADS[a.workload]
     a.custom = any(v is not None for v in (a.batch, a.width, a.height, a.switches))
     for k in ("batch", "width", "height", "switches"):
@@ -177,6 +183,25 @@ class ClockSampler:
         sm = [x[0] for x in win]; mx = [x[1] for x in win]; reasons = set(r for x in win for r in x[2])
         return {"sm_mhz": statistics.median(sm) if sm else None, "sm_max_mhz": max(mx) if mx else None,
                 "reasons": sorted(reasons), "samples": len(sm), "source": self.source, "window": window}
+
+
+def power_limit_w(index: int):
+    """The enforced board power limit (W) the numbers were measured at: NVML, else a read-only nvidia-smi query (the
+    device addressed by UUID, like ClockSampler)."""
+    sel = ClockSampler(index).sel
+    try:
+        import pynvml as nv
+        nv.nvmlInit()
+        h = nv.nvmlDeviceGetHandleByUUID(sel) if sel.startswith("GPU-") else nv.nvmlDeviceGetHandleByIndex(index)
+        return nv.nvmlDeviceGetEnforcedPowerLimit(h) / 1000.0
+    except Exception:
+        pass
+    try:
+        r = subprocess.run(["nvidia-smi", "-i", sel, "--query-gpu=power.limit", "--format=csv,noheader,nounits"],
+                           capture_output=True, text=True, timeout=30)
+        return float(r.stdout.strip())
+    except Exception:
+        return None
 
 
 # ---------------------------------------------------------------------------
@@ -430,6 +455,7 @@ def measure(a, sw, enc, host, devbuf, base, rank, world, local, dev, stream, dis
     else:
         step_e2e()                                     # the parity gate needs files
         jpeg_bytes = sum(enc.output_size(i) for i in range(B))
+    outputs = sample_outputs(enc, B) if a.dump_outputs else None
 
     # ---- parity gate (untimed): first and last image of this rank's batch against the reference ----
     gate = None
@@ -437,7 +463,34 @@ def measure(a, sw, enc, host, devbuf, base, rank, world, local, dev, stream, dis
         idx = sorted({0, B - 1})
         gate = parity_gate([enc.get_output(i) for i in idx], [base[i % len(base)] for i in idx], sw, f"rank {rank}, {' '.join(sw)}")
     return {"ms_total": ms_total, "launches": launches, "stages": stages, "chunk": chunk, "clk": clk, "e2e_ms": e2e_ms,
-            "jpeg_bytes": jpeg_bytes, "gate": gate, "B": B}
+            "jpeg_bytes": jpeg_bytes, "gate": gate, "B": B, "outputs": outputs}
+
+
+DUMP_BUDGET = 64_000_000
+
+
+def sample_outputs(enc, B):
+    """The files the encoder's last call returned: every file's size, and the bytes of whole files taken in a fixed
+    seeded order while they fit DUMP_BUDGET as float32 (four bytes per file byte)."""
+    sizes = np.array([enc.output_size(i) for i in range(B)], dtype=np.float64)
+    used = sizes.nbytes + 2 * 4096
+    pick = []
+    for i in np.random.default_rng(0).permutation(B):
+        if used + 8 + 4 * sizes[i] <= DUMP_BUDGET:
+            pick.append(int(i)); used += 8 + 4 * sizes[i]
+    pick.sort()
+    data = np.frombuffer(b"".join(enc.get_output(i) for i in pick), dtype=np.uint8).astype(np.float32)
+    return {"jpeg_sizes": sizes, "jpeg_sample_index": np.array(pick, dtype=np.float64), "jpeg_sample_bytes": data}
+
+
+def dump_outputs(dirpath, outputs):
+    """--dump-outputs: jpeg_sizes (every image of the batch), jpeg_sample_index (images sampled) and jpeg_sample_bytes
+    (their files, concatenated in index order), so that two builds can be compared output for output.  They are the files
+    of the end-to-end path (host pixels in, files out): the resident path, whose time is `value`, runs the same kernels on
+    the same pixels but stops with the entropy-coded bytes in device memory, which the C-ABI does not hand out."""
+    os.makedirs(dirpath, exist_ok=True)
+    for name, arr in outputs.items():
+        np.save(os.path.join(dirpath, name + ".npy"), arr)
 
 
 def main():
@@ -474,7 +527,7 @@ def main():
     B = a.batch if a.scaling == "weak" else (a.batch + world - 1) // world
     global_images = B * world
 
-    # ---- synthetic inputs: `distinct` images per rank, tiled to B (inputs >> 126 MB L2)
+    # ---- synthetic inputs: `distinct` images per rank, tiled to B (inputs >> L2)
     gen = synth_image12 if a.precision == 12 else synth_image
     cache = os.environ.get("B200JPEG_BENCH_CACHE")           # development aid: reuse the synthetic images between A/B runs
     cpath = os.path.join(cache, f"synth_{W}x{H}_{a.precision}_{a.distinct}_{rank}.npy") if cache else None
@@ -520,8 +573,8 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
-    peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6.65 TB/s (B200_PROFILING.md)"
+    peak = float(peaks.get("hbm_gbs", 3350.0))
+    peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "H100 SXM data sheet, 3.35 TB/s"
     out_bytes = r["jpeg_bytes"] / B
     # the dominant stage is launched once per chunk of the batch; its stage time is the sum over the chunks, so
     # (algorithmic bytes of the whole batch) / (summed time) is the mean over launches of bytes-per-launch / duration
@@ -577,8 +630,12 @@ def main():
                    "what": "b200jpeg_start_compress + write_scanlines (all rows, pageable host memory) + finish_compress, one image, median of 4"}
 
     if rank == 0:
+        if a.dump_outputs:
+            dump_outputs(a.dump_outputs, r["outputs"])
+        props = torch.cuda.get_device_properties(local)
         cfg = {"workload": workload_name(a), "images_per_gpu": B, "global_images": global_images,
-               "l2": "inputs (%.1f GB per GPU) exceed the 126 MB L2" % (B * in_bytes / 1e9),
+               "gpu": {"name": props.name, "power_limit_w": power_limit_w(local), "sms": props.multi_processor_count},
+               "l2": "inputs (%.1f GB per GPU) exceed the %.0f MB L2" % (B * in_bytes / 1e9, props.L2_cache_size / 2**20),
                "parallelism": f"images sharded over {world} GPU(s), no data-path collective", "host_affinity": numa,
                "parity_gate": r["gate"]}
         if runs:

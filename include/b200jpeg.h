@@ -1,5 +1,5 @@
 /*
- * b200jpeg.h -- C-ABI of the B200-native JPEG encode hot path.
+ * b200jpeg.h -- C-ABI of the GPU-native (H100) JPEG encode hot path.
  *
  * Drop-in boundary for the encoder pipeline of mozilla/mozjpeg (libjpeg-turbo
  * 3.0.x + Mozilla encoder extensions).  Everything here is `extern "C"`, plain
@@ -10,7 +10,7 @@
  *   1. HOST-ONLY parameter logic (no GPU needed): mirrors the reference's
  *      jcparam.c / jcext.c / jcmaster.c decisions, because the output bytes
  *      depend on them (quant tables, sampling, scan script, pass plan).
- *   2. ENCODE entry points: stage pixels in HBM and run the sm_100a kernels
+ *   2. ENCODE entry points: stage pixels in HBM and run the sm_90a kernels
  *      (colour conversion + downsample, FDCT + quantize + deringing, trellis
  *      quantization, Huffman statistics / optimal tables / bit packing).
  *

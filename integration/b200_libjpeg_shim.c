@@ -12,7 +12,7 @@
  *     jpeg_finish_compress     (jcapimin.c:176-229)
  *     jpeg_write_marker        (jcapimin.c:232-261; segments are spliced in after the file header)
  *
- * and runs the image through the C-ABI of include/b200jpeg.h (sm_100a kernels).
+ * and runs the image through the C-ABI of include/b200jpeg.h (sm_90a kernels).
  * Everything else -- jpeg_create_compress, jpeg_set_defaults, jpeg_set_quality,
  * jpeg_c_set_*_param, destination managers, error handling -- stays the
  * reference's own code, so an unmodified application (the reference's `cjpeg`

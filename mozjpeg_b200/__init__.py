@@ -1,7 +1,7 @@
-"""mozjpeg_b200 -- B200-native JPEG encode hot path behind the reference's API.
+"""mozjpeg_b200 -- GPU-native (H100) JPEG encode hot path behind the reference's API.
 
 Python here is plumbing only: it sequences calls into ``libb200jpeg.so`` (the
-C-ABI of ``include/b200jpeg.h``; hand-written sm_100a kernels).  There is no
+C-ABI of ``include/b200jpeg.h``; hand-written sm_90a kernels).  There is no
 CPU path: importing fails if the library is not built, encoding fails if no
 CUDA device is usable.
 """

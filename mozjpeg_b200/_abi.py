@@ -1,6 +1,6 @@
 """ctypes binding of libb200jpeg.so (the C-ABI in include/b200jpeg.h).
 
-The library is built in-tree by ``__graft_entry__.build()`` (nvcc, sm_100a).
+The library is built in-tree by ``__graft_entry__.build()`` (nvcc, sm_90a).
 There is no fallback: if the shared object is missing the import fails loudly,
 and the encode entry points fail with B200JPEG_ERR_NO_DEVICE when no CUDA
 device is usable.

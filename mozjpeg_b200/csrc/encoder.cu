@@ -90,6 +90,7 @@ struct Arena {
 
 struct b200jpeg_encoder {
   int device = 0;
+  int sms = 0;                       // SM count of `device`, read once at creation (sizes the AC trellis grid)
   cudaStream_t stream = nullptr;     // compute stream (caller-replaceable)
   cudaStream_t s_in = nullptr;       // host->device staging of the pixels
   cudaStream_t s_out = nullptr;      // device->host read-back of the entropy-coded bytes
@@ -566,7 +567,7 @@ static int run_pipeline(b200jpeg_encoder *e, const ChunkIO &io, Timer &tm)
     if (!generic_rounds) {
       tm.mark("trellis_ac");
       if (so.hist) CU(cudaMemsetAsync(A.d_hist.p, 0, hist_bytes, s));
-      launch_trellis_ac3(gr, e->d_tc.as<TrellisConsts>(), tset, tabset, A.d_rec.as<DcRec>(), rlr, A.d_srec.p, A.d_splits.as<uint32_t>(), so, n, s);
+      launch_trellis_ac3(gr, e->d_tc.as<TrellisConsts>(), tset, tabset, A.d_rec.as<DcRec>(), rlr, A.d_srec.p, A.d_splits.as<uint32_t>(), so, n, e->sms, s);
     } else {
       tm.mark("trellis_ac");
       float4 *eo = eobopt ? A.d_eo.as<float4>() : nullptr;
@@ -1054,27 +1055,25 @@ static int choose_chunk(const b200jpeg_encoder *e, const Plan &pl, int n_images,
   if (e->chunk_images_override > 0) return std::min(std::min(n_images, e->chunk_images_override), grid_cap);
   long long per = 0; for (int ci = 0; ci < pl.g.nc; ci++) per += pl.g.c[ci].blocks_per_image;
   // pixels already in HBM: no staging to overlap, so chunks only bound the arenas and give the two compute streams one
-  // large chunk each to run against each other (131 images of 4K 4:2:0: 256 images in chunks of 128 take 26.9 ms on B200,
-  // in chunks of 65 28.1, of 32 29.0; three streams x 86 images 27.5)
+  // large chunk each to run against each other (131 images of 4K 4:2:0: two such arenas fit an 80 GB H100 beside a
+  // resident batch of 256)
   static const long long resident_target = getenv("B200JPEG_RESIDENT_CHUNK_BLOCKS") ? atoll(getenv("B200JPEG_RESIDENT_CHUNK_BLOCKS")) : 25600000LL;
   if (!host_pixels) {
     long long c = std::min<long long>(std::min(n_images, grid_cap), std::max(1LL, resident_target / std::max(1LL, per)));
     // a batch that fits one chunk goes out as two, one per compute stream, when the halves stay large (6.4 M blocks, 33
-    // images of 4K 4:2:0): halves of 64 images run 10 % faster than the whole on one stream (both the baseline and the
-    // progressive profile), halves of 16 images slower (library default profile, 32 x 4K: 36.2 vs 33.9 ms -- the 64
-    // candidate scans' kernels lose more by shrinking than the latency-bound table / layout launches gain by overlapping)
+    // images of 4K 4:2:0); smaller halves are not split: the 64 candidate scans' kernels of the library default profile
+    // lose more by shrinking than the latency-bound table / layout launches gain by overlapping
     if (c >= n_images && e->n_streams > 1 && (long long)n_images * per >= 2 * 6400000LL) c = (n_images + 1) / 2;
     return (int)c;
   }
   // about 1.6 M blocks (8 images of 3840x2160 4:2:0) per chunk: large enough to fill
-  // the 148 SMs several waves deep, small enough that staging the next chunk's
+  // the 132 SMs several waves deep, small enough that staging the next chunk's
   // pixels overlaps this chunk's kernels.
   static const long long target = getenv("B200JPEG_CHUNK_BLOCKS") ? atoll(getenv("B200JPEG_CHUNK_BLOCKS")) : 1600000LL;
   long long c = std::max(1LL, target / std::max(1LL, per));
   // scan search: the 64 candidate scans make the device the slower side (1 ms per 4K image against 0.45 ms of staging) and
   // launch ~700 kernels per chunk, so chunks are four times larger, but a batch still goes out in at least two so that the
-  // second half's staging hides behind the first half's kernels (32 x 4K end to end on B200: chunks of 8 / 16 / 32 images
-  // 51.4 / 41.2 / 45.7 ms)
+  // second half's staging hides behind the first half's kernels
   if (pl.search) c = std::max(1LL, std::min(4 * c, ((long long)n_images + 1) / 2));
   return (int)std::min<long long>(std::min(n_images, grid_cap), c);
 }
@@ -1258,6 +1257,7 @@ int b200jpeg_encoder_create(b200jpeg_encoder **enc, int device)
   CU(cudaSetDevice(device));
   b200jpeg_encoder *o = new b200jpeg_encoder();
   o->device = device;
+  if ((e = cudaDeviceGetAttribute(&o->sms, cudaDevAttrMultiProcessorCount, device)) != cudaSuccess) { set_error("cudaDeviceGetAttribute failed: %s", cudaGetErrorString(e)); delete o; return B200JPEG_ERR_CUDA; }
   cudaError_t e2 = cudaStreamCreateWithFlags(&o->stream, cudaStreamNonBlocking);
   if (e2 == cudaSuccess) e2 = cudaStreamCreateWithFlags(&o->s_in, cudaStreamNonBlocking);
   if (e2 == cudaSuccess) e2 = cudaStreamCreateWithFlags(&o->s_out, cudaStreamNonBlocking);

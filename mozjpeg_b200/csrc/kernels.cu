@@ -1,5 +1,5 @@
-// kernels.cu -- sm_100a kernels of the JPEG-encode hot path (see kernels.cuh).
-// Compile with: -gencode arch=compute_100a,code=sm_100a -fmad=false -lineinfo
+// kernels.cu -- sm_90a kernels of the JPEG-encode hot path (see kernels.cuh).
+// Compile with: -gencode arch=compute_90a,code=sm_90a -fmad=false -lineinfo
 #include "kernels.cuh"
 #include <cuda_fp16.h>
 #include <cuda.h>           // CUtensorMap (the encode function itself is fetched through the runtime, no libcuda link)
@@ -885,9 +885,9 @@ __global__ void __launch_bounds__(128, FWD_MIN_CTAS) k_forward_tile(Geom g, cons
       const int4 *rows = reinterpret_cast<const int4 *>(reinterpret_cast<const int16_t *>(sW + b * 72));
       float norm = 0.0f; int raw_dc = 0;
       // (float)(v * v) without the conversion unit: v as an exact float by the exponent trick, squared in fp32 -- the
-      // product of two 16-bit integers rounds to the same float as the converted integer square; two values per
-      // packed fp32x2 operation, the sum itself stays the reference's serial chain
-      const float2 bias = make_float2(-8421376.0f, -8421376.0f);   // -(2^23 + 2^15)
+      // product of two 16-bit integers rounds to the same float as the converted integer square; the sum itself
+      // stays the reference's serial chain
+      const float bias = -8421376.0f;   // -(2^23 + 2^15)
 #pragma unroll
       for (int r = 0; r < 8; r++) {
         const int4 rv = rows[r];
@@ -895,8 +895,9 @@ __global__ void __launch_bounds__(128, FWD_MIN_CTAS) k_forward_tile(Geom g, cons
 #pragma unroll
         for (int cp = 0; cp < 4; cp++) {
           const unsigned u = pw[cp] ^ 0x80008000u;
-          float2 f = make_float2(__uint_as_float(__byte_perm(u, 0x4B000000u, 0x7610)), __uint_as_float(__byte_perm(u, 0x4B000000u, 0x7632)));
-          f = __fadd2_rn(f, bias); f = __fmul2_rn(f, f);
+          float2 f = make_float2(__fadd_rn(__uint_as_float(__byte_perm(u, 0x4B000000u, 0x7610)), bias),
+                                 __fadd_rn(__uint_as_float(__byte_perm(u, 0x4B000000u, 0x7632)), bias));
+          f.x = __fmul_rn(f.x, f.x); f.y = __fmul_rn(f.y, f.y);
           if (r == 0 && cp == 0) raw_dc = (int)(int16_t)(pw[0] & 0xFFFFu); else norm += f.x;
           norm += f.y;
         }
@@ -1365,9 +1366,8 @@ __device__ __forceinline__ void walk_seq_rec(const Geom &g, const ScanDesc &sd, 
 // ---------------------------------------------------------------------
 // shared-memory histogram increment (warp-aggregating the atomics per counter was measured slower).  A few symbols
 // (EOB, 0x01, 0x11, 0x02) make up most of a scan, so the lanes of a warp mostly hit the same few counters; keeping
-// GATHER_COPIES copies of the histograms per CTA (a thread uses copy lane mod copies) was measured on B200: no gain with
-// 4 or 8 copies in the per-component kernel (0.52 vs 0.54 ms per 64 4K images), a loss in the per-scan kernels whose
-// copies are 8 KB each (0.97 vs 0.53 ms) -- same-counter serialisation is not what bounds these kernels.  Default 1.
+// GATHER_COPIES copies of the histograms per CTA (a thread uses copy lane mod copies) is a build-time option; the
+// per-scan kernels' copies are 8 KB each, so more copies cost occupancy there.  Default 1 (not re-measured on H100).
 #ifndef GATHER_COPIES
 #define GATHER_COPIES 1
 #endif
@@ -2171,8 +2171,7 @@ k_trellis_ac3(Geom g, const TrellisConsts *__restrict__ tc, const DevHuff *__res
     // (a warp whose 32 blocks have no entry at all -- the tail of the sorted order -- needs neither the prefix nor the search)
     if (mmax != 0) {
       uint2 *push = myrec;
-      const float2 l2 = make_float2(lambda, lambda);
-      const float2 bias = make_float2(-8421376.0f, -8421376.0f);   // -(2^23 + 2^15): undoes the exponent trick and the +32768 offset
+      const float bias = -8421376.0f;   // -(2^23 + 2^15): undoes the exponent trick and the +32768 offset
 #pragma unroll
       for (int v = 0; v < 8; v++) {
         const unsigned aw[4] = {rv[v].x, rv[v].y, rv[v].z, rv[v].w};
@@ -2182,9 +2181,10 @@ k_trellis_ac3(Geom g, const TrellisConsts *__restrict__ tc, const DevHuff *__res
 #pragma unroll
         for (int jj = 0; jj < 4; jj++) {
           const unsigned u = aw[jj] ^ 0x80008000u;               // both halves + 32768
-          float2 f = make_float2(__uint_as_float(__byte_perm(u, 0x4B000000u, 0x7610)), __uint_as_float(__byte_perm(u, 0x4B000000u, 0x7632)));
-          f = __fadd2_rn(f, bias);                               // the raw values as floats, exact
-          const float2 z = __fmul2_rn(__fmul2_rn(__fmul2_rn(f, f), l2), make_float2(ww[2 * jj], ww[2 * jj + 1]));
+          const float fx = __fadd_rn(__uint_as_float(__byte_perm(u, 0x4B000000u, 0x7610)), bias);   // the raw values as floats, exact
+          const float fy = __fadd_rn(__uint_as_float(__byte_perm(u, 0x4B000000u, 0x7632)), bias);
+          const float2 z = make_float2(__fmul_rn(__fmul_rn(__fmul_rn(fx, fx), lambda), ww[2 * jj]),
+                                       __fmul_rn(__fmul_rn(__fmul_rn(fy, fy), lambda), ww[2 * jj + 1]));
           const int i = 8 * v + 2 * jj;
           if (i != 0) {
             // entry word: position | raw value << 16 (one byte permute)
@@ -2363,7 +2363,7 @@ static void launch_t3(dim3 grid, cudaStream_t s, const Geom &g, const TrellisCon
   k_trellis_ac3<MM><<<grid, T3_THREADS, sizeof(T3Smem<MM>), s>>>(g, tc, tabs, tabs_set_stride, rec, rl, srec, splits, so); LAUNCHED();
 }
 void launch_trellis_ac3(const Geom &g, const TrellisConsts *tc, const DevHuff *tabs, size_t tabs_set_stride,
-                        DcRec *rec, const RecLayout &rl, void *srec, uint32_t *splits, const SymOut &so, int n, cudaStream_t s)
+                        DcRec *rec, const RecLayout &rl, void *srec, uint32_t *splits, const SymOut &so, int n, int sms, cudaStream_t s)
 {
   // splits: 4 words per (image, component), followed by the sort's scratch counters (2 x 64 words each)
   launch_sort2(g, rec, rl, static_cast<SRec *>(srec), splits, splits + (size_t)n * g.nc * 4, 15, n, s);
@@ -2371,7 +2371,7 @@ void launch_trellis_ac3(const Geom &g, const TrellisConsts *tc, const DevHuff *t
   for (int ci = 0; ci < g.nc; ci++) mb = max(mb, (long long)g.c[ci].wib * g.c[ci].hib);
   const unsigned full = (unsigned)((mb + T3_THREADS - 1) / T3_THREADS);
   // CTAs loop over their class's chunks: enough of them per (image, component) to fill the device, few enough to amortise the tables
-  unsigned gx = (unsigned)max(1, min((int)full, (148 * 8 * 3 + n * g.nc - 1) / (n * g.nc)));
+  unsigned gx = (unsigned)max(1, min((int)full, (sms * 8 * 3 + n * g.nc - 1) / (n * g.nc)));
   dim3 grid(gx, n * g.nc);
   const SRec *sr = static_cast<const SRec *>(srec);
   // largest blocks first: the classes touch disjoint blocks.  The two big-list classes hold 2 / 4 CTAs per SM (96 / 48 KB of

@@ -1,4 +1,4 @@
-// kernels.cuh -- sm_100a device code of the JPEG-encode hot path.
+// kernels.cuh -- sm_90a device code of the JPEG-encode hot path.
 //
 // Everything here is integer / bit-serial or un-fused fp32 work: no tensor
 // cores.  The file is compiled with -fmad=false because the trellis rate/
@@ -147,7 +147,7 @@ void launch_gen_tables(const uint32_t *hist, DevHuff *tabs, size_t tabs_set_stri
 // splits: 4 class boundaries per (image, component) followed by 128 words of sorting counters each) and runs one
 // class-specific kernel per count class
 void launch_trellis_ac3(const Geom &g, const TrellisConsts *tc, const DevHuff *tabs, size_t tabs_set_stride,
-                        DcRec *rec, const RecLayout &rl, void *srec, uint32_t *splits, const SymOut &so, int n, cudaStream_t s);
+                        DcRec *rec, const RecLayout &rl, void *srec, uint32_t *splits, const SymOut &so, int n, int sms, cudaStream_t s);
 // use_scans_in_trellis: quantize_trellis restricted to the zigzag band [Ss, Se]
 void launch_trellis_ac_band(const Geom &g, const TrellisConsts *tc, const DevHuff *tabs, size_t tabs_set_stride,
                             DcRec *rec, const RecLayout &rl, int Ss, int Se, const uint16_t *qimg, float4 *eo, int n, cudaStream_t s);

@@ -23,7 +23,7 @@ void set_error(const char *fmt, ...) {
 extern "C" {
 
 const char *b200jpeg_last_error(void) { return b200::g_last_error; }
-const char *b200jpeg_version(void) { return "b200jpeg 0.1 (sm_100a)"; }
+const char *b200jpeg_version(void) { return "b200jpeg 0.1 (sm_90a)"; }
 
 const unsigned int *b200jpeg_std_quant_tbl(int set_idx, int chroma) {
   static unsigned int tmp[9][2][64];

@@ -61,13 +61,18 @@ def _bench_module():
     return m
 
 
-def test_clock_sampler_window_and_fallback():
+def test_clock_sampler_window_and_fallback(monkeypatch):
     """bench.py's `clocks` entry: the samples between the two marks are the ones reported (median SM clock, union of the
     throttle reasons), a timed region shorter than one sampling period falls back to warm-up + timed region and says so,
     and a box without NVML / nvidia-smi yields a null entry instead of an exception."""
     b = _bench_module()
+
+    def no_smi(*args, **kw):
+        raise FileNotFoundError("nvidia-smi")
+    monkeypatch.setitem(sys.modules, "pynvml", None)      # neither source comes up, whether or not this box has a GPU
+    monkeypatch.setattr(b.subprocess, "Popen", no_smi)
     c = b.ClockSampler(0)
-    c.start(); out = c.stop(0, None)                      # no GPU here: neither source comes up
+    c.start(); out = c.stop(0, None)
     assert out["samples"] == 0 and out["sm_mhz"] is None
     c = b.ClockSampler(0); c.source = "nvml"
     c.samples = [(1500.0, 1965.0, ()), (1600.0, 1965.0, ())]                       # warm-up

@@ -14,6 +14,7 @@ for r in rows:
     if name not in per: per[name] = [0, 0.0, r[8], r[7]]; order.append(name)
     per[name][0] += 1; per[name][1] += ns
 tot = sum(v[1] for v in per.values())
+os.makedirs(os.path.join(ROOT, "profiles"), exist_ok=True)      # git-ignored output directory
 out = os.path.join(ROOT, "profiles", f"{rnd}_launches_{tag}.md")
 with open(out, "w") as f:
     f.write(f"# ncu launch list `{tag}` (`tools/profile.sh {tag}`: bench.py --batch 16 --steps 1 --warmup 1, every launch, "

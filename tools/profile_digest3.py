@@ -35,6 +35,7 @@ for name, p in per.items():
     s = stages.setdefault(stage_of(name), {"ns": 0.0, "bytes": 0.0}); s["ns"] += p["ns"]; s["bytes"] += p["rd"] + p["wr"]
 # the bench step runs W warm-up + K timed + one single-stream pass: every kernel appears (launches / images-per-chunk) times
 passes = max(1, min(p["n"] for n_, p in per.items() if n_.startswith("k_forward")) if any(n_.startswith("k_forward") for n_ in per) else 1)
+os.makedirs(os.path.join(ROOT, "profiles"), exist_ok=True)      # git-ignored output directory
 out = os.path.join(ROOT, "profiles", f"{rnd}_launches_{tag}.md")
 with open(out, "w") as f:
     f.write(f"# ncu launch list `{tag}` (`tools/profile3.sh {tag}`: bench.py --batch {nimg} --steps 1 --warmup 1, every launch, "
