@@ -35,6 +35,7 @@ extern "C" {
 
 /* J_COLOR_SPACE subset (jpeglib.h:243-266), same numeric values. */
 enum { B200JPEG_CS_UNKNOWN = 0, B200JPEG_CS_GRAYSCALE = 1, B200JPEG_CS_RGB = 2, B200JPEG_CS_YCbCr = 3,
+       B200JPEG_CS_CMYK = 4, B200JPEG_CS_YCCK = 5,   /* 4 samples per pixel; CMYK -> YCCK as Adobe defines it (jccolor.c:395-441) */
        /* input pixel orders of the RGB family (in_color_space only; jccolor.c:253-291 dispatches them into jccolext.c:30-75):
         * 3 samples per pixel for EXT_RGB / EXT_BGR, 4 for the others (the filler / alpha sample is ignored) */
        B200JPEG_CS_EXT_RGB = 6, B200JPEG_CS_EXT_RGBX = 7, B200JPEG_CS_EXT_BGR = 8, B200JPEG_CS_EXT_BGRX = 9,
@@ -93,7 +94,7 @@ typedef struct {
   /* source image (jpeglib.h:396-402) */
   int image_width, image_height;
   int input_components;
-  int in_color_space;                     /* B200JPEG_CS_GRAYSCALE / RGB / YCbCr or one of the B200JPEG_CS_EXT_* pixel orders */
+  int in_color_space;                     /* B200JPEG_CS_* (UNKNOWN: input_components samples, 1 to 4, passed through) */
   int data_precision;                     /* 8, or 12 (samples in uint16; trellis and deringing off, as the reference requires) */
   /* JPEG parameters */
   int jpeg_color_space;

@@ -193,6 +193,9 @@ static int fill_params(j_compress_ptr cinfo, boolean write_all_tables, b200jpeg_
   case JCS_GRAYSCALE: p->in_color_space = B200JPEG_CS_GRAYSCALE; break;
   case JCS_RGB: case JCS_EXT_RGB: p->in_color_space = B200JPEG_CS_RGB; break;
   case JCS_YCbCr: p->in_color_space = B200JPEG_CS_YCbCr; break;
+  case JCS_CMYK: p->in_color_space = B200JPEG_CS_CMYK; break;
+  case JCS_YCCK: p->in_color_space = B200JPEG_CS_YCCK; break;
+  case JCS_UNKNOWN: p->in_color_space = B200JPEG_CS_UNKNOWN; break;
   /* the other pixel orders of the RGB family (jccolor.c:253-291): same numeric values as J_COLOR_SPACE */
   case JCS_EXT_RGBX: case JCS_EXT_BGR: case JCS_EXT_BGRX: case JCS_EXT_XBGR: case JCS_EXT_XRGB:
   case JCS_EXT_RGBA: case JCS_EXT_BGRA: case JCS_EXT_ABGR: case JCS_EXT_ARGB:
@@ -203,6 +206,9 @@ static int fill_params(j_compress_ptr cinfo, boolean write_all_tables, b200jpeg_
   case JCS_GRAYSCALE: p->jpeg_color_space = B200JPEG_CS_GRAYSCALE; break;
   case JCS_YCbCr: p->jpeg_color_space = B200JPEG_CS_YCbCr; break;
   case JCS_RGB: p->jpeg_color_space = B200JPEG_CS_RGB; break;
+  case JCS_CMYK: p->jpeg_color_space = B200JPEG_CS_CMYK; break;
+  case JCS_YCCK: p->jpeg_color_space = B200JPEG_CS_YCCK; break;
+  case JCS_UNKNOWN: p->jpeg_color_space = B200JPEG_CS_UNKNOWN; break;
   default: return 0;
   }
   p->image_width = (int)cinfo->image_width;   p->image_height = (int)cinfo->image_height;

@@ -114,7 +114,8 @@ class Encoder:
         A.check(_lib.b200jpeg_start_compress(self._h, C.byref(p)), "start_compress")
 
     def write_scanlines(self, rows: np.ndarray) -> int:
-        r = np.ascontiguousarray(rows, dtype=np.uint8)
+        """rows: (n, W, C) or one (W, C) row of uint8 samples, or of uint16 holding 12-bit samples (J12SAMPLE rows)."""
+        r = np.ascontiguousarray(rows, dtype=np.uint16 if np.asarray(rows).dtype == np.uint16 else np.uint8)
         if r.ndim == 2:
             r = r[None]
         ptrs = (C.POINTER(C.c_uint8) * r.shape[0])()
@@ -168,13 +169,15 @@ def cjpeg(switches: Sequence[str], ppm: bytes, encoder: Optional[Encoder] = None
 
 
 def tj3_params(width: int, height: int, quality: int = 75, subsamp: str = "420", optimize: bool = False,
-               progressive: bool = False, gray_input: bool = False) -> Params:
+               progressive: bool = False, gray_input: bool = False, cmyk: bool = False, colorspace: int = None) -> Params:
     """The parameter block tj3Compress8 builds (turbojpeg.c:330-397
     setCompDefaults): JCP_FASTEST, quality via jpeg_set_quality(.., TRUE),
-    YCbCr (or grayscale) with the luma sampling factors of TJSAMP_*."""
+    YCbCr (or grayscale) with the luma sampling factors of TJSAMP_*.
+    cmyk: TJPF_CMYK pixels, written as YCCK unless ``colorspace`` (TJPARAM_COLORSPACE as a CS_* value) says
+    otherwise; component 3 gets the luma sampling factors."""
     p = Params()
-    p.in_color_space = A.CS_GRAYSCALE if gray_input else A.CS_RGB
-    p.input_components = 1 if gray_input else 3
+    p.in_color_space = A.CS_GRAYSCALE if gray_input else (A.CS_CMYK if cmyk else A.CS_RGB)
+    p.input_components = 1 if gray_input else (4 if cmyk else 3)
     p.data_precision = 8
     p.image_width, p.image_height = width, height
     _lib.b200jpeg_set_defaults(C.byref(p), A.PROFILE_FASTEST)
@@ -182,11 +185,15 @@ def tj3_params(width: int, height: int, quality: int = 75, subsamp: str = "420",
     p.optimize_coding = int(optimize)
     _lib.b200jpeg_set_quality(C.byref(p), quality, 1)
     gray = gray_input or subsamp == "gray"
-    A.check(_lib.b200jpeg_set_colorspace(C.byref(p), A.CS_GRAYSCALE if gray else A.CS_YCbCr), "set_colorspace")
+    if colorspace is None:
+        colorspace = A.CS_GRAYSCALE if gray else (A.CS_YCCK if cmyk else A.CS_YCbCr)
+    A.check(_lib.b200jpeg_set_colorspace(C.byref(p), colorspace), "set_colorspace")
     if progressive:
         A.check(_lib.b200jpeg_simple_progression(C.byref(p)), "simple_progression")
     hv = {"444": (1, 1), "422": (2, 1), "420": (2, 2), "440": (1, 2), "411": (4, 1), "441": (1, 4), "gray": (1, 1)}[subsamp]
     p.comp_info[0].h_samp_factor, p.comp_info[0].v_samp_factor = hv
     for ci in range(1, p.num_components):
         p.comp_info[ci].h_samp_factor = p.comp_info[ci].v_samp_factor = 1
+    if p.num_components > 3:
+        p.comp_info[3].h_samp_factor, p.comp_info[3].v_samp_factor = hv
     return p

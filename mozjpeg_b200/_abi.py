@@ -20,7 +20,7 @@ NUM_QUANT_TBLS = 4
 NUM_HUFF_TBLS = 4
 MAX_SCANS = 64
 
-CS_UNKNOWN, CS_GRAYSCALE, CS_RGB, CS_YCbCr = 0, 1, 2, 3
+CS_UNKNOWN, CS_GRAYSCALE, CS_RGB, CS_YCbCr, CS_CMYK, CS_YCCK = 0, 1, 2, 3, 4, 5
 # input pixel orders of the RGB family (J_COLOR_SPACE values, jpeglib.h:243-266): name -> (value, samples per pixel, R, G, B offsets)
 CS_EXT = {"EXT_RGB": (6, 3, 0, 1, 2), "EXT_RGBX": (7, 4, 0, 1, 2), "EXT_BGR": (8, 3, 2, 1, 0), "EXT_BGRX": (9, 4, 2, 1, 0),
           "EXT_XBGR": (10, 4, 3, 2, 1), "EXT_XRGB": (11, 4, 1, 2, 3), "EXT_RGBA": (12, 4, 0, 1, 2), "EXT_BGRA": (13, 4, 2, 1, 0),

@@ -289,8 +289,13 @@ def _parse(p: A.Params, argv: Sequence[str], for_real: bool) -> None:
 
 
 def params_from_switches(switches: Sequence[str], width: int, height: int,
-                         input_components: int = 3) -> A.Params:
-    """What cjpeg's cinfo looks like at jpeg_start_compress for ``switches``."""
+                         input_components: int = 3, in_color_space: int = None,
+                         jpeg_color_space: int = None) -> A.Params:
+    """What cjpeg's cinfo looks like at jpeg_start_compress for ``switches``.
+
+    ``in_color_space`` (default: grayscale for 1 component, else RGB) is what the image header reports, e.g.
+    CS_CMYK for a 4-sample CMYK source; ``jpeg_color_space`` is a jpeg_set_colorspace call made right after
+    jpeg_default_colorspace, before the switches are applied for real."""
     lib = A.load()
     p = A.Params()
     p.in_color_space = A.CS_RGB
@@ -299,10 +304,14 @@ def params_from_switches(switches: Sequence[str], width: int, height: int,
     lib.b200jpeg_set_defaults(C.byref(p), A.PROFILE_MAX_COMPRESSION)
     _parse(p, list(switches), False)
     # image header (rdppm.c start_input_ppm): P5 -> grayscale, P6 -> RGB
-    p.in_color_space = A.CS_GRAYSCALE if input_components == 1 else A.CS_RGB
+    if in_color_space is None:
+        in_color_space = A.CS_GRAYSCALE if input_components == 1 else A.CS_RGB
+    p.in_color_space = in_color_space
     p.input_components = input_components
     p.image_width, p.image_height = width, height
     A.check(lib.b200jpeg_default_colorspace(C.byref(p)), "default_colorspace")
+    if jpeg_color_space is not None:
+        A.check(lib.b200jpeg_set_colorspace(C.byref(p), jpeg_color_space), "set_colorspace")
     _parse(p, list(switches), True)
     # jpeg_start_compress (jcapistd.c:53-56)
     if p.num_scans == 0:

@@ -162,7 +162,8 @@ static int build_plan(const b200jpeg_params *p, size_t row_pitch, size_t image_s
   const bool rgb_in = B200JPEG_CS_IS_RGB(p->in_color_space);
   if (rgb_in && p->jpeg_color_space == B200JPEG_CS_YCbCr) g.cs_mode = 0;
   else if (rgb_in && p->jpeg_color_space == B200JPEG_CS_GRAYSCALE) g.cs_mode = 1;
-  else g.cs_mode = 2;
+  else if (p->in_color_space == B200JPEG_CS_CMYK && p->jpeg_color_space == B200JPEG_CS_YCCK) g.cs_mode = 3;
+  else g.cs_mode = 2;                               // RGB->RGB, gray, YCbCr->YCbCr/gray, CMYK, YCCK, UNKNOWN: null_convert
   g.px_first = rgb_in ? B200JPEG_CS_FIRST(p->in_color_space) : 0;             // jccolor.c:253-291 (JCS_EXT_* pixel orders)
   g.px_swap = rgb_in ? B200JPEG_CS_BLUE_FIRST(p->in_color_space) : 0;
   pl.max_real_blocks = 0; pl.sum_real_blocks = 0;
@@ -704,7 +705,7 @@ static void write_file_header(const b200jpeg_params *p, Bytes o)                
   }
   if (p->write_Adobe_marker) {                                                        // :564-620
     o.w(0xFFEE); o.w(14); o.b('A'); o.b('d'); o.b('o'); o.b('b'); o.b('e'); o.w(100); o.w(0); o.w(0);
-    o.b(p->jpeg_color_space == B200JPEG_CS_YCbCr ? 1 : 0);
+    o.b(p->jpeg_color_space == B200JPEG_CS_YCbCr ? 1 : p->jpeg_color_space == B200JPEG_CS_YCCK ? 2 : 0);   // colour transform
   }
 }
 static void write_frame_header(const b200jpeg_params *p, bool progressive, Bytes o)   // jcmarker.c:674-735

@@ -48,15 +48,28 @@ __device__ __forceinline__ int nbits_of(int v) { return 32 - __clz(v); }   // v 
 //     jcprepct.c:135-192 (edge rules), jcdctmgr.c:416-498,576-604,611-682,
 //     693-772, jfdctint.c:142-286.
 // =====================================================================
+// Component `comp` (in the JPEG colour space) of the pixel at `px`; SB = bytes per sample (1: 8-bit, 2: 12-bit uint16).
+//   cs_mode 0: rgb_ycc_convert (jccolext.c:30-75)   1: rgb_gray_convert (Y only)
+//           2: null_convert / grayscale_convert (sample `comp`)   3: cmyk_ycck_convert (jccolor.c:395-441)
 // first / swap: where the three colour samples sit inside an RGB-family pixel (jccolor.c:253-291, the JCS_EXT_* orders):
-// they start at sample `first` and are stored blue-first when `swap` is set; other inputs have first = swap = 0
-__device__ __forceinline__ int load_component(const uint8_t *__restrict__ px, int cs_mode, int comp, int first, int swap)
+// they start at sample `first` and are stored blue-first when `swap` is set; other inputs have first = swap = 0.
+// 12-bit samples are masked like the reference's RANGE_LIMIT (jccolext.c:52-54), except YCCK's K, which passes through
+// as is (jccolor.c:420).  The fixed-point sums equal the reference's rgb_ycc_tab lookups.
+template <int SB>
+__device__ __forceinline__ int convert_sample(const uint8_t *__restrict__ px, int cs_mode, int comp, int first, int swap)
 {
-  if (cs_mode == 2) return px[first + (swap ? 2 - comp : comp)];
-  int r = px[first + (swap ? 2 : 0)], g = px[first + 1], b = px[first + (swap ? 0 : 2)];
+  constexpr int MAXJ = SB == 1 ? 255 : 4095, CENTRE = (MAXJ + 1) / 2;
+  auto smp = [&](int k) -> int { return SB == 1 ? (int)px[k] : (int)(reinterpret_cast<const uint16_t *>(px)[k] & 0xFFF); };
+  if (cs_mode == 2 || comp == 3) {                 // component 3 exists in modes 2 and 3 only
+    const int k = first + (swap ? 2 - comp : comp);
+    return SB == 1 || cs_mode == 2 ? smp(k) : (int)reinterpret_cast<const uint16_t *>(px)[k];
+  }
+  // cmyk_ycck_convert: R, G, B = MAXJSAMPLE - C, M, Y, which is an XOR for samples in 0..MAXJSAMPLE
+  const int inv = cs_mode == 3 ? MAXJ : 0;
+  const int r = smp(first + (swap ? 2 : 0)) ^ inv, g = smp(first + 1) ^ inv, b = smp(first + (swap ? 0 : 2)) ^ inv;
   if (comp == 0) return (19595 * r + 38470 * g + 7471 * b + 32768) >> 16;
-  if (comp == 1) return (-11059 * r - 21709 * g + 32768 * b + (128 << 16) + 32767) >> 16;
-  return (32768 * r - 27439 * g - 5329 * b + (128 << 16) + 32767) >> 16;
+  if (comp == 1) return (-11059 * r - 21709 * g + 32768 * b + (CENTRE << 16) + 32767) >> 16;
+  return (32768 * r - 27439 * g - 5329 * b + (CENTRE << 16) + 32767) >> 16;
 }
 
 #define DESCALE(x, n) (((x) + (1 << ((n) - 1))) >> (n))
@@ -234,17 +247,7 @@ __global__ void __launch_bounds__(128) k_forward(Geom g, const uint8_t *__restri
   const uint8_t *base = src + (size_t)img * g.image_stride;
   int ws[64];
   const int comp = g.cs_mode == 1 ? 0 : ci;
-  // one component sample of the pixel at `px` (12-bit samples are masked like the reference's RANGE_LIMIT, jccolext.c:52-54)
-  auto component = [&](const uint8_t *px) -> int {
-    if (SB == 1) return load_component(px, g.cs_mode, comp, g.px_first, g.px_swap);
-    const uint16_t *q = reinterpret_cast<const uint16_t *>(px);
-    const int first = g.px_first, swap = g.px_swap;
-    if (g.cs_mode == 2) return q[first + (swap ? 2 - comp : comp)] & 0xFFF;
-    const int r = q[first + (swap ? 2 : 0)] & 0xFFF, gg = q[first + 1] & 0xFFF, bb = q[first + (swap ? 0 : 2)] & 0xFFF;
-    if (comp == 0) return (19595 * r + 38470 * gg + 7471 * bb + 32768) >> 16;
-    if (comp == 1) return (-11059 * r - 21709 * gg + 32768 * bb + (CENTRE << 16) + 32767) >> 16;
-    return (32768 * r - 27439 * gg - 5329 * bb + (CENTRE << 16) + 32767) >> 16;
-  };
+  auto component = [&](const uint8_t *px) -> int { return convert_sample<SB>(px, g.cs_mode, comp, g.px_first, g.px_swap); };
 #pragma unroll
   for (int y = 0; y < 8; y++) {
     int yo = by * 8 + y;
@@ -999,17 +1002,9 @@ __global__ void __launch_bounds__(128) k_prep_planes(Geom g, const uint8_t *__re
   if (xo >= c.wib * 8 || yo >= c.hib * 8) return;
   const uint8_t *base = src + (size_t)img * g.image_stride;
   const int comp = g.cs_mode == 1 ? 0 : ci;
-  constexpr int CENTRE = SB == 1 ? 128 : 2048;
   auto at = [&](int y, int x) -> int {
     y = max(0, min(y, g.H - 1)); x = max(0, min(x, g.W - 1));
-    const uint8_t *px = base + (size_t)y * g.row_pitch + (size_t)x * g.in_comps * SB;
-    auto smp = [&](int k) -> int { return SB == 1 ? (int)px[k] : (int)(reinterpret_cast<const uint16_t *>(px)[k] & 0xFFF); };
-    const int f0 = g.px_first, sw = g.px_swap;
-    if (g.cs_mode == 2) return smp(f0 + (sw ? 2 - comp : comp));
-    const int r = smp(f0 + (sw ? 2 : 0)), gg = smp(f0 + 1), b = smp(f0 + (sw ? 0 : 2));
-    if (comp == 0) return (19595 * r + 38470 * gg + 7471 * b + 32768) >> 16;
-    if (comp == 1) return (-11059 * r - 21709 * gg + 32768 * b + (CENTRE << 16) + 32767) >> 16;
-    return (32768 * r - 27439 * gg - 5329 * b + (CENTRE << 16) + 32767) >> 16;
+    return convert_sample<SB>(base + (size_t)y * g.row_pitch + (size_t)x * g.in_comps * SB, g.cs_mode, comp, g.px_first, g.px_swap);
   };
   int val;
   if (c.hx == 1 && c.vx == 1) {

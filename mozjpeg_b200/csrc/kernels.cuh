@@ -38,7 +38,7 @@ struct Geom {
   int mcus_per_row, mcu_rows;
   int in_comps;        // samples per input pixel
   int max_coef_bits;   // data_precision + 2
-  int cs_mode;         // 0: RGB->YCbCr  1: RGB->gray  2: pass-through
+  int cs_mode;         // 0: RGB->YCbCr  1: RGB->gray  2: pass-through (sample ci of the pixel)  3: CMYK->YCCK
   int px_first, px_swap; // RGB-family pixel order (JCS_EXT_*): first colour sample inside the pixel, blue-first storage
   size_t row_pitch, image_stride;
   // raw-data input (jpeg_write_raw_data, jcapistd.c:145-195): downsampled component planes instead of pixels;

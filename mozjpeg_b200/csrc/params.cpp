@@ -104,6 +104,19 @@ int b200jpeg_set_colorspace(b200jpeg_params *p, int colorspace) {
   case B200JPEG_CS_YCbCr:
     p->write_JFIF_header = 1; p->num_components = 3;
     set_comp(p, 0, 1, 2, 2, 0, 0, 0); set_comp(p, 1, 2, 1, 1, 1, 1, 1); set_comp(p, 2, 3, 1, 1, 1, 1, 1); break;
+  case B200JPEG_CS_CMYK:
+    p->write_Adobe_marker = 1; p->num_components = 4;
+    set_comp(p, 0, 0x43, 1, 1, 0, 0, 0); set_comp(p, 1, 0x4D, 1, 1, 0, 0, 0); set_comp(p, 2, 0x59, 1, 1, 0, 0, 0); set_comp(p, 3, 0x4B, 1, 1, 0, 0, 0); break;
+  case B200JPEG_CS_YCCK:
+    p->write_Adobe_marker = 1; p->num_components = 4;
+    set_comp(p, 0, 1, 2, 2, 0, 0, 0); set_comp(p, 1, 2, 1, 1, 1, 1, 1); set_comp(p, 2, 3, 1, 1, 1, 1, 1); set_comp(p, 3, 4, 2, 2, 0, 0, 0); break;
+  case B200JPEG_CS_UNKNOWN:
+    p->num_components = p->input_components;
+    // MAX_COMPONENTS is 10 in the reference (JERR_COMPONENT_COUNT); the parameter block has room for 4
+    if (p->num_components < 1 || p->num_components > 10) { b200::set_error("Too many color components: %d, max 10", p->num_components); return B200JPEG_ERR_PARAM; }
+    if (p->num_components > B200JPEG_MAX_COMPONENTS) { b200::set_error("%d components: the device path takes at most %d", p->num_components, B200JPEG_MAX_COMPONENTS); return B200JPEG_ERR_UNSUPPORTED; }
+    for (int ci = 0; ci < p->num_components; ci++) set_comp(p, ci, ci, 1, 1, 0, 0, 0);
+    break;
   default: b200::set_error("unsupported JPEG colorspace %d", colorspace); return B200JPEG_ERR_UNSUPPORTED;
   }
   return B200JPEG_OK;
@@ -114,6 +127,9 @@ int b200jpeg_default_colorspace(b200jpeg_params *p) {
   case B200JPEG_CS_GRAYSCALE: return b200jpeg_set_colorspace(p, B200JPEG_CS_GRAYSCALE);
   case B200JPEG_CS_RGB:       return b200jpeg_set_colorspace(p, B200JPEG_CS_YCbCr);
   case B200JPEG_CS_YCbCr:     return b200jpeg_set_colorspace(p, B200JPEG_CS_YCbCr);
+  case B200JPEG_CS_CMYK:      return b200jpeg_set_colorspace(p, B200JPEG_CS_CMYK);        // by default, no translation
+  case B200JPEG_CS_YCCK:      return b200jpeg_set_colorspace(p, B200JPEG_CS_YCCK);
+  case B200JPEG_CS_UNKNOWN:   return b200jpeg_set_colorspace(p, B200JPEG_CS_UNKNOWN);
   default:
     if (B200JPEG_CS_IS_RGB(p->in_color_space)) return b200jpeg_set_colorspace(p, B200JPEG_CS_YCbCr);     // jcparam.c:535-546
     b200::set_error("unsupported input colorspace %d", p->in_color_space); return B200JPEG_ERR_UNSUPPORTED;
@@ -255,7 +271,8 @@ int b200jpeg_validate(const b200jpeg_params *p) {
   // 12-bit: the coefficient controller has no JBUF_REQUANT mode (jccoefct.c:132-138), so the reference cannot run the
   // trellis passes ("Bogus buffer control mode"); its 12-bit deringing is unusable (jcdctmgr.c:419)
   if (p->data_precision == 12 && (p->trellis_quant || p->overshoot_deringing)) { set_error("12-bit precision needs trellis quantization and overshoot deringing off (cjpeg -notrellis -noovershoot), as in the reference"); return B200JPEG_ERR_PARAM; }
-  if (p->num_components > B200JPEG_MAX_COMPONENTS) { set_error("Too many color components: %d", p->num_components); return B200JPEG_ERR_PARAM; }
+  if (p->num_components > 10) { set_error("Too many color components: %d, max 10", p->num_components); return B200JPEG_ERR_PARAM; }   // JERR_COMPONENT_COUNT
+  if (p->num_components > B200JPEG_MAX_COMPONENTS) { set_error("%d components: the device path takes at most %d", p->num_components, B200JPEG_MAX_COMPONENTS); return B200JPEG_ERR_UNSUPPORTED; }
   int hmax = 1, vmax = 1;
   for (int ci = 0; ci < p->num_components; ci++) {
     const b200jpeg_component_info *c = &p->comp_info[ci];
@@ -272,17 +289,37 @@ int b200jpeg_validate(const b200jpeg_params *p) {
     blocks_in_mcu += c->h_samp_factor * c->v_samp_factor;
   }
   if (blocks_in_mcu > 10) { set_error("Sampling factors too large for interleaved scan"); return B200JPEG_ERR_PARAM; }   // C_MAX_BLOCKS_IN_MCU
-  // jinit_color_converter (jccolor.c:618-648, :680-760): the JPEG colour space fixes the component count
-  if ((p->jpeg_color_space == B200JPEG_CS_GRAYSCALE && p->num_components != 1) ||
-      ((p->jpeg_color_space == B200JPEG_CS_YCbCr || p->jpeg_color_space == B200JPEG_CS_RGB) && p->num_components != 3)) { set_error("Bogus JPEG colorspace"); return B200JPEG_ERR_PARAM; }
-  if (B200JPEG_CS_IS_RGB(p->in_color_space)) {
-    if (p->input_components != B200JPEG_CS_PIXELSIZE(p->in_color_space)) { set_error("Bogus input colorspace"); return B200JPEG_ERR_PARAM; }   // rgb_pixelsize[], jccolor.c:640-660
-    if (p->jpeg_color_space != B200JPEG_CS_YCbCr && p->jpeg_color_space != B200JPEG_CS_GRAYSCALE && p->jpeg_color_space != B200JPEG_CS_RGB) { set_error("Unsupported color conversion request"); return B200JPEG_ERR_PARAM; }
-  } else if (p->in_color_space == B200JPEG_CS_GRAYSCALE) {
-    if (p->input_components != 1 || p->jpeg_color_space != B200JPEG_CS_GRAYSCALE) { set_error("Unsupported color conversion request"); return B200JPEG_ERR_PARAM; }
-  } else if (p->in_color_space == B200JPEG_CS_YCbCr) {
-    if (p->input_components != 3 || p->jpeg_color_space != B200JPEG_CS_YCbCr) { set_error("Unsupported color conversion request"); return B200JPEG_ERR_PARAM; }
-  } else { set_error("Bogus input colorspace"); return B200JPEG_ERR_PARAM; }
+  // jinit_color_converter (jccolor.c:551-740), its two switches: input_components against in_color_space ...
+  const int in_cs = p->in_color_space, jcs = p->jpeg_color_space, nc = p->num_components;
+  int in_size = 0;                                    // 0: any count (JCS_UNKNOWN and values the reference does not name)
+  if (B200JPEG_CS_IS_RGB(in_cs)) in_size = B200JPEG_CS_PIXELSIZE(in_cs);   // rgb_pixelsize[]
+  else if (in_cs == B200JPEG_CS_GRAYSCALE) in_size = 1;
+  else if (in_cs == B200JPEG_CS_YCbCr) in_size = 3;
+  else if (in_cs == B200JPEG_CS_CMYK || in_cs == B200JPEG_CS_YCCK) in_size = 4;
+  if (in_size && p->input_components != in_size) { set_error("Bogus input colorspace"); return B200JPEG_ERR_PARAM; }
+  // ... then num_components against jpeg_color_space, and the conversions it implements
+  bool conv;
+  switch (jcs) {
+  case B200JPEG_CS_GRAYSCALE:
+    if (nc != 1) { set_error("Bogus JPEG colorspace"); return B200JPEG_ERR_PARAM; }
+    conv = in_cs == B200JPEG_CS_GRAYSCALE || B200JPEG_CS_IS_RGB(in_cs) || in_cs == B200JPEG_CS_YCbCr; break;
+  case B200JPEG_CS_RGB:
+    if (nc != 3) { set_error("Bogus JPEG colorspace"); return B200JPEG_ERR_PARAM; }
+    conv = B200JPEG_CS_IS_RGB(in_cs); break;
+  case B200JPEG_CS_YCbCr:
+    if (nc != 3) { set_error("Bogus JPEG colorspace"); return B200JPEG_ERR_PARAM; }
+    conv = B200JPEG_CS_IS_RGB(in_cs) || in_cs == B200JPEG_CS_YCbCr; break;
+  case B200JPEG_CS_CMYK:
+    if (nc != 4) { set_error("Bogus JPEG colorspace"); return B200JPEG_ERR_PARAM; }
+    conv = in_cs == B200JPEG_CS_CMYK; break;
+  case B200JPEG_CS_YCCK:
+    if (nc != 4) { set_error("Bogus JPEG colorspace"); return B200JPEG_ERR_PARAM; }
+    conv = in_cs == B200JPEG_CS_CMYK || in_cs == B200JPEG_CS_YCCK; break;
+  default:                                            // null conversion of JCS_UNKNOWN
+    conv = jcs == in_cs && nc == p->input_components;
+    if (conv && jcs != B200JPEG_CS_UNKNOWN) { set_error("null conversion of colour space %d: the device path takes it for JCS_UNKNOWN only", jcs); return B200JPEG_ERR_UNSUPPORTED; }
+  }
+  if (!conv) { set_error("Unsupported color conversion request"); return B200JPEG_ERR_PARAM; }
   // things the reference can do that the device path cannot (yet)
   if (p->restart_interval < 0 || p->restart_interval > 65535 || p->restart_in_rows < 0) { set_error("restart interval out of range"); return B200JPEG_ERR_PARAM; }
   if (p->dct_method < B200JPEG_DCT_ISLOW || p->dct_method > B200JPEG_DCT_FLOAT) { set_error("unknown dct_method %d", p->dct_method); return B200JPEG_ERR_PARAM; }

@@ -115,9 +115,16 @@ def parse_header(jpeg: bytes) -> SourceInfo:
             s.jpeg_color_space = A.CS_RGB
         else:
             s.jpeg_color_space = A.CS_YCbCr
+    elif s.num_components == 4:
+        # Adobe transform 2 marks YCCK, anything else (or no Adobe marker) CMYK
+        s.jpeg_color_space = A.CS_YCCK if s.saw_Adobe and s.Adobe_transform == 2 else A.CS_CMYK
     else:
-        raise ValueError("only 1- and 3-component files are on the device path")
+        raise ValueError("only 1-, 3- and 4-component files are on the device path")
     return s
+
+
+class ConversionError(ValueError):
+    """The reference refuses the request with JERR_CONVERSION_NOTIMPL and writes no file."""
 
 
 def _copy_critical_parameters(src: SourceInfo, profile: int) -> A.Params:
@@ -195,6 +202,10 @@ def params_for_transcode(src: SourceInfo, switches: Sequence[str]) -> Tuple[A.Pa
     """(dstinfo at jpeg_write_coefficients, prefer_smallest) for ``jpegtran <switches> file``."""
     # first pass on the bare object (profile JCP_MAX_COMPRESSION, jcapimin.c:108): everything it sets is overwritten by
     # the jpeg_set_defaults inside jpeg_copy_critical_parameters - except the profile itself, which that call reads
+    if any(_keymatch(a[1:], "grayscale", 2) or _keymatch(a[1:], "greyscale", 2) for a in switches if a.startswith("-")):
+        if src.num_components == 4:                   # jtransform_adjust_parameters (transupp.c:2048-2071)
+            raise ConversionError("Unsupported color conversion request")
+        raise UsageError("-grayscale is not on the device path")
     p0 = A.Params()
     p0.compress_profile = A.PROFILE_MAX_COMPRESSION
     _parse(p0, list(switches), False)

@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
 """Randomised device-vs-oracle cross-check (runs on a GPU box): random shapes, cjpeg switch sets, extension parameters
-(the optional trellis modes), pixel orders of the RGB family and small batches through the C-ABI, every file compared
+(the optional trellis modes), pixel orders of the RGB family, the CMYK / YCCK / YCbCr->gray / JCS_UNKNOWN conversions and small batches through the C-ABI, every file compared
 byte for byte with the CPU oracle (itself pinned to the reference).  Test infrastructure.
 usage: fuzz_gpu.py [seed] [cases] [seconds]      (exit status 1 if anything differs)"""
 import os, random, sys, time
@@ -11,6 +11,8 @@ from oracle import oracle as O
 import mozjpeg_b200 as mj
 from mozjpeg_b200 import _abi as A
 from mozjpeg_b200.synth import synth_image12
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
+import colorspace_cases as CC       # CMYK / YCCK / YCbCr->gray / JCS_UNKNOWN conversions and their restatement
 
 seed = int(sys.argv[1]) if len(sys.argv) > 1 else 1
 cases = int(sys.argv[2]) if len(sys.argv) > 2 else 300
@@ -37,8 +39,12 @@ for it in range(cases):
     if rng.random() < 0.1: sw += ["-smooth", str(rng.choice([1, 10, 50, 100]))]
     if twelve: sw = ["-precision", "12", "-notrellis", "-noovershoot"] + sw
     elif rng.random() < 0.15: sw += [rng.choice(["-notrellis", "-notrellis-dc", "-noovershoot", "-optimize"])]
+    conv = rng.choice(list(CC.CONVERSIONS)) if rng.random() < 0.25 else None
+    if conv and "-grayscale" in sw:
+        sw.remove("-grayscale")
+    in_cs, ic, jcs = CC.CONVERSIONS[conv] if conv else (A.CS_RGB, 3, None)
     try:
-        p = mj.params_from_switches(sw, w, h, 3)
+        p = mj.params_from_switches(sw, w, h, ic, in_cs, jcs)
     except Exception:
         continue
     ext = {}
@@ -53,12 +59,15 @@ for it in range(cases):
         refused += 1
         continue
     n = rng.choice([1, 1, 2, 3])
-    imgs = [synth_image12(rng.randrange(1 << 20), w, h) if twelve else O.synth_image(rng.randrange(1 << 20), w, h) for _ in range(n)]
-    refs = [O.oracle_encode(p, im).jpeg for im in imgs]
+    if conv:
+        imgs = [CC.cmyk_image(rng.randrange(1 << 20), w, h, ic, 12 if twelve else 8) for _ in range(n)]
+    else:
+        imgs = [synth_image12(rng.randrange(1 << 20), w, h) if twelve else O.synth_image(rng.randrange(1 << 20), w, h) for _ in range(n)]
+    refs = [CC.oracle_encode(p, im).jpeg for im in imgs]
     arr = np.stack(imgs)
     q = p
     order = None
-    if rng.random() < 0.3:
+    if rng.random() < 0.3 and not conv:
         order = rng.choice(list(A.CS_EXT))
         val, size, ro, go, bo = A.CS_EXT[order]
         out = np.random.default_rng(it).integers(0, 4096 if twelve else 256, arr.shape[:3] + (size,), dtype=arr.dtype)
@@ -82,7 +91,7 @@ for it in range(cases):
     tot += 1
     for i in range(n):
         if got[i] != refs[i]:
-            bad += 1; print("MISMATCH", sw, ext, order, (w, h, n), "image", i, len(got[i]), len(refs[i])); break
+            bad += 1; print("MISMATCH", sw, ext, conv or order, (w, h, n), "image", i, len(got[i]), len(refs[i])); break
 print("seed", seed, "bad", bad, "compared", tot, "refused", refused, "seconds %.0f" % (time.time() - t0))
 enc.close()
 sys.exit(1 if bad else 0)

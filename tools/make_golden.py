@@ -192,9 +192,49 @@ def fullsize():
     print("wrote", len(cases), "full-size cases")
 
 
+def colorspaces():
+    """tests/golden/colorspace_golden.json: CMYK / YCCK / YCbCr->gray / JCS_UNKNOWN encodes by the reference (through
+    build/librefcs.so, tests/refcs.c), raw-data input with 4 planes, and jpegtran on CMYK / YCCK sources."""
+    import subprocess
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import colorspace_cases as CC
+    path = CC.GOLDEN
+    if os.path.exists(path) and "--force" not in sys.argv:
+        sys.exit(f"{path} exists; pass --force to overwrite it")
+    if not CC.have_reference():
+        sys.exit("build/librefcs.so is missing: run __graft_entry__.build() with the reference build under oracle/_ref/")
+    cases = []
+    for c in CC.pixel_cases():
+        a = CC.reference_file(c)
+        cases.append(dict(c, md5=CC.md5(a), size=len(a)))
+    raw = []
+    for conv, (in_cs, jcs) in CC.RAW_CONVERSIONS.items():
+        for sw in CC.RAW_SETS:
+            p = cjpeg.params_from_switches(sw, 227, 149, 4, in_cs, jcs)
+            planes = CC.raw_planes(5, p, 4)
+            a = CC.ref_encode(None, in_cs, 4, jcs, sw, planes=planes, size=(227, 149))
+            raw.append(dict(id=CC.case_id(conv, " ".join(sw)), conv=conv, switches=sw, seed=5, w=227, h=149, md5=CC.md5(a), size=len(a)))
+    tran = []
+    for src in CC.TRAN_SOURCES:
+        data = CC.tran_source(src)
+        for sw in CC.TRAN_SETS + [["-grayscale"]]:
+            r = subprocess.run([os.path.join(CC.REF, "jpegtran"), *sw], input=data, capture_output=True)
+            rec = dict(id=CC.case_id(src, " ".join(sw)), source=src, switches=sw, source_md5=CC.md5(data))
+            if r.returncode != 0 or not r.stdout:
+                rec["error"] = r.stderr.decode().strip()
+            else:
+                rec.update(md5=CC.md5(r.stdout), size=len(r.stdout))
+            tran.append(rec)
+    json.dump({"generator": "tools/make_golden.py --colorspaces", "reference": "mozilla/mozjpeg 5.0.0 (C path, WITH_SIMD=0), oracle/_ref",
+               "cases": cases, "raw": raw, "transcode": tran}, open(path, "w"), indent=0)
+    print("wrote", len(cases), "pixel,", len(raw), "raw-data and", len(tran), "jpegtran cases")
+
+
 def main():
     if "--fullsize" in sys.argv:
         return fullsize()
+    if "--colorspaces" in sys.argv:
+        return colorspaces()
     os.makedirs(GOLD, exist_ok=True)
     # cases already recorded are kept as they are unless --force is given (a full regeneration takes a while)
     have = {}
