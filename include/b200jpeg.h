@@ -245,7 +245,35 @@ int  b200jpeg_encode_batch_coefs(b200jpeg_encoder *enc, const b200jpeg_params *p
                                  const int16_t *const *planes, int planes_on_device,
                                  const size_t *row_pitch_blocks, const size_t *image_stride_blocks, int n_images);
 
-/* Same, but stops after the entropy-coded bytes are in HBM: no device->host
+/*
+ * Per-image quantization tables: the three batch entry points above with one table set per image.  Image i is the
+ * file the reference writes for it from a compress object holding `p` with quant_tbl replaced by image i's tables:
+ * its DQT, its choice between SOF0 and SOF1 (a table entry above 255 makes it SOF1) and its quantization come from
+ * them; everything else (geometry, sampling, scan script, trellis and Huffman options, markers, precision) is p's.
+ *
+ * qtables     : n_images x B200JPEG_NUM_QUANT_TBLS x 64 entries, natural order (like JQUANT_TBL.quantval); only the
+ *               slots p->quant_tbl_present names are read.  Every entry read must lie in 1..32767 (the range
+ *               jpeg_add_quant_table clamps to), else B200JPEG_ERR_PARAM naming the image and the slot.  With the
+ *               trellis on, a table whose entries lie too far apart for the device divider returns
+ *               B200JPEG_ERR_UNSUPPORTED naming the image.  A refused batch writes no file.
+ * image_stride: may be 0 here (each image_stride[ci] on the raw and coefficient variants): every image then reads
+ *               the same pixels, planes or blocks, e.g. one picture at several qualities.  Host input is staged once.
+ * Images that share a table set share its device constants; a batch costs the same kernel launches as with one set.
+ */
+int  b200jpeg_encode_batch_qtables(b200jpeg_encoder *enc, const b200jpeg_params *p,
+                                   const void *pixels, int pixels_on_device,
+                                   size_t row_pitch, size_t image_stride,
+                                   const uint16_t *qtables, int n_images);
+int  b200jpeg_encode_batch_raw_qtables(b200jpeg_encoder *enc, const b200jpeg_params *p,
+                                       const uint8_t *const *planes, int planes_on_device,
+                                       const size_t *row_pitch, const size_t *image_stride,
+                                       const uint16_t *qtables, int n_images);
+int  b200jpeg_encode_batch_coefs_qtables(b200jpeg_encoder *enc, const b200jpeg_params *p,
+                                         const int16_t *const *planes, int planes_on_device,
+                                         const size_t *row_pitch_blocks, const size_t *image_stride_blocks,
+                                         const uint16_t *qtables, int n_images);
+
+/* b200jpeg_encode_batch, but stops after the entropy-coded bytes are in HBM: no device->host
  * copy, no host-side file assembly.  Used to time the device pipeline alone. */
 int  b200jpeg_encode_batch_device_only(b200jpeg_encoder *enc, const b200jpeg_params *p,
                                        const void *pixels_device,

@@ -18,7 +18,7 @@ from .cjpeg import params_from_switches, read_ppm  # noqa: F401
 
 _lib = A.load()          # raises ImportError with build instructions if missing
 
-__all__ = ["Encoder", "Params", "params_from_switches", "read_ppm", "cjpeg", "tj3_params", "B200JpegError"]
+__all__ = ["Encoder", "Params", "params_from_switches", "read_ppm", "cjpeg", "tj3_params", "quality_tables", "B200JpegError"]
 
 
 class Encoder:
@@ -56,7 +56,23 @@ class Encoder:
         A.check(_lib.b200jpeg_encoder_set_streams(self._h, n), "set_streams")
 
     # -- batch API -------------------------------------------------------
-    def encode_batch(self, p: Params, images: np.ndarray) -> List[bytes]:
+    # qtables (all three forms): None, or an (N, 4, 64) uint16 array of per-image quantization tables in natural order
+    # (the slots p.quant_tbl_present names are read); image i is then written with its own tables.  Input holding ONE
+    # image with N table sets is encoded N times from the same pixels (image stride 0, staged once): a quality ladder.
+    @staticmethod
+    def _qtables(qtables, n: int):
+        a = np.asarray(qtables)
+        # the conversion to uint16 must not change a value (65537 would become 1 and pass the library's 1..32767 check)
+        if a.dtype.kind not in "iu" or (a.size and (a.min() < 0 or a.max() > 0xFFFF)):
+            raise ValueError("qtables must hold integers in 0..65535 (the library accepts 1..32767)")
+        q = np.ascontiguousarray(a, dtype=np.uint16)
+        if q.ndim != 3 or q.shape[1:] != (A.NUM_QUANT_TBLS, 64):
+            raise ValueError("qtables must have shape (N, 4, 64)")
+        if n != 1 and q.shape[0] != n:
+            raise ValueError(f"qtables holds {q.shape[0]} table sets for {n} images")
+        return q, q.shape[0], n == 1 and q.shape[0] != 1
+
+    def encode_batch(self, p: Params, images: np.ndarray, qtables: Optional[np.ndarray] = None) -> List[bytes]:
         """images: (N, H, W, C) or (N, H, W) host array -> N JPEG files (uint8, or uint16
         holding 12-bit samples when p.data_precision == 12, like J12SAMPLE rows).
         Host->device staging and device->host read-back happen inside."""
@@ -66,30 +82,55 @@ class Encoder:
         n, h, w, c = a.shape
         if (w, h, c) != (p.image_width, p.image_height, p.input_components):
             raise ValueError("array shape does not match params")
-        A.check(_lib.b200jpeg_encode_batch(self._h, C.byref(p), a.ctypes.data, 0, a.strides[1], a.strides[0], n), "encode_batch")
+        if qtables is None:
+            A.check(_lib.b200jpeg_encode_batch(self._h, C.byref(p), a.ctypes.data, 0, a.strides[1], a.strides[0], n), "encode_batch")
+        else:
+            q, n, shared = self._qtables(qtables, n)
+            A.check(_lib.b200jpeg_encode_batch_qtables(self._h, C.byref(p), a.ctypes.data, 0, a.strides[1], 0 if shared else a.strides[0],
+                                                       q.ctypes.data_as(C.POINTER(C.c_uint16)), n), "encode_batch_qtables")
         return [self.get_output(i) for i in range(n)]
 
-    def encode_batch_raw(self, p: Params, planes: Sequence[np.ndarray]) -> List[bytes]:
+    def encode_batch_raw(self, p: Params, planes: Sequence[np.ndarray], qtables: Optional[np.ndarray] = None) -> List[bytes]:
         """Raw-data input (jpeg_write_raw_data): planes[ci] is an (N, rows, cols) uint8 array holding
         the converted, downsampled samples of component ci (at least hib*8 x wib*8 per image)."""
         arrs = [np.ascontiguousarray(a, dtype=np.uint8) for a in planes]
         n = arrs[0].shape[0]
         ptrs = (C.c_void_p * len(arrs))(*[a.ctypes.data for a in arrs])
         pitch = (C.c_size_t * len(arrs))(*[a.strides[1] for a in arrs])
-        stride = (C.c_size_t * len(arrs))(*[a.strides[0] for a in arrs])
-        A.check(_lib.b200jpeg_encode_batch_raw(self._h, C.byref(p), ptrs, 0, pitch, stride, n), "encode_batch_raw")
+        if qtables is None:
+            stride = (C.c_size_t * len(arrs))(*[a.strides[0] for a in arrs])
+            A.check(_lib.b200jpeg_encode_batch_raw(self._h, C.byref(p), ptrs, 0, pitch, stride, n), "encode_batch_raw")
+        else:
+            q, n, shared = self._qtables(qtables, n)
+            stride = (C.c_size_t * len(arrs))(*[0 if shared else a.strides[0] for a in arrs])
+            A.check(_lib.b200jpeg_encode_batch_raw_qtables(self._h, C.byref(p), ptrs, 0, pitch, stride, q.ctypes.data_as(C.POINTER(C.c_uint16)), n),
+                    "encode_batch_raw_qtables")
         return [self.get_output(i) for i in range(n)]
 
-    def encode_batch_coefs(self, p: Params, planes: Sequence[np.ndarray]) -> List[bytes]:
+    def encode_batch_coefs(self, p: Params, planes: Sequence[np.ndarray], qtables: Optional[np.ndarray] = None) -> List[bytes]:
         """Coefficient-domain input (jpeg_write_coefficients): planes[ci] is an (N, hib, wib, 64) int16 array of
         quantized coefficients in natural order (libjpeg JBLOCKs)."""
         arrs = [np.ascontiguousarray(a, dtype=np.int16) for a in planes]
         n = arrs[0].shape[0]
         ptrs = (C.c_void_p * len(arrs))(*[a.ctypes.data for a in arrs])
         pitch = (C.c_size_t * len(arrs))(*[a.strides[1] // 128 for a in arrs])
-        stride = (C.c_size_t * len(arrs))(*[a.strides[0] // 128 for a in arrs])
-        A.check(_lib.b200jpeg_encode_batch_coefs(self._h, C.byref(p), ptrs, 0, pitch, stride, n), "encode_batch_coefs")
+        if qtables is None:
+            stride = (C.c_size_t * len(arrs))(*[a.strides[0] // 128 for a in arrs])
+            A.check(_lib.b200jpeg_encode_batch_coefs(self._h, C.byref(p), ptrs, 0, pitch, stride, n), "encode_batch_coefs")
+        else:
+            q, n, shared = self._qtables(qtables, n)
+            stride = (C.c_size_t * len(arrs))(*[0 if shared else a.strides[0] // 128 for a in arrs])
+            A.check(_lib.b200jpeg_encode_batch_coefs_qtables(self._h, C.byref(p), ptrs, 0, pitch, stride, q.ctypes.data_as(C.POINTER(C.c_uint16)), n),
+                    "encode_batch_coefs_qtables")
         return [self.get_output(i) for i in range(n)]
+
+    def encode_batch_qtables_ptr(self, p: Params, ptr: int, on_device: bool, row_pitch: int, image_stride: int,
+                                 qtables: np.ndarray) -> None:
+        """Raw-pointer form of encode_batch with per-image tables (device tensors, pinned host buffers); one image per
+        table set, image_stride 0 = every image reads the same pixels."""
+        q, n, _ = self._qtables(qtables, len(qtables))
+        A.check(_lib.b200jpeg_encode_batch_qtables(self._h, C.byref(p), ptr, int(on_device), row_pitch, image_stride,
+                                                   q.ctypes.data_as(C.POINTER(C.c_uint16)), n), "encode_batch_qtables")
 
     def encode_batch_ptr(self, p: Params, ptr: int, on_device: bool, row_pitch: int, image_stride: int, n: int,
                          device_only: bool = False) -> None:
@@ -197,3 +238,17 @@ def tj3_params(width: int, height: int, quality: int = 75, subsamp: str = "420",
     if p.num_components > 3:
         p.comp_info[3].h_samp_factor, p.comp_info[3].v_samp_factor = hv
     return p
+
+
+def quality_tables(p: Params, qualities: Sequence[int], force_baseline: bool = True) -> np.ndarray:
+    """Per-image quantization tables for Encoder.encode_batch(..., qtables=): (len(qualities), 4, 64) uint16, natural
+    order.  Set i is what jpeg_set_quality(cinfo, qualities[i], force_baseline) leaves in quant_tbl when applied to a
+    copy of ``p`` (jcparam.c:351-373: the scaled base tables of p.quant_tbl_master_idx in slots 0 and 1, the other
+    slots as p has them).  It is jpeg_set_quality semantics only: unlike cjpeg's -quality switch it does not change
+    the sampling factors at quality 80 and above."""
+    out = np.zeros((len(qualities), A.NUM_QUANT_TBLS, 64), dtype=np.uint16)
+    for i, q in enumerate(qualities):
+        c = p.copy()
+        _lib.b200jpeg_set_quality(C.byref(c), int(q), int(bool(force_baseline)))
+        out[i] = np.ctypeslib.as_array(c.quant_tbl)
+    return out

@@ -89,7 +89,8 @@ EXPORTS = [
     "b200jpeg_simple_progression", "b200jpeg_std_huff_tables", "b200jpeg_std_quant_tbl",
     "b200jpeg_validate", "b200jpeg_total_passes",
     "b200jpeg_encoder_create", "b200jpeg_encoder_destroy", "b200jpeg_encoder_set_stream", "b200jpeg_encoder_set_chunk_images", "b200jpeg_last_chunk_images", "b200jpeg_encoder_set_streams", "b200jpeg_encode_batch",
-    "b200jpeg_encode_batch_device_only", "b200jpeg_encode_batch_raw", "b200jpeg_encode_batch_coefs", "b200jpeg_get_output", "b200jpeg_last_scan_bytes",
+    "b200jpeg_encode_batch_device_only", "b200jpeg_encode_batch_raw", "b200jpeg_encode_batch_coefs",
+    "b200jpeg_encode_batch_qtables", "b200jpeg_encode_batch_raw_qtables", "b200jpeg_encode_batch_coefs_qtables", "b200jpeg_get_output", "b200jpeg_last_scan_bytes",
     "b200jpeg_kernel_launches", "b200jpeg_last_stage_times", "b200jpeg_debug_get_coefs",
     "b200jpeg_debug_get_huff", "b200jpeg_start_compress", "b200jpeg_write_scanlines",
     "b200jpeg_finish_compress", "b200jpeg_last_error", "b200jpeg_version",
@@ -132,6 +133,10 @@ def load() -> C.CDLL:
     lib.b200jpeg_encode_batch.argtypes = [C.c_void_p, P, C.c_void_p, C.c_int, C.c_size_t, C.c_size_t, C.c_int]; lib.b200jpeg_encode_batch.restype = C.c_int
     lib.b200jpeg_encode_batch_raw.argtypes = [C.c_void_p, P, C.POINTER(C.c_void_p), C.c_int, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t), C.c_int]; lib.b200jpeg_encode_batch_raw.restype = C.c_int
     lib.b200jpeg_encode_batch_coefs.argtypes = [C.c_void_p, P, C.POINTER(C.c_void_p), C.c_int, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t), C.c_int]; lib.b200jpeg_encode_batch_coefs.restype = C.c_int
+    Q = C.POINTER(C.c_uint16)
+    lib.b200jpeg_encode_batch_qtables.argtypes = [C.c_void_p, P, C.c_void_p, C.c_int, C.c_size_t, C.c_size_t, Q, C.c_int]; lib.b200jpeg_encode_batch_qtables.restype = C.c_int
+    lib.b200jpeg_encode_batch_raw_qtables.argtypes = [C.c_void_p, P, C.POINTER(C.c_void_p), C.c_int, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t), Q, C.c_int]; lib.b200jpeg_encode_batch_raw_qtables.restype = C.c_int
+    lib.b200jpeg_encode_batch_coefs_qtables.argtypes = [C.c_void_p, P, C.POINTER(C.c_void_p), C.c_int, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t), Q, C.c_int]; lib.b200jpeg_encode_batch_coefs_qtables.restype = C.c_int
     lib.b200jpeg_encode_batch_device_only.argtypes = [C.c_void_p, P, C.c_void_p, C.c_size_t, C.c_size_t, C.c_int]; lib.b200jpeg_encode_batch_device_only.restype = C.c_int
     lib.b200jpeg_get_output.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.POINTER(C.c_uint8)), C.POINTER(C.c_size_t)]; lib.b200jpeg_get_output.restype = C.c_int
     lib.b200jpeg_last_scan_bytes.argtypes = [C.c_void_p]; lib.b200jpeg_last_scan_bytes.restype = C.c_size_t

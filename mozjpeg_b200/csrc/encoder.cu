@@ -10,6 +10,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <map>
 #include <string>
 #include <vector>
 
@@ -108,13 +109,16 @@ struct b200jpeg_encoder {
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
   int n_streams = 2;
   // device buffers sized for the WHOLE batch
-  DevBuf d_src, d_tabs_scan, d_tabs_fixed, d_status, d_out_pos, d_scan_size, d_out, d_qt, d_tc, d_best_al_all, d_qimg_all;
+  DevBuf d_src, d_tabs_scan, d_tabs_fixed, d_status, d_out_pos, d_scan_size, d_out, d_qt, d_tc, d_best_al_all, d_qimg_all, d_qset;
+  // quantization table sets of the last batch: the distinct [4][64] tables (natural order) its images use, and each
+  // image's set; one set (the parameter block's) and no per-image index unless the caller passed per-image tables
+  std::vector<uint16_t> qsets; std::vector<int> img_set; int nsets = 1;
   size_t bitbuf_words_per_image = 0, out_cap_per_image = 0;
   double cap_factor = 0.25;      // entropy-coded bytes the buffers hold per coefficient; grows on overflow, falls back after calm batches
   int calm_batches = 0;
   size_t max_image_scan_bytes = 0;   // largest entropy-coded size of one image in the last host-visible batch
   // pinned host mirrors
-  PinBuf h_qt, h_tc, h_fixed, h_status, h_out_pos, h_scan_size, h_tabs, h_stage, h_best_al, h_qinit, h_qimg;
+  PinBuf h_qt, h_tc, h_fixed, h_status, h_out_pos, h_scan_size, h_tabs, h_stage, h_best_al, h_qinit, h_qimg, h_qset;
   // finished files: bump-allocated from pinned arenas, valid until the next encode call
   std::vector<PinBuf> file_arenas; size_t arena_idx = 0, arena_off = 0;
   std::vector<std::pair<uint8_t *, size_t>> files;
@@ -143,6 +147,7 @@ struct ChunkIO {
   b200::DevHuff *tabs_scan;         // [n][nscans][8]
   int *best_al;                     // [2][n] scan search: best luma / chroma Al per image
   uint16_t *qimg;                   // [n][4][64] trellis_q_opt: the re-fitted quantization tables per image (natural order)
+  const int *qset;                  // [n] each image's quantization table set (device), or nullptr: set 0
 };
 
 namespace b200 {
@@ -173,7 +178,6 @@ static int build_plan(const b200jpeg_params *p, size_t row_pitch, size_t image_s
     c.wib = div_up((long long)g.W * c.h, g.hmax * 8); c.hib = div_up((long long)g.H * c.v, g.vmax * 8);   // jcmaster.c:221-226
     c.wpad = g.mcus_per_row * c.h; c.hpad = g.mcu_rows * c.v;
     c.qt = ic.quant_tbl_no; c.dc_tbl = ic.dc_tbl_no; c.ac_tbl = ic.ac_tbl_no;
-    c.dc_q8 = 8 * (int)p->quant_tbl[c.qt][0];
     c.rows_avail = div_up(g.H, g.vmax) * c.v;
     c.blocks_per_image = (long long)c.wpad * c.hpad;
     pl.coef_bytes[ci] = (size_t)c.blocks_per_image * 128;
@@ -300,6 +304,14 @@ static void make_trellis_consts(const b200jpeg_params *p, TrellisConsts *tc)
     int L = 0; while ((1ull << L) < dmax) L++;
     tc->qL[t] = L;
     for (int k = 0; k < 64; k++) { unsigned d = 8u * p->quant_tbl[t][kZigzag[k]]; tc->qmul_zz[t][k] = (unsigned)std::min<unsigned long long>(((1ull << (18 + L)) + d - 1) / d, 0xFFFFFFFFull); }
+    // the DC trellis' divider; its fast form needs 9 candidates (get_num_dc_trellis_candidates, jcdctmgr.c:929-933) and
+    // no candidate that can reach the coefficient limit
+    const unsigned d = 8u * p->quant_tbl[t][0];
+    int l = 0; while ((1ull << l) < d) l++;
+    tc->dc_shift[t] = 18 + l;
+    tc->dc_mul[t] = (unsigned)(((1ull << tc->dc_shift[t]) + d - 1) / d);
+    int ncand = (2 + 60 / (int)(d >> 3)) | 1; if (ncand > 9) ncand = 9;
+    tc->dc_fast[t] = ncand == 9 && (int)((32768 + d / 2) / d) + 9 < (1 << (p->data_precision + 2)) - 1;
   }
   tc->use_norm = p->lambda_log_scale2 > 0.0f;
   tc->delta_dc_weight = p->trellis_delta_dc_weight;
@@ -433,24 +445,43 @@ static int prepare_batch(b200jpeg_encoder *e, int n_total, int chunk, bool host_
   if ((rc = e->d_out_pos.reserve((size_t)n_total * (nscans + 1) * 8))) return rc;
   if ((rc = e->d_scan_size.reserve((size_t)n_total * nscans * 4))) return rc;
   if ((rc = e->d_best_al_all.reserve((size_t)n_total * 2 * 4))) return rc;
+  const int ns = e->nsets;
   if (p->trellis_quant && p->trellis_q_opt) {
     if ((rc = e->d_qimg_all.reserve((size_t)n_total * 512))) return rc;
-    if ((rc = e->h_qinit.reserve(512))) return rc;
-    memcpy(e->h_qinit.p, p->quant_tbl, 512);
+    if ((rc = e->h_qinit.reserve((size_t)ns * 512))) return rc;
+    memcpy(e->h_qinit.p, e->qsets.data(), (size_t)ns * 512);              // every image starts from its own tables
   }
   if ((rc = e->d_out.reserve(e->out_cap_per_image * n_total))) return rc;
-  if ((rc = e->d_qt.reserve(sizeof(QuantTables)))) return rc;
-  if ((rc = e->d_tc.reserve(sizeof(TrellisConsts)))) return rc;
-  if ((rc = e->h_qt.reserve(sizeof(QuantTables)))) return rc;
-  if ((rc = e->h_tc.reserve(sizeof(TrellisConsts)))) return rc;
+  if ((rc = e->d_qt.reserve(sizeof(QuantTables) * ns))) return rc;
+  if ((rc = e->d_tc.reserve(sizeof(TrellisConsts) * ns))) return rc;
+  if ((rc = e->h_qt.reserve(sizeof(QuantTables) * ns))) return rc;
+  if ((rc = e->h_tc.reserve(sizeof(TrellisConsts) * ns))) return rc;
   if ((rc = e->h_fixed.reserve(tabset))) return rc;
 
-  make_quant_consts(p, e->h_qt.as<QuantTables>());
-  make_trellis_consts(p, e->h_tc.as<TrellisConsts>());
-  if (pl.trellis) for (int t = 0; t < 4; t++) {
-    if (!p->quant_tbl_present[t]) continue;
-    unsigned dmin = ~0u; for (int k = 0; k < 64; k++) dmin = std::min(dmin, 8u * p->quant_tbl[t][k]);
-    if ((((1ull << (18 + e->h_tc.as<TrellisConsts>()->qL[t])) + dmin - 1) / dmin) >= (1ull << 32)) { set_error("trellis quantization: quantization table %d mixes values too far apart for the device divider", t); return B200JPEG_ERR_UNSUPPORTED; }
+  // the constants of every distinct table set (a parameter block that differs from p in quant_tbl only)
+  for (int si = 0; si < ns; si++) {
+    static thread_local b200jpeg_params ps;
+    ps = *p; memcpy(ps.quant_tbl, &e->qsets[(size_t)si * 256], 512);
+    make_quant_consts(&ps, e->h_qt.as<QuantTables>() + si);
+    make_trellis_consts(&ps, e->h_tc.as<TrellisConsts>() + si);
+    if (pl.trellis) for (int t = 0; t < 4; t++) {
+      if (!ps.quant_tbl_present[t]) continue;
+      unsigned dmin = ~0u; for (int k = 0; k < 64; k++) dmin = std::min(dmin, 8u * ps.quant_tbl[t][k]);
+      if ((((1ull << (18 + e->h_tc.as<TrellisConsts>()[si].qL[t])) + dmin - 1) / dmin) >= (1ull << 32)) {
+        if (e->img_set.empty()) set_error("trellis quantization: quantization table %d mixes values too far apart for the device divider", t);
+        else {
+          int img = 0; while (e->img_set[img] != si) img++;
+          set_error("trellis quantization: image %d: quantization table %d mixes values too far apart for the device divider", img, t);
+        }
+        return B200JPEG_ERR_UNSUPPORTED;
+      }
+    }
+  }
+  if (!e->img_set.empty()) {
+    if ((rc = e->d_qset.reserve((size_t)n_total * sizeof(int)))) return rc;
+    if ((rc = e->h_qset.reserve((size_t)n_total * sizeof(int)))) return rc;
+    memcpy(e->h_qset.p, e->img_set.data(), (size_t)n_total * sizeof(int));
+    CU(cudaMemcpyAsync(e->d_qset.p, e->h_qset.p, (size_t)n_total * sizeof(int), cudaMemcpyHostToDevice, s));
   }
   {
     DevHuff *f = e->h_fixed.as<DevHuff>();
@@ -458,8 +489,8 @@ static int prepare_batch(b200jpeg_encoder *e, int n_total, int chunk, bool host_
       if (make_fixed_table(p->dc_huff_tbl[t], true, &f[t]) || make_fixed_table(p->ac_huff_tbl[t], false, &f[4 + t])) { set_error("Bogus Huffman table definition"); return B200JPEG_ERR_PARAM; }
     }
   }
-  CU(cudaMemcpyAsync(e->d_qt.p, e->h_qt.p, sizeof(QuantTables), cudaMemcpyHostToDevice, s));
-  CU(cudaMemcpyAsync(e->d_tc.p, e->h_tc.p, sizeof(TrellisConsts), cudaMemcpyHostToDevice, s));
+  CU(cudaMemcpyAsync(e->d_qt.p, e->h_qt.p, sizeof(QuantTables) * ns, cudaMemcpyHostToDevice, s));
+  CU(cudaMemcpyAsync(e->d_tc.p, e->h_tc.p, sizeof(TrellisConsts) * ns, cudaMemcpyHostToDevice, s));
   CU(cudaMemcpyAsync(e->d_tabs_fixed.p, e->h_fixed.p, tabset, cudaMemcpyHostToDevice, s));
   return B200JPEG_OK;
 }
@@ -477,6 +508,7 @@ static int run_pipeline(b200jpeg_encoder *e, const ChunkIO &io, Timer &tm)
   const size_t tabset = sizeof(DevHuff) * HIST_SLOTS;
   const uint8_t *src_dev = io.src;
   for (int ci = 0; ci < 4; ci++) g.plane[ci] = io.plane[ci];
+  g.qset = io.qset;
   uint32_t *status = io.status;
 
   const bool symrec = use_symrec(pl, p);
@@ -486,7 +518,16 @@ static int run_pipeline(b200jpeg_encoder *e, const ChunkIO &io, Timer &tm)
   for (int ci = 0; ci < g.nc; ci++) { rl.comp_off[ci] = rl.per_image; rl.per_image += (long long)g.c[ci].wib * g.c[ci].hib; }
   rl.sym_hi = (long long)n * rl.per_image * (SYMREC_BYTES / 2);      // second plane of the symbol records (SYMREC_SPLIT)
   tm.mark("forward");
-  int qfast = 1; for (int ci = 0; ci < g.nc; ci++) qfast &= e->h_qt.as<QuantTables>()->fast[g.c[ci].qt];
+  // the fast quantizer / DC-trellis forms serve a launch only if every table set allows them for the launch's components
+  int qfast = 1;
+  for (int si = 0; si < e->nsets; si++)
+    for (int ci = 0; ci < g.nc; ci++) qfast &= e->h_qt.as<QuantTables>()[si].fast[g.c[ci].qt];
+  auto dc_fast_of = [&](const Geom &gr) {
+    int f = 1;
+    for (int si = 0; si < e->nsets; si++)
+      for (int ci = 0; ci < gr.nc; ci++) f &= e->h_tc.as<TrellisConsts>()[si].dc_fast[gr.c[ci].qt];
+    return f;
+  };
   Geom gf = g;
   if (g.raw_in == 2) {
     launch_import_coefs(g, n, s);
@@ -534,8 +575,11 @@ static int run_pipeline(b200jpeg_encoder *e, const ChunkIO &io, Timer &tm)
     so.dcq_ac = p->trellis_quant_dc ? 0 : 1;
     uint16_t *qimg = qopt ? A.d_qimg.as<uint16_t>() : nullptr;
     if (qopt) {
-      // every image starts from the batch's tables (natural order, like JQUANT_TBL.quantval)
-      for (int i = 0; i < n; i++) CU(cudaMemcpyAsync(qimg + (size_t)i * 256, e->h_qinit.p, 512, cudaMemcpyHostToDevice, s));
+      // every image starts from its own table set (natural order, like JQUANT_TBL.quantval)
+      for (int i = 0; i < n; i++) {
+        const int si = e->img_set.empty() ? 0 : e->img_set[io.i0 + i];
+        CU(cudaMemcpyAsync(qimg + (size_t)i * 256, e->h_qinit.as<uint16_t>() + (size_t)si * 256, 512, cudaMemcpyHostToDevice, s));
+      }
     }
     // one statistics -> tables -> quantize_trellis round over the components of gr (all of them, or one)
     auto round = [&](const Geom &gr, const RecLayout &rlr, int bSs, int bSe) -> int {
@@ -578,8 +622,8 @@ static int run_pipeline(b200jpeg_encoder *e, const ChunkIO &io, Timer &tm)
     }
     if (p->trellis_quant_dc) {
       tm.mark("trellis_dc");
-      if (pl.progressive) launch_trellis_dc(gr, e->d_tc.as<TrellisConsts>(), e->d_tabs_fixed.as<DevHuff>(), 0, A.d_rec.as<DcRec>(), A.d_bt.as<unsigned long long>(), rlr, p->trellis_delta_dc_weight > 0.0f, nullptr, 1, n, s);
-      else launch_trellis_dc(gr, e->d_tc.as<TrellisConsts>(), tset, tabset, A.d_rec.as<DcRec>(), A.d_bt.as<unsigned long long>(), rlr, p->trellis_delta_dc_weight > 0.0f, so.dcq, so.keep_coef, n, s);
+      if (pl.progressive) launch_trellis_dc(gr, e->d_tc.as<TrellisConsts>(), e->d_tabs_fixed.as<DevHuff>(), 0, A.d_rec.as<DcRec>(), A.d_bt.as<unsigned long long>(), rlr, p->trellis_delta_dc_weight > 0.0f, dc_fast_of(gr), nullptr, 1, n, s);
+      else launch_trellis_dc(gr, e->d_tc.as<TrellisConsts>(), tset, tabset, A.d_rec.as<DcRec>(), A.d_bt.as<unsigned long long>(), rlr, p->trellis_delta_dc_weight > 0.0f, dc_fast_of(gr), so.dcq, so.keep_coef, n, s);
     }
     return B200JPEG_OK;
     };
@@ -1017,9 +1061,13 @@ static int finish_chunk(b200jpeg_encoder *e, const ChunkIO &io, int k)
         }
       }
       if (k2 == 0) {
-        if (pl.trellis && p->trellis_q_opt) {                       // this image's re-fitted tables go into its DQT (jcmaster.c:1014-1030)
+        // the image's own tables go into its DQT and decide its SOF0 / SOF1: the re-fitted ones under trellis_q_opt
+        // (jcmaster.c:1014-1030), else those of its table set
+        const uint16_t *qimg = pl.trellis && p->trellis_q_opt ? e->h_qimg.as<uint16_t>() + (size_t)gi * 256
+                             : !e->img_set.empty() ? &e->qsets[(size_t)e->img_set[gi] * 256] : nullptr;
+        if (qimg) {
           static thread_local b200jpeg_params pq;
-          pq = *p; memcpy(pq.quant_tbl, e->h_qimg.as<uint16_t>() + (size_t)gi * 256, 512);
+          pq = *p; memcpy(pq.quant_tbl, qimg, 512);
           write_frame_header(&pq, pl.progressive, o);
         } else write_frame_header(p, pl.progressive, o);
       }
@@ -1082,18 +1130,52 @@ static int choose_chunk(const b200jpeg_encoder *e, const Plan &pl, int n_images,
 // raw-data input (jpeg_write_raw_data): one plane per component instead of interleaved pixels
 struct RawDesc { const uint8_t *plane[4]; size_t pitch[4], stride[4]; bool coefs; };   // pitch, stride in bytes; coefs: planes hold JBLOCK rows
 
+// The batch's quantization table sets: without per-image tables one set, the parameter block's; with them
+// (qtables: [n_images][4][64], natural order, the slots quant_tbl_present names) the distinct ones, in order of first
+// use, and every image's set.
+static int collect_qsets(b200jpeg_encoder *e, const b200jpeg_params *p, const uint16_t *qtables, int n_images)
+{
+  e->qsets.assign(&p->quant_tbl[0][0], &p->quant_tbl[0][0] + 256);
+  e->img_set.clear(); e->nsets = 1;
+  if (!qtables) return B200JPEG_OK;
+  for (int i = 0; i < n_images; i++)
+    for (int t = 0; t < 4; t++) {
+      if (!p->quant_tbl_present[t]) continue;
+      for (int k = 0; k < 64; k++) {
+        const unsigned v = qtables[((size_t)i * 4 + t) * 64 + k];
+        if (v < 1 || v > 32767) { set_error("image %d: quantization table %d: entry %d is %u, outside 1..32767", i, t, k, v); return B200JPEG_ERR_PARAM; }
+      }
+    }
+  e->qsets.clear(); e->img_set.resize(n_images);
+  std::map<std::string, int> seen;
+  std::vector<uint16_t> set(256);
+  for (int i = 0; i < n_images; i++) {
+    for (int t = 0; t < 4; t++)
+      memcpy(&set[(size_t)t * 64], p->quant_tbl_present[t] ? qtables + ((size_t)i * 4 + t) * 64 : p->quant_tbl[t], 128);
+    auto ins = seen.emplace(std::string(reinterpret_cast<const char *>(set.data()), 512), (int)seen.size());
+    if (ins.second) e->qsets.insert(e->qsets.end(), set.begin(), set.end());
+    e->img_set[i] = ins.first->second;
+  }
+  e->nsets = (int)seen.size();
+  return B200JPEG_OK;
+}
+
 static int encode_common(b200jpeg_encoder *e, const b200jpeg_params *p, const void *pixels, int on_device,
-                         size_t row_pitch, size_t image_stride, int n_images, bool device_only, const RawDesc *raw = nullptr)
+                         size_t row_pitch, size_t image_stride, int n_images, bool device_only, const RawDesc *raw = nullptr,
+                         const uint16_t *qtables = nullptr)
 {
   if (!e || !p || (!pixels && !raw) || n_images <= 0) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
   int rc = b200jpeg_validate(p);
   if (rc) return rc;
   const size_t sample_bytes = p->data_precision > 8 ? 2 : 1;                       // 12-bit samples are uint16 (J12SAMPLE)
   const size_t row_bytes = (size_t)p->image_width * p->input_components * sample_bytes;
+  // per-image tables allow a zero image stride: every image reads the same input (a quality ladder)
+  const bool shared_ok = qtables != nullptr;
   if (!raw) {
     if (row_pitch < row_bytes) { set_error("row_pitch smaller than a row"); return B200JPEG_ERR_PARAM; }
-    if (n_images > 1 && image_stride < row_pitch * (size_t)(p->image_height - 1) + row_bytes) { set_error("image_stride smaller than an image"); return B200JPEG_ERR_PARAM; }
+    if (n_images > 1 && !(shared_ok && image_stride == 0) && image_stride < row_pitch * (size_t)(p->image_height - 1) + row_bytes) { set_error("image_stride smaller than an image"); return B200JPEG_ERR_PARAM; }
   }
+  if ((rc = collect_qsets(e, p, qtables, n_images))) return rc;
   CU(cudaSetDevice(e->device));
   e->params = *p; e->n = n_images;
   if ((rc = build_plan(p, row_pitch, image_stride, e->plan))) return rc;
@@ -1106,7 +1188,7 @@ static int encode_common(b200jpeg_encoder *e, const b200jpeg_params *p, const vo
     g.raw_in = 2;
     for (int ci = 0; ci < g.nc; ci++) {
       const size_t rows = (size_t)g.c[ci].hib, cols = (size_t)g.c[ci].wib * 128;
-      if (!raw->plane[ci] || raw->pitch[ci] < cols || (n_images > 1 && raw->stride[ci] < raw->pitch[ci] * (rows - 1) + cols)) { set_error("coefficient plane %d: bad pointer, pitch or stride (needs %zu rows of %zu blocks)", ci, rows, cols / 128); return B200JPEG_ERR_PARAM; }
+      if (!raw->plane[ci] || raw->pitch[ci] < cols || (n_images > 1 && !(shared_ok && raw->stride[ci] == 0) && raw->stride[ci] < raw->pitch[ci] * (rows - 1) + cols)) { set_error("coefficient plane %d: bad pointer, pitch or stride (needs %zu rows of %zu blocks)", ci, rows, cols / 128); return B200JPEG_ERR_PARAM; }
       raw_plane_bytes[ci] = raw->pitch[ci] * (rows - 1) + cols;
       raw_total[ci] = raw->stride[ci] * (size_t)(n_images - 1) + raw_plane_bytes[ci];
       raw_off[ci] = raw_sum; raw_sum += (raw_total[ci] + 255) & ~(size_t)255;
@@ -1118,7 +1200,7 @@ static int encode_common(b200jpeg_encoder *e, const b200jpeg_params *p, const vo
     g.raw_in = 1;
     for (int ci = 0; ci < g.nc; ci++) {
       const size_t rows = (size_t)g.c[ci].hib * 8, cols = (size_t)g.c[ci].wib * 8;      // what compress_first_pass reads (jccoefct.c:262-353)
-      if (!raw->plane[ci] || raw->pitch[ci] < cols || (n_images > 1 && raw->stride[ci] < raw->pitch[ci] * (rows - 1) + cols)) { set_error("raw-data plane %d: bad pointer, pitch or stride (needs %zu rows of %zu samples)", ci, rows, cols); return B200JPEG_ERR_PARAM; }
+      if (!raw->plane[ci] || raw->pitch[ci] < cols || (n_images > 1 && !(shared_ok && raw->stride[ci] == 0) && raw->stride[ci] < raw->pitch[ci] * (rows - 1) + cols)) { set_error("raw-data plane %d: bad pointer, pitch or stride (needs %zu rows of %zu samples)", ci, rows, cols); return B200JPEG_ERR_PARAM; }
       raw_plane_bytes[ci] = raw->pitch[ci] * (rows - 1) + cols;
       raw_total[ci] = raw->stride[ci] * (size_t)(n_images - 1) + raw_plane_bytes[ci];
       raw_off[ci] = raw_sum; raw_sum += (raw_total[ci] + 255) & ~(size_t)255;
@@ -1166,12 +1248,14 @@ static int encode_common(b200jpeg_encoder *e, const b200jpeg_params *p, const vo
     if (!on_device) {
       for (int k = 0; k < nchunks; k++) {
         const int i0 = k * C, nk = std::min(C, n_images - i0);
+        // input shared by every image (zero stride) is staged once, with the first chunk
         if (raw) {
           for (int ci = 0; ci < pl.g.nc; ci++) {
+            if (k > 0 && raw->stride[ci] == 0) continue;
             const size_t off = (size_t)i0 * raw->stride[ci], bytes = raw->stride[ci] * (size_t)(nk - 1) + raw_plane_bytes[ci];
             CU(cudaMemcpyAsync(e->d_src.as<uint8_t>() + raw_off[ci] + off, raw->plane[ci] + off, bytes, cudaMemcpyHostToDevice, e->s_in));
           }
-        } else {
+        } else if (k == 0 || image_stride != 0) {
           const size_t off = (size_t)i0 * image_stride, bytes = image_stride * (size_t)(nk - 1) + image_bytes;
           CU(cudaMemcpyAsync(e->d_src.as<uint8_t>() + off, static_cast<const uint8_t *>(pixels) + off, bytes, cudaMemcpyHostToDevice, e->s_in));
         }
@@ -1201,6 +1285,7 @@ static int encode_common(b200jpeg_encoder *e, const b200jpeg_params *p, const vo
       io.tabs_scan = e->d_tabs_scan.as<DevHuff>() + (size_t)io.i0 * nscans * HIST_SLOTS;
       io.best_al = e->d_best_al_all.as<int>() + (size_t)io.i0 * 2;
       io.qimg = e->d_qimg_all.as<uint16_t>() + (size_t)io.i0 * 256;
+      io.qset = e->img_set.empty() ? nullptr : e->d_qset.as<int>() + io.i0;
       if (!on_device) { tm.s = e->sc[io.slot]; tm.mark("h2d_wait"); CU(cudaStreamWaitEvent(e->sc[io.slot], e->ev_in[k], 0)); }
       if ((rc = run_pipeline(e, io, tm))) break;
       if (!device_only) {
@@ -1286,10 +1371,10 @@ void b200jpeg_encoder_destroy(b200jpeg_encoder *e)
   if (e->s_in) cudaStreamSynchronize(e->s_in);
   if (e->s_out) cudaStreamSynchronize(e->s_out);
   for (int i = 1; i < MAX_ARENAS; i++) if (e->sc[i]) cudaStreamSynchronize(e->sc[i]);
-  DevBuf *db[] = {&e->d_src, &e->d_tabs_scan, &e->d_tabs_fixed, &e->d_status, &e->d_out_pos, &e->d_scan_size, &e->d_out, &e->d_qt, &e->d_tc, &e->d_best_al_all, &e->d_qimg_all};
+  DevBuf *db[] = {&e->d_src, &e->d_tabs_scan, &e->d_tabs_fixed, &e->d_status, &e->d_out_pos, &e->d_scan_size, &e->d_out, &e->d_qt, &e->d_tc, &e->d_best_al_all, &e->d_qimg_all, &e->d_qset};
   for (DevBuf *b : db) b->release();
   for (int i = 0; i < MAX_ARENAS; i++) e->ar[i].release();
-  PinBuf *pb[] = {&e->h_qt, &e->h_tc, &e->h_fixed, &e->h_status, &e->h_out_pos, &e->h_scan_size, &e->h_tabs, &e->h_stage, &e->h_best_al, &e->h_qinit, &e->h_qimg};
+  PinBuf *pb[] = {&e->h_qt, &e->h_tc, &e->h_fixed, &e->h_status, &e->h_out_pos, &e->h_scan_size, &e->h_tabs, &e->h_stage, &e->h_best_al, &e->h_qinit, &e->h_qimg, &e->h_qset};
   for (PinBuf *b : pb) b->release();
   for (PinBuf &b : e->file_arenas) b.release();
   for (cudaEvent_t ev : e->ev) cudaEventDestroy(ev);
@@ -1365,6 +1450,35 @@ int b200jpeg_encode_batch_coefs(b200jpeg_encoder *enc, const b200jpeg_params *p,
   b200jpeg_params q = *p;
   q.overshoot_deringing = 0; q.smoothing_factor = 0; q.dct_method = B200JPEG_DCT_ISLOW;
   return encode_common(enc, &q, nullptr, planes_on_device, 0, 0, n_images, false, &rd);
+}
+
+int b200jpeg_encode_batch_qtables(b200jpeg_encoder *enc, const b200jpeg_params *p, const void *pixels, int pixels_on_device,
+                                  size_t row_pitch, size_t image_stride, const uint16_t *qtables, int n_images)
+{
+  if (!qtables) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
+  return encode_common(enc, p, pixels, pixels_on_device, row_pitch, image_stride, n_images, false, nullptr, qtables);
+}
+
+int b200jpeg_encode_batch_raw_qtables(b200jpeg_encoder *enc, const b200jpeg_params *p, const uint8_t *const *planes, int planes_on_device,
+                                      const size_t *row_pitch, const size_t *image_stride, const uint16_t *qtables, int n_images)
+{
+  if (!enc || !p || !planes || !row_pitch || !image_stride || !qtables) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
+  RawDesc rd; memset(&rd, 0, sizeof rd);
+  for (int ci = 0; ci < p->num_components && ci < 4; ci++) { rd.plane[ci] = planes[ci]; rd.pitch[ci] = row_pitch[ci]; rd.stride[ci] = image_stride[ci]; }
+  return encode_common(enc, p, nullptr, planes_on_device, 0, 0, n_images, false, &rd, qtables);
+}
+
+int b200jpeg_encode_batch_coefs_qtables(b200jpeg_encoder *enc, const b200jpeg_params *p, const int16_t *const *planes, int planes_on_device,
+                                        const size_t *row_pitch_blocks, const size_t *image_stride_blocks, const uint16_t *qtables, int n_images)
+{
+  if (!enc || !p || !planes || !row_pitch_blocks || !image_stride_blocks || !qtables) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
+  RawDesc rd; memset(&rd, 0, sizeof rd); rd.coefs = true;
+  for (int ci = 0; ci < p->num_components && ci < 4; ci++) {
+    rd.plane[ci] = reinterpret_cast<const uint8_t *>(planes[ci]); rd.pitch[ci] = row_pitch_blocks[ci] * 128; rd.stride[ci] = image_stride_blocks[ci] * 128;
+  }
+  b200jpeg_params q = *p;                 // as b200jpeg_encode_batch_coefs
+  q.overshoot_deringing = 0; q.smoothing_factor = 0; q.dct_method = B200JPEG_DCT_ISLOW;
+  return encode_common(enc, &q, nullptr, planes_on_device, 0, 0, n_images, false, &rd, qtables);
 }
 
 int b200jpeg_get_output(b200jpeg_encoder *e, int i, const uint8_t **data, size_t *size)

@@ -244,6 +244,8 @@ __global__ void __launch_bounds__(128) k_forward(Geom g, const uint8_t *__restri
   int bx = blockIdx.x * blockDim.x + threadIdx.x;
   int by = blockIdx.y;
   if (bx >= c.wib || by >= c.hib) return;
+  // the image's table set, re-derived at each use (a pointer held across the kernel costs spills)
+  auto set = [&] { return qset_of(qt, g, img); };
   const uint8_t *base = src + (size_t)img * g.image_stride;
   int ws[64];
   const int comp = g.cs_mode == 1 ? 0 : ci;
@@ -286,12 +288,12 @@ __global__ void __launch_bounds__(128) k_forward(Geom g, const uint8_t *__restri
     int sum = 0, cnt = 0;
 #pragma unroll
     for (int i = 0; i < 64; i++) { wf[i] = (float)ws[i]; sum += ws[i]; cnt += (ws[i] >= 127); }
-    if (dering && cnt != 0 && cnt != 64) deringing_block_float(wf, (int)qt->q[c.qt][0].d >> 3, (float)sum, cnt);
+    if (dering && cnt != 0 && cnt != 64) deringing_block_float(wf, (int)set()->q[c.qt][0].d >> 3, (float)sum, cnt);
 #pragma unroll
     for (int r = 0; r < 8; r++) fdct_float_1d(wf[8 * r], wf[8 * r + 1], wf[8 * r + 2], wf[8 * r + 3], wf[8 * r + 4], wf[8 * r + 5], wf[8 * r + 6], wf[8 * r + 7]);
 #pragma unroll
     for (int col = 0; col < 8; col++) fdct_float_1d(wf[col], wf[8 + col], wf[16 + col], wf[24 + col], wf[32 + col], wf[40 + col], wf[48 + col], wf[56 + col]);
-    const float *fd = qt->fdiv[c.qt];
+    const float *fd = set()->fdiv[c.qt];
 #pragma unroll
     for (int i = 0; i < 64; i++) {
       float v = wf[i];
@@ -311,7 +313,7 @@ __global__ void __launch_bounds__(128) k_forward(Geom g, const uint8_t *__restri
         int tmp[64];
 #pragma unroll
         for (int i = 0; i < 64; i++) tmp[i] = ws[i];
-        deringing_block(LocalAcc{tmp}, (int)qt->q[c.qt][0].d >> 3, sum, cnt);
+        deringing_block(LocalAcc{tmp}, (int)set()->q[c.qt][0].d >> 3, sum, cnt);
 #pragma unroll
         for (int i = 0; i < 64; i++) ws[i] = tmp[i];
       }
@@ -321,7 +323,7 @@ __global__ void __launch_bounds__(128) k_forward(Geom g, const uint8_t *__restri
       for (int r = 0; r < 8; r++) fdct_ifast_1d(ws[8 * r], ws[8 * r + 1], ws[8 * r + 2], ws[8 * r + 3], ws[8 * r + 4], ws[8 * r + 5], ws[8 * r + 6], ws[8 * r + 7]);
 #pragma unroll
       for (int col = 0; col < 8; col++) fdct_ifast_1d(ws[col], ws[8 + col], ws[16 + col], ws[24 + col], ws[32 + col], ws[40 + col], ws[48 + col], ws[56 + col]);
-      const IfastConst *ic = qt->ifast[c.qt];
+      const IfastConst *ic = set()->ifast[c.qt];
 #pragma unroll
       for (int i = 0; i < 64; i++) {
         const int x = ws[i], sc = c_aanscales[i];
@@ -332,7 +334,7 @@ __global__ void __launch_bounds__(128) k_forward(Geom g, const uint8_t *__restri
           q = (int)(int16_t)(int)(((unsigned long long)(unsigned)(a + (int)k.corr) * k.recip) >> (k.shift + 32));
         } else {
           // 12-bit build: the scaled divisor stays a JLONG (jcdctmgr.c:332-336) and quantize() divides literally (:646-678)
-          const int d = (int)(((long long)((int)qc_d(qt, c.qt, i) >> 3) * sc + (1 << 10)) >> 11);
+          const int d = (int)(((long long)((int)qc_d(set(), c.qt, i) >> 3) * sc + (1 << 10)) >> 11);
           q = (int)(int16_t)((a + (d >> 1)) / d);
         }
         if (x < 0) q = (int)(int16_t)(-q);
@@ -349,7 +351,7 @@ __global__ void __launch_bounds__(128) k_forward(Geom g, const uint8_t *__restri
         fdct_1d<1, P1>(ws[col], ws[8 + col], ws[16 + col], ws[24 + col], ws[32 + col], ws[40 + col], ws[48 + col], ws[56 + col]);
     }
   }
-  const QuantConst *qc = qt->q[c.qt];
+  const QuantConst *qc = set()->q[c.qt];
   if (rec) {       // side record for the trellis: norm numerator in natural order (jcdctmgr.c:1026-1029), raw DC, #non-zero ACs
     float norm = 0.0f; unsigned long long mask = 0;
 #pragma unroll
@@ -518,6 +520,7 @@ __global__ void __launch_bounds__(128, FWD_MIN_CTAS) k_forward_tile(Geom g, cons
   const int tx = blockIdx.x, ty = blockIdx.y, img = blockIdx.z;
   const int x0 = tx * TW, y0 = ty * TR;
   const uint8_t *base = src + (size_t)img * g.image_stride;
+  qt = qset_of(qt, g, img);
 
   for (int i = tid; i < NC * 64; i += 128) { int ci = i >> 6, n = i & 63; const QuantConst &k = qt->q[g.c[ci].qt][n]; sQC[ci][n] = make_uint2(k.mul2, k.bias << 14); }
   if (tid < NC) sQL[tid] = qt->L[g.c[tid].qt];
@@ -539,7 +542,7 @@ __global__ void __launch_bounds__(128, FWD_MIN_CTAS) k_forward_tile(Geom g, cons
       for (int bx = 0; bx < TMA_NBOX; bx++)
         asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];"
                      :: "r"((unsigned)__cvta_generic_to_shared(sIO + bx * TMA_BOXW * TR)), "l"(reinterpret_cast<unsigned long long>(&tmap)),
-                        "r"(x0 * IC + bx * TMA_BOXW), "r"(y0), "r"(img), "r"(bar) : "memory");
+                        "r"(x0 * IC + bx * TMA_BOXW), "r"(y0), "r"(g.image_stride ? img : 0), "r"(bar) : "memory");   // stride 0: one image for all
     }
     __syncthreads();                                             // the barrier word is initialised before anyone polls it
     {
@@ -953,13 +956,15 @@ static EncodeTiledFn tensor_map_encoder()
 }
 // The batch's pixels as a rank-3 byte tensor {W * samples per pixel, H, n}; box = one tile (or half of one) of the
 // forward kernel.  Returns 0 when the layout does not qualify (alignment, pixel order, sample size): the kernel
-// then loads with ordinary global loads.
+// then loads with ordinary global loads.  A zero image stride (every image reads the same pixels) maps one image,
+// which the kernel addresses as image 0.
 static int make_pixel_tensor_map(const Geom &g, const uint8_t *src, int n, int ic, int tile_rows, CUtensorMap *tm)
 {
   static const bool off = getenv("B200JPEG_NO_TMA") != nullptr;     // A/B aid
   memset(tm, 0, sizeof *tm);
   EncodeTiledFn enc = tensor_map_encoder();
   if (off || !enc || g.raw_in || !src || g.in_comps != ic || g.px_swap || g.px_first || g.max_coef_bits != 10) return 0;
+  if (g.image_stride == 0) n = 1;
   if (((size_t)src & 15) || (g.row_pitch & 15) || (n > 1 && (g.image_stride & 15))) return 0;
   const cuuint64_t dims[3] = {(cuuint64_t)g.W * ic, (cuuint64_t)g.H, (cuuint64_t)n};
   const cuuint64_t strides[2] = {(cuuint64_t)g.row_pitch, (cuuint64_t)(n > 1 ? g.image_stride : ((g.row_pitch * (size_t)g.H + 15) & ~(size_t)15))};
@@ -1676,6 +1681,7 @@ __global__ void __launch_bounds__(128) k_trellis_ac_band(Geom g, const TrellisCo
   __shared__ uint8_t acsi[256];
   const long long nblk = (long long)c.wib * c.hib;
   if ((long long)blockIdx.x * blockDim.x >= nblk) return;
+  tc = qset_of(tc, g, img);
   {
     const DevHuff *ac = reinterpret_cast<const DevHuff *>(reinterpret_cast<const char *>(tabs) + (size_t)blockIdx.y * tabs_set_stride) + (4 + c.ac_tbl);
     for (int i = threadIdx.x; i < 256; i += blockDim.x) acsi[i] = ac->size[i];
@@ -2102,12 +2108,13 @@ k_trellis_ac3(Geom g, const TrellisConsts *__restrict__ tc, const DevHuff *__res
   {
     const DevHuff *ac = reinterpret_cast<const DevHuff *>(reinterpret_cast<const char *>(tabs) + (size_t)blockIdx.y * tabs_set_stride) + (4 + c.ac_tbl);
     for (int i = tid; i < 256; i += T3_THREADS) acsi[i] = ac->size[i];
+    const TrellisConsts *tq = qset_of(tc, g, img);             // the image's table set (the other fields are the batch's)
     if (tid < 64) {
-      const float w = tc->w_zz[c.qt][tid];
+      const float w = tq->w_zz[c.qt][tid];
       swz[tid] = w;
-      sEnt[tid] = make_uint4((unsigned)tc->q8_zz[c.qt][tid], tc->qmul_zz[c.qt][tid], __float_as_uint(w), 0u);
+      sEnt[tid] = make_uint4((unsigned)tq->q8_zz[c.qt][tid], tq->qmul_zz[c.qt][tid], __float_as_uint(w), 0u);
     }
-    if (tid == 0) sqL = tc->qL[c.qt];
+    if (tid == 0) sqL = tq->qL[c.qt];
   }
   __syncthreads();
   for (int e = tid; e < 640; e += T3_THREADS) {
@@ -2418,7 +2425,7 @@ __global__ void __launch_bounds__(64) k_trellis_dc(Geom g, const TrellisConsts *
   int imcu = blockIdx.x * blockDim.x + threadIdx.x;
   int n_imcu = (c.hib + c.v - 1) / c.v;
   if (imcu >= n_imcu) return;
-  const int q = tc->q8_zz[c.qt][0];
+  const int q = qset_of(tc, g, img)->q8_zz[c.qt][0];            // the image's table set (the other fields are the batch's)
   int ncand = (2 + 60 / (q >> 3)) | 1; if (ncand > 9) ncand = 9;     // get_num_dc_trellis_candidates (:929-933)
   const int half = ncand / 2;
   const int lim = 1 << tc->max_coef_bits;
@@ -2526,6 +2533,7 @@ __global__ void __launch_bounds__(64) k_trellis_dc_warp(Geom g, const TrellisCon
   const bool active = grp < 3 && imcu < n_imcu;
   int16_t *qs = reinterpret_cast<int16_t *>(dsm) + (size_t)chain_in_cta * max_wib;
   uint8_t *bt8 = dsm + (size_t)chains_per_cta * max_wib * 2 + (size_t)chain_in_cta * max_wib * 9;
+  tc = qset_of(tc, g, img);
   const int q = tc->q8_zz[c.qt][0];
   int ncand = (2 + 60 / (q >> 3)) | 1; if (ncand > 9) ncand = 9;
   const int half = ncand / 2;
@@ -2614,7 +2622,6 @@ __global__ void __launch_bounds__(64) k_trellis_dc_warp(Geom g, const TrellisCon
 #define DC_TABLE 1
 #endif
 #define DC_TAB_HALF 512
-struct DcDiv { unsigned mul[4]; int shift[4]; };
 // FLO: index of the most significant set bit, 0xFFFFFFFF for 0, so that
 // nbits(v) == bfind(v) + 1 (JPEG_NBITS) without the clz arithmetic.
 __device__ __forceinline__ int bfind_u32(unsigned v) { int r; asm("bfind.u32 %0, %1;" : "=r"(r) : "r"(v)); return r; }
@@ -2625,7 +2632,7 @@ __device__ __forceinline__ int bfind_u32(unsigned v) { int r; asm("bfind.u32 %0,
 template <bool FAST>
 __global__ void __launch_bounds__(DC2_WARPS * 32) k_trellis_dc_v2(Geom g, const TrellisConsts *__restrict__ tc,
                                                                  const DevHuff *__restrict__ tabs, size_t tabs_set_stride,
-                                                                 const DcRec *__restrict__ rec, RecLayout rl, int max_wib, DcDiv dv, int16_t *__restrict__ dcq, int write_coef)
+                                                                 const DcRec *__restrict__ rec, RecLayout rl, int max_wib, int16_t *__restrict__ dcq, int write_coef)
 {
   extern __shared__ __align__(16) unsigned char dsm[];
   __shared__ float T[36];                                   // T[1 + bfind(|d|)] = (float)(bits + ehufsi[bits])
@@ -2653,6 +2660,7 @@ __global__ void __launch_bounds__(DC2_WARPS * 32) k_trellis_dc_v2(Geom g, const 
   // low nibble, and after the back-track the block's chosen candidate in the high nibble)
   uint8_t *btw = dsm + (size_t)warp * 3 * max_wib * 5;          // [3][max_wib][5]
   uint8_t *bt = btw + (size_t)gsel * max_wib * 5;
+  tc = qset_of(tc, g, img);
   const int q = tc->q8_zz[c.qt][0];
   int ncand = (2 + 60 / (q >> 3)) | 1; if (ncand > 9) ncand = 9;     // get_num_dc_trellis_candidates (:929-933)
   const int half = ncand / 2;
@@ -2660,7 +2668,7 @@ __global__ void __launch_bounds__(DC2_WARPS * 32) k_trellis_dc_v2(Geom g, const 
   const float INF = __int_as_float(0x7f800000);
   const size_t comp_rec = (size_t)img * rl.per_image + rl.comp_off[ci];
   const int qhalf = q / 2;
-  const unsigned qmul = dv.mul[ci]; const int qshift = dv.shift[ci];
+  const unsigned qmul = tc->dc_mul[c.qt]; const int qshift = tc->dc_shift[c.qt];
   int last_dc = 0;                                                // per chain (uniform inside a 9-lane group)
   for (int br = 0; br < c.v; br++) {
     // rows of the three chains; a chain without this row idles on row 0 of the component
@@ -2788,7 +2796,7 @@ __global__ void __launch_bounds__(DC2_WARPS * 32) k_trellis_dc_v2(Geom g, const 
 }
 
 void launch_trellis_dc(const Geom &g, const TrellisConsts *tc, const DevHuff *tabs, size_t tabs_set_stride,
-                       const DcRec *rec, unsigned long long *bt, const RecLayout &rl, int vertical, int16_t *dcq, int write_coef, int n, cudaStream_t s)
+                       const DcRec *rec, unsigned long long *bt, const RecLayout &rl, int vertical, int dc_fast, int16_t *dcq, int write_coef, int n, cudaStream_t s)
 {
   int n_imcu = 0, max_wib = 0;
   for (int ci = 0; ci < g.nc; ci++) { n_imcu = max(n_imcu, (g.c[ci].hib + g.c[ci].v - 1) / g.c[ci].v); max_wib = max(max_wib, g.c[ci].wib); }
@@ -2808,19 +2816,9 @@ void launch_trellis_dc(const Geom &g, const TrellisConsts *tc, const DevHuff *ta
     // (per device, so not cached: encoders on several GPUs may live in one process)
     if (smem2 > 40 * 1024) { cudaFuncSetAttribute(k_trellis_dc_v2<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024); cudaFuncSetAttribute(k_trellis_dc_v2<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024); }
     dim3 grid((n_imcu + DC2_WARPS * 3 - 1) / (DC2_WARPS * 3), n * g.nc);
-    // the DC quantizer per component as an exact multiply-shift division (like make_quant_consts)
-    DcDiv dv; bool fast = true;
-    for (int ci = 0; ci < 4; ci++) { dv.mul[ci] = 0; dv.shift[ci] = 0; }
-    for (int ci = 0; ci < g.nc; ci++) {
-      const unsigned d = (unsigned)g.c[ci].dc_q8;
-      int l = 0; while ((1ull << l) < d) l++;
-      dv.shift[ci] = 18 + l;
-      dv.mul[ci] = (unsigned)(((1ull << dv.shift[ci]) + d - 1) / d);
-      int ncand = (2 + 60 / (int)(d >> 3)) | 1; if (ncand > 9) ncand = 9;
-      fast = fast && ncand == 9 && (int)((32768 + d / 2) / d) + 9 < (1 << g.max_coef_bits) - 1;
-    }
-    if (fast) k_trellis_dc_v2<true><<<grid, DC2_WARPS * 32, smem2, s>>>(g, tc, tabs, tabs_set_stride, rec, rl, max_wib, dv, dcq, write_coef || !dcq);
-    else k_trellis_dc_v2<false><<<grid, DC2_WARPS * 32, smem2, s>>>(g, tc, tabs, tabs_set_stride, rec, rl, max_wib, dv, dcq, write_coef || !dcq);
+    // the DC quantizer comes from each image's table set (TrellisConsts.dc_mul / dc_shift)
+    if (dc_fast) k_trellis_dc_v2<true><<<grid, DC2_WARPS * 32, smem2, s>>>(g, tc, tabs, tabs_set_stride, rec, rl, max_wib, dcq, write_coef || !dcq);
+    else k_trellis_dc_v2<false><<<grid, DC2_WARPS * 32, smem2, s>>>(g, tc, tabs, tabs_set_stride, rec, rl, max_wib, dcq, write_coef || !dcq);
     LAUNCHED();
     return;
   }

@@ -27,7 +27,6 @@ struct CompGeom {
   int qt;              // quant table slot
   int dc_tbl, ac_tbl;  // Huffman table slots
   int rows_avail;      // downsampled rows holding real data (jcprepct.c:135-192)
-  int dc_q8;           // 8 * quantval[0] of the component's table
   long long blocks_per_image;   // wpad*hpad
   int16_t *coef, *raw;
 };
@@ -45,8 +44,13 @@ struct Geom {
   // plane ci holds at least hib*8 rows of wib*8 samples; pitch and stride in bytes
   int raw_in;          // 1: sample planes; 2: quantized coefficient blocks (jpeg_write_coefficients), natural order
   const uint8_t *plane[4]; size_t plane_pitch[4], plane_stride[4];
+  // per-image quantization: qset[img] (img counted inside the launch) is the index of the image's table set in the
+  // QuantTables / TrellisConsts arrays the kernels receive; nullptr = every image uses set 0
+  const int *qset;
   CompGeom c[4];
 };
+// the image's table set: base + qset[img]
+template <class T> __device__ __forceinline__ const T *qset_of(const T *base, const Geom &g, int img) { return g.qset ? base + g.qset[img] : base; }
 
 // component planes written by the input-smoothing pre-pass (pitch, stride in bytes)
 struct PlanesOut { uint8_t *p[4]; size_t pitch[4], stride[4]; };
@@ -82,6 +86,9 @@ struct TrellisConsts {
   int   use_norm;         // lambda_log_scale2 > 0
   int   max_coef_bits;    // data_precision + 2
   int   dc_trellis;       // trellis_quant_dc
+  // the DC trellis' quantizer per table: (x + 4Q) / 8Q as an exact multiply-shift (like make_quant_consts), and whether
+  // the table allows its FAST instantiation (9 candidates, no clamping reachable)
+  unsigned dc_mul[4]; int dc_shift[4]; int dc_fast[4];
 };
 
 // Huffman table as the device keeps it: DHT payload + derived encode table.
@@ -133,6 +140,8 @@ struct SymOut { uint8_t *sym; int16_t *dcq; uint32_t *hist; int keep_coef; int d
 // ---------------------------------------------------------------- launches (defined in kernels.cu)
 // status[img] bits: 2 = JERR_BAD_DCT_COEF / missing Huffman code, 4 = output buffer too small (host retries)
 // the raw DCT plane is written only when the trellis (rec != nullptr) or the debug tap (keep_raw) will read it
+// qt / tc (here and in the trellis launches): the batch's table sets, image img reads set g.qset[img] (qset_of);
+// qfast / dc_fast: every set the launch's images use allows the fast form
 void launch_prep_planes(const Geom &g, const uint8_t *src, int smoothing_factor, const PlanesOut &out, int n, cudaStream_t s);
 void launch_import_coefs(const Geom &g, int n, cudaStream_t s);     // raw_in == 2: planes hold JBLOCK rows
 void launch_forward(const Geom &g, const uint8_t *src, const QuantTables *qt, int qfast, int dct_method /* J_DCT_METHOD */, int dering, DcRec *rec, const RecLayout &rl, int keep_raw, int n, cudaStream_t s);
@@ -160,7 +169,7 @@ void launch_qopt_update(long long *qsum, uint16_t *qimg, int n, cudaStream_t s);
 // dcq (or nullptr): dense array of the final DC values, one per real block, indexed like the side records; with it and
 // write_coef == 0 the coefficient planes are not touched (where the kernel in use can do without)
 void launch_trellis_dc(const Geom &g, const TrellisConsts *tc, const DevHuff *tabs, size_t tabs_set_stride,
-                       const DcRec *rec, unsigned long long *bt, const RecLayout &rl, int vertical, int16_t *dcq, int write_coef, int n, cudaStream_t s);
+                       const DcRec *rec, unsigned long long *bt, const RecLayout &rl, int vertical, int dc_fast, int16_t *dcq, int write_coef, int n, cudaStream_t s);
 // DC statistics of a sequential scan from the dense DC array (+ the EOB of every dummy block): with the AC counts the
 // trellis back-track left in `hist`, the scan's complete statistics (encode_mcu_gather, jchuff.c:886-915)
 void launch_gather_seq_dc(const Geom &g, const ScanDesc &sd, const int16_t *dcq, const RecLayout &rl, uint32_t *hist, uint32_t *status, int n, cudaStream_t s);

@@ -27,6 +27,8 @@ import ctypes as C
 import struct
 from typing import Dict, List, Sequence, Tuple
 
+import numpy as np
+
 from . import _abi as A
 from .cjpeg import UsageError, _keymatch
 
@@ -219,12 +221,30 @@ def params_for_transcode(src: SourceInfo, switches: Sequence[str]) -> Tuple[A.Pa
     return p, prefer_smallest
 
 
+def _same_except_quant(a: SourceInfo, b: SourceInfo) -> bool:
+    """Everything jpeg_copy_critical_parameters reads from a source, except the quantization tables' values: geometry,
+    components, sampling, slot mapping and defined slots, precision, colour space, JFIF fields."""
+    keys = ("image_width", "image_height", "data_precision", "num_components", "comps", "jpeg_color_space",
+            "saw_JFIF", "JFIF_version", "density", "saw_Adobe", "Adobe_transform")
+    return all(getattr(a, k) == getattr(b, k) for k in keys) and sorted(a.quant) == sorted(b.quant)
+
+
 def transcode(encoder, sources: Sequence[bytes], coef_planes: Sequence[Sequence], switches: Sequence[str]) -> List[bytes]:
     """``jpegtran <switches>`` on same-shaped source files: sources[i] is the original file, coef_planes[ci] an
-    (N, height_in_blocks, width_in_blocks, 64) int16 array of its quantized coefficients (natural order)."""
-    src = parse_header(sources[0])
-    p, prefer_smallest = params_for_transcode(src, switches)
-    out = encoder.encode_batch_coefs(p, coef_planes)
+    (N, height_in_blocks, width_in_blocks, 64) int16 array of its quantized coefficients (natural order).
+    Every source keeps its own quantization tables (its DQT); everything else jpeg_copy_critical_parameters takes
+    from a source must match the first one, else ValueError names the first source that differs."""
+    infos = [parse_header(s) for s in sources]
+    for i, info in enumerate(infos[1:], 1):
+        if not _same_except_quant(infos[0], info):
+            raise ValueError(f"source {i} differs from source 0 in more than its quantization tables")
+    p, prefer_smallest = params_for_transcode(infos[0], switches)
+    qt = np.zeros((len(infos), A.NUM_QUANT_TBLS, 64), dtype=np.uint16)
+    for i, info in enumerate(infos):
+        qt[i] = np.ctypeslib.as_array(p.quant_tbl)
+        for slot, vals in info.quant.items():
+            qt[i, slot] = vals
+    out = encoder.encode_batch_coefs(p, coef_planes, qtables=qt)
     if prefer_smallest and p.compress_profile == A.PROFILE_MAX_COMPRESSION:
         out = [s if len(s) < len(o) else o for s, o in zip(sources, out)]      # jpegtran.c:772-775
     return out

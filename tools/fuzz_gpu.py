@@ -1,6 +1,7 @@
 #!/usr/bin/env python3
 """Randomised device-vs-oracle cross-check (runs on a GPU box): random shapes, cjpeg switch sets, extension parameters
-(the optional trellis modes), pixel orders of the RGB family, the CMYK / YCCK / YCbCr->gray / JCS_UNKNOWN conversions and small batches through the C-ABI, every file compared
+(the optional trellis modes), pixel orders of the RGB family, the CMYK / YCCK / YCbCr->gray / JCS_UNKNOWN conversions and small batches (some with
+per-image quantization tables) through the C-ABI, every file compared
 byte for byte with the CPU oracle (itself pinned to the reference).  Test infrastructure.
 usage: fuzz_gpu.py [seed] [cases] [seconds]      (exit status 1 if anything differs)"""
 import os, random, sys, time
@@ -63,7 +64,17 @@ for it in range(cases):
         imgs = [CC.cmyk_image(rng.randrange(1 << 20), w, h, ic, 12 if twelve else 8) for _ in range(n)]
     else:
         imgs = [synth_image12(rng.randrange(1 << 20), w, h) if twelve else O.synth_image(rng.randrange(1 << 20), w, h) for _ in range(n)]
-    refs = [CC.oracle_encode(p, im).jpeg for im in imgs]
+    # small batches sometimes carry per-image quantization tables (each image's reference: p with its tables)
+    qt = None
+    if n > 1 and rng.random() < 0.4:
+        qt = mj.quality_tables(p, [rng.choice([1, 10, 30, 50, 75, 90, 100]) for _ in range(n)], force_baseline=rng.random() < 0.5)
+
+    def with_tables(pp, i):
+        if qt is None:
+            return pp
+        c = pp.copy(); np.ctypeslib.as_array(c.quant_tbl)[:] = qt[i]
+        return c
+    refs = [CC.oracle_encode(with_tables(p, i), im).jpeg for i, im in enumerate(imgs)]
     arr = np.stack(imgs)
     q = p
     order = None
@@ -81,7 +92,7 @@ for it in range(cases):
             refused += 1
             continue
     try:
-        got = enc.encode_batch(q, arr)
+        got = enc.encode_batch(q, arr, qtables=qt)
     except mj.B200JpegError as ex:
         if ex.code == -2:                       # B200JPEG_ERR_UNSUPPORTED decided at encode time (e.g. fast / float DCT with a non-tiled sampling layout)
             refused += 1; continue

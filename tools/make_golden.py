@@ -229,8 +229,59 @@ def colorspaces():
                "cases": cases, "raw": raw, "transcode": tran}, open(path, "w"), indent=0)
     print("wrote", len(cases), "pixel,", len(raw), "raw-data and", len(tran), "jpegtran cases")
 
+# per-image quantization tables (Encoder.encode_batch(..., qtables=)): every case is a batch of same-shaped images that
+# share the base switches; image i adds its own table switches.  With -sample given explicitly the per-image parameter
+# blocks differ in their tables only (cjpeg's -quality >= 80 would otherwise change the sampling factors).
+PERIMAGE_Q = [
+    # (seed, w, h, base switches, per-image table switches, extension parameters)
+    (61, 227, 149, ["-baseline", "-sample", "2x2"], [["-quality", q] for q in ("30", "50", "75", "90", "95", "60")], None),
+    (62, 1000, 664, ["-fastcrush", "-sample", "2x2"], [["-quality", q] for q in ("40", "85", "75", "20", "95")], None),
+    (63, 227, 149, ["-sample", "2x2"], [["-quality", q] for q in ("50", "90", "75", "35")], None),
+    (64, 227, 149, ["-baseline", "-sample", "2x1"], [["-quality", q] for q in ("60", "80", "45", "92")],
+     {"trellis_q_opt": 1, "trellis_eob_opt": 1, "use_scans_in_trellis": 1}),
+    (65, 227, 149, ["-dct", "fast", "-baseline", "-sample", "2x2"], [["-quality", q] for q in ("40", "75", "95", "55")], None),
+    (66, 227, 149, ["-dct", "float", "-fastcrush", "-sample", "1x1"], [["-quality", q] for q in ("50", "90", "70", "25", "80")], None),
+    (67, 227, 149, ["-baseline", "-sample", "2x2", "-smooth", "30"], [["-quality", q] for q in ("50", "85", "70", "30")], None),
+    (68, 227, 149, ["-baseline", "-sample", "2x2", "-restart", "1"], [["-quality", q] for q in ("45", "75", "90", "65", "20", "99")], None),
+    (69, 227, 149, ["-baseline", "-grayscale", "-sample", "1x1"], [["-quality", q] for q in ("30", "60", "90", "75")], None),
+    (70, 1000, 664, ["-baseline", "-sample", "2x2"], [["-quality", "75"], ["-qtables", "@GOLD/qtables_a.txt"], ["-quality", "50"], ["-qtables", "@GOLD/qtables_a.txt", "-quality", "40"]], None),
+    ([71, 12], 227, 149, ["-precision", "12", "-notrellis", "-noovershoot", "-fastcrush", "-sample", "2x2"], [["-quality", q] for q in ("1", "3", "50", "10", "90")], None),
+    (72, 227, 149, ["-revert", "-sample", "2x2"], [["-quality", "1"], ["-quality", "1", "-baseline"], ["-quality", "5"], ["-quality", "30", "-baseline"], ["-quality", "2"]], None),
+    # refused on the device: with the trellis on, a table holding 1 and 32767 is beyond the device divider
+    (73, 227, 149, ["-fastcrush", "-sample", "2x2"], [["-quality", "75"], ["-quality", "50"], ["-qtables", "@GOLD/qtables_wide.txt"], ["-quality", "90"]], None),
+]
+
+
+def perimage_image(seed, w, h, i):
+    """Image i of a per-image-table case: seeds count up from the case's; [seed, 12] = 12-bit samples."""
+    if isinstance(seed, list):
+        from mozjpeg_b200.synth import synth_image12
+        return synth_image12(seed[0] + i, w, h)
+    return O.synth_image(seed + i, w, h)
+
+
+def perimage_q():
+    """tests/golden/perimage_q_golden.json: per case and image the reference's file for base + that image's switches."""
+    path = os.path.join(GOLD, "perimage_q_golden.json")
+    if os.path.exists(path) and "--force" not in sys.argv:
+        sys.exit(f"{path} exists; pass --force to overwrite it")
+    expand = lambda sw: [os.path.join(GOLD, x[6:]) if x.startswith("@GOLD/") else x for x in sw]
+    cases = []
+    for seed, w, h, base, per_image, ext in PERIMAGE_Q:
+        files = []
+        for i, isw in enumerate(per_image):
+            a = O.ref_encode(perimage_image(seed, w, h, i), expand(base + isw), ext)
+            files.append({"switches": isw, "md5": hashlib.md5(a).hexdigest(), "size": len(a)})
+        cases.append({"seed": seed, "width": w, "height": h, "switches": base, "ext": ext, "images": files})
+        print(seed, w, h, base, [f["size"] for f in files], flush=True)
+    json.dump({"generator": "tools/make_golden.py --perimage-q", "reference": "mozilla/mozjpeg 5.0.0 (C path, WITH_SIMD=0), oracle/_ref",
+               "cases": cases}, open(path, "w"), indent=0)
+    print("wrote", len(cases), "per-image-table cases")
+
 
 def main():
+    if "--perimage-q" in sys.argv:
+        return perimage_q()
     if "--fullsize" in sys.argv:
         return fullsize()
     if "--colorspaces" in sys.argv:

@@ -39,6 +39,19 @@ n += len(enc.encode_batch_raw(p, [a[None] for a in synth_planes(p, 5)]))
 q = mj.params_from_switches(["-baseline", "-quality", "75"], w, h)
 q.in_color_space, q.input_components = 13, 4                        # JCS_EXT_BGRA
 n += len(enc.encode_batch(q, np.concatenate([img[..., ::-1], img[..., :1]], axis=-1)))
+# per-image quantization tables: one 1024-pixel-wide image at three qualities (image stride 0: one TMA tensor map that
+# every image addresses as image 0), a mixed batch at that width (TMA with per-image sets) and one at 203 (per-thread
+# loads), and raw-data / coefficient input shared by every image (zero plane stride, staged once)
+wide = np.stack([synth_image(s, 1024, 64) for s in range(2)])
+pw = mj.params_from_switches(["-baseline", "-quality", "75", "-sample", "2x2"], 1024, 64)
+n += len(enc.encode_batch(pw, wide[:1], qtables=mj.quality_tables(pw, (30, 60, 90))))
+n += len(enc.encode_batch(pw, wide, qtables=mj.quality_tables(pw, (20, 95))))
+p = mj.params_from_switches(["-baseline", "-quality", "75", "-sample", "2x2"], w, h)
+n += len(enc.encode_batch(mj.params_from_switches(["-quality", "75"], w, h), img, qtables=mj.quality_tables(p, (20, 95))))
+n += len(enc.encode_batch_raw(p, [a[None] for a in synth_planes(p, 6)], qtables=mj.quality_tables(p, (30, 60, 90))))
+pc = mj.params_from_switches(["-revert", "-quality", "75"], w, h)
+n += len(enc.encode_batch_coefs(pc, [np.zeros((1, (h + 15) // 16 * (2 if ci == 0 else 1), (w + 15) // 16 * (2 if ci == 0 else 1), 64), np.int16) for ci in range(3)],
+                                qtables=mj.quality_tables(pc, (30, 60, 90))))
 # an interior-tile-rich frame for the TMA path and a wide one
 big = np.stack([synth_image(9, 1024, 256)])
 n += len(enc.encode_batch(mj.params_from_switches(["-baseline", "-quality", "75", "-sample", "2x2"], 1024, 256), big))
