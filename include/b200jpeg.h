@@ -299,7 +299,8 @@ int  b200jpeg_last_stage_times(const b200jpeg_encoder *enc, const char **names, 
  * int16 in NATURAL order (JBLOCK, jpeglib.h).  Returns blocks written or <0.
  * Planes 0 and 2 need the encoder created with B200JPEG_KEEP_PLAIN=1 in the environment: without it the
  * pipeline keeps no copy of the plain-quantized plane and, for sequential scans behind the trellis, leaves the final
- * values in compact symbol records instead of writing the coefficient planes back. */
+ * values in compact symbol records instead of writing the coefficient planes back (where the forward kernel also
+ * counts the trellis statistics, the plain-quantized values never reach the planes at all). */
 long b200jpeg_debug_get_coefs(b200jpeg_encoder *enc, int image, int component, int plane,
                               int16_t *dst, size_t dst_blocks, int *width_in_blocks, int *height_in_blocks);
 /* Huffman tables actually written for scan `scan` of image `i` (as in the DHT). */

@@ -529,6 +529,10 @@ static int run_pipeline(b200jpeg_encoder *e, const ChunkIO &io, Timer &tm)
     return f;
   };
   Geom gf = g;
+  // the default sequential trellis behind the tiled forward kernel: that kernel counts the trellis-phase AC statistics
+  // and leaves the plain DC values in dcq, so the plain-quantized planes are neither written nor read (the debug taps
+  // of B200JPEG_KEEP_PLAIN read them, and keep the separate statistics pass)
+  bool fwd_stats = false;
   if (g.raw_in == 2) {
     launch_import_coefs(g, n, s);
   } else {
@@ -546,10 +550,20 @@ static int run_pipeline(b200jpeg_encoder *e, const ChunkIO &io, Timer &tm)
     gf.raw_in = 1;
     tm.mark("forward");
   }
-  launch_forward(gf, src_dev, e->d_qt.as<QuantTables>(), qfast, p->dct_method, pl.dering, pl.trellis ? A.d_rec.as<DcRec>() : nullptr, rl, e->keep_plain ? 1 : 0, n, s);
+  fwd_stats = symrec && !e->keep_plain && forward_tiled(gf, p->dct_method);
+  FwdStats fs = {nullptr, nullptr, nullptr};
+  if (fwd_stats) {
+    CU(cudaMemsetAsync(A.d_hist.p, 0, hist_bytes * g.nc, s));
+    fs = {A.d_hist.as<uint32_t>(), A.d_dcq.as<int16_t>(), status};
   }
-  tm.mark("dummy");
-  launch_dummy(g, n, s);
+  launch_forward(gf, src_dev, e->d_qt.as<QuantTables>(), qfast, p->dct_method, pl.dering, pl.trellis ? A.d_rec.as<DcRec>() : nullptr, rl, e->keep_plain ? 1 : 0, fs, n, s);
+  }
+  // dummy blocks: on the fwd_stats path nothing reads them from the planes (the scans take a dummy block as an EOB with
+  // the DC of dense_dc)
+  if (!fwd_stats) {
+    tm.mark("dummy");
+    launch_dummy(g, n, s);
+  }
 
   // ---- trellis phase (jcmaster.c pass list, SURVEY 3.1).  The three
   //      per-component chains (statistics on the plain-quantized coefficients
@@ -572,7 +586,7 @@ static int run_pipeline(b200jpeg_encoder *e, const ChunkIO &io, Timer &tm)
     SymOut so; so.sym = symrec ? A.d_sym.as<uint8_t>() : nullptr; so.dcq = symrec ? A.d_dcq.as<int16_t>() : nullptr;
     so.hist = symstats ? A.d_hist.as<uint32_t>() : nullptr;
     so.keep_coef = e->keep_plain ? 1 : 0;                       // B200JPEG_KEEP_PLAIN=1: the debug taps read the final planes
-    so.dcq_ac = p->trellis_quant_dc ? 0 : 1;
+    so.dcq_ac = (p->trellis_quant_dc || fwd_stats) ? 0 : 1;    // (the forward kernel wrote the plain DC values)
     uint16_t *qimg = qopt ? A.d_qimg.as<uint16_t>() : nullptr;
     if (qopt) {
       // every image starts from its own table set (natural order, like JQUANT_TBL.quantval)
@@ -584,9 +598,14 @@ static int run_pipeline(b200jpeg_encoder *e, const ChunkIO &io, Timer &tm)
     // one statistics -> tables -> quantize_trellis round over the components of gr (all of them, or one)
     auto round = [&](const Geom &gr, const RecLayout &rlr, int bSs, int bSe) -> int {
     if (!pl.progressive) {
-      tm.mark("trellis_stats");
-      CU(cudaMemsetAsync(A.d_hist.p, 0, hist_bytes * gr.nc, s));
-      launch_gather_comp(gr, pl.rs, A.d_hist.as<uint32_t>(), status, n, s);
+      if (fwd_stats) {                                        // one round, its AC counts are in already
+        tm.mark("trellis_dc_stats");
+        launch_gather_comp_dc(gr, pl.rs, so.dcq, rlr, A.d_hist.as<uint32_t>(), status, n, s);
+      } else {
+        tm.mark("trellis_stats");
+        CU(cudaMemsetAsync(A.d_hist.p, 0, hist_bytes * gr.nc, s));
+        launch_gather_comp(gr, pl.rs, A.d_hist.as<uint32_t>(), status, n, s);
+      }
       tm.mark("trellis_tables");
       SlotMasks masks; memset(&masks, 0, sizeof masks); masks.period = gr.nc;
       for (int ci = 0; ci < gr.nc; ci++) masks.m[ci] = (1u << gr.c[ci].dc_tbl) | (1u << (4 + gr.c[ci].ac_tbl));
@@ -654,8 +673,10 @@ static int run_pipeline(b200jpeg_encoder *e, const ChunkIO &io, Timer &tm)
       }
       CU(cudaMemcpyAsync(io.qimg, qimg, (size_t)n * 512, cudaMemcpyDeviceToDevice, s));      // kept per chunk for the DQT markers
     }
-    tm.mark("dummy");
-    launch_dummy(g, n, s);
+    if (!fwd_stats) {
+      tm.mark("dummy");
+      launch_dummy(g, n, s);
+    }
   }
 
   // ---- scans: huff_opt_pass (statistics -> tables) + output_pass.  With the scan search on, all 64 (23) candidate

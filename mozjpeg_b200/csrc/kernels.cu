@@ -494,7 +494,7 @@ __device__ __forceinline__ int quant_fast(int x, uint2 k, int L, int dering)
 template <int HMAX, int VMAX, int NC, bool QFAST, int PREC, int DCTM>
 __global__ void __launch_bounds__(128, FWD_MIN_CTAS) k_forward_tile(Geom g, const uint8_t *__restrict__ src,
                                                       const QuantTables *__restrict__ qt, int dering,
-                                                      DcRec *__restrict__ rec, RecLayout rl, int write_raw,
+                                                      DcRec *__restrict__ rec, RecLayout rl, int write_raw, FwdStats fs,
                                                       const __grid_constant__ CUtensorMap tmap, const int use_tma)
 {
   constexpr int TW = 128, TR = 8 * VMAX;
@@ -515,12 +515,14 @@ __global__ void __launch_bounds__(128, FWD_MIN_CTAS) k_forward_tile(Geom g, cons
   __shared__ uint2 sQC[NC][64];                           // quantizer constants per component, natural order
   __shared__ uint2 sMask[NB];                             // per block: zigzag positions of its non-zero AC values
   __shared__ int sQL[NC];
+  __shared__ unsigned sHist[NC][HIST_BINS];               // fs.hist: the tile's AC symbol counts per component
 
   const int tid = threadIdx.x;
   const int tx = blockIdx.x, ty = blockIdx.y, img = blockIdx.z;
   const int x0 = tx * TW, y0 = ty * TR;
   const uint8_t *base = src + (size_t)img * g.image_stride;
   qt = qset_of(qt, g, img);
+  if (fs.hist) for (int i = tid; i < NC * HIST_BINS; i += 128) (&sHist[0][0])[i] = 0;
 
   for (int i = tid; i < NC * 64; i += 128) { int ci = i >> 6, n = i & 63; const QuantConst &k = qt->q[g.c[ci].qt][n]; sQC[ci][n] = make_uint2(k.mul2, k.bias << 14); }
   if (tid < NC) sQL[tid] = qt->L[g.c[tid].qt];
@@ -911,7 +913,55 @@ __global__ void __launch_bounds__(128, FWD_MIN_CTAS) k_forward_tile(Geom g, cons
       const uint2 mk = sMask[b];
       DcRec rr; rr.lambda_dc = norm; rr.raw_dc = (int16_t)raw_dc; rr.nz = (uint8_t)(__popc(mk.x) + __popc(mk.y)); rr.pad = 0;
       rr.nzmask = ((unsigned long long)mk.y << 32) | mk.x;
-      rec[(size_t)img * rl.per_image + rl.comp_off[ci] + (size_t)row * c.wib + col] = rr;
+      const size_t ridx = (size_t)img * rl.per_image + rl.comp_off[ci] + (size_t)row * c.wib + col;
+      rec[ridx] = rr;
+      // fs.hist: the trellis-phase statistics of the plain-quantized block, encode_mcu_gather's AC half (jchuff.c:886-915,
+      // htest_one_block :836-878) walked over the block's non-zero mask -- from sQ itself: with the fast and float DCTs
+      // sMask holds the trellis' entries, which come from the raw coefficients -- and its DC value for the DC half
+      if (fs.hist) {
+        const int16_t *q = sQ + b * 64;
+        fs.dcq[ridx] = q[0];
+        unsigned long long m;
+        if (FWD_MASK_SQ && DCTM == 0) m = rr.nzmask;
+        else {
+          m = 0;
+#pragma unroll
+          for (int v = 0; v < 8; v++) {
+            const uint4 zq = reinterpret_cast<const uint4 *>(q)[v];
+            const unsigned zw[4] = {zq.x, zq.y, zq.z, zq.w};
+#pragma unroll
+            for (int i = 0; i < 4; i++) {
+              const unsigned nz = (((zw[i] & 0x7FFF7FFFu) + 0x7FFF7FFFu) | zw[i]) & 0x80008000u;
+              const unsigned t2 = nz >> 15;
+              m |= (unsigned long long)((t2 | (t2 >> 15)) & 3u) << (8 * v + 2 * i);
+            }
+          }
+          m &= ~1ull;
+        }
+        unsigned *h = sHist[NC == 1 ? 0 : ci];
+        if (!(m >> 63)) atomicAdd(&h[0], 1u);                  // EOB
+        int prev = 0; bool bad = false;
+        while (m) {
+          const int k = __ffsll((long long)m) - 1;
+          m &= m - 1;
+          const int run = k - prev - 1; prev = k;
+          const int nb = nbits_of(abs((int)q[k]));
+          bad |= nb > g.max_coef_bits;
+          if (run >> 4) atomicAdd(&h[0xF0], (unsigned)(run >> 4));
+          atomicAdd(&h[((run & 15) << 4) + nb], 1u);             // '+' as walk_seq_block: a 16-bit size lands in bin 256
+        }
+        if (bad) atomicOr(&fs.status[img], 2u);                 // JERR_BAD_DCT_COEF
+      }
+    }
+  }
+
+  // ---- flush (fs.hist): the tile's non-zero AC counts into the image's histograms ----
+  if (PREC == 8 && fs.hist) {
+    __syncthreads();
+    for (int i = tid; i < NC * HIST_BINS; i += 128) {
+      const unsigned v = (&sHist[0][0])[i];
+      const int ci = i / HIST_BINS, sym = i - ci * HIST_BINS;
+      if (v) atomicAdd(&fs.hist[(((size_t)img * g.nc + ci) * HIST_SLOTS + 4 + g.c[ci].ac_tbl) * HIST_BINS + sym], v);
     }
   }
 
@@ -930,8 +980,9 @@ __global__ void __launch_bounds__(128, FWD_MIN_CTAS) k_forward_tile(Geom g, cons
       if (cnt > 0) {
         const size_t blk = ((size_t)img * c.hpad + row) * c.wpad + col0;
         const unsigned bytes = (unsigned)cnt * 128u;
-        asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;"
-                     :: "l"(c.coef + blk * 64), "r"((unsigned)__cvta_generic_to_shared(sQ + b0 * 64)), "r"(bytes) : "memory");
+        if (!fs.hist)                                            // with the statistics counted here nobody reads the plain plane
+          asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;"
+                       :: "l"(c.coef + blk * 64), "r"((unsigned)__cvta_generic_to_shared(sQ + b0 * 64)), "r"(bytes) : "memory");
         if (write_raw)                                           // only the trellis (and the debug tap) read the raw DCT
           asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;"
                        :: "l"(c.raw + blk * 64), "r"((unsigned)__cvta_generic_to_shared(sR + b0 * 64)), "r"(bytes) : "memory");
@@ -975,16 +1026,16 @@ static int make_pixel_tensor_map(const Geom &g, const uint8_t *src, int n, int i
 }
 
 template <bool QFAST, int PREC, int DCTM>
-static void launch_forward_tile(const Geom &g, const uint8_t *src, const QuantTables *qt, int dering, DcRec *rec, const RecLayout &rl, int n, cudaStream_t s, bool gray, int write_raw)
+static void launch_forward_tile(const Geom &g, const uint8_t *src, const QuantTables *qt, int dering, DcRec *rec, const RecLayout &rl, const FwdStats &fs, int n, cudaStream_t s, bool gray, int write_raw)
 {
   dim3 grid((g.W + 127) / 128, g.mcu_rows, n);
   CUtensorMap tm;
   const int use_tma = PREC == 8 ? make_pixel_tensor_map(g, src, n, gray ? 1 : 3, 8 * (gray ? 1 : g.vmax), &tm) : (memset(&tm, 0, sizeof tm), 0);
-  if (gray) k_forward_tile<1, 1, 1, QFAST, PREC, DCTM><<<grid, 128, 0, s>>>(g, src, qt, dering, rec, rl, write_raw, tm, use_tma);
-  else if (g.hmax == 1 && g.vmax == 1) k_forward_tile<1, 1, 3, QFAST, PREC, DCTM><<<grid, 128, 0, s>>>(g, src, qt, dering, rec, rl, write_raw, tm, use_tma);
-  else if (g.hmax == 2 && g.vmax == 1) k_forward_tile<2, 1, 3, QFAST, PREC, DCTM><<<grid, 128, 0, s>>>(g, src, qt, dering, rec, rl, write_raw, tm, use_tma);
-  else if (g.hmax == 1 && g.vmax == 2) k_forward_tile<1, 2, 3, QFAST, PREC, DCTM><<<grid, 128, 0, s>>>(g, src, qt, dering, rec, rl, write_raw, tm, use_tma);
-  else k_forward_tile<2, 2, 3, QFAST, PREC, DCTM><<<grid, 128, 0, s>>>(g, src, qt, dering, rec, rl, write_raw, tm, use_tma);
+  if (gray) k_forward_tile<1, 1, 1, QFAST, PREC, DCTM><<<grid, 128, 0, s>>>(g, src, qt, dering, rec, rl, write_raw, fs, tm, use_tma);
+  else if (g.hmax == 1 && g.vmax == 1) k_forward_tile<1, 1, 3, QFAST, PREC, DCTM><<<grid, 128, 0, s>>>(g, src, qt, dering, rec, rl, write_raw, fs, tm, use_tma);
+  else if (g.hmax == 2 && g.vmax == 1) k_forward_tile<2, 1, 3, QFAST, PREC, DCTM><<<grid, 128, 0, s>>>(g, src, qt, dering, rec, rl, write_raw, fs, tm, use_tma);
+  else if (g.hmax == 1 && g.vmax == 2) k_forward_tile<1, 2, 3, QFAST, PREC, DCTM><<<grid, 128, 0, s>>>(g, src, qt, dering, rec, rl, write_raw, fs, tm, use_tma);
+  else k_forward_tile<2, 2, 3, QFAST, PREC, DCTM><<<grid, 128, 0, s>>>(g, src, qt, dering, rec, rl, write_raw, fs, tm, use_tma);
 }
 // =====================================================================
 // Input smoothing (cinfo->smoothing_factor, cjpeg -smooth N).  The smoothing downsamplers (jcsample.c:298-455) read a
@@ -1042,23 +1093,30 @@ void launch_prep_planes(const Geom &g, const uint8_t *src, int smoothing_factor,
   LAUNCHED();
 }
 
-void launch_forward(const Geom &g, const uint8_t *src, const QuantTables *qt, int qfast, int dct_method, int dering, DcRec *rec, const RecLayout &rl, int keep_raw, int n, cudaStream_t s)
+// fast path: full-size first component, (for colour) two 1x1-sampled chroma components
+static bool forward_gray(const Geom &g) { return g.nc == 1 && (g.raw_in || g.cs_mode == 1 || (g.cs_mode == 2 && g.in_comps == 1)); }
+bool forward_tiled(const Geom &g, int dct_method)
 {
-  const int write_raw = rec != nullptr || keep_raw;
-  // fast path: full-size first component, (for colour) two 1x1-sampled chroma components
-  bool gray = g.nc == 1 && (g.raw_in || g.cs_mode == 1 || (g.cs_mode == 2 && g.in_comps == 1));
-  bool ycc = g.nc == 3 && (g.raw_in || (g.cs_mode == 0 && (g.in_comps == 3 || g.in_comps == 4))) && g.c[0].h == g.hmax && g.c[0].v == g.vmax &&
-             g.c[1].h == 1 && g.c[1].v == 1 && g.c[2].h == 1 && g.c[2].v == 1 && g.hmax <= 2 && g.vmax <= 2;
+  const bool ycc = g.nc == 3 && (g.raw_in || (g.cs_mode == 0 && (g.in_comps == 3 || g.in_comps == 4))) && g.c[0].h == g.hmax && g.c[0].v == g.vmax &&
+                   g.c[1].h == 1 && g.c[1].v == 1 && g.c[2].h == 1 && g.c[2].v == 1 && g.hmax <= 2 && g.vmax <= 2;
   static const bool force_generic = getenv("B200JPEG_GENERIC_FORWARD") != nullptr;   // A/B switch for debugging
   // (12-bit samples with the fast / float DCT: the one-thread-per-block kernel only)
-  if (!force_generic && ((gray && g.hmax == 1 && g.vmax == 1) || ycc) && !(g.max_coef_bits == 14 && dct_method != 0)) {
+  return !force_generic && ((forward_gray(g) && g.hmax == 1 && g.vmax == 1) || ycc) && !(g.max_coef_bits == 14 && dct_method != 0);
+}
+void launch_forward(const Geom &g, const uint8_t *src, const QuantTables *qt, int qfast, int dct_method, int dering, DcRec *rec, const RecLayout &rl, int keep_raw,
+                    const FwdStats &fs, int n, cudaStream_t s)
+{
+  const int write_raw = rec != nullptr || keep_raw;
+  const bool gray = forward_gray(g);
+  if (forward_tiled(g, dct_method)) {
+    const FwdStats none = {nullptr, nullptr, nullptr};
     if (g.max_coef_bits == 14) {                       // 12-bit samples (uint16)
-      if (qfast) launch_forward_tile<true, 12, 0>(g, src, qt, 0, nullptr, rl, n, s, gray, 0);
-      else launch_forward_tile<false, 12, 0>(g, src, qt, 0, nullptr, rl, n, s, gray, 0);
-    } else if (dct_method == 2) launch_forward_tile<true, 8, 2>(g, src, qt, dering, rec, rl, n, s, gray, write_raw);
-    else if (dct_method == 1) launch_forward_tile<true, 8, 1>(g, src, qt, dering, rec, rl, n, s, gray, write_raw);
-    else if (qfast) launch_forward_tile<true, 8, 0>(g, src, qt, dering, rec, rl, n, s, gray, write_raw);
-    else launch_forward_tile<false, 8, 0>(g, src, qt, dering, rec, rl, n, s, gray, write_raw);
+      if (qfast) launch_forward_tile<true, 12, 0>(g, src, qt, 0, nullptr, rl, none, n, s, gray, 0);
+      else launch_forward_tile<false, 12, 0>(g, src, qt, 0, nullptr, rl, none, n, s, gray, 0);
+    } else if (dct_method == 2) launch_forward_tile<true, 8, 2>(g, src, qt, dering, rec, rl, fs, n, s, gray, write_raw);
+    else if (dct_method == 1) launch_forward_tile<true, 8, 1>(g, src, qt, dering, rec, rl, fs, n, s, gray, write_raw);
+    else if (qfast) launch_forward_tile<true, 8, 0>(g, src, qt, dering, rec, rl, fs, n, s, gray, write_raw);
+    else launch_forward_tile<false, 8, 0>(g, src, qt, dering, rec, rl, fs, n, s, gray, write_raw);
     LAUNCHED();
     return;
   }
@@ -1494,6 +1552,45 @@ void launch_gather_comp(const Geom &g, const RestartSpec &rs, uint32_t *hist, ui
   for (int ci = 0; ci < g.nc; ci++) mb = max(mb, (long long)g.c[ci].wib * g.c[ci].hib);
   dim3 grid((unsigned)((mb + 256 * GATHER_TILES - 1) / (256 * GATHER_TILES)), n * g.nc);
   k_gather_comp<<<grid, 256, 0, s>>>(g, rs, hist, status);
+  LAUNCHED();
+}
+
+// k_gather_comp's DC half from the dense plain-quantized DC values the tiled forward kernel left (it counted the AC
+// half): the same scan order, restart rule and JERR_BAD_DCT_COEF check, 2 bytes read per block
+__global__ void __launch_bounds__(256) k_gather_comp_dc(Geom g, RestartSpec rs, const int16_t *__restrict__ dcq, RecLayout rl, uint32_t *__restrict__ hist, uint32_t *__restrict__ status)
+{
+  __shared__ unsigned sdc[4][17];                              // |DC difference| < 2^16: sizes 0..16
+  const int ci = blockIdx.y % g.nc, img = blockIdx.y / g.nc;
+  const CompGeom &c = g.c[ci];
+  const long long nblk = (long long)c.wib * c.hib;
+  if ((long long)blockIdx.x * GATHER_TILES * blockDim.x >= nblk) return;
+  for (int i = threadIdx.x; i < 4 * 17; i += blockDim.x) (&sdc[0][0])[i] = 0;
+  __syncthreads();
+  const int16_t *d = dcq + (size_t)img * rl.per_image + rl.comp_off[ci];
+  const long long ri = rs.in_rows > 0 ? min((long long)rs.in_rows * c.wib, 65535LL) : rs.interval;      // per_scan_setup, jcmaster.c:594-599
+  bool bad = false;
+#pragma unroll 1
+  for (int tile = 0; tile < GATHER_TILES; tile++) {
+    const long long t = ((long long)blockIdx.x * GATHER_TILES + tile) * blockDim.x + threadIdx.x;
+    if (t >= nblk) break;
+    const int last = (t > 0 && !(ri && t % ri == 0)) ? d[t - 1] : 0;
+    const int nb = nbits_of(abs((int)d[t] - last));
+    bad |= nb > g.max_coef_bits + 1;
+    atomicAdd(&sdc[threadIdx.x & 3][nb], 1u);
+  }
+  if (bad) atomicOr(&status[img], 2u);                        // JERR_BAD_DCT_COEF (jchuff.c:836)
+  __syncthreads();
+  if (threadIdx.x < 17) {
+    const unsigned v = sdc[0][threadIdx.x] + sdc[1][threadIdx.x] + sdc[2][threadIdx.x] + sdc[3][threadIdx.x];
+    if (v) atomicAdd(&hist[(((size_t)img * g.nc + ci) * HIST_SLOTS + c.dc_tbl) * HIST_BINS + threadIdx.x], v);
+  }
+}
+void launch_gather_comp_dc(const Geom &g, const RestartSpec &rs, const int16_t *dcq, const RecLayout &rl, uint32_t *hist, uint32_t *status, int n, cudaStream_t s)
+{
+  long long mb = 0;
+  for (int ci = 0; ci < g.nc; ci++) mb = max(mb, (long long)g.c[ci].wib * g.c[ci].hib);
+  dim3 grid((unsigned)((mb + 256 * GATHER_TILES - 1) / (256 * GATHER_TILES)), n * g.nc);
+  k_gather_comp_dc<<<grid, 256, 0, s>>>(g, rs, dcq, rl, hist, status);
   LAUNCHED();
 }
 
@@ -2276,7 +2373,10 @@ k_trellis_ac3(Geom g, const TrellisConsts *__restrict__ tc, const DevHuff *__res
       // output: zeros except the back-tracked chain (:1211-1222)
       uint4 *q4 = reinterpret_cast<uint4 *>(o16);
       auto write_block = [&](int lst) {
-        q4[0] = make_uint4(want_dc ? dc_q : (unsigned)(unsigned short)o16[0], 0, 0, 0);        // (late fetch: only blocks whose record overflowed)
+        // without want_dc a DC trellis follows and the scans read the DC from dcq: the plane's DC is never read (the
+        // fallback DC trellis kernels write every real block's DC before they read it), and on the path where the
+        // forward kernel counted the statistics nobody wrote it
+        q4[0] = make_uint4(want_dc ? dc_q : 0u, 0, 0, 0);
 #pragma unroll
         for (int v = 1; v < 8; v++) q4[v] = make_uint4(0, 0, 0, 0);
         unsigned long long fm = 0;

@@ -11,7 +11,9 @@
 // (one 128-byte line per 8x8 block; wpad/hpad include the dummy blocks that
 // pad each component to whole interleaved MCUs, jccoefct.c:312-345).
 // Sequential scans behind the default trellis additionally keep, per real block, a 128-byte symbol record and a dense
-// int16 DC value (SymOut below): the entropy stages then read those, and coef[] keeps the plain-quantized values.
+// int16 DC value (SymOut below): the entropy stages then read those, and coef[] keeps the plain-quantized values --
+// except behind the tiled forward kernel (FwdStats), which counts the trellis statistics itself and writes no coef[]
+// block; there coef[] holds only the blocks whose symbol record overflowed.
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -144,9 +146,17 @@ struct SymOut { uint8_t *sym; int16_t *dcq; uint32_t *hist; int keep_coef; int d
 // qfast / dc_fast: every set the launch's images use allows the fast form
 void launch_prep_planes(const Geom &g, const uint8_t *src, int smoothing_factor, const PlanesOut &out, int n, cudaStream_t s);
 void launch_import_coefs(const Geom &g, int n, cudaStream_t s);     // raw_in == 2: planes hold JBLOCK rows
-void launch_forward(const Geom &g, const uint8_t *src, const QuantTables *qt, int qfast, int dct_method /* J_DCT_METHOD */, int dering, DcRec *rec, const RecLayout &rl, int keep_raw, int n, cudaStream_t s);
+// Trellis-phase statistics counted by the tiled forward kernel (fs.hist != nullptr, only where forward_tiled() holds):
+// every real block's AC symbols go into hist [img*nc + ci][4 + ac_tbl][sym] (zeroed by the caller), its plain-quantized
+// DC into dcq (indexed like the side records), JERR_BAD_DCT_COEF into status; the coefficient planes are not written
+struct FwdStats { uint32_t *hist; int16_t *dcq; uint32_t *status; };
+bool forward_tiled(const Geom &g, int dct_method);   // launch_forward runs k_forward_tile for this geometry
+void launch_forward(const Geom &g, const uint8_t *src, const QuantTables *qt, int qfast, int dct_method /* J_DCT_METHOD */, int dering, DcRec *rec, const RecLayout &rl, int keep_raw,
+                    const FwdStats &fs, int n, cudaStream_t s);
 void launch_dummy(const Geom &g, int n, cudaStream_t s);
 void launch_gather_comp(const Geom &g, const RestartSpec &rs, uint32_t *hist, uint32_t *status, int n, cudaStream_t s);
+// the DC half of the trellis-phase statistics from the dense DC values (the AC half came from the forward kernel)
+void launch_gather_comp_dc(const Geom &g, const RestartSpec &rs, const int16_t *dcq, const RecLayout &rl, uint32_t *hist, uint32_t *status, int n, cudaStream_t s);
 // nz_rec (here and in launch_block_bits / launch_encode): the side records holding every block's final non-zero positions
 // (trellis on, sequential scans), or nullptr
 void launch_gather_seq(const Geom &g, const ScanDesc &sd, const DcRec *nz_rec, const uint8_t *sym, const int16_t *dcq, const RecLayout &rl, uint32_t *hist, uint32_t *status, int n, cudaStream_t s);
