@@ -79,11 +79,11 @@ using namespace b200;
 struct Arena {
   b200::DevBuf d_planes;             // input smoothing: the pre-pass's component planes
   b200::DevBuf d_coef[4], d_raw[4], d_plain[4], d_hist, d_tabs_trellis, d_rec, d_bt, d_srec, d_splits, d_best_al, d_qimg, d_qsum, d_eo, d_es;
-  b200::DevBuf d_blk_bits, d_tile_bits, d_tile_base, d_seg_corr, d_mark, d_ff_tile, d_blk_aux, d_blk_run, d_blk_mask, d_total_bits, d_bitbuf;
+  b200::DevBuf d_blk_bits, d_tile_bits, d_tile_base, d_seg_corr, d_mark, d_stuff_lb, d_blk_aux, d_blk_run, d_blk_mask, d_total_bits, d_bitbuf;
   b200::DevBuf d_sym, d_dcq;         // sequential scans after the trellis: symbol records + dense DC values (SymOut, kernels.cuh)
   b200::Geom g;                      // the plan's geometry with this arena's coefficient pointers
   void release() {
-    b200::DevBuf *db[] = {&d_planes, &d_hist, &d_tabs_trellis, &d_rec, &d_bt, &d_srec, &d_splits, &d_best_al, &d_qimg, &d_qsum, &d_eo, &d_es, &d_blk_bits, &d_tile_bits, &d_tile_base, &d_seg_corr, &d_mark, &d_ff_tile, &d_blk_aux, &d_blk_run, &d_blk_mask, &d_total_bits, &d_bitbuf, &d_sym, &d_dcq};
+    b200::DevBuf *db[] = {&d_planes, &d_hist, &d_tabs_trellis, &d_rec, &d_bt, &d_srec, &d_splits, &d_best_al, &d_qimg, &d_qsum, &d_eo, &d_es, &d_blk_bits, &d_tile_bits, &d_tile_base, &d_seg_corr, &d_mark, &d_stuff_lb, &d_blk_aux, &d_blk_run, &d_blk_mask, &d_total_bits, &d_bitbuf, &d_sym, &d_dcq};
     for (b200::DevBuf *b : db) b->release();
     for (int i = 0; i < 4; i++) { d_coef[i].release(); d_raw[i].release(); d_plain[i].release(); }
   }
@@ -435,7 +435,7 @@ static int prepare_batch(b200jpeg_encoder *e, int n_total, int chunk, bool host_
       if ((rc = a.d_mark.reserve((size_t)n * (cap / 8 + 64)))) return rc;
     }
     if ((rc = a.d_bitbuf.reserve(cap * n))) return rc;
-    if ((rc = a.d_ff_tile.reserve((size_t)n * stuff_tiles(e->bitbuf_words_per_image) * 4))) return rc;
+    if ((rc = a.d_stuff_lb.reserve(stuff_lookback_bytes(e->bitbuf_words_per_image, n)))) return rc;
   }
   // whole batch
   if (host_pixels) { if ((rc = e->d_src.reserve(src_bytes))) return rc; }
@@ -742,7 +742,8 @@ static int run_pipeline(b200jpeg_encoder *e, const ChunkIO &io, Timer &tm)
                   A.d_seg_corr.as<uint32_t>(), pl.max_scan_blocks, aux, run_e, pm,
                   A.d_bitbuf.as<uint32_t>(), e->bitbuf_words_per_image, A.d_mark.as<uint32_t>(), mark_words, status, n, s);
     tm.mark("stuff");
-    launch_stuff(A.d_bitbuf.as<uint32_t>(), e->bitbuf_words_per_image, A.d_total_bits.as<unsigned long long>(), A.d_ff_tile.as<uint32_t>(),
+    CU(cudaMemsetAsync(A.d_stuff_lb.p, 0, stuff_lookback_bytes(e->bitbuf_words_per_image, n), s));
+    launch_stuff(A.d_bitbuf.as<uint32_t>(), e->bitbuf_words_per_image, A.d_total_bits.as<unsigned long long>(), A.d_stuff_lb.p,
                  io.out, e->out_cap_per_image, e->out_cap_per_image, io.out_pos + j * n, io.out_pos + (j + 1) * n,
                  io.scan_size + (size_t)si * n, status, sd.ri ? A.d_mark.as<uint32_t>() : nullptr, mark_words, n, s);
   }

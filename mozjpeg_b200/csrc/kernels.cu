@@ -3163,14 +3163,55 @@ __global__ void __launch_bounds__(256) k_encode_seq(Geom g, ScanDesc sd, const D
   }
 }
 
-// byte stuffing (jchuff.c:386-435 emit byte / 0xFF00) + final 1-bit padding
-// (flush_bits: 7 one-bits, then drop the partial byte).  The unstuffed stream of
-// an image is cut into tiles of STUFF_TILE_WORDS 32-bit words, one CTA each:
-//   k_stuff_count : 0xFF bytes per tile;
-//   k_stuff_write : every CTA sums the counts of the tiles before it (a scan has
-//                   at most a few hundred tiles), scans inside the tile, and
-//                   writes its bytes at out[img][out_start[img] + ...]; the last
-//                   tile publishes the scan size and the next scan's start.
+// ---------------------------------------------------------------------
+// Single-pass scan with decoupled look-back (Merrill & Garland, "Single-pass Parallel Prefix Scan with Decoupled
+// Look-back", NVIDIA 2016) for the stuffer's output offsets.  A CTA takes its tile from a per-(launch, image) ticket, so
+// it only ever waits for tiles that started before it, and every tile that can be a predecessor publishes its
+// descriptor whatever the image's status says: the waits end by construction.
+// Descriptor (64-bit, written with st.release, read with ld.acquire): bits 62..63 flag (0 not yet, 1 aggregate: the
+// tile's own count, 2 inclusive: the count of the tile and all before it), bits 0..61 the value.
+// ---------------------------------------------------------------------
+#define LB_AGG (1ull << 62)
+#define LB_INC (2ull << 62)
+__device__ __forceinline__ void lb_publish(unsigned long long *d, unsigned long long v)
+{
+  asm volatile("st.release.gpu.global.u64 [%0], %1;" :: "l"(d), "l"(v) : "memory");
+}
+__device__ __forceinline__ unsigned long long lb_peek(const unsigned long long *d)
+{
+  unsigned long long v;
+  asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(d) : "memory");
+  return v;
+}
+// sum of the values of the tiles before `tile` (> 0) of the descriptor array desc, called by a whole warp: the lanes read
+// 32 predecessors' descriptors at a time (waiting until all have published), add the aggregates after the nearest
+// inclusive one, and step back 32 tiles when there is none.  Every predecessor holds an earlier ticket, is running or
+// done, and publishes without waiting on anything, so the spin ends.
+__device__ __forceinline__ unsigned long long lb_lookback(const unsigned long long *desc, int tile)
+{
+  const int lane = threadIdx.x & 31;
+  unsigned long long sum = 0;
+  for (int j_end = tile;; j_end -= 32) {
+    const int j = j_end - 32 + lane;
+    unsigned long long d = LB_INC;                            // before tile 0: never chosen, tile 0 is inclusive
+    if (j >= 0) while (!((d = lb_peek(desc + j)) >> 62)) __nanosleep(32);
+    const unsigned inc = __ballot_sync(0xffffffffu, (d >> 62) == 2);
+    const int hi = inc ? 31 - __clz(inc) : -1;                // nearest inclusive predecessor in the window
+    unsigned long long v = lane >= hi ? d & ((1ull << 62) - 1) : 0ull;
+    for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    sum += v;
+    if (inc) return sum;
+  }
+}
+
+// ---------------------------------------------------------------------
+// byte stuffing (jchuff.c:386-435 emit byte / 0xFF00) + final 1-bit padding (flush_bits: 7 one-bits, then drop the
+// partial byte), in one pass.  A tile is STUFF_TILE_WORDS words = 4096 stream bytes, one CTA: it counts its 0xFF bytes
+// (not the restart markers'), publishes that count at once, takes its output offset from the look-back, stages its
+// stuffed bytes (at most 8 KB) in shared memory at the output's 16-byte phase and stores them with 16-byte stores (byte
+// stores only at its two ends: neighbouring tiles write disjoint bytes).  The tile holding the last stream byte
+// publishes the scan size and the next scan's start.
+// ---------------------------------------------------------------------
 #define STUFF_THREADS 256
 #define STUFF_TILE_WORDS (STUFF_THREADS * 4)
 __device__ __forceinline__ uint4 stuff_load(const uint32_t *__restrict__ src, unsigned long long nbytes, unsigned padbits,
@@ -3206,81 +3247,84 @@ __device__ __forceinline__ unsigned count_ff16(uint4 q, int nb, unsigned mk)
   for (int j = 0; j < 16; j++) c += (j < nb) && (((w[j >> 2] >> (24 - 8 * (j & 3))) & 0xFF) == 0xFF) && !((mk >> j) & 1u);
   return c;
 }
-__global__ void __launch_bounds__(STUFF_THREADS) k_stuff_count(const uint32_t *__restrict__ bitbuf, size_t bitbuf_stride_words,
-                                                               const unsigned long long *__restrict__ total_bits,
-                                                               uint32_t *__restrict__ ff_tile, const uint32_t *__restrict__ status,
-                                                               const uint32_t *__restrict__ mark, size_t mark_stride_words)
+__global__ void __launch_bounds__(STUFF_THREADS) k_stuff(const uint32_t *__restrict__ bitbuf, size_t bitbuf_stride_words,
+                                                         const unsigned long long *__restrict__ total_bits,
+                                                         unsigned long long *__restrict__ lb_desc, uint32_t *__restrict__ ticket,
+                                                         uint8_t *__restrict__ out, size_t out_stride, size_t out_capacity,
+                                                         const unsigned long long *__restrict__ out_start, unsigned long long *__restrict__ out_next,
+                                                         uint32_t *__restrict__ scan_size, uint32_t *__restrict__ status,
+                                                         const uint32_t *__restrict__ mark, size_t mark_stride_words)
 {
+  __shared__ __align__(16) uint8_t stage[2 * STUFF_TILE_WORDS * 4 + 16];
   __shared__ unsigned ws[8];
+  __shared__ unsigned long long s_base;
+  __shared__ int s_tile, s_over;
   const int img = blockIdx.y;
-  if (status[img] & ~1u) return;
-  const unsigned long long bits = total_bits[img], nbytes = (bits + 7) >> 3;
-  const unsigned long long tile0 = (unsigned long long)blockIdx.x * STUFF_TILE_WORDS;
-  if (tile0 * 4 >= nbytes && blockIdx.x != 0) return;
-  const unsigned padbits = (unsigned)(nbytes * 8 - bits);
-  int nb;
-  uint4 q = stuff_load(bitbuf + (size_t)img * bitbuf_stride_words, nbytes, padbits, tile0 + threadIdx.x * 4, nb);
-  const unsigned mk = marker_bits16(mark ? mark + (size_t)img * mark_stride_words : nullptr, tile0 + threadIdx.x * 4);
-  unsigned tot = cta_sum_256(count_ff16(q, nb, mk), ws);
-  if (threadIdx.x == 0) ff_tile[(size_t)img * gridDim.x + blockIdx.x] = tot;
-}
-__global__ void __launch_bounds__(STUFF_THREADS) k_stuff_write(const uint32_t *__restrict__ bitbuf, size_t bitbuf_stride_words,
-                                                               const unsigned long long *__restrict__ total_bits,
-                                                               const uint32_t *__restrict__ ff_tile,
-                                                               uint8_t *__restrict__ out, size_t out_stride, size_t out_capacity,
-                                                               const unsigned long long *__restrict__ out_start, unsigned long long *__restrict__ out_next,
-                                                               uint32_t *__restrict__ scan_size, uint32_t *__restrict__ status,
-                                                               const uint32_t *__restrict__ mark, size_t mark_stride_words)
-{
-  __shared__ unsigned red[8], wsum[8];
-  __shared__ unsigned base_s;
-  const int img = blockIdx.y, lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  if (threadIdx.x == 0) { s_tile = (int)atomicAdd(&ticket[img], 1u); s_over = 0; }
+  __syncthreads();
+  const int tile = s_tile;
+  unsigned long long *desc = lb_desc + (size_t)img * gridDim.x;
   const unsigned long long start = out_start[img];
-  if (status[img] & ~1u) { if (blockIdx.x == 0 && threadIdx.x == 0) { scan_size[img] = 0; out_next[img] = start; } return; }
   const unsigned long long bits = total_bits[img], nbytes = (bits + 7) >> 3;
-  const unsigned long long tile0 = (unsigned long long)blockIdx.x * STUFF_TILE_WORDS;
-  if (tile0 * 4 >= nbytes && blockIdx.x != 0) return;
-  const unsigned padbits = (unsigned)(nbytes * 8 - bits);
-  unsigned part = 0;
-  for (int i = threadIdx.x; i < (int)blockIdx.x; i += STUFF_THREADS) part += ff_tile[(size_t)img * gridDim.x + i];
-  for (int o = 16; o; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
-  int nb;
-  uint4 q = stuff_load(bitbuf + (size_t)img * bitbuf_stride_words, nbytes, padbits, tile0 + threadIdx.x * 4, nb);
-  const unsigned mk = marker_bits16(mark ? mark + (size_t)img * mark_stride_words : nullptr, tile0 + threadIdx.x * 4);
-  unsigned ff = count_ff16(q, nb, mk), x = ff;
-  for (int o = 1; o < 32; o <<= 1) { unsigned y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
-  if (lane == 0) red[wid] = part;
-  if (lane == 31) wsum[wid] = x;
-  __syncthreads();
-  if (threadIdx.x == 0) { unsigned b = 0; for (int i = 0; i < 8; i++) b += red[i]; base_s = b; }
-  __syncthreads();
-  unsigned before = base_s;
-  for (int i = 0; i < wid; i++) before += wsum[i];
-  before += x - ff;
-  if (nb) {
-    unsigned long long o = start + (tile0 + threadIdx.x * 4) * 4 + before;
-    if (o + 32 <= out_capacity) {
-      uint8_t *dst = out + (size_t)img * out_stride;
-      unsigned w[4] = {q.x, q.y, q.z, q.w};
-#pragma unroll
-      for (int j = 0; j < 16; j++) {
-        if (j < nb) {
-          unsigned b = (w[j >> 2] >> (24 - 8 * (j & 3))) & 0xFF;
-          dst[o++] = (uint8_t)b;
-          if (b == 0xFF && !((mk >> j) & 1u)) dst[o++] = 0;
-        }
-      }
-    } else atomicOr(&status[img], 4u);
+  const unsigned long long tile0 = (unsigned long long)tile * STUFF_TILE_WORDS;
+  if (tile0 * 4 >= nbytes && tile != 0) return;                      // past the stream: never a live tile's predecessor
+  const bool last = tile0 * 4 + STUFF_TILE_WORDS * 4 >= nbytes;       // holds the last stream byte (or the stream is empty)
+  if (status[img] & ~1u) {                                            // an earlier stage flagged this image: publish, store nothing
+    if (threadIdx.x == 0) {
+      lb_publish(desc + tile, tile == 0 ? LB_INC : LB_AGG);
+      if (tile == 0) { scan_size[img] = 0; out_next[img] = start; }
+    }
+    return;
   }
-  // the thread holding the last stream byte (or thread 0 of tile 0 for an empty stream) publishes the totals
-  const unsigned long long myb0 = (tile0 + threadIdx.x * 4) * 4;
-  if ((nbytes == 0 && blockIdx.x == 0 && threadIdx.x == 0) || (nb && myb0 + nb == nbytes)) {
-    unsigned long long total = nbytes + before + ff;
+  const unsigned padbits = (unsigned)(nbytes * 8 - bits);
+  const unsigned long long w0 = tile0 + threadIdx.x * 4;
+  int nb;
+  const uint4 q = stuff_load(bitbuf + (size_t)img * bitbuf_stride_words, nbytes, padbits, w0, nb);
+  const unsigned mk = marker_bits16(mark ? mark + (size_t)img * mark_stride_words : nullptr, w0);
+  const unsigned ff = count_ff16(q, nb, mk);
+  unsigned tot;
+  const unsigned before = cta_excl_scan_256(ff, ws, tot);
+  if (threadIdx.x < 32) {
+    unsigned long long base = 0;
+    if (tile > 0) { if (threadIdx.x == 0) lb_publish(desc + tile, LB_AGG | tot); base = lb_lookback(desc, tile); }
+    if (threadIdx.x == 0) { lb_publish(desc + tile, LB_INC | (base + tot)); s_base = base; }
+  }
+  __syncthreads();
+  const unsigned long long o0 = start + tile0 * 4 + s_base;          // output offset of the tile's first byte
+  uint8_t *dst = out + (size_t)img * out_stride + o0;
+  const int ph = (int)((uintptr_t)dst & 15);
+  const int pos = threadIdx.x * 16 + (int)before;                    // this thread's first byte inside the tile's output
+  if (nb) {
+    if (o0 + pos + 32 > out_capacity) s_over = 1;
+    const unsigned w[4] = {q.x, q.y, q.z, q.w};
+    uint8_t *sp = stage + ph + pos;
+#pragma unroll
+    for (int j = 0; j < 16; j++) {
+      if (j < nb) {
+        const unsigned b = (w[j >> 2] >> (24 - 8 * (j & 3))) & 0xFF;
+        *sp++ = (uint8_t)b;
+        if (b == 0xFF && !((mk >> j) & 1u)) *sp++ = 0;
+      }
+    }
+  }
+  const unsigned long long tile_bytes = min(nbytes - tile0 * 4, (unsigned long long)STUFF_TILE_WORDS * 4);
+  const int len = (int)(tile_bytes + tot), span = ph + len;
+  __syncthreads();
+  if (s_over) { if (threadIdx.x == 0) atomicOr(&status[img], 4u); }
+  else {
+    uint8_t *base = dst - ph;                                         // 16-byte aligned; bytes [ph, span) are the tile's
+    for (int k = threadIdx.x; k * 16 < span; k += blockDim.x) {
+      const int b0 = k * 16;
+      if (b0 >= ph && b0 + 16 <= span) *reinterpret_cast<uint4 *>(base + b0) = *reinterpret_cast<const uint4 *>(stage + b0);
+      else for (int i = max(b0, ph); i < min(b0 + 16, span); i++) base[i] = stage[i];
+    }
+  }
+  if (last && threadIdx.x == 0) {
+    const unsigned long long total = nbytes + s_base + tot;
     scan_size[img] = (uint32_t)total;
     out_next[img] = start + total;
   }
 }
-
 // =====================================================================
 // progressive scans (jcphuff.c).  DC scans walk blocks in MCU order like
 // the sequential coder.  AC scans are non-interleaved; their cross-block
@@ -3785,13 +3829,16 @@ void launch_encode(const Geom &g, const ScanDesc &sd, const DcRec *nz_rec, const
   LAUNCHED();
 }
 size_t stuff_tiles(size_t bitbuf_stride_words) { return (bitbuf_stride_words + STUFF_TILE_WORDS - 1) / STUFF_TILE_WORDS; }
-void launch_stuff(const uint32_t *bitbuf, size_t bitbuf_stride_words, const unsigned long long *total_bits, uint32_t *ff_tile,
+size_t stuff_lookback_bytes(size_t bitbuf_stride_words, int n) { return (size_t)n * 8 + (size_t)n * stuff_tiles(bitbuf_stride_words) * 8; }
+void launch_stuff(const uint32_t *bitbuf, size_t bitbuf_stride_words, const unsigned long long *total_bits, void *lookback,
                   uint8_t *out, size_t out_stride, size_t out_capacity, const unsigned long long *out_start, unsigned long long *out_next,
                   uint32_t *scan_size, uint32_t *status, const uint32_t *mark, size_t mark_stride_words, int n, cudaStream_t s)
 {
   dim3 grid((unsigned)stuff_tiles(bitbuf_stride_words), n);
-  k_stuff_count<<<grid, STUFF_THREADS, 0, s>>>(bitbuf, bitbuf_stride_words, total_bits, ff_tile, status, mark, mark_stride_words); LAUNCHED();
-  k_stuff_write<<<grid, STUFF_THREADS, 0, s>>>(bitbuf, bitbuf_stride_words, total_bits, ff_tile, out, out_stride, out_capacity, out_start, out_next, scan_size, status, mark, mark_stride_words); LAUNCHED();
+  unsigned long long *desc = static_cast<unsigned long long *>(lookback);
+  uint32_t *ticket = reinterpret_cast<uint32_t *>(desc + (size_t)n * grid.x);
+  k_stuff<<<grid, STUFF_THREADS, 0, s>>>(bitbuf, bitbuf_stride_words, total_bits, desc, ticket, out, out_stride, out_capacity, out_start, out_next, scan_size, status, mark, mark_stride_words);
+  LAUNCHED();
 }
 
 }  // namespace b200

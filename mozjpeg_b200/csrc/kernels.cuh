@@ -202,8 +202,12 @@ void launch_encode(const Geom &g, const ScanDesc &sd, const DcRec *nz_rec, const
                    const uint32_t *blk_bits, const uint32_t *tile_bits, const unsigned long long *tile_base, const uint32_t *seg_corr, long long seg_stride,
                    const uint32_t *blk_aux, const uint32_t *run_e, const unsigned long long *pm,
                    uint32_t *bitbuf, size_t bitbuf_image_stride_words, uint32_t *mark, size_t mark_stride_words, const uint32_t *status, int n, cudaStream_t s);
-size_t stuff_tiles(size_t bitbuf_image_stride_words);     // ff_tile entries per image
-void launch_stuff(const uint32_t *bitbuf, size_t bitbuf_image_stride_words, const unsigned long long *total_bits, uint32_t *ff_tile,
+// byte stuffing of every scan in one pass with a decoupled look-back (k_stuff): out[img][out_start[img] ...], scan_size,
+// out_next.  lookback: stuff_lookback_bytes() of look-back state (a descriptor per tile, a ticket per image), all zero
+// before each launch.
+size_t stuff_tiles(size_t bitbuf_image_stride_words);
+size_t stuff_lookback_bytes(size_t bitbuf_image_stride_words, int n);
+void launch_stuff(const uint32_t *bitbuf, size_t bitbuf_image_stride_words, const unsigned long long *total_bits, void *lookback,
                   uint8_t *out, size_t out_image_stride, size_t out_capacity, const unsigned long long *out_start, unsigned long long *out_next,
                   uint32_t *scan_size, uint32_t *status, const uint32_t *mark, size_t mark_stride_words, int n, cudaStream_t s);
 
