@@ -95,7 +95,7 @@ typedef struct {
   int image_width, image_height;
   int input_components;
   int in_color_space;                     /* B200JPEG_CS_* (UNKNOWN: input_components samples, 1 to 4, passed through) */
-  int data_precision;                     /* 8, or 12 (samples in uint16; trellis and deringing off, as the reference requires) */
+  int data_precision;                     /* 8, or 12 (samples in uint16; trellis and deringing off, as the reference requires), or 16 (lossless only) */
   /* JPEG parameters */
   int jpeg_color_space;
   int num_components;
@@ -160,6 +160,22 @@ void b200jpeg_default_qtables(b200jpeg_params *p, int force_baseline);
 /* jpeg_simple_progression (jcparam.c:859-1004); with optimize_scans set it installs the candidate script of
  * jpeg_search_progression (jcparam.c:733-852: 64 scans, 23 for one component) like the reference. */
 int  b200jpeg_simple_progression(b200jpeg_params *p);
+/* jpeg_enable_lossless (jcparam.c:1015-1039): lossless (SOF3) coding with predictor psv (1..7) and point transform pt
+ * (0..data_precision-1).  Lossless mode is a scan script whose first entry has Ss != 0, Se == 0, as the reference's
+ * validate_script detects it (jcmaster.c:302-311).  Without a script (num_scans == 0) or over the one an earlier call
+ * installed, this call installs one scan of all components in SOF order and turns the scan search off: it stands in for
+ * the reference's scan_info == NULL, follows the component count jpeg_start_compress settles on, and is marked by
+ * scan_info[1].comps_in_scan == -1.  A script of several lossless scans may be installed by hand instead.  Over any
+ * other installed script the call changes nothing (the reference's validate_script then clears lossless mode), except
+ * over the scan search's script, where the reference keeps lossless mode beside progressive mode: B200JPEG_ERR_PARAM
+ * with trellis quantization on ("Bogus buffer control mode"), else B200JPEG_ERR_UNSUPPORTED.  Out-of-range values are
+ * B200JPEG_ERR_PARAM.
+ * At start the reference overrides (jcmaster.c:1072-1094): colour space from jpeg_default_colorspace (an RGB-family
+ * input is coded as RGB), 1x1 sampling, no smoothing, optimal Huffman tables.  Precision 8, 12 or 16 (16 only here);
+ * trellis quantization must be off; a restart interval must be a whole number of rows; pixels are uint16 at 12 and 16
+ * bits and are not masked (12-bit samples are read as J12SAMPLE, i.e. signed short).  The raw-data and coefficient entry
+ * points refuse lossless parameter blocks. */
+int  b200jpeg_enable_lossless(b200jpeg_params *p, int psv, int pt);
 /* std_huff_tables (jstdhuff.c) */
 void b200jpeg_std_huff_tables(b200jpeg_params *p);
 /* the base tables of jcparam.c:76-292, for inspection: 9 sets x {luma,chroma} */

@@ -14,7 +14,7 @@ import numpy as np
 
 from . import _abi as A
 from ._abi import B200JpegError, Params  # noqa: F401
-from .cjpeg import params_from_switches, read_ppm  # noqa: F401
+from .cjpeg import params_from_switches, pnm_samples, read_pnm, read_ppm  # noqa: F401
 
 _lib = A.load()          # raises ImportError with build instructions if missing
 
@@ -74,9 +74,9 @@ class Encoder:
 
     def encode_batch(self, p: Params, images: np.ndarray, qtables: Optional[np.ndarray] = None) -> List[bytes]:
         """images: (N, H, W, C) or (N, H, W) host array -> N JPEG files (uint8, or uint16
-        holding 12-bit samples when p.data_precision == 12, like J12SAMPLE rows).
+        holding 12- or 16-bit samples when p.data_precision is 12 or 16, like J12SAMPLE / J16SAMPLE rows).
         Host->device staging and device->host read-back happen inside."""
-        a = np.ascontiguousarray(images, dtype=np.uint16 if p.data_precision == 12 else np.uint8)
+        a = np.ascontiguousarray(images, dtype=np.uint16 if p.data_precision > 8 else np.uint8)
         if a.ndim == 3 and p.input_components == 1:
             a = a[..., None]
         n, h, w, c = a.shape
@@ -198,9 +198,9 @@ class Encoder:
 
 def cjpeg(switches: Sequence[str], ppm: bytes, encoder: Optional[Encoder] = None) -> bytes:
     """``cjpeg <switches> file.ppm`` on the device path: PPM/PGM bytes -> JPEG bytes."""
-    w, h, nc, data = read_ppm(ppm)
+    w, h, nc, maxv, a = read_pnm(ppm)
     p = params_from_switches(switches, w, h, nc)
-    img = np.frombuffer(data, dtype=np.uint8).reshape(1, h, w, nc)
+    img = pnm_samples(maxv, a, p.data_precision)[None]
     enc = encoder or Encoder(0)
     try:
         return enc.encode_batch(p, img)[0]

@@ -86,7 +86,7 @@ EXPORTS = [
     "b200jpeg_set_defaults", "b200jpeg_default_colorspace", "b200jpeg_set_colorspace",
     "b200jpeg_quality_scaling", "b200jpeg_float_quality_scaling", "b200jpeg_add_quant_table",
     "b200jpeg_set_linear_quality", "b200jpeg_set_quality", "b200jpeg_default_qtables",
-    "b200jpeg_simple_progression", "b200jpeg_std_huff_tables", "b200jpeg_std_quant_tbl",
+    "b200jpeg_simple_progression", "b200jpeg_enable_lossless", "b200jpeg_std_huff_tables", "b200jpeg_std_quant_tbl",
     "b200jpeg_validate", "b200jpeg_total_passes",
     "b200jpeg_encoder_create", "b200jpeg_encoder_destroy", "b200jpeg_encoder_set_stream", "b200jpeg_encoder_set_chunk_images", "b200jpeg_last_chunk_images", "b200jpeg_encoder_set_streams", "b200jpeg_encode_batch",
     "b200jpeg_encode_batch_device_only", "b200jpeg_encode_batch_raw", "b200jpeg_encode_batch_coefs",
@@ -120,6 +120,7 @@ def load() -> C.CDLL:
     lib.b200jpeg_set_quality.argtypes = [P, C.c_int, C.c_int]; lib.b200jpeg_set_quality.restype = None
     lib.b200jpeg_default_qtables.argtypes = [P, C.c_int]; lib.b200jpeg_default_qtables.restype = None
     lib.b200jpeg_simple_progression.argtypes = [P]; lib.b200jpeg_simple_progression.restype = C.c_int
+    lib.b200jpeg_enable_lossless.argtypes = [P, C.c_int, C.c_int]; lib.b200jpeg_enable_lossless.restype = C.c_int
     lib.b200jpeg_std_huff_tables.argtypes = [P]; lib.b200jpeg_std_huff_tables.restype = None
     lib.b200jpeg_std_quant_tbl.argtypes = [C.c_int, C.c_int]; lib.b200jpeg_std_quant_tbl.restype = C.POINTER(C.c_uint)
     lib.b200jpeg_validate.argtypes = [P]; lib.b200jpeg_validate.restype = C.c_int

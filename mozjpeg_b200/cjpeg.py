@@ -20,6 +20,7 @@ sequences the calls.
 from __future__ import annotations
 
 import ctypes as C
+import re
 from typing import List, Sequence, Tuple
 
 from . import _abi as A
@@ -158,6 +159,7 @@ def _parse(p: A.Params, argv: Sequence[str], for_real: bool) -> None:
     force_baseline = False
     simple_progressive = p.num_scans != 0          # cjpeg.c:343
     qualityarg = samplearg = qtablefile = qslotsarg = scansarg = None
+    psv, pt = 0, 0
     i = 0
     n = len(argv)
 
@@ -189,6 +191,18 @@ def _parse(p: A.Params, argv: Sequence[str], for_real: bool) -> None:
             A.check(lib.b200jpeg_set_colorspace(C.byref(p), A.CS_GRAYSCALE), "set_colorspace")
         elif _keymatch(a, "rgb", 3):
             A.check(lib.b200jpeg_set_colorspace(C.byref(p), A.CS_RGB), "set_colorspace")
+        elif _keymatch(a, "lossless", 1):
+            # cjpeg.c:459-480: "psv[,Pt]"; executed after the other switches, once data_precision is known
+            v = nextarg("lossless")
+            m = re.match(r"\s*([+-]?\d+)(.?)", v)
+            if not m or (m.group(2) and m.group(2) != ","):
+                raise UsageError("invalid argument for lossless")
+            psv = int(m.group(1))
+            rest = v.split(",", 1)
+            if len(rest) == 2:
+                m2 = re.match(r"\s*([+-]?\d+)", rest[1])
+                if m2:
+                    pt = int(m2.group(1))
         elif _keymatch(a, "lambda1", 7):
             p.lambda_log_scale1 = float(nextarg("lambda1"))
         elif _keymatch(a, "lambda2", 7):
@@ -199,8 +213,8 @@ def _parse(p: A.Params, argv: Sequence[str], for_real: bool) -> None:
             p.optimize_coding = 1
         elif _keymatch(a, "precision", 3):
             v = nextarg("precision")
-            if int(v) not in (8, 12):
-                raise UsageError("precision must be 8 or 12")
+            if int(v) not in (8, 12, 16):
+                raise UsageError("precision must be 8, 12 or 16")
             p.data_precision = int(v)
         elif _keymatch(a, "progressive", 1):
             simple_progressive = True
@@ -284,6 +298,8 @@ def _parse(p: A.Params, argv: Sequence[str], for_real: bool) -> None:
             _set_sample_factors(p, samplearg)
         if simple_progressive:
             A.check(lib.b200jpeg_simple_progression(C.byref(p)), "simple_progression")
+        if psv != 0:                                                  # cjpeg.c:752-755
+            A.check(lib.b200jpeg_enable_lossless(C.byref(p), psv, pt), "enable_lossless")
         if scansarg is not None:
             _read_scan_script(p, scansarg)
 
@@ -319,8 +335,10 @@ def params_from_switches(switches: Sequence[str], width: int, height: int,
     return p
 
 
-def read_ppm(data: bytes) -> Tuple[int, int, int, bytes]:
-    """Minimal binary PGM/PPM reader (P5/P6, maxval 255) -> (w, h, ncomp, samples)."""
+def read_pnm(data: bytes):
+    """Minimal binary PGM/PPM reader (P5/P6) -> (w, h, ncomp, maxval, samples): samples is an (h, w, ncomp) uint8 array
+    for maxval <= 255, else uint16 (two bytes per sample, big-endian in the file, as rdppm.c reads them)."""
+    import numpy as np
     toks: List[bytes] = []
     pos = 0
     while len(toks) < 4:
@@ -336,10 +354,34 @@ def read_ppm(data: bytes) -> Tuple[int, int, int, bytes]:
         toks.append(data[st:pos])
     pos += 1
     magic, w, h, maxv = toks[0], int(toks[1]), int(toks[2]), int(toks[3])
-    if magic not in (b"P5", b"P6") or maxv != 255:
-        raise ValueError("only binary 8-bit PGM/PPM supported")
+    if magic not in (b"P5", b"P6") or not 1 <= maxv <= 65535:
+        raise ValueError("only binary PGM/PPM (P5/P6) supported")
     nc = 3 if magic == b"P6" else 1
-    return w, h, nc, data[pos:pos + w * h * nc]
+    if maxv <= 255:
+        a = np.frombuffer(data[pos:pos + w * h * nc], dtype=np.uint8)
+    else:
+        a = np.frombuffer(data[pos:pos + 2 * w * h * nc], dtype=">u2").astype(np.uint16)
+    if a.size != w * h * nc:
+        raise ValueError("PGM/PPM file is truncated")
+    return w, h, nc, maxv, a.reshape(h, w, nc)
+
+
+def pnm_samples(maxval: int, samples, data_precision: int):
+    """The samples as the encoder takes them at ``data_precision``.  rdppm.c rescales every maxval other than the
+    precision's largest sample value (its rescale[] tables); that is not mirrored here, so such a file is refused rather
+    than coded with samples the reference would not see."""
+    if maxval != (1 << data_precision) - 1:
+        raise ValueError(f"maxval {maxval} at data precision {data_precision}: only maxval {(1 << data_precision) - 1} "
+                         "is read without rescaling")
+    return samples
+
+
+def read_ppm(data: bytes) -> Tuple[int, int, int, bytes]:
+    """Minimal binary PGM/PPM reader (P5/P6, maxval 255) -> (w, h, ncomp, samples)."""
+    w, h, nc, maxv, a = read_pnm(data)
+    if maxv != 255:
+        raise ValueError("only binary 8-bit PGM/PPM supported")
+    return w, h, nc, a.tobytes()
 
 
 def main(argv: Sequence[str] = None) -> int:
@@ -352,7 +394,7 @@ def main(argv: Sequence[str] = None) -> int:
     outfile = None
     switches: List[str] = []
     files: List[str] = []
-    takes_arg = ("dct", "lambda1", "lambda2", "dc-scan-opt", "precision", "quality", "qslots", "qtables", "scans", "quant-table",
+    takes_arg = ("dct", "lambda1", "lambda2", "dc-scan-opt", "lossless", "precision", "quality", "qslots", "qtables", "scans", "quant-table",
                  "restart", "sample", "smooth", "trellis-dc-ver-weight")
     i = 0
     while i < len(args):
@@ -369,15 +411,20 @@ def main(argv: Sequence[str] = None) -> int:
     if not files:
         print("usage: python -m mozjpeg_b200.cjpeg [switches] [-outfile name] file.ppm [more.ppm ...]", file=sys.stderr)
         return 2
-    imgs = []
+    raw = []
     for f in files:
-        w, h, nc, data = read_ppm(open(f, "rb").read())
-        imgs.append(np.frombuffer(data, dtype=np.uint8).reshape(h, w, nc))
-    if len({im.shape for im in imgs}) != 1:
+        w, h, nc, maxv, a = read_pnm(open(f, "rb").read())
+        raw.append((maxv, a))
+    if len({a.shape for _, a in raw}) != 1:
         print("all input files of one call must have the same size", file=sys.stderr)
         return 2
-    h, w, nc = imgs[0].shape
+    h, w, nc = raw[0][1].shape
     p = params_from_switches(switches, w, h, nc)
+    try:
+        imgs = [pnm_samples(maxv, a, p.data_precision) for maxv, a in raw]
+    except ValueError as e:
+        print(str(e), file=sys.stderr)
+        return 2
     out = Encoder(0).encode_batch(p, np.stack(imgs))
     for f, jpg in zip(files, out):
         name = outfile if (outfile and len(files) == 1) else f.rsplit(".", 1)[0] + ".jpg"

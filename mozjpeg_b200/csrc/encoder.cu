@@ -61,6 +61,7 @@ struct Plan {                // everything derived from b200jpeg_params
   Geom g;
   std::vector<ScanDesc> scans;
   bool progressive = false, optimize = false, trellis = false, dering = false, restarts = false;
+  bool lossless = false;         // SOF3: every scan is predicted and coded sample by sample (run_lossless)
   int smooth = 0;                // smoothing_factor: colour conversion + (smoothing) downsampling run as a pre-pass into planes
   // scan search (optimize_scans): the script of jpeg_search_progression (jcparam.c:733-852) and where its groups start
   bool search = false; int n_luma = 0, luma_split0 = 0, chroma_split0 = 0, chroma_al0 = 0;
@@ -81,9 +82,10 @@ struct Arena {
   b200::DevBuf d_coef[4], d_raw[4], d_plain[4], d_hist, d_tabs_trellis, d_rec, d_bt, d_srec, d_splits, d_best_al, d_qimg, d_qsum, d_eo, d_es;
   b200::DevBuf d_blk_bits, d_tile_bits, d_tile_base, d_seg_corr, d_mark, d_stuff_lb, d_blk_aux, d_blk_run, d_blk_mask, d_total_bits, d_bitbuf;
   b200::DevBuf d_sym, d_dcq;         // sequential scans after the trellis: symbol records + dense DC values (SymOut, kernels.cuh)
+  b200::DevBuf d_diff;               // lossless scans: the differences of the scan being coded (launch_lossless_diff)
   b200::Geom g;                      // the plan's geometry with this arena's coefficient pointers
   void release() {
-    b200::DevBuf *db[] = {&d_planes, &d_hist, &d_tabs_trellis, &d_rec, &d_bt, &d_srec, &d_splits, &d_best_al, &d_qimg, &d_qsum, &d_eo, &d_es, &d_blk_bits, &d_tile_bits, &d_tile_base, &d_seg_corr, &d_mark, &d_stuff_lb, &d_blk_aux, &d_blk_run, &d_blk_mask, &d_total_bits, &d_bitbuf, &d_sym, &d_dcq};
+    b200::DevBuf *db[] = {&d_planes, &d_hist, &d_tabs_trellis, &d_rec, &d_bt, &d_srec, &d_splits, &d_best_al, &d_qimg, &d_qsum, &d_eo, &d_es, &d_blk_bits, &d_tile_bits, &d_tile_base, &d_seg_corr, &d_mark, &d_stuff_lb, &d_blk_aux, &d_blk_run, &d_blk_mask, &d_total_bits, &d_bitbuf, &d_sym, &d_dcq, &d_diff};
     for (b200::DevBuf *b : db) b->release();
     for (int i = 0; i < 4; i++) { d_coef[i].release(); d_raw[i].release(); d_plain[i].release(); }
   }
@@ -154,6 +156,39 @@ namespace b200 {
 
 static int div_up(long long a, long long b) { return (int)((a + b - 1) / b); }
 
+// Lossless mode (p after the start-time overrides, lossless_start): one data unit = one sample, every component 1x1,
+// so a scan is W*H MCUs of one sample per scan component (per_scan_setup, jcmaster.c:518-601 with data_unit 1).
+static void build_plan_lossless(const b200jpeg_params *p, Plan &pl)
+{
+  Geom &g = pl.g;
+  g.mcus_per_row = g.W; g.mcu_rows = g.H;
+  pl.max_real_blocks = pl.sum_real_blocks = 0;
+  for (int ci = 0; ci < g.nc; ci++) {
+    CompGeom &c = g.c[ci]; const b200jpeg_component_info &ic = p->comp_info[ci];
+    c.h = c.v = c.hx = c.vx = 1;
+    c.wib = c.wpad = g.W; c.hib = c.hpad = g.H; c.rows_avail = g.H;
+    c.qt = ic.quant_tbl_no; c.dc_tbl = ic.dc_tbl_no; c.ac_tbl = ic.ac_tbl_no;
+    c.blocks_per_image = (long long)g.W * g.H;
+    pl.coef_bytes[ci] = 0;
+  }
+  pl.scans.clear();
+  pl.max_scan_blocks = (long long)g.W * g.H;
+  for (int si = 0; si < p->num_scans; si++) {
+    const b200jpeg_scan_info &s = p->scan_info[si];
+    ScanDesc sd; memset(&sd, 0, sizeof sd);
+    sd.ncomps = s.comps_in_scan; for (int k = 0; k < 4; k++) sd.ci[k] = s.component_index[k];
+    sd.Ss = s.Ss; sd.Se = s.Se; sd.Ah = s.Ah; sd.Al = s.Al;
+    sd.bim = 1; sd.per_row = g.W; sd.rows = g.H; sd.nblocks = (long long)g.W * g.H;
+    sd.ri = p->restart_in_rows > 0 ? (int)std::min((long long)p->restart_in_rows * g.W, 65535LL) : p->restart_interval;
+    pl.scans.push_back(sd);
+  }
+  pl.lossless = true; pl.progressive = false; pl.optimize = true; pl.trellis = false; pl.dering = false; pl.smooth = 0; pl.search = false;
+  pl.restarts = p->restart_interval != 0 || p->restart_in_rows > 0;
+  pl.rs.interval = p->restart_interval; pl.rs.in_rows = p->restart_in_rows;
+  pl.order.clear();
+  for (int si = 0; si < p->num_scans; si++) pl.order.push_back(si);
+}
+
 static int build_plan(const b200jpeg_params *p, size_t row_pitch, size_t image_stride, Plan &pl)
 {
   Geom &g = pl.g;
@@ -171,6 +206,8 @@ static int build_plan(const b200jpeg_params *p, size_t row_pitch, size_t image_s
   else g.cs_mode = 2;                               // RGB->RGB, gray, YCbCr->YCbCr/gray, CMYK, YCCK, UNKNOWN: null_convert
   g.px_first = rgb_in ? B200JPEG_CS_FIRST(p->in_color_space) : 0;             // jccolor.c:253-291 (JCS_EXT_* pixel orders)
   g.px_swap = rgb_in ? B200JPEG_CS_BLUE_FIRST(p->in_color_space) : 0;
+  pl.lossless = false;
+  if (is_lossless(p)) { build_plan_lossless(p, pl); return B200JPEG_OK; }
   pl.max_real_blocks = 0; pl.sum_real_blocks = 0;
   for (int ci = 0; ci < g.nc; ci++) {
     CompGeom &c = g.c[ci]; const b200jpeg_component_info &ic = p->comp_info[ci];
@@ -391,6 +428,7 @@ static int prepare_batch(b200jpeg_encoder *e, int n_total, int chunk, bool host_
   int rc;
   const int n = chunk;
   long long total_blocks = 0; for (int ci = 0; ci < g.nc; ci++) total_blocks += g.c[ci].blocks_per_image;
+  if (pl.lossless) total_blocks = (total_blocks + 7) / 8;       // one sample per data unit: the buffers start at 2 bytes per sample
   size_t cap = (size_t)((double)total_blocks * 64 * e->cap_factor) + 65536;
   cap = (cap + 255) & ~(size_t)255;
   e->bitbuf_words_per_image = cap / 4; e->out_cap_per_image = (cap + cap / 64 + 4096) * (pl.search ? 6 : 1);   // scan search keeps all 64 candidate scans
@@ -425,6 +463,7 @@ static int prepare_batch(b200jpeg_encoder *e, int n_total, int chunk, bool host_
       if ((rc = a.d_eo.reserve((size_t)n * pl.sum_real_blocks * 16))) return rc;
       if ((rc = a.d_es.reserve((size_t)n * pl.sum_real_blocks * 16))) return rc;
     }
+    if (pl.lossless) { if ((rc = a.d_diff.reserve((size_t)n * pl.max_scan_blocks * g.nc * 2))) return rc; }
     if ((rc = a.d_blk_bits.reserve((size_t)n * pl.max_scan_blocks * 4))) return rc;
     if (pl.progressive) { if ((rc = a.d_blk_aux.reserve((size_t)n * pl.max_scan_blocks * 4))) return rc; if ((rc = a.d_blk_run.reserve((size_t)n * pl.max_scan_blocks * 4))) return rc; if ((rc = a.d_blk_mask.reserve((size_t)n * pl.max_scan_blocks * 24))) return rc; }
     if ((rc = a.d_total_bits.reserve((size_t)n * 8))) return rc;
@@ -495,10 +534,58 @@ static int prepare_batch(b200jpeg_encoder *e, int n_total, int chunk, bool host_
   return B200JPEG_OK;
 }
 
+// The lossless pipeline for one chunk: per scan, differences + category counts -> optimal DC tables (one set per scan,
+// finish_pass_gather, jclhuff.c:531-556) -> bits per MCU -> layout -> packing -> byte stuffing.
+static int run_lossless(b200jpeg_encoder *e, const ChunkIO &io, Timer &tm)
+{
+  Plan &pl = e->plan; const b200jpeg_params *p = &e->params; const int n = io.n; cudaStream_t s = e->sc[io.slot];
+  Arena &A = e->ar[io.slot];
+  const Geom &g = A.g;
+  tm.s = s;
+  const int nscans = (int)pl.scans.size();
+  const size_t hist_bytes = (size_t)n * HIST_SLOTS * HIST_BINS * 4;
+  const size_t tabset = sizeof(DevHuff) * HIST_SLOTS, tstride = tabset * nscans;
+  const size_t mark_words = (e->bitbuf_words_per_image * 4 / 8 + 64) / 4;
+  for (size_t j = 0; j < pl.order.size(); j++) {
+    const int si = pl.order[j];
+    const ScanDesc &sd = pl.scans[si];
+    DevHuff *tset = io.tabs_scan + (size_t)si * HIST_SLOTS;
+    tm.mark("lossless_diff");
+    CU(cudaMemsetAsync(A.d_hist.p, 0, hist_bytes, s));
+    launch_lossless_diff(g, sd, p->data_precision, io.src, A.d_diff.as<uint16_t>(), A.d_hist.as<uint32_t>(), n, s);
+    tm.mark("scan_tables");
+    SlotMasks masks; memset(&masks, 0, sizeof masks); masks.period = 1;
+    for (int i = 0; i < sd.ncomps; i++) masks.m[0] |= 1u << g.c[sd.ci[i]].dc_tbl;
+    launch_gen_tables(A.d_hist.as<uint32_t>(), tset, tstride, masks, n, s);
+    tm.mark("block_bits");
+    launch_lossless_bits(g, sd, A.d_diff.as<uint16_t>(), tset, tstride, A.d_blk_bits.as<uint32_t>(), A.d_tile_bits.as<uint32_t>(), io.status, n, s);
+    tm.mark("scan_layout");
+    launch_scan_layout(sd, A.d_blk_bits.as<uint32_t>(), A.d_tile_bits.as<uint32_t>(), A.d_tile_base.as<unsigned long long>(),
+                       A.d_seg_corr.as<uint32_t>(), pl.max_scan_blocks, A.d_total_bits.as<unsigned long long>(),
+                       (size_t)e->bitbuf_words_per_image * 32, io.status, n, s);
+    tm.mark("encode");
+    launch_zero_stream(A.d_bitbuf.as<uint32_t>(), e->bitbuf_words_per_image, A.d_total_bits.as<unsigned long long>(), n, s);
+    if (sd.ri) CU(cudaMemsetAsync(A.d_mark.p, 0, mark_words * 4 * n, s));
+    launch_lossless_encode(g, sd, A.d_diff.as<uint16_t>(), tset, tstride, A.d_blk_bits.as<uint32_t>(), A.d_tile_base.as<unsigned long long>(),
+                           A.d_seg_corr.as<uint32_t>(), pl.max_scan_blocks, A.d_bitbuf.as<uint32_t>(), e->bitbuf_words_per_image,
+                           A.d_mark.as<uint32_t>(), mark_words, io.status, n, s);
+    tm.mark("stuff");
+    CU(cudaMemsetAsync(A.d_stuff_lb.p, 0, stuff_lookback_bytes(e->bitbuf_words_per_image, n), s));
+    launch_stuff(A.d_bitbuf.as<uint32_t>(), e->bitbuf_words_per_image, A.d_total_bits.as<unsigned long long>(), A.d_stuff_lb.p,
+                 io.out, e->out_cap_per_image, e->out_cap_per_image, io.out_pos + j * n, io.out_pos + (j + 1) * n,
+                 io.scan_size + (size_t)si * n, io.status, sd.ri ? A.d_mark.as<uint32_t>() : nullptr, mark_words, n, s);
+  }
+  tm.mark("end");
+  CU(cudaGetLastError());
+  e->last_chunk_i0 = io.i0; e->last_chunk_n = io.n; e->last_chunk_slot = io.slot;
+  return B200JPEG_OK;
+}
+
 // The device pipeline for one chunk (pixels already in HBM): the pass plan of
 // jcmaster.c with every pass one launch over all images of the chunk.
 static int run_pipeline(b200jpeg_encoder *e, const ChunkIO &io, Timer &tm)
 {
+  if (e->plan.lossless) return run_lossless(e, io, tm);
   Plan &pl = e->plan; const b200jpeg_params *p = &e->params; const int n = io.n; cudaStream_t s = e->sc[io.slot];
   Arena &A = e->ar[io.slot];
   Geom &g = A.g;
@@ -777,7 +864,10 @@ static void write_file_header(const b200jpeg_params *p, Bytes o)                
 static void write_frame_header(const b200jpeg_params *p, bool progressive, Bytes o)   // jcmarker.c:674-735
 {
   int nc = p->num_components, prec = 0;
+  const bool lossless = is_lossless(p);
   bool multi = p->compress_profile != B200JPEG_PROFILE_FASTEST;                       // emit_multi_dqt :189-254
+  // emit_multi_dqt runs before the lossless test (:684-697) and gives up when a component's table is missing (:207-208)
+  for (int ci = 0; ci < nc; ci++) if (!p->quant_tbl_present[p->comp_info[ci].quant_tbl_no & 3]) multi = false;
   bool sent[4] = {false, false, false, false};
   if (multi) {
     int precs[4] = {0, 0, 0, 0}, size = 0; bool seen[4] = {false, false, false, false};
@@ -792,7 +882,7 @@ static void write_frame_header(const b200jpeg_params *p, bool progressive, Bytes
       for (int i = 0; i < 64; i++) { unsigned q = p->quant_tbl[t][kZigzag[i]]; if (precs[ci]) o.b(q >> 8); o.b(q & 0xFF); }
       sent[t] = true;
     }
-  } else {
+  } else if (!lossless) {
     for (int ci = 0; ci < nc; ci++) {                                                  // emit_dqt :140-187
       int t = p->comp_info[ci].quant_tbl_no, pr = 0;
       for (int i = 0; i < 64; i++) if (p->quant_tbl[t][i] > 255) pr = 1;
@@ -805,13 +895,13 @@ static void write_frame_header(const b200jpeg_params *p, bool progressive, Bytes
     }
   }
   bool is_baseline;
-  if (progressive || p->data_precision != 8) is_baseline = false;
+  if (progressive || lossless || p->data_precision != 8) is_baseline = false;
   else {
     is_baseline = true;
     for (int ci = 0; ci < nc; ci++) if (p->comp_info[ci].dc_tbl_no > 1 || p->comp_info[ci].ac_tbl_no > 1) is_baseline = false;
     if (prec && is_baseline) is_baseline = false;
   }
-  o.w(progressive ? 0xFFC2 : (is_baseline ? 0xFFC0 : 0xFFC1));                          // emit_sof :464-491
+  o.w(progressive ? 0xFFC2 : lossless ? 0xFFC3 : (is_baseline ? 0xFFC0 : 0xFFC1));     // emit_sof :464-491, :720-733
   o.w(3 * nc + 2 + 5 + 1); o.b(p->data_precision); o.w(p->image_height); o.w(p->image_width); o.b(nc);
   for (int ci = 0; ci < nc; ci++) { o.b(p->comp_info[ci].component_id); o.b((p->comp_info[ci].h_samp_factor << 4) + p->comp_info[ci].v_samp_factor); o.b(p->comp_info[ci].quant_tbl_no); }
 }
@@ -863,8 +953,8 @@ static void write_scan_header(const b200jpeg_params *p, const ScanDesc &sd, TblS
       const b200jpeg_component_info &c = p->comp_info[sd.ci[i]];
       for (int z = 0; z < 2; z++) {
         bool is_ac = z == 1;
-        if (!is_ac && !(sd.Ss == 0 && sd.Ah == 0)) continue;
-        if (is_ac && !sd.Se) continue;
+        if (!is_ac && !((sd.Ss == 0 && sd.Ah == 0) || is_lossless(p))) continue;        // lossless: DC tables only (:765-770)
+        if (is_ac && (!sd.Se || is_lossless(p))) continue;
         int idx = is_ac ? c.ac_tbl_no : c.dc_tbl_no;
         bool &sent = is_ac ? ts.ac_sent[idx] : ts.dc_sent[idx];
         const HostHuff *h = is_ac ? ts.ac[idx] : ts.dc[idx];
@@ -1189,7 +1279,15 @@ static int encode_common(b200jpeg_encoder *e, const b200jpeg_params *p, const vo
   if (!e || !p || (!pixels && !raw) || n_images <= 0) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
   int rc = b200jpeg_validate(p);
   if (rc) return rc;
-  const size_t sample_bytes = p->data_precision > 8 ? 2 : 1;                       // 12-bit samples are uint16 (J12SAMPLE)
+  // lossless mode: the block jpeg_start_compress works with (jcmaster.c:1072-1094); the plan and the markers follow it
+  b200jpeg_params eff;
+  if (is_lossless(p)) {
+    if (raw) { set_error("%s input cannot be coded lossless (jcmaster.c:1076 clears raw_data_in)", raw->coefs ? "coefficient" : "raw-data"); return B200JPEG_ERR_PARAM; }
+    if (qtables) { set_error("per-image quantization tables have no meaning in lossless mode"); return B200JPEG_ERR_PARAM; }
+    lossless_start(p, &eff);
+    p = &eff;
+  }
+  const size_t sample_bytes = p->data_precision > 8 ? 2 : 1;                       // 12- and 16-bit samples are uint16 (J12SAMPLE / J16SAMPLE)
   const size_t row_bytes = (size_t)p->image_width * p->input_components * sample_bytes;
   // per-image tables allow a zero image stride: every image reads the same input (a quality ladder)
   const bool shared_ok = qtables != nullptr;
@@ -1253,6 +1351,7 @@ static int encode_common(b200jpeg_encoder *e, const b200jpeg_params *p, const vo
   // e.g. 12-bit noise at 15 MB per image, keep it; device-only runs never shrink: their sizes are not read back)
   {
     long long tb = 0; for (int ci = 0; ci < pl.g.nc; ci++) tb += pl.g.c[ci].blocks_per_image;
+    if (pl.lossless) tb = (tb + 7) / 8;                      // the per-sample scale prepare_batch sizes the buffers with
     if (e->calm_batches >= 2 && !device_only && e->cap_factor > 0.25 && e->max_image_scan_bytes * 8 < (size_t)((double)tb * 64 * 0.25)) e->cap_factor = 0.25;
     if (!device_only) e->max_image_scan_bytes = 0;
   }

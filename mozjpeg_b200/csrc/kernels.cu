@@ -3828,6 +3828,180 @@ void launch_encode(const Geom &g, const ScanDesc &sd, const DcRec *nz_rec, const
   else k_encode_seq<<<grid, 256, 0, s>>>(g, sd, nz_rec, sym, dcq, rl, tabs, stride, blk_bits, tile_bits, tile_base, seg_corr, seg_stride, bitbuf, bitbuf_stride_words, mark, mark_stride_words, status);
   LAUNCHED();
 }
+// =====================================================================
+// lossless (SOF3) coding: prediction + point transform (jclossls.c:43-250, jcdiffct.c:156-232) and the lossless
+// Huffman coder (jclhuff.c:316-530).  One MCU = one sample of each scan component (all components are 1x1 in lossless
+// mode, jcmaster.c:1079-1081); MCU t of a scan is the pixel (t % W, t / W).
+// =====================================================================
+// sample `k` of the pixel at px, unmasked as the null-type conversions leave it (jccolor.c:604-715 apply no
+// RANGE_LIMIT): 8-bit JSAMPLE, 12-bit J12SAMPLE (signed short), 16-bit J16SAMPLE (unsigned short).  The C-ABI takes
+// pitches, strides and pointers with no alignment, so a 16-bit sample is assembled from its two bytes (little endian).
+template <int PREC>
+__device__ __forceinline__ int ll_sample(const uint8_t *__restrict__ px, int k)
+{
+  if (PREC == 8) return (int)__ldg(px + k);
+  const unsigned short v = (unsigned short)(__ldg(px + 2 * k) | (unsigned)__ldg(px + 2 * k + 1) << 8);
+  return PREC == 12 ? (int)(short)v : (int)v;
+}
+// category (0..16) of a difference taken mod 2^16, and the value bits that follow it (jclhuff.c:356-391): the magnitude
+// is masked with 0x7FFF; -32768 mod 2^16 is category 16 with no value bits (the temp == 0 case at :361-369)
+__device__ __forceinline__ int ll_category(unsigned d16, unsigned &vbits)
+{
+  if (d16 & 0x8000u) {
+    const unsigned m = (0u - d16) & 0x7FFFu;
+    vbits = ~m;
+    return m ? 32 - __clz(m) : 16;
+  }
+  vbits = d16;
+  return d16 ? 32 - __clz(d16) : 0;
+}
+
+// The differences of one scan: diff[(img * ncomps + i) * W*H + t] for scan component i, and the categories counted into
+// hist[img][dc_tbl][0..16] (encode_mcus_gather, jclhuff.c:460-524) through a per-CTA histogram.
+// Row y restarts the prediction (first-row predictors) when y is a multiple of the rows per restart interval: reset_predictor
+// fires when restart_rows_to_go reaches 0, and the first-row differencer keeps itself for the next row exactly then
+// (jclossls.c:73-79, :111-114, :200-232); without restarts only row 0 is a first row.
+template <int PREC>
+__global__ void __launch_bounds__(256) k_lossless_diff(Geom g, ScanDesc sd, const uint8_t *__restrict__ src,
+                                                       uint16_t *__restrict__ diff, uint32_t *__restrict__ hist)
+{
+  __shared__ unsigned sh[4][17];
+  for (int i = threadIdx.x; i < 4 * 17; i += blockDim.x) sh[i / 17][i % 17] = 0;
+  __syncthreads();
+  const int img = blockIdx.y;
+  const long long npix = (long long)g.W * g.H;
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t < npix) {
+    const int y = (int)(t / g.W), x = (int)(t - (long long)y * g.W);
+    const int rows_per_restart = sd.ri ? sd.ri / g.W : 0;
+    const bool first_row = rows_per_restart ? (y % rows_per_restart) == 0 : y == 0;
+    constexpr int SB = PREC == 8 ? 1 : 2;
+    const size_t pxb = (size_t)g.in_comps * SB;
+    const uint8_t *row = src + (size_t)img * g.image_stride + (size_t)y * g.row_pitch;
+    const uint8_t *up = row - g.row_pitch;
+    const int Al = sd.Al;
+    for (int i = 0; i < sd.ncomps; i++) {
+      const int c = sd.ci[i];
+      const int k = g.px_first + (g.px_swap ? 2 - c : c);          // the RGB-family orders (jccolor.c:253-291); k = c otherwise
+      const int samp = ll_sample<PREC>(row + x * pxb, k) >> Al;      // RIGHT_SHIFT by Pt (jclossls.c:255-262)
+      int pred;
+      if (first_row) pred = x == 0 ? 1 << (PREC - Al - 1) : ll_sample<PREC>(row + (x - 1) * pxb, k) >> Al;
+      else {
+        const int Rb = ll_sample<PREC>(up + x * pxb, k) >> Al;
+        if (x == 0) pred = Rb;
+        else {
+          const int Ra = ll_sample<PREC>(row + (x - 1) * pxb, k) >> Al, Rc = ll_sample<PREC>(up + (x - 1) * pxb, k) >> Al;
+          switch (sd.Ss) {                                          // PREDICTOR1..7 (jlossls.h:37-43)
+          case 1: pred = Ra; break;
+          case 2: pred = Rb; break;
+          case 3: pred = Rc; break;
+          case 4: pred = Ra + Rb - Rc; break;
+          case 5: pred = Ra + ((Rb - Rc) >> 1); break;
+          case 6: pred = Rb + ((Ra - Rc) >> 1); break;
+          default: pred = (Ra + Rb) >> 1; break;
+          }
+        }
+      }
+      const unsigned d16 = (unsigned)(samp - pred) & 0xFFFFu;
+      diff[((size_t)img * sd.ncomps + i) * npix + t] = (uint16_t)d16;
+      unsigned vb;
+      atomicAdd(&sh[g.c[c].dc_tbl][ll_category(d16, vb)], 1u);
+    }
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < 4 * 17; i += blockDim.x) {
+    const unsigned v = sh[i / 17][i % 17];
+    if (v) atomicAdd(&hist[((size_t)img * HIST_SLOTS + i / 17) * HIST_BINS + i % 17], v);
+  }
+}
+
+// bits of every MCU (category codes + value bits), exclusive prefix inside the 256-MCU tile and the tile sums, in the
+// layout k_scan_layout reads
+__global__ void __launch_bounds__(256) k_lossless_bits(Geom g, ScanDesc sd, const uint16_t *__restrict__ diff,
+                                                       const DevHuff *__restrict__ tabs, size_t stride,
+                                                       uint32_t *__restrict__ blk_bits, uint32_t *__restrict__ tile_bits, uint32_t *__restrict__ status)
+{
+  __shared__ uint8_t size[4][17];
+  __shared__ unsigned ws[9];
+  const int img = blockIdx.y;
+  const DevHuff *t8 = reinterpret_cast<const DevHuff *>(reinterpret_cast<const char *>(tabs) + (size_t)img * stride);
+  for (int i = threadIdx.x; i < 4 * 17; i += blockDim.x) size[i / 17][i % 17] = t8[i / 17].size[i % 17];
+  __syncthreads();
+  const long long npix = (long long)g.W * g.H;
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  unsigned bits = 0; int bad = 0;
+  if (t < npix) {
+    for (int i = 0; i < sd.ncomps; i++) {
+      unsigned vb;
+      const int nb = ll_category(diff[((size_t)img * sd.ncomps + i) * npix + t], vb);
+      const int sz = size[g.c[sd.ci[i]].dc_tbl][nb];
+      if (!sz) bad = 1;
+      bits += sz + (nb == 16 ? 0 : nb);
+    }
+  }
+  if (bad) atomicOr(&status[img], 2u);
+  unsigned tot;
+  const unsigned pre = cta_excl_scan_256(bits, ws, tot);
+  if (t < npix) blk_bits[(size_t)img * npix + t] = pre;
+  if (threadIdx.x == 0) tile_bits[(size_t)img * gridDim.x + blockIdx.x] = tot;
+}
+
+// pack every MCU at its offset; restart markers as k_encode_seq writes them (emit_restart, jclhuff.c:286-309)
+__global__ void __launch_bounds__(256) k_lossless_encode(Geom g, ScanDesc sd, const uint16_t *__restrict__ diff,
+                                                         const DevHuff *__restrict__ tabs, size_t stride,
+                                                         const uint32_t *__restrict__ blk_bits, const unsigned long long *__restrict__ tile_base,
+                                                         const uint32_t *__restrict__ seg_corr, long long seg_stride,
+                                                         uint32_t *__restrict__ bitbuf, size_t bitbuf_stride_words,
+                                                         uint32_t *__restrict__ mark, size_t mark_stride_words, const uint32_t *__restrict__ status)
+{
+  __shared__ uint32_t cs[4][17];             // code | size << 16
+  const int img = blockIdx.y;
+  const DevHuff *t8 = reinterpret_cast<const DevHuff *>(reinterpret_cast<const char *>(tabs) + (size_t)img * stride);
+  for (int i = threadIdx.x; i < 4 * 17; i += blockDim.x) cs[i / 17][i % 17] = (uint32_t)t8[i / 17].code[i % 17] | (uint32_t)t8[i / 17].size[i % 17] << 16;
+  __syncthreads();
+  if (status[img] & ~1u) return;            // an earlier stage flagged this image (overflow / missing code)
+  const long long npix = (long long)g.W * g.H;
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= npix) return;
+  unsigned long long off = tile_base[(size_t)img * gridDim.x + blockIdx.x] + blk_bits[(size_t)img * npix + t];
+  if (sd.ri) off += seg_corr[(size_t)img * seg_stride + t / sd.ri];
+  BitSink sink;
+  sink.buf = bitbuf + (size_t)img * bitbuf_stride_words; sink.widx = off >> 5; sink.acc = 0; sink.nacc = (int)(off & 31);
+  for (int i = 0; i < sd.ncomps; i++) {
+    unsigned vb;
+    const int nb = ll_category(diff[((size_t)img * sd.ncomps + i) * npix + t], vb);
+    const uint32_t e = cs[g.c[sd.ci[i]].dc_tbl][nb];
+    const int vn = nb == 16 ? 0 : nb;
+    sink.put(((e & 0xFFFFu) << vn) | (vb & ((1u << vn) - 1u)), (int)(e >> 16) + vn);
+  }
+  if (sd.ri) emit_restart_marker(sink, sd, t, mark + (size_t)img * mark_stride_words);
+  sink.finish();
+}
+
+void launch_lossless_diff(const Geom &g, const ScanDesc &sd, int precision, const uint8_t *src, uint16_t *diff, uint32_t *hist, int n, cudaStream_t s)
+{
+  dim3 grid((unsigned)(((long long)g.W * g.H + 255) / 256), n);
+  if (precision == 8) k_lossless_diff<8><<<grid, 256, 0, s>>>(g, sd, src, diff, hist);
+  else if (precision == 12) k_lossless_diff<12><<<grid, 256, 0, s>>>(g, sd, src, diff, hist);
+  else k_lossless_diff<16><<<grid, 256, 0, s>>>(g, sd, src, diff, hist);
+  LAUNCHED();
+}
+void launch_lossless_bits(const Geom &g, const ScanDesc &sd, const uint16_t *diff, const DevHuff *tabs, size_t stride,
+                          uint32_t *blk_bits, uint32_t *tile_bits, uint32_t *status, int n, cudaStream_t s)
+{
+  dim3 grid((unsigned)(((long long)g.W * g.H + 255) / 256), n);
+  k_lossless_bits<<<grid, 256, 0, s>>>(g, sd, diff, tabs, stride, blk_bits, tile_bits, status);
+  LAUNCHED();
+}
+void launch_lossless_encode(const Geom &g, const ScanDesc &sd, const uint16_t *diff, const DevHuff *tabs, size_t stride,
+                            const uint32_t *blk_bits, const unsigned long long *tile_base, const uint32_t *seg_corr, long long seg_stride,
+                            uint32_t *bitbuf, size_t bitbuf_stride_words, uint32_t *mark, size_t mark_stride_words, const uint32_t *status, int n, cudaStream_t s)
+{
+  dim3 grid((unsigned)(((long long)g.W * g.H + 255) / 256), n);
+  k_lossless_encode<<<grid, 256, 0, s>>>(g, sd, diff, tabs, stride, blk_bits, tile_base, seg_corr, seg_stride, bitbuf, bitbuf_stride_words, mark, mark_stride_words, status);
+  LAUNCHED();
+}
+
 size_t stuff_tiles(size_t bitbuf_stride_words) { return (bitbuf_stride_words + STUFF_TILE_WORDS - 1) / STUFF_TILE_WORDS; }
 size_t stuff_lookback_bytes(size_t bitbuf_stride_words, int n) { return (size_t)n * 8 + (size_t)n * stuff_tiles(bitbuf_stride_words) * 8; }
 void launch_stuff(const uint32_t *bitbuf, size_t bitbuf_stride_words, const unsigned long long *total_bits, void *lookback,

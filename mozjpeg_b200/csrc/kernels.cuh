@@ -211,6 +211,17 @@ void launch_stuff(const uint32_t *bitbuf, size_t bitbuf_image_stride_words, cons
                   uint8_t *out, size_t out_image_stride, size_t out_capacity, const unsigned long long *out_start, unsigned long long *out_next,
                   uint32_t *scan_size, uint32_t *status, const uint32_t *mark, size_t mark_stride_words, int n, cudaStream_t s);
 
+// lossless (SOF3) scans: sd.ncomps components of one sample per MCU, sd.nblocks = W*H MCUs, sd.Ss the predictor, sd.Al
+// the point transform, sd.ri the restart interval in MCUs (whole rows).  diff: [n][sd.ncomps][W*H] uint16 differences
+// (mod 2^16); hist: the categories per DC table, [img][HIST_SLOTS][HIST_BINS] (zeroed by the caller).  The bit counts,
+// layout, packing and stuffing follow the sequential scans' stages (launch_scan_layout, launch_zero_stream, launch_stuff).
+void launch_lossless_diff(const Geom &g, const ScanDesc &sd, int precision, const uint8_t *src, uint16_t *diff, uint32_t *hist, int n, cudaStream_t s);
+void launch_lossless_bits(const Geom &g, const ScanDesc &sd, const uint16_t *diff, const DevHuff *tabs, size_t tabs_image_stride,
+                          uint32_t *blk_bits, uint32_t *tile_bits, uint32_t *status, int n, cudaStream_t s);
+void launch_lossless_encode(const Geom &g, const ScanDesc &sd, const uint16_t *diff, const DevHuff *tabs, size_t tabs_image_stride,
+                            const uint32_t *blk_bits, const unsigned long long *tile_base, const uint32_t *seg_corr, long long seg_stride,
+                            uint32_t *bitbuf, size_t bitbuf_image_stride_words, uint32_t *mark, size_t mark_stride_words, const uint32_t *status, int n, cudaStream_t s);
+
 // scan search: per-image best point transform of one Al-search group (see k_select_al)
 struct AlSearch { ScanDesc sd[24]; int first, per_al, nband, al_max, nscans_total; };
 void launch_select_al(const Geom &g, const AlSearch &as, const DevHuff *tabs_scan, const uint32_t *scan_size, int n, int *best_al, cudaStream_t s);

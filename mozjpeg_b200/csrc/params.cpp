@@ -10,6 +10,7 @@
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
+#include <algorithm>
 
 #include "std_tables.inc"
 
@@ -125,13 +126,13 @@ int b200jpeg_set_colorspace(b200jpeg_params *p, int colorspace) {
 int b200jpeg_default_colorspace(b200jpeg_params *p) {
   switch (p->in_color_space) {
   case B200JPEG_CS_GRAYSCALE: return b200jpeg_set_colorspace(p, B200JPEG_CS_GRAYSCALE);
-  case B200JPEG_CS_RGB:       return b200jpeg_set_colorspace(p, B200JPEG_CS_YCbCr);
+  case B200JPEG_CS_RGB:       return b200jpeg_set_colorspace(p, b200::is_lossless(p) ? B200JPEG_CS_RGB : B200JPEG_CS_YCbCr);   // jcparam.c:544-549
   case B200JPEG_CS_YCbCr:     return b200jpeg_set_colorspace(p, B200JPEG_CS_YCbCr);
   case B200JPEG_CS_CMYK:      return b200jpeg_set_colorspace(p, B200JPEG_CS_CMYK);        // by default, no translation
   case B200JPEG_CS_YCCK:      return b200jpeg_set_colorspace(p, B200JPEG_CS_YCCK);
   case B200JPEG_CS_UNKNOWN:   return b200jpeg_set_colorspace(p, B200JPEG_CS_UNKNOWN);
   default:
-    if (B200JPEG_CS_IS_RGB(p->in_color_space)) return b200jpeg_set_colorspace(p, B200JPEG_CS_YCbCr);     // jcparam.c:535-546
+    if (B200JPEG_CS_IS_RGB(p->in_color_space)) return b200jpeg_set_colorspace(p, b200::is_lossless(p) ? B200JPEG_CS_RGB : B200JPEG_CS_YCbCr);     // jcparam.c:535-549
     b200::set_error("unsupported input colorspace %d", p->in_color_space); return B200JPEG_ERR_UNSUPPORTED;
   }
 }
@@ -187,6 +188,10 @@ int b200jpeg_simple_progression(b200jpeg_params *p) {
     if (search_progression(p)) return B200JPEG_OK;
     p->optimize_scans = 0;   // jcparam.c:754 num_scans_luma=0 -> jcapistd.c:53-56 turns the search off
   }
+  if (b200::is_lossless(p)) {   // jcparam.c:875-880: lossless off again, colour space re-derived
+    p->num_scans = 0;
+    b200jpeg_default_colorspace(p);
+  }
   int n = p->num_components;
   bool maxc = p->compress_profile == B200JPEG_PROFILE_MAX_COMPRESSION;
   b200jpeg_scan_info *s = p->scan_info;
@@ -220,6 +225,71 @@ int b200jpeg_simple_progression(b200jpeg_params *p) {
     }
   }
   p->num_scans = (int)(s - p->scan_info);
+  return B200JPEG_OK;
+}
+
+}  // extern "C"
+
+namespace b200 {
+bool is_lossless(const b200jpeg_params *p)
+{
+  return !p->optimize_scans && p->num_scans > 0 && p->scan_info[0].Ss != 0 && p->scan_info[0].Se == 0;
+}
+
+// the script b200jpeg_enable_lossless installs in place of the reference's scan_info == NULL: one scan, marked by the
+// unused entry after it (comps_in_scan = -1), which no script the reference can express has
+static bool enable_lossless_script(const b200jpeg_params *p)
+{
+  return p->num_scans == 1 && p->scan_info[1].comps_in_scan == -1;
+}
+
+void lossless_start(const b200jpeg_params *in, b200jpeg_params *out)
+{
+  *out = *in;
+  out->smoothing_factor = 0;                                             // jcmaster.c:1077
+  b200jpeg_default_colorspace(out);                                      // :1078
+  for (int ci = 0; ci < out->num_components && ci < B200JPEG_MAX_COMPONENTS; ci++)
+    out->comp_info[ci].h_samp_factor = out->comp_info[ci].v_samp_factor = 1;   // :1079-1081
+  out->optimize_coding = 1;                                              // :1091-1094
+  // the reference keeps scan_info == NULL after jpeg_enable_lossless and codes one scan of all components as they are
+  // AFTER jpeg_default_colorspace (select_scan_parameters, jcmaster.c:500-513); the script stands in for that
+  if (enable_lossless_script(in) && out->num_components <= B200JPEG_MAX_COMPONENTS) {
+    b200jpeg_scan_info &s = out->scan_info[0];
+    s.comps_in_scan = out->num_components;
+    for (int k = 0; k < B200JPEG_MAX_COMPONENTS; k++) s.component_index[k] = k < out->num_components ? k : 0;
+  }
+}
+}  // namespace b200
+
+extern "C" {
+
+// jpeg_enable_lossless (jcparam.c:1015-1039)
+int b200jpeg_enable_lossless(b200jpeg_params *p, int psv, int pt)
+{
+  if (psv < 1 || psv > 7 || pt < 0 || pt >= p->data_precision) { b200::set_error("Invalid progression parameters Ss=%d Se=0 Ah=0 Al=%d", psv, pt); return B200JPEG_ERR_PARAM; }
+  if (p->num_scans > 0 && !b200::enable_lossless_script(p)) {
+    // the reference keeps an installed script next to its lossless flag.  The scan search's script skips
+    // validate_script (jcmaster.c:285-291), so the flag stays on beside progressive mode: with the trellis the passes fail
+    // ("Bogus buffer control mode"), without it the file gets SOF2 headers over the lossless compressor's data, which
+    // the device path does not represent.  Any other script decides by its first entry (jcmaster.c:302-330), which
+    // clears the flag for a sequential or progressive script: then the call changes nothing.
+    if (p->optimize_scans) {
+      if (p->trellis_quant) { b200::set_error("lossless mode needs trellis quantization off (cjpeg -notrellis), as in the reference"); return B200JPEG_ERR_PARAM; }
+      b200::set_error("lossless mode beside the scan search's script (the reference writes SOF2 headers over lossless data) is not on the device path");
+      return B200JPEG_ERR_UNSUPPORTED;
+    }
+    return B200JPEG_OK;
+  }
+  const int n = p->num_components;
+  if (n < 1 || n > B200JPEG_MAX_COMPONENTS) { b200::set_error("Too many color components: %d, max 4", n); return B200JPEG_ERR_PARAM; }
+  memset(p->scan_info, 0, sizeof p->scan_info);
+  b200jpeg_scan_info &s = p->scan_info[0];
+  s.comps_in_scan = n;
+  for (int k = 0; k < n; k++) s.component_index[k] = k;
+  s.Ss = psv; s.Se = 0; s.Ah = 0; s.Al = pt;
+  p->scan_info[1].comps_in_scan = -1;
+  p->num_scans = 1;
+  p->optimize_scans = 0;        // scan_info == NULL turns the scan search off at jpeg_start_compress (jcapistd.c:53-56)
   return B200JPEG_OK;
 }
 
@@ -262,15 +332,62 @@ void b200jpeg_set_defaults(b200jpeg_params *p, int profile) {
 
 static int div_round_up(long a, long b) { return (int)((a + b - 1) / b); }
 
+// validate_script's lossless branch (jcmaster.c:302-311, :389-415) on the script as given, before the start-time overrides
+static int validate_lossless_script(const b200jpeg_params *p)
+{
+  using b200::set_error;
+  if (p->num_scans > B200JPEG_MAX_SCANS) { set_error("Invalid scan script at entry 0"); return B200JPEG_ERR_PARAM; }
+  bool sent[4] = {false, false, false, false};
+  const b200jpeg_scan_info *s = p->scan_info;
+  for (int scanno = 1; scanno <= p->num_scans; scanno++, s++) {
+    const int n = s->comps_in_scan;
+    if (n <= 0 || n > 4) { set_error("Too many color components: %d, max 4", n); return B200JPEG_ERR_PARAM; }
+    for (int ci = 0; ci < n; ci++) {
+      const int t = s->component_index[ci];
+      if (t < 0 || t >= p->num_components || (ci > 0 && t <= s->component_index[ci - 1])) { set_error("Invalid scan script at entry %d", scanno); return B200JPEG_ERR_PARAM; }
+    }
+    if (s->Ss < 1 || s->Ss > 7 || s->Se != 0 || s->Ah != 0 || s->Al < 0 || s->Al >= p->data_precision) { set_error("Invalid progressive parameters at scan script entry %d", scanno); return B200JPEG_ERR_PARAM; }
+    for (int ci = 0; ci < n; ci++) { const int t = s->component_index[ci]; if (sent[t]) { set_error("Invalid scan script at entry %d", scanno); return B200JPEG_ERR_PARAM; } sent[t] = true; }
+  }
+  for (int ci = 0; ci < p->num_components && ci < 4; ci++) if (!sent[ci]) { set_error("Scan script does not transmit all data"); return B200JPEG_ERR_PARAM; }
+  return B200JPEG_OK;
+}
+
+static int validate_effective(const b200jpeg_params *p, bool lossless);
+
 int b200jpeg_validate(const b200jpeg_params *p) {
   using b200::set_error;
+  const bool lossless = b200::is_lossless(p);
+  if (lossless) {
+    if (p->num_components > 10) { set_error("Too many color components: %d, max 10", p->num_components); return B200JPEG_ERR_PARAM; }
+    if (p->num_components > B200JPEG_MAX_COMPONENTS) { set_error("%d components: the device path takes at most %d", p->num_components, B200JPEG_MAX_COMPONENTS); return B200JPEG_ERR_UNSUPPORTED; }
+    if (p->data_precision != 8 && p->data_precision != 12 && p->data_precision != 16) { set_error("Unsupported JPEG data precision %d", p->data_precision); return B200JPEG_ERR_PARAM; }
+    int rc = validate_lossless_script(p);
+    if (rc) return rc;
+    // the rest is checked on the block jpeg_start_compress works with
+    b200jpeg_params eff;
+    b200::lossless_start(p, &eff);
+    return validate_effective(&eff, true);
+  }
+  return validate_effective(p, false);
+}
+
+// everything validate checks on the parameter block jpeg_start_compress works with
+static int validate_effective(const b200jpeg_params *p, const bool lossless) {
+  using b200::set_error;
+  if (lossless) {
+    if (p->num_components > B200JPEG_MAX_COMPONENTS) { set_error("%d components: the device path takes at most %d", p->num_components, B200JPEG_MAX_COMPONENTS); return B200JPEG_ERR_UNSUPPORTED; }
+    // the difference controller has no JBUF_REQUANT mode (jcdiffct.c:116-137): the trellis passes fail with "Bogus buffer control mode"
+    if (p->trellis_quant) { set_error("lossless mode needs trellis quantization off (cjpeg -notrellis), as in the reference"); return B200JPEG_ERR_PARAM; }
+  }
   // initial_setup (jcmaster.c:169-249)
   if (p->image_height <= 0 || p->image_width <= 0 || p->num_components <= 0 || p->input_components <= 0) { set_error("Empty input image"); return B200JPEG_ERR_PARAM; }
   if (p->image_height > 65500 || p->image_width > 65500) { set_error("Maximum supported image dimension is 65500 pixels"); return B200JPEG_ERR_PARAM; }
-  if (p->data_precision != 8 && p->data_precision != 12) { set_error("Unsupported JPEG data precision %d", p->data_precision); return B200JPEG_ERR_PARAM; }   // JERR_BAD_PRECISION
+  // 16-bit samples exist in lossless mode only (jcinit.c:95-96)
+  if (p->data_precision != 8 && p->data_precision != 12 && !(lossless && p->data_precision == 16)) { set_error("Unsupported JPEG data precision %d", p->data_precision); return B200JPEG_ERR_PARAM; }   // JERR_BAD_PRECISION
   // 12-bit: the coefficient controller has no JBUF_REQUANT mode (jccoefct.c:132-138), so the reference cannot run the
   // trellis passes ("Bogus buffer control mode"); its 12-bit deringing is unusable (jcdctmgr.c:419)
-  if (p->data_precision == 12 && (p->trellis_quant || p->overshoot_deringing)) { set_error("12-bit precision needs trellis quantization and overshoot deringing off (cjpeg -notrellis -noovershoot), as in the reference"); return B200JPEG_ERR_PARAM; }
+  if (!lossless && p->data_precision == 12 && (p->trellis_quant || p->overshoot_deringing)) { set_error("12-bit precision needs trellis quantization and overshoot deringing off (cjpeg -notrellis -noovershoot), as in the reference"); return B200JPEG_ERR_PARAM; }
   if (p->num_components > 10) { set_error("Too many color components: %d, max 10", p->num_components); return B200JPEG_ERR_PARAM; }   // JERR_COMPONENT_COUNT
   if (p->num_components > B200JPEG_MAX_COMPONENTS) { set_error("%d components: the device path takes at most %d", p->num_components, B200JPEG_MAX_COMPONENTS); return B200JPEG_ERR_UNSUPPORTED; }
   int hmax = 1, vmax = 1;
@@ -279,7 +396,7 @@ int b200jpeg_validate(const b200jpeg_params *p) {
     if (c->h_samp_factor <= 0 || c->h_samp_factor > 4 || c->v_samp_factor <= 0 || c->v_samp_factor > 4) { set_error("Bogus sampling factors"); return B200JPEG_ERR_PARAM; }
     if (c->h_samp_factor > hmax) hmax = c->h_samp_factor;
     if (c->v_samp_factor > vmax) vmax = c->v_samp_factor;
-    if (c->quant_tbl_no < 0 || c->quant_tbl_no >= 4 || !p->quant_tbl_present[c->quant_tbl_no]) { set_error("Quantization table 0x%02x was not defined", c->quant_tbl_no); return B200JPEG_ERR_PARAM; }
+    if (!lossless && (c->quant_tbl_no < 0 || c->quant_tbl_no >= 4 || !p->quant_tbl_present[c->quant_tbl_no])) { set_error("Quantization table 0x%02x was not defined", c->quant_tbl_no); return B200JPEG_ERR_PARAM; }
     if (c->dc_tbl_no < 0 || c->dc_tbl_no >= 4 || c->ac_tbl_no < 0 || c->ac_tbl_no >= 4) { set_error("Huffman table index out of range"); return B200JPEG_ERR_PARAM; }
   }
   int blocks_in_mcu = 0;
@@ -299,6 +416,13 @@ int b200jpeg_validate(const b200jpeg_params *p) {
   if (in_size && p->input_components != in_size) { set_error("Bogus input colorspace"); return B200JPEG_ERR_PARAM; }
   // ... then num_components against jpeg_color_space, and the conversions it implements
   bool conv;
+  if (lossless) {
+    // only the null-type conversions exist in lossless mode (jccolor.c:604-715: JERR_CONVERSION_NOTIMPL otherwise)
+    const int want = jcs == B200JPEG_CS_GRAYSCALE ? 1 : jcs == B200JPEG_CS_RGB || jcs == B200JPEG_CS_YCbCr ? 3 : jcs == B200JPEG_CS_CMYK || jcs == B200JPEG_CS_YCCK ? 4 : p->input_components;
+    if (nc != want) { set_error("Bogus JPEG colorspace"); return B200JPEG_ERR_PARAM; }
+    conv = jcs == B200JPEG_CS_RGB ? B200JPEG_CS_IS_RGB(in_cs) : jcs == in_cs;
+    if (!conv) { set_error("Unsupported color conversion request"); return B200JPEG_ERR_PARAM; }
+  } else
   switch (jcs) {
   case B200JPEG_CS_GRAYSCALE:
     if (nc != 1) { set_error("Bogus JPEG colorspace"); return B200JPEG_ERR_PARAM; }
@@ -322,6 +446,13 @@ int b200jpeg_validate(const b200jpeg_params *p) {
   if (!conv) { set_error("Unsupported color conversion request"); return B200JPEG_ERR_PARAM; }
   // things the reference can do that the device path cannot (yet)
   if (p->restart_interval < 0 || p->restart_interval > 65535 || p->restart_in_rows < 0) { set_error("restart interval out of range"); return B200JPEG_ERR_PARAM; }
+  if (lossless) {
+    // the restart interval of every scan (jcmaster.c:595-600) must be whole rows: MCUs_per_row is the image width, all
+    // components being 1x1 (start_pass_lossless, jclossls.c:292-294: JERR_BAD_RESTART)
+    const int ri = p->restart_in_rows > 0 ? (int)std::min((long)p->restart_in_rows * p->image_width, 65535L) : p->restart_interval;
+    if (ri % p->image_width) { set_error("Restart interval %d is not a multiple of the number of MCUs per row (%d)", ri, p->image_width); return B200JPEG_ERR_PARAM; }
+    return B200JPEG_OK;
+  }
   if (p->dct_method < B200JPEG_DCT_ISLOW || p->dct_method > B200JPEG_DCT_FLOAT) { set_error("unknown dct_method %d", p->dct_method); return B200JPEG_ERR_PARAM; }
   if (p->smoothing_factor < 0 || p->smoothing_factor > 100) { set_error("smoothing_factor %d out of range 0..100", p->smoothing_factor); return B200JPEG_ERR_PARAM; }
   if (p->trellis_quant && p->use_scans_in_trellis && (p->trellis_freq_split < 1 || p->trellis_freq_split > 62)) { set_error("trellis_freq_split %d: the device path takes 1..62 with use_scans_in_trellis", p->trellis_freq_split); return B200JPEG_ERR_UNSUPPORTED; }

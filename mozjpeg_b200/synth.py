@@ -46,3 +46,17 @@ def synth_planes(p, seed: int):
         a = 128 + 90 * np.sin(xx / (7 + 3 * ci)) * np.cos(yy / (9 + 2 * ci)) + rng.normal(0, 10, (hib * 8, wib * 8))
         out.append(np.clip(a, 0, 255).astype(np.uint8))
     return out
+
+
+def synth_image16(seed: int, width: int, height: int, channels: int = 1) -> np.ndarray:
+    """16-bit input for the lossless encoder (medical / scientific content): a smooth field over the full 0..65535
+    range per channel plus N(0, 64) noise, clipped; uint16 samples, (height, width, channels)."""
+    rng = np.random.default_rng(seed)
+    y, x = np.mgrid[0:height, 0:width].astype(np.float32)
+    out = np.empty((height, width, channels), dtype=np.uint16)
+    for c in range(channels):
+        px, py = rng.uniform(200, 900, 2)
+        ph = rng.uniform(0, 6.28, 2)
+        f = 32768 + 30000 * np.sin(x * (6.2831853 / px) + ph[0]) * np.cos(y * (6.2831853 / py) + ph[1])
+        out[..., c] = np.clip(f + rng.normal(0, 64, f.shape).astype(np.float32), 0, 65535).astype(np.uint16)
+    return out

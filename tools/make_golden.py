@@ -279,7 +279,38 @@ def perimage_q():
     print("wrote", len(cases), "per-image-table cases")
 
 
+def lossless():
+    """tests/golden/lossless_golden.json: every case of tests/test_lossless.py (lossless mode at 8, 12 and 16 bits) encoded
+    by the reference library through build/librefll.so (tests/refll.c).  Wherever the reference's own cjpeg binary can
+    express the case (grayscale or RGB input read from a PGM / PPM whose maxval is the precision's largest sample, no
+    hand-made script), the binary's bytes must equal the driver's."""
+    import tempfile
+    import zlib
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import test_lossless as T
+    from mozjpeg_b200 import _abi as A
+    cases, checked = [], 0
+    for c in T.CASES:
+        sw, cs, nc, prec, (h, w), kind, script = c
+        pix = T.image(zlib.crc32(T._id(c).encode()), h, w, nc, prec, kind)
+        a = T.ref_encode(pix, sw, cs, script)
+        if cs in (A.CS_GRAYSCALE, A.CS_RGB) and script is None and int(pix.max()) <= (1 << prec) - 1:
+            with tempfile.NamedTemporaryFile(suffix=".pnm") as f:
+                f.write(b"%s\n%d %d\n%d\n" % (b"P5" if nc == 1 else b"P6", w, h, (1 << prec) - 1))
+                f.write(pix.astype(">u2").tobytes() if prec > 8 else pix.tobytes())
+                f.flush()
+                b = O.ref_cjpeg(f.name, sw)
+            assert a == b, ("refll disagrees with cjpeg", sw)
+            checked += 1
+        cases.append({"id": T._id(c), "md5": hashlib.md5(a).hexdigest(), "size": len(a)})
+    json.dump({"generator": "tools/make_golden.py --lossless", "reference": "mozilla/mozjpeg 5.0.0 (C path, WITH_SIMD=0), oracle/_ref",
+               "cjpeg_binary_checked": checked, "cases": cases}, open(os.path.join(GOLD, "lossless_golden.json"), "w"), indent=0)
+    print("wrote", len(cases), "lossless cases;", checked, "checked against the cjpeg binary")
+
+
 def main():
+    if "--lossless" in sys.argv:
+        return lossless()
     if "--perimage-q" in sys.argv:
         return perimage_q()
     if "--fullsize" in sys.argv:
