@@ -190,6 +190,12 @@ int  b200jpeg_validate(const b200jpeg_params *p);
  * what a progress monitor would be told. */
 int  b200jpeg_total_passes(const b200jpeg_params *p);
 
+/* Size of plane `ci` of the YUV image b200jpeg_encode_yuv_batch writes, as tj3EncodeYUVPlanes8 lays it out
+ * (turbojpeg.c:1528-1578): pw0 = image_width padded to a multiple of the largest h_samp_factor, ph0 = image_height
+ * padded to a multiple of the largest v_samp_factor; plane ci is pw0 * h_ci / hmax samples wide and
+ * ph0 * v_ci / vmax rows high.  B200JPEG_ERR_PARAM for ci outside the components or non-positive sizes / factors. */
+int  b200jpeg_yuv_plane_dims(const b200jpeg_params *p, int ci, int *width, int *height);
+
 /* ------------------------------------------------------------------ */
 /* 2. Encode entry points (device path).                               */
 /* ------------------------------------------------------------------ */
@@ -288,6 +294,27 @@ int  b200jpeg_encode_batch_coefs_qtables(b200jpeg_encoder *enc, const b200jpeg_p
                                          const int16_t *const *planes, int planes_on_device,
                                          const size_t *row_pitch_blocks, const size_t *image_stride_blocks,
                                          const uint16_t *qtables, int n_images);
+
+/*
+ * YUV encoding: replaces tj3EncodeYUVPlanes8 (turbojpeg.c:1467-1619), the colour conversion and downsampling of a
+ * compress without the JPEG stages, for a batch of `n_images` images sharing `p` (what setCompDefaults builds for the
+ * pixel format and TJSAMP_*).  Image i's plane ci (component ci of p) goes to planes[ci] + i * plane_stride[ci] as
+ * b200jpeg_yuv_plane_dims rows of samples, plane_pitch[ci] bytes apart; bytes between pw and the pitch and between
+ * images are not written.  Rows past image_height repeat the last row, columns past image_width the last column,
+ * like the reference; the downsamplers are those jinit_downsampler picks without smoothing (jcsample.c:463-545).
+ * pixels / pixels_on_device / row_pitch / image_stride as in b200jpeg_encode_batch; planes_on_device says where the
+ * planes are.  Host input or output is processed in chunks on the encoder's streams (staging of chunk k+1 and
+ * read-back of chunk k-1 overlap chunk k's kernel); with both sides on the device the call only enqueues the kernel
+ * on the encoder's stream (b200jpeg_encoder_set_stream) and returns.
+ * Besides b200jpeg_validate's checks: precision must be 8 and lossless parameter blocks are B200JPEG_ERR_PARAM, as is
+ * a plane pitch below the plane's width or a plane stride below one plane; a smoothing factor, or a sampling layout
+ * other than component 0 at the largest factors (1, 2 or 4 each way) with 1x1 components 1 and 2 (every TJSAMP_*),
+ * is B200JPEG_ERR_UNSUPPORTED, as are 2 or 4 components.
+ */
+int  b200jpeg_encode_yuv_batch(b200jpeg_encoder *enc, const b200jpeg_params *p,
+                               const void *pixels, int pixels_on_device, size_t row_pitch, size_t image_stride,
+                               uint8_t *const *planes, int planes_on_device, const size_t *plane_pitch,
+                               const size_t *plane_stride, int n_images);
 
 /* b200jpeg_encode_batch, but stops after the entropy-coded bytes are in HBM: no device->host
  * copy, no host-side file assembly.  Used to time the device pipeline alone. */

@@ -11,6 +11,7 @@
  *     jpeg_write_coefficients  (jctrans.c:39-66; the encode half of jpegtran)
  *     jpeg_finish_compress     (jcapimin.c:176-229)
  *     jpeg_write_marker        (jcapimin.c:232-261; segments are spliced in after the file header)
+ *     tj3EncodeYUVPlanes8 / tj3EncodeYUV8  (turbojpeg.c:1467-1690; TurboJPEG's YUV encoding, interposer form only)
  *
  * and runs the image through the C-ABI of include/b200jpeg.h (sm_90a kernels).
  * Everything else -- jpeg_create_compress, jpeg_set_defaults, jpeg_set_quality,
@@ -33,6 +34,7 @@
  */
 #define _GNU_SOURCE
 #include <dlfcn.h>
+#include <limits.h>
 #include <pthread.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -606,3 +608,136 @@ jpeg_write_m_byte(j_compress_ptr cinfo, int val)
   if (!real) real = (mbyte_fn)next_sym("jpeg_write_m_byte");
   real(cinfo, val);
 }
+
+#ifndef B200_SHIM_STANDALONE
+/*
+ * TurboJPEG YUV encoding: tj3EncodeYUVPlanes8 (turbojpeg.c:1467-1619) and tj3EncodeYUV8 (turbojpeg.c:1647-1690) run
+ * through b200jpeg_encode_yuv_batch.  The parameter block is what setCompDefaults (turbojpeg.c:330-397) builds from the
+ * handle's settings (read with tj3Get).  Bottom-up rows, lossless mode, anything the reference would refuse (so that
+ * its error text and tj3GetErrorStr stay its own), MOZ_B200_FORCE_CPU, a host without a device and any refusal of the
+ * C-ABI go to the reference's implementation.  (The standalone libjpeg.so.62 carries no TurboJPEG API.)
+ */
+#include "turbojpeg.h"
+
+typedef int (*tjget_fn)(tjhandle, int);
+typedef int (*tjset_fn)(tjhandle, int, int);
+typedef int (*tjyuvplanes_fn)(tjhandle, const unsigned char *, int, int, int, int, unsigned char **, int *);
+typedef int (*tjyuv8_fn)(tjhandle, const unsigned char *, int, int, int, int, unsigned char *, int);
+typedef int (*tjplanedim_fn)(int, int, int);
+
+/* an encoder for one call: the spare one, else a new one (NULL and g_no_device set when there is no device) */
+static b200jpeg_encoder *take_encoder(void)
+{
+  pthread_mutex_lock(&g_lock);
+  b200jpeg_encoder *enc = g_idle_enc; g_idle_enc = NULL;
+  const int no_device = g_no_device;
+  pthread_mutex_unlock(&g_lock);
+  if (!enc && !no_device && b200jpeg_encoder_create(&enc, 0) != B200JPEG_OK) {
+    enc = NULL; pthread_mutex_lock(&g_lock); g_no_device = 1; pthread_mutex_unlock(&g_lock);
+  }
+  return enc;
+}
+static void give_encoder(b200jpeg_encoder *enc)
+{
+  pthread_mutex_lock(&g_lock);
+  if (!g_idle_enc) { g_idle_enc = enc; enc = NULL; }
+  pthread_mutex_unlock(&g_lock);
+  if (enc) b200jpeg_encoder_destroy(enc);
+}
+
+/* the device path of tj3EncodeYUVPlanes8: NULL when the planes are written, else why the reference has to run */
+static const char *encode_yuv_device(tjhandle handle, const unsigned char *srcBuf, int width, int pitch, int height,
+                                     int pixelFormat, unsigned char **dstPlanes, int *strides)
+{
+  static tjget_fn get; static tjset_fn set;
+  if (!get) get = (tjget_fn)next_sym("tj3Get");
+  if (!set) set = (tjset_fn)next_sym("tj3Set");
+  if (getenv("MOZ_B200_FORCE_CPU")) return "MOZ_B200_FORCE_CPU is set";
+  /* turbojpeg.c:1488-1503 */
+  if (!handle || !srcBuf || width <= 0 || pitch < 0 || height <= 0 || pixelFormat < 0 || pixelFormat >= TJ_NUMPF || !dstPlanes || !dstPlanes[0])
+    return "an argument the reference refuses";
+  /* a compress instance takes TJPARAM_OPTIMIZE, a decompress-only one refuses it: setting the current value tells them
+   * apart without changing anything */
+  if (set(handle, TJPARAM_OPTIMIZE, get(handle, TJPARAM_OPTIMIZE)) != 0) return "not a compress instance";
+  const int subsamp = get(handle, TJPARAM_SUBSAMP);
+  if (subsamp < 0 || subsamp >= TJ_NUMSAMP) return "TJPARAM_SUBSAMP is not set";
+  if (subsamp != TJSAMP_GRAY && (!dstPlanes[1] || !dstPlanes[2])) return "an argument the reference refuses";
+  if (pixelFormat == TJPF_CMYK) return "CMYK pixels";
+  if (get(handle, TJPARAM_BOTTOMUP) == 1) return "bottom-up rows";
+  if (get(handle, TJPARAM_LOSSLESS) == 1) return "lossless mode";
+  /* setCompDefaults: pf2cs, jpeg_set_defaults under JCP_FASTEST, the colour space, the luma sampling factors */
+  static const int pf2cs[TJ_NUMPF] = { B200JPEG_CS_EXT_RGB, B200JPEG_CS_EXT_BGR, B200JPEG_CS_EXT_RGBX, B200JPEG_CS_EXT_BGRX,
+    B200JPEG_CS_EXT_XBGR, B200JPEG_CS_EXT_XRGB, B200JPEG_CS_GRAYSCALE, B200JPEG_CS_EXT_RGBA, B200JPEG_CS_EXT_BGRA,
+    B200JPEG_CS_EXT_ABGR, B200JPEG_CS_EXT_ARGB, B200JPEG_CS_CMYK };
+  static const int tjcs2cs[TJ_NUMCS] = { B200JPEG_CS_RGB, B200JPEG_CS_YCbCr, B200JPEG_CS_GRAYSCALE, B200JPEG_CS_CMYK, B200JPEG_CS_YCCK };
+  b200jpeg_params p;
+  memset(&p, 0, sizeof p);
+  p.in_color_space = pf2cs[pixelFormat]; p.input_components = tjPixelSize[pixelFormat];
+  p.data_precision = 8;
+  b200jpeg_set_defaults(&p, B200JPEG_PROFILE_FASTEST);
+  p.image_width = width; p.image_height = height;
+  const int tjcs = get(handle, TJPARAM_COLORSPACE);
+  const int jcs = tjcs >= 0 && tjcs < TJ_NUMCS ? tjcs2cs[tjcs] : subsamp == TJSAMP_GRAY ? B200JPEG_CS_GRAYSCALE : B200JPEG_CS_YCbCr;
+  if (b200jpeg_set_colorspace(&p, jcs) != B200JPEG_OK) return b200jpeg_last_error();
+  /* the reference writes three planes unless TJSAMP_GRAY: other component counts are its business */
+  if (p.num_components != (subsamp == TJSAMP_GRAY ? 1 : 3)) return "component count differs from the subsampling's planes";
+  p.comp_info[0].h_samp_factor = tjMCUWidth[subsamp] / 8; p.comp_info[0].v_samp_factor = tjMCUHeight[subsamp] / 8;
+  for (int ci = 1; ci < p.num_components; ci++) p.comp_info[ci].h_samp_factor = p.comp_info[ci].v_samp_factor = 1;
+  if (b200jpeg_validate(&p) != B200JPEG_OK) return b200jpeg_last_error();
+  size_t pitch_b[3] = {0, 0, 0}, stride_b[3] = {0, 0, 0};
+  for (int ci = 0; ci < p.num_components; ci++) {
+    int pw, ph;
+    if (b200jpeg_yuv_plane_dims(&p, ci, &pw, &ph) != B200JPEG_OK) return b200jpeg_last_error();
+    const int s = strides && strides[ci] != 0 ? strides[ci] : pw;                 /* turbojpeg.c:1585 */
+    if (s < pw) return "plane stride below the plane width";
+    pitch_b[ci] = (size_t)s;
+  }
+  b200jpeg_encoder *enc = take_encoder();
+  if (!enc) return b200jpeg_last_error();
+  const size_t row_pitch = pitch ? (size_t)pitch : (size_t)width * tjPixelSize[pixelFormat];
+  const int rc = b200jpeg_encode_yuv_batch(enc, &p, srcBuf, 0, row_pitch, 0, (uint8_t *const *)dstPlanes, 0, pitch_b, stride_b, 1);
+  give_encoder(enc);
+  if (rc != B200JPEG_OK) return b200jpeg_last_error();
+  if (verbose()) fprintf(stderr, "b200 shim: device path (YUV planes %dx%d, TJSAMP %d, TJPF %d)\n", width, height, subsamp, pixelFormat);
+  return NULL;
+}
+
+DLLEXPORT int tj3EncodeYUVPlanes8(tjhandle handle, const unsigned char *srcBuf, int width, int pitch, int height,
+                                  int pixelFormat, unsigned char **dstPlanes, int *strides)
+{
+  static tjyuvplanes_fn real;
+  if (!real) real = (tjyuvplanes_fn)next_sym("tj3EncodeYUVPlanes8");
+  const char *why = encode_yuv_device(handle, srcBuf, width, pitch, height, pixelFormat, dstPlanes, strides);
+  if (!why) return 0;
+  if (verbose()) fprintf(stderr, "b200 shim: reference path (YUV planes: %s)\n", why);
+  if (required()) { fprintf(stderr, "b200 shim: B200_SHIM_REQUIRE=1 and the device path was not taken: %s\n", why); return -1; }
+  return real(handle, srcBuf, width, pitch, height, pixelFormat, dstPlanes, strides);
+}
+
+/* tj3EncodeYUV8: the planes back to back, rows padded to `align` (turbojpeg.c:1657-1686), then the planes function */
+DLLEXPORT int tj3EncodeYUV8(tjhandle handle, const unsigned char *srcBuf, int width, int pitch, int height,
+                            int pixelFormat, unsigned char *dstBuf, int align)
+{
+  static tjyuv8_fn real; static tjget_fn get; static tjplanedim_fn plane_w, plane_h;
+  if (!real) real = (tjyuv8_fn)next_sym("tj3EncodeYUV8");
+  if (!get) get = (tjget_fn)next_sym("tj3Get");
+  if (!plane_w) plane_w = (tjplanedim_fn)next_sym("tj3YUVPlaneWidth");
+  if (!plane_h) plane_h = (tjplanedim_fn)next_sym("tj3YUVPlaneHeight");
+  const int subsamp = handle ? get(handle, TJPARAM_SUBSAMP) : -1;
+  if (!handle || width <= 0 || height <= 0 || !dstBuf || align < 1 || (align & (align - 1)) || subsamp < 0 || subsamp >= TJ_NUMSAMP)
+    return real(handle, srcBuf, width, pitch, height, pixelFormat, dstBuf, align);    /* the reference's refusals */
+  unsigned char *planes[3] = {dstBuf, NULL, NULL};
+  int strides[3] = {0, 0, 0};
+  const int pw0 = plane_w(0, width, subsamp), ph0 = plane_h(0, height, subsamp);
+  strides[0] = (pw0 + align - 1) & ~(align - 1);
+  if (subsamp != TJSAMP_GRAY) {
+    const int pw1 = plane_w(1, width, subsamp), ph1 = plane_h(1, height, subsamp);
+    strides[1] = strides[2] = (pw1 + align - 1) & ~(align - 1);
+    if ((unsigned long long)strides[0] * ph0 > (unsigned long long)INT_MAX || (unsigned long long)strides[1] * ph1 > (unsigned long long)INT_MAX)
+      return real(handle, srcBuf, width, pitch, height, pixelFormat, dstBuf, align);
+    planes[1] = planes[0] + (size_t)strides[0] * ph0;
+    planes[2] = planes[1] + (size_t)strides[1] * ph1;
+  }
+  return tj3EncodeYUVPlanes8(handle, srcBuf, width, pitch, height, pixelFormat, planes, strides);
+}
+#endif

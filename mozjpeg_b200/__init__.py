@@ -18,7 +18,7 @@ from .cjpeg import params_from_switches, pnm_samples, read_pnm, read_ppm  # noqa
 
 _lib = A.load()          # raises ImportError with build instructions if missing
 
-__all__ = ["Encoder", "Params", "params_from_switches", "read_ppm", "cjpeg", "tj3_params", "quality_tables", "B200JpegError"]
+__all__ = ["Encoder", "Params", "params_from_switches", "read_ppm", "cjpeg", "tj3_params", "quality_tables", "yuv_plane_dims", "B200JpegError"]
 
 
 class Encoder:
@@ -140,6 +140,30 @@ class Encoder:
         else:
             A.check(_lib.b200jpeg_encode_batch(self._h, C.byref(p), ptr, int(on_device), row_pitch, image_stride, n), "encode_batch")
 
+    # -- YUV encoding (tj3EncodeYUVPlanes8) ---------------------------------
+    def encode_yuv_batch(self, p: Params, images: np.ndarray) -> List[List[np.ndarray]]:
+        """images: (N, H, W, C) or (N, H, W) uint8 host array -> per image, the list of its (ph, pw) uint8 planes
+        (one per component of p, sizes from yuv_plane_dims), as tj3EncodeYUVPlanes8 writes them."""
+        a = np.ascontiguousarray(images, dtype=np.uint8)
+        if a.ndim == 3 and p.input_components == 1:
+            a = a[..., None]
+        n, h, w, c = a.shape
+        if (w, h, c) != (p.image_width, p.image_height, p.input_components):
+            raise ValueError("array shape does not match params")
+        planes = [np.empty((n,) + yuv_plane_dims(p, ci)[::-1], dtype=np.uint8) for ci in range(p.num_components)]
+        self.encode_yuv_batch_ptr(p, a.ctypes.data, False, a.strides[1], a.strides[0],
+                                  [q.ctypes.data for q in planes], False, [q.strides[1] for q in planes], [q.strides[0] for q in planes], n)
+        return [[q[i] for q in planes] for i in range(n)]
+
+    def encode_yuv_batch_ptr(self, p: Params, ptr: int, on_device: bool, row_pitch: int, image_stride: int,
+                             planes: Sequence[int], planes_on_device: bool, plane_pitch: Sequence[int], plane_stride: Sequence[int], n: int) -> None:
+        """Raw-pointer form of encode_yuv_batch (device tensors, pinned host buffers): planes[ci] is image 0's plane of
+        component ci, plane_pitch / plane_stride in bytes.  With pixels and planes on the device the call only enqueues."""
+        k = len(planes)
+        A.check(_lib.b200jpeg_encode_yuv_batch(self._h, C.byref(p), ptr, int(on_device), row_pitch, image_stride,
+                                               (C.c_void_p * k)(*planes), int(planes_on_device), (C.c_size_t * k)(*plane_pitch),
+                                               (C.c_size_t * k)(*plane_stride), n), "encode_yuv_batch")
+
     def get_output(self, i: int) -> bytes:
         d = C.POINTER(C.c_uint8)(); n = C.c_size_t(0)
         A.check(_lib.b200jpeg_get_output(self._h, i, C.byref(d), C.byref(n)), "get_output")
@@ -210,15 +234,22 @@ def cjpeg(switches: Sequence[str], ppm: bytes, encoder: Optional[Encoder] = None
 
 
 def tj3_params(width: int, height: int, quality: int = 75, subsamp: str = "420", optimize: bool = False,
-               progressive: bool = False, gray_input: bool = False, cmyk: bool = False, colorspace: int = None) -> Params:
+               progressive: bool = False, gray_input: bool = False, cmyk: bool = False, colorspace: int = None,
+               pixel_format: str = None) -> Params:
     """The parameter block tj3Compress8 builds (turbojpeg.c:330-397
     setCompDefaults): JCP_FASTEST, quality via jpeg_set_quality(.., TRUE),
     YCbCr (or grayscale) with the luma sampling factors of TJSAMP_*.
     cmyk: TJPF_CMYK pixels, written as YCCK unless ``colorspace`` (TJPARAM_COLORSPACE as a CS_* value) says
-    otherwise; component 3 gets the luma sampling factors."""
+    otherwise; component 3 gets the luma sampling factors.
+    pixel_format: a TJPF_* name ("RGB", "BGR", "RGBX", ..., "ARGB", "GRAY", "CMYK") instead of gray_input / cmyk; the
+    RGB family sets the matching JCS_EXT_* input order (pf2cs, turbojpeg.c)."""
+    if pixel_format is not None:
+        gray_input, cmyk = pixel_format == "GRAY", pixel_format == "CMYK"
     p = Params()
     p.in_color_space = A.CS_GRAYSCALE if gray_input else (A.CS_CMYK if cmyk else A.CS_RGB)
     p.input_components = 1 if gray_input else (4 if cmyk else 3)
+    if pixel_format is not None and not (gray_input or cmyk):
+        p.in_color_space, p.input_components = A.CS_EXT["EXT_" + pixel_format][:2]
     p.data_precision = 8
     p.image_width, p.image_height = width, height
     _lib.b200jpeg_set_defaults(C.byref(p), A.PROFILE_FASTEST)
@@ -238,6 +269,13 @@ def tj3_params(width: int, height: int, quality: int = 75, subsamp: str = "420",
     if p.num_components > 3:
         p.comp_info[3].h_samp_factor, p.comp_info[3].v_samp_factor = hv
     return p
+
+
+def yuv_plane_dims(p: Params, ci: int):
+    """(width, height) of plane ci of the YUV image Encoder.encode_yuv_batch writes (b200jpeg_yuv_plane_dims)."""
+    w = C.c_int(0); h = C.c_int(0)
+    A.check(_lib.b200jpeg_yuv_plane_dims(C.byref(p), ci, C.byref(w), C.byref(h)), "yuv_plane_dims")
+    return w.value, h.value
 
 
 def quality_tables(p: Params, qualities: Sequence[int], force_baseline: bool = True) -> np.ndarray:

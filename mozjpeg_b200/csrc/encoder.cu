@@ -129,6 +129,8 @@ struct b200jpeg_encoder {
   unsigned long long launches_at_create = 0;
   // timing
   std::vector<cudaEvent_t> ev; std::vector<const char *> ev_names, stage_names; std::vector<float> stage_ms; std::vector<int> stage_calls;
+  size_t pending_marks = 0;                     // device-resident YUV batch: timer events not yet summed into stage_ms
+  DevBuf d_yuv;                                 // YUV planes bound for host memory, staged per chunk
   std::vector<cudaEvent_t> ev_in, ev_done;      // per chunk: pixels staged / pipeline + metadata read-back queued
   bool own_stream = true;
   // streaming shim state
@@ -388,6 +390,23 @@ struct Timer {
     idx++;
   }
 };
+
+// per-stage device times from the first `marks` timer events, summed by stage name over the chunks; an interval starts
+// at every mark but "end" (with two streams the intervals of concurrent chunks overlap)
+static void collect_stage_times(b200jpeg_encoder *e, size_t marks)
+{
+  e->pending_marks = 0;
+  e->stage_names.clear(); e->stage_ms.clear(); e->stage_calls.clear();
+  if (marks) cudaEventSynchronize(e->ev[marks - 1]);
+  for (size_t i = 0; i + 1 < marks; i++) {
+    if (!strcmp(e->ev_names[i], "end")) continue;
+    float ms = 0.f; cudaEventElapsedTime(&ms, e->ev[i], e->ev[i + 1]);
+    size_t k = 0;
+    for (; k < e->stage_names.size(); k++) if (!strcmp(e->stage_names[k], e->ev_names[i])) break;
+    if (k == e->stage_names.size()) { e->stage_names.push_back(e->ev_names[i]); e->stage_ms.push_back(0.f); e->stage_calls.push_back(0); }
+    e->stage_ms[k] += ms; e->stage_calls[k]++;
+  }
+}
 
 static uint32_t scan_slot_mask(const Plan &pl, const ScanDesc &sd)
 {
@@ -1436,16 +1455,114 @@ static int encode_common(b200jpeg_encoder *e, const b200jpeg_params *p, const vo
   e->calm_batches = grew ? 0 : e->calm_batches + 1;
   if (rc == 1) { set_error("output does not fit even after growing buffers"); return B200JPEG_ERR_BUFFER; }
   if (rc) return rc;
-  // per-stage device times (CUDA events on the encoder's stream), summed by stage name over the chunks
-  e->stage_names.clear(); e->stage_ms.clear(); e->stage_calls.clear();
-  for (size_t i = 0; i + 1 < tm.idx; i++) {
-    if (!strcmp(e->ev_names[i], "end")) continue;           // (with two streams the intervals of concurrent chunks overlap)
-    float ms = 0.f; cudaEventElapsedTime(&ms, e->ev[i], e->ev[i + 1]);
-    size_t k = 0;
-    for (; k < e->stage_names.size(); k++) if (!strcmp(e->stage_names[k], e->ev_names[i])) break;
-    if (k == e->stage_names.size()) { e->stage_names.push_back(e->ev_names[i]); e->stage_ms.push_back(0.f); e->stage_calls.push_back(0); }
-    e->stage_ms[k] += ms; e->stage_calls[k]++;
+  collect_stage_times(e, tm.idx);
+  return B200JPEG_OK;
+}
+
+// tj3EncodeYUVPlanes8 on the device (b200jpeg_encode_yuv_batch)
+static int encode_yuv(b200jpeg_encoder *e, const b200jpeg_params *p, const void *pixels, int pixels_on_device, size_t row_pitch, size_t image_stride,
+                      uint8_t *const *planes, int planes_on_device, const size_t *plane_pitch, const size_t *plane_stride, int n_images)
+{
+  if (!e || !p || !pixels || !planes || !plane_pitch || !plane_stride || n_images <= 0) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
+  int rc = b200jpeg_validate(p);
+  if (rc) return rc;
+  if (is_lossless(p)) { set_error("YUV encoding has no lossless mode"); return B200JPEG_ERR_PARAM; }
+  if (p->data_precision != 8) { set_error("YUV encoding takes 8-bit samples only (data precision %d)", p->data_precision); return B200JPEG_ERR_PARAM; }
+  if (p->smoothing_factor) { set_error("YUV encoding with input smoothing is not on the device path"); return B200JPEG_ERR_UNSUPPORTED; }
+  if ((rc = build_plan(p, row_pitch, image_stride, e->plan))) return rc;
+  const Geom &g = e->plan.g;
+  const bool pow2 = (g.hmax == 1 || g.hmax == 2 || g.hmax == 4) && (g.vmax == 1 || g.vmax == 2 || g.vmax == 4);
+  const bool layout = (g.nc == 1 || g.nc == 3) && g.c[0].h == g.hmax && g.c[0].v == g.vmax &&
+                      (g.nc == 1 || (g.c[1].h == 1 && g.c[1].v == 1 && g.c[2].h == 1 && g.c[2].v == 1));
+  if (!pow2 || !layout) { set_error("YUV encoding: the device path takes component 0 at sampling factors of 1, 2 or 4 and 1x1 components 1 and 2 (the TJSAMP_* layouts)"); return B200JPEG_ERR_UNSUPPORTED; }
+  const size_t row_bytes = (size_t)g.W * g.in_comps, image_bytes = row_pitch * (size_t)(g.H - 1) + row_bytes;
+  if (row_pitch < row_bytes) { set_error("row_pitch smaller than a row"); return B200JPEG_ERR_PARAM; }
+  if (n_images > 1 && image_stride < image_bytes) { set_error("image_stride smaller than an image"); return B200JPEG_ERR_PARAM; }
+  YuvOut out; memset(&out, 0, sizeof out);
+  size_t plane_bytes[3] = {0, 0, 0};
+  for (int ci = 0; ci < g.nc; ci++) {
+    b200jpeg_yuv_plane_dims(p, ci, &out.pw[ci], &out.ph[ci]);
+    plane_bytes[ci] = plane_pitch[ci] * (size_t)(out.ph[ci] - 1) + out.pw[ci];
+    if (!planes[ci] || plane_pitch[ci] < (size_t)out.pw[ci] || (n_images > 1 && plane_stride[ci] < plane_bytes[ci])) {
+      set_error("YUV plane %d: bad pointer, pitch or stride (needs %d rows of %d samples)", ci, out.ph[ci], out.pw[ci]); return B200JPEG_ERR_PARAM;
+    }
   }
+  CU(cudaSetDevice(e->device));
+  e->n = 0; e->files.clear();                    // no JPEG files from this call
+  Timer tm{e};
+  if (pixels_on_device && planes_on_device) {
+    // launches only, on the encoder's (or the caller's) stream: stage times are read when asked for
+    for (int ci = 0; ci < g.nc; ci++) { out.p[ci] = planes[ci]; out.pitch[ci] = plane_pitch[ci]; out.stride[ci] = plane_stride[ci]; }
+    for (int i0 = 0; i0 < n_images; i0 += 65535) {
+      const int nk = std::min(65535, n_images - i0);
+      YuvOut o = out;
+      for (int ci = 0; ci < g.nc; ci++) o.p[ci] += (size_t)i0 * plane_stride[ci];
+      tm.mark("encode_yuv");
+      launch_encode_yuv(g, static_cast<const uint8_t *>(pixels) + (size_t)i0 * image_stride, o, nk, e->stream);
+      tm.mark("end");
+    }
+    CU(cudaGetLastError());
+    e->stage_names.clear(); e->stage_ms.clear(); e->stage_calls.clear();
+    e->pending_marks = tm.idx;
+    return B200JPEG_OK;
+  }
+  // host input and / or output: chunks of about 128 MB of pixels rotating over three staging slots, so that chunk k+1's
+  // host->device copy (s_in) and chunk k-1's device->host copy (s_out) overlap chunk k's kernel (e->stream)
+  int C = e->chunk_images_override > 0 ? e->chunk_images_override : (int)std::max<size_t>(1, ((size_t)128 << 20) / std::max(image_bytes, image_stride));
+  C = std::min(std::min(C, n_images), 65535);
+  const int nchunks = (n_images + C - 1) / C, NSLOT = 3;
+  e->chunk = C;
+  const size_t in_slot = pixels_on_device ? 0 : ((image_stride * (size_t)(C - 1) + image_bytes + 255) & ~(size_t)255);
+  size_t out_off[3] = {0, 0, 0}, out_slot = 0;
+  if (!planes_on_device)
+    for (int ci = 0; ci < g.nc; ci++) { out_off[ci] = out_slot; out_slot += ((size_t)out.pw[ci] * out.ph[ci] * C + 255) & ~(size_t)255; }
+  if (in_slot && (rc = e->d_src.reserve(in_slot * NSLOT))) return rc;
+  if (out_slot && (rc = e->d_yuv.reserve(out_slot * NSLOT))) return rc;
+  while ((int)e->ev_in.size() < nchunks) { cudaEvent_t ev; CU(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming)); e->ev_in.push_back(ev); }
+  while ((int)e->ev_done.size() < nchunks) { cudaEvent_t ev; CU(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming)); e->ev_done.push_back(ev); }
+  std::vector<cudaEvent_t> ev_read(nchunks);     // chunk k's read-back done: its output slot may be reused
+  for (int k = 0; k < nchunks; k++) { CU(cudaEventCreateWithFlags(&ev_read[k], cudaEventDisableTiming)); }
+  rc = B200JPEG_OK;
+  for (int k = 0; k < nchunks && rc == B200JPEG_OK; k++) {
+    const int i0 = k * C, nk = std::min(C, n_images - i0), slot = k % NSLOT;
+    const uint8_t *src = static_cast<const uint8_t *>(pixels) + (size_t)i0 * image_stride;
+    if (!pixels_on_device) {
+      uint8_t *dst = e->d_src.as<uint8_t>() + slot * in_slot;
+      if (k >= NSLOT) cudaStreamWaitEvent(e->s_in, e->ev_done[k - NSLOT], 0);        // the slot's previous kernel has read it
+      tm.s = e->s_in; tm.mark("h2d");
+      if (cudaMemcpyAsync(dst, src, image_stride * (size_t)(nk - 1) + image_bytes, cudaMemcpyHostToDevice, e->s_in) != cudaSuccess) { set_error("host->device copy failed"); rc = B200JPEG_ERR_CUDA; break; }
+      tm.mark("end");
+      cudaEventRecord(e->ev_in[k], e->s_in);
+      cudaStreamWaitEvent(e->stream, e->ev_in[k], 0);
+      src = dst;
+    }
+    YuvOut o = out;
+    for (int ci = 0; ci < g.nc; ci++) {
+      if (planes_on_device) { o.p[ci] = planes[ci] + (size_t)i0 * plane_stride[ci]; o.pitch[ci] = plane_pitch[ci]; o.stride[ci] = plane_stride[ci]; }
+      else { o.p[ci] = e->d_yuv.as<uint8_t>() + slot * out_slot + out_off[ci]; o.pitch[ci] = out.pw[ci]; o.stride[ci] = (size_t)out.pw[ci] * out.ph[ci]; }
+    }
+    if (!planes_on_device && k >= NSLOT) cudaStreamWaitEvent(e->stream, ev_read[k - NSLOT], 0);   // the slot's previous read-back is done
+    tm.s = e->stream; tm.mark("encode_yuv");
+    launch_encode_yuv(g, src, o, nk, e->stream);
+    tm.mark("end");
+    if (cudaGetLastError() != cudaSuccess) { set_error("k_encode_yuv launch failed"); rc = B200JPEG_ERR_CUDA; break; }
+    cudaEventRecord(e->ev_done[k], e->stream);
+    if (!planes_on_device) {
+      cudaStreamWaitEvent(e->s_out, e->ev_done[k], 0);
+      tm.s = e->s_out; tm.mark("d2h");
+      for (int i = 0; i < nk && rc == B200JPEG_OK; i++)
+        for (int ci = 0; ci < g.nc; ci++)
+          if (cudaMemcpy2DAsync(planes[ci] + (size_t)(i0 + i) * plane_stride[ci], plane_pitch[ci], o.p[ci] + (size_t)i * o.stride[ci], o.pitch[ci],
+                                out.pw[ci], out.ph[ci], cudaMemcpyDeviceToHost, e->s_out) != cudaSuccess) { set_error("device->host copy failed"); rc = B200JPEG_ERR_CUDA; break; }
+      tm.mark("end");
+      cudaEventRecord(ev_read[k], e->s_out);
+    }
+  }
+  cudaStreamSynchronize(e->s_in); cudaStreamSynchronize(e->stream); cudaStreamSynchronize(e->s_out);
+  for (cudaEvent_t ev : ev_read) cudaEventDestroy(ev);
+  if (rc) return rc;
+  CU(cudaGetLastError());
+  collect_stage_times(e, tm.idx);
   return B200JPEG_OK;
 }
 
@@ -1492,7 +1609,7 @@ void b200jpeg_encoder_destroy(b200jpeg_encoder *e)
   if (e->s_in) cudaStreamSynchronize(e->s_in);
   if (e->s_out) cudaStreamSynchronize(e->s_out);
   for (int i = 1; i < MAX_ARENAS; i++) if (e->sc[i]) cudaStreamSynchronize(e->sc[i]);
-  DevBuf *db[] = {&e->d_src, &e->d_tabs_scan, &e->d_tabs_fixed, &e->d_status, &e->d_out_pos, &e->d_scan_size, &e->d_out, &e->d_qt, &e->d_tc, &e->d_best_al_all, &e->d_qimg_all, &e->d_qset};
+  DevBuf *db[] = {&e->d_src, &e->d_yuv, &e->d_tabs_scan, &e->d_tabs_fixed, &e->d_status, &e->d_out_pos, &e->d_scan_size, &e->d_out, &e->d_qt, &e->d_tc, &e->d_best_al_all, &e->d_qimg_all, &e->d_qset};
   for (DevBuf *b : db) b->release();
   for (int i = 0; i < MAX_ARENAS; i++) e->ar[i].release();
   PinBuf *pb[] = {&e->h_qt, &e->h_tc, &e->h_fixed, &e->h_status, &e->h_out_pos, &e->h_scan_size, &e->h_tabs, &e->h_stage, &e->h_best_al, &e->h_qinit, &e->h_qimg, &e->h_qset};
@@ -1542,6 +1659,12 @@ int b200jpeg_encode_batch(b200jpeg_encoder *enc, const b200jpeg_params *p, const
                           size_t row_pitch, size_t image_stride, int n_images)
 {
   return encode_common(enc, p, pixels, pixels_on_device, row_pitch, image_stride, n_images, false);
+}
+int b200jpeg_encode_yuv_batch(b200jpeg_encoder *enc, const b200jpeg_params *p, const void *pixels, int pixels_on_device,
+                              size_t row_pitch, size_t image_stride, uint8_t *const *planes, int planes_on_device,
+                              const size_t *plane_pitch, const size_t *plane_stride, int n_images)
+{
+  return encode_yuv(enc, p, pixels, pixels_on_device, row_pitch, image_stride, planes, planes_on_device, plane_pitch, plane_stride, n_images);
 }
 int b200jpeg_encode_batch_device_only(b200jpeg_encoder *enc, const b200jpeg_params *p, const void *pixels_device,
                                       size_t row_pitch, size_t image_stride, int n_images)
@@ -1615,6 +1738,7 @@ unsigned long long b200jpeg_kernel_launches(const b200jpeg_encoder *e) { return 
 int b200jpeg_last_stage_times(const b200jpeg_encoder *e, const char **names, float *ms, int max)
 {
   if (!e) return 0;
+  if (e->pending_marks) collect_stage_times(const_cast<b200jpeg_encoder *>(e), e->pending_marks);
   int n = (int)e->stage_ms.size();
   for (int i = 0; i < n && i < max; i++) { if (names) names[i] = e->stage_names[i]; if (ms) ms[i] = e->stage_ms[i]; }
   return n < max ? n : max;

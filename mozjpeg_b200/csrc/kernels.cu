@@ -1093,6 +1093,126 @@ void launch_prep_planes(const Geom &g, const uint8_t *src, int smoothing_factor,
   LAUNCHED();
 }
 
+// =====================================================================
+// TurboJPEG YUV planes (tj3EncodeYUVPlanes8, turbojpeg.c:1467-1619): colour conversion + the downsamplers
+// jinit_downsampler picks without smoothing (jcsample.c:463-545), written straight into the caller's planes.
+// One CTA = one tile of YUV_TH rows x YUV_TW pixels of one image:
+//   A. the tile's input rows are read once, with 16-byte loads at 16-byte aligned addresses (byte loads at the ragged
+//      ends), into shared memory at the source's 16-byte phase; rows past the image are the last row (turbojpeg.c:
+//      1539-1540), columns past it the last column (expand_right_edge, jcsample.c:98-116);
+//   B. every pixel is converted once (convert_sample) and its luma sample stored, and each HX x VX group of pixels sums
+//      into one sample per chroma plane: h2v1_downsample (bias 0,1,..), h2v2_downsample (bias 1,2,..), int_downsample
+//      (rounded mean) for the other ratios; the output rows are staged at the destination's 16-byte phase;
+//   C. every plane row segment is written with 16-byte stores, byte stores only at its two ends, so bytes of the
+//      caller's pitch padding past pw[ci] are never touched.
+// The layout the kernel covers is every TJSAMP_*: component 0 at the maximum sampling factors (HX = hmax, VX = vmax),
+// components 1 and 2 (if any) 1x1.
+// =====================================================================
+#define YUV_TW 256
+#define YUV_TH 16
+template <int HX, int VX, int PS>
+__global__ void __launch_bounds__(256) k_encode_yuv(Geom g, const uint8_t *__restrict__ src, YuvOut out)
+{
+  constexpr int CW = YUV_TW / HX, CH = YUV_TH / VX;
+  __shared__ __align__(16) uint8_t s_in[YUV_TH][YUV_TW * PS + 16];
+  __shared__ __align__(16) uint8_t s_y[YUV_TH][YUV_TW + 16];
+  __shared__ __align__(16) uint8_t s_c[2][CH][CW + 16];
+  __shared__ int s_head[YUV_TH], s_hy[YUV_TH], s_hc[2][CH];
+  const int img = blockIdx.z, x0 = blockIdx.x * YUV_TW, y0 = blockIdx.y * YUV_TH;
+  const int ncols = min(YUV_TW, g.W - x0);              // >= 1: YUV_TW is a multiple of hmax, so no tile starts in pw0's padding
+  const int ow = min(YUV_TW, out.pw[0] - x0);           // luma columns of this tile inside the plane
+  const uint8_t *base = src + (size_t)img * g.image_stride;
+  auto plane_row = [&](int ci, int y) { return out.p[ci] + (size_t)img * out.stride[ci] + (size_t)y * out.pitch[ci] + x0 / (ci ? HX : 1); };
+  if (threadIdx.x < YUV_TH) {
+    const int r = threadIdx.x;
+    s_head[r] = (int)((uintptr_t)(base + (size_t)min(y0 + r, g.H - 1) * g.row_pitch + (size_t)x0 * PS) & 15);
+    s_hy[r] = (int)((uintptr_t)plane_row(0, y0 + r) & 15);
+    if (r < CH && g.nc == 3) { s_hc[0][r] = (int)((uintptr_t)plane_row(1, y0 / VX + r) & 15); s_hc[1][r] = (int)((uintptr_t)plane_row(2, y0 / VX + r) & 15); }
+  }
+  __syncthreads();
+  // A. load
+  {
+    const int nbytes = ncols * PS, words = (YUV_TW * PS + 16) / 16;
+    for (int i = threadIdx.x; i < YUV_TH * words; i += blockDim.x) {
+      const int r = i / words, w = i - r * words, head = s_head[r];
+      const int b0 = 16 * w - head;                      // first byte of the word, relative to the row's first byte
+      if (b0 >= nbytes) continue;
+      const uint8_t *row = base + (size_t)min(y0 + r, g.H - 1) * g.row_pitch + (size_t)x0 * PS;
+      if (b0 >= 0 && b0 + 16 <= nbytes) {
+        *reinterpret_cast<uint4 *>(&s_in[r][16 * w]) = __ldg(reinterpret_cast<const uint4 *>(row + b0));
+      } else {
+        for (int b = max(b0, 0); b < min(b0 + 16, nbytes); b++) s_in[r][head + b] = __ldg(row + b);
+      }
+    }
+  }
+  __syncthreads();
+  // B. convert + downsample
+  for (int i = threadIdx.x; i < CH * CW; i += blockDim.x) {
+    const int gr = i / CW, gc = i - gr * CW;
+    int sum1 = 0, sum2 = 0;
+#pragma unroll
+    for (int dv = 0; dv < VX; dv++) {
+      const int r = gr * VX + dv;
+#pragma unroll
+      for (int du = 0; du < HX; du++) {
+        const int x = gc * HX + du;
+        const uint8_t *px = &s_in[r][s_head[r] + min(x, ncols - 1) * PS];
+        s_y[r][s_hy[r] + x] = (uint8_t)convert_sample<1>(px, g.cs_mode, 0, g.px_first, g.px_swap);
+        if (g.nc == 3) { sum1 += convert_sample<1>(px, g.cs_mode, 1, g.px_first, g.px_swap); sum2 += convert_sample<1>(px, g.cs_mode, 2, g.px_first, g.px_swap); }
+      }
+    }
+    if (g.nc == 3) {
+      int v1, v2;
+      if (HX == 1 && VX == 1) { v1 = sum1; v2 = sum2; }
+      else if (HX == 2 && VX == 1) { const int bias = gc & 1; v1 = (sum1 + bias) >> 1; v2 = (sum2 + bias) >> 1; }          // x0 is even
+      else if (HX == 2 && VX == 2) { const int bias = 1 + (gc & 1); v1 = (sum1 + bias) >> 2; v2 = (sum2 + bias) >> 2; }
+      else { constexpr int NP = HX * VX; v1 = (sum1 + NP / 2) / NP; v2 = (sum2 + NP / 2) / NP; }
+      s_c[0][gr][s_hc[0][gr] + gc] = (uint8_t)v1; s_c[1][gr][s_hc[1][gr] + gc] = (uint8_t)v2;
+    }
+  }
+  __syncthreads();
+  // C. store: plane 0 (YUV_TH rows of ow samples), then planes 1, 2 (CH rows of ow / HX samples)
+  const int nplanes = g.nc == 3 ? 3 : 1;
+  for (int ci = 0; ci < nplanes; ci++) {
+    const int rows = ci ? CH : YUV_TH, cols = ci ? ow / HX : ow, ry0 = ci ? y0 / VX : y0;
+    const int words = ((ci ? CW : YUV_TW) + 16) / 16;
+    for (int i = threadIdx.x; i < rows * words; i += blockDim.x) {
+      const int r = i / words, w = i - r * words;
+      if (ry0 + r >= out.ph[ci]) continue;
+      const int head = ci ? s_hc[ci - 1][r] : s_hy[r];
+      const uint8_t *srow = ci ? &s_c[ci - 1][r][0] : &s_y[r][0];
+      const int b0 = 16 * w - head;
+      if (b0 >= cols) continue;
+      uint8_t *drow = plane_row(ci, ry0 + r);
+      if (b0 >= 0 && b0 + 16 <= cols) *reinterpret_cast<uint4 *>(drow + b0) = *reinterpret_cast<const uint4 *>(srow + 16 * w);
+      else for (int b = max(b0, 0); b < min(b0 + 16, cols); b++) drow[b] = srow[head + b];
+    }
+  }
+}
+template <int HX, int VX>
+static void launch_encode_yuv_hv(const Geom &g, const uint8_t *src, const YuvOut &out, dim3 grid, cudaStream_t s)
+{
+  if (g.in_comps == 1) k_encode_yuv<HX, VX, 1><<<grid, 256, 0, s>>>(g, src, out);
+  else if (g.in_comps == 3) k_encode_yuv<HX, VX, 3><<<grid, 256, 0, s>>>(g, src, out);
+  else k_encode_yuv<HX, VX, 4><<<grid, 256, 0, s>>>(g, src, out);
+}
+void launch_encode_yuv(const Geom &g, const uint8_t *src, const YuvOut &out, int n, cudaStream_t s)
+{
+  const dim3 grid((out.pw[0] + YUV_TW - 1) / YUV_TW, (out.ph[0] + YUV_TH - 1) / YUV_TH, n);
+  switch (g.hmax * 8 + g.vmax) {
+  case 9:  launch_encode_yuv_hv<1, 1>(g, src, out, grid, s); break;
+  case 10: launch_encode_yuv_hv<1, 2>(g, src, out, grid, s); break;
+  case 12: launch_encode_yuv_hv<1, 4>(g, src, out, grid, s); break;
+  case 17: launch_encode_yuv_hv<2, 1>(g, src, out, grid, s); break;
+  case 18: launch_encode_yuv_hv<2, 2>(g, src, out, grid, s); break;
+  case 20: launch_encode_yuv_hv<2, 4>(g, src, out, grid, s); break;
+  case 33: launch_encode_yuv_hv<4, 1>(g, src, out, grid, s); break;
+  case 34: launch_encode_yuv_hv<4, 2>(g, src, out, grid, s); break;
+  default: launch_encode_yuv_hv<4, 4>(g, src, out, grid, s); break;
+  }
+  LAUNCHED();
+}
+
 // fast path: full-size first component, (for colour) two 1x1-sampled chroma components
 static bool forward_gray(const Geom &g) { return g.nc == 1 && (g.raw_in || g.cs_mode == 1 || (g.cs_mode == 2 && g.in_comps == 1)); }
 bool forward_tiled(const Geom &g, int dct_method)

@@ -145,6 +145,11 @@ struct SymOut { uint8_t *sym; int16_t *dcq; uint32_t *hist; int keep_coef; int d
 // qt / tc (here and in the trellis launches): the batch's table sets, image img reads set g.qset[img] (qset_of);
 // qfast / dc_fast: every set the launch's images use allows the fast form
 void launch_prep_planes(const Geom &g, const uint8_t *src, int smoothing_factor, const PlanesOut &out, int n, cudaStream_t s);
+// TurboJPEG YUV planes (k_encode_yuv): plane ci of image img starts at p[ci] + img * stride[ci] and holds ph[ci] rows of
+// pw[ci] samples pitch[ci] bytes apart (b200jpeg_yuv_plane_dims); g.hmax, g.vmax in {1, 2, 4}, component 0 at them and
+// components 1, 2 (g.nc == 3) 1x1; 8-bit samples
+struct YuvOut { uint8_t *p[3]; size_t pitch[3], stride[3]; int pw[3], ph[3]; };
+void launch_encode_yuv(const Geom &g, const uint8_t *src, const YuvOut &out, int n, cudaStream_t s);
 void launch_import_coefs(const Geom &g, int n, cudaStream_t s);     // raw_in == 2: planes hold JBLOCK rows
 // Trellis-phase statistics counted by the tiled forward kernel (fs.hist != nullptr, only where forward_tiled() holds):
 // every real block's AC symbols go into hist [img*nc + ci][4 + ac_tbl][sym] (zeroed by the caller), its plain-quantized

@@ -538,4 +538,22 @@ int b200jpeg_total_passes(const b200jpeg_params *p) {
   return total;
 }
 
+// tj3EncodeYUVPlanes8's plane geometry (turbojpeg.c:1528-1578); tj3YUVPlaneWidth / tj3YUVPlaneHeight give the same for
+// the TJSAMP_* factors
+int b200jpeg_yuv_plane_dims(const b200jpeg_params *p, int ci, int *width, int *height) {
+  if (!p || p->image_width <= 0 || p->image_height <= 0 || p->num_components <= 0 || p->num_components > B200JPEG_MAX_COMPONENTS || ci < 0 || ci >= p->num_components) {
+    b200::set_error("bad argument"); return B200JPEG_ERR_PARAM;
+  }
+  int hmax = 1, vmax = 1;
+  for (int c = 0; c < p->num_components; c++) {
+    const b200jpeg_component_info &k = p->comp_info[c];
+    if (k.h_samp_factor <= 0 || k.h_samp_factor > 4 || k.v_samp_factor <= 0 || k.v_samp_factor > 4) { b200::set_error("Bogus sampling factors"); return B200JPEG_ERR_PARAM; }
+    hmax = std::max(hmax, k.h_samp_factor); vmax = std::max(vmax, k.v_samp_factor);
+  }
+  const long pw0 = (p->image_width + hmax - 1) / hmax * (long)hmax, ph0 = (p->image_height + vmax - 1) / vmax * (long)vmax;
+  if (width) *width = (int)(pw0 * p->comp_info[ci].h_samp_factor / hmax);
+  if (height) *height = (int)(ph0 * p->comp_info[ci].v_samp_factor / vmax);
+  return B200JPEG_OK;
+}
+
 }  // extern "C"

@@ -15,6 +15,70 @@ from mozjpeg_b200.synth import synth_image12
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
 import colorspace_cases as CC       # CMYK / YCCK / YCbCr->gray / JCS_UNKNOWN conversions and their restatement
 
+
+def fuzz_yuv(seed, cases, budget):
+    """fuzz_gpu.py --yuv [seed] [cases] [seconds]: tj3EncodeYUVPlanes8 on the device against the reference library
+    (oracle/_ref/libturbojpeg_ref.so) for random shapes, subsamplings, pixel formats, source pitches, plane pitches and
+    small batches, every plane byte for byte and every pitch / gap byte untouched."""
+    import yuv_cases as Y
+    rng = random.Random(seed)
+    ref = Y.RefTJ()
+    bad = tot = refused = 0
+    t0 = time.time()
+    for it in range(cases):
+        if time.time() - t0 > budget:
+            break
+        w = rng.choice([1, 2, 3, 5, 7, 8, 15, 16, 17, 31, 33, 63, 100, 255, 256, 257, 300, 513, 1023])
+        h = rng.choice([1, 2, 3, 4, 5, 7, 8, 15, 16, 17, 33, 64, 99, 200])
+        ss, pf = rng.choice(Y.SUBSAMPS), rng.choice([f for f in Y.PIXEL_FORMATS if f != "CMYK"])
+        if pf == "GRAY" and ss != "gray":
+            refused += 1; continue
+        n = rng.choice([1, 1, 2, 3, 5])
+        ps = Y.PIXEL_FORMATS[pf]
+        imgs = [Y.to_pixel_format(Y.synth_rgb(rng.randrange(1 << 20), w, h), pf, rng.randrange(1 << 20)) for _ in range(n)]
+        row_pitch = w * ps + rng.choice([0, 0, 1, 3, 16])
+        image_stride = row_pitch * h + rng.choice([0, 5, 64])
+        src = np.zeros(image_stride * n + 16, np.uint8)
+        off = rng.choice([0, 0, 1, 7])                    # unaligned first pixel
+        for i, im in enumerate(imgs):
+            for y in range(h):
+                a = off + i * image_stride + y * row_pitch
+                src[a: a + w * ps] = im[y].reshape(-1)
+        cs = A.CS_GRAYSCALE if ss == "gray" else A.CS_YCbCr
+        p = mj.tj3_params(w, h, subsamp=ss, pixel_format=pf, colorspace=cs)
+        geo = [mj.yuv_plane_dims(p, ci) for ci in range(p.num_components)]
+        pitch = [pw + rng.choice([0, 0, 1, 13, 64]) for pw, _ in geo]
+        stride = [pt * ph + rng.choice([0, 3, 100]) for pt, (_, ph) in zip(pitch, geo)]
+        pofs = [rng.choice([0, 0, 1, 5]) for _ in geo]
+        outs = [np.full(st * n + 8, 0xEE, np.uint8) for st in stride]
+        try:
+            enc.encode_yuv_batch_ptr(p, src.ctypes.data + off, False, row_pitch, image_stride, [o.ctypes.data + po for o, po in zip(outs, pofs)],
+                                     False, pitch, stride, n)
+        except Exception as ex:
+            bad += 1; print("YUV DEVICE FAIL", (w, h, n), ss, pf, ex); continue
+        tot += 1
+        for i, im in enumerate(imgs):
+            want, err = ref.encode_planes(im, pf, ss)
+            ok = err is None
+            for ci, ((pw, ph), pt, st, po, o) in enumerate(zip(geo, pitch, stride, pofs, outs)):
+                blk = o[po + i * st: po + i * st + pt * ph].reshape(ph, pt)
+                ok = ok and np.array_equal(blk[:, :pw], want[ci]) and (blk[:, pw:] == 0xEE).all()
+                ok = ok and (o[po + i * st + pt * ph: po + (i + 1) * st] == 0xEE).all() and (o[:po] == 0xEE).all()
+            if not ok:
+                bad += 1; print("YUV MISMATCH", (w, h, n), ss, pf, "image", i, (row_pitch, image_stride, off, pitch, stride, pofs)); break
+    ref.close()
+    print("yuv seed", seed, "bad", bad, "compared", tot, "refused", refused, "seconds %.0f" % (time.time() - t0))
+    return bad
+
+
+if "--yuv" in sys.argv:
+    sys.argv.remove("--yuv")
+    enc = mj.Encoder(0)
+    nbad = fuzz_yuv(int(sys.argv[1]) if len(sys.argv) > 1 else 1, int(sys.argv[2]) if len(sys.argv) > 2 else 2000,
+                    float(sys.argv[3]) if len(sys.argv) > 3 else 300.0)
+    enc.close()
+    sys.exit(1 if nbad else 0)
+
 seed = int(sys.argv[1]) if len(sys.argv) > 1 else 1
 cases = int(sys.argv[2]) if len(sys.argv) > 2 else 300
 budget = float(sys.argv[3]) if len(sys.argv) > 3 else 120.0

@@ -308,7 +308,36 @@ def lossless():
     print("wrote", len(cases), "lossless cases;", checked, "checked against the cjpeg binary")
 
 
+def yuv():
+    """tests/golden/yuv_golden.json: the reference's tj3EncodeYUVPlanes8 (oracle/_ref/libturbojpeg_ref.so through ctypes)
+    on every subsampling x pixel format x size x plane stride of tests/yuv_cases.py: the md5 of every plane's pw x ph
+    samples, or the reference's refusal."""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import yuv_cases as Y
+    ref = Y.RefTJ()
+    cases = []
+    for size in Y.SIZES:
+        for pf in Y.PIXEL_FORMATS:
+            pix = Y.case_pixels(size, pf)
+            for ss in Y.SUBSAMPS:
+                for pad in Y.PADS:
+                    planes, err = ref.encode_planes(pix, pf, ss, pad)
+                    c = {"size": Y.size_id(size), "pf": pf, "subsamp": ss, "pad": pad}
+                    if err is not None:
+                        c["error"] = err
+                    else:
+                        c["dims"] = [list(p.shape[::-1]) for p in planes]
+                        c["md5"] = [Y.md5(p) for p in planes]
+                    cases.append(c)
+    ref.close()
+    json.dump({"generator": "tools/make_golden.py --yuv", "reference": "mozilla/mozjpeg 5.0.0 (C path, WITH_SIMD=0), oracle/_ref",
+               "cases": cases}, open(os.path.join(GOLD, "yuv_golden.json"), "w"), indent=0)
+    print("wrote", len(cases), "YUV cases;", sum("error" in c for c in cases), "refusals")
+
+
 def main():
+    if "--yuv" in sys.argv:
+        return yuv()
     if "--lossless" in sys.argv:
         return lossless()
     if "--perimage-q" in sys.argv:
