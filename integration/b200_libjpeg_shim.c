@@ -6,7 +6,8 @@
  * it takes over the calls that bracket the encode hot path,
  *
  *     jpeg_start_compress      (jcapistd.c:44-70)
- *     jpeg_write_scanlines     (jcapistd.c:90-135; jpeg12_write_scanlines for 12-bit samples)
+ *     jpeg_write_scanlines     (jcapistd.c:90-135; jpeg12_write_scanlines for 12-bit samples; 16-bit samples reach the
+ *                               device through the reference's own jpeg16_write_scanlines, see device_process_data_16)
  *     jpeg_write_raw_data      (jcapistd.c:145-195; under tj3CompressFromYUV*)
  *     jpeg_write_coefficients  (jctrans.c:39-66; the encode half of jpegtran)
  *     jpeg_finish_compress     (jcapimin.c:176-229)
@@ -20,7 +21,7 @@
  * binary, in tests/test_libjpeg_shim.py) produces its files on the GPU.
  *
  * Parameter sets the device path does not cover (B200JPEG_ERR_UNSUPPORTED from
- * b200jpeg_start_compress: arithmetic coding, lossless, the optional trellis modes, abbreviated
+ * b200jpeg_start_compress: arithmetic coding, the optional trellis modes, abbreviated
  * datastreams, ...) and hosts without a CUDA device fall through to the reference's
  * implementation of the same three functions (dlsym RTLD_NEXT): that is the
  * REFERENCE running, not a CPU path of this library.  B200_SHIM_VERBOSE=1
@@ -54,6 +55,7 @@ static struct {
   unsigned char *extra; size_t extra_len, extra_cap;         /* jpeg_write_marker segments, in call order */
   size_t header_len;                                         /* SOI + JFIF APP0 + Adobe APP14 (write_file_header, jcmarker.c:649-663) */
   int total_passes;                                          /* what jinit_c_master_control would have counted (jcmaster.c:1114-1139) */
+  int lossless;                                              /* a lossless (SOF3) object */
 } g_active[MAX_ACTIVE];
 static b200jpeg_encoder *g_idle_enc;          /* encoders are reused: creating one costs a CUDA context */
 static int g_no_device;
@@ -149,14 +151,18 @@ static int claim_slot(j_compress_ptr cinfo, const char **why)
   return slot;
 }
 
-/* width_in_blocks / height_in_blocks as initial_setup computes them (jcmaster.c:215-236); the reference's master
+/* the data unit initial_setup sizes components in: a block, or one sample in lossless mode (jcmaster.c:171) */
+static int data_unit(j_compress_ptr cinfo) { return cinfo->master->lossless ? 1 : DCTSIZE; }
+
+/* width_in_blocks / height_in_blocks as initial_setup computes them (jcmaster.c:215-242); the reference's master
  * control is not run on objects that take the device path, so they are derived here */
 static void comp_blocks(j_compress_ptr cinfo, int ci, JDIMENSION *wib, JDIMENSION *hib)
 {
   int hmax = 1, vmax = 1;
+  const int du = data_unit(cinfo);
   for (int k = 0; k < cinfo->num_components; k++) { if (cinfo->comp_info[k].h_samp_factor > hmax) hmax = cinfo->comp_info[k].h_samp_factor; if (cinfo->comp_info[k].v_samp_factor > vmax) vmax = cinfo->comp_info[k].v_samp_factor; }
-  *wib = (JDIMENSION)(((long)cinfo->image_width * cinfo->comp_info[ci].h_samp_factor + hmax * DCTSIZE - 1) / (hmax * DCTSIZE));
-  *hib = (JDIMENSION)(((long)cinfo->image_height * cinfo->comp_info[ci].v_samp_factor + vmax * DCTSIZE - 1) / (vmax * DCTSIZE));
+  *wib = (JDIMENSION)(((long)cinfo->image_width * cinfo->comp_info[ci].h_samp_factor + hmax * du - 1) / (hmax * du));
+  *hib = (JDIMENSION)(((long)cinfo->image_height * cinfo->comp_info[ci].v_samp_factor + vmax * du - 1) / (vmax * du));
 }
 
 /* The derived fields initial_setup (jcmaster.c:209-257) leaves in the object: applications read them after
@@ -172,13 +178,32 @@ static void derive_geometry(j_compress_ptr cinfo)
   for (int ci = 0; ci < cinfo->num_components; ci++) {
     jpeg_component_info *c = &cinfo->comp_info[ci];
     c->component_index = ci;
-    c->DCT_scaled_size = DCTSIZE;
+    c->DCT_scaled_size = data_unit(cinfo);
     comp_blocks(cinfo, ci, &c->width_in_blocks, &c->height_in_blocks);
     c->downsampled_width = (JDIMENSION)(((long)cinfo->image_width * c->h_samp_factor + cinfo->max_h_samp_factor - 1) / cinfo->max_h_samp_factor);
     c->downsampled_height = (JDIMENSION)(((long)cinfo->image_height * c->v_samp_factor + cinfo->max_v_samp_factor - 1) / cinfo->max_v_samp_factor);
     c->component_needed = TRUE;
   }
-  cinfo->total_iMCU_rows = (JDIMENSION)(((long)cinfo->image_height + cinfo->max_v_samp_factor * DCTSIZE - 1) / (cinfo->max_v_samp_factor * DCTSIZE));
+  const long rows = (long)cinfo->max_v_samp_factor * data_unit(cinfo);
+  cinfo->total_iMCU_rows = (JDIMENSION)(((long)cinfo->image_height + rows - 1) / rows);
+}
+
+/* jinit_c_master_control's lossless decisions (jcmaster.c:1055-1094), made on the object before its parameters are
+ * read.  A script decides lossless mode by its first entry (validate_script, jcmaster.c:301-329), except the scan
+ * search's script, which is not validated; without a script jpeg_enable_lossless has decided it.  Lossless mode then
+ * overrides smoothing, the colour space, subsampling and raw-data input, and forces optimal Huffman tables.  The
+ * reference makes the same changes when it runs instead, so an object it gets back is already in the state it would
+ * put it in. */
+static void lossless_overrides(j_compress_ptr cinfo)
+{
+  if (cinfo->scan_info != NULL && cinfo->num_scans > 0 && !cinfo->master->optimize_scans)
+    cinfo->master->lossless = cinfo->scan_info[0].Ss != 0 && cinfo->scan_info[0].Se == 0;
+  if (!cinfo->master->lossless) return;
+  cinfo->raw_data_in = FALSE;
+  cinfo->smoothing_factor = 0;
+  jpeg_default_colorspace(cinfo);
+  for (int ci = 0; ci < cinfo->num_components; ci++) cinfo->comp_info[ci].h_samp_factor = cinfo->comp_info[ci].v_samp_factor = 1;
+  if (!cinfo->arith_code) cinfo->optimize_coding = TRUE;
 }
 
 /* the encoder-relevant state of the reference's object -> b200jpeg_params.  Returns 0 if the
@@ -188,8 +213,10 @@ static int fill_params(j_compress_ptr cinfo, boolean write_all_tables, b200jpeg_
   int i, ci;
   memset(p, 0, sizeof(*p));
   if (!write_all_tables) return 0;                       /* abbreviated datastreams: reference only */
-  if ((cinfo->data_precision != 8 && cinfo->data_precision != 12) || cinfo->arith_code || cinfo->master->lossless) return 0;
+  const int lossless = cinfo->master->lossless;
+  if ((cinfo->data_precision != 8 && cinfo->data_precision != 12 && !(lossless && cinfo->data_precision == 16)) || cinfo->arith_code) return 0;
   if (cinfo->data_precision == 12 && cinfo->raw_data_in) return 0;   /* jpeg12_write_raw_data: reference only */
+  if (lossless && cinfo->scan_info != NULL && cinfo->num_scans <= 0) return 0;   /* the reference refuses the empty script */
   if (cinfo->num_components > B200JPEG_MAX_COMPONENTS || cinfo->num_scans > B200JPEG_MAX_SCANS) return 0;
   switch (cinfo->in_color_space) {
   case JCS_GRAYSCALE: p->in_color_space = B200JPEG_CS_GRAYSCALE; break;
@@ -260,6 +287,30 @@ static int fill_params(j_compress_ptr cinfo, boolean write_all_tables, b200jpeg_
   return 1;
 }
 
+/* jpeg_enable_lossless keeps its predictor and point transform in cinfo->Ss / Al and leaves scan_info alone: the block
+ * gets the same call.  Beside the scan search's script the C-ABI refuses it (the reference writes SOF2 headers there).
+ * A script that is itself lossless is in the block already. */
+static const char *finish_lossless_params(j_compress_ptr cinfo, b200jpeg_params *p)
+{
+  if (!cinfo->master->lossless || (cinfo->scan_info != NULL && !cinfo->master->optimize_scans)) return NULL;
+  return b200jpeg_enable_lossless(p, cinfo->Ss, cinfo->Al) == B200JPEG_OK ? NULL : b200jpeg_last_error();
+}
+
+/* 16-bit samples (J16SAMPLE = unsigned short, lossless mode only).  jpeg16_write_scanlines is not taken over: the
+ * reference's own (jcapistd.c:90-135 compiled with BITS_IN_JSAMPLE 16) checks precision and state, calls the progress
+ * monitor, drops rows past the bottom of the image and hands the rest to the main controller's process_data_16
+ * (jcapistd.c:126-129).  jpeg_start_compress installs this function there for 16-bit device-path objects, so the rows
+ * go to b200jpeg_write_scanlines as uint16 rows; the reference advances next_scanline by what it reports. */
+static void device_process_data_16(j_compress_ptr cinfo, J16SAMPARRAY rows, JDIMENSION *row_ctr, JDIMENSION rows_avail)
+{
+  int slot = find_active(cinfo);
+  if (slot < 0) ERREXIT1(cinfo, JERR_BAD_STATE, cinfo->global_state);
+  if (rows_avail == 0) return;
+  int took = b200jpeg_write_scanlines(g_active[slot].enc, (const uint8_t *const *)rows, (int)rows_avail);
+  if (took < 0) ERREXIT1(cinfo, JERR_BAD_STATE, cinfo->global_state);
+  *row_ctr += (JDIMENSION)took;
+}
+
 GLOBAL(void)
 jpeg_start_compress(j_compress_ptr cinfo, boolean write_all_tables)
 {
@@ -273,7 +324,9 @@ jpeg_start_compress(j_compress_ptr cinfo, boolean write_all_tables)
   /* jcapistd.c:53-56 */
   if (cinfo->master->num_scans_luma == 0 || cinfo->scan_info == NULL || cinfo->num_scans == 0)
     cinfo->master->optimize_scans = FALSE;
+  if (!why) lossless_overrides(cinfo);
   if (!why && !fill_params(cinfo, write_all_tables, &p)) why = "parameter set outside b200jpeg_params";
+  if (!why) why = finish_lossless_params(cinfo, &p);
   if (!why && b200jpeg_validate(&p) != B200JPEG_OK) why = b200jpeg_last_error();
   if (!why) slot = claim_slot(cinfo, &why);
   if (!why && !cinfo->raw_data_in) {
@@ -286,9 +339,11 @@ jpeg_start_compress(j_compress_ptr cinfo, boolean write_all_tables)
     real(cinfo, write_all_tables);
     return;
   }
-  if (verbose()) fprintf(stderr, "b200 shim: device path (%s%ux%u, %d scans)\n", cinfo->raw_data_in ? "raw data, " : "", cinfo->image_width, cinfo->image_height, p.num_scans);
+  if (verbose()) fprintf(stderr, "b200 shim: device path (%s%ux%u, %d scans)\n", cinfo->raw_data_in ? "raw data, " : cinfo->master->lossless ? "lossless, " : "",
+                         cinfo->image_width, cinfo->image_height, p.num_scans);
   g_active[slot].header_len = 2 + (p.write_JFIF_header ? 18 : 0) + (p.write_Adobe_marker ? 16 : 0);
   g_active[slot].total_passes = b200jpeg_total_passes(&p);
+  g_active[slot].lossless = cinfo->master->lossless;
   if (cinfo->progress != NULL) { cinfo->progress->completed_passes = 0; cinfo->progress->total_passes = g_active[slot].total_passes; }   /* prepare_for_pass, jcmaster.c:711-714 */
   if (cinfo->raw_data_in) {
     g_active[slot].raw = 1; g_active[slot].params = p;
@@ -298,6 +353,15 @@ jpeg_start_compress(j_compress_ptr cinfo, boolean write_all_tables)
       g_active[slot].plane[ci] = (uint8_t *)calloc(g_active[slot].plane_pitch[ci], g_active[slot].plane_rows[ci]);
       if (!g_active[slot].plane[ci]) { release_slot(slot); ERREXIT1(cinfo, JERR_OUT_OF_MEMORY, 0); }
     }
+  }
+  if (cinfo->data_precision == 16) {
+    /* the main controller jinit_c_main_controller would have made, reduced to what jpeg16_write_scanlines calls; in the
+     * image pool like the reference's, so jpeg_abort frees it */
+    struct jpeg_c_main_controller *m = (struct jpeg_c_main_controller *)(*cinfo->mem->alloc_small) ((j_common_ptr)cinfo, JPOOL_IMAGE, sizeof *m);
+    memset(m, 0, sizeof *m);
+    m->process_data_16 = device_process_data_16;
+    cinfo->main = m;
+    cinfo->master->call_pass_startup = FALSE;                       /* the headers are the device's (jcapistd.c:117-118) */
   }
   derive_geometry(cinfo);
   jpeg_suppress_tables(cinfo, FALSE);                               /* jcapistd.c:50-51 (write_all_tables is TRUE here) */
@@ -435,13 +499,18 @@ jpeg_finish_compress(j_compress_ptr cinfo)
   }
   /* the remaining passes ran inside the one device call; the application's monitor hears about each of them, on this
    * thread, with the counters the reference's loop would show at the end of the pass (jcapimin.c:193-215,
-   * jcmaster.c:711-714) */
+   * jcmaster.c:711-714).  Lossless objects hear every row of the reference's loop, as they did when the reference
+   * encoded them. */
   if (cinfo->progress != NULL) {
     const int tp = g_active[slot].total_passes;
+    const long rows = (long)cinfo->total_iMCU_rows;
+    const long first = g_active[slot].lossless ? 0 : rows, last = g_active[slot].lossless ? rows - 1 : rows;
     for (int pass = from_coefs ? 0 : 1; pass < tp; pass++) {
-      cinfo->progress->completed_passes = pass; cinfo->progress->total_passes = tp;
-      cinfo->progress->pass_counter = (long)cinfo->total_iMCU_rows; cinfo->progress->pass_limit = (long)cinfo->total_iMCU_rows;
-      (*cinfo->progress->progress_monitor) ((j_common_ptr)cinfo);
+      for (long r = first; r <= last; r++) {
+        cinfo->progress->completed_passes = pass; cinfo->progress->total_passes = tp;
+        cinfo->progress->pass_counter = r; cinfo->progress->pass_limit = rows;
+        (*cinfo->progress->progress_monitor) ((j_common_ptr)cinfo);
+      }
     }
   }
   if (!from_coefs) (*cinfo->dest->init_destination) (cinfo);         /* jpeg_write_coefficients did it already (jctrans.c:57) */
