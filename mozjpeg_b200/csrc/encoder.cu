@@ -735,6 +735,8 @@ static int run_pipeline(b200jpeg_encoder *e, const ChunkIO &io, Timer &tm)
       }
     }
     if (!generic_rounds) {
+      tm.mark("trellis_sort");
+      launch_trellis_sort(gr, A.d_rec.as<DcRec>(), rlr, A.d_srec.p, A.d_splits.as<uint32_t>(), n, s);
       tm.mark("trellis_ac");
       if (so.hist) CU(cudaMemsetAsync(A.d_hist.p, 0, hist_bytes, s));
       launch_trellis_ac3(gr, e->d_tc.as<TrellisConsts>(), tset, tabset, A.d_rec.as<DcRec>(), rlr, A.d_srec.p, A.d_splits.as<uint32_t>(), so, n, e->sms, s);
@@ -747,8 +749,11 @@ static int run_pipeline(b200jpeg_encoder *e, const ChunkIO &io, Timer &tm)
     }
     if (p->trellis_quant_dc) {
       tm.mark("trellis_dc");
-      if (pl.progressive) launch_trellis_dc(gr, e->d_tc.as<TrellisConsts>(), e->d_tabs_fixed.as<DevHuff>(), 0, A.d_rec.as<DcRec>(), A.d_bt.as<unsigned long long>(), rlr, p->trellis_delta_dc_weight > 0.0f, dc_fast_of(gr), nullptr, 1, n, s);
-      else launch_trellis_dc(gr, e->d_tc.as<TrellisConsts>(), tset, tabset, A.d_rec.as<DcRec>(), A.d_bt.as<unsigned long long>(), rlr, p->trellis_delta_dc_weight > 0.0f, dc_fast_of(gr), so.dcq, so.keep_coef, n, s);
+      // behind k_trellis_ac3 the records still hold the norm; the band kernel stores lambda_dc (from re-fitted tables
+      // with trellis_q_opt)
+      const int lambda_from_norm = generic_rounds ? 0 : 1;
+      if (pl.progressive) launch_trellis_dc(gr, e->d_tc.as<TrellisConsts>(), e->d_tabs_fixed.as<DevHuff>(), 0, A.d_rec.as<DcRec>(), A.d_bt.as<unsigned long long>(), rlr, p->trellis_delta_dc_weight > 0.0f, dc_fast_of(gr), nullptr, 1, lambda_from_norm, n, s);
+      else launch_trellis_dc(gr, e->d_tc.as<TrellisConsts>(), tset, tabset, A.d_rec.as<DcRec>(), A.d_bt.as<unsigned long long>(), rlr, p->trellis_delta_dc_weight > 0.0f, dc_fast_of(gr), so.dcq, so.keep_coef, lambda_from_norm, n, s);
     }
     return B200JPEG_OK;
     };

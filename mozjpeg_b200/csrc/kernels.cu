@@ -2255,11 +2255,14 @@ __device__ __forceinline__ float u2f_exact(unsigned v) { return __uint_as_float(
 #define SYMREC_DIRECT 0
 #endif
 static_assert(!(SYMREC_DIRECT && SYMREC_SPLIT), "the direct-store A/B aid writes whole 128-byte slots");
+// resident CTAs per SM the compiler must allow for the <= 8 entries class, and for the 9..15 entries class.  H100, cfg2:
+// 6 (80 registers, no spills) ran the AC stage in 9.84-9.87 ms against 10.06-10.13 at 8 (64 registers, 18 / 20 bytes of
+// spill stores / loads); an earlier GPU measured 12 slower than 8
 #ifndef T3_MINB_8
-#define T3_MINB_8 8            // resident CTAs per SM the compiler must allow for the <= 8 entries class (12: measured slower)
+#define T3_MINB_8 6
 #endif
 #ifndef T3_MINB_15
-#define T3_MINB_15 8           // ... and for the 9..15 entries class
+#define T3_MINB_15 6
 #endif
 #ifndef T3_PRED_UNROLL
 #define T3_PRED_UNROLL 4       // predecessor loop: iterations in flight (their shared-memory loads are independent); 1 / 2 / 4: 2.56 / 2.49 / 2.44 ms per 64 4K images
@@ -2376,11 +2379,11 @@ k_trellis_ac3(Geom g, const TrellisConsts *__restrict__ tc, const DevHuff *__res
       for (int v = 0; v < 8; v++) rv[v] = r4[v];
       if (want_dc) dc_q = (unsigned)(unsigned short)o16[0];
     }
+    // (the record keeps the norm: the DC trellis derives lambda_dc from it, dc_lambda)
     float lambda;
     {
       const float norm = (float)((double)sr.norm / 63.0);      // :1026-1035
       if (use_norm) lambda = (float)(p1 / (p2 + (double)norm)); else lambda = lambda_const;
-      if (live) rec[rbase + lin].lambda_dc = lambda * swz[0];
     }
     // phase 1: accumulated zero distortion, zigzag order, serial fp32 (:1134); entries pushed where the mask says so
     const unsigned mlo = (unsigned)sr.nzmask, mhi = (unsigned)(sr.nzmask >> 32);
@@ -2584,11 +2587,14 @@ static void launch_t3(dim3 grid, cudaStream_t s, const Geom &g, const TrellisCon
   if (sizeof(T3Smem<MM>) + 8192 > 48 * 1024) cudaFuncSetAttribute(k_trellis_ac3<MM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(T3Smem<MM>));
   k_trellis_ac3<MM><<<grid, T3_THREADS, sizeof(T3Smem<MM>), s>>>(g, tc, tabs, tabs_set_stride, rec, rl, srec, splits, so); LAUNCHED();
 }
-void launch_trellis_ac3(const Geom &g, const TrellisConsts *tc, const DevHuff *tabs, size_t tabs_set_stride,
-                        DcRec *rec, const RecLayout &rl, void *srec, uint32_t *splits, const SymOut &so, int n, int sms, cudaStream_t s)
+void launch_trellis_sort(const Geom &g, const DcRec *rec, const RecLayout &rl, void *srec, uint32_t *splits, int n, cudaStream_t s)
 {
   // splits: 4 words per (image, component), followed by the sort's scratch counters (2 x 64 words each)
   launch_sort2(g, rec, rl, static_cast<SRec *>(srec), splits, splits + (size_t)n * g.nc * 4, 15, n, s);
+}
+void launch_trellis_ac3(const Geom &g, const TrellisConsts *tc, const DevHuff *tabs, size_t tabs_set_stride,
+                        DcRec *rec, const RecLayout &rl, const void *srec, const uint32_t *splits, const SymOut &so, int n, int sms, cudaStream_t s)
+{
   long long mb = 0;
   for (int ci = 0; ci < g.nc; ci++) mb = max(mb, (long long)g.c[ci].wib * g.c[ci].hib);
   const unsigned full = (unsigned)((mb + T3_THREADS - 1) / T3_THREADS);
@@ -2630,9 +2636,23 @@ static void launch_dc_collect(const Geom &g, const RecLayout &rl, int16_t *dcq, 
 // One thread per (image, iMCU row).  bt[] holds, per block, the 9 back
 // pointers (4 bits each), the unsigned quantized value and the sign.
 // =====================================================================
+// The block's lambda_dc from its record's first word.  Behind k_trellis_ac_band that word holds lambda_dc; behind
+// k_trellis_ac3 (from_norm) it still holds the forward kernel's norm, and lambda_dc is derived here with the expression
+// of :1026-1035 the AC trellis uses, times the DC weight w0 of the image's table (ac3 does not store it: one scattered
+// 4-byte write per block into an array far larger than L2).  tc: lambda fields (the same in every table set).
+// (float)((double)f / 63.0) is the correctly rounded fp32 quotient (a double quotient of two floats rounds to float
+// without a double-rounding error, 53 >= 2*24 + 2), so one fp32 division gives the same norm for one fp64 division less.
+__device__ __forceinline__ float dc_lambda(const float f, const int from_norm, const TrellisConsts *__restrict__ tc, const float w0)
+{
+  if (!from_norm) return f;
+  const float norm = __fdiv_rn(f, 63.0f);
+  const float lambda = tc->use_norm ? (float)(tc->p1 / (tc->p2 + (double)norm)) : tc->lambda_const;
+  return lambda * w0;
+}
+
 __global__ void __launch_bounds__(64) k_trellis_dc(Geom g, const TrellisConsts *__restrict__ tc,
                                                    const DevHuff *__restrict__ tabs, size_t tabs_set_stride,
-                                                   const DcRec *__restrict__ rec, unsigned long long *__restrict__ bt, RecLayout rl)
+                                                   const DcRec *__restrict__ rec, unsigned long long *__restrict__ bt, RecLayout rl, int lambda_from_norm)
 {
   const int ci = blockIdx.y % g.nc, img = blockIdx.y / g.nc;
   const CompGeom &c = g.c[ci];
@@ -2646,6 +2666,7 @@ __global__ void __launch_bounds__(64) k_trellis_dc(Geom g, const TrellisConsts *
   int n_imcu = (c.hib + c.v - 1) / c.v;
   if (imcu >= n_imcu) return;
   const int q = qset_of(tc, g, img)->q8_zz[c.qt][0];            // the image's table set (the other fields are the batch's)
+  const float w0 = qset_of(tc, g, img)->w_zz[c.qt][0];
   int ncand = (2 + 60 / (q >> 3)) | 1; if (ncand > 9) ncand = 9;     // get_num_dc_trellis_candidates (:929-933)
   const int half = ncand / 2;
   const int lim = 1 << tc->max_coef_bits;
@@ -2661,6 +2682,7 @@ __global__ void __launch_bounds__(64) k_trellis_dc(Geom g, const TrellisConsts *
       DcRec r = rec[rbase + bi];
       int raw = r.raw_dc, sign = raw >> 31, x = abs(raw);
       int qval = (x + q / 2) / q;
+      const float lambda_dc = dc_lambda(r.lambda_dc, lambda_from_norm, tc, w0);
       // trellis_delta_dc_weight: the block above inside the same iMCU row (lastblockrow, jccoefct.c:420) - its raw DC and
       // the value this thread's back-track of the previous block row left in the coefficient plane
       const bool vert = br > 0 && tc->delta_dc_weight > 0.0f;
@@ -2676,12 +2698,12 @@ __global__ void __launch_bounds__(64) k_trellis_dc(Geom g, const TrellisConsts *
           if (cd >= lim) cd = lim - 1;
           if (cd <= -lim) cd = -lim + 1;
           int delta = cd * q - x;
-          float dist = (float)(delta * delta) * r.lambda_dc;
+          float dist = (float)(delta * delta) * lambda_dc;
           cd *= 1 + 2 * sign;
           cand[k] = cd;
           if (vert) {                                               // difference of vertical gradients (:1069-1086)
             const int d2 = (above_raw - raw) - (above_fin * q - cd * q);
-            const float vd = (float)(d2 * d2) * r.lambda_dc;
+            const float vd = (float)(d2 * d2) * lambda_dc;
             dist += tc->delta_dc_weight * (vd - dist);
           }
           if (bi == 0) {
@@ -2733,7 +2755,7 @@ __global__ void __launch_bounds__(64) k_trellis_dc(Geom g, const TrellisConsts *
 // ---------------------------------------------------------------------
 __global__ void __launch_bounds__(64) k_trellis_dc_warp(Geom g, const TrellisConsts *__restrict__ tc,
                                                         const DevHuff *__restrict__ tabs, size_t tabs_set_stride,
-                                                        const DcRec *__restrict__ rec, RecLayout rl, int max_wib)
+                                                        const DcRec *__restrict__ rec, RecLayout rl, int max_wib, int lambda_from_norm)
 {
   extern __shared__ unsigned char dsm[];
   const int ci = blockIdx.y % g.nc, img = blockIdx.y / g.nc;
@@ -2755,6 +2777,7 @@ __global__ void __launch_bounds__(64) k_trellis_dc_warp(Geom g, const TrellisCon
   uint8_t *bt8 = dsm + (size_t)chains_per_cta * max_wib * 2 + (size_t)chain_in_cta * max_wib * 9;
   tc = qset_of(tc, g, img);
   const int q = tc->q8_zz[c.qt][0];
+  const float w0 = tc->w_zz[c.qt][0];
   int ncand = (2 + 60 / (q >> 3)) | 1; if (ncand > 9) ncand = 9;
   const int half = ncand / 2;
   const int lim = 1 << tc->max_coef_bits;
@@ -2774,7 +2797,7 @@ __global__ void __launch_bounds__(64) k_trellis_dc_warp(Geom g, const TrellisCon
       if (cd >= lim) cd = lim - 1;
       if (cd <= -lim) cd = -lim + 1;
       int delta = cd * q - x;
-      float dist = (float)(delta * delta) * r.lambda_dc;
+      float dist = (float)(delta * delta) * dc_lambda(r.lambda_dc, lambda_from_norm, tc, w0);
       cd *= 1 + 2 * sign;
       float best; int bl = 0;
       if (bi == 0) {
@@ -2852,7 +2875,8 @@ __device__ __forceinline__ int bfind_u32(unsigned v) { int r; asm("bfind.u32 %0,
 template <bool FAST>
 __global__ void __launch_bounds__(DC2_WARPS * 32) k_trellis_dc_v2(Geom g, const TrellisConsts *__restrict__ tc,
                                                                  const DevHuff *__restrict__ tabs, size_t tabs_set_stride,
-                                                                 const DcRec *__restrict__ rec, RecLayout rl, int max_wib, int16_t *__restrict__ dcq, int write_coef)
+                                                                 const DcRec *__restrict__ rec, RecLayout rl, int max_wib, int16_t *__restrict__ dcq, int write_coef,
+                                                                 int lambda_from_norm)
 {
   extern __shared__ __align__(16) unsigned char dsm[];
   __shared__ float T[36];                                   // T[1 + bfind(|d|)] = (float)(bits + ehufsi[bits])
@@ -2882,6 +2906,7 @@ __global__ void __launch_bounds__(DC2_WARPS * 32) k_trellis_dc_v2(Geom g, const 
   uint8_t *bt = btw + (size_t)gsel * max_wib * 5;
   tc = qset_of(tc, g, img);
   const int q = tc->q8_zz[c.qt][0];
+  const float w0 = tc->w_zz[c.qt][0];
   int ncand = (2 + 60 / (q >> 3)) | 1; if (ncand > 9) ncand = 9;     // get_num_dc_trellis_candidates (:929-933)
   const int half = ncand / 2;
   const int lim = 1 << tc->max_coef_bits;
@@ -2910,7 +2935,7 @@ __global__ void __launch_bounds__(DC2_WARPS * 32) k_trellis_dc_v2(Geom g, const 
       for (int gg = 0; gg < 3; gg++) {
         const int raw = nxt[gg].raw_dc, x = abs(raw);
         const int qval = (int)(((unsigned long long)(unsigned)(x + qhalf) * qmul) >> qshift);       // (x + q/2) / q, exact
-        stage[warp][gg][lane] = make_int4(x, qval - half, 1 + 2 * (raw >> 31), __float_as_int(nxt[gg].lambda_dc));
+        stage[warp][gg][lane] = make_int4(x, qval - half, 1 + 2 * (raw >> 31), __float_as_int(dc_lambda(nxt[gg].lambda_dc, lambda_from_norm, tc, w0)));
       }
       __syncwarp();
       if (bi0 + 32 < wib) {
@@ -3016,7 +3041,8 @@ __global__ void __launch_bounds__(DC2_WARPS * 32) k_trellis_dc_v2(Geom g, const 
 }
 
 void launch_trellis_dc(const Geom &g, const TrellisConsts *tc, const DevHuff *tabs, size_t tabs_set_stride,
-                       const DcRec *rec, unsigned long long *bt, const RecLayout &rl, int vertical, int dc_fast, int16_t *dcq, int write_coef, int n, cudaStream_t s)
+                       const DcRec *rec, unsigned long long *bt, const RecLayout &rl, int vertical, int dc_fast, int16_t *dcq, int write_coef,
+                       int lambda_from_norm, int n, cudaStream_t s)
 {
   int n_imcu = 0, max_wib = 0;
   for (int ci = 0; ci < g.nc; ci++) { n_imcu = max(n_imcu, (g.c[ci].hib + g.c[ci].v - 1) / g.c[ci].v); max_wib = max(max_wib, g.c[ci].wib); }
@@ -3024,7 +3050,7 @@ void launch_trellis_dc(const Geom &g, const TrellisConsts *tc, const DevHuff *ta
     // trellis_delta_dc_weight > 0 (cjpeg -trellis-dc-ver-weight): the candidates' distortion reads the finished block
     // row above; only the one-thread-per-chain kernel carries that term (a non-default tuning option)
     dim3 grid((n_imcu + 63) / 64, n * g.nc);
-    k_trellis_dc<<<grid, 64, 0, s>>>(g, tc, tabs, tabs_set_stride, rec, bt, rl);
+    k_trellis_dc<<<grid, 64, 0, s>>>(g, tc, tabs, tabs_set_stride, rec, bt, rl, lambda_from_norm);
     LAUNCHED();
     if (dcq) launch_dc_collect(g, rl, dcq, n, s);
     return;
@@ -3037,8 +3063,8 @@ void launch_trellis_dc(const Geom &g, const TrellisConsts *tc, const DevHuff *ta
     if (smem2 > 40 * 1024) { cudaFuncSetAttribute(k_trellis_dc_v2<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024); cudaFuncSetAttribute(k_trellis_dc_v2<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024); }
     dim3 grid((n_imcu + DC2_WARPS * 3 - 1) / (DC2_WARPS * 3), n * g.nc);
     // the DC quantizer comes from each image's table set (TrellisConsts.dc_mul / dc_shift)
-    if (dc_fast) k_trellis_dc_v2<true><<<grid, DC2_WARPS * 32, smem2, s>>>(g, tc, tabs, tabs_set_stride, rec, rl, max_wib, dcq, write_coef || !dcq);
-    else k_trellis_dc_v2<false><<<grid, DC2_WARPS * 32, smem2, s>>>(g, tc, tabs, tabs_set_stride, rec, rl, max_wib, dcq, write_coef || !dcq);
+    if (dc_fast) k_trellis_dc_v2<true><<<grid, DC2_WARPS * 32, smem2, s>>>(g, tc, tabs, tabs_set_stride, rec, rl, max_wib, dcq, write_coef || !dcq, lambda_from_norm);
+    else k_trellis_dc_v2<false><<<grid, DC2_WARPS * 32, smem2, s>>>(g, tc, tabs, tabs_set_stride, rec, rl, max_wib, dcq, write_coef || !dcq, lambda_from_norm);
     LAUNCHED();
     return;
   }
@@ -3048,10 +3074,10 @@ void launch_trellis_dc(const Geom &g, const TrellisConsts *tc, const DevHuff *ta
   if (smem <= 200 * 1024) {
     if (smem > 48 * 1024) cudaFuncSetAttribute(k_trellis_dc_warp, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
     dim3 grid((n_imcu + warps * 3 - 1) / (warps * 3), n * g.nc);
-    k_trellis_dc_warp<<<grid, warps * 32, smem, s>>>(g, tc, tabs, tabs_set_stride, rec, rl, max_wib);
+    k_trellis_dc_warp<<<grid, warps * 32, smem, s>>>(g, tc, tabs, tabs_set_stride, rec, rl, max_wib, lambda_from_norm);
   } else {
     dim3 grid((n_imcu + 63) / 64, n * g.nc);
-    k_trellis_dc<<<grid, 64, 0, s>>>(g, tc, tabs, tabs_set_stride, rec, bt, rl);
+    k_trellis_dc<<<grid, 64, 0, s>>>(g, tc, tabs, tabs_set_stride, rec, bt, rl, lambda_from_norm);
   }
   LAUNCHED();
   if (dcq) launch_dc_collect(g, rl, dcq, n, s);

@@ -107,8 +107,8 @@ static_assert(sizeof(DevHuff) == 17 + 256 + 1 + 12 + 2 + 512 + 256, "DevHuff lay
 
 // per real block side record: K1 writes {f = norm (jcdctmgr.c:1026-1030, before the /63),
 // raw_dc, nz = number of non-zero plain-quantized AC coefficients, nzmask = their zigzag
-// positions (bit i = position i, bit 0 clear)}; the AC trellis replaces f by lambda_dc for
-// the DC trellis.
+// positions (bit i = position i, bit 0 clear)}; the band AC trellis (k_trellis_ac_band) replaces
+// f by lambda_dc for the DC trellis, k_trellis_ac3 leaves it.
 struct DcRec { float lambda_dc; int16_t raw_dc; uint8_t nz; uint8_t pad; unsigned long long nzmask; };
 static_assert(sizeof(DcRec) == 16, "DcRec layout");
 // where component ci's records start inside an image's record array
@@ -167,11 +167,13 @@ void launch_gather_comp_dc(const Geom &g, const RestartSpec &rs, const int16_t *
 void launch_gather_seq(const Geom &g, const ScanDesc &sd, const DcRec *nz_rec, const uint8_t *sym, const int16_t *dcq, const RecLayout &rl, uint32_t *hist, uint32_t *status, int n, cudaStream_t s);
 void launch_seed_hist(uint32_t *hist, int slot, int n, cudaStream_t s);
 void launch_gen_tables(const uint32_t *hist, DevHuff *tabs, size_t tabs_set_stride, const SlotMasks &masks, int nsets, cudaStream_t s);
-// AC trellis of the default option set: sorts the side records by non-zero count (srec: 16 bytes per real block;
-// splits: 4 class boundaries per (image, component) followed by 128 words of sorting counters each) and runs one
-// class-specific kernel per count class
+// AC trellis of the default option set: launch_trellis_sort sorts the side records by non-zero count (srec: 16 bytes
+// per real block; splits: 4 class boundaries per (image, component) followed by 128 words of sorting counters each),
+// then launch_trellis_ac3 runs one class-specific kernel per count class.  The records keep the forward kernel's norm
+// (the DC trellis behind it derives lambda_dc: launch_trellis_dc with lambda_from_norm)
+void launch_trellis_sort(const Geom &g, const DcRec *rec, const RecLayout &rl, void *srec, uint32_t *splits, int n, cudaStream_t s);
 void launch_trellis_ac3(const Geom &g, const TrellisConsts *tc, const DevHuff *tabs, size_t tabs_set_stride,
-                        DcRec *rec, const RecLayout &rl, void *srec, uint32_t *splits, const SymOut &so, int n, int sms, cudaStream_t s);
+                        DcRec *rec, const RecLayout &rl, const void *srec, const uint32_t *splits, const SymOut &so, int n, int sms, cudaStream_t s);
 // use_scans_in_trellis: quantize_trellis restricted to the zigzag band [Ss, Se]
 void launch_trellis_ac_band(const Geom &g, const TrellisConsts *tc, const DevHuff *tabs, size_t tabs_set_stride,
                             DcRec *rec, const RecLayout &rl, int Ss, int Se, const uint16_t *qimg, float4 *eo, int n, cudaStream_t s);
@@ -182,9 +184,11 @@ void launch_trellis_eob_rows(const Geom &g, const DevHuff *tabs, size_t tabs_set
 void launch_qopt_sums(const Geom &g, long long *qsum, int n, cudaStream_t s);
 void launch_qopt_update(long long *qsum, uint16_t *qimg, int n, cudaStream_t s);
 // dcq (or nullptr): dense array of the final DC values, one per real block, indexed like the side records; with it and
-// write_coef == 0 the coefficient planes are not touched (where the kernel in use can do without)
+// write_coef == 0 the coefficient planes are not touched (where the kernel in use can do without).  lambda_from_norm:
+// the records hold the forward kernel's norm (behind launch_trellis_ac3), not lambda_dc (behind launch_trellis_ac_band)
 void launch_trellis_dc(const Geom &g, const TrellisConsts *tc, const DevHuff *tabs, size_t tabs_set_stride,
-                       const DcRec *rec, unsigned long long *bt, const RecLayout &rl, int vertical, int dc_fast, int16_t *dcq, int write_coef, int n, cudaStream_t s);
+                       const DcRec *rec, unsigned long long *bt, const RecLayout &rl, int vertical, int dc_fast, int16_t *dcq, int write_coef,
+                       int lambda_from_norm, int n, cudaStream_t s);
 // DC statistics of a sequential scan from the dense DC array (+ the EOB of every dummy block): with the AC counts the
 // trellis back-track left in `hist`, the scan's complete statistics (encode_mcu_gather, jchuff.c:886-915)
 void launch_gather_seq_dc(const Geom &g, const ScanDesc &sd, const int16_t *dcq, const RecLayout &rl, uint32_t *hist, uint32_t *status, int n, cudaStream_t s);
