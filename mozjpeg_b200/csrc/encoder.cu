@@ -307,6 +307,7 @@ static void make_quant_consts(const b200jpeg_params *p, QuantTables *qt)
     qt->L[t] = L;
     qt->fast[t] = (((1ull << (18 + L)) + dmin - 1) / dmin) < (1ull << 32) ? 1 : 0;
     for (int i = 0; i < 64; i++) { unsigned d = qt->q[t][i].d; qt->q[t][i].mul2 = qt->fast[t] ? (uint32_t)(((1ull << (18 + L)) + d - 1) / d) : 0; }
+    for (int i = 0; i < 64; i++) qt->qpack[t][i] = make_uint2(qt->q[t][i].mul2, qt->q[t][i].bias << 14);
     static const short aanscales[64] = {16384, 22725, 21407, 19266, 16384, 12873, 8867, 4520, 22725, 31521, 29692, 26722, 22725, 17855, 12299, 6270,
       21407, 29692, 27969, 25172, 21407, 16819, 11585, 5906, 19266, 26722, 25172, 22654, 19266, 15137, 10426, 5315,
       16384, 22725, 21407, 19266, 16384, 12873, 8867, 4520, 12873, 17855, 16819, 15137, 12873, 10114, 6967, 3552,

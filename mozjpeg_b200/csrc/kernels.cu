@@ -512,40 +512,46 @@ __global__ void __launch_bounds__(128, FWD_MIN_CTAS) k_forward_tile(Geom g, cons
   __shared__ __align__(16) wtype sW[NB * 72];
   __shared__ __align__(128) unsigned char sIO[NB * 256];  // phase A: the tile's pixels as the TMA delivers them; phases D/E: output staging
   __shared__ __align__(8) unsigned long long tma_bar;
-  __shared__ uint2 sQC[NC][64];                           // quantizer constants per component, natural order
+  __shared__ __align__(16) uint2 sQC[NC][64];            // quantizer constants per component, natural order
   __shared__ uint2 sMask[NB];                             // per block: zigzag positions of its non-zero AC values
   __shared__ int sQL[NC];
-  __shared__ unsigned sHist[NC][HIST_BINS];               // fs.hist: the tile's AC symbol counts per component
+  constexpr int HW4 = (HIST_BINS + 3) / 4;                 // 16-byte words per histogram (the padding bins stay 0)
+  __shared__ __align__(16) unsigned sHist[NC][4 * HW4];    // fs.hist: the tile's AC symbol counts per component
 
   const int tid = threadIdx.x;
   const int tx = blockIdx.x, ty = blockIdx.y, img = blockIdx.z;
   const int x0 = tx * TW, y0 = ty * TR;
   const uint8_t *base = src + (size_t)img * g.image_stride;
   qt = qset_of(qt, g, img);
-  if (fs.hist) for (int i = tid; i < NC * HIST_BINS; i += 128) (&sHist[0][0])[i] = 0;
-
-  for (int i = tid; i < NC * 64; i += 128) { int ci = i >> 6, n = i & 63; const QuantConst &k = qt->q[g.c[ci].qt][n]; sQC[ci][n] = make_uint2(k.mul2, k.bias << 14); }
-  if (tid < NC) sQL[tid] = qt->L[g.c[tid].qt];
 
   // ---- A0: interior tiles of 8-bit RGB / gray input arrive by TMA: one thread posts the tile's box(es) of the
   //      (bytes per row, rows, images) tensor map -- 128 pixels x TR rows, 192-byte boxes because a box dimension is
   //      capped at 256 elements -- and everybody waits on the mbarrier the copies complete on.  Edge tiles (pixel
-  //      replication) and unaligned inputs keep the per-thread global loads. ----
+  //      replication) and unaligned inputs keep the per-thread global loads.  The copy is posted first, so that the
+  //      quantizer constants and the histogram clear below run while it is in flight. ----
   constexpr int TMA_BOXW = IC == 3 ? 192 : 128, TMA_NBOX = IC == 3 ? 2 : 1;
   static_assert(TMA_NBOX * TMA_BOXW * TR <= NB * 256, "the pixel tile fits the staging buffer it borrows");
   const bool tma_tile = PREC == 8 && use_tma && x0 + TW <= g.W && y0 + TR <= g.H;
-  if (tma_tile) {
-    const unsigned bar = (unsigned)__cvta_generic_to_shared(&tma_bar);
-    if (tid == 0) {
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"(bar) : "memory");
-      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-      asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(bar), "r"((unsigned)(TMA_NBOX * TMA_BOXW * TR)) : "memory");
+  const unsigned bar = (unsigned)__cvta_generic_to_shared(&tma_bar);
+  if (tma_tile && tid == 0) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"(bar) : "memory");
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(bar), "r"((unsigned)(TMA_NBOX * TMA_BOXW * TR)) : "memory");
 #pragma unroll
-      for (int bx = 0; bx < TMA_NBOX; bx++)
-        asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];"
-                     :: "r"((unsigned)__cvta_generic_to_shared(sIO + bx * TMA_BOXW * TR)), "l"(reinterpret_cast<unsigned long long>(&tmap)),
-                        "r"(x0 * IC + bx * TMA_BOXW), "r"(y0), "r"(g.image_stride ? img : 0), "r"(bar) : "memory");   // stride 0: one image for all
-    }
+    for (int bx = 0; bx < TMA_NBOX; bx++)
+      asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];"
+                   :: "r"((unsigned)__cvta_generic_to_shared(sIO + bx * TMA_BOXW * TR)), "l"(reinterpret_cast<unsigned long long>(&tmap)),
+                      "r"(x0 * IC + bx * TMA_BOXW), "r"(y0), "r"(g.image_stride ? img : 0), "r"(bar) : "memory");   // stride 0: one image for all
+  }
+
+  if (fs.hist) for (int i = tid; i < NC * HW4; i += 128) reinterpret_cast<uint4 *>(&sHist[0][0])[i] = make_uint4(0, 0, 0, 0);
+  // the packed {mul2, bias << 14} pairs, built once per table set on the host (QuantTables.qpack): 16-byte copies
+  if (QFAST && DCTM == 0)                                    // the only quantizer that reads them
+    for (int i = tid; i < NC * 32; i += 128)
+      reinterpret_cast<uint4 *>(sQC[i >> 5])[i & 31] = reinterpret_cast<const uint4 *>(qt->qpack[g.c[i >> 5].qt])[i & 31];
+  if (tid < NC) sQL[tid] = qt->L[g.c[tid].qt];
+
+  if (tma_tile) {
     __syncthreads();                                             // the barrier word is initialised before anyone polls it
     {
       unsigned done = 0;
@@ -940,17 +946,23 @@ __global__ void __launch_bounds__(128, FWD_MIN_CTAS) k_forward_tile(Geom g, cons
         }
         unsigned *h = sHist[NC == 1 ? 0 : ci];
         if (!(m >> 63)) atomicAdd(&h[0], 1u);                  // EOB
-        int prev = 0; bool bad = false;
-        while (m) {
-          const int k = __ffsll((long long)m) - 1;
-          m &= m - 1;
-          const int run = k - prev - 1; prev = k;
-          const int nb = nbits_of(abs((int)q[k]));
-          bad |= nb > g.max_coef_bits;
-          if (run >> 4) atomicAdd(&h[0xF0], (unsigned)(run >> 4));
-          atomicAdd(&h[((run & 15) << 4) + nb], 1u);             // '+' as walk_seq_block: a 16-bit size lands in bin 256
+        // the mask in two 32-bit halves: a 32-bit lowest-set-bit step is two instructions, the 64-bit one eight
+        int prev = 0; unsigned any = 0;
+#pragma unroll
+        for (int half = 0; half < 2; half++) {
+          unsigned w = (unsigned)(m >> (32 * half));
+          while (w) {
+            const int k = 32 * half + __ffs(w) - 1;
+            w &= w - 1;
+            const int run = k - prev - 1; prev = k;
+            const int a = abs((int)q[k]);
+            any |= (unsigned)a;
+            if (run >> 4) atomicAdd(&h[0xF0], (unsigned)(run >> 4));
+            atomicAdd(&h[((run & 15) << 4) + nbits_of(a)], 1u);  // '+' as walk_seq_block: a 16-bit size lands in bin 256
+          }
         }
-        if (bad) atomicOr(&fs.status[img], 2u);                 // JERR_BAD_DCT_COEF
+        // the largest size of the block is the size of the OR of its magnitudes
+        if (nbits_of((int)any) > g.max_coef_bits) atomicOr(&fs.status[img], 2u);   // JERR_BAD_DCT_COEF
       }
     }
   }
@@ -958,10 +970,15 @@ __global__ void __launch_bounds__(128, FWD_MIN_CTAS) k_forward_tile(Geom g, cons
   // ---- flush (fs.hist): the tile's non-zero AC counts into the image's histograms ----
   if (PREC == 8 && fs.hist) {
     __syncthreads();
-    for (int i = tid; i < NC * HIST_BINS; i += 128) {
-      const unsigned v = (&sHist[0][0])[i];
-      const int ci = i / HIST_BINS, sym = i - ci * HIST_BINS;
-      if (v) atomicAdd(&fs.hist[(((size_t)img * g.nc + ci) * HIST_SLOTS + 4 + g.c[ci].ac_tbl) * HIST_BINS + sym], v);
+    for (int i = tid; i < NC * HW4; i += 128) {              // four bins per thread and step
+      const uint4 v = reinterpret_cast<const uint4 *>(&sHist[0][0])[i];
+      if ((v.x | v.y | v.z | v.w) == 0) continue;
+      const int ci = i / HW4, sym = 4 * (i - ci * HW4);
+      unsigned *gh = &fs.hist[(((size_t)img * g.nc + ci) * HIST_SLOTS + 4 + g.c[ci].ac_tbl) * HIST_BINS + sym];
+      if (v.x) atomicAdd(gh, v.x);
+      if (v.y) atomicAdd(gh + 1, v.y);
+      if (v.z) atomicAdd(gh + 2, v.z);
+      if (v.w) atomicAdd(gh + 3, v.w);
     }
   }
 

@@ -77,7 +77,8 @@ struct ScanDesc {
 struct QuantConst { uint32_t mul; uint16_t shift; uint16_t pad; uint32_t bias; uint32_t d; uint32_t mul2; };
 // JDCT_IFAST: the scaled divisor's reciprocal / correction / shift (compute_reciprocal, jcdctmgr.c:181-230, DCTELEM = int)
 struct IfastConst { uint32_t recip, corr; int shift; int pad; };
-struct QuantTables { QuantConst q[4][64]; int L[4]; int fast[4]; float fdiv[4][64]; IfastConst ifast[4][64]; };   // fdiv: JDCT_FLOAT divisors (jcdctmgr.c:355-379)                 // natural order
+// qpack: {mul2, bias << 14} per natural position, the tiled forward kernel's shared copy of the fast quantizer
+struct QuantTables { QuantConst q[4][64]; int L[4]; int fast[4]; float fdiv[4][64]; IfastConst ifast[4][64]; alignas(16) uint2 qpack[4][64]; };   // fdiv: JDCT_FLOAT divisors (jcdctmgr.c:355-379)                 // natural order
 struct TrellisConsts {
   float w_zz[4][64];      // (float)(1.0/(Q*Q)) per zigzag position   jcdctmgr.c:1017-1021
   int   q8_zz[4][64];     // 8*Q per zigzag position
