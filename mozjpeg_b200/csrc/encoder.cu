@@ -316,6 +316,10 @@ static void make_quant_consts(const b200jpeg_params *p, QuantTables *qt)
       unsigned divisor = (unsigned)(unsigned short)(((long)p->quant_tbl[t][i] * aanscales[i] + (1L << 10)) >> 11);
       IfastConst &k = qt->ifast[t][i]; k.pad = 0;
       if (divisor == 1) { k.recip = 1; k.corr = 0; k.shift = -32; continue; }
+      // the 16-bit divisor wraps to 0 for 14 table values (16384 at the 16384-scaled positions, ...); only the fast DCT
+      // reads these constants, and the reference cannot quantize such a table with it either (compute_reciprocal
+      // divides by the wrapped value), so leave them zero instead of dividing by zero for every DCT method
+      if (divisor == 0) { k.recip = 0; k.corr = 0; k.shift = 0; continue; }
       int b = 0; for (unsigned v = divisor; v; v >>= 1) b++; b -= 1;
       int r = 32 + b;
       unsigned long long fq = (1ULL << r) / divisor, fr = (1ULL << r) % divisor; unsigned c = divisor / 2;

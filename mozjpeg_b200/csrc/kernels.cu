@@ -3769,7 +3769,8 @@ __device__ __forceinline__ void load_prog_aux(const ScanDesc &sd, const uint32_t
 struct HistSinkP {
   unsigned *dc_hist, *ac_hist; int bad; int maxbits;
   __device__ void dc(int nb, int) { if (nb > maxbits + 1) bad = 1; atomicAdd(&dc_hist[nb], 1u); }
-  __device__ void ac(int sym, int nb, int) { if (nb > 14) bad = 1; atomicAdd(&ac_hist[sym], 1u); }
+  // a value's size against max_coef_bits (jcphuff.c:633); an EOBRUN symbol (low nibble 0) carries up to 14 run bits
+  __device__ void ac(int sym, int nb, int) { if (nb > 14 || ((sym & 15) && nb > maxbits)) bad = 1; atomicAdd(&ac_hist[sym], 1u); }
   __device__ void raw(unsigned, int) {}
 };
 struct CountSinkP {

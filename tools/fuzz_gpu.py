@@ -3,7 +3,7 @@
 (the optional trellis modes), pixel orders of the RGB family, the CMYK / YCCK / YCbCr->gray / JCS_UNKNOWN conversions and small batches (some with
 per-image quantization tables) through the C-ABI, every file compared
 byte for byte with the CPU oracle (itself pinned to the reference).  Test infrastructure.
-usage: fuzz_gpu.py [seed] [cases] [seconds]      (exit status 1 if anything differs)"""
+usage: fuzz_gpu.py [--yuv | --content] [seed] [cases] [seconds]      (exit status 1 if anything differs)"""
 import os, random, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import ctypes as C
@@ -70,6 +70,63 @@ def fuzz_yuv(seed, cases, budget):
     print("yuv seed", seed, "bad", bad, "compared", tot, "refused", refused, "seconds %.0f" % (time.time() - t0))
     return bad
 
+
+def fuzz_content(seed, cases, budget):
+    """fuzz_gpu.py --content [seed] [cases] [seconds]: the constructed families of tests/adversarial_cases.py (flat-block
+    ladders under random flat tables, basis-sum blocks, screen content) cropped at random, under random switch sets and
+    sampling layouts, device against the CPU oracle."""
+    import adversarial_cases as ADV
+    rng = random.Random(seed)
+    screens = list(ADV.screen_images(seed).values())
+    bad = tot = refused = 0
+    t0 = time.time()
+    for it in range(cases):
+        if time.time() - t0 > budget:
+            break
+        fam = rng.choice(["ladder", "basis", "screen"])
+        qt = None
+        if fam == "ladder":
+            img = ADV.flat_ladder()
+            qt = ADV.flat_tables([rng.randint(1, 255) for _ in range(rng.choice([1, 2, 5]))])
+        elif fam == "basis":
+            img = ADV.basis_image(rng.choice([6, 8, 12, 16, 24]), rng.randrange(1 << 20))
+        else:
+            img = rng.choice(screens)
+        h, w = img.shape[:2]
+        img = np.ascontiguousarray(img[:rng.randint(max(1, h - 9), h), :rng.randint(max(1, w - 9), w)])
+        sw = rng.choice([["-baseline"], ["-baseline", "-notrellis"], ["-fastcrush"], [], ["-revert"], ["-baseline", "-restart", "1"]])
+        sw = sw + ["-quality", str(rng.choice([30, 75, 95, 100]))] if rng.random() < 0.4 else list(sw)
+        if rng.random() < 0.3: sw += ["-dct", rng.choice(["fast", "float"])]
+        if img.ndim == 3: sw += rng.choice([["-sample", s] for s in ("1x1", "2x1", "1x2", "2x2", "3x2")] + [["-grayscale"]])
+        try:
+            p = mj.params_from_switches(sw, img.shape[1], img.shape[0], 1 if img.ndim == 2 else 3)
+        except Exception:
+            refused += 1; continue
+        imgs = img[None]
+        try:
+            got = enc.encode_batch(p, imgs, qtables=qt)
+        except mj.B200JpegError as ex:
+            if ex.code == -2:
+                refused += 1; continue
+            bad += 1; print("CONTENT DEVICE FAIL", fam, sw, img.shape, ex); continue
+        tot += 1
+        for i, out in enumerate(got):
+            pi = p
+            if qt is not None:
+                pi = p.copy(); np.ctypeslib.as_array(pi.quant_tbl)[:] = qt[i]
+            if out != O.oracle_encode(pi, img).jpeg:
+                bad += 1; print("CONTENT MISMATCH", fam, sw, img.shape, "table set", i); break
+    print("content seed", seed, "bad", bad, "compared", tot, "refused", refused, "seconds %.0f" % (time.time() - t0))
+    return bad
+
+
+if "--content" in sys.argv:
+    sys.argv.remove("--content")
+    enc = mj.Encoder(0)
+    nbad = fuzz_content(int(sys.argv[1]) if len(sys.argv) > 1 else 1, int(sys.argv[2]) if len(sys.argv) > 2 else 300,
+                        float(sys.argv[3]) if len(sys.argv) > 3 else 120.0)
+    enc.close()
+    sys.exit(1 if nbad else 0)
 
 if "--yuv" in sys.argv:
     sys.argv.remove("--yuv")
