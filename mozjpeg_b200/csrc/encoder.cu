@@ -79,13 +79,13 @@ using namespace b200;
 #define MAX_ARENAS 4
 struct Arena {
   b200::DevBuf d_planes;             // input smoothing: the pre-pass's component planes
-  b200::DevBuf d_coef[4], d_raw[4], d_plain[4], d_hist, d_tabs_trellis, d_rec, d_bt, d_srec, d_splits, d_best_al, d_qimg, d_qsum, d_eo, d_es;
+  b200::DevBuf d_coef[4], d_raw[4], d_plain[4], d_hist, d_tabs_trellis, d_rec, d_srec, d_splits, d_best_al, d_qimg, d_qsum, d_eo, d_es;
   b200::DevBuf d_blk_bits, d_tile_bits, d_tile_base, d_seg_corr, d_mark, d_stuff_lb, d_blk_aux, d_blk_run, d_blk_mask, d_total_bits, d_bitbuf;
   b200::DevBuf d_sym, d_dcq;         // sequential scans after the trellis: symbol records + dense DC values (SymOut, kernels.cuh)
   b200::DevBuf d_diff;               // lossless scans: the differences of the scan being coded (launch_lossless_diff)
   b200::Geom g;                      // the plan's geometry with this arena's coefficient pointers
   void release() {
-    b200::DevBuf *db[] = {&d_planes, &d_hist, &d_tabs_trellis, &d_rec, &d_bt, &d_srec, &d_splits, &d_best_al, &d_qimg, &d_qsum, &d_eo, &d_es, &d_blk_bits, &d_tile_bits, &d_tile_base, &d_seg_corr, &d_mark, &d_stuff_lb, &d_blk_aux, &d_blk_run, &d_blk_mask, &d_total_bits, &d_bitbuf, &d_sym, &d_dcq, &d_diff};
+    b200::DevBuf *db[] = {&d_planes, &d_hist, &d_tabs_trellis, &d_rec, &d_srec, &d_splits, &d_best_al, &d_qimg, &d_qsum, &d_eo, &d_es, &d_blk_bits, &d_tile_bits, &d_tile_base, &d_seg_corr, &d_mark, &d_stuff_lb, &d_blk_aux, &d_blk_run, &d_blk_mask, &d_total_bits, &d_bitbuf, &d_sym, &d_dcq, &d_diff};
     for (b200::DevBuf *b : db) b->release();
     for (int i = 0; i < 4; i++) { d_coef[i].release(); d_raw[i].release(); d_plain[i].release(); }
   }
@@ -471,7 +471,6 @@ static int prepare_batch(b200jpeg_encoder *e, int n_total, int chunk, bool host_
     if ((rc = a.d_hist.reserve(hist_bytes * g.nc))) return rc;
     if ((rc = a.d_tabs_trellis.reserve(tabset * 4 * n))) return rc;
     if ((rc = a.d_rec.reserve((size_t)n * pl.sum_real_blocks * sizeof(DcRec)))) return rc;
-    if ((rc = a.d_bt.reserve((size_t)n * pl.sum_real_blocks * 8))) return rc;
     if ((rc = a.d_srec.reserve((size_t)n * pl.sum_real_blocks * 16))) return rc;
     if ((rc = a.d_splits.reserve((size_t)n * 4 * (4 + 128) * 4))) return rc;      // class boundaries + the sort's counters
     if (use_symrec(pl, p)) {
@@ -757,8 +756,8 @@ static int run_pipeline(b200jpeg_encoder *e, const ChunkIO &io, Timer &tm)
       // behind k_trellis_ac3 the records still hold the norm; the band kernel stores lambda_dc (from re-fitted tables
       // with trellis_q_opt)
       const int lambda_from_norm = generic_rounds ? 0 : 1;
-      if (pl.progressive) launch_trellis_dc(gr, e->d_tc.as<TrellisConsts>(), e->d_tabs_fixed.as<DevHuff>(), 0, A.d_rec.as<DcRec>(), A.d_bt.as<unsigned long long>(), rlr, p->trellis_delta_dc_weight > 0.0f, dc_fast_of(gr), nullptr, 1, lambda_from_norm, n, s);
-      else launch_trellis_dc(gr, e->d_tc.as<TrellisConsts>(), tset, tabset, A.d_rec.as<DcRec>(), A.d_bt.as<unsigned long long>(), rlr, p->trellis_delta_dc_weight > 0.0f, dc_fast_of(gr), so.dcq, so.keep_coef, lambda_from_norm, n, s);
+      if (pl.progressive) launch_trellis_dc(gr, e->d_tc.as<TrellisConsts>(), e->d_tabs_fixed.as<DevHuff>(), 0, A.d_rec.as<DcRec>(), rlr, p->trellis_delta_dc_weight > 0.0f, dc_fast_of(gr), nullptr, 1, lambda_from_norm, n, s);
+      else launch_trellis_dc(gr, e->d_tc.as<TrellisConsts>(), tset, tabset, A.d_rec.as<DcRec>(), rlr, p->trellis_delta_dc_weight > 0.0f, dc_fast_of(gr), so.dcq, so.keep_coef, lambda_from_norm, n, s);
     }
     return B200JPEG_OK;
     };

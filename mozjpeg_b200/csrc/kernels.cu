@@ -2514,8 +2514,8 @@ k_trellis_ac3(Geom g, const TrellisConsts *__restrict__ tc, const DevHuff *__res
       uint4 *q4 = reinterpret_cast<uint4 *>(o16);
       auto write_block = [&](int lst) {
         // without want_dc a DC trellis follows and the scans read the DC from dcq: the plane's DC is never read (the
-        // fallback DC trellis kernels write every real block's DC before they read it), and on the path where the
-        // forward kernel counted the statistics nobody wrote it
+        // DC trellis reads the side records), and on the path where the forward kernel counted the statistics nobody
+        // wrote it
         q4[0] = make_uint4(want_dc ? dc_q : 0u, 0, 0, 0);
 #pragma unroll
         for (int v = 1; v < 8; v++) q4[v] = make_uint4(0, 0, 0, 0);
@@ -2628,30 +2628,10 @@ void launch_trellis_ac3(const Geom &g, const TrellisConsts *tc, const DevHuff *t
   launch_t3<8>(grid, s, g, tc, tabs, tabs_set_stride, rec, rl, sr, splits, so);
 }
 
-// the real blocks' DC values gathered into the dense array (after the DC trellis kernels that do not write it themselves)
-__global__ void __launch_bounds__(256) k_dc_collect(Geom g, RecLayout rl, int16_t *__restrict__ dcq)
-{
-  const int ci = blockIdx.y % g.nc, img = blockIdx.y / g.nc;
-  const CompGeom &c = g.c[ci];
-  const long long nblk = (long long)c.wib * c.hib, t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= nblk) return;
-  const int row = (int)(t / c.wib), col = (int)(t - (long long)row * c.wib);
-  dcq[(size_t)img * rl.per_image + rl.comp_off[ci] + t] = c.coef[(((size_t)img * c.hpad + row) * c.wpad + col) * 64];
-}
-static void launch_dc_collect(const Geom &g, const RecLayout &rl, int16_t *dcq, int n, cudaStream_t s)
-{
-  long long mb = 0;
-  for (int ci = 0; ci < g.nc; ci++) mb = max(mb, (long long)g.c[ci].wib * g.c[ci].hib);
-  dim3 grid((unsigned)((mb + 255) / 256), n * g.nc);
-  k_dc_collect<<<grid, 256, 0, s>>>(g, rl, dcq); LAUNCHED();
-}
-
 // =====================================================================
 // trellis quantization, DC part (jcdctmgr.c:1045-1118 forward, :1308-1327
 // back-track).  The Viterbi chain runs along one block row; last_dc carries
 // from block row to block row inside an iMCU row (jccoefct.c:418, :1320).
-// One thread per (image, iMCU row).  bt[] holds, per block, the 9 back
-// pointers (4 bits each), the unsigned quantized value and the sign.
 // =====================================================================
 // The block's lambda_dc from its record's first word.  Behind k_trellis_ac_band that word holds lambda_dc; behind
 // k_trellis_ac3 (from_norm) it still holds the forward kernel's norm, and lambda_dc is derived here with the expression
@@ -2667,201 +2647,10 @@ __device__ __forceinline__ float dc_lambda(const float f, const int from_norm, c
   return lambda * w0;
 }
 
-__global__ void __launch_bounds__(64) k_trellis_dc(Geom g, const TrellisConsts *__restrict__ tc,
-                                                   const DevHuff *__restrict__ tabs, size_t tabs_set_stride,
-                                                   const DcRec *__restrict__ rec, unsigned long long *__restrict__ bt, RecLayout rl, int lambda_from_norm)
-{
-  const int ci = blockIdx.y % g.nc, img = blockIdx.y / g.nc;
-  const CompGeom &c = g.c[ci];
-  __shared__ uint8_t dcsi[32];
-  {
-    const DevHuff *dc = reinterpret_cast<const DevHuff *>(reinterpret_cast<const char *>(tabs) + (size_t)blockIdx.y * tabs_set_stride) + c.dc_tbl;
-    if (threadIdx.x < 32) dcsi[threadIdx.x] = dc->size[threadIdx.x];
-  }
-  __syncthreads();
-  int imcu = blockIdx.x * blockDim.x + threadIdx.x;
-  int n_imcu = (c.hib + c.v - 1) / c.v;
-  if (imcu >= n_imcu) return;
-  const int q = qset_of(tc, g, img)->q8_zz[c.qt][0];            // the image's table set (the other fields are the batch's)
-  const float w0 = qset_of(tc, g, img)->w_zz[c.qt][0];
-  int ncand = (2 + 60 / (q >> 3)) | 1; if (ncand > 9) ncand = 9;     // get_num_dc_trellis_candidates (:929-933)
-  const int half = ncand / 2;
-  const int lim = 1 << tc->max_coef_bits;
-  int last_dc = 0;
-  for (int br = 0; br < c.v; br++) {
-    int row = imcu * c.v + br;
-    if (row >= c.hib) break;
-    size_t rbase = (size_t)img * rl.per_image + rl.comp_off[ci] + (size_t)row * c.wib;
-    float acc[9]; int prevc[9];
-#pragma unroll
-    for (int k = 0; k < 9; k++) { acc[k] = 0.f; prevc[k] = 0; }
-    for (int bi = 0; bi < c.wib; bi++) {
-      DcRec r = rec[rbase + bi];
-      int raw = r.raw_dc, sign = raw >> 31, x = abs(raw);
-      int qval = (x + q / 2) / q;
-      const float lambda_dc = dc_lambda(r.lambda_dc, lambda_from_norm, tc, w0);
-      // trellis_delta_dc_weight: the block above inside the same iMCU row (lastblockrow, jccoefct.c:420) - its raw DC and
-      // the value this thread's back-track of the previous block row left in the coefficient plane
-      const bool vert = br > 0 && tc->delta_dc_weight > 0.0f;
-      int above_raw = 0, above_fin = 0;
-      if (vert) { above_raw = rec[rbase - c.wib + bi].raw_dc; above_fin = c.coef[(((size_t)img * c.hpad + row - 1) * c.wpad + bi) * 64]; }
-      float nacc[9]; int cand[9];
-      unsigned long long w = 0;
-#pragma unroll
-      for (int k = 0; k < 9; k++) {
-        nacc[k] = 0.f; cand[k] = 0;
-        if (k < ncand) {
-          int cd = qval - half + k;
-          if (cd >= lim) cd = lim - 1;
-          if (cd <= -lim) cd = -lim + 1;
-          int delta = cd * q - x;
-          float dist = (float)(delta * delta) * lambda_dc;
-          cd *= 1 + 2 * sign;
-          cand[k] = cd;
-          if (vert) {                                               // difference of vertical gradients (:1069-1086)
-            const int d2 = (above_raw - raw) - (above_fin * q - cd * q);
-            const float vd = (float)(d2 * d2) * lambda_dc;
-            dist += tc->delta_dc_weight * (vd - dist);
-          }
-          if (bi == 0) {
-            int bits = nbits_of(abs(cd - last_dc));
-            nacc[k] = (float)(bits + dcsi[bits]) + dist;
-          } else {
-            float best = 0.f; int bl = 0;
-#pragma unroll
-            for (int l = 0; l < 9; l++) {
-              if (l < ncand) {
-                int bits = nbits_of(abs(cd - prevc[l]));
-                float cost = (float)(bits + dcsi[bits]) + dist + acc[l];
-                if (l == 0 || cost < best) { best = cost; bl = l; }
-              }
-            }
-            nacc[k] = best; w |= (unsigned long long)bl << (4 * k);
-          }
-        }
-      }
-#pragma unroll
-      for (int k = 0; k < 9; k++) { acc[k] = nacc[k]; prevc[k] = cand[k]; }
-      w |= (unsigned long long)(qval & 0xFFF) << 36;
-      w |= (unsigned long long)(sign & 1) << 48;
-      bt[rbase + bi] = w;
-    }
-    int j = 0; float bj = acc[0];
-#pragma unroll
-    for (int i = 1; i < 9; i++) if (i < ncand && acc[i] < bj) { bj = acc[i]; j = i; }
-    for (int bi = c.wib - 1; bi >= 0; bi--) {
-      unsigned long long w = bt[rbase + bi];
-      int qval = (int)((w >> 36) & 0xFFF), sg = (int)((w >> 48) & 1);
-      int cd = qval - half + j;
-      if (cd >= lim) cd = lim - 1;
-      if (cd <= -lim) cd = -lim + 1;
-      if (sg) cd = -cd;
-      c.coef[(((size_t)img * c.hpad + row) * c.wpad + bi) * 64] = (int16_t)cd;
-      if (bi == c.wib - 1) last_dc = cd;
-      j = (int)((w >> (4 * j)) & 0xF);
-    }
-  }
-}
 // ---------------------------------------------------------------------
-// DC trellis, warp-cooperative version: 9 lanes per Viterbi chain (lane k =
-// candidate k), 3 chains per warp.  Back pointers and the per-block candidate
-// base live in shared memory, so the serial back-track (:1308-1327) chases
-// pointers at shared-memory latency.  Same arithmetic and tie-breaks as
-// k_trellis_dc (the one-thread-per-chain fallback for very wide images).
-// smem per chain: wib * 11 bytes (9 back pointers + int16 signed base).
-// ---------------------------------------------------------------------
-__global__ void __launch_bounds__(64) k_trellis_dc_warp(Geom g, const TrellisConsts *__restrict__ tc,
-                                                        const DevHuff *__restrict__ tabs, size_t tabs_set_stride,
-                                                        const DcRec *__restrict__ rec, RecLayout rl, int max_wib, int lambda_from_norm)
-{
-  extern __shared__ unsigned char dsm[];
-  const int ci = blockIdx.y % g.nc, img = blockIdx.y / g.nc;
-  const CompGeom &c = g.c[ci];
-  __shared__ uint8_t dcsi[32];
-  {
-    const DevHuff *dc = reinterpret_cast<const DevHuff *>(reinterpret_cast<const char *>(tabs) + (size_t)blockIdx.y * tabs_set_stride) + c.dc_tbl;
-    if (threadIdx.x < 32) dcsi[threadIdx.x] = dc->size[threadIdx.x];
-  }
-  __syncthreads();
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int grp = lane / 9, k = lane - grp * 9;                 // lanes 27..31: grp == 3, idle
-  const int chain_in_cta = warp * 3 + grp;
-  const int chains_per_cta = (blockDim.x >> 5) * 3;
-  const int imcu = blockIdx.x * chains_per_cta + chain_in_cta;
-  const int n_imcu = (c.hib + c.v - 1) / c.v;
-  const bool active = grp < 3 && imcu < n_imcu;
-  int16_t *qs = reinterpret_cast<int16_t *>(dsm) + (size_t)chain_in_cta * max_wib;
-  uint8_t *bt8 = dsm + (size_t)chains_per_cta * max_wib * 2 + (size_t)chain_in_cta * max_wib * 9;
-  tc = qset_of(tc, g, img);
-  const int q = tc->q8_zz[c.qt][0];
-  const float w0 = tc->w_zz[c.qt][0];
-  int ncand = (2 + 60 / (q >> 3)) | 1; if (ncand > 9) ncand = 9;
-  const int half = ncand / 2;
-  const int lim = 1 << tc->max_coef_bits;
-  const int gbase = grp * 9;
-  int last_dc = 0;
-  for (int br = 0; br < c.v; br++) {
-    int row = imcu * c.v + br;
-    bool rowok = active && row < c.hib;                        // uniform within a 9-lane group
-    size_t rbase = (size_t)img * rl.per_image + rl.comp_off[ci] + (size_t)(rowok ? row : 0) * c.wib;
-    float acc = 0.f; int prevc = 0;
-    DcRec r = rec[rbase];
-    for (int bi = 0; bi < c.wib; bi++) {
-      DcRec rn = rec[rbase + min(bi + 1, c.wib - 1)];          // prefetch the next record
-      int raw = r.raw_dc, sign = raw >> 31, x = abs(raw);
-      int qval = (x + q / 2) / q;
-      int cd = qval - half + k;
-      if (cd >= lim) cd = lim - 1;
-      if (cd <= -lim) cd = -lim + 1;
-      int delta = cd * q - x;
-      float dist = (float)(delta * delta) * dc_lambda(r.lambda_dc, lambda_from_norm, tc, w0);
-      cd *= 1 + 2 * sign;
-      float best; int bl = 0;
-      if (bi == 0) {
-        int bits = nbits_of(abs(cd - last_dc));
-        best = (float)(bits + dcsi[bits]) + dist;
-      } else {
-        best = 0.f;
-#pragma unroll
-        for (int l = 0; l < 9; l++) {
-          int pc = __shfl_sync(0xffffffffu, prevc, gbase + l);
-          float pa = __shfl_sync(0xffffffffu, acc, gbase + l);
-          if (l < ncand) {
-            int bits = nbits_of(abs(cd - pc));
-            float cost = (float)(bits + dcsi[bits]) + dist + pa;
-            if (l == 0 || cost < best) { best = cost; bl = l; }
-          }
-        }
-      }
-      acc = best; prevc = cd;
-      if (rowok && k < ncand) bt8[(size_t)bi * 9 + k] = (uint8_t)bl;
-      if (rowok && k == 0) qs[bi] = (int16_t)(sign ? -qval - 1 : qval);     // sign folded in (one's complement keeps -0 distinct)
-      r = rn;
-    }
-    // first minimum over the candidates (:1309-1313)
-    int j = 0; float bj = __shfl_sync(0xffffffffu, acc, gbase);
-#pragma unroll
-    for (int i = 1; i < 9; i++) { float a = __shfl_sync(0xffffffffu, acc, gbase + i); if (i < ncand && a < bj) { bj = a; j = i; } }
-    __syncwarp();
-    if (rowok && k == 0) {
-      for (int bi = c.wib - 1; bi >= 0; bi--) {
-        int e = qs[bi]; int sg = e < 0; int qval = sg ? -e - 1 : e;
-        int cd = qval - half + j;
-        if (cd >= lim) cd = lim - 1;
-        if (cd <= -lim) cd = -lim + 1;
-        if (sg) cd = -cd;
-        c.coef[(((size_t)img * c.hpad + row) * c.wpad + bi) * 64] = (int16_t)cd;
-        if (bi == c.wib - 1) last_dc = cd;
-        j = bt8[(size_t)bi * 9 + j];
-      }
-    }
-    last_dc = __shfl_sync(0xffffffffu, last_dc, gbase < 27 ? gbase : 0);
-    __syncwarp();
-  }
-}
-// ---------------------------------------------------------------------
-// DC trellis, latency-oriented version.  Layout as above (9 lanes per chain,
-// lane k = candidate k, 3 chains per warp) but:
+// k_trellis_dc_v2: 9 lanes per Viterbi chain (lane k = candidate k), 3 chains
+// (iMCU rows) per warp, DC2_WARPS warps per CTA (one where the rows are too
+// wide for that many chains' back pointers in shared memory).
 //   * the side records of the next 32 blocks are fetched by the whole warp
 //     (coalesced) while the current 32 are processed from shared memory;
 //   * everything that does not depend on the Viterbi state -- candidate values,
@@ -2871,16 +2660,13 @@ __global__ void __launch_bounds__(64) k_trellis_dc_warp(Geom g, const TrellisCon
 //     4-level first-minimum tree;
 //   * the serial back-track only chases one byte per block through shared
 //     memory; candidates are turned into coefficients by all 32 lanes afterwards.
-// Arithmetic, association order and tie-breaks are those of k_trellis_dc.
+// Arithmetic, association order and tie-breaks are those of quantize_trellis.
 // ---------------------------------------------------------------------
 #ifndef DC2_WARPS
 #define DC2_WARPS 2
 #endif
 // FAST instantiation: the rates of a step's 9 predecessor differences, |D0 -+ l|, come from one table indexed by the
 // signed difference (consecutive words from one base address) instead of abs / find-leading-one / table per difference
-#ifndef DC_TABLE
-#define DC_TABLE 1
-#endif
 #define DC_TAB_HALF 512
 // FLO: index of the most significant set bit, 0xFFFFFFFF for 0, so that
 // nbits(v) == bfind(v) + 1 (JPEG_NBITS) without the clz arithmetic.
@@ -2889,7 +2675,9 @@ __device__ __forceinline__ int bfind_u32(unsigned v) { int r; asm("bfind.u32 %0,
 // FAST: 9 candidates and no clamping possible for any DC value (lim - 1 >= the
 // largest reachable candidate): the 81 candidate differences of a step collapse
 // to D0 - psgn*l, and no candidate needs masking.
-template <bool FAST>
+// VERT: trellis_delta_dc_weight > 0 (cjpeg -trellis-dc-ver-weight): from an iMCU row's second block row on, a candidate's
+// distortion is blended with the difference of vertical gradients to the finished block above (:1069-1086).
+template <bool FAST, bool VERT>
 __global__ void __launch_bounds__(DC2_WARPS * 32) k_trellis_dc_v2(Geom g, const TrellisConsts *__restrict__ tc,
                                                                  const DevHuff *__restrict__ tabs, size_t tabs_set_stride,
                                                                  const DcRec *__restrict__ rec, RecLayout rl, int max_wib, int16_t *__restrict__ dcq, int write_coef,
@@ -2897,17 +2685,22 @@ __global__ void __launch_bounds__(DC2_WARPS * 32) k_trellis_dc_v2(Geom g, const 
 {
   extern __shared__ __align__(16) unsigned char dsm[];
   __shared__ float T[36];                                   // T[1 + bfind(|d|)] = (float)(bits + ehufsi[bits])
-  __shared__ float Tt[(FAST && DC_TABLE) ? 2 * DC_TAB_HALF + 8 : 1];   // Tt[d + DC_TAB_HALF] = T[1 + bfind(|d|)], -DC_TAB_HALF <= d < DC_TAB_HALF + 8
+  __shared__ float Tt[FAST ? 2 * DC_TAB_HALF + 8 : 1];      // Tt[d + DC_TAB_HALF] = T[1 + bfind(|d|)], -DC_TAB_HALF <= d < DC_TAB_HALF + 8
   __shared__ int4 stage[DC2_WARPS][3][32];                  // per staged block {|raw DC|, qval - half, +1 / -1, lambda bits}: what a step needs of the record
+  __shared__ int2 vstage[DC2_WARPS][3][32];                 // VERT: per staged block {raw DC above - raw DC, final DC above * q}
   const int ci = blockIdx.y % g.nc, img = blockIdx.y / g.nc;
   const CompGeom &c = g.c[ci];
+  // the tables are filled in strides of DC2_WARPS * 32 entries, a one-warp CTA's threads taking two slots each (with a
+  // stride of blockDim.x the FAST kernel needs one register more)
   {
     const DevHuff *dc = reinterpret_cast<const DevHuff *>(reinterpret_cast<const char *>(tabs) + (size_t)blockIdx.y * tabs_set_stride) + c.dc_tbl;
-    if (threadIdx.x < 33) T[threadIdx.x] = (float)((int)threadIdx.x + (int)dc->size[threadIdx.x & 255]);
+    for (int t = threadIdx.x; t < DC2_WARPS * 32; t += blockDim.x)
+      for (int i = t; i < 33; i += DC2_WARPS * 32) T[i] = (float)(i + (int)dc->size[i]);
   }
   __syncthreads();
-  if (FAST && DC_TABLE) {
-    for (int i = threadIdx.x; i < 2 * DC_TAB_HALF + 8; i += DC2_WARPS * 32) Tt[i] = T[1 + bfind_u32((unsigned)abs(i - DC_TAB_HALF))];
+  if (FAST) {
+    for (int t = threadIdx.x; t < DC2_WARPS * 32; t += blockDim.x)
+      for (int i = t; i < 2 * DC_TAB_HALF + 8; i += DC2_WARPS * 32) Tt[i] = T[1 + bfind_u32((unsigned)abs(i - DC_TAB_HALF))];
     __syncthreads();
   }
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -2915,7 +2708,7 @@ __global__ void __launch_bounds__(DC2_WARPS * 32) k_trellis_dc_v2(Geom g, const 
   const int gsel = grp < 3 ? grp : 0;
   const int gbase = gsel * 9;
   const int n_imcu = (c.hib + c.v - 1) / c.v;
-  const int imcu0 = (blockIdx.x * DC2_WARPS + warp) * 3;        // first of this warp's three chains
+  const int imcu0 = (blockIdx.x * (blockDim.x >> 5) + warp) * 3; // first of this warp's three chains
   const int wib = c.wib;
   // back pointers: 9 nibbles per block packed into 5 bytes (candidates 2i, 2i+1 in byte i; byte 4 = candidate 8 in the
   // low nibble, and after the back-track the block's chosen candidate in the high nibble)
@@ -2931,16 +2724,28 @@ __global__ void __launch_bounds__(DC2_WARPS * 32) k_trellis_dc_v2(Geom g, const 
   const size_t comp_rec = (size_t)img * rl.per_image + rl.comp_off[ci];
   const int qhalf = q / 2;
   const unsigned qmul = tc->dc_mul[c.qt]; const int qshift = tc->dc_shift[c.qt];
+  const float vweight = tc->delta_dc_weight;
+  // a block's final DC from its raw DC and its chosen candidate j
+  auto final_dc = [&](const int raw, const int j) {
+    int v = (int)(((unsigned long long)(unsigned)(abs(raw) + qhalf) * qmul) >> qshift) - half + j;
+    if (v >= lim) v = lim - 1;
+    if (v <= -lim) v = -lim + 1;
+    return raw < 0 ? -v : v;
+  };
   int last_dc = 0;                                                // per chain (uniform inside a 9-lane group)
   for (int br = 0; br < c.v; br++) {
+    const bool vert = VERT && br > 0;
     // rows of the three chains; a chain without this row idles on row 0 of the component
     int rowg[3]; bool okg[3];
 #pragma unroll
     for (int gg = 0; gg < 3; gg++) { int r = (imcu0 + gg) * c.v + br; okg[gg] = (imcu0 + gg) < n_imcu && r < c.hib; rowg[gg] = okg[gg] ? r : 0; }
     const bool rowok = grp < 3 && okg[gsel];
-    DcRec nxt[3];
+    DcRec nxt[3]; int up[3];                                      // up: raw DC of the block above (vert)
 #pragma unroll
-    for (int gg = 0; gg < 3; gg++) nxt[gg] = rec[comp_rec + (size_t)rowg[gg] * wib + min(lane, wib - 1)];
+    for (int gg = 0; gg < 3; gg++) {
+      nxt[gg] = rec[comp_rec + (size_t)rowg[gg] * wib + min(lane, wib - 1)];
+      if (vert) up[gg] = rec[comp_rec + (size_t)max(rowg[gg] - 1, 0) * wib + min(lane, wib - 1)].raw_dc;
+    }
     float acc = 0.f;
     // previous block's candidate l is psgn * clamp(pbase + l); for the row's first block every
     // predecessor is last_dc with zero accumulated cost (pstep = 0)
@@ -2953,14 +2758,21 @@ __global__ void __launch_bounds__(DC2_WARPS * 32) k_trellis_dc_v2(Geom g, const 
         const int raw = nxt[gg].raw_dc, x = abs(raw);
         const int qval = (int)(((unsigned long long)(unsigned)(x + qhalf) * qmul) >> qshift);       // (x + q/2) / q, exact
         stage[warp][gg][lane] = make_int4(x, qval - half, 1 + 2 * (raw >> 31), __float_as_int(dc_lambda(nxt[gg].lambda_dc, lambda_from_norm, tc, w0)));
+        // the block above still has the candidate the last back-track chose in its back-pointer entry: this row's steps
+        // overwrite an entry only when they reach its block
+        if (vert) vstage[warp][gg][lane] = make_int2(up[gg] - raw, final_dc(up[gg], btw[((size_t)gg * max_wib + min(bi0 + lane, wib - 1)) * 5 + 4] >> 4) * q);
       }
       __syncwarp();
       if (bi0 + 32 < wib) {
 #pragma unroll
-        for (int gg = 0; gg < 3; gg++) nxt[gg] = rec[comp_rec + (size_t)rowg[gg] * wib + min(bi0 + 32 + lane, wib - 1)];
+        for (int gg = 0; gg < 3; gg++) {
+          nxt[gg] = rec[comp_rec + (size_t)rowg[gg] * wib + min(bi0 + 32 + lane, wib - 1)];
+          if (vert) up[gg] = rec[comp_rec + (size_t)max(rowg[gg] - 1, 0) * wib + min(bi0 + 32 + lane, wib - 1)].raw_dc;
+        }
       }
       const int nstep = min(32, wib - bi0);
       const int4 *sp = &stage[warp][gsel][0];
+      const int2 *vp = &vstage[warp][gsel][0];
 #pragma unroll 1
       for (int st = 0; st < nstep; st++) {
         const int4 r = sp[st];
@@ -2968,15 +2780,21 @@ __global__ void __launch_bounds__(DC2_WARPS * 32) k_trellis_dc_v2(Geom g, const 
         int cd = base + k;
         if (!FAST) { if (cd >= lim) cd = lim - 1; if (cd <= -lim) cd = -lim + 1; }
         const int delta = cd * q - x;
-        const float dist = (float)(delta * delta) * __int_as_float(r.w);
+        float dist = (float)(delta * delta) * __int_as_float(r.w);
         cd *= sgn;
+        if (vert) {
+          const int2 v = vp[st];
+          const int d2 = v.x - (v.y - cd * q);
+          const float vd = (float)(d2 * d2) * __int_as_float(r.w);
+          dist += vweight * (vd - dist);
+        }
         // rate + distortion against every predecessor candidate l (independent of the Viterbi state)
         float rd[9];
         if (FAST) {
           const int D0 = cd - psgn * pbase, dstep = -psgn * pstep;
           // |D0 + dstep l| = |E0 + l| with E0 = -+D0 when dstep = -+1 (every block but a row's first)
           const int E0 = dstep < 0 ? -D0 : D0;
-          if (DC_TABLE && __all_sync(0xffffffffu, pstep != 0 && (unsigned)(E0 + DC_TAB_HALF) < (unsigned)(2 * DC_TAB_HALF))) {
+          if (__all_sync(0xffffffffu, pstep != 0 && (unsigned)(E0 + DC_TAB_HALF) < (unsigned)(2 * DC_TAB_HALF))) {
             const float *tp = Tt + (E0 + DC_TAB_HALF);
 #pragma unroll
             for (int l = 0; l < 9; l++) rd[l] = tp[l] + dist;
@@ -3040,12 +2858,7 @@ __global__ void __launch_bounds__(DC2_WARPS * 32) k_trellis_dc_v2(Geom g, const 
       const uint8_t *btg = btw + (size_t)gg * max_wib * 5;
       int lastv = 0;
       for (int bi = lane; bi < wib && okg[gg]; bi += 32) {
-        DcRec r = rec[comp_rec + (size_t)rowg[gg] * wib + bi];
-        int raw = r.raw_dc, sign = raw >> 31, x = abs(raw);
-        int cdv = (int)(((unsigned long long)(unsigned)(x + qhalf) * qmul) >> qshift) - half + (btg[(size_t)bi * 5 + 4] >> 4);
-        if (cdv >= lim) cdv = lim - 1;
-        if (cdv <= -lim) cdv = -lim + 1;
-        if (sign) cdv = -cdv;
+        const int cdv = final_dc(rec[comp_rec + (size_t)rowg[gg] * wib + bi].raw_dc, btg[(size_t)bi * 5 + 4] >> 4);
         if (write_coef) c.coef[(((size_t)img * c.hpad + rowg[gg]) * c.wpad + bi) * 64] = (int16_t)cdv;
         if (dcq) dcq[comp_rec + (size_t)rowg[gg] * wib + bi] = (int16_t)cdv;
         if (bi == wib - 1) lastv = cdv;
@@ -3058,46 +2871,25 @@ __global__ void __launch_bounds__(DC2_WARPS * 32) k_trellis_dc_v2(Geom g, const 
 }
 
 void launch_trellis_dc(const Geom &g, const TrellisConsts *tc, const DevHuff *tabs, size_t tabs_set_stride,
-                       const DcRec *rec, unsigned long long *bt, const RecLayout &rl, int vertical, int dc_fast, int16_t *dcq, int write_coef,
+                       const DcRec *rec, const RecLayout &rl, int vertical, int dc_fast, int16_t *dcq, int write_coef,
                        int lambda_from_norm, int n, cudaStream_t s)
 {
   int n_imcu = 0, max_wib = 0;
   for (int ci = 0; ci < g.nc; ci++) { n_imcu = max(n_imcu, (g.c[ci].hib + g.c[ci].v - 1) / g.c[ci].v); max_wib = max(max_wib, g.c[ci].wib); }
-  if (vertical) {
-    // trellis_delta_dc_weight > 0 (cjpeg -trellis-dc-ver-weight): the candidates' distortion reads the finished block
-    // row above; only the one-thread-per-chain kernel carries that term (a non-default tuning option)
-    dim3 grid((n_imcu + 63) / 64, n * g.nc);
-    k_trellis_dc<<<grid, 64, 0, s>>>(g, tc, tabs, tabs_set_stride, rec, bt, rl, lambda_from_norm);
-    LAUNCHED();
-    if (dcq) launch_dc_collect(g, rl, dcq, n, s);
-    return;
-  }
-  // warp-cooperative kernel when the chains' back pointers fit in shared memory
-  static const bool use_v1 = getenv("B200JPEG_DC_V1") != nullptr;      // A/B switch
-  size_t smem2 = (size_t)DC2_WARPS * 3 * max_wib * 5;
-  if (!use_v1 && smem2 <= 200 * 1024) {
-    // (per device, so not cached: encoders on several GPUs may live in one process)
-    if (smem2 > 40 * 1024) { cudaFuncSetAttribute(k_trellis_dc_v2<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024); cudaFuncSetAttribute(k_trellis_dc_v2<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024); }
-    dim3 grid((n_imcu + DC2_WARPS * 3 - 1) / (DC2_WARPS * 3), n * g.nc);
-    // the DC quantizer comes from each image's table set (TrellisConsts.dc_mul / dc_shift)
-    if (dc_fast) k_trellis_dc_v2<true><<<grid, DC2_WARPS * 32, smem2, s>>>(g, tc, tabs, tabs_set_stride, rec, rl, max_wib, dcq, write_coef || !dcq, lambda_from_norm);
-    else k_trellis_dc_v2<false><<<grid, DC2_WARPS * 32, smem2, s>>>(g, tc, tabs, tabs_set_stride, rec, rl, max_wib, dcq, write_coef || !dcq, lambda_from_norm);
-    LAUNCHED();
-    return;
-  }
-  int warps = 2;
-  size_t smem = (size_t)warps * 3 * max_wib * 11;
-  if (smem > 200 * 1024) { warps = 1; smem = (size_t)3 * max_wib * 11; }
-  if (smem <= 200 * 1024) {
-    if (smem > 48 * 1024) cudaFuncSetAttribute(k_trellis_dc_warp, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    dim3 grid((n_imcu + warps * 3 - 1) / (warps * 3), n * g.nc);
-    k_trellis_dc_warp<<<grid, warps * 32, smem, s>>>(g, tc, tabs, tabs_set_stride, rec, rl, max_wib, lambda_from_norm);
-  } else {
-    dim3 grid((n_imcu + 63) / 64, n * g.nc);
-    k_trellis_dc<<<grid, 64, 0, s>>>(g, tc, tabs, tabs_set_stride, rec, bt, rl, lambda_from_norm);
-  }
+  // 5 bytes of back pointers per block for each of a warp's 3 chains: DC2_WARPS warps per CTA up to 200 KB, one warp for
+  // wider rows (8188 blocks, 65500 samples, take 122 820 bytes)
+  int warps = DC2_WARPS;
+  size_t smem = (size_t)warps * 3 * max_wib * 5;
+  if (smem > 200 * 1024) { warps = 1; smem = (size_t)3 * max_wib * 5; }
+  auto kern = vertical ? (dc_fast ? k_trellis_dc_v2<true, true> : k_trellis_dc_v2<false, true>)
+                       : (dc_fast ? k_trellis_dc_v2<true, false> : k_trellis_dc_v2<false, false>);
+  // beyond 48 KB with the kernel's static shared memory (under 9 KB); per device, so not cached: encoders on several
+  // GPUs may live in one process
+  if (smem + 9 * 1024 > 48 * 1024) cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+  dim3 grid((n_imcu + warps * 3 - 1) / (warps * 3), n * g.nc);
+  // the DC quantizer comes from each image's table set (TrellisConsts.dc_mul / dc_shift)
+  kern<<<grid, warps * 32, smem, s>>>(g, tc, tabs, tabs_set_stride, rec, rl, max_wib, dcq, write_coef || !dcq, lambda_from_norm);
   LAUNCHED();
-  if (dcq) launch_dc_collect(g, rl, dcq, n, s);
 }
 
 // =====================================================================

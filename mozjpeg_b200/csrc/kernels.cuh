@@ -185,10 +185,10 @@ void launch_trellis_eob_rows(const Geom &g, const DevHuff *tabs, size_t tabs_set
 void launch_qopt_sums(const Geom &g, long long *qsum, int n, cudaStream_t s);
 void launch_qopt_update(long long *qsum, uint16_t *qimg, int n, cudaStream_t s);
 // dcq (or nullptr): dense array of the final DC values, one per real block, indexed like the side records; with it and
-// write_coef == 0 the coefficient planes are not touched (where the kernel in use can do without).  lambda_from_norm:
+// write_coef == 0 the coefficient planes are not touched.  vertical: trellis_delta_dc_weight > 0.  lambda_from_norm:
 // the records hold the forward kernel's norm (behind launch_trellis_ac3), not lambda_dc (behind launch_trellis_ac_band)
 void launch_trellis_dc(const Geom &g, const TrellisConsts *tc, const DevHuff *tabs, size_t tabs_set_stride,
-                       const DcRec *rec, unsigned long long *bt, const RecLayout &rl, int vertical, int dc_fast, int16_t *dcq, int write_coef,
+                       const DcRec *rec, const RecLayout &rl, int vertical, int dc_fast, int16_t *dcq, int write_coef,
                        int lambda_from_norm, int n, cudaStream_t s);
 // DC statistics of a sequential scan from the dense DC array (+ the EOB of every dummy block): with the AC counts the
 // trellis back-track left in `hist`, the scan's complete statistics (encode_mcu_gather, jchuff.c:886-915)

@@ -237,15 +237,19 @@ def test_chunked_pipeline_matches_oracle(built, sw, chunk):
 
 
 def test_very_wide_image_takes_the_fallback_dc_trellis(encoder):
-    """A row of 3750 blocks does not fit the warp-cooperative DC trellis's shared-memory back pointers:
-    the launch falls back to the older kernels, which must give the same bytes."""
+    """The DC trellis keeps 5 bytes of back pointers per block for each of its chains in shared memory.  Rows of 3750
+    blocks need more than the 48 KB default for the two-warp CTAs; rows of 7500 do not fit two warps' chains in 200 KB,
+    and the launch falls back to one warp per CTA.  At that width the vertical-gradient term (-trellis-dc-ver-weight) is
+    also checked on a component with two block rows per iMCU row, sequential and progressive."""
     import mozjpeg_b200 as mj
     from oracle import oracle as O
-    w, h = 30000, 16
-    img = O.synth_image(77, w, h)
-    sw = ["-baseline", "-quality", "75", "-sample", "1x1"]
-    p = mj.params_from_switches(sw, w, h)
-    assert encoder.encode_batch(p, img[None])[0] == O.oracle_encode(p, img).jpeg
+    for w, h, sw in [(30000, 16, ["-baseline", "-quality", "75", "-sample", "1x1"]),
+                     (60000, 16, ["-baseline", "-quality", "75", "-sample", "1x1"]),
+                     (60000, 32, ["-baseline", "-quality", "75", "-sample", "2x2", "-trellis-dc-ver-weight", "1.0"]),
+                     (60000, 32, ["-fastcrush", "-trellis-dc-ver-weight", "1.0"])]:
+        img = O.synth_image(77, w, h)
+        p = mj.params_from_switches(sw, w, h)
+        assert encoder.encode_batch(p, img[None])[0] == O.oracle_encode(p, img).jpeg, (w, h, sw)
 
 
 def test_incompressible_input_grows_the_output_buffers(built):

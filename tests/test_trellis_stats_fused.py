@@ -71,8 +71,10 @@ def test_generic_forward_layout_keeps_the_statistics_pass(enc):
 
 
 def test_very_wide_image(enc):
-    """Rows too long for the warp-cooperative DC trellis: the fallback kernels write the DC values themselves."""
-    _run(enc, BASE + ["-sample", "1x1"], 30000, 16, n=1, seed=77)
+    """Rows of 3750 blocks take the DC trellis's two-warp CTAs beyond the 48 KB shared-memory default, rows of 7500
+    its one-warp CTAs."""
+    for w in (30000, 60000):
+        _run(enc, BASE + ["-sample", "1x1"], w, 16, n=1, seed=77)
 
 
 def test_extreme_content(enc):

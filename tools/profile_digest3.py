@@ -10,7 +10,7 @@ src = os.path.join(ROOT, "gpurun_out", f"launches_{tag}.csv")
 rows = [r for r in csv.reader(open(src)) if r and r[0].isdigit()]
 # kernel -> pipeline stage (the names b200jpeg_last_stage_times reports)
 STAGE = [("k_forward", "forward"), ("k_prep_planes", "smooth_planes"), ("k_import_coefs", "forward"), ("k_dummy", "dummy"), ("k_gather_comp", "trellis_stats"),
-         ("k_sort", "trellis_ac"), ("k_trellis_ac", "trellis_ac"), ("k_trellis_eob", "trellis_ac"), ("k_qopt", "trellis_ac"), ("k_trellis_dc", "trellis_dc"), ("k_dc_collect", "trellis_dc"),
+         ("k_sort", "trellis_ac"), ("k_trellis_ac", "trellis_ac"), ("k_trellis_eob", "trellis_ac"), ("k_qopt", "trellis_ac"), ("k_trellis_dc_v2", "trellis_dc"),
          ("k_gather_seq", "scan_stats"), ("k_gather_prog", "scan_stats"), ("k_seed_hist", "scan_stats"), ("k_gen_tables", "tables"), ("k_block_bits", "block_bits"),
          ("k_scan_layout", "scan_layout"), ("k_zero_stream", "encode"), ("k_encode", "encode"), ("k_stuff", "stuff"), ("k_prog", "eobrun_runs"), ("k_select_al", "select_al")]
 def stage_of(name):
