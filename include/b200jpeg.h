@@ -61,7 +61,8 @@ enum {
   B200JPEG_ERR_CUDA = -4,         /* a CUDA call failed (message via b200jpeg_last_error) */
   B200JPEG_ERR_BUFFER = -5,       /* output buffer too small */
   B200JPEG_ERR_BAD_DCT_COEF = -6, /* ~ JERR_BAD_DCT_COEF (jchuff.c:596-600) */
-  B200JPEG_ERR_STATE = -7         /* ~ JERR_BAD_STATE: streaming calls out of order */
+  B200JPEG_ERR_STATE = -7,        /* ~ JERR_BAD_STATE: streaming calls out of order */
+  B200JPEG_ERR_BAD_SOURCE = -8    /* a source JPEG file is malformed or its entropy-coded data is corrupt (the message names the image) */
 };
 
 /* jpeg_scan_info (jpeglib.h:205-210) */
@@ -196,6 +197,49 @@ int  b200jpeg_total_passes(const b200jpeg_params *p);
  * ph0 * v_ci / vmax rows high.  B200JPEG_ERR_PARAM for ci outside the components or non-positive sizes / factors. */
 int  b200jpeg_yuv_plane_dims(const b200jpeg_params *p, int ci, int *width, int *height);
 
+/* Source-file header parser: the marker segments of a JPEG file as jdmarker.c read_markers walks them (SOI, APPn,
+ * DQT, SOF0/SOF1/SOF2, DHT, DRI, SOS, COM, DNL, EOI), for every scan.  Huffman table definitions are pooled in file
+ * order; a scan names the definitions in force at its SOS.  In a sequential file, slots 0 and 1 still undefined at the
+ * first SOS receive the standard tables, appended to the pool (std_huff_tables, jdhuff.c:819-823).  A component keeps the quantization table its slot held at
+ * the component's first scan (latch_quant_tables, jdinput.c:257-283). */
+#define B200JPEG_MAX_SOURCE_SCANS 128
+#define B200JPEG_MAX_SOURCE_HUFF  64
+typedef struct {
+  int comps_in_scan;
+  int component_index[B200JPEG_MAX_COMPONENTS];
+  int dc_huff[B200JPEG_MAX_COMPONENTS], ac_huff[B200JPEG_MAX_COMPONENTS];   /* index into huff[], -1 when undefined */
+  int dc_tbl_no[B200JPEG_MAX_COMPONENTS], ac_tbl_no[B200JPEG_MAX_COMPONENTS];
+  int Ss, Se, Ah, Al;
+  int restart_interval;                   /* DRI in force at this SOS */
+  size_t data_offset, data_size;          /* entropy-coded bytes: the end of the SOS header up to the first marker that is
+                                             neither RSTn nor a stuffed 0xFF00 (fill bytes before it excluded) */
+} b200jpeg_source_scan;
+typedef struct {
+  int sof;                                /* 0xC0, 0xC1 or 0xC2 */
+  int image_width, image_height, data_precision, num_components;
+  int component_id[B200JPEG_MAX_COMPONENTS], h_samp_factor[B200JPEG_MAX_COMPONENTS], v_samp_factor[B200JPEG_MAX_COMPONENTS];
+  int quant_tbl_no[B200JPEG_MAX_COMPONENTS];
+  uint16_t quant_tbl[B200JPEG_NUM_QUANT_TBLS][B200JPEG_DCTSIZE2];   /* the slots as defined before the first SOS, natural order */
+  int quant_tbl_present[B200JPEG_NUM_QUANT_TBLS];
+  uint16_t comp_quant[B200JPEG_MAX_COMPONENTS][B200JPEG_DCTSIZE2];  /* latched at each component's first scan, natural order */
+  int comp_quant_present[B200JPEG_MAX_COMPONENTS];
+  int saw_JFIF, JFIF_major_version, JFIF_minor_version, density_unit, X_density, Y_density;
+  int saw_Adobe, Adobe_transform;
+  int jpeg_color_space;                   /* the guess of default_decompress_parms (jdapimin.c:111-213) */
+  int has_extra_markers;                  /* COM, or APPn other than JFIF and Adobe */
+  int num_huff;
+  b200jpeg_huff_tbl huff[B200JPEG_MAX_SOURCE_HUFF];
+  int huff_is_dc[B200JPEG_MAX_SOURCE_HUFF];
+  int num_scans;
+  b200jpeg_source_scan scans[B200JPEG_MAX_SOURCE_SCANS];
+} b200jpeg_source_info;
+/* B200JPEG_OK, or B200JPEG_ERR_PARAM for a file that is not a JPEG file or whose header is corrupt,
+ * B200JPEG_ERR_UNSUPPORTED for lossless / hierarchical / arithmetic-coded files and component counts other than 1, 3
+ * and 4, B200JPEG_ERR_BAD_SOURCE for a header the reference refuses (zero height, bad precision or sampling factors, a
+ * Huffman table jpeg_make_d_derived_tbl refuses, a scan naming an undefined table or component, an unknown marker);
+ * the message says which. */
+int  b200jpeg_parse_source(const uint8_t *data, size_t size, b200jpeg_source_info *out);
+
 /* ------------------------------------------------------------------ */
 /* 2. Encode entry points (device path).                               */
 /* ------------------------------------------------------------------ */
@@ -315,6 +359,31 @@ int  b200jpeg_encode_yuv_batch(b200jpeg_encoder *enc, const b200jpeg_params *p,
                                const void *pixels, int pixels_on_device, size_t row_pitch, size_t image_stride,
                                uint8_t *const *planes, int planes_on_device, const size_t *plane_pitch,
                                const size_t *plane_stride, int n_images);
+
+/*
+ * Device entropy decode of sequential Huffman JPEG files (SOF0 / SOF1, 8 and 12 bits; one interleaved scan or several
+ * non-interleaved ones; restart intervals): replaces jpeg_read_coefficients (jdtrans.c:47-124) for a batch of files of
+ * one geometry (size, precision, components and sampling); Huffman tables, quantization tables, restart interval and
+ * scan layout may differ per file.  Progressive (SOF2) files are B200JPEG_ERR_UNSUPPORTED: pass their coefficients
+ * to b200jpeg_encode_batch_coefs instead.  Corrupt entropy-coded data (an invalid code, too few bits for a segment's
+ * MCUs, a wrong RSTn, an unexpected marker) is B200JPEG_ERR_BAD_SOURCE naming the first such image; the reference only
+ * warns there and fills the gap.  Bytes after a segment's last MCU are ignored, like the reference does.
+ *
+ * b200jpeg_decode_coefs_batch writes the real blocks of image i's component ci, natural-order JBLOCKs, to planes[ci] +
+ * i * image_stride_blocks[ci] blocks, height_in_blocks rows of width_in_blocks blocks row_pitch_blocks[ci] apart, in
+ * host or device memory (planes_on_device).
+ */
+int  b200jpeg_decode_coefs_batch(b200jpeg_encoder *enc, const uint8_t *const *files, const size_t *sizes, int n_images,
+                                 int16_t *const *planes, int planes_on_device, const size_t *row_pitch_blocks,
+                                 const size_t *image_stride_blocks);
+/* jpegtran from file bytes: the decode above feeding b200jpeg_encode_batch_coefs_qtables with `p` (what
+ * jpeg_copy_critical_parameters and the switches leave, e.g. from the Python params_for_transcode) and, per image, the
+ * quantization tables the file's components latched.  The finished files are read with b200jpeg_get_output. */
+int  b200jpeg_transcode_batch(b200jpeg_encoder *enc, const b200jpeg_params *p, const uint8_t *const *files,
+                              const size_t *sizes, int n_images);
+/* Synchronisation work of the last decode: the most rounds a CTA of the speculative decoder needed and the number of
+ * subsequences the cross-CTA pass decoded again. */
+int  b200jpeg_last_decode_sync(const b200jpeg_encoder *enc, int *max_cta_rounds, long long *resync_subsequences);
 
 /* b200jpeg_encode_batch, but stops after the entropy-coded bytes are in HBM: no device->host
  * copy, no host-side file assembly.  Used to time the device pipeline alone. */

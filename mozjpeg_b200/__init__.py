@@ -124,6 +124,46 @@ class Encoder:
                     "encode_batch_coefs_qtables")
         return [self.get_output(i) for i in range(n)]
 
+    # -- source files (device entropy decode of sequential Huffman JPEG files) ---------------------------------------
+    @staticmethod
+    def _files(files: Sequence[bytes]):
+        bufs = [bytes(f) for f in files]
+        ptrs = (C.c_void_p * len(bufs))(*[C.cast(C.c_char_p(b), C.c_void_p).value for b in bufs])
+        sizes = (C.c_size_t * len(bufs))(*[len(b) for b in bufs])
+        return bufs, ptrs, sizes
+
+    def read_coefficients(self, files: Sequence[bytes]) -> List[np.ndarray]:
+        """jpeg_read_coefficients for same-geometry files, decoded on the device: per component an (N, hib, wib, 64)
+        int16 array of quantized coefficients in natural order (libjpeg JBLOCKs)."""
+        info = _parse_first(files)
+        bufs, ptrs, sizes = self._files(files)
+        n = len(bufs)
+        hmax = max(info.h_samp_factor[c] for c in range(info.num_components))
+        vmax = max(info.v_samp_factor[c] for c in range(info.num_components))
+        out = []
+        for c in range(info.num_components):
+            wib = -(-info.image_width * info.h_samp_factor[c] // (hmax * 8))
+            hib = -(-info.image_height * info.v_samp_factor[c] // (vmax * 8))
+            out.append(np.empty((n, hib, wib, 64), dtype=np.int16))
+        k = len(out)
+        A.check(_lib.b200jpeg_decode_coefs_batch(self._h, ptrs, sizes, n, (C.c_void_p * k)(*[a.ctypes.data for a in out]), 0,
+                                                 (C.c_size_t * k)(*[a.shape[2] for a in out]),
+                                                 (C.c_size_t * k)(*[a.shape[1] * a.shape[2] for a in out])), "decode_coefs_batch")
+        return out
+
+    def transcode_files(self, p: Params, files: Sequence[bytes]) -> List[bytes]:
+        """b200jpeg_transcode_batch: the files decoded on the device and re-encoded with ``p`` (jpegtran.transcode
+        builds it), each with the quantization tables its components latched."""
+        bufs, ptrs, sizes = self._files(files)
+        A.check(_lib.b200jpeg_transcode_batch(self._h, C.byref(p), ptrs, sizes, len(bufs)), "transcode_batch")
+        return [self.get_output(i) for i in range(len(bufs))]
+
+    def last_decode_sync(self):
+        """(most rounds a CTA of the speculative decoder needed, subsequences the cross-CTA pass decoded again)."""
+        r = C.c_int(0); q = C.c_longlong(0)
+        A.check(_lib.b200jpeg_last_decode_sync(self._h, C.byref(r), C.byref(q)), "last_decode_sync")
+        return r.value, q.value
+
     def encode_batch_qtables_ptr(self, p: Params, ptr: int, on_device: bool, row_pitch: int, image_stride: int,
                                  qtables: np.ndarray) -> None:
         """Raw-pointer form of encode_batch with per-image tables (device tensors, pinned host buffers); one image per
@@ -218,6 +258,14 @@ class Encoder:
         A.check(_lib.b200jpeg_debug_get_huff(self._h, image, scan, int(is_ac), tbl_no, C.byref(h)), "debug_get_huff")
         bits = tuple(h.bits); n = sum(bits[1:])
         return bits, tuple(h.huffval)[:n]
+
+
+def _parse_first(files: Sequence[bytes]) -> A.SourceInfo:
+    if not len(files):
+        raise ValueError("no files")
+    info = A.SourceInfo()
+    A.check(_lib.b200jpeg_parse_source(bytes(files[0]), len(files[0]), C.byref(info)), "parse_source: image 0")
+    return info
 
 
 def cjpeg(switches: Sequence[str], ppm: bytes, encoder: Optional[Encoder] = None) -> bytes:

@@ -31,6 +31,9 @@ PROFILE_FASTEST = 0x2AEA5CB4
 
 OK = 0
 ERR_PARAM, ERR_UNSUPPORTED, ERR_NO_DEVICE, ERR_CUDA, ERR_BUFFER, ERR_BAD_DCT_COEF, ERR_STATE = -1, -2, -3, -4, -5, -6, -7
+ERR_BAD_SOURCE = -8
+MAX_SOURCE_SCANS = 128
+MAX_SOURCE_HUFF = 64
 
 
 class ScanInfo(C.Structure):
@@ -81,6 +84,33 @@ class Params(C.Structure):
         return q
 
 
+class SourceScan(C.Structure):
+    """b200jpeg_source_scan"""
+    _fields_ = [
+        ("comps_in_scan", C.c_int), ("component_index", C.c_int * MAX_COMPONENTS),
+        ("dc_huff", C.c_int * MAX_COMPONENTS), ("ac_huff", C.c_int * MAX_COMPONENTS),
+        ("dc_tbl_no", C.c_int * MAX_COMPONENTS), ("ac_tbl_no", C.c_int * MAX_COMPONENTS),
+        ("Ss", C.c_int), ("Se", C.c_int), ("Ah", C.c_int), ("Al", C.c_int),
+        ("restart_interval", C.c_int), ("data_offset", C.c_size_t), ("data_size", C.c_size_t),
+    ]
+
+
+class SourceInfo(C.Structure):
+    """b200jpeg_source_info: the marker segments of a source JPEG file (b200jpeg_parse_source)."""
+    _fields_ = [
+        ("sof", C.c_int), ("image_width", C.c_int), ("image_height", C.c_int), ("data_precision", C.c_int), ("num_components", C.c_int),
+        ("component_id", C.c_int * MAX_COMPONENTS), ("h_samp_factor", C.c_int * MAX_COMPONENTS), ("v_samp_factor", C.c_int * MAX_COMPONENTS),
+        ("quant_tbl_no", C.c_int * MAX_COMPONENTS),
+        ("quant_tbl", (C.c_uint16 * 64) * NUM_QUANT_TBLS), ("quant_tbl_present", C.c_int * NUM_QUANT_TBLS),
+        ("comp_quant", (C.c_uint16 * 64) * MAX_COMPONENTS), ("comp_quant_present", C.c_int * MAX_COMPONENTS),
+        ("saw_JFIF", C.c_int), ("JFIF_major_version", C.c_int), ("JFIF_minor_version", C.c_int),
+        ("density_unit", C.c_int), ("X_density", C.c_int), ("Y_density", C.c_int),
+        ("saw_Adobe", C.c_int), ("Adobe_transform", C.c_int), ("jpeg_color_space", C.c_int), ("has_extra_markers", C.c_int),
+        ("num_huff", C.c_int), ("huff", HuffTbl * MAX_SOURCE_HUFF), ("huff_is_dc", C.c_int * MAX_SOURCE_HUFF),
+        ("num_scans", C.c_int), ("scans", SourceScan * MAX_SOURCE_SCANS),
+    ]
+
+
 # every symbol include/b200jpeg.h declares (checked by tests/test_abi.py)
 EXPORTS = [
     "b200jpeg_set_defaults", "b200jpeg_default_colorspace", "b200jpeg_set_colorspace",
@@ -94,6 +124,7 @@ EXPORTS = [
     "b200jpeg_kernel_launches", "b200jpeg_last_stage_times", "b200jpeg_debug_get_coefs",
     "b200jpeg_debug_get_huff", "b200jpeg_start_compress", "b200jpeg_write_scanlines",
     "b200jpeg_finish_compress", "b200jpeg_last_error", "b200jpeg_version",
+    "b200jpeg_parse_source", "b200jpeg_decode_coefs_batch", "b200jpeg_transcode_batch", "b200jpeg_last_decode_sync",
 ]
 
 _lib = None
@@ -151,6 +182,11 @@ def load() -> C.CDLL:
     lib.b200jpeg_start_compress.argtypes = [C.c_void_p, P]; lib.b200jpeg_start_compress.restype = C.c_int
     lib.b200jpeg_write_scanlines.argtypes = [C.c_void_p, C.POINTER(C.POINTER(C.c_uint8)), C.c_int]; lib.b200jpeg_write_scanlines.restype = C.c_int
     lib.b200jpeg_finish_compress.argtypes = [C.c_void_p, C.POINTER(C.POINTER(C.c_uint8)), C.POINTER(C.c_size_t)]; lib.b200jpeg_finish_compress.restype = C.c_int
+    PB = C.POINTER(C.c_void_p); PS = C.POINTER(C.c_size_t)
+    lib.b200jpeg_parse_source.argtypes = [C.c_char_p, C.c_size_t, C.POINTER(SourceInfo)]; lib.b200jpeg_parse_source.restype = C.c_int
+    lib.b200jpeg_decode_coefs_batch.argtypes = [C.c_void_p, PB, PS, C.c_int, PB, C.c_int, PS, PS]; lib.b200jpeg_decode_coefs_batch.restype = C.c_int
+    lib.b200jpeg_transcode_batch.argtypes = [C.c_void_p, P, PB, PS, C.c_int]; lib.b200jpeg_transcode_batch.restype = C.c_int
+    lib.b200jpeg_last_decode_sync.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_longlong)]; lib.b200jpeg_last_decode_sync.restype = C.c_int
     lib.b200jpeg_last_error.argtypes = []; lib.b200jpeg_last_error.restype = C.c_char_p
     lib.b200jpeg_version.argtypes = []; lib.b200jpeg_version.restype = C.c_char_p
     _lib = lib

@@ -136,6 +136,14 @@ struct b200jpeg_encoder {
   // streaming shim state
   int st_state = 0, st_next_row = 0;
   b200jpeg_params st_params;
+  // device entropy decode (b200jpeg_decode_coefs_batch / b200jpeg_transcode_batch): descriptors of the last batch, the
+  // upload buffer of its unstuffed segments, and the decoded planes ([n][hib][wib][64] per component, natural order)
+  b200::DecBatch dec;
+  PinBuf h_dec_words, h_dec_stat;
+  DevBuf d_dec_words, d_dec_segs, d_dec_scans, d_dec_tabs, d_dec_out, d_dec_rec, d_dec_pre, d_dec_tsum, d_dec_dcd, d_dec_planes, d_dec_stat;
+  size_t dec_plane_off[4] = {0, 0, 0, 0};
+  cudaEvent_t dec_ev[7] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+  int dec_rounds = 0; long long dec_redone = 0;
 };
 
 // One chunk of a batch: images [i0, i0+n) and where their results go.
@@ -1577,7 +1585,136 @@ static int encode_yuv(b200jpeg_encoder *e, const b200jpeg_params *p, const void 
 
 }  // namespace b200
 
+namespace b200 {
+
+static uint32_t *dec_words_alloc(void *ctx, size_t words)
+{
+  b200jpeg_encoder *e = static_cast<b200jpeg_encoder *>(ctx);
+  return e->h_dec_words.reserve(words * 4) ? nullptr : e->h_dec_words.as<uint32_t>();
+}
+
+static const char *const kDecStages[6] = {"dec_h2d", "dec_sync", "dec_fix", "dec_scan", "dec_write", "dec_dc"};
+
+// the decode stages of the last decode, appended to the stage times
+static void add_decode_stage_times(b200jpeg_encoder *e)
+{
+  for (int k = 0; k < 6; k++) {
+    float ms = 0.f; cudaEventElapsedTime(&ms, e->dec_ev[k], e->dec_ev[k + 1]);
+    e->stage_names.push_back(kDecStages[k]); e->stage_ms.push_back(ms); e->stage_calls.push_back(1);
+  }
+}
+
+// Entropy decode of n sequential files into e->d_dec_planes (jpeg_read_coefficients for the batch).
+static int decode_files(b200jpeg_encoder *e, const uint8_t *const *files, const size_t *sizes, int n)
+{
+  if (!e || !files || !sizes || n <= 0) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
+  CU(cudaSetDevice(e->device));
+  DecBatch &b = e->dec;
+  int rc = build_decode_batch(files, sizes, n, b, dec_words_alloc, e);
+  if (rc) return rc;
+  size_t total = 0;
+  for (int c = 0; c < b.nc; c++) { e->dec_plane_off[c] = total; total += ((size_t)n * b.wib[c] * b.hib[c] * 128 + 255) & ~(size_t)255; }
+  const long long ntiles = (b.nsub + 1023) / 1024;
+  if ((rc = e->d_dec_words.reserve(b.nwords * 4 + 16)) || (rc = e->d_dec_segs.reserve(b.segs.size() * sizeof(DecSeg))) ||
+      (rc = e->d_dec_scans.reserve(b.scans.size() * sizeof(DecScan))) || (rc = e->d_dec_tabs.reserve(b.tabs.size() * sizeof(DecTable))) ||
+      (rc = e->d_dec_out.reserve(sizeof(DecOut))) || (rc = e->d_dec_rec.reserve((size_t)b.nsub * sizeof(DecRec))) ||
+      (rc = e->d_dec_pre.reserve((size_t)b.nsub * 4)) || (rc = e->d_dec_tsum.reserve((size_t)ntiles * 8)) ||
+      (rc = e->d_dec_dcd.reserve((size_t)b.nblocks * 4 + 4)) || (rc = e->d_dec_planes.reserve(total)) ||
+      (rc = e->d_dec_stat.reserve((size_t)n * 4 + 24)) || (rc = e->h_dec_stat.reserve((size_t)n * 4 + 24)))
+    return rc;
+  for (cudaEvent_t &ev : e->dec_ev) if (!ev) CU(cudaEventCreate(&ev));
+  DecOut o; memset(&o, 0, sizeof o);
+  for (int c = 0; c < b.nc; c++) { o.plane[c] = reinterpret_cast<int16_t *>(e->d_dec_planes.as<uint8_t>() + e->dec_plane_off[c]); o.wib[c] = b.wib[c]; o.hib[c] = b.hib[c]; }
+  cudaStream_t s = e->stream;
+  uint8_t *stat = e->d_dec_stat.as<uint8_t>();          // [n] status words, max rounds (int), resynchronised subsequences (u64)
+  const size_t rounds_off = ((size_t)n * 4 + 7) & ~(size_t)7, stat_bytes = rounds_off + 16;
+  CU(cudaEventRecord(e->dec_ev[0], s));
+  CU(cudaMemcpyAsync(e->d_dec_words.p, e->h_dec_words.p, b.nwords * 4, cudaMemcpyHostToDevice, s));
+  CU(cudaMemcpyAsync(e->d_dec_segs.p, b.segs.data(), b.segs.size() * sizeof(DecSeg), cudaMemcpyHostToDevice, s));
+  CU(cudaMemcpyAsync(e->d_dec_scans.p, b.scans.data(), b.scans.size() * sizeof(DecScan), cudaMemcpyHostToDevice, s));
+  CU(cudaMemcpyAsync(e->d_dec_tabs.p, b.tabs.data(), b.tabs.size() * sizeof(DecTable), cudaMemcpyHostToDevice, s));
+  CU(cudaMemcpyAsync(e->d_dec_out.p, &o, sizeof o, cudaMemcpyHostToDevice, s));
+  CU(cudaMemsetAsync(e->d_dec_planes.p, 0, total, s));
+  CU(cudaMemsetAsync(stat, 0, stat_bytes, s));
+  launch_decode(e->d_dec_words.as<uint32_t>(), e->d_dec_segs.as<DecSeg>(), (int)b.segs.size(), e->d_dec_scans.as<DecScan>(), e->d_dec_tabs.as<DecTable>(), b.nsub,
+                e->d_dec_rec.as<DecRec>(), e->d_dec_pre.as<uint32_t>(), e->d_dec_tsum.as<unsigned long long>(), e->d_dec_dcd.as<int>(), e->d_dec_out.as<DecOut>(),
+                reinterpret_cast<uint32_t *>(stat), reinterpret_cast<int *>(stat + rounds_off), reinterpret_cast<unsigned long long *>(stat + rounds_off + 8),
+                e->dec_ev + 1, s);
+  CU(cudaGetLastError());
+  CU(cudaMemcpyAsync(e->h_dec_stat.p, stat, stat_bytes, cudaMemcpyDeviceToHost, s));
+  CU(cudaStreamSynchronize(s));
+  const uint8_t *hs = e->h_dec_stat.as<uint8_t>();
+  e->dec_rounds = *reinterpret_cast<const int *>(hs + rounds_off);
+  e->dec_redone = (long long)*reinterpret_cast<const unsigned long long *>(hs + rounds_off + 8);
+  for (int i = 0; i < n; i++)
+    if (reinterpret_cast<const uint32_t *>(hs)[i]) { set_error("image %d: corrupt entropy-coded data (an invalid Huffman code, or too few bits for a segment's MCUs)", i); return B200JPEG_ERR_BAD_SOURCE; }
+  return B200JPEG_OK;
+}
+
+}  // namespace b200
+
 extern "C" {
+
+int b200jpeg_decode_coefs_batch(b200jpeg_encoder *e, const uint8_t *const *files, const size_t *sizes, int n_images,
+                                int16_t *const *planes, int planes_on_device, const size_t *row_pitch_blocks, const size_t *image_stride_blocks)
+{
+  if (!e || !planes || !row_pitch_blocks || !image_stride_blocks) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
+  int rc = decode_files(e, files, sizes, n_images);
+  if (rc) return rc;
+  const DecBatch &b = e->dec;
+  for (int c = 0; c < b.nc; c++) {
+    const size_t wib = (size_t)b.wib[c], hib = (size_t)b.hib[c];
+    if (!planes[c] || row_pitch_blocks[c] < wib || (n_images > 1 && image_stride_blocks[c] < row_pitch_blocks[c] * (hib - 1) + wib)) {
+      set_error("coefficient plane %d: bad pointer, pitch or stride (needs %zu rows of %zu blocks)", c, hib, wib); return B200JPEG_ERR_PARAM;
+    }
+    const uint8_t *src = e->d_dec_planes.as<uint8_t>() + e->dec_plane_off[c];
+    for (int i = 0; i < n_images; i++)
+      CU(cudaMemcpy2DAsync(reinterpret_cast<uint8_t *>(planes[c]) + (size_t)i * image_stride_blocks[c] * 128, row_pitch_blocks[c] * 128,
+                           src + (size_t)i * hib * wib * 128, wib * 128, wib * 128, hib, planes_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, e->stream));
+  }
+  CU(cudaStreamSynchronize(e->stream));
+  e->pending_marks = 0;
+  e->stage_names.clear(); e->stage_ms.clear(); e->stage_calls.clear();
+  add_decode_stage_times(e);
+  return B200JPEG_OK;
+}
+
+int b200jpeg_transcode_batch(b200jpeg_encoder *e, const b200jpeg_params *p, const uint8_t *const *files, const size_t *sizes, int n_images)
+{
+  if (!e || !p) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
+  int rc = decode_files(e, files, sizes, n_images);
+  if (rc) return rc;
+  const DecBatch &b = e->dec;
+  if (p->num_components != b.nc) { set_error("the parameter block has %d components, the sources %d", p->num_components, b.nc); return B200JPEG_ERR_PARAM; }
+  // each image's quantization tables: what its components latched, in the slots p assigns them
+  std::vector<uint16_t> qt((size_t)n_images * B200JPEG_NUM_QUANT_TBLS * 64);
+  for (int i = 0; i < n_images; i++) {
+    uint16_t *q = qt.data() + (size_t)i * B200JPEG_NUM_QUANT_TBLS * 64;
+    memcpy(q, p->quant_tbl, sizeof p->quant_tbl);
+    for (int c = 0; c < b.nc; c++) {
+      const int slot = p->comp_info[c].quant_tbl_no;
+      if (slot < 0 || slot >= B200JPEG_NUM_QUANT_TBLS || !b.info[i].comp_quant_present[c]) { set_error("image %d: Quantization table 0x%02x was not defined", i, slot); return B200JPEG_ERR_PARAM; }
+      memcpy(q + slot * 64, b.info[i].comp_quant[c], 128);
+    }
+  }
+  int16_t *planes[4]; size_t pitch[4], stride[4];
+  for (int c = 0; c < 4; c++) {
+    planes[c] = c < b.nc ? reinterpret_cast<int16_t *>(e->d_dec_planes.as<uint8_t>() + e->dec_plane_off[c]) : nullptr;
+    pitch[c] = c < b.nc ? (size_t)b.wib[c] : 0; stride[c] = c < b.nc ? (size_t)b.wib[c] * b.hib[c] : 0;
+  }
+  rc = b200jpeg_encode_batch_coefs_qtables(e, p, planes, 1, pitch, stride, qt.data(), n_images);
+  if (rc) return rc;
+  add_decode_stage_times(e);
+  return B200JPEG_OK;
+}
+
+int b200jpeg_last_decode_sync(const b200jpeg_encoder *e, int *max_cta_rounds, long long *resync_subsequences)
+{
+  if (!e) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
+  if (max_cta_rounds) *max_cta_rounds = e->dec_rounds;
+  if (resync_subsequences) *resync_subsequences = e->dec_redone;
+  return B200JPEG_OK;
+}
 
 int b200jpeg_encoder_create(b200jpeg_encoder **enc, int device)
 {
@@ -1621,7 +1758,10 @@ void b200jpeg_encoder_destroy(b200jpeg_encoder *e)
   DevBuf *db[] = {&e->d_src, &e->d_yuv, &e->d_tabs_scan, &e->d_tabs_fixed, &e->d_status, &e->d_out_pos, &e->d_scan_size, &e->d_out, &e->d_qt, &e->d_tc, &e->d_best_al_all, &e->d_qimg_all, &e->d_qset};
   for (DevBuf *b : db) b->release();
   for (int i = 0; i < MAX_ARENAS; i++) e->ar[i].release();
-  PinBuf *pb[] = {&e->h_qt, &e->h_tc, &e->h_fixed, &e->h_status, &e->h_out_pos, &e->h_scan_size, &e->h_tabs, &e->h_stage, &e->h_best_al, &e->h_qinit, &e->h_qimg, &e->h_qset};
+  DevBuf *dd[] = {&e->d_dec_words, &e->d_dec_segs, &e->d_dec_scans, &e->d_dec_tabs, &e->d_dec_out, &e->d_dec_rec, &e->d_dec_pre, &e->d_dec_tsum, &e->d_dec_dcd, &e->d_dec_planes, &e->d_dec_stat};
+  for (DevBuf *b : dd) b->release();
+  for (cudaEvent_t ev : e->dec_ev) if (ev) cudaEventDestroy(ev);
+  PinBuf *pb[] = {&e->h_qt, &e->h_tc, &e->h_fixed, &e->h_status, &e->h_out_pos, &e->h_scan_size, &e->h_tabs, &e->h_stage, &e->h_best_al, &e->h_qinit, &e->h_qimg, &e->h_qset, &e->h_dec_words, &e->h_dec_stat};
   for (PinBuf *b : pb) b->release();
   for (PinBuf &b : e->file_arenas) b.release();
   for (cudaEvent_t ev : e->ev) cudaEventDestroy(ev);

@@ -3972,3 +3972,239 @@ void launch_stuff(const uint32_t *bitbuf, size_t bitbuf_stride_words, const unsi
 }
 
 }  // namespace b200
+
+namespace b200 {
+
+// ================================================================ sequential Huffman decode (jpeg_read_coefficients)
+// Speculative decode with self-synchronisation over DEC_SUB_BITS-bit subsequences of every restart segment (decode.cuh).
+// A subsequence's record holds the (position, state) its last decode started from and where it stopped.  Every
+// segment's first subsequence starts exact; any other is right once its start equals its predecessor's stop.
+
+// the segment holding global subsequence j (segments are ordered by sub0)
+__device__ __forceinline__ int dec_find_seg(const DecSeg *__restrict__ segs, int nsegs, long long j)
+{
+  int lo = 0, hi = nsegs - 1;
+  while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (segs[mid].sub0 <= j) lo = mid; else hi = mid - 1; }
+  return lo;
+}
+
+// one CTA = DEC_CTA consecutive subsequences: decode each from a guessed start (the block's DC, slot 0), then
+// re-decode every subsequence whose start differs from its predecessor's stop until none does (at most DEC_CTA rounds)
+__global__ void __launch_bounds__(DEC_CTA) k_dec_sync(const uint32_t *__restrict__ words, const DecSeg *__restrict__ segs, int nsegs,
+                                                      const DecScan *__restrict__ scans, const DecTable *__restrict__ tabs,
+                                                      DecRec *__restrict__ rec, long long nsub, int *__restrict__ max_rounds)
+{
+  __shared__ uint32_t s_pos[DEC_CTA], s_st[DEC_CTA];
+  const int t = threadIdx.x;
+  const long long j = (long long)blockIdx.x * DEC_CTA + t;
+  const bool live = j < nsub;
+  DecSeg g; g.nbits = 0; g.scan = 0; const uint32_t *w = words; uint32_t a = 0, b = 0;
+  bool seg_first = true;
+  uint32_t in_pos = 0, in_st = 0, pos = 0, st = 0, cnt = 0;
+  if (live) {
+    g = segs[dec_find_seg(segs, nsegs, j)];
+    w = words + g.word0;
+    a = (uint32_t)(j - g.sub0) * DEC_SUB_BITS; b = min(a + DEC_SUB_BITS, g.nbits);
+    seg_first = j == g.sub0;
+    in_pos = pos = a; in_st = st = 0;
+    cnt = dec_run(w, g.nbits, b, pos, st, scans[g.scan], tabs);
+  }
+  s_pos[t] = pos; s_st[t] = st;
+  int rounds = 0;
+  for (;;) {
+    __syncthreads();
+    const bool has_pred = live && !seg_first && t > 0;
+    const uint32_t pp = has_pred ? s_pos[t - 1] : 0, ps = has_pred ? s_st[t - 1] : 0;
+    __syncthreads();
+    const bool change = has_pred && (pp != in_pos || ps != in_st);
+    if (change) {
+      in_pos = pos = pp; in_st = st = ps;
+      cnt = dec_run(w, g.nbits, b, pos, st, scans[g.scan], tabs);
+      s_pos[t] = pos; s_st[t] = st;
+    }
+    if (!__syncthreads_or(change)) break;
+    rounds++;
+  }
+  if (live) { DecRec r; r.in_pos = in_pos; r.in_st = in_st; r.out_pos = pos; r.out_st = st; r.count = cnt; r.pad = 0; rec[j] = r; }
+  if (t == 0 && rounds) atomicMax(max_rounds, rounds);
+}
+
+// one thread per segment: the subsequences that open a CTA inside the segment started from a guess; decode them
+// again from their predecessor's stop until one agrees with what it recorded (the rest of its CTA then holds)
+__global__ void __launch_bounds__(128) k_dec_fix(const uint32_t *__restrict__ words, const DecSeg *__restrict__ segs, int nsegs,
+                                                 const DecScan *__restrict__ scans, const DecTable *__restrict__ tabs,
+                                                 DecRec *__restrict__ rec, unsigned long long *__restrict__ redone)
+{
+  const int si = blockIdx.x * blockDim.x + threadIdx.x;
+  if (si >= nsegs) return;
+  const DecSeg g = segs[si];
+  if (g.nsub == 1) return;
+  const DecScan &sc = scans[g.scan];
+  const uint32_t *w = words + g.word0;
+  const long long end = g.sub0 + g.nsub;
+  unsigned long long n = 0;
+  for (long long j = (g.sub0 / DEC_CTA + 1) * DEC_CTA; j < end; j += DEC_CTA) {
+    long long q = j;
+    for (; q < end; q++) {
+      const DecRec p = rec[q - 1];
+      DecRec r = rec[q];
+      if (r.in_pos == p.out_pos && r.in_st == p.out_st) break;
+      const uint32_t a = (uint32_t)(q - g.sub0) * DEC_SUB_BITS, b = min(a + DEC_SUB_BITS, g.nbits);
+      r.in_pos = p.out_pos; r.in_st = p.out_st;
+      uint32_t pos = r.in_pos, st = r.in_st;
+      r.count = dec_run(w, g.nbits, b, pos, st, sc, tabs);
+      r.out_pos = pos; r.out_st = st;
+      rec[q] = r; n++;
+    }
+  }
+  if (n) atomicAdd(redone, n);
+}
+
+// exclusive scan of the blocks completed per subsequence: in tiles of 1024 (pre), then over the tile sums (tsum)
+__global__ void __launch_bounds__(1024) k_dec_scan_tiles(const DecRec *__restrict__ rec, long long nsub, uint32_t *__restrict__ pre, unsigned long long *__restrict__ tsum)
+{
+  __shared__ uint32_t s_w[32];
+  const long long j = (long long)blockIdx.x * 1024 + threadIdx.x;
+  const uint32_t v = j < nsub ? rec[j].count : 0u;
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  uint32_t x = v;
+  for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
+  if (lane == 31) s_w[wid] = x;
+  __syncthreads();
+  if (wid == 0) {
+    uint32_t y = s_w[lane];
+    for (int o = 1; o < 32; o <<= 1) { const uint32_t z = __shfl_up_sync(0xffffffffu, y, o); if (lane >= o) y += z; }
+    s_w[lane] = y;
+  }
+  __syncthreads();
+  const uint32_t incl = x + (wid ? s_w[wid - 1] : 0u);
+  if (j < nsub) pre[j] = incl - v;
+  if (threadIdx.x == 1023) tsum[blockIdx.x] = incl;
+}
+__global__ void __launch_bounds__(1024) k_dec_scan_sums(unsigned long long *__restrict__ tsum, long long ntiles)
+{
+  __shared__ unsigned long long s_w[32];
+  __shared__ unsigned long long s_carry;
+  if (threadIdx.x == 0) s_carry = 0;
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  for (long long base = 0; base < ntiles; base += 1024) {
+    __syncthreads();
+    const long long i = base + threadIdx.x;
+    const unsigned long long v = i < ntiles ? tsum[i] : 0ull;
+    unsigned long long x = v;
+    for (int o = 1; o < 32; o <<= 1) { const unsigned long long y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
+    if (lane == 31) s_w[wid] = x;
+    __syncthreads();
+    if (wid == 0) {
+      unsigned long long y = s_w[lane];
+      for (int o = 1; o < 32; o <<= 1) { const unsigned long long z = __shfl_up_sync(0xffffffffu, y, o); if (lane >= o) y += z; }
+      s_w[lane] = y;
+    }
+    __syncthreads();
+    const unsigned long long incl = x + (wid ? s_w[wid - 1] : 0ull) + s_carry;
+    if (i < ntiles) tsum[i] = incl - v;
+    __syncthreads();
+    if (threadIdx.x == 1023) s_carry = incl;
+  }
+}
+
+__device__ __forceinline__ unsigned long long dec_prefix(const uint32_t *pre, const unsigned long long *tsum, long long j)
+{
+  return tsum[j >> 10] + pre[j];
+}
+
+__device__ __forceinline__ int16_t *dec_block(const DecOut &o, const DecScan &sc, long long mcu, int slot)
+{
+  const int c = sc.comp[slot];
+  const long long col = (mcu % sc.per_row) * sc.mx[c] + sc.dx[slot], row = (mcu / sc.per_row) * sc.my[c] + sc.dy[slot];
+  if (col >= o.wib[c] || row >= o.hib[c]) return nullptr;          // a dummy block of an interleaved scan
+  return o.plane[c] + (((long long)sc.img * o.hib[c] + row) * o.wib[c] + col) * 64;
+}
+
+// one thread per subsequence: decode again from the synchronised start and write the AC coefficients of every block
+// that starts inside the subsequence (finishing the last one past its end) into the planes (zeroed before), the DC
+// differences into dcd; the segment's last subsequence checks that the segment holds all its MCUs
+__global__ void __launch_bounds__(128) k_dec_write(const uint32_t *__restrict__ words, const DecSeg *__restrict__ segs, int nsegs,
+                                                   const DecScan *__restrict__ scans, const DecTable *__restrict__ tabs,
+                                                   const DecRec *__restrict__ rec, long long nsub, const uint32_t *__restrict__ pre,
+                                                   const unsigned long long *__restrict__ tsum, const DecOut *__restrict__ o, int *__restrict__ dcd,
+                                                   uint32_t *__restrict__ status)
+{
+  const long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= nsub) return;
+  const DecSeg g = segs[dec_find_seg(segs, nsegs, j)];
+  const DecScan &sc = scans[g.scan];
+  const uint32_t *w = words + g.word0;
+  const DecRec r = rec[j];
+  const long long need = (long long)g.nmcu * sc.nb;
+  const unsigned long long seg_base = dec_prefix(pre, tsum, g.sub0);
+  long long blk = (long long)(dec_prefix(pre, tsum, j) - seg_base);
+  if (j == g.sub0 + g.nsub - 1 && blk + (long long)r.count < need) atomicOr(&status[sc.img], 1u);
+  const uint32_t b = min((uint32_t)(j - g.sub0 + 1) * DEC_SUB_BITS, g.nbits);
+  uint32_t pos = r.in_pos, st = r.in_st;
+  bool skip = (st & 127) != 0 && st != DEC_DEAD;         // the block in progress belongs to the predecessor
+  int16_t *dst = nullptr;
+  while (st != DEC_DEAD && blk < need) {
+    if ((st & 127) == 0) {                                // a block starts here
+      if (pos >= b) break;
+      dst = dec_block(*o, sc, g.mcu0 + blk / sc.nb, (int)(st >> 7));
+    }
+    int zz, val; bool done;
+    st = dec_step(w, g.nbits, pos, st, sc, tabs, zz, val, done);
+    if (st == DEC_DEAD) break;
+    if (!skip) {
+      if (zz == 0) dcd[g.blk0 + blk] = val;
+      else if (zz > 0 && dst) dst[c_zz[zz]] = (int16_t)val;
+    }
+    if (done) { blk++; skip = false; }
+  }
+}
+
+// one warp per (segment, scan component): DC values = running sum of the differences over the component's blocks in
+// scan order, dummy blocks included, reset at the segment start (decode_mcu: int accumulation, JCOEF store)
+__global__ void __launch_bounds__(128) k_dec_dc(const DecSeg *__restrict__ segs, int nsegs, const DecScan *__restrict__ scans,
+                                                const int *__restrict__ dcd, const DecOut *__restrict__ o)
+{
+  const long long gw = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (gw >= (long long)nsegs * 4) return;
+  const DecSeg g = segs[gw >> 2];
+  const int k = (int)(gw & 3);
+  const DecScan &sc = scans[g.scan];
+  if (k >= sc.ncomp) return;
+  const int cnt = sc.cnt[k], first = sc.first[k];
+  const long long total = (long long)g.nmcu * cnt;
+  unsigned carry = 0;
+  for (long long base = 0; base < total; base += 32) {
+    const long long e = base + lane;
+    unsigned v = 0; long long m = 0; int slot = 0;
+    if (e < total) { m = e / cnt; slot = first + (int)(e % cnt); v = (unsigned)dcd[g.blk0 + m * sc.nb + slot]; }
+    unsigned x = v;
+    for (int of = 1; of < 32; of <<= 1) { const unsigned y = __shfl_up_sync(0xffffffffu, x, of); if (lane >= of) x += y; }
+    const unsigned s = x + carry;
+    if (e < total) { int16_t *dst = dec_block(*o, sc, g.mcu0 + m, slot); if (dst) dst[0] = (int16_t)s; }
+    carry = __shfl_sync(0xffffffffu, s, 31);
+  }
+}
+
+void launch_decode(const uint32_t *words, const DecSeg *segs, int nsegs, const DecScan *scans, const DecTable *tabs, long long nsub,
+                   DecRec *rec, uint32_t *pre, unsigned long long *tsum, int *dcd, const DecOut *o, uint32_t *status,
+                   int *max_rounds, unsigned long long *redone, cudaEvent_t *marks, cudaStream_t s)
+{
+  const unsigned nb_sync = (unsigned)((nsub + DEC_CTA - 1) / DEC_CTA);
+  const long long ntiles = (nsub + 1023) / 1024;
+  cudaEventRecord(marks[0], s);
+  k_dec_sync<<<nb_sync, DEC_CTA, 0, s>>>(words, segs, nsegs, scans, tabs, rec, nsub, max_rounds); LAUNCHED();
+  cudaEventRecord(marks[1], s);
+  k_dec_fix<<<(nsegs + 127) / 128, 128, 0, s>>>(words, segs, nsegs, scans, tabs, rec, redone); LAUNCHED();
+  cudaEventRecord(marks[2], s);
+  k_dec_scan_tiles<<<(unsigned)ntiles, 1024, 0, s>>>(rec, nsub, pre, tsum); LAUNCHED();
+  k_dec_scan_sums<<<1, 1024, 0, s>>>(tsum, ntiles); LAUNCHED();
+  cudaEventRecord(marks[3], s);
+  k_dec_write<<<(unsigned)((nsub + 127) / 128), 128, 0, s>>>(words, segs, nsegs, scans, tabs, rec, nsub, pre, tsum, o, dcd, status); LAUNCHED();
+  cudaEventRecord(marks[4], s);
+  k_dec_dc<<<(unsigned)(((long long)nsegs * 4 * 32 + 127) / 128), 128, 0, s>>>(segs, nsegs, scans, dcd, o); LAUNCHED();
+  cudaEventRecord(marks[5], s);
+}
+
+}  // namespace b200

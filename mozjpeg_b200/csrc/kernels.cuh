@@ -17,6 +17,7 @@
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
+#include "decode.cuh"
 
 namespace b200 {
 
@@ -235,6 +236,14 @@ void launch_lossless_encode(const Geom &g, const ScanDesc &sd, const uint16_t *d
 // scan search: per-image best point transform of one Al-search group (see k_select_al)
 struct AlSearch { ScanDesc sd[24]; int first, per_al, nband, al_max, nscans_total; };
 void launch_select_al(const Geom &g, const AlSearch &as, const DevHuff *tabs_scan, const uint32_t *scan_size, int n, int *best_al, cudaStream_t s);
+
+// sequential Huffman decode (decode.cuh): k_dec_sync, k_dec_fix, the block-count scan, k_dec_write, k_dec_dc on the
+// batch's descriptors; rec: nsub records, pre: nsub words, tsum: ceil(nsub / 1024) words, dcd: one int per block of
+// every scan (dummy blocks included); o: the destination in device memory; the planes are zeroed by the caller; status[img] bit 0 = corrupt data;
+// max_rounds / redone: synchronisation work (zeroed by the caller); marks: 6 events recorded around the stages
+void launch_decode(const uint32_t *words, const DecSeg *segs, int nsegs, const DecScan *scans, const DecTable *tabs, long long nsub,
+                   DecRec *rec, uint32_t *pre, unsigned long long *tsum, int *dcd, const DecOut *o, uint32_t *status,
+                   int *max_rounds, unsigned long long *redone, cudaEvent_t *marks, cudaStream_t s);
 
 extern unsigned long long g_kernel_launches;
 

@@ -5,10 +5,11 @@ coefficients (jpeg_read_coefficients), copies the critical parameters into a
 fresh compression object (jpeg_copy_critical_parameters, jctrans.c:76-166),
 applies its switches and re-encodes with jpeg_write_coefficients - by default
 with mozjpeg's scan search and optimal Huffman tables, which is the original
-"jpegrescan" use of the library.  The decoder is out of this repo's scope:
-the caller brings the coefficient planes (any JPEG decoder's
-``jpeg_read_coefficients`` output); this file rebuilds the parameter block
-from the source file's header and sequences the same API calls,
+"jpegrescan" use of the library.  The coefficient planes come from the
+library's device entropy decode of sequential Huffman files, or from the
+caller (any JPEG decoder's ``jpeg_read_coefficients`` output, e.g. for
+progressive sources); this file rebuilds the parameter block from the source
+file's header and sequences the same API calls,
 
     jpeg_create_compress ; parse_switches(for_real=FALSE)        jpegtran.c:545-556
     jpeg_copy_critical_parameters                                jpegtran.c:700
@@ -25,7 +26,7 @@ from __future__ import annotations
 
 import ctypes as C
 import struct
-from typing import Dict, List, Sequence, Tuple
+from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 
@@ -54,74 +55,31 @@ class SourceInfo:
         self.has_extra_markers = False                           # COM / APPn other than JFIF and Adobe
 
 
+def parse_source(jpeg: bytes) -> A.SourceInfo:
+    """b200jpeg_parse_source: every marker segment and scan of the file (ValueError with the library's message when it
+    refuses the file)."""
+    out = A.SourceInfo()
+    rc = A.load().b200jpeg_parse_source(bytes(jpeg), len(jpeg), C.byref(out))
+    if rc < 0:
+        raise ValueError(A.load().b200jpeg_last_error().decode("utf-8", "replace"))
+    return out
+
+
 def parse_header(jpeg: bytes) -> SourceInfo:
     """The marker segments up to the first SOS (jdmarker.c read_markers), then the colour-space guess of
-    default_decompress_parms (jdapimin.c:111-213) for 1- and 3-component files."""
+    default_decompress_parms (jdapimin.c:111-213) for 1- and 3-component files; parsed by b200jpeg_parse_source."""
+    r = parse_source(jpeg)
     s = SourceInfo()
-    if jpeg[:2] != b"\xff\xd8":
-        raise ValueError("not a JPEG file")
-    pos = 2
-    while pos + 4 <= len(jpeg):
-        if jpeg[pos] != 0xFF:
-            raise ValueError("corrupt JPEG header")
-        m = jpeg[pos + 1]
-        if m == 0xFF:
-            pos += 1
-            continue
-        ln = struct.unpack(">H", jpeg[pos + 2:pos + 4])[0]
-        seg = jpeg[pos + 4:pos + 2 + ln]
-        if m in (0xC0, 0xC1, 0xC2):
-            s.data_precision, s.image_height, s.image_width, nc = struct.unpack(">BHHB", seg[:6])
-            s.num_components = nc
-            for i in range(nc):
-                cid, hv, tq = seg[6 + 3 * i:9 + 3 * i]
-                s.comps.append((cid, hv >> 4, hv & 15, tq))
-        elif m in (0xC3, 0xC5, 0xC6, 0xC7, 0xC9, 0xCA, 0xCB, 0xCD, 0xCE, 0xCF):
-            raise ValueError("lossless / hierarchical / arithmetic-coded source files are out of scope")
-        elif m == 0xDB:
-            q = 0
-            while q < len(seg):
-                pq, tq = seg[q] >> 4, seg[q] & 15
-                q += 1
-                vals = [0] * 64
-                for k in range(64):
-                    if pq:
-                        v = struct.unpack(">H", seg[q:q + 2])[0]; q += 2
-                    else:
-                        v = seg[q]; q += 1
-                    vals[_ZZ[k]] = v
-                s.quant[tq] = vals
-        elif m == 0xE0 and seg[:5] == b"JFIF\0" and len(seg) >= 14:
-            s.saw_JFIF = True
-            s.JFIF_version = (seg[5], seg[6])
-            s.density = (seg[7], struct.unpack(">H", seg[8:10])[0], struct.unpack(">H", seg[10:12])[0])
-        elif m == 0xEE and seg[:5] == b"Adobe" and len(seg) >= 12:
-            s.saw_Adobe = True
-            s.Adobe_transform = seg[11]
-        elif m == 0xFE or 0xE0 <= m <= 0xEF:
-            s.has_extra_markers = True
-        elif m == 0xDA:
-            break
-        pos += 2 + ln
-    if s.num_components == 1:
-        s.jpeg_color_space = A.CS_GRAYSCALE
-    elif s.num_components == 3:
-        ids = [c[0] for c in s.comps]
-        if s.saw_JFIF:
-            s.jpeg_color_space = A.CS_YCbCr
-        elif s.saw_Adobe:
-            s.jpeg_color_space = A.CS_RGB if s.Adobe_transform == 0 else A.CS_YCbCr
-        elif ids == [1, 2, 3]:
-            s.jpeg_color_space = A.CS_YCbCr
-        elif ids == [0x52, 0x47, 0x42]:
-            s.jpeg_color_space = A.CS_RGB
-        else:
-            s.jpeg_color_space = A.CS_YCbCr
-    elif s.num_components == 4:
-        # Adobe transform 2 marks YCCK, anything else (or no Adobe marker) CMYK
-        s.jpeg_color_space = A.CS_YCCK if s.saw_Adobe and s.Adobe_transform == 2 else A.CS_CMYK
-    else:
-        raise ValueError("only 1-, 3- and 4-component files are on the device path")
+    s.image_width, s.image_height, s.data_precision, s.num_components = r.image_width, r.image_height, r.data_precision, r.num_components
+    s.comps = [(r.component_id[i], r.h_samp_factor[i], r.v_samp_factor[i], r.quant_tbl_no[i]) for i in range(r.num_components)]
+    s.quant = {t: list(r.quant_tbl[t]) for t in range(A.NUM_QUANT_TBLS) if r.quant_tbl_present[t]}
+    s.saw_JFIF = bool(r.saw_JFIF)
+    s.JFIF_version = (r.JFIF_major_version, r.JFIF_minor_version)
+    s.density = (r.density_unit, r.X_density, r.Y_density)
+    s.saw_Adobe = bool(r.saw_Adobe)
+    s.Adobe_transform = r.Adobe_transform
+    s.jpeg_color_space = r.jpeg_color_space
+    s.has_extra_markers = bool(r.has_extra_markers)
     return s
 
 
@@ -229,9 +187,11 @@ def _same_except_quant(a: SourceInfo, b: SourceInfo) -> bool:
     return all(getattr(a, k) == getattr(b, k) for k in keys) and sorted(a.quant) == sorted(b.quant)
 
 
-def transcode(encoder, sources: Sequence[bytes], coef_planes: Sequence[Sequence], switches: Sequence[str]) -> List[bytes]:
+def transcode(encoder, sources: Sequence[bytes], coef_planes: Optional[Sequence[Sequence]], switches: Sequence[str]) -> List[bytes]:
     """``jpegtran <switches>`` on same-shaped source files: sources[i] is the original file, coef_planes[ci] an
-    (N, height_in_blocks, width_in_blocks, 64) int16 array of its quantized coefficients (natural order).
+    (N, height_in_blocks, width_in_blocks, 64) int16 array of its quantized coefficients (natural order), or None:
+    the sources' entropy-coded data is then decoded on the device (sequential Huffman files; a progressive source
+    raises ValueError, pass its planes instead).
     Every source keeps its own quantization tables (its DQT); everything else jpeg_copy_critical_parameters takes
     from a source must match the first one, else ValueError names the first source that differs."""
     infos = [parse_header(s) for s in sources]
@@ -239,12 +199,66 @@ def transcode(encoder, sources: Sequence[bytes], coef_planes: Sequence[Sequence]
         if not _same_except_quant(infos[0], info):
             raise ValueError(f"source {i} differs from source 0 in more than its quantization tables")
     p, prefer_smallest = params_for_transcode(infos[0], switches)
-    qt = np.zeros((len(infos), A.NUM_QUANT_TBLS, 64), dtype=np.uint16)
-    for i, info in enumerate(infos):
-        qt[i] = np.ctypeslib.as_array(p.quant_tbl)
-        for slot, vals in info.quant.items():
-            qt[i, slot] = vals
-    out = encoder.encode_batch_coefs(p, coef_planes, qtables=qt)
+    if coef_planes is None:
+        try:
+            out = encoder.transcode_files(p, sources)
+        except A.B200JpegError as e:
+            if e.code == A.ERR_UNSUPPORTED and "progressive" in str(e):
+                raise ValueError(f"{e}: decode such sources with any JPEG decoder's jpeg_read_coefficients and pass "
+                                 "their planes as coef_planes") from e
+            raise
+    else:
+        qt = np.zeros((len(infos), A.NUM_QUANT_TBLS, 64), dtype=np.uint16)
+        for i, info in enumerate(infos):
+            qt[i] = np.ctypeslib.as_array(p.quant_tbl)
+            for slot, vals in info.quant.items():
+                qt[i, slot] = vals
+        out = encoder.encode_batch_coefs(p, coef_planes, qtables=qt)
     if prefer_smallest and p.compress_profile == A.PROFILE_MAX_COMPRESSION:
         out = [s if len(s) < len(o) else o for s, o in zip(sources, out)]      # jpegtran.c:772-775
     return out
+
+
+def main(argv: Sequence[str] = None) -> int:
+    """``python -m mozjpeg_b200.jpegtran [switches] [-outfile name] file.jpg`` - jpegtran's command line on the device
+    path, from the file's bytes (sequential Huffman sources)."""
+    import sys
+    from . import Encoder
+    args = list(sys.argv[1:] if argv is None else argv)
+    outfile = None
+    switches: List[str] = []
+    files: List[str] = []
+    i = 0
+    while i < len(args):
+        a = args[i]
+        if a.startswith("-") and len(a) > 1:
+            if _keymatch(a[1:], "outfile", 4):
+                if i + 1 >= len(args):
+                    raise UsageError("missing argument for -outfile")
+                outfile = args[i + 1]; i += 2; continue
+            switches.append(a)
+            if (_keymatch(a[1:], "restart", 1) or _keymatch(a[1:], "copy", 2)) and i + 1 < len(args):
+                switches.append(args[i + 1]); i += 1
+        else:
+            files.append(a)
+        i += 1
+    if len(files) != 1:
+        print("usage: python -m mozjpeg_b200.jpegtran [switches] [-outfile name] file.jpg", file=sys.stderr)
+        return 2
+    with open(files[0], "rb") as f:
+        src = f.read()
+    enc = Encoder(0)
+    try:
+        out = transcode(enc, [src], None, switches)[0]
+    finally:
+        enc.close()
+    if outfile:
+        with open(outfile, "wb") as fo:
+            fo.write(out)
+    else:
+        sys.stdout.buffer.write(out)
+    return 0
+
+
+if __name__ == "__main__":
+    raise SystemExit(main())

@@ -335,7 +335,28 @@ def yuv():
     print("wrote", len(cases), "YUV cases;", sum("error" in c for c in cases), "refusals")
 
 
+def decode():
+    """tests/golden/decode_golden.json: for every source of tests/decode_cases.py, the md5 of the file and of the
+    reference's jpeg_read_coefficients planes for it (oracle/_ref/librefshim.so through ctypes)."""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import decode_cases as D
+    cases = []
+    for c in D.CASES:
+        src, _ = D.source(c)
+        ref = O.ref_read_coefs(src)["coefs"]
+        cases.append({"id": c[0], "src_md5": hashlib.md5(src).hexdigest(), "coef_md5": D.md5_planes(ref)})
+    for name in D.EXTRA_IDS:
+        src = D.extra_source(name)
+        ref = O.ref_read_coefs(src)["coefs"]
+        cases.append({"id": name, "src_md5": hashlib.md5(src).hexdigest(), "coef_md5": D.md5_planes(ref)})
+    json.dump({"generator": "tools/make_golden.py --decode", "reference": "mozilla/mozjpeg 5.0.0 (C path, WITH_SIMD=0), oracle/_ref",
+               "cases": cases}, open(os.path.join(GOLD, "decode_golden.json"), "w"), indent=0)
+    print("wrote", len(cases), "decode cases")
+
+
 def main():
+    if "--decode" in sys.argv:
+        return decode()
     if "--yuv" in sys.argv:
         return yuv()
     if "--lossless" in sys.argv:

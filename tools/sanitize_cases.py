@@ -55,5 +55,22 @@ n += len(enc.encode_batch_coefs(pc, [np.zeros((1, (h + 15) // 16 * (2 if ci == 0
 # an interior-tile-rich frame for the TMA path and a wide one
 big = np.stack([synth_image(9, 1024, 256)])
 n += len(enc.encode_batch(mj.params_from_switches(["-baseline", "-quality", "75", "-sample", "2x2"], 1024, 256), big))
+# device entropy decode: good sources, then the malformed ones it must refuse without reading or writing out of bounds
+# (truncated segment, invalid code, wrong RSTn) and garbage after the last MCU, which it accepts
+from mozjpeg_b200 import jpegtran as T
+srcs = enc.encode_batch(mj.params_from_switches(["-revert", "-quality", "90"], w, h), img)
+rst = enc.encode_batch(mj.params_from_switches(["-revert", "-quality", "90", "-restart", "1"], w, h), img[:1])[0]
+n += len(T.transcode(enc, srcs, None, ["-optimize"]))
+n += len(enc.read_coefficients(srcs))
+n += len(enc.read_coefficients([rst]))
+sc = T.parse_source(srcs[0]).scans[0]
+mid = sc.data_offset + sc.data_size // 2
+k = rst.index(b"\xff\xd1", T.parse_source(rst).scans[0].data_offset)
+for bad in (srcs[0][:mid], srcs[0][:mid] + b"\xff\x00" * 8 + srcs[0][mid + 16:], rst[:k + 1] + b"\xd5" + rst[k + 2:]):
+    try:
+        enc.read_coefficients([bad])
+    except mj.B200JpegError as e:
+        assert e.code == mj._abi.ERR_BAD_SOURCE, e
+n += len(enc.read_coefficients([srcs[0][:sc.data_offset + sc.data_size] + bytes(range(1, 200)) + srcs[0][sc.data_offset + sc.data_size:]]))
 print("sanitize cases done:", n, "files, kernel launches", enc.kernel_launches())
 enc.close()
