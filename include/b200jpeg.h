@@ -240,6 +240,43 @@ typedef struct {
  * the message says which. */
 int  b200jpeg_parse_source(const uint8_t *data, size_t size, b200jpeg_source_info *out);
 
+/* Lossless transforms (jpegtran -rotate / -flip / -transpose / -transverse / -crop / -trim / -perfect / -grayscale):
+ * the fields of jpeg_transform_info (transupp.h) that jpegtran's switches set, and what b200jpeg_transform_setup
+ * derives from them.  Transform codes follow JXFORM_CODE, crop kinds JCROP_CODE. */
+enum { B200JPEG_XFORM_NONE = 0, B200JPEG_XFORM_FLIP_H, B200JPEG_XFORM_FLIP_V, B200JPEG_XFORM_TRANSPOSE,
+       B200JPEG_XFORM_TRANSVERSE, B200JPEG_XFORM_ROT_90, B200JPEG_XFORM_ROT_180, B200JPEG_XFORM_ROT_270 };
+enum { B200JPEG_CROP_UNSET = 0, B200JPEG_CROP_POS, B200JPEG_CROP_NEG, B200JPEG_CROP_FORCE, B200JPEG_CROP_REFLECT };
+typedef struct {
+  /* set by the caller (jtransform_parse_crop_spec for the crop fields) */
+  int transform, perfect, trim, force_grayscale;
+  int crop;
+  unsigned crop_width, crop_height, crop_xoffset, crop_yoffset;
+  int crop_width_set, crop_height_set, crop_xoffset_set, crop_yoffset_set;
+  /* filled by b200jpeg_transform_setup */
+  int num_components;                       /* destination components (1 under -grayscale on a YCbCr source) */
+  int output_width, output_height;          /* destination image size */
+  int iMCU_sample_width, iMCU_sample_height;
+  int x_crop_offset, y_crop_offset;         /* in iMCUs of the destination */
+  /* the block mapping of the coefficient import, per destination component ci (source component ci): destination
+   * block (row r, column c) reads, along each destination axis, a = c + x_crop_blocks (resp. r + y_crop_blocks),
+   * mirrored to x_mirror - 1 - a when a < x_mirror (resp. y_mirror); with `transposed` the x axis indexes source
+   * rows and the y axis source columns.  The block's coefficients are transposed with it, and a mirrored axis
+   * negates its odd frequencies.  src_wib / src_hib: the source component's real blocks, the only ones read. */
+  int transposed;
+  int x_crop_blocks[B200JPEG_MAX_COMPONENTS], y_crop_blocks[B200JPEG_MAX_COMPONENTS];
+  int x_mirror[B200JPEG_MAX_COMPONENTS], y_mirror[B200JPEG_MAX_COMPONENTS];
+  int src_wib[B200JPEG_MAX_COMPONENTS], src_hib[B200JPEG_MAX_COMPONENTS];
+} b200jpeg_transform_info;
+/* jtransform_request_workspace + jtransform_adjust_parameters (transupp.c) as jpegtran calls them, for a source whose
+ * header is `src`, on `p` as jpeg_copy_critical_parameters left it: p receives the destination size, 1x1 sampling for
+ * a single component, -grayscale's colour space (component 0 keeps its table slot), and for transposing transforms
+ * swapped sampling factors and transposed quantization tables; t receives the derived fields.  Errors (nothing is
+ * changed): B200JPEG_ERR_PARAM with "transformation is not perfect" under -perfect, "Invalid crop request" for a crop
+ * the reference refuses (JERR_BAD_CROP_SPEC), "Unsupported color conversion request" for -grayscale on a source that
+ * is not YCbCr with 3 components or gray with luma at the largest factors (JERR_CONVERSION_NOTIMPL);
+ * B200JPEG_ERR_UNSUPPORTED for a crop region larger than the image (crop extension). */
+int  b200jpeg_transform_setup(const b200jpeg_source_info *src, b200jpeg_transform_info *t, b200jpeg_params *p);
+
 /* ------------------------------------------------------------------ */
 /* 2. Encode entry points (device path).                               */
 /* ------------------------------------------------------------------ */
@@ -381,6 +418,18 @@ int  b200jpeg_decode_coefs_batch(b200jpeg_encoder *enc, const uint8_t *const *fi
  * quantization tables the file's components latched.  The finished files are read with b200jpeg_get_output. */
 int  b200jpeg_transcode_batch(b200jpeg_encoder *enc, const b200jpeg_params *p, const uint8_t *const *files,
                               const size_t *sizes, int n_images);
+/* The two routes above with a lossless transform applied while the coefficients are imported: `p` and `t` as
+ * b200jpeg_transform_setup left them.  b200jpeg_transcode_batch_transform decodes the files on the device (sequential
+ * sources only) and transposes each image's latched tables for transposing transforms.
+ * b200jpeg_encode_batch_coefs_transform takes planes in the SOURCE geometry (t->src_wib / t->src_hib blocks per
+ * component), e.g. any decoder's jpeg_read_coefficients output for progressive sources; qtables (or NULL for p's) are
+ * the sources' tables, [n_images][4][64] natural order, transposed here like p's were. */
+int  b200jpeg_transcode_batch_transform(b200jpeg_encoder *enc, const b200jpeg_params *p, const b200jpeg_transform_info *t,
+                                        const uint8_t *const *files, const size_t *sizes, int n_images);
+int  b200jpeg_encode_batch_coefs_transform(b200jpeg_encoder *enc, const b200jpeg_params *p, const b200jpeg_transform_info *t,
+                                           const int16_t *const *planes, int planes_on_device,
+                                           const size_t *row_pitch_blocks, const size_t *image_stride_blocks,
+                                           const uint16_t *qtables, int n_images);
 /* Synchronisation work of the last decode: the most rounds a CTA of the speculative decoder needed and the number of
  * subsequences the cross-CTA pass decoded again. */
 int  b200jpeg_last_decode_sync(const b200jpeg_encoder *enc, int *max_cta_rounds, long long *resync_subsequences);

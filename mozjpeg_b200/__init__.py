@@ -158,6 +158,32 @@ class Encoder:
         A.check(_lib.b200jpeg_transcode_batch(self._h, C.byref(p), ptrs, sizes, len(bufs)), "transcode_batch")
         return [self.get_output(i) for i in range(len(bufs))]
 
+    def transcode_files_transform(self, p: Params, t: "A.TransformInfo", files: Sequence[bytes]) -> List[bytes]:
+        """b200jpeg_transcode_batch_transform: transcode_files with the lossless transform ``t`` (b200jpeg_transform_setup
+        filled it and ``p``) applied while the decoded coefficients are imported."""
+        bufs, ptrs, sizes = self._files(files)
+        A.check(_lib.b200jpeg_transcode_batch_transform(self._h, C.byref(p), C.byref(t), ptrs, sizes, len(bufs)), "transcode_batch_transform")
+        return [self.get_output(i) for i in range(len(bufs))]
+
+    def encode_batch_coefs_transform(self, p: Params, t: "A.TransformInfo", planes: Sequence[np.ndarray],
+                                     qtables: Optional[np.ndarray] = None) -> List[bytes]:
+        """b200jpeg_encode_batch_coefs_transform: planes[ci] is an (N, hib, wib, 64) int16 array in the SOURCE's
+        geometry (any decoder's jpeg_read_coefficients output); qtables the sources' tables, (N, 4, 64) or None."""
+        arrs = [np.ascontiguousarray(a, dtype=np.int16) for a in planes[:t.num_components]]
+        n = arrs[0].shape[0]
+        ptrs = (C.c_void_p * len(arrs))(*[a.ctypes.data for a in arrs])
+        pitch = (C.c_size_t * len(arrs))(*[a.strides[1] // 128 for a in arrs])
+        stride = (C.c_size_t * len(arrs))(*[a.strides[0] // 128 for a in arrs])
+        q = None
+        if qtables is not None:
+            q, nq, _ = self._qtables(qtables, n)
+            if nq != n:
+                raise ValueError(f"qtables holds {nq} table sets for {n} images")
+        A.check(_lib.b200jpeg_encode_batch_coefs_transform(self._h, C.byref(p), C.byref(t), ptrs, 0, pitch, stride,
+                                                           None if q is None else q.ctypes.data_as(C.POINTER(C.c_uint16)), n),
+                "encode_batch_coefs_transform")
+        return [self.get_output(i) for i in range(n)]
+
     def last_decode_sync(self):
         """(most rounds a CTA of the speculative decoder needed, subsequences the cross-CTA pass decoded again)."""
         r = C.c_int(0); q = C.c_longlong(0)

@@ -111,6 +111,25 @@ class SourceInfo(C.Structure):
     ]
 
 
+XFORM_NONE, XFORM_FLIP_H, XFORM_FLIP_V, XFORM_TRANSPOSE, XFORM_TRANSVERSE, XFORM_ROT_90, XFORM_ROT_180, XFORM_ROT_270 = range(8)
+CROP_UNSET, CROP_POS, CROP_NEG, CROP_FORCE, CROP_REFLECT = range(5)
+
+
+class TransformInfo(C.Structure):
+    """b200jpeg_transform_info: jpeg_transform_info's switch fields (transupp.h) and what b200jpeg_transform_setup derives."""
+    _fields_ = [
+        ("transform", C.c_int), ("perfect", C.c_int), ("trim", C.c_int), ("force_grayscale", C.c_int),
+        ("crop", C.c_int), ("crop_width", C.c_uint), ("crop_height", C.c_uint), ("crop_xoffset", C.c_uint), ("crop_yoffset", C.c_uint),
+        ("crop_width_set", C.c_int), ("crop_height_set", C.c_int), ("crop_xoffset_set", C.c_int), ("crop_yoffset_set", C.c_int),
+        ("num_components", C.c_int), ("output_width", C.c_int), ("output_height", C.c_int),
+        ("iMCU_sample_width", C.c_int), ("iMCU_sample_height", C.c_int), ("x_crop_offset", C.c_int), ("y_crop_offset", C.c_int),
+        ("transposed", C.c_int),
+        ("x_crop_blocks", C.c_int * MAX_COMPONENTS), ("y_crop_blocks", C.c_int * MAX_COMPONENTS),
+        ("x_mirror", C.c_int * MAX_COMPONENTS), ("y_mirror", C.c_int * MAX_COMPONENTS),
+        ("src_wib", C.c_int * MAX_COMPONENTS), ("src_hib", C.c_int * MAX_COMPONENTS),
+    ]
+
+
 # every symbol include/b200jpeg.h declares (checked by tests/test_abi.py)
 EXPORTS = [
     "b200jpeg_set_defaults", "b200jpeg_default_colorspace", "b200jpeg_set_colorspace",
@@ -125,6 +144,7 @@ EXPORTS = [
     "b200jpeg_debug_get_huff", "b200jpeg_start_compress", "b200jpeg_write_scanlines",
     "b200jpeg_finish_compress", "b200jpeg_last_error", "b200jpeg_version",
     "b200jpeg_parse_source", "b200jpeg_decode_coefs_batch", "b200jpeg_transcode_batch", "b200jpeg_last_decode_sync",
+    "b200jpeg_transform_setup", "b200jpeg_transcode_batch_transform", "b200jpeg_encode_batch_coefs_transform",
 ]
 
 _lib = None
@@ -186,6 +206,10 @@ def load() -> C.CDLL:
     lib.b200jpeg_parse_source.argtypes = [C.c_char_p, C.c_size_t, C.POINTER(SourceInfo)]; lib.b200jpeg_parse_source.restype = C.c_int
     lib.b200jpeg_decode_coefs_batch.argtypes = [C.c_void_p, PB, PS, C.c_int, PB, C.c_int, PS, PS]; lib.b200jpeg_decode_coefs_batch.restype = C.c_int
     lib.b200jpeg_transcode_batch.argtypes = [C.c_void_p, P, PB, PS, C.c_int]; lib.b200jpeg_transcode_batch.restype = C.c_int
+    PT = C.POINTER(TransformInfo)
+    lib.b200jpeg_transform_setup.argtypes = [C.POINTER(SourceInfo), PT, P]; lib.b200jpeg_transform_setup.restype = C.c_int
+    lib.b200jpeg_transcode_batch_transform.argtypes = [C.c_void_p, P, PT, PB, PS, C.c_int]; lib.b200jpeg_transcode_batch_transform.restype = C.c_int
+    lib.b200jpeg_encode_batch_coefs_transform.argtypes = [C.c_void_p, P, PT, PB, C.c_int, PS, PS, Q, C.c_int]; lib.b200jpeg_encode_batch_coefs_transform.restype = C.c_int
     lib.b200jpeg_last_decode_sync.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_longlong)]; lib.b200jpeg_last_decode_sync.restype = C.c_int
     lib.b200jpeg_last_error.argtypes = []; lib.b200jpeg_last_error.restype = C.c_char_p
     lib.b200jpeg_version.argtypes = []; lib.b200jpeg_version.restype = C.c_char_p

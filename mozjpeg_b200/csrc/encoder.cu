@@ -144,6 +144,7 @@ struct b200jpeg_encoder {
   size_t dec_plane_off[4] = {0, 0, 0, 0};
   cudaEvent_t dec_ev[7] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
   int dec_rounds = 0; long long dec_redone = 0;
+  CoefXform xform{};                            // the coefficient import's block mapping in the current batch (all zero: a copy)
 };
 
 // One chunk of a batch: images [i0, i0+n) and where their results go.
@@ -652,7 +653,7 @@ static int run_pipeline(b200jpeg_encoder *e, const ChunkIO &io, Timer &tm)
   // of B200JPEG_KEEP_PLAIN read them, and keep the separate statistics pass)
   bool fwd_stats = false;
   if (g.raw_in == 2) {
-    launch_import_coefs(g, n, s);
+    launch_import_coefs(g, e->xform, n, s);
   } else {
   if (pl.smooth && !g.raw_in) {
     // input smoothing: conversion + context-mode downsampling as a pre-pass; the forward kernel then reads planes
@@ -1276,7 +1277,9 @@ static int choose_chunk(const b200jpeg_encoder *e, const Plan &pl, int n_images,
 }
 
 // raw-data input (jpeg_write_raw_data): one plane per component instead of interleaved pixels
-struct RawDesc { const uint8_t *plane[4]; size_t pitch[4], stride[4]; bool coefs; };   // pitch, stride in bytes; coefs: planes hold JBLOCK rows
+// pitch, stride in bytes; coefs: planes hold JBLOCK rows; xf (coefficients only, or nullptr): a lossless transform's
+// mapping, the planes are then in the source's geometry
+struct RawDesc { const uint8_t *plane[4]; size_t pitch[4], stride[4]; bool coefs; const b200jpeg_transform_info *xf; };
 
 // The batch's quantization table sets: without per-image tables one set, the parameter block's; with them
 // (qtables: [n_images][4][64], natural order, the slots quant_tbl_present names) the distinct ones, in order of first
@@ -1342,8 +1345,16 @@ static int encode_common(b200jpeg_encoder *e, const b200jpeg_params *p, const vo
     Geom &g = pl.g;
     if (p->trellis_quant) { set_error("coefficient input: trellis quantization needs the unquantized coefficients (trellis_quant must be 0, as jpeg_copy_critical_parameters sets it)"); return B200JPEG_ERR_PARAM; }
     g.raw_in = 2;
+    e->xform = CoefXform{};
+    if (const b200jpeg_transform_info *t = raw->xf) {
+      e->xform.transposed = t->transposed;
+      for (int ci = 0; ci < g.nc; ci++) {
+        e->xform.x_crop[ci] = t->x_crop_blocks[ci]; e->xform.y_crop[ci] = t->y_crop_blocks[ci];
+        e->xform.x_mirror[ci] = t->x_mirror[ci]; e->xform.y_mirror[ci] = t->y_mirror[ci];
+      }
+    }
     for (int ci = 0; ci < g.nc; ci++) {
-      const size_t rows = (size_t)g.c[ci].hib, cols = (size_t)g.c[ci].wib * 128;
+      const size_t rows = (size_t)(raw->xf ? raw->xf->src_hib[ci] : g.c[ci].hib), cols = (size_t)(raw->xf ? raw->xf->src_wib[ci] : g.c[ci].wib) * 128;
       if (!raw->plane[ci] || raw->pitch[ci] < cols || (n_images > 1 && !(shared_ok && raw->stride[ci] == 0) && raw->stride[ci] < raw->pitch[ci] * (rows - 1) + cols)) { set_error("coefficient plane %d: bad pointer, pitch or stride (needs %zu rows of %zu blocks)", ci, rows, cols / 128); return B200JPEG_ERR_PARAM; }
       raw_plane_bytes[ci] = raw->pitch[ci] * (rows - 1) + cols;
       raw_total[ci] = raw->stride[ci] * (size_t)(n_images - 1) + raw_plane_bytes[ci];
@@ -1651,6 +1662,84 @@ static int decode_files(b200jpeg_encoder *e, const uint8_t *const *files, const 
   return B200JPEG_OK;
 }
 
+// a transform description must be the one b200jpeg_transform_setup left beside p
+static int check_xform(const b200jpeg_params *p, const b200jpeg_transform_info *t)
+{
+  if (t->num_components != p->num_components || t->output_width != p->image_width || t->output_height != p->image_height) {
+    set_error("the transform description (%d components, %dx%d) does not match the parameter block (%d components, %dx%d): run b200jpeg_transform_setup on it",
+              t->num_components, t->output_width, t->output_height, p->num_components, p->image_width, p->image_height);
+    return B200JPEG_ERR_PARAM;
+  }
+  return B200JPEG_OK;
+}
+
+// transpose_critical_parameters (transupp.c:1858-1871) on every slot of n table sets ([n][4][64], natural order)
+static void transpose_qsets(uint16_t *q, int n)
+{
+  for (size_t s = 0; s < (size_t)n * B200JPEG_NUM_QUANT_TBLS; s++)
+    for (int i = 0; i < 8; i++)
+      for (int j = 0; j < i; j++) std::swap(q[s * 64 + i * 8 + j], q[s * 64 + j * 8 + i]);
+}
+
+static int encode_coefs_xform(b200jpeg_encoder *enc, const b200jpeg_params *p, const b200jpeg_transform_info *t, const int16_t *const *planes, int planes_on_device,
+                              const size_t *row_pitch_blocks, const size_t *image_stride_blocks, const uint16_t *qtables, int n_images)
+{
+  if (!enc || !p || !t || !planes || !row_pitch_blocks || !image_stride_blocks || n_images <= 0) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
+  int rc = check_xform(p, t);
+  if (rc) return rc;
+  RawDesc rd; memset(&rd, 0, sizeof rd); rd.coefs = true; rd.xf = t;
+  for (int ci = 0; ci < p->num_components && ci < 4; ci++) {
+    rd.plane[ci] = reinterpret_cast<const uint8_t *>(planes[ci]); rd.pitch[ci] = row_pitch_blocks[ci] * 128; rd.stride[ci] = image_stride_blocks[ci] * 128;
+  }
+  std::vector<uint16_t> qt;
+  if (qtables) {
+    qt.assign(qtables, qtables + (size_t)n_images * B200JPEG_NUM_QUANT_TBLS * 64);
+    if (t->transposed) transpose_qsets(qt.data(), n_images);
+  }
+  b200jpeg_params q = *p;                 // as b200jpeg_encode_batch_coefs
+  q.overshoot_deringing = 0; q.smoothing_factor = 0; q.dct_method = B200JPEG_DCT_ISLOW;
+  return encode_common(enc, &q, nullptr, planes_on_device, 0, 0, n_images, false, &rd, qtables ? qt.data() : nullptr);
+}
+
+// jpegtran from file bytes (b200jpeg_transcode_batch, and with a transform b200jpeg_transcode_batch_transform)
+static int transcode_files(b200jpeg_encoder *e, const b200jpeg_params *p, const b200jpeg_transform_info *t, const uint8_t *const *files, const size_t *sizes, int n_images)
+{
+  if (!e || !p) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
+  int rc = decode_files(e, files, sizes, n_images);
+  if (rc) return rc;
+  const DecBatch &b = e->dec;
+  // -grayscale keeps the first component of a 3-component source; every other destination has the source's components
+  const bool comps_ok = p->num_components == b.nc || (t && t->force_grayscale && p->num_components == 1);
+  if (!comps_ok) { set_error("the parameter block has %d components, the sources %d", p->num_components, b.nc); return B200JPEG_ERR_PARAM; }
+  if (t) {
+    for (int c = 0; c < p->num_components; c++)
+      if (t->src_wib[c] != b.wib[c] || t->src_hib[c] != b.hib[c]) { set_error("the sources' component %d has %dx%d blocks, the transform description %dx%d", c, b.wib[c], b.hib[c], t->src_wib[c], t->src_hib[c]); return B200JPEG_ERR_PARAM; }
+  }
+  // each image's quantization tables: what its components latched, in the slots p assigns them; in the source's
+  // orientation (p's are transposed back), encode_coefs_xform transposes them with the blocks
+  std::vector<uint16_t> qt((size_t)n_images * B200JPEG_NUM_QUANT_TBLS * 64);
+  for (int i = 0; i < n_images; i++) {
+    uint16_t *q = qt.data() + (size_t)i * B200JPEG_NUM_QUANT_TBLS * 64;
+    memcpy(q, p->quant_tbl, sizeof p->quant_tbl);
+    if (t && t->transposed) transpose_qsets(q, 1);
+    for (int c = 0; c < p->num_components; c++) {
+      const int slot = p->comp_info[c].quant_tbl_no;
+      if (slot < 0 || slot >= B200JPEG_NUM_QUANT_TBLS || !b.info[i].comp_quant_present[c]) { set_error("image %d: Quantization table 0x%02x was not defined", i, slot); return B200JPEG_ERR_PARAM; }
+      memcpy(q + slot * 64, b.info[i].comp_quant[c], 128);
+    }
+  }
+  int16_t *planes[4]; size_t pitch[4], stride[4];
+  for (int c = 0; c < 4; c++) {
+    planes[c] = c < b.nc ? reinterpret_cast<int16_t *>(e->d_dec_planes.as<uint8_t>() + e->dec_plane_off[c]) : nullptr;
+    pitch[c] = c < b.nc ? (size_t)b.wib[c] : 0; stride[c] = c < b.nc ? (size_t)b.wib[c] * b.hib[c] : 0;
+  }
+  rc = t ? encode_coefs_xform(e, p, t, planes, 1, pitch, stride, qt.data(), n_images)
+         : b200jpeg_encode_batch_coefs_qtables(e, p, planes, 1, pitch, stride, qt.data(), n_images);
+  if (rc) return rc;
+  add_decode_stage_times(e);
+  return B200JPEG_OK;
+}
+
 }  // namespace b200
 
 extern "C" {
@@ -1681,31 +1770,14 @@ int b200jpeg_decode_coefs_batch(b200jpeg_encoder *e, const uint8_t *const *files
 
 int b200jpeg_transcode_batch(b200jpeg_encoder *e, const b200jpeg_params *p, const uint8_t *const *files, const size_t *sizes, int n_images)
 {
-  if (!e || !p) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
-  int rc = decode_files(e, files, sizes, n_images);
-  if (rc) return rc;
-  const DecBatch &b = e->dec;
-  if (p->num_components != b.nc) { set_error("the parameter block has %d components, the sources %d", p->num_components, b.nc); return B200JPEG_ERR_PARAM; }
-  // each image's quantization tables: what its components latched, in the slots p assigns them
-  std::vector<uint16_t> qt((size_t)n_images * B200JPEG_NUM_QUANT_TBLS * 64);
-  for (int i = 0; i < n_images; i++) {
-    uint16_t *q = qt.data() + (size_t)i * B200JPEG_NUM_QUANT_TBLS * 64;
-    memcpy(q, p->quant_tbl, sizeof p->quant_tbl);
-    for (int c = 0; c < b.nc; c++) {
-      const int slot = p->comp_info[c].quant_tbl_no;
-      if (slot < 0 || slot >= B200JPEG_NUM_QUANT_TBLS || !b.info[i].comp_quant_present[c]) { set_error("image %d: Quantization table 0x%02x was not defined", i, slot); return B200JPEG_ERR_PARAM; }
-      memcpy(q + slot * 64, b.info[i].comp_quant[c], 128);
-    }
-  }
-  int16_t *planes[4]; size_t pitch[4], stride[4];
-  for (int c = 0; c < 4; c++) {
-    planes[c] = c < b.nc ? reinterpret_cast<int16_t *>(e->d_dec_planes.as<uint8_t>() + e->dec_plane_off[c]) : nullptr;
-    pitch[c] = c < b.nc ? (size_t)b.wib[c] : 0; stride[c] = c < b.nc ? (size_t)b.wib[c] * b.hib[c] : 0;
-  }
-  rc = b200jpeg_encode_batch_coefs_qtables(e, p, planes, 1, pitch, stride, qt.data(), n_images);
-  if (rc) return rc;
-  add_decode_stage_times(e);
-  return B200JPEG_OK;
+  return b200::transcode_files(e, p, nullptr, files, sizes, n_images);
+}
+
+int b200jpeg_transcode_batch_transform(b200jpeg_encoder *e, const b200jpeg_params *p, const b200jpeg_transform_info *t,
+                                       const uint8_t *const *files, const size_t *sizes, int n_images)
+{
+  if (!t) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
+  return b200::transcode_files(e, p, t, files, sizes, n_images);
 }
 
 int b200jpeg_last_decode_sync(const b200jpeg_encoder *e, int *max_cta_rounds, long long *resync_subsequences)
@@ -1872,6 +1944,13 @@ int b200jpeg_encode_batch_coefs_qtables(b200jpeg_encoder *enc, const b200jpeg_pa
   b200jpeg_params q = *p;                 // as b200jpeg_encode_batch_coefs
   q.overshoot_deringing = 0; q.smoothing_factor = 0; q.dct_method = B200JPEG_DCT_ISLOW;
   return encode_common(enc, &q, nullptr, planes_on_device, 0, 0, n_images, false, &rd, qtables);
+}
+
+int b200jpeg_encode_batch_coefs_transform(b200jpeg_encoder *enc, const b200jpeg_params *p, const b200jpeg_transform_info *t,
+                                          const int16_t *const *planes, int planes_on_device,
+                                          const size_t *row_pitch_blocks, const size_t *image_stride_blocks, const uint16_t *qtables, int n_images)
+{
+  return b200::encode_coefs_xform(enc, p, t, planes, planes_on_device, row_pitch_blocks, image_stride_blocks, qtables, n_images);
 }
 
 int b200jpeg_get_output(b200jpeg_encoder *e, int i, const uint8_t **data, size_t *size)

@@ -1277,8 +1277,30 @@ void launch_forward(const Geom &g, const uint8_t *src, const QuantTables *qt, in
 // blocks are libjpeg JBLOCKs (natural order, width_in_blocks x height_in_blocks per component); they go into the
 // padded zigzag-order planes every later stage reads.  Dummy blocks are made by k_dummy as on the pixel path: the
 // transcoder's rule (DC of the previous block of the MCU, jctrans.c:352-362) gives the same values.
+// A lossless transform (jpegtran's do_* routines, transupp.c:727-1357) is this copy's gather: the destination block
+// picks its source block by the CoefXform mapping and its coefficients through one of eight in-block operations.
 // =====================================================================
-__global__ void __launch_bounds__(256) k_import_coefs(Geom g)
+// in-block operation op = transposed * 4 + (x axis mirrored) * 2 + (y axis mirrored): for destination zigzag position
+// k, the natural source index | 0x100 when the value is negated (a mirrored axis negates its odd frequencies).  Kept in
+// global memory and read through L1: a warp's 32 lanes read 32 different entries, which __constant__ memory would
+// serialise.
+struct XfTab { unsigned short e[8][64]; };
+constexpr XfTab make_xf_tab()
+{
+  constexpr unsigned char zz[64] = {0, 1, 8, 16, 9, 2, 3, 10, 17, 24, 32, 25, 18, 11, 4, 5, 12, 19, 26, 33, 40, 48, 41, 34, 27, 20, 13, 6, 7, 14, 21, 28,
+                                    35, 42, 49, 56, 57, 50, 43, 36, 29, 22, 15, 23, 30, 37, 44, 51, 58, 59, 52, 45, 38, 31, 39, 46, 53, 60, 61, 54, 47, 55, 62, 63};
+  XfTab t{};
+  for (int op = 0; op < 8; op++)
+    for (int k = 0; k < 64; k++) {
+      const int n = zz[k], r = n >> 3, c = n & 7;
+      const int neg = (((op >> 1) & 1) & c) ^ ((op & 1) & r);
+      t.e[op][k] = (unsigned short)(((op & 4) ? c * 8 + r : n) | (neg << 8));
+    }
+  return t;
+}
+__device__ const XfTab g_xf = make_xf_tab();
+
+__global__ void __launch_bounds__(256) k_import_coefs(Geom g, const __grid_constant__ CoefXform xf)
 {
   const int ci = blockIdx.y % g.nc, img = blockIdx.y / g.nc;
   const CompGeom &c = g.c[ci];
@@ -1287,15 +1309,22 @@ __global__ void __launch_bounds__(256) k_import_coefs(Geom g)
   if (t >= nblk * 64) return;
   const long long b = t >> 6; const int k = (int)(t & 63);
   const int row = (int)(b / c.wib), col = (int)(b - (long long)row * c.wib);
-  const int16_t *src = reinterpret_cast<const int16_t *>(g.plane[ci] + (size_t)img * g.plane_stride[ci] + (size_t)row * g.plane_pitch[ci]) + (size_t)col * 64;
-  c.coef[(((size_t)img * c.hpad + row) * c.wpad + col) * 64 + k] = src[c_zz[k]];
+  int ax = col + xf.x_crop[ci], ay = row + xf.y_crop[ci];
+  const int xm = ax < xf.x_mirror[ci], ym = ay < xf.y_mirror[ci];
+  if (xm) ax = xf.x_mirror[ci] - 1 - ax;
+  if (ym) ay = xf.y_mirror[ci] - 1 - ay;
+  const int sr = xf.transposed ? ax : ay, sc = xf.transposed ? ay : ax;
+  const int e = __ldg(&g_xf.e[xf.transposed * 4 + xm * 2 + ym][k]);
+  const int16_t *src = reinterpret_cast<const int16_t *>(g.plane[ci] + (size_t)img * g.plane_stride[ci] + (size_t)sr * g.plane_pitch[ci]) + (size_t)sc * 64;
+  const int16_t v = src[e & 63];
+  c.coef[(((size_t)img * c.hpad + row) * c.wpad + col) * 64 + k] = (e & 0x100) ? (int16_t)-v : v;
 }
-void launch_import_coefs(const Geom &g, int n, cudaStream_t s)
+void launch_import_coefs(const Geom &g, const CoefXform &xf, int n, cudaStream_t s)
 {
   long long mb = 0;
   for (int ci = 0; ci < g.nc; ci++) mb = max(mb, (long long)g.c[ci].wib * g.c[ci].hib);
   dim3 grid((unsigned)((mb * 64 + 255) / 256), n * g.nc);
-  k_import_coefs<<<grid, 256, 0, s>>>(g);
+  k_import_coefs<<<grid, 256, 0, s>>>(g, xf);
   LAUNCHED();
 }
 

@@ -152,7 +152,10 @@ void launch_prep_planes(const Geom &g, const uint8_t *src, int smoothing_factor,
 // components 1, 2 (g.nc == 3) 1x1; 8-bit samples
 struct YuvOut { uint8_t *p[3]; size_t pitch[3], stride[3]; int pw[3], ph[3]; };
 void launch_encode_yuv(const Geom &g, const uint8_t *src, const YuvOut &out, int n, cudaStream_t s);
-void launch_import_coefs(const Geom &g, int n, cudaStream_t s);     // raw_in == 2: planes hold JBLOCK rows
+// raw_in == 2: planes hold JBLOCK rows.  xf: the block mapping of a lossless transform (b200jpeg_transform_info, per
+// component; all zero = the plain copy): the planes are then in the source's geometry, pitch and stride
+struct CoefXform { int transposed; int x_crop[4], y_crop[4], x_mirror[4], y_mirror[4]; };
+void launch_import_coefs(const Geom &g, const CoefXform &xf, int n, cudaStream_t s);
 // Trellis-phase statistics counted by the tiled forward kernel (fs.hist != nullptr, only where forward_tiled() holds):
 // every real block's AC symbols go into hist [img*nc + ci][4 + ac_tbl][sym] (zeroed by the caller), its plain-quantized
 // DC into dcq (indexed like the side records), JERR_BAD_DCT_COEF into status; the coefficient planes are not written

@@ -354,7 +354,38 @@ def decode():
     print("wrote", len(cases), "decode cases")
 
 
+def transform():
+    """tests/golden/transform_golden.json: the reference's own jpegtran on the sources of tests/transform_cases.py, per
+    case the output's md5, size, SOF fields and component tables, or the reference's refusal."""
+    import subprocess
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import transform_cases as X
+    srcs = {sid: X.source(sid)[0] for sid in X.source_ids()}
+
+    def run(cid, sid, sw):
+        rec = {"id": cid, "source": sid, "switches": sw}
+        r = subprocess.run([os.path.join(O.REF_DIR, "jpegtran"), *sw], input=srcs[sid], capture_output=True)
+        if r.returncode != 0:
+            msg = r.stderr.decode().strip().splitlines()[0] if r.stderr else f"exit {r.returncode}"
+            rec["error"] = msg.replace(os.path.join(O.REF_DIR, "jpegtran"), "jpegtran")
+            return rec
+        w, h, comps, qmd5 = X.sof_dqt(r.stdout)
+        rec.update(md5=X.md5(r.stdout), size=len(r.stdout), sof=[w, h, comps], qt_md5=qmd5)
+        return rec
+
+    cases = [run(*c) for c in X.main_matrix() + X.other_cases()]
+    cases += [run(f"mixed_{sid}", sid, ["-rotate", "90"]) for sid in X.mixed_ids()]
+    cases += [run(f"prog_{'_'.join(a.lstrip('-') for a in sw)}", "prog_420", sw) for sw in (["-rotate", "90"], ["-crop", "64x48+5+3", "-transpose"])]
+    refusals = [run(f"refuse{k}", sid, sw) for k, (sid, sw) in enumerate(X.REFUSALS)]
+    json.dump({"generator": "tools/make_golden.py --transform", "reference": "mozilla/mozjpeg 5.0.0 (C path, WITH_SIMD=0), oracle/_ref",
+               "sources": {sid: X.md5(b) for sid, b in srcs.items()}, "cases": cases, "refusals": refusals},
+              open(os.path.join(GOLD, "transform_golden.json"), "w"), indent=0)
+    print("wrote", len(cases), "transform cases,", sum("error" in c for c in cases), "refused;", len(refusals), "refusals")
+
+
 def main():
+    if "--transform" in sys.argv:
+        return transform()
     if "--decode" in sys.argv:
         return decode()
     if "--yuv" in sys.argv:

@@ -61,6 +61,11 @@ from mozjpeg_b200 import jpegtran as T
 srcs = enc.encode_batch(mj.params_from_switches(["-revert", "-quality", "90"], w, h), img)
 rst = enc.encode_batch(mj.params_from_switches(["-revert", "-quality", "90", "-restart", "1"], w, h), img[:1])[0]
 n += len(T.transcode(enc, srcs, None, ["-optimize"]))
+# lossless transforms in the coefficient import: partial edge iMCUs (rotations, transverse), crops, gray output, and
+# caller planes in the source's geometry
+for tsw in (["-rotate", "90"], ["-transverse"], ["-rotate", "180", "-crop", "64x48+5+3"], ["-grayscale", "-flip", "horizontal"]):
+    n += len(T.transcode(enc, srcs, None, tsw))
+n += len(T.transcode(enc, srcs[:1], enc.read_coefficients(srcs[:1]), ["-rotate", "270", "-trim"]))
 n += len(enc.read_coefficients(srcs))
 n += len(enc.read_coefficients([rst]))
 sc = T.parse_source(srcs[0]).scans[0]
