@@ -434,6 +434,36 @@ int  b200jpeg_encode_batch_coefs_transform(b200jpeg_encoder *enc, const b200jpeg
  * subsequences the cross-CTA pass decoded again. */
 int  b200jpeg_last_decode_sync(const b200jpeg_encoder *enc, int *max_cta_rounds, long long *resync_subsequences);
 
+/*
+ * Decompression to pixels on the device: replaces jpeg_read_header + jpeg_start_decompress + jpeg_read_scanlines of a
+ * decompress object left at its defaults (JDCT_ISLOW, fancy upsampling, no scaling or colour quantization,
+ * out_color_space as default_decompress_parms picks it: gray -> gray, YCbCr -> RGB, RGB -> RGB), sample for sample, for
+ * a batch of sequential files of one geometry and colour space.  It is what the reference's cjpeg does with a JPEG
+ * input file (rdjpeg.c).  The entropy decode is b200jpeg_decode_coefs_batch's, with its error reporting; dequantization
+ * uses each file's own latched tables.
+ *
+ * Accepted: SOF0 / SOF1, 8 bits, one component, or three with component 0 at the largest sampling factors (1 or 2 each
+ * way) over 1x1 chroma (4:4:4, 4:2:2, 4:4:0, 4:2:0).  12-bit, 4-component, progressive files and every other sampling
+ * layout are B200JPEG_ERR_UNSUPPORTED naming the first such image, before any device work.
+ *
+ * b200jpeg_decompress_batch writes image i's rows (image_width * components bytes, see b200jpeg_decompress_output) to
+ * pixels + i * image_stride, row_pitch bytes apart, in host or device memory (pixels_on_device).  The batch is
+ * processed in chunks (b200jpeg_encoder_set_chunk_images): coefficient and sample planes are one chunk's.
+ */
+int  b200jpeg_decompress_batch(b200jpeg_encoder *enc, const uint8_t *const *files, const size_t *sizes, int n_images,
+                               void *pixels, int pixels_on_device, size_t row_pitch, size_t image_stride);
+/* cjpeg with JPEG input files: the decode above into device memory, then b200jpeg_encode_batch on the pixels where they
+ * lie, so every encoder option applies.  p is the compress parameter block: image size, in_color_space,
+ * input_components (and data_precision 8) must be what the sources decode to (b200jpeg_decompress_output), else
+ * B200JPEG_ERR_PARAM.  Like cjpeg (cjpeg.c:960-990) each file receives, behind its JFIF / Adobe header, the COM and
+ * APPn segments of its source in file order, except a JFIF APP0 when p->write_JFIF_header and an Adobe APP14 when
+ * p->write_Adobe_marker.  The finished files are read with b200jpeg_get_output. */
+int  b200jpeg_recompress_batch(b200jpeg_encoder *enc, const b200jpeg_params *p, const uint8_t *const *files,
+                               const size_t *sizes, int n_images);
+/* What rdjpeg.c's start_input_jpeg copies from the decompress object into the compress object: image size,
+ * out_color_space (B200JPEG_CS_GRAYSCALE, _RGB, or _CMYK for 4-component files) and output_components. */
+int  b200jpeg_decompress_output(const b200jpeg_source_info *src, int *width, int *height, int *color_space, int *components);
+
 /* b200jpeg_encode_batch, but stops after the entropy-coded bytes are in HBM: no device->host
  * copy, no host-side file assembly.  Used to time the device pipeline alone. */
 int  b200jpeg_encode_batch_device_only(b200jpeg_encoder *enc, const b200jpeg_params *p,

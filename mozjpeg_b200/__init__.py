@@ -14,7 +14,7 @@ import numpy as np
 
 from . import _abi as A
 from ._abi import B200JpegError, Params  # noqa: F401
-from .cjpeg import params_from_switches, pnm_samples, read_pnm, read_ppm  # noqa: F401
+from .cjpeg import params_for_jpeg_input, params_from_switches, pnm_samples, read_pnm, read_ppm  # noqa: F401
 
 _lib = A.load()          # raises ImportError with build instructions if missing
 
@@ -184,6 +184,28 @@ class Encoder:
                 "encode_batch_coefs_transform")
         return [self.get_output(i) for i in range(n)]
 
+    def decompress(self, files: Sequence[bytes]) -> np.ndarray:
+        """jpeg_read_scanlines of a default decompress object for same-geometry sequential files, on the device:
+        an (N, H, W, C) uint8 array, (N, H, W) for gray files (b200jpeg_decompress_batch)."""
+        w, h, _, nc = decompress_output(_parse_first(files))
+        bufs, ptrs, sizes = self._files(files)
+        out = np.empty((len(bufs), h, w, nc), dtype=np.uint8)
+        A.check(_lib.b200jpeg_decompress_batch(self._h, ptrs, sizes, len(bufs), out.ctypes.data, 0, out.strides[1], out.strides[0]), "decompress_batch")
+        return out[..., 0] if nc == 1 else out
+
+    def decompress_ptr(self, files: Sequence[bytes], ptr: int, row_pitch: int, image_stride: int) -> None:
+        """Raw-pointer form of decompress: the pixels go to device memory at ``ptr`` and stay there."""
+        bufs, ptrs, sizes = self._files(files)
+        A.check(_lib.b200jpeg_decompress_batch(self._h, ptrs, sizes, len(bufs), ptr, 1, row_pitch, image_stride), "decompress_batch")
+
+    def recompress(self, p: Params, files: Sequence[bytes]) -> List[bytes]:
+        """cjpeg with JPEG input files (b200jpeg_recompress_batch): the files decoded to pixels on the device and
+        encoded from there with ``p`` (cjpeg.params_for_jpeg_input builds it); each output carries its source's COM and
+        APPn segments as cjpeg copies them."""
+        bufs, ptrs, sizes = self._files(files)
+        A.check(_lib.b200jpeg_recompress_batch(self._h, C.byref(p), ptrs, sizes, len(bufs)), "recompress_batch")
+        return [self.get_output(i) for i in range(len(bufs))]
+
     def last_decode_sync(self):
         """(most rounds a CTA of the speculative decoder needed, subsequences the cross-CTA pass decoded again)."""
         r = C.c_int(0); q = C.c_longlong(0)
@@ -294,8 +316,24 @@ def _parse_first(files: Sequence[bytes]) -> A.SourceInfo:
     return info
 
 
+def decompress_output(info: "A.SourceInfo"):
+    """(width, height, out_color_space, output_components) of a source decoded with the decompress defaults
+    (b200jpeg_decompress_output): what rdjpeg.c copies into the compress object."""
+    w = C.c_int(0); h = C.c_int(0); cs = C.c_int(0); nc = C.c_int(0)
+    A.check(_lib.b200jpeg_decompress_output(C.byref(info), C.byref(w), C.byref(h), C.byref(cs), C.byref(nc)), "decompress_output")
+    return w.value, h.value, cs.value, nc.value
+
+
 def cjpeg(switches: Sequence[str], ppm: bytes, encoder: Optional[Encoder] = None) -> bytes:
-    """``cjpeg <switches> file.ppm`` on the device path: PPM/PGM bytes -> JPEG bytes."""
+    """``cjpeg <switches> file`` on the device path: PPM/PGM or JPEG bytes -> JPEG bytes.  The input format follows
+    cjpeg's select_file_type: a first byte 0xFF is a JPEG file, recompressed on the device."""
+    if ppm[:1] == b"\xff":
+        enc = encoder or Encoder(0)
+        try:
+            return enc.recompress(params_for_jpeg_input(switches, ppm), [ppm])[0]
+        finally:
+            if encoder is None:
+                enc.close()
     w, h, nc, maxv, a = read_pnm(ppm)
     p = params_from_switches(switches, w, h, nc)
     img = pnm_samples(maxv, a, p.data_precision)[None]

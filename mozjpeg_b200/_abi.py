@@ -145,6 +145,7 @@ EXPORTS = [
     "b200jpeg_finish_compress", "b200jpeg_last_error", "b200jpeg_version",
     "b200jpeg_parse_source", "b200jpeg_decode_coefs_batch", "b200jpeg_transcode_batch", "b200jpeg_last_decode_sync",
     "b200jpeg_transform_setup", "b200jpeg_transcode_batch_transform", "b200jpeg_encode_batch_coefs_transform",
+    "b200jpeg_decompress_batch", "b200jpeg_recompress_batch", "b200jpeg_decompress_output",
 ]
 
 _lib = None
@@ -211,6 +212,10 @@ def load() -> C.CDLL:
     lib.b200jpeg_transcode_batch_transform.argtypes = [C.c_void_p, P, PT, PB, PS, C.c_int]; lib.b200jpeg_transcode_batch_transform.restype = C.c_int
     lib.b200jpeg_encode_batch_coefs_transform.argtypes = [C.c_void_p, P, PT, PB, C.c_int, PS, PS, Q, C.c_int]; lib.b200jpeg_encode_batch_coefs_transform.restype = C.c_int
     lib.b200jpeg_last_decode_sync.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_longlong)]; lib.b200jpeg_last_decode_sync.restype = C.c_int
+    lib.b200jpeg_decompress_batch.argtypes = [C.c_void_p, PB, PS, C.c_int, C.c_void_p, C.c_int, C.c_size_t, C.c_size_t]; lib.b200jpeg_decompress_batch.restype = C.c_int
+    lib.b200jpeg_recompress_batch.argtypes = [C.c_void_p, P, PB, PS, C.c_int]; lib.b200jpeg_recompress_batch.restype = C.c_int
+    PI = C.POINTER(C.c_int)
+    lib.b200jpeg_decompress_output.argtypes = [C.POINTER(SourceInfo), PI, PI, PI, PI]; lib.b200jpeg_decompress_output.restype = C.c_int
     lib.b200jpeg_last_error.argtypes = []; lib.b200jpeg_last_error.restype = C.c_char_p
     lib.b200jpeg_version.argtypes = []; lib.b200jpeg_version.restype = C.c_char_p
     _lib = lib

@@ -335,6 +335,18 @@ def params_from_switches(switches: Sequence[str], width: int, height: int,
     return p
 
 
+def params_for_jpeg_input(switches: Sequence[str], jpeg: bytes) -> A.Params:
+    """cjpeg's cinfo at jpeg_start_compress for a JPEG input file: rdjpeg.c's start_input_jpeg takes the image size,
+    in_color_space (the decompressor's out_color_space) and input_components from the source (data_precision is 8 for
+    every source the device decodes), then jpeg_default_colorspace and the second switch pass run as for any input."""
+    lib = A.load()
+    info = A.SourceInfo()
+    A.check(lib.b200jpeg_parse_source(bytes(jpeg), len(jpeg), C.byref(info)), "parse_source")
+    w = C.c_int(0); h = C.c_int(0); cs = C.c_int(0); nc = C.c_int(0)
+    A.check(lib.b200jpeg_decompress_output(C.byref(info), C.byref(w), C.byref(h), C.byref(cs), C.byref(nc)), "decompress_output")
+    return params_from_switches(switches, w.value, h.value, nc.value, in_color_space=cs.value)
+
+
 def read_pnm(data: bytes):
     """Minimal binary PGM/PPM reader (P5/P6) -> (w, h, ncomp, maxval, samples): samples is an (h, w, ncomp) uint8 array
     for maxval <= 255, else uint16 (two bytes per sample, big-endian in the file, as rdppm.c reads them)."""
@@ -386,7 +398,9 @@ def read_ppm(data: bytes) -> Tuple[int, int, int, bytes]:
 
 def main(argv: Sequence[str] = None) -> int:
     """``python -m mozjpeg_b200.cjpeg [switches] [-outfile name] file.ppm [more.ppm ...]`` - cjpeg's command line on
-    the device path.  Several input files of one size are encoded as one batch (outputs: <input>.jpg)."""
+    the device path.  Several input files of one size are encoded as one batch (outputs: <input>.jpg).  Input files
+    that start with 0xFF are JPEG files (select_file_type, cjpeg.c:145-148): they are decoded and recompressed on the
+    device, and must then all be JPEG files of one geometry."""
     import sys
     import numpy as np
     from . import Encoder
@@ -411,9 +425,21 @@ def main(argv: Sequence[str] = None) -> int:
     if not files:
         print("usage: python -m mozjpeg_b200.cjpeg [switches] [-outfile name] file.ppm [more.ppm ...]", file=sys.stderr)
         return 2
+    data = [open(f, "rb").read() for f in files]
+    if any(d[:1] == b"\xff" for d in data):
+        if not all(d[:1] == b"\xff" for d in data):
+            print("all input files of one call must have the same format", file=sys.stderr)
+            return 2
+        out = Encoder(0).recompress(params_for_jpeg_input(switches, data[0]), data)
+        for f, jpg in zip(files, out):
+            # a JPEG input named x.jpg must not be overwritten by its own output
+            name = outfile if (outfile and len(files) == 1) else f.rsplit(".", 1)[0] + ".out.jpg"
+            with open(name, "wb") as fo:
+                fo.write(jpg)
+        return 0
     raw = []
-    for f in files:
-        w, h, nc, maxv, a = read_pnm(open(f, "rb").read())
+    for d in data:
+        w, h, nc, maxv, a = read_pnm(d)
         raw.append((maxv, a))
     if len({a.shape for _, a in raw}) != 1:
         print("all input files of one call must have the same size", file=sys.stderr)

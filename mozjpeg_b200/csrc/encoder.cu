@@ -144,6 +144,14 @@ struct b200jpeg_encoder {
   size_t dec_plane_off[4] = {0, 0, 0, 0};
   cudaEvent_t dec_ev[7] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
   int dec_rounds = 0; long long dec_redone = 0;
+  // decompression to pixels (b200jpeg_decompress_batch / b200jpeg_recompress_batch): one chunk's sample planes and
+  // quantization tables, the whole batch's pixels where the caller gave no device buffer, the stage times summed over
+  // the chunks, and per image the source's COM / APPn segments a recompress copies into its file
+  DevBuf d_dec_samples, d_dec_quant, d_dec_pixels;
+  cudaEvent_t pix_ev[3] = {nullptr, nullptr, nullptr};
+  float dec_ms[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  std::vector<std::vector<uint8_t>> dec_markers;
+  const std::vector<std::vector<uint8_t>> *copy_markers = nullptr;   // of the batch being encoded, or nullptr
   CoefXform xform{};                            // the coefficient import's block mapping in the current batch (all zero: a copy)
 };
 
@@ -1192,6 +1200,19 @@ static int finish_chunk(b200jpeg_encoder *e, const ChunkIO &io, int k)
     hdr.clear(); hdr_end.assign(emit.size(), 0);
     Bytes o{hdr};
     write_file_header(p, o);
+    if (e->copy_markers) {
+      // cjpeg's copy of the source's saved markers right behind jpeg_start_compress (cjpeg.c:960-990): all but a JFIF
+      // APP0 / Adobe APP14 where the file header above already holds the compressor's own
+      const std::vector<uint8_t> &mk = (*e->copy_markers)[gi];
+      for (size_t q = 0; q + 4 <= mk.size();) {
+        const size_t len = 2 + ((size_t)mk[q + 2] << 8 | mk[q + 3]);
+        const uint8_t *dat = mk.data() + q + 4; const size_t dl = len - 4;
+        const bool dup = (p->write_JFIF_header && mk[q + 1] == 0xE0 && dl >= 5 && !memcmp(dat, "JFIF\0", 5)) ||
+                         (p->write_Adobe_marker && mk[q + 1] == 0xEE && dl >= 5 && !memcmp(dat, "Adobe", 5));
+        if (!dup) hdr.insert(hdr.end(), mk.begin() + q, mk.begin() + q + len);
+        q += len;
+      }
+    }
     TblState ts;
     const HostHuff *fixed = pl.optimize ? nullptr : ht;
     for (int t = 0; t < 4; t++) { ts.dc[t] = fixed ? &fixed[t] : nullptr; ts.ac[t] = fixed ? &fixed[4 + t] : nullptr; ts.dc_sent[t] = ts.ac_sent[t] = false; }
@@ -1313,9 +1334,10 @@ static int collect_qsets(b200jpeg_encoder *e, const b200jpeg_params *p, const ui
 
 static int encode_common(b200jpeg_encoder *e, const b200jpeg_params *p, const void *pixels, int on_device,
                          size_t row_pitch, size_t image_stride, int n_images, bool device_only, const RawDesc *raw = nullptr,
-                         const uint16_t *qtables = nullptr)
+                         const uint16_t *qtables = nullptr, const std::vector<std::vector<uint8_t>> *markers = nullptr)
 {
   if (!e || !p || (!pixels && !raw) || n_images <= 0) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
+  e->copy_markers = markers;
   int rc = b200jpeg_validate(p);
   if (rc) return rc;
   // lossless mode: the block jpeg_start_compress works with (jcmaster.c:1072-1094); the plan and the markers follow it
@@ -1616,12 +1638,13 @@ static void add_decode_stage_times(b200jpeg_encoder *e)
 }
 
 // Entropy decode of n sequential files into e->d_dec_planes (jpeg_read_coefficients for the batch).
-static int decode_files(b200jpeg_encoder *e, const uint8_t *const *files, const size_t *sizes, int n)
+// first: the batch index of files[0], for the messages.
+static int decode_files(b200jpeg_encoder *e, const uint8_t *const *files, const size_t *sizes, int n, int first = 0)
 {
   if (!e || !files || !sizes || n <= 0) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
   CU(cudaSetDevice(e->device));
   DecBatch &b = e->dec;
-  int rc = build_decode_batch(files, sizes, n, b, dec_words_alloc, e);
+  int rc = build_decode_batch(files, sizes, n, b, dec_words_alloc, e, first);
   if (rc) return rc;
   size_t total = 0;
   for (int c = 0; c < b.nc; c++) { e->dec_plane_off[c] = total; total += ((size_t)n * b.wib[c] * b.hib[c] * 128 + 255) & ~(size_t)255; }
@@ -1658,7 +1681,7 @@ static int decode_files(b200jpeg_encoder *e, const uint8_t *const *files, const 
   e->dec_rounds = *reinterpret_cast<const int *>(hs + rounds_off);
   e->dec_redone = (long long)*reinterpret_cast<const unsigned long long *>(hs + rounds_off + 8);
   for (int i = 0; i < n; i++)
-    if (reinterpret_cast<const uint32_t *>(hs)[i]) { set_error("image %d: corrupt entropy-coded data (an invalid Huffman code, or too few bits for a segment's MCUs)", i); return B200JPEG_ERR_BAD_SOURCE; }
+    if (reinterpret_cast<const uint32_t *>(hs)[i]) { set_error("image %d: corrupt entropy-coded data (an invalid Huffman code, or too few bits for a segment's MCUs)", first + i); return B200JPEG_ERR_BAD_SOURCE; }
   return B200JPEG_OK;
 }
 
@@ -1705,6 +1728,7 @@ static int encode_coefs_xform(b200jpeg_encoder *enc, const b200jpeg_params *p, c
 static int transcode_files(b200jpeg_encoder *e, const b200jpeg_params *p, const b200jpeg_transform_info *t, const uint8_t *const *files, const size_t *sizes, int n_images)
 {
   if (!e || !p) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
+  e->dec.want_markers = false;
   int rc = decode_files(e, files, sizes, n_images);
   if (rc) return rc;
   const DecBatch &b = e->dec;
@@ -1740,14 +1764,169 @@ static int transcode_files(b200jpeg_encoder *e, const b200jpeg_params *p, const 
   return B200JPEG_OK;
 }
 
+// A source b200jpeg_decompress_batch takes: sequential, 8-bit, gray or three components with component 0 at the
+// largest factors (1 or 2 each way) over 1x1 chroma; everything else is refused, never approximated.
+static int check_decompress_source(const b200jpeg_source_info &s, int i)
+{
+  const char *why = nullptr;
+  if (s.sof == 0xC2) why = "progressive (SOF2) source: only sequential files are decoded to pixels";
+  else if (s.data_precision != 8) why = "12-bit source: only 8-bit files are decoded to pixels";
+  else if (s.num_components != 1 && s.num_components != 3) why = "4-component (CMYK / YCCK) source: only gray and 3-component files are decoded to pixels";
+  else if (s.num_components == 3 && (s.h_samp_factor[0] > 2 || s.v_samp_factor[0] > 2 || s.h_samp_factor[1] != 1 || s.v_samp_factor[1] != 1 ||
+                                     s.h_samp_factor[2] != 1 || s.v_samp_factor[2] != 1))
+    why = "sampling layout other than 4:4:4, 4:2:2, 4:4:0 or 4:2:0 (the reference's int_upsample and 2:1 non-fancy cases are not on the device)";
+  if (why) { set_error("image %d: %s", i, why); return B200JPEG_ERR_UNSUPPORTED; }
+  for (int c = 0; c < s.num_components; c++)
+    if (!s.comp_quant_present[c]) { set_error("image %d: Quantization table 0x%02x was not defined", i, s.quant_tbl_no[c]); return B200JPEG_ERR_BAD_SOURCE; }
+  return B200JPEG_OK;
+}
+
+// jpeg_read_scanlines for a batch of files: entropy decode, IDCT and upsampling / colour conversion chunk by chunk
+// (the coefficient and sample planes are one chunk's), into pixels on the device.
+static int decompress_files(b200jpeg_encoder *e, const uint8_t *const *files, const size_t *sizes, int n, uint8_t *pix, size_t row_pitch, size_t image_stride,
+                            bool want_markers)
+{
+  // every refusal comes before any device work
+  b200jpeg_source_info s0;
+  {
+    static thread_local b200jpeg_source_info s;
+    for (int i = 0; i < n; i++) {
+      if (!files[i]) { set_error("image %d: no file", i); return B200JPEG_ERR_PARAM; }
+      int rc = b200jpeg_parse_source(files[i], sizes[i], &s);
+      if (rc) { std::string m = b200jpeg_last_error(); set_error("image %d: %s", i, m.c_str()); return rc; }
+      if ((rc = check_decompress_source(s, i))) return rc;
+      if (i == 0) s0 = s;
+      bool same = s.image_width == s0.image_width && s.image_height == s0.image_height && s.num_components == s0.num_components;
+      for (int c = 0; same && c < s.num_components; c++) same = s.h_samp_factor[c] == s0.h_samp_factor[c] && s.v_samp_factor[c] == s0.v_samp_factor[c];
+      if (same && s.num_components == 3) same = (s.jpeg_color_space == B200JPEG_CS_RGB) == (s0.jpeg_color_space == B200JPEG_CS_RGB);
+      if (!same) { set_error("image %d: geometry (size, components, sampling, colour space) differs from image 0", i); return B200JPEG_ERR_PARAM; }
+    }
+  }
+  const int W = s0.image_width, H = s0.image_height, nc = s0.num_components;
+  const int hx = nc == 3 ? s0.h_samp_factor[0] : 1, vx = nc == 3 ? s0.v_samp_factor[0] : 1;
+  if (row_pitch < (size_t)W * nc || (n > 1 && image_stride < row_pitch * (size_t)(H - 1) + (size_t)W * nc)) { set_error("row_pitch or image_stride smaller than the decoded image (%dx%d, %d components)", W, H, nc); return B200JPEG_ERR_PARAM; }
+  CU(cudaSetDevice(e->device));
+  for (cudaEvent_t &ev : e->pix_ev) if (!ev) CU(cudaEventCreate(&ev));
+  for (float &m : e->dec_ms) m = 0.f;
+  e->dec.want_markers = want_markers;
+  if (want_markers) e->dec_markers.assign(n, std::vector<uint8_t>());
+  // chunks of about 1.6 M blocks (8 images of 3840x2160 4:2:0, 300 MB of coefficient and sample planes)
+  long long per = 0;
+  for (int c = 0; c < nc; c++) per += (long long)div_up((long long)W * s0.h_samp_factor[c], (nc == 3 ? hx : s0.h_samp_factor[0]) * 8) * div_up((long long)H * s0.v_samp_factor[c], (nc == 3 ? vx : s0.v_samp_factor[0]) * 8);
+  const int C = std::min(n, e->chunk_images_override > 0 ? e->chunk_images_override : (int)std::max(1LL, 1600000LL / std::max(1LL, per)));
+  cudaStream_t s = e->stream;
+  std::vector<uint16_t> qt;
+  for (int i0 = 0; i0 < n; i0 += C) {
+    const int nk = std::min(C, n - i0);
+    int rc = decode_files(e, files + i0, sizes + i0, nk, i0);
+    if (rc) return rc;
+    const DecBatch &b = e->dec;
+    if (want_markers) for (int i = 0; i < nk; i++) e->dec_markers[i0 + i].swap(e->dec.markers[i]);
+    size_t off[4] = {0, 0, 0, 0}, total = 0;
+    for (int c = 0; c < nc; c++) { off[c] = total; total += ((size_t)nk * b.hib[c] * b.wib[c] * 64 + 255) & ~(size_t)255; }
+    if ((rc = e->d_dec_samples.reserve(total)) || (rc = e->d_dec_quant.reserve((size_t)nk * nc * 128))) return rc;
+    qt.resize((size_t)nk * nc * 64);
+    for (int i = 0; i < nk; i++)
+      for (int c = 0; c < nc; c++) memcpy(&qt[((size_t)i * nc + c) * 64], b.info[i].comp_quant[c], 128);
+    CU(cudaMemcpyAsync(e->d_dec_quant.p, qt.data(), qt.size() * 2, cudaMemcpyHostToDevice, s));
+    CU(cudaEventRecord(e->pix_ev[0], s));
+    const uint8_t *planes[4] = {nullptr, nullptr, nullptr, nullptr}; int pitch[4] = {0, 0, 0, 0}; long long stride[4] = {0, 0, 0, 0};
+    for (int c = 0; c < nc; c++) {
+      uint8_t *dst = e->d_dec_samples.as<uint8_t>() + off[c];
+      launch_idct_islow(reinterpret_cast<const int16_t *>(e->d_dec_planes.as<uint8_t>() + e->dec_plane_off[c]), e->d_dec_quant.as<uint16_t>() + c * 64, nc * 64,
+                        dst, b.wib[c], b.hib[c], nk, s);
+      planes[c] = dst; pitch[c] = b.wib[c] * 8; stride[c] = (long long)b.hib[c] * 8 * pitch[c];
+    }
+    CU(cudaEventRecord(e->pix_ev[1], s));
+    const int dw = div_up(W, hx), dh = div_up(H, vx);                    // downsampled_width / _height of the chroma (jdmaster.c)
+    if (launch_upsample_color(hx, vx, nc, planes, pitch, stride, dw, dh, nc == 3 && s0.jpeg_color_space != B200JPEG_CS_RGB,
+                              pix + (size_t)i0 * image_stride, row_pitch, image_stride, W, H, nk, s)) { set_error("no upsampling kernel for %dx%d sampling of %d components", hx, vx, nc); return B200JPEG_ERR_UNSUPPORTED; }
+    CU(cudaEventRecord(e->pix_ev[2], s));
+    CU(cudaGetLastError());
+    CU(cudaStreamSynchronize(s));
+    for (int k = 0; k < 6; k++) { float ms = 0.f; cudaEventElapsedTime(&ms, e->dec_ev[k], e->dec_ev[k + 1]); e->dec_ms[k] += ms; }
+    for (int k = 0; k < 2; k++) { float ms = 0.f; cudaEventElapsedTime(&ms, e->pix_ev[k], e->pix_ev[k + 1]); e->dec_ms[6 + k] += ms; }
+  }
+  return B200JPEG_OK;
+}
+
+// the stages of the last decompress, appended to the stage times
+static void add_decompress_stage_times(b200jpeg_encoder *e)
+{
+  static const char *const extra[2] = {"idct", "upsample_color"};
+  for (int k = 0; k < 8; k++) { e->stage_names.push_back(k < 6 ? kDecStages[k] : extra[k - 6]); e->stage_ms.push_back(e->dec_ms[k]); e->stage_calls.push_back(1); }
+}
+
 }  // namespace b200
 
 extern "C" {
+
+int b200jpeg_decompress_batch(b200jpeg_encoder *e, const uint8_t *const *files, const size_t *sizes, int n_images,
+                              void *pixels, int pixels_on_device, size_t row_pitch, size_t image_stride)
+{
+  if (!e || !files || !sizes || !pixels || n_images <= 0) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
+  uint8_t *dst = static_cast<uint8_t *>(pixels);
+  size_t dp = row_pitch, ds = image_stride;
+  if (!pixels_on_device) {
+    // decode into a buffer of the batch's size on the device, then copy the rows out
+    b200jpeg_source_info *s = new b200jpeg_source_info;
+    int rc = b200jpeg_parse_source(files[0], files[0] ? sizes[0] : 0, s);
+    const size_t row = rc ? 0 : (size_t)s->image_width * s->num_components, rows = rc ? 0 : (size_t)s->image_height;
+    delete s;
+    if (rc) { std::string m = b200jpeg_last_error(); set_error("image 0: %s", m.c_str()); return rc; }
+    if (row_pitch < row || (n_images > 1 && image_stride < row_pitch * (rows - 1) + row)) { set_error("row_pitch or image_stride smaller than the decoded image"); return B200JPEG_ERR_PARAM; }
+    dp = (row + 3) & ~(size_t)3; ds = dp * rows;
+    CU(cudaSetDevice(e->device));
+    if ((rc = e->d_dec_pixels.reserve(ds * (size_t)n_images))) return rc;
+    dst = e->d_dec_pixels.as<uint8_t>();
+    rc = b200::decompress_files(e, files, sizes, n_images, dst, dp, ds, false);
+    if (rc) return rc;
+    for (int i = 0; i < n_images; i++)
+      CU(cudaMemcpy2DAsync(static_cast<uint8_t *>(pixels) + (size_t)i * image_stride, row_pitch, dst + (size_t)i * ds, dp, row, rows, cudaMemcpyDeviceToHost, e->stream));
+    CU(cudaStreamSynchronize(e->stream));
+  } else {
+    int rc = b200::decompress_files(e, files, sizes, n_images, dst, dp, ds, false);
+    if (rc) return rc;
+  }
+  e->pending_marks = 0;
+  e->stage_names.clear(); e->stage_ms.clear(); e->stage_calls.clear();
+  b200::add_decompress_stage_times(e);
+  return B200JPEG_OK;
+}
+
+int b200jpeg_recompress_batch(b200jpeg_encoder *e, const b200jpeg_params *p, const uint8_t *const *files, const size_t *sizes, int n_images)
+{
+  if (!e || !p || !files || !sizes || n_images <= 0) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
+  int rc = b200jpeg_validate(p);
+  if (rc) return rc;
+  if (p->data_precision != 8) { set_error("the sources decode to 8-bit samples, the parameter block has data_precision %d", p->data_precision); return B200JPEG_ERR_PARAM; }
+  const size_t pitch = ((size_t)p->image_width * p->input_components + 3) & ~(size_t)3, stride = pitch * (size_t)p->image_height;
+  {
+    b200jpeg_source_info *s = new b200jpeg_source_info;
+    int w = 0, h = 0, cs = 0, nc = 0;
+    rc = files[0] ? b200jpeg_parse_source(files[0], sizes[0], s) : B200JPEG_OK;
+    if (!rc && files[0]) rc = b200jpeg_decompress_output(s, &w, &h, &cs, &nc);
+    delete s;
+    if (rc) { std::string m = b200jpeg_last_error(); set_error("image 0: %s", m.c_str()); return rc; }
+    if (files[0] && (w != p->image_width || h != p->image_height || cs != p->in_color_space || nc != p->input_components)) {
+      set_error("the sources decode to %dx%d pixels of %d samples in colour space %d, the parameter block describes %dx%d of %d in %d (see b200jpeg_decompress_output)",
+                w, h, nc, cs, p->image_width, p->image_height, p->input_components, p->in_color_space);
+      return B200JPEG_ERR_PARAM;
+    }
+  }
+  CU(cudaSetDevice(e->device));
+  if ((rc = e->d_dec_pixels.reserve(stride * (size_t)n_images))) return rc;
+  if ((rc = b200::decompress_files(e, files, sizes, n_images, e->d_dec_pixels.as<uint8_t>(), pitch, stride, true))) return rc;
+  if ((rc = b200::encode_common(e, p, e->d_dec_pixels.p, 1, pitch, stride, n_images, false, nullptr, nullptr, &e->dec_markers))) return rc;
+  b200::add_decompress_stage_times(e);
+  return B200JPEG_OK;
+}
 
 int b200jpeg_decode_coefs_batch(b200jpeg_encoder *e, const uint8_t *const *files, const size_t *sizes, int n_images,
                                 int16_t *const *planes, int planes_on_device, const size_t *row_pitch_blocks, const size_t *image_stride_blocks)
 {
   if (!e || !planes || !row_pitch_blocks || !image_stride_blocks) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
+  e->dec.want_markers = false;
   int rc = decode_files(e, files, sizes, n_images);
   if (rc) return rc;
   const DecBatch &b = e->dec;
@@ -1830,9 +2009,11 @@ void b200jpeg_encoder_destroy(b200jpeg_encoder *e)
   DevBuf *db[] = {&e->d_src, &e->d_yuv, &e->d_tabs_scan, &e->d_tabs_fixed, &e->d_status, &e->d_out_pos, &e->d_scan_size, &e->d_out, &e->d_qt, &e->d_tc, &e->d_best_al_all, &e->d_qimg_all, &e->d_qset};
   for (DevBuf *b : db) b->release();
   for (int i = 0; i < MAX_ARENAS; i++) e->ar[i].release();
-  DevBuf *dd[] = {&e->d_dec_words, &e->d_dec_segs, &e->d_dec_scans, &e->d_dec_tabs, &e->d_dec_out, &e->d_dec_rec, &e->d_dec_pre, &e->d_dec_tsum, &e->d_dec_dcd, &e->d_dec_planes, &e->d_dec_stat};
+  DevBuf *dd[] = {&e->d_dec_words, &e->d_dec_segs, &e->d_dec_scans, &e->d_dec_tabs, &e->d_dec_out, &e->d_dec_rec, &e->d_dec_pre, &e->d_dec_tsum, &e->d_dec_dcd, &e->d_dec_planes, &e->d_dec_stat,
+                  &e->d_dec_samples, &e->d_dec_quant, &e->d_dec_pixels};
   for (DevBuf *b : dd) b->release();
   for (cudaEvent_t ev : e->dec_ev) if (ev) cudaEventDestroy(ev);
+  for (cudaEvent_t ev : e->pix_ev) if (ev) cudaEventDestroy(ev);
   PinBuf *pb[] = {&e->h_qt, &e->h_tc, &e->h_fixed, &e->h_status, &e->h_out_pos, &e->h_scan_size, &e->h_tabs, &e->h_stage, &e->h_best_al, &e->h_qinit, &e->h_qimg, &e->h_qset, &e->h_dec_words, &e->h_dec_stat};
   for (PinBuf *b : pb) b->release();
   for (PinBuf &b : e->file_arenas) b.release();

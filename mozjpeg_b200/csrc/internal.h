@@ -22,6 +22,11 @@ struct DecBatch {
   long long nsub = 0, nblocks = 0; unsigned long long nwords = 0;
   int W = 0, H = 0, nc = 0, precision = 8;
   int wib[4] = {0, 0, 0, 0}, hib[4] = {0, 0, 0, 0}, h[4] = {0, 0, 0, 0}, v[4] = {0, 0, 0, 0};
+  // want_markers: also collect each file's COM / APPn segments as cjpeg copies them from a JPEG input (raw segments,
+  // file order; see parse_source)
+  bool want_markers = false;
+  std::vector<std::vector<uint8_t>> markers;
 };
-int build_decode_batch(const uint8_t *const *files, const size_t *sizes, int n, DecBatch &b, uint32_t *(*alloc)(void *, size_t), void *ctx);
+// first: the batch index of files[0], for the messages (a caller that decodes a batch in chunks)
+int build_decode_batch(const uint8_t *const *files, const size_t *sizes, int n, DecBatch &b, uint32_t *(*alloc)(void *, size_t), void *ctx, int first = 0);
 }

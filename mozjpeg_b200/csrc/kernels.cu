@@ -4236,4 +4236,205 @@ void launch_decode(const uint32_t *words, const DecSeg *segs, int nsegs, const D
   cudaEventRecord(marks[5], s);
 }
 
+// ------------------------------------------------------------------ decompression to pixels: the stages behind the
+// entropy decode of a default decompress object (JDCT_ISLOW, fancy upsampling, out_color_space of
+// default_decompress_parms), sample for sample
+
+// IDCT_range_limit (jdmaster.c prepare_range_limit_table) indexed with x & RANGE_MASK (jidctint.c:283-291): the low ten
+// bits of x taken as a signed number, plus the level shift, clamped
+__device__ __forceinline__ int idct_range_limit(int x)
+{
+  const int s = (((x & 1023) ^ 512) - 512) + 128;
+  return min(max(s, 0), 255);
+}
+
+#define IDCT_BLOCKS 32           // blocks per CTA of k_idct_islow (8 lanes each)
+#define IDCT_WS 73               // ints per block of its workspace: 8 rows of 9, and one more so that blocks start in different banks
+
+// jpeg_idct_islow (jidctint.c:171-419, 8-bit: CONST_BITS 13, PASS1_BITS 2) with the dequantization of jddctmgr.c:
+// 134-146 (ISLOW_MULT_TYPE is a short: the table entries are taken as int16).  Eight lanes per block: each loads one
+// 16-byte row of the JBLOCK, transforms one column into the int workspace (pass 1), then one row into eight samples
+// (pass 2) stored as one 8-byte word.  The reference's shortcuts for all-zero columns and rows give what the general
+// butterfly gives, so there is no branch.  Pass 1 keeps the reference's 64-bit intermediates (JLONG): a file may carry
+// 16-bit coefficients under a 16-bit table; pass 2 needs bits 18..27 of its sums only, which 32-bit arithmetic keeps.
+// coef: [nblocks][64] natural order ([n][hib][wib] blocks); quant: image i's table at quant + i * qstride;
+// out: [n][hib * 8][wib * 8] samples.
+__global__ void __launch_bounds__(IDCT_BLOCKS * 8) k_idct_islow(const int16_t *__restrict__ coef, const uint16_t *__restrict__ quant, int qstride,
+                                                                uint8_t *__restrict__ out, int wib, int hib, long long nblocks)
+{
+  __shared__ int4 s_coef[IDCT_BLOCKS * 8];
+  __shared__ int s_ws[IDCT_BLOCKS * IDCT_WS];
+  const int lb = threadIdx.x >> 3, lane = threadIdx.x & 7;
+  const long long blk = (long long)blockIdx.x * IDCT_BLOCKS + lb;
+  const bool valid = blk < nblocks;
+  const long long per = (long long)wib * hib;
+  const long long img = valid ? blk / per : 0;
+  s_coef[threadIdx.x] = valid ? reinterpret_cast<const int4 *>(coef)[blk * 8 + lane] : make_int4(0, 0, 0, 0);
+  __syncwarp();
+  // pass 1: column `lane`
+  {
+    const int16_t *c = reinterpret_cast<const int16_t *>(s_coef + lb * 8) + lane;
+    const uint16_t *q = quant + img * qstride + lane;
+    long long d[8];
+#pragma unroll
+    for (int r = 0; r < 8; r++) d[r] = (long long)c[r * 8] * (int16_t)q[r * 8];
+    long long z2 = d[2], z3 = d[6];
+    long long z1 = (z2 + z3) * 4433;
+    long long tmp2 = z1 + z3 * -15137, tmp3 = z1 + z2 * 6270;
+    z2 = d[0]; z3 = d[4];
+    long long tmp0 = (z2 + z3) * 8192, tmp1 = (z2 - z3) * 8192;
+    const long long tmp10 = tmp0 + tmp3, tmp13 = tmp0 - tmp3, tmp11 = tmp1 + tmp2, tmp12 = tmp1 - tmp2;
+    tmp0 = d[7]; tmp1 = d[5]; tmp2 = d[3]; tmp3 = d[1];
+    z1 = tmp0 + tmp3; z2 = tmp1 + tmp2; z3 = tmp0 + tmp2;
+    long long z4 = tmp1 + tmp3;
+    const long long z5 = (z3 + z4) * 9633;
+    tmp0 *= 2446; tmp1 *= 16819; tmp2 *= 25172; tmp3 *= 12299;
+    z1 *= -7373; z2 *= -20995; z3 *= -16069; z4 *= -3196;
+    z3 += z5; z4 += z5;
+    tmp0 += z1 + z3; tmp1 += z2 + z4; tmp2 += z2 + z3; tmp3 += z1 + z4;
+    int *ws = s_ws + lb * IDCT_WS + lane;
+    ws[0 * 9] = (int)((tmp10 + tmp3 + 1024) >> 11); ws[7 * 9] = (int)((tmp10 - tmp3 + 1024) >> 11);
+    ws[1 * 9] = (int)((tmp11 + tmp2 + 1024) >> 11); ws[6 * 9] = (int)((tmp11 - tmp2 + 1024) >> 11);
+    ws[2 * 9] = (int)((tmp12 + tmp1 + 1024) >> 11); ws[5 * 9] = (int)((tmp12 - tmp1 + 1024) >> 11);
+    ws[3 * 9] = (int)((tmp13 + tmp0 + 1024) >> 11); ws[4 * 9] = (int)((tmp13 - tmp0 + 1024) >> 11);
+  }
+  __syncwarp();
+  // pass 2: row `lane`, modulo 2^32
+  {
+    const int *ws = s_ws + lb * IDCT_WS + lane * 9;
+    unsigned d[8];
+#pragma unroll
+    for (int k = 0; k < 8; k++) d[k] = (unsigned)ws[k];
+    unsigned z2 = d[2], z3 = d[6];
+    unsigned z1 = (z2 + z3) * 4433u;
+    unsigned tmp2 = z1 - z3 * 15137u, tmp3 = z1 + z2 * 6270u;
+    unsigned tmp0 = (d[0] + d[4]) << 13, tmp1 = (d[0] - d[4]) << 13;
+    const unsigned tmp10 = tmp0 + tmp3, tmp13 = tmp0 - tmp3, tmp11 = tmp1 + tmp2, tmp12 = tmp1 - tmp2;
+    tmp0 = d[7]; tmp1 = d[5]; tmp2 = d[3]; tmp3 = d[1];
+    z1 = tmp0 + tmp3; z2 = tmp1 + tmp2; z3 = tmp0 + tmp2;
+    unsigned z4 = tmp1 + tmp3;
+    const unsigned z5 = (z3 + z4) * 9633u;
+    tmp0 *= 2446u; tmp1 *= 16819u; tmp2 *= 25172u; tmp3 *= 12299u;
+    z1 *= 0u - 7373u; z2 *= 0u - 20995u; z3 *= 0u - 16069u; z4 *= 0u - 3196u;
+    z3 += z5; z4 += z5;
+    tmp0 += z1 + z3; tmp1 += z2 + z4; tmp2 += z2 + z3; tmp3 += z1 + z4;
+    const unsigned rnd = 1u << 17;
+    const unsigned o0 = idct_range_limit((int)((tmp10 + tmp3 + rnd) >> 18)), o7 = idct_range_limit((int)((tmp10 - tmp3 + rnd) >> 18));
+    const unsigned o1 = idct_range_limit((int)((tmp11 + tmp2 + rnd) >> 18)), o6 = idct_range_limit((int)((tmp11 - tmp2 + rnd) >> 18));
+    const unsigned o2 = idct_range_limit((int)((tmp12 + tmp1 + rnd) >> 18)), o5 = idct_range_limit((int)((tmp12 - tmp1 + rnd) >> 18));
+    const unsigned o3 = idct_range_limit((int)((tmp13 + tmp0 + rnd) >> 18)), o4 = idct_range_limit((int)((tmp13 - tmp0 + rnd) >> 18));
+    if (valid) {
+      const long long rem = blk - img * per;
+      const int by = (int)(rem / wib), bx = (int)(rem - (long long)by * wib);
+      uint8_t *dst = out + ((img * hib + by) * 8 + lane) * ((long long)wib * 8) + bx * 8;
+      *reinterpret_cast<uint2 *>(dst) = make_uint2(o0 | o1 << 8 | o2 << 16 | o3 << 24, o4 | o5 << 8 | o6 << 16 | o7 << 24);
+    }
+  }
+}
+
+void launch_idct_islow(const int16_t *coef, const uint16_t *quant, int qstride, uint8_t *out, int wib, int hib, int n, cudaStream_t s)
+{
+  const long long nblocks = (long long)n * wib * hib;
+  k_idct_islow<<<(unsigned)((nblocks + IDCT_BLOCKS - 1) / IDCT_BLOCKS), IDCT_BLOCKS * 8, 0, s>>>(coef, quant, qstride, out, wib, hib, nblocks); LAUNCHED();
+}
+
+// the sample of a chroma plane at (row, col), both clamped to the real downsampled samples: the row above the first is
+// the first and the row below the last real one is that row again (jdmainct.c set_wraparound_pointers :240-266,
+// set_bottom_pointers :269-297); a column clamped the same way turns the general filter step into the reference's
+// first / last column cases (3 * a + a = 4 * a)
+__device__ __forceinline__ int up_at(const uint8_t *__restrict__ p, int pitch, int dw, int dh, int r, int c)
+{
+  return __ldg(p + (long long)min(max(r, 0), dh - 1) * pitch + min(max(c, 0), dw - 1));
+}
+
+// output pixels x0 .. x0+3 of row y of one chroma plane (dw x dh real samples): the upsamplers jinit_upsampler picks
+// with do_fancy_upsampling (jdsample.c:444-530).  fancy: downsampled_width > 2, below which the 2:1 horizontal cases
+// fall back to replication (h2v1_upsample, h2v2_upsample), which has no vertical filter either.
+template <int HX, int VX>
+__device__ __forceinline__ void upsample4(const uint8_t *__restrict__ p, int pitch, int dw, int dh, int x0, int y, bool fancy, int v[4])
+{
+  if (HX == 1 && VX == 1) {                               // fullsize_upsample (:129-135)
+    const uchar4 q = __ldg(reinterpret_cast<const uchar4 *>(p + (long long)y * pitch + x0));
+    v[0] = q.x; v[1] = q.y; v[2] = q.z; v[3] = q.w;
+  } else if (HX == 1) {                                   // h1v2_fancy_upsample (:316-352): 3/4 nearer row + 1/4 further, bias 1 / 2
+    const int r = y >> 1, r1 = (y & 1) ? r + 1 : r - 1, bias = (y & 1) ? 2 : 1;
+#pragma unroll
+    for (int k = 0; k < 4; k++) v[k] = (3 * up_at(p, pitch, dw, dh, r, x0 + k) + up_at(p, pitch, dw, dh, r1, x0 + k) + bias) >> 2;
+  } else {
+    const int c0 = x0 >> 1, r = VX == 2 ? y >> 1 : y;
+    if (!fancy) {                                         // h2v1_upsample / h2v2_upsample (:205-266)
+      const int a = up_at(p, pitch, dw, dh, r, c0), b = up_at(p, pitch, dw, dh, r, c0 + 1);
+      v[0] = v[1] = a; v[2] = v[3] = b;
+    } else if (VX == 1) {                                 // h2v1_fancy_upsample (:276-306)
+      const int l = up_at(p, pitch, dw, dh, r, c0 - 1), a = up_at(p, pitch, dw, dh, r, c0), b = up_at(p, pitch, dw, dh, r, c0 + 1), n = up_at(p, pitch, dw, dh, r, c0 + 2);
+      v[0] = (3 * a + l + 1) >> 2; v[1] = (3 * a + b + 2) >> 2; v[2] = (3 * b + a + 1) >> 2; v[3] = (3 * b + n + 2) >> 2;
+    } else {                                              // h2v2_fancy_upsample (:362-411): column sums 3 * nearer row + further row
+      const int r1 = (y & 1) ? r + 1 : r - 1;
+      int cs[4];
+#pragma unroll
+      for (int k = 0; k < 4; k++) cs[k] = 3 * up_at(p, pitch, dw, dh, r, c0 - 1 + k) + up_at(p, pitch, dw, dh, r1, c0 - 1 + k);
+      v[0] = (3 * cs[1] + cs[0] + 8) >> 4; v[1] = (3 * cs[1] + cs[2] + 7) >> 4; v[2] = (3 * cs[2] + cs[1] + 8) >> 4; v[3] = (3 * cs[2] + cs[3] + 7) >> 4;
+    }
+  }
+}
+
+// Sample planes -> interleaved pixels, each written once: chroma upsampling (upsample4), then ycc_rgb_convert with the
+// tables of build_ycc_rgb_table (jdcolor.c:210-252, SCALEBITS 16) computed in place, or the components as they are
+// (grayscale_convert, null_convert / rgb_rgb_convert for an RGB-coded file).  One thread makes four pixels of a row:
+// the luma word and the chroma samples around it come through L1 (neighbouring threads and rows share them), the
+// pixels leave as 4-byte words where the destination allows (aligned: base, pitch and stride multiples of 4), bytes at
+// a ragged right edge.  y0 / c1 / c2: image 0's planes, strides in bytes; dw x dh: the real chroma samples.
+template <int HX, int VX, int NC>
+__global__ void __launch_bounds__(256) k_upsample_color(const uint8_t *__restrict__ y0, const uint8_t *__restrict__ c1, const uint8_t *__restrict__ c2,
+                                                        int ypitch, long long ystride, int cpitch, long long cstride, int dw, int dh, bool fancy, bool ycc,
+                                                        uint8_t *__restrict__ pix, long long row_pitch, long long image_stride, int W, int H, bool aligned)
+{
+  const int x0 = (blockIdx.x * blockDim.x + threadIdx.x) * 4, y = blockIdx.y * blockDim.y + threadIdx.y, img = blockIdx.z;
+  if (x0 >= W || y >= H) return;
+  const uchar4 l = __ldg(reinterpret_cast<const uchar4 *>(y0 + img * ystride + (long long)y * ypitch + x0));
+  const int lum[4] = {l.x, l.y, l.z, l.w};
+  uint8_t *dst = pix + img * image_stride + y * row_pitch + (long long)x0 * NC;
+  const int nx = min(4, W - x0);
+  if (NC == 1) {
+    if (aligned && nx == 4) *reinterpret_cast<uchar4 *>(dst) = l;
+    else for (int k = 0; k < nx; k++) dst[k] = (uint8_t)lum[k];
+    return;
+  }
+  int cb[4], cr[4];
+  upsample4<HX, VX>(c1 + img * cstride, cpitch, dw, dh, x0, y, fancy, cb);
+  upsample4<HX, VX>(c2 + img * cstride, cpitch, dw, dh, x0, y, fancy, cr);
+  uint8_t o[12];
+#pragma unroll
+  for (int k = 0; k < 4; k++) {
+    if (ycc) {
+      const int u = cb[k] - 128, w = cr[k] - 128;
+      o[3 * k + 0] = (uint8_t)min(max(lum[k] + ((91881 * w + 32768) >> 16), 0), 255);
+      o[3 * k + 1] = (uint8_t)min(max(lum[k] + ((-22554 * u + 32768 - 46802 * w) >> 16), 0), 255);
+      o[3 * k + 2] = (uint8_t)min(max(lum[k] + ((116130 * u + 32768) >> 16), 0), 255);
+    } else { o[3 * k + 0] = (uint8_t)lum[k]; o[3 * k + 1] = (uint8_t)cb[k]; o[3 * k + 2] = (uint8_t)cr[k]; }
+  }
+  if (aligned && nx == 4) {
+#pragma unroll
+    for (int k = 0; k < 3; k++) reinterpret_cast<uint32_t *>(dst)[k] = o[4 * k] | o[4 * k + 1] << 8 | o[4 * k + 2] << 16 | (uint32_t)o[4 * k + 3] << 24;
+  } else {
+#pragma unroll
+    for (int k = 0; k < 12; k++) if (k < nx * 3) dst[k] = o[k];
+  }
+}
+
+int launch_upsample_color(int hx, int vx, int nc, const uint8_t *const *planes, const int *pitch, const long long *stride, int dw, int dh, bool ycc,
+                          uint8_t *pix, size_t row_pitch, size_t image_stride, int W, int H, int n, cudaStream_t s)
+{
+  const dim3 cta(64, 4), grid((unsigned)((W + 255) / 256), (unsigned)((H + 3) / 4), (unsigned)n);
+  const bool aligned = reinterpret_cast<uintptr_t>(pix) % 4 == 0 && row_pitch % 4 == 0 && image_stride % 4 == 0;
+  const bool fancy = dw > 2;
+#define UPSAMPLE_CASE(HX, VX, NC) \
+  if (hx == HX && vx == VX && nc == NC) { \
+    k_upsample_color<HX, VX, NC><<<grid, cta, 0, s>>>(planes[0], planes[1], planes[2], pitch[0], stride[0], pitch[1], stride[1], dw, dh, fancy, ycc, \
+                                                      pix, (long long)row_pitch, (long long)image_stride, W, H, aligned); LAUNCHED(); return 0; }
+  UPSAMPLE_CASE(1, 1, 1) UPSAMPLE_CASE(1, 1, 3) UPSAMPLE_CASE(2, 1, 3) UPSAMPLE_CASE(1, 2, 3) UPSAMPLE_CASE(2, 2, 3)
+#undef UPSAMPLE_CASE
+  return -1;
+}
+
 }  // namespace b200

@@ -248,6 +248,16 @@ void launch_decode(const uint32_t *words, const DecSeg *segs, int nsegs, const D
                    DecRec *rec, uint32_t *pre, unsigned long long *tsum, int *dcd, const DecOut *o, uint32_t *status,
                    int *max_rounds, unsigned long long *redone, cudaEvent_t *marks, cudaStream_t s);
 
+// decompression to pixels behind the entropy decode (jpeg_read_scanlines of a default decompress object, 8-bit).
+// k_idct_islow: coef [n][hib][wib][64] natural order -> out [n][hib * 8][wib * 8] samples, dequantized with image i's
+// table (natural order) at quant + i * qstride.
+void launch_idct_islow(const int16_t *coef, const uint16_t *quant, int qstride, uint8_t *out, int wib, int hib, int n, cudaStream_t s);
+// k_upsample_color<hx, vx, nc>: the sample planes (image 0's, pitch / stride in bytes; planes 1 and 2 share theirs and
+// hold dw x dh real samples) -> W x H interleaved pixels of nc samples; hx, vx: luma over chroma sampling, 1 or 2 each;
+// ycc: convert YCbCr to RGB, else copy the components.  Returns -1 for a layout it has no kernel for.
+int launch_upsample_color(int hx, int vx, int nc, const uint8_t *const *planes, const int *pitch, const long long *stride, int dw, int dh, bool ycc,
+                          uint8_t *pix, size_t row_pitch, size_t image_stride, int W, int H, int n, cudaStream_t s);
+
 extern unsigned long long g_kernel_launches;
 
 }  // namespace b200

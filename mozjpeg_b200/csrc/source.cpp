@@ -76,9 +76,15 @@ static size_t scan_data_end(const uint8_t *d, size_t n, size_t pos)
 
 using namespace b200;
 
-extern "C" int b200jpeg_parse_source(const uint8_t *d, size_t n, b200jpeg_source_info *s)
+// b200jpeg_parse_source; markers (or nullptr): receives, in file order, the COM and APPn segments (marker, length,
+// data) a decompress object with jpeg_save_markers on all of them holds once jpeg_start_decompress returns, which is
+// what rdjpeg.c hands cjpeg to copy: those in front of the first SOS and, for a file of several scans, which
+// jpeg_start_decompress reads to its end (jdapistd.c:80-103), the later ones too
+static int parse_source(const uint8_t *d, size_t n, b200jpeg_source_info *s, std::vector<uint8_t> *markers)
 {
   if (!d || !s) return bad(B200JPEG_ERR_PARAM, "bad argument");
+  struct Saved { size_t pos, len; int scans_seen; };
+  std::vector<Saved> saved;
   memset(s, 0, sizeof *s);
   s->data_precision = 8; s->JFIF_major_version = 1; s->JFIF_minor_version = 1; s->X_density = s->Y_density = 1;
   if (n < 2 || d[0] != 0xFF || d[1] != 0xD8) return bad(B200JPEG_ERR_PARAM, "not a JPEG file");
@@ -147,6 +153,7 @@ extern "C" int b200jpeg_parse_source(const uint8_t *d, size_t n, b200jpeg_source
     } else if (m == 0xDC) {
       // DNL: ignored, like the reference (jdmarker.c:1104)
     } else if (m == 0xE0 || m == 0xEE || m == 0xFE || (m >= 0xE1 && m <= 0xEF)) {
+      if (markers) saved.push_back({pos, 2 + ln, s->num_scans});
       if (m == 0xE0 && sl >= 14 && !memcmp(seg, "JFIF\0", 5)) {
         s->saw_JFIF = 1; s->JFIF_major_version = seg[5]; s->JFIF_minor_version = seg[6];
         s->density_unit = seg[7]; s->X_density = (int)be16(seg + 8); s->Y_density = (int)be16(seg + 10);
@@ -225,27 +232,51 @@ extern "C" int b200jpeg_parse_source(const uint8_t *d, size_t n, b200jpeg_source
   } else {
     s->jpeg_color_space = s->saw_Adobe && s->Adobe_transform == 2 ? B200JPEG_CS_YCCK : B200JPEG_CS_CMYK;
   }
+  if (markers) {
+    markers->clear();
+    const bool multi = s->sof == 0xC2 || (s->num_scans && s->scans[0].comps_in_scan != nc);       // has_multiple_scans (jdinput.c)
+    for (const Saved &m : saved)
+      if (m.scans_seen == 0 || multi) markers->insert(markers->end(), d + m.pos, d + m.pos + m.len);
+  }
+  return B200JPEG_OK;
+}
+
+extern "C" int b200jpeg_parse_source(const uint8_t *d, size_t n, b200jpeg_source_info *s)
+{
+  return parse_source(d, n, s, nullptr);
+}
+
+// what default_decompress_parms (jdapimin.c:118-240) makes of the file's colour space
+extern "C" int b200jpeg_decompress_output(const b200jpeg_source_info *src, int *width, int *height, int *color_space, int *components)
+{
+  if (!src || src->num_components < 1) return bad(B200JPEG_ERR_PARAM, "bad argument");
+  const int cs = src->jpeg_color_space;
+  if (width) *width = src->image_width;
+  if (height) *height = src->image_height;
+  if (color_space) *color_space = cs == B200JPEG_CS_GRAYSCALE ? B200JPEG_CS_GRAYSCALE : cs == B200JPEG_CS_YCbCr || cs == B200JPEG_CS_RGB ? B200JPEG_CS_RGB : B200JPEG_CS_CMYK;
+  if (components) *components = src->num_components;
   return B200JPEG_OK;
 }
 
 namespace b200 {
 
 // The descriptors of a batch of sequential files (see decode.cuh).  The unstuffed words go to alloc(bound) first.
-int build_decode_batch(const uint8_t *const *files, const size_t *sizes, int n, DecBatch &b, uint32_t *(*alloc)(void *, size_t), void *ctx)
+int build_decode_batch(const uint8_t *const *files, const size_t *sizes, int n, DecBatch &b, uint32_t *(*alloc)(void *, size_t), void *ctx, int first)
 {
+  if (b.want_markers) b.markers.resize(n);
   b.info.resize(n); b.scans.clear(); b.segs.clear(); b.tabs.clear();
   b.nsub = 0; b.nblocks = 0;
   size_t bound = 0;
   for (int i = 0; i < n; i++) {
-    if (!files[i]) { set_error("image %d: no file", i); return B200JPEG_ERR_PARAM; }
+    if (!files[i]) { set_error("image %d: no file", first + i); return B200JPEG_ERR_PARAM; }
     b200jpeg_source_info &s = b.info[i];
-    int rc = b200jpeg_parse_source(files[i], sizes[i], &s);
-    if (rc) { std::string m = b200jpeg_last_error(); set_error("image %d: %s", i, m.c_str()); return rc; }
-    if (s.sof == 0xC2) { set_error("image %d: progressive (SOF2) source: the device decode takes sequential files; pass its coefficients instead", i); return B200JPEG_ERR_UNSUPPORTED; }
+    int rc = parse_source(files[i], sizes[i], &s, b.want_markers ? &b.markers[i] : nullptr);
+    if (rc) { std::string m = b200jpeg_last_error(); set_error("image %d: %s", first + i, m.c_str()); return rc; }
+    if (s.sof == 0xC2) { set_error("image %d: progressive (SOF2) source: the device decode takes sequential files; pass its coefficients instead", first + i); return B200JPEG_ERR_UNSUPPORTED; }
     const b200jpeg_source_info &s0 = b.info[0];
     bool same = s.image_width == s0.image_width && s.image_height == s0.image_height && s.data_precision == s0.data_precision && s.num_components == s0.num_components;
     for (int c = 0; same && c < s.num_components; c++) same = s.h_samp_factor[c] == s0.h_samp_factor[c] && s.v_samp_factor[c] == s0.v_samp_factor[c];
-    if (!same) { set_error("image %d: geometry (size, precision, components, sampling) differs from image 0", i); return B200JPEG_ERR_PARAM; }
+    if (!same) { set_error("image %d: geometry (size, precision, components, sampling) differs from image 0", first + i); return B200JPEG_ERR_PARAM; }
   }
   const b200jpeg_source_info &s0 = b.info[0];
   b.W = s0.image_width; b.H = s0.image_height; b.nc = s0.num_components; b.precision = s0.data_precision;
@@ -283,7 +314,7 @@ int build_decode_batch(const uint8_t *const *files, const size_t *sizes, int n, 
     int scanned[4] = {0, 0, 0, 0};
     for (int k = 0; k < s.num_scans; k++) {
       const b200jpeg_source_scan &ss = s.scans[k];
-      if (ss.Ss != 0 || ss.Se != 63 || ss.Ah != 0 || ss.Al != 0) { set_error("image %d: scan %d is not a sequential scan (Ss=%d Se=%d Ah=%d Al=%d)", i, k, ss.Ss, ss.Se, ss.Ah, ss.Al); return B200JPEG_ERR_BAD_SOURCE; }
+      if (ss.Ss != 0 || ss.Se != 63 || ss.Ah != 0 || ss.Al != 0) { set_error("image %d: scan %d is not a sequential scan (Ss=%d Se=%d Ah=%d Al=%d)", first + i, k, ss.Ss, ss.Se, ss.Ah, ss.Al); return B200JPEG_ERR_BAD_SOURCE; }
       DecScan sc; memset(&sc, 0, sizeof sc);
       sc.img = i; sc.ncomp = ss.comps_in_scan;
       const long long mcus = scan_mcus(ss);
@@ -291,10 +322,10 @@ int build_decode_batch(const uint8_t *const *files, const size_t *sizes, int n, 
       int slot = 0;
       for (int j = 0; j < sc.ncomp; j++) {
         const int c = ss.component_index[j];
-        if (scanned[c]++) { set_error("image %d: component %d appears in two sequential scans", i, c); return B200JPEG_ERR_UNSUPPORTED; }
+        if (scanned[c]++) { set_error("image %d: component %d appears in two sequential scans", first + i, c); return B200JPEG_ERR_UNSUPPORTED; }
         const int hh = sc.ncomp == 1 ? 1 : b.h[c], vv = sc.ncomp == 1 ? 1 : b.v[c];
         sc.ci[j] = c; sc.first[j] = slot; sc.cnt[j] = hh * vv; sc.mx[c] = hh; sc.my[c] = vv;
-        if (slot + hh * vv > 10) { set_error("image %d: scan %d has more than 10 blocks per MCU", i, k); return B200JPEG_ERR_BAD_SOURCE; }   // JERR_BAD_MCU_SIZE
+        if (slot + hh * vv > 10) { set_error("image %d: scan %d has more than 10 blocks per MCU", first + i, k); return B200JPEG_ERR_BAD_SOURCE; }   // JERR_BAD_MCU_SIZE
         const int td = table(ss.dc_huff[j], true), ta = table(ss.ac_huff[j], false);
         for (int y = 0; y < vv; y++)
           for (int x = 0; x < hh; x++, slot++) { sc.comp[slot] = (int8_t)c; sc.dx[slot] = (int8_t)x; sc.dy[slot] = (int8_t)y; sc.tdc[slot] = (int16_t)td; sc.tac[slot] = (int16_t)ta; }
@@ -320,12 +351,12 @@ int build_decode_batch(const uint8_t *const *files, const size_t *sizes, int n, 
           if (r >= end) { p = end; break; }
           if (d[r] == 0x00) { o[cnt++] = 0xFF; p = r + 1; continue; }
           // RSTn (scan_data_end stops at every other marker)
-          if (!ri) { set_error("image %d: scan %d: restart marker in a scan without restart interval", i, k); return B200JPEG_ERR_BAD_SOURCE; }
-          if (d[r] - 0xD0 != (int)(sg & 7)) { set_error("image %d: scan %d: restart marker RST%d where RST%d was due", i, k, d[r] - 0xD0, (int)(sg & 7)); return B200JPEG_ERR_BAD_SOURCE; }
+          if (!ri) { set_error("image %d: scan %d: restart marker in a scan without restart interval", first + i, k); return B200JPEG_ERR_BAD_SOURCE; }
+          if (d[r] - 0xD0 != (int)(sg & 7)) { set_error("image %d: scan %d: restart marker RST%d where RST%d was due", first + i, k, d[r] - 0xD0, (int)(sg & 7)); return B200JPEG_ERR_BAD_SOURCE; }
           p = r + 1; rst = true;
           break;
         }
-        if (!rst && p >= end && sg + 1 < nseg) { set_error("image %d: scan %d ends after %lld of its %lld restart segments", i, k, sg + 1, nseg); return B200JPEG_ERR_BAD_SOURCE; }
+        if (!rst && p >= end && sg + 1 < nseg) { set_error("image %d: scan %d ends after %lld of its %lld restart segments", first + i, k, sg + 1, nseg); return B200JPEG_ERR_BAD_SOURCE; }
         const size_t words = (cnt + 3) / 4 + 2;                // at least one zero word behind the data
         memset(o + cnt, 0, words * 4 - cnt);
         DecSeg g;
@@ -336,7 +367,7 @@ int build_decode_batch(const uint8_t *const *files, const size_t *sizes, int n, 
         b.nsub += g.nsub; b.nblocks += (long long)g.nmcu * sc.nb;
         b.segs.push_back(g);
         wpos += words;
-        if (cnt >= (1u << 29)) { set_error("image %d: a restart segment of 512 MB or more", i); return B200JPEG_ERR_UNSUPPORTED; }
+        if (cnt >= (1u << 29)) { set_error("image %d: a restart segment of 512 MB or more", first + i); return B200JPEG_ERR_UNSUPPORTED; }
       }
       // anything after the last segment's MCUs (further RSTn included) is ignored, like the reference
     }

@@ -383,7 +383,31 @@ def transform():
     print("wrote", len(cases), "transform cases,", sum("error" in c for c in cases), "refused;", len(refusals), "refusals")
 
 
+def recompress():
+    """tests/golden/recompress_golden.json: for every source of tests/recompress_cases.py the md5 of the file and of the
+    pixels the reference decodes from it (build/librefdec.so: jpeg_read_scanlines of a default decompress object), and
+    for every (source, switches) of its RECOMPRESS list the md5 and size of what the reference's cjpeg writes."""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import recompress_cases as R
+    if not R.have_reference():
+        sys.exit("build/librefdec.so or oracle/_ref/cjpeg is missing: run __graft_entry__.build() with the reference build under oracle/_ref/")
+    cases = []
+    for sid in R.all_ids():
+        src, _ = R.source(sid)
+        px, info = R.ref_decompress(src)
+        cases.append({"id": sid, "src_md5": R.md5(src), "pix_md5": R.md5(px), "shape": list(px.shape), "out_color_space": info[3], "warnings": info[5]})
+    rec = []
+    for sid, sw in R.RECOMPRESS:
+        out = R.ref_cjpeg(R.source(sid)[0], sw)
+        rec.append({"source": sid, "switches": sw, "md5": R.md5(out), "size": len(out)})
+    json.dump({"generator": "tools/make_golden.py --recompress", "reference": "mozilla/mozjpeg 5.0.0 (C path, WITH_SIMD=0), oracle/_ref",
+               "cases": cases, "recompress": rec}, open(os.path.join(GOLD, "recompress_golden.json"), "w"), indent=0)
+    print("wrote", len(cases), "decompress cases,", len(rec), "recompress cases")
+
+
 def main():
+    if "--recompress" in sys.argv:
+        return recompress()
     if "--transform" in sys.argv:
         return transform()
     if "--decode" in sys.argv:

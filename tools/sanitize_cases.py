@@ -77,5 +77,8 @@ for bad in (srcs[0][:mid], srcs[0][:mid] + b"\xff\x00" * 8 + srcs[0][mid + 16:],
     except mj.B200JpegError as e:
         assert e.code == mj._abi.ERR_BAD_SOURCE, e
 n += len(enc.read_coefficients([srcs[0][:sc.data_offset + sc.data_size] + bytes(range(1, 200)) + srcs[0][sc.data_offset + sc.data_size:]]))
+# recompression (IDCT, upsampling + colour conversion, then the pixel encode): 4:2:0 at a ragged size
+rag = enc.encode_batch(mj.params_from_switches(["-revert", "-quality", "90"], 203, 131), np.stack([synth_image(11, 203, 131), synth_image(12, 203, 131)]))
+n += len(enc.recompress(mj.params_for_jpeg_input(["-baseline", "-quality", "75", "-sample", "2x2"], rag[0]), rag))
 print("sanitize cases done:", n, "files, kernel launches", enc.kernel_launches())
 enc.close()
