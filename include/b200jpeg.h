@@ -464,6 +464,33 @@ int  b200jpeg_recompress_batch(b200jpeg_encoder *enc, const b200jpeg_params *p, 
  * out_color_space (B200JPEG_CS_GRAYSCALE, _RGB, or _CMYK for 4-component files) and output_components. */
 int  b200jpeg_decompress_output(const b200jpeg_source_info *src, int *width, int *height, int *color_space, int *components);
 
+/*
+ * Decompression with the decompress object's options (djpeg -scale, -dct, -nosmooth, -fast, -grayscale, -rgb and the
+ * EXT_* output orders), sample for sample, on the sources b200jpeg_decompress_batch accepts (same checks, same
+ * messages).
+ *   scale_num / scale_denom: as jpeg_core_output_dimensions buckets them into a block size k (1/5 is k = 2); k must be
+ *     1, 2, 4 or 8 (1/8, 1/4, 1/2, 1/1), other k are B200JPEG_ERR_UNSUPPORTED.  Output: ceil(W k / 8) x ceil(H k / 8).
+ *   dct_method: B200JPEG_DCT_*, for components whose DCT_scaled_size is 8 (jddctmgr.c); smaller sizes use
+ *     jidctred.c's IDCTs whatever the method.
+ *   do_fancy_upsampling: 0 replicates chroma (and the merged upsampler, which gives the same pixels).
+ *   out_color_space: -1 for what default_decompress_parms picks; else GRAYSCALE, RGB, EXT_*, or YCbCr from a YCbCr
+ *     file.  Pairs the reference refuses are B200JPEG_ERR_PARAM "Unsupported color conversion request"; CMYK, YCCK
+ *     and B200JPEG_CS_RGB565 output are B200JPEG_ERR_UNSUPPORTED.
+ * The default options give b200jpeg_decompress_batch's and b200jpeg_recompress_batch's route and bytes.
+ */
+#define B200JPEG_CS_RGB565 16
+typedef struct { int scale_num, scale_denom, dct_method, do_fancy_upsampling, out_color_space; } b200jpeg_decompress_options;
+b200jpeg_decompress_options b200jpeg_default_decompress_options(void);
+/* jpeg_calc_output_dimensions + out_color_components for these options: B200JPEG_ERR_* as the batch would refuse. */
+int  b200jpeg_decompress_output_opts(const b200jpeg_source_info *src, const b200jpeg_decompress_options *opts,
+                                     int *width, int *height, int *color_space, int *components);
+int  b200jpeg_decompress_batch_opts(b200jpeg_encoder *enc, const b200jpeg_decompress_options *opts, const uint8_t *const *files,
+                                    const size_t *sizes, int n_images, void *pixels, int pixels_on_device, size_t row_pitch,
+                                    size_t image_stride);
+/* b200jpeg_recompress_batch from the decode with opts: p must describe the decoded (scaled) pixels. */
+int  b200jpeg_recompress_batch_opts(b200jpeg_encoder *enc, const b200jpeg_decompress_options *opts, const b200jpeg_params *p,
+                                    const uint8_t *const *files, const size_t *sizes, int n_images);
+
 /* b200jpeg_encode_batch, but stops after the entropy-coded bytes are in HBM: no device->host
  * copy, no host-side file assembly.  Used to time the device pipeline alone. */
 int  b200jpeg_encode_batch_device_only(b200jpeg_encoder *enc, const b200jpeg_params *p,

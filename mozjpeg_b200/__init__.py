@@ -14,7 +14,7 @@ import numpy as np
 
 from . import _abi as A
 from ._abi import B200JpegError, Params  # noqa: F401
-from .cjpeg import params_for_jpeg_input, params_from_switches, pnm_samples, read_pnm, read_ppm  # noqa: F401
+from .cjpeg import decompress_options, params_for_jpeg_input, params_from_switches, pnm_samples, read_pnm, read_ppm  # noqa: F401
 
 _lib = A.load()          # raises ImportError with build instructions if missing
 
@@ -184,26 +184,41 @@ class Encoder:
                 "encode_batch_coefs_transform")
         return [self.get_output(i) for i in range(n)]
 
-    def decompress(self, files: Sequence[bytes]) -> np.ndarray:
-        """jpeg_read_scanlines of a default decompress object for same-geometry sequential files, on the device:
-        an (N, H, W, C) uint8 array, (N, H, W) for gray files (b200jpeg_decompress_batch)."""
-        w, h, _, nc = decompress_output(_parse_first(files))
+    def decompress(self, files: Sequence[bytes], **opts) -> np.ndarray:
+        """jpeg_read_scanlines for same-geometry sequential files, on the device: an (N, H, W, C) uint8 array, (N, H,
+        W) for one output component.  Keyword options (decompress_options): scale=(num, denom), dct="int" | "fast" |
+        "float", fancy=True, colorspace=None; without them a default decompress object (b200jpeg_decompress_batch)."""
+        o = decompress_options(**opts) if opts else None
+        w, h, _, nc = decompress_output(_parse_first(files), **opts)
         bufs, ptrs, sizes = self._files(files)
         out = np.empty((len(bufs), h, w, nc), dtype=np.uint8)
-        A.check(_lib.b200jpeg_decompress_batch(self._h, ptrs, sizes, len(bufs), out.ctypes.data, 0, out.strides[1], out.strides[0]), "decompress_batch")
+        if o is None:
+            A.check(_lib.b200jpeg_decompress_batch(self._h, ptrs, sizes, len(bufs), out.ctypes.data, 0, out.strides[1], out.strides[0]), "decompress_batch")
+        else:
+            A.check(_lib.b200jpeg_decompress_batch_opts(self._h, C.byref(o), ptrs, sizes, len(bufs), out.ctypes.data, 0, out.strides[1], out.strides[0]),
+                    "decompress_batch_opts")
         return out[..., 0] if nc == 1 else out
 
-    def decompress_ptr(self, files: Sequence[bytes], ptr: int, row_pitch: int, image_stride: int) -> None:
+    def decompress_ptr(self, files: Sequence[bytes], ptr: int, row_pitch: int, image_stride: int, **opts) -> None:
         """Raw-pointer form of decompress: the pixels go to device memory at ``ptr`` and stay there."""
         bufs, ptrs, sizes = self._files(files)
-        A.check(_lib.b200jpeg_decompress_batch(self._h, ptrs, sizes, len(bufs), ptr, 1, row_pitch, image_stride), "decompress_batch")
+        if not opts:
+            A.check(_lib.b200jpeg_decompress_batch(self._h, ptrs, sizes, len(bufs), ptr, 1, row_pitch, image_stride), "decompress_batch")
+        else:
+            o = decompress_options(**opts)
+            A.check(_lib.b200jpeg_decompress_batch_opts(self._h, C.byref(o), ptrs, sizes, len(bufs), ptr, 1, row_pitch, image_stride), "decompress_batch_opts")
 
-    def recompress(self, p: Params, files: Sequence[bytes]) -> List[bytes]:
+    def recompress(self, p: Params, files: Sequence[bytes], **opts) -> List[bytes]:
         """cjpeg with JPEG input files (b200jpeg_recompress_batch): the files decoded to pixels on the device and
-        encoded from there with ``p`` (cjpeg.params_for_jpeg_input builds it); each output carries its source's COM and
-        APPn segments as cjpeg copies them."""
+        encoded from there with ``p`` (cjpeg.params_for_jpeg_input builds it, with the same options); each output
+        carries its source's COM and APPn segments as cjpeg copies them.  Keyword options as for decompress: a scaled
+        rendition is recompressed from the scaled decode (b200jpeg_recompress_batch_opts)."""
         bufs, ptrs, sizes = self._files(files)
-        A.check(_lib.b200jpeg_recompress_batch(self._h, C.byref(p), ptrs, sizes, len(bufs)), "recompress_batch")
+        if not opts:
+            A.check(_lib.b200jpeg_recompress_batch(self._h, C.byref(p), ptrs, sizes, len(bufs)), "recompress_batch")
+        else:
+            o = decompress_options(**opts)
+            A.check(_lib.b200jpeg_recompress_batch_opts(self._h, C.byref(o), C.byref(p), ptrs, sizes, len(bufs)), "recompress_batch_opts")
         return [self.get_output(i) for i in range(len(bufs))]
 
     def last_decode_sync(self):
@@ -316,11 +331,16 @@ def _parse_first(files: Sequence[bytes]) -> A.SourceInfo:
     return info
 
 
-def decompress_output(info: "A.SourceInfo"):
+def decompress_output(info: "A.SourceInfo", **opts):
     """(width, height, out_color_space, output_components) of a source decoded with the decompress defaults
-    (b200jpeg_decompress_output): what rdjpeg.c copies into the compress object."""
+    (b200jpeg_decompress_output): what rdjpeg.c copies into the compress object.  With keyword options
+    (decompress_options) the same for a decompress object set up with them (b200jpeg_decompress_output_opts)."""
     w = C.c_int(0); h = C.c_int(0); cs = C.c_int(0); nc = C.c_int(0)
-    A.check(_lib.b200jpeg_decompress_output(C.byref(info), C.byref(w), C.byref(h), C.byref(cs), C.byref(nc)), "decompress_output")
+    if not opts:
+        A.check(_lib.b200jpeg_decompress_output(C.byref(info), C.byref(w), C.byref(h), C.byref(cs), C.byref(nc)), "decompress_output")
+    else:
+        o = decompress_options(**opts)
+        A.check(_lib.b200jpeg_decompress_output_opts(C.byref(info), C.byref(o), C.byref(w), C.byref(h), C.byref(cs), C.byref(nc)), "decompress_output_opts")
     return w.value, h.value, cs.value, nc.value
 
 

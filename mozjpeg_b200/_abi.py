@@ -95,6 +95,13 @@ class SourceScan(C.Structure):
     ]
 
 
+class DecompressOptions(C.Structure):
+    """b200jpeg_decompress_options: scale_num / scale_denom, dct_method (B200JPEG_DCT_*), do_fancy_upsampling and
+    out_color_space (-1: the decompressor's default)."""
+    _fields_ = [("scale_num", C.c_int), ("scale_denom", C.c_int), ("dct_method", C.c_int), ("do_fancy_upsampling", C.c_int),
+                ("out_color_space", C.c_int)]
+
+
 class SourceInfo(C.Structure):
     """b200jpeg_source_info: the marker segments of a source JPEG file (b200jpeg_parse_source)."""
     _fields_ = [
@@ -146,6 +153,7 @@ EXPORTS = [
     "b200jpeg_parse_source", "b200jpeg_decode_coefs_batch", "b200jpeg_transcode_batch", "b200jpeg_last_decode_sync",
     "b200jpeg_transform_setup", "b200jpeg_transcode_batch_transform", "b200jpeg_encode_batch_coefs_transform",
     "b200jpeg_decompress_batch", "b200jpeg_recompress_batch", "b200jpeg_decompress_output",
+    "b200jpeg_default_decompress_options", "b200jpeg_decompress_output_opts", "b200jpeg_decompress_batch_opts", "b200jpeg_recompress_batch_opts",
 ]
 
 _lib = None
@@ -216,6 +224,11 @@ def load() -> C.CDLL:
     lib.b200jpeg_recompress_batch.argtypes = [C.c_void_p, P, PB, PS, C.c_int]; lib.b200jpeg_recompress_batch.restype = C.c_int
     PI = C.POINTER(C.c_int)
     lib.b200jpeg_decompress_output.argtypes = [C.POINTER(SourceInfo), PI, PI, PI, PI]; lib.b200jpeg_decompress_output.restype = C.c_int
+    PO = C.POINTER(DecompressOptions)
+    lib.b200jpeg_default_decompress_options.argtypes = []; lib.b200jpeg_default_decompress_options.restype = DecompressOptions
+    lib.b200jpeg_decompress_output_opts.argtypes = [C.POINTER(SourceInfo), PO, PI, PI, PI, PI]; lib.b200jpeg_decompress_output_opts.restype = C.c_int
+    lib.b200jpeg_decompress_batch_opts.argtypes = [C.c_void_p, PO, PB, PS, C.c_int, C.c_void_p, C.c_int, C.c_size_t, C.c_size_t]; lib.b200jpeg_decompress_batch_opts.restype = C.c_int
+    lib.b200jpeg_recompress_batch_opts.argtypes = [C.c_void_p, PO, P, PB, PS, C.c_int]; lib.b200jpeg_recompress_batch_opts.restype = C.c_int
     lib.b200jpeg_last_error.argtypes = []; lib.b200jpeg_last_error.restype = C.c_char_p
     lib.b200jpeg_version.argtypes = []; lib.b200jpeg_version.restype = C.c_char_p
     _lib = lib

@@ -335,16 +335,46 @@ def params_from_switches(switches: Sequence[str], width: int, height: int,
     return p
 
 
-def params_for_jpeg_input(switches: Sequence[str], jpeg: bytes) -> A.Params:
+def params_for_jpeg_input(switches: Sequence[str], jpeg: bytes, **opts) -> A.Params:
     """cjpeg's cinfo at jpeg_start_compress for a JPEG input file: rdjpeg.c's start_input_jpeg takes the image size,
     in_color_space (the decompressor's out_color_space) and input_components from the source (data_precision is 8 for
-    every source the device decodes), then jpeg_default_colorspace and the second switch pass run as for any input."""
+    every source the device decodes), then jpeg_default_colorspace and the second switch pass run as for any input.
+    Keyword options (decompress_options: scale, dct, fancy, colorspace) describe a rendition decoded with them, for
+    Encoder.recompress with the same options; without them the decompress defaults."""
     lib = A.load()
     info = A.SourceInfo()
     A.check(lib.b200jpeg_parse_source(bytes(jpeg), len(jpeg), C.byref(info)), "parse_source")
     w = C.c_int(0); h = C.c_int(0); cs = C.c_int(0); nc = C.c_int(0)
-    A.check(lib.b200jpeg_decompress_output(C.byref(info), C.byref(w), C.byref(h), C.byref(cs), C.byref(nc)), "decompress_output")
+    if not opts:
+        A.check(lib.b200jpeg_decompress_output(C.byref(info), C.byref(w), C.byref(h), C.byref(cs), C.byref(nc)), "decompress_output")
+    else:
+        o = decompress_options(**opts)
+        A.check(lib.b200jpeg_decompress_output_opts(C.byref(info), C.byref(o), C.byref(w), C.byref(h), C.byref(cs), C.byref(nc)), "decompress_output_opts")
     return params_from_switches(switches, w.value, h.value, nc.value, in_color_space=cs.value)
+
+
+DCT_METHODS = {"int": 0, "fast": 1, "float": 2}
+# out_color_space names (J_COLOR_SPACE, B200JPEG_CS_*)
+COLOR_SPACES = {"gray": 1, "grayscale": 1, "rgb": 2, "ycbcr": 3, "cmyk": 4, "ycck": 5, "ext_rgb": 6, "rgbx": 7, "bgr": 8, "bgrx": 9,
+                "xbgr": 10, "xrgb": 11, "rgba": 12, "bgra": 13, "abgr": 14, "argb": 15, "rgb565": 16}
+
+
+def decompress_options(scale=(1, 1), dct: str = "int", fancy: bool = True, colorspace=None) -> A.DecompressOptions:
+    """b200jpeg_decompress_options from keywords: scale=(scale_num, scale_denom), dct "int" | "fast" | "float"
+    (JDCT_ISLOW / IFAST / FLOAT), fancy (do_fancy_upsampling), colorspace None (the decompressor's default), a
+    B200JPEG_CS_* number or a name of COLOR_SPACES."""
+    if dct not in DCT_METHODS:
+        raise ValueError(f"dct must be one of {sorted(DCT_METHODS)}, not {dct!r}")
+    if colorspace is None:
+        cs = -1
+    elif isinstance(colorspace, str):
+        if colorspace.lower() not in COLOR_SPACES:
+            raise ValueError(f"unknown colorspace {colorspace!r}")
+        cs = COLOR_SPACES[colorspace.lower()]
+    else:
+        cs = int(colorspace)
+    num, denom = scale
+    return A.DecompressOptions(int(num), int(denom), DCT_METHODS[dct], int(bool(fancy)), cs)
 
 
 def read_pnm(data: bytes):

@@ -20,6 +20,10 @@ namespace b200 {
 #define DEC_SUB_BITS 1024      // bits per speculatively decoded subsequence
 #define DEC_CTA 128            // subsequences per CTA of the synchronisation kernel
 
+// the colour conversions behind the decode with options (DecPlan::conv, k_upsample_opts): grayscale_convert,
+// ycc_rgb_convert, null_convert / rgb_rgb_convert, gray_rgb_convert, rgb_gray_convert
+enum { UPS_GRAY = 0, UPS_YCC_RGB = 1, UPS_COPY3 = 2, UPS_GRAY_RGB = 3, UPS_RGB_GRAY = 4 };
+
 // jpeg_make_d_derived_tbl (jdhuff.c:143-261): 8-bit lookahead ((length << 8) | symbol, 0 = longer code), maxcode /
 // valoffset per code length
 struct DecTable { uint16_t look[256]; int32_t maxcode[18]; int32_t valoff[18]; uint8_t huffval[256]; };

@@ -147,7 +147,7 @@ struct b200jpeg_encoder {
   // decompression to pixels (b200jpeg_decompress_batch / b200jpeg_recompress_batch): one chunk's sample planes and
   // quantization tables, the whole batch's pixels where the caller gave no device buffer, the stage times summed over
   // the chunks, and per image the source's COM / APPn segments a recompress copies into its file
-  DevBuf d_dec_samples, d_dec_quant, d_dec_pixels;
+  DevBuf d_dec_samples, d_dec_quant, d_dec_pixels, d_dec_mtab;   // d_dec_mtab: ifast / float multiplier tables
   cudaEvent_t pix_ev[3] = {nullptr, nullptr, nullptr};
   float dec_ms[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   std::vector<std::vector<uint8_t>> dec_markers;
@@ -1781,10 +1781,87 @@ static int check_decompress_source(const b200jpeg_source_info &s, int i)
   return B200JPEG_OK;
 }
 
+// the multiplier tables of jddctmgr.c start_pass for the ifast and float IDCTs, from one quantization table
+static const int kAanScales[64] = {
+  16384, 22725, 21407, 19266, 16384, 12873,  8867,  4520, 22725, 31521, 29692, 26722, 22725, 17855, 12299,  6270,
+  21407, 29692, 27969, 25172, 21407, 16819, 11585,  5906, 19266, 26722, 25172, 22654, 19266, 15137, 10426,  5315,
+  16384, 22725, 21407, 19266, 16384, 12873,  8867,  4520, 12873, 17855, 16819, 15137, 12873, 10114,  6967,  3552,
+   8867, 12299, 11585, 10426,  8867,  6967,  4799,  2446,  4520,  6270,  5906,  5315,  4520,  3552,  2446,  1247};
+static const double kAanScaleFactor[8] = {1.0, 1.387039845, 1.306562965, 1.175875602, 1.0, 0.785694958, 0.541196100, 0.275899379};
+static void method_table(int method, const uint16_t *q, uint32_t *out)
+{
+  for (int i = 0; i < 64; i++) {
+    if (method == B200JPEG_DCT_IFAST) {
+      const int v = (int)(((long long)q[i] * kAanScales[i] + 2048) >> 12);                 // DESCALE(.., 14 - IFAST_SCALE_BITS)
+      memcpy(&out[i], &v, 4);
+    } else {
+      const float f = (float)((double)q[i] * kAanScaleFactor[i >> 3] * kAanScaleFactor[i & 7]);
+      memcpy(&out[i], &f, 4);
+    }
+  }
+}
+
+// the IDCT and upsampling / colour conversion stages of one decoded chunk (e->dec) for a non-default plan: each
+// needed component through the IDCT of its DCT_scaled_size into a plane of wib * size samples a row, then
+// k_upsample_opts into the pixels.  qt / mt: host staging for the tables.
+static int idct_upsample_opts(b200jpeg_encoder *e, const DecPlan &plan, int nk, uint8_t *pix, size_t row_pitch, size_t image_stride,
+                              std::vector<uint16_t> &qt, std::vector<uint32_t> &mt)
+{
+  const DecBatch &b = e->dec;
+  const int nc = b.nc;
+  cudaStream_t s = e->stream;
+  size_t off[4] = {0, 0, 0, 0}, total = 0;
+  bool need_mt = false;
+  for (int c = 0; c < nc; c++) {
+    if (!plan.needed[c]) continue;
+    off[c] = total; total += ((size_t)nk * b.hib[c] * b.wib[c] * plan.ssize[c] * plan.ssize[c] + 255) & ~(size_t)255;
+    need_mt |= plan.ssize[c] == 8 && plan.method != B200JPEG_DCT_ISLOW;
+  }
+  int rc;
+  if ((rc = e->d_dec_samples.reserve(total)) || (rc = e->d_dec_quant.reserve((size_t)nk * nc * 128)) ||
+      (need_mt && (rc = e->d_dec_mtab.reserve((size_t)nk * nc * 256)))) return rc;
+  qt.resize((size_t)nk * nc * 64);
+  for (int i = 0; i < nk; i++)
+    for (int c = 0; c < nc; c++) memcpy(&qt[((size_t)i * nc + c) * 64], b.info[i].comp_quant[c], 128);
+  CU(cudaMemcpyAsync(e->d_dec_quant.p, qt.data(), qt.size() * 2, cudaMemcpyHostToDevice, s));
+  if (need_mt) {
+    mt.resize((size_t)nk * nc * 64);
+    for (size_t t = 0; t < (size_t)nk * nc; t++) method_table(plan.method, &qt[t * 64], &mt[t * 64]);
+    CU(cudaMemcpyAsync(e->d_dec_mtab.p, mt.data(), mt.size() * 4, cudaMemcpyHostToDevice, s));
+  }
+  CU(cudaEventRecord(e->pix_ev[0], s));
+  UpsOpt u;
+  memset(&u, 0, sizeof u);
+  for (int c = 0; c < nc; c++) {
+    if (!plan.needed[c]) continue;
+    const int sz = plan.ssize[c];
+    uint8_t *dst = e->d_dec_samples.as<uint8_t>() + off[c];
+    const bool by_method = sz == 8 && plan.method != B200JPEG_DCT_ISLOW;
+    const void *tab = by_method ? static_cast<const void *>(e->d_dec_mtab.as<uint32_t>() + c * 64) : static_cast<const void *>(e->d_dec_quant.as<uint16_t>() + c * 64);
+    launch_idct_opts(sz, plan.method, reinterpret_cast<const int16_t *>(e->d_dec_planes.as<uint8_t>() + e->dec_plane_off[c]), tab, nc * 64, dst, b.wib[c], b.hib[c], nk, s);
+    if (c < 3) {
+      u.plane[c] = dst; u.pitch[c] = b.wib[c] * sz; u.stride[c] = (long long)b.hib[c] * sz * u.pitch[c];
+      u.dw[c] = plan.dw[c]; u.dh[c] = plan.dh[c]; u.hr[c] = plan.hr[c]; u.vr[c] = plan.vr[c]; u.fancy[c] = plan.fancy[c];
+    }
+  }
+  CU(cudaEventRecord(e->pix_ev[1], s));
+  u.nin = plan.nin; u.conv = plan.conv; u.ps = plan.ps;
+  for (int k = 0; k < 4; k++) u.off[k] = plan.off[k];
+  launch_upsample_opts(u, pix, row_pitch, image_stride, plan.out_w, plan.out_h, nk, s);
+  CU(cudaEventRecord(e->pix_ev[2], s));
+  CU(cudaGetLastError());
+  CU(cudaStreamSynchronize(s));
+  for (int k = 0; k < 6; k++) { float ms = 0.f; cudaEventElapsedTime(&ms, e->dec_ev[k], e->dec_ev[k + 1]); e->dec_ms[k] += ms; }
+  for (int k = 0; k < 2; k++) { float ms = 0.f; cudaEventElapsedTime(&ms, e->pix_ev[k], e->pix_ev[k + 1]); e->dec_ms[6 + k] += ms; }
+  return B200JPEG_OK;
+}
+
 // jpeg_read_scanlines for a batch of files: entropy decode, IDCT and upsampling / colour conversion chunk by chunk
 // (the coefficient and sample planes are one chunk's), into pixels on the device.
+// opts: the decompress object's options (nullptr: its defaults); options that give what the defaults give take the
+// default route.
 static int decompress_files(b200jpeg_encoder *e, const uint8_t *const *files, const size_t *sizes, int n, uint8_t *pix, size_t row_pitch, size_t image_stride,
-                            bool want_markers)
+                            bool want_markers, const b200jpeg_decompress_options *opts = nullptr)
 {
   // every refusal comes before any device work
   b200jpeg_source_info s0;
@@ -1804,7 +1881,11 @@ static int decompress_files(b200jpeg_encoder *e, const uint8_t *const *files, co
   }
   const int W = s0.image_width, H = s0.image_height, nc = s0.num_components;
   const int hx = nc == 3 ? s0.h_samp_factor[0] : 1, vx = nc == 3 ? s0.v_samp_factor[0] : 1;
-  if (row_pitch < (size_t)W * nc || (n > 1 && image_stride < row_pitch * (size_t)(H - 1) + (size_t)W * nc)) { set_error("row_pitch or image_stride smaller than the decoded image (%dx%d, %d components)", W, H, nc); return B200JPEG_ERR_PARAM; }
+  DecPlan plan;
+  if (opts) { int rc = plan_decompress(s0, *opts, plan); if (rc) return rc; }
+  const bool def = plan.is_default;
+  const int OW = def ? W : plan.out_w, OH = def ? H : plan.out_h, onc = def ? nc : plan.out_nc;
+  if (row_pitch < (size_t)OW * onc || (n > 1 && image_stride < row_pitch * (size_t)(OH - 1) + (size_t)OW * onc)) { set_error("row_pitch or image_stride smaller than the decoded image (%dx%d, %d components)", OW, OH, onc); return B200JPEG_ERR_PARAM; }
   CU(cudaSetDevice(e->device));
   for (cudaEvent_t &ev : e->pix_ev) if (!ev) CU(cudaEventCreate(&ev));
   for (float &m : e->dec_ms) m = 0.f;
@@ -1816,12 +1897,14 @@ static int decompress_files(b200jpeg_encoder *e, const uint8_t *const *files, co
   const int C = std::min(n, e->chunk_images_override > 0 ? e->chunk_images_override : (int)std::max(1LL, 1600000LL / std::max(1LL, per)));
   cudaStream_t s = e->stream;
   std::vector<uint16_t> qt;
+  std::vector<uint32_t> mt;
   for (int i0 = 0; i0 < n; i0 += C) {
     const int nk = std::min(C, n - i0);
     int rc = decode_files(e, files + i0, sizes + i0, nk, i0);
     if (rc) return rc;
     const DecBatch &b = e->dec;
     if (want_markers) for (int i = 0; i < nk; i++) e->dec_markers[i0 + i].swap(e->dec.markers[i]);
+    if (!def) { if ((rc = idct_upsample_opts(e, plan, nk, pix + (size_t)i0 * image_stride, row_pitch, image_stride, qt, mt))) return rc; continue; }
     size_t off[4] = {0, 0, 0, 0}, total = 0;
     for (int c = 0; c < nc; c++) { off[c] = total; total += ((size_t)nk * b.hib[c] * b.wib[c] * 64 + 255) & ~(size_t)255; }
     if ((rc = e->d_dec_samples.reserve(total)) || (rc = e->d_dec_quant.reserve((size_t)nk * nc * 128))) return rc;
@@ -1857,12 +1940,9 @@ static void add_decompress_stage_times(b200jpeg_encoder *e)
   for (int k = 0; k < 8; k++) { e->stage_names.push_back(k < 6 ? kDecStages[k] : extra[k - 6]); e->stage_ms.push_back(e->dec_ms[k]); e->stage_calls.push_back(1); }
 }
 
-}  // namespace b200
-
-extern "C" {
-
-int b200jpeg_decompress_batch(b200jpeg_encoder *e, const uint8_t *const *files, const size_t *sizes, int n_images,
-                              void *pixels, int pixels_on_device, size_t row_pitch, size_t image_stride)
+// b200jpeg_decompress_batch (opts nullptr) and b200jpeg_decompress_batch_opts
+static int decompress_batch(b200jpeg_encoder *e, const b200jpeg_decompress_options *opts, const uint8_t *const *files, const size_t *sizes, int n_images,
+                            void *pixels, int pixels_on_device, size_t row_pitch, size_t image_stride)
 {
   if (!e || !files || !sizes || !pixels || n_images <= 0) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
   uint8_t *dst = static_cast<uint8_t *>(pixels);
@@ -1871,7 +1951,9 @@ int b200jpeg_decompress_batch(b200jpeg_encoder *e, const uint8_t *const *files, 
     // decode into a buffer of the batch's size on the device, then copy the rows out
     b200jpeg_source_info *s = new b200jpeg_source_info;
     int rc = b200jpeg_parse_source(files[0], files[0] ? sizes[0] : 0, s);
-    const size_t row = rc ? 0 : (size_t)s->image_width * s->num_components, rows = rc ? 0 : (size_t)s->image_height;
+    int ow = 0, oh = 0, ocs = 0, onc = 0;
+    if (!rc) rc = opts ? b200jpeg_decompress_output_opts(s, opts, &ow, &oh, &ocs, &onc) : b200jpeg_decompress_output(s, &ow, &oh, &ocs, &onc);
+    const size_t row = rc ? 0 : (size_t)ow * onc, rows = rc ? 0 : (size_t)oh;
     delete s;
     if (rc) { std::string m = b200jpeg_last_error(); set_error("image 0: %s", m.c_str()); return rc; }
     if (row_pitch < row || (n_images > 1 && image_stride < row_pitch * (rows - 1) + row)) { set_error("row_pitch or image_stride smaller than the decoded image"); return B200JPEG_ERR_PARAM; }
@@ -1879,22 +1961,24 @@ int b200jpeg_decompress_batch(b200jpeg_encoder *e, const uint8_t *const *files, 
     CU(cudaSetDevice(e->device));
     if ((rc = e->d_dec_pixels.reserve(ds * (size_t)n_images))) return rc;
     dst = e->d_dec_pixels.as<uint8_t>();
-    rc = b200::decompress_files(e, files, sizes, n_images, dst, dp, ds, false);
+    rc = decompress_files(e, files, sizes, n_images, dst, dp, ds, false, opts);
     if (rc) return rc;
     for (int i = 0; i < n_images; i++)
       CU(cudaMemcpy2DAsync(static_cast<uint8_t *>(pixels) + (size_t)i * image_stride, row_pitch, dst + (size_t)i * ds, dp, row, rows, cudaMemcpyDeviceToHost, e->stream));
     CU(cudaStreamSynchronize(e->stream));
   } else {
-    int rc = b200::decompress_files(e, files, sizes, n_images, dst, dp, ds, false);
+    int rc = decompress_files(e, files, sizes, n_images, dst, dp, ds, false, opts);
     if (rc) return rc;
   }
   e->pending_marks = 0;
   e->stage_names.clear(); e->stage_ms.clear(); e->stage_calls.clear();
-  b200::add_decompress_stage_times(e);
+  add_decompress_stage_times(e);
   return B200JPEG_OK;
 }
 
-int b200jpeg_recompress_batch(b200jpeg_encoder *e, const b200jpeg_params *p, const uint8_t *const *files, const size_t *sizes, int n_images)
+// b200jpeg_recompress_batch (opts nullptr) and b200jpeg_recompress_batch_opts
+static int recompress_batch(b200jpeg_encoder *e, const b200jpeg_decompress_options *opts, const b200jpeg_params *p, const uint8_t *const *files,
+                            const size_t *sizes, int n_images)
 {
   if (!e || !p || !files || !sizes || n_images <= 0) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
   int rc = b200jpeg_validate(p);
@@ -1905,7 +1989,7 @@ int b200jpeg_recompress_batch(b200jpeg_encoder *e, const b200jpeg_params *p, con
     b200jpeg_source_info *s = new b200jpeg_source_info;
     int w = 0, h = 0, cs = 0, nc = 0;
     rc = files[0] ? b200jpeg_parse_source(files[0], sizes[0], s) : B200JPEG_OK;
-    if (!rc && files[0]) rc = b200jpeg_decompress_output(s, &w, &h, &cs, &nc);
+    if (!rc && files[0]) rc = opts ? b200jpeg_decompress_output_opts(s, opts, &w, &h, &cs, &nc) : b200jpeg_decompress_output(s, &w, &h, &cs, &nc);
     delete s;
     if (rc) { std::string m = b200jpeg_last_error(); set_error("image 0: %s", m.c_str()); return rc; }
     if (files[0] && (w != p->image_width || h != p->image_height || cs != p->in_color_space || nc != p->input_components)) {
@@ -1916,10 +2000,39 @@ int b200jpeg_recompress_batch(b200jpeg_encoder *e, const b200jpeg_params *p, con
   }
   CU(cudaSetDevice(e->device));
   if ((rc = e->d_dec_pixels.reserve(stride * (size_t)n_images))) return rc;
-  if ((rc = b200::decompress_files(e, files, sizes, n_images, e->d_dec_pixels.as<uint8_t>(), pitch, stride, true))) return rc;
-  if ((rc = b200::encode_common(e, p, e->d_dec_pixels.p, 1, pitch, stride, n_images, false, nullptr, nullptr, &e->dec_markers))) return rc;
-  b200::add_decompress_stage_times(e);
+  if ((rc = decompress_files(e, files, sizes, n_images, e->d_dec_pixels.as<uint8_t>(), pitch, stride, true, opts))) return rc;
+  if ((rc = encode_common(e, p, e->d_dec_pixels.p, 1, pitch, stride, n_images, false, nullptr, nullptr, &e->dec_markers))) return rc;
+  add_decompress_stage_times(e);
   return B200JPEG_OK;
+}
+
+}  // namespace b200
+
+extern "C" {
+
+int b200jpeg_decompress_batch(b200jpeg_encoder *e, const uint8_t *const *files, const size_t *sizes, int n_images,
+                              void *pixels, int pixels_on_device, size_t row_pitch, size_t image_stride)
+{
+  return b200::decompress_batch(e, nullptr, files, sizes, n_images, pixels, pixels_on_device, row_pitch, image_stride);
+}
+
+int b200jpeg_decompress_batch_opts(b200jpeg_encoder *e, const b200jpeg_decompress_options *opts, const uint8_t *const *files,
+                                   const size_t *sizes, int n_images, void *pixels, int pixels_on_device, size_t row_pitch, size_t image_stride)
+{
+  if (!opts) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
+  return b200::decompress_batch(e, opts, files, sizes, n_images, pixels, pixels_on_device, row_pitch, image_stride);
+}
+
+int b200jpeg_recompress_batch(b200jpeg_encoder *e, const b200jpeg_params *p, const uint8_t *const *files, const size_t *sizes, int n_images)
+{
+  return b200::recompress_batch(e, nullptr, p, files, sizes, n_images);
+}
+
+int b200jpeg_recompress_batch_opts(b200jpeg_encoder *e, const b200jpeg_decompress_options *opts, const b200jpeg_params *p,
+                                   const uint8_t *const *files, const size_t *sizes, int n_images)
+{
+  if (!opts) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
+  return b200::recompress_batch(e, opts, p, files, sizes, n_images);
 }
 
 int b200jpeg_decode_coefs_batch(b200jpeg_encoder *e, const uint8_t *const *files, const size_t *sizes, int n_images,
@@ -2010,7 +2123,7 @@ void b200jpeg_encoder_destroy(b200jpeg_encoder *e)
   for (DevBuf *b : db) b->release();
   for (int i = 0; i < MAX_ARENAS; i++) e->ar[i].release();
   DevBuf *dd[] = {&e->d_dec_words, &e->d_dec_segs, &e->d_dec_scans, &e->d_dec_tabs, &e->d_dec_out, &e->d_dec_rec, &e->d_dec_pre, &e->d_dec_tsum, &e->d_dec_dcd, &e->d_dec_planes, &e->d_dec_stat,
-                  &e->d_dec_samples, &e->d_dec_quant, &e->d_dec_pixels};
+                  &e->d_dec_samples, &e->d_dec_quant, &e->d_dec_pixels, &e->d_dec_mtab};
   for (DevBuf *b : dd) b->release();
   for (cudaEvent_t ev : e->dec_ev) if (ev) cudaEventDestroy(ev);
   for (cudaEvent_t ev : e->pix_ev) if (ev) cudaEventDestroy(ev);

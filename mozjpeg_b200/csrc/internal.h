@@ -29,4 +29,17 @@ struct DecBatch {
 };
 // first: the batch index of files[0], for the messages (a caller that decodes a batch in chunks)
 int build_decode_batch(const uint8_t *const *files, const size_t *sizes, int n, DecBatch &b, uint32_t *(*alloc)(void *, size_t), void *ctx, int first = 0);
+
+// What jpeg_calc_output_dimensions, jinit_upsampler and jinit_color_deconverter decide for one source and one set of
+// decompress options (source.cpp): output size and format, per component its DCT_scaled_size, downsampled size,
+// replication factors after IDCT scaling and upsampler, whether it is needed at all, and the conversion (UPS_* of
+// kernels.cuh) into ps bytes per pixel at off[].  is_default: the options give what a default decompress object gives.
+struct DecPlan {
+  int k = 8, method = 0, out_w = 0, out_h = 0, out_cs = 0, out_nc = 0;
+  int ssize[4] = {8, 8, 8, 8}, dw[4] = {0, 0, 0, 0}, dh[4] = {0, 0, 0, 0}, hr[4] = {1, 1, 1, 1}, vr[4] = {1, 1, 1, 1};
+  bool fancy[4] = {false, false, false, false}, needed[4] = {true, true, true, true};
+  int conv = 0, nin = 1, ps = 1, off[4] = {0, 0, 0, 0};
+  bool is_default = true;
+};
+int plan_decompress(const b200jpeg_source_info &s, const b200jpeg_decompress_options &o, DecPlan &p);
 }

@@ -4437,4 +4437,295 @@ int launch_upsample_color(int hx, int vx, int nc, const uint8_t *const *planes, 
   return -1;
 }
 
+// ------------------------------------------------------------------ decompression with the decompress object's options
+// (scale_num / scale_denom, dct_method, do_fancy_upsampling, out_color_space): the reduced IDCTs of jidctred.c, the
+// ifast and float IDCTs, and one upsampling / colour conversion kernel whose choices are parameters
+
+// jpeg_idct_4x4 / jpeg_idct_2x2 (jidctred.c:121-275, 279-387; CONST_BITS 13, PASS1_BITS 2, JLONG intermediates) and
+// jpeg_idct_1x1 (:390-407), with the islow-style table (ISLOW_MULT_TYPE int without SIMD: the entries as unsigned
+// 16-bit values).  N = 4 and 2: eight lanes per block as in k_idct_islow; lane r loads row r, lane c transforms column c
+// (column 4, and for N = 2 columns 2, 4 and 6, are skipped as the reference skips them), lanes 0 .. N-1 one row each.
+// The reference's shortcuts for all-zero AC columns and rows give what the general path gives (pass 1: DESCALE of
+// dq << (CONST_BITS + 1 or 2) is dq << PASS1_BITS, truncated to int the same way; pass 2: both are DESCALE(w0, 5)), so
+// there is no branch.  N = 1: one thread per block reads the DC term only.
+// out: [n][hib * N][wib * N] samples.
+template <int N>
+__global__ void __launch_bounds__(IDCT_BLOCKS * 8) k_idct_red(const int16_t *__restrict__ coef, const uint16_t *__restrict__ quant, int qstride,
+                                                              uint8_t *__restrict__ out, int wib, int hib, long long nblocks)
+{
+  const long long per = (long long)wib * hib;
+  if (N == 1) {
+    const long long blk = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (blk >= nblocks) return;
+    const long long img = blk / per, rem = blk - img * per;
+    const int by = (int)(rem / wib), bx = (int)(rem - (long long)by * wib);
+    const int dq = (int)__ldg(coef + blk * 64) * (int)__ldg(quant + img * qstride);
+    out[(img * hib + by) * (long long)wib + bx] = (uint8_t)idct_range_limit((int)(((long long)dq + 4) >> 3));
+    return;
+  }
+  __shared__ int4 s_coef[IDCT_BLOCKS * 8];
+  __shared__ int s_ws[IDCT_BLOCKS * IDCT_WS];
+  const int lb = threadIdx.x >> 3, lane = threadIdx.x & 7;
+  const long long blk = (long long)blockIdx.x * IDCT_BLOCKS + lb;
+  const bool valid = blk < nblocks;
+  const long long img = valid ? blk / per : 0;
+  s_coef[threadIdx.x] = valid ? reinterpret_cast<const int4 *>(coef)[blk * 8 + lane] : make_int4(0, 0, 0, 0);
+  __syncwarp();
+  const bool col_used = N == 4 ? lane != 4 : (lane & 1) || lane == 0;
+  if (col_used) {                                         // pass 1: column `lane` -> ws rows 0 .. N-1
+    const int16_t *c = reinterpret_cast<const int16_t *>(s_coef + lb * 8) + lane;
+    const uint16_t *q = quant + img * qstride + lane;
+    long long d[8];
+#pragma unroll
+    for (int r = 0; r < 8; r++) d[r] = (N == 4 && r == 4) || (N == 2 && (r == 2 || r == 4 || r == 6)) ? 0 : (long long)((int)c[r * 8] * (int)q[r * 8]);
+    int *ws = s_ws + lb * IDCT_WS + lane;
+    if (N == 4) {
+      const long long t0 = d[0] * 16384, t2 = d[2] * 15137 + d[6] * -6270;
+      const long long tmp10 = t0 + t2, tmp12 = t0 - t2;
+      const long long o0 = d[7] * -1730 + d[5] * 11893 + d[3] * -17799 + d[1] * 8697;
+      const long long o2 = d[7] * -4176 + d[5] * -4926 + d[3] * 7373 + d[1] * 20995;
+      ws[0 * 9] = (int)((tmp10 + o2 + 2048) >> 12); ws[3 * 9] = (int)((tmp10 - o2 + 2048) >> 12);
+      ws[1 * 9] = (int)((tmp12 + o0 + 2048) >> 12); ws[2 * 9] = (int)((tmp12 - o0 + 2048) >> 12);
+    } else {
+      const long long tmp10 = d[0] * 32768, o0 = d[7] * -5906 + d[5] * 6967 + d[3] * -10426 + d[1] * 29692;
+      ws[0 * 9] = (int)((tmp10 + o0 + 4096) >> 13); ws[1 * 9] = (int)((tmp10 - o0 + 4096) >> 13);
+    }
+  }
+  __syncwarp();
+  if (valid && lane < N) {                                // pass 2: row `lane`
+    const int *w = s_ws + lb * IDCT_WS + lane * 9;
+    const long long rem = blk - img * per;
+    const int by = (int)(rem / wib), bx = (int)(rem - (long long)by * wib);
+    uint8_t *dst = out + ((img * hib + by) * N + lane) * ((long long)wib * N) + bx * N;
+    if (N == 4) {
+      const long long t0 = (long long)w[0] * 16384, t2 = (long long)w[2] * 15137 + (long long)w[6] * -6270;
+      const long long tmp10 = t0 + t2, tmp12 = t0 - t2;
+      const long long z1 = w[7], z2 = w[5], z3 = w[3], z4 = w[1];
+      const long long o0 = z1 * -1730 + z2 * 11893 + z3 * -17799 + z4 * 8697;
+      const long long o2 = z1 * -4176 + z2 * -4926 + z3 * 7373 + z4 * 20995;
+      const long long rnd = 1LL << 18;
+      const unsigned s0 = idct_range_limit((int)((tmp10 + o2 + rnd) >> 19)), s3 = idct_range_limit((int)((tmp10 - o2 + rnd) >> 19));
+      const unsigned s1 = idct_range_limit((int)((tmp12 + o0 + rnd) >> 19)), s2 = idct_range_limit((int)((tmp12 - o0 + rnd) >> 19));
+      *reinterpret_cast<uint32_t *>(dst) = s0 | s1 << 8 | s2 << 16 | s3 << 24;
+    } else {
+      const long long tmp10 = (long long)w[0] * 32768;
+      const long long o0 = (long long)w[7] * -5906 + (long long)w[5] * 6967 + (long long)w[3] * -10426 + (long long)w[1] * 29692;
+      const long long rnd = 1LL << 19;
+      const unsigned s0 = idct_range_limit((int)((tmp10 + o0 + rnd) >> 20)), s1 = idct_range_limit((int)((tmp10 - o0 + rnd) >> 20));
+      *reinterpret_cast<uint16_t *>(dst) = (uint16_t)(s0 | s1 << 8);
+    }
+  }
+}
+
+// MULTIPLY of jidctfst.c (8-bit: CONST_BITS 8, no rounding): the int times a JLONG constant in 64 bits, shifted, and
+// truncated back to DCTELEM (int)
+__device__ __forceinline__ unsigned ifast_mul(unsigned v, int c)
+{
+  return (unsigned)(int)(((long long)(int)v * c) >> 8);
+}
+
+// one 8-point pass of jpeg_idct_ifast (jidctfst.c:171-368) on DCTELEM = int, modulo 2^32 as the reference's int
+// arithmetic behaves where a 16-bit table makes it overflow; o[k] is output k of the pass
+__device__ __forceinline__ void ifast_1d(const unsigned d[8], unsigned o[8])
+{
+  unsigned tmp10 = d[0] + d[4], tmp11 = d[0] - d[4];
+  unsigned tmp13 = d[2] + d[6], tmp12 = ifast_mul(d[2] - d[6], 362) - tmp13;
+  const unsigned tmp0 = tmp10 + tmp13, tmp3 = tmp10 - tmp13, tmp1 = tmp11 + tmp12, tmp2 = tmp11 - tmp12;
+  const unsigned z13 = d[5] + d[3], z10 = d[5] - d[3], z11 = d[1] + d[7], z12 = d[1] - d[7];
+  const unsigned tmp7 = z11 + z13;
+  tmp11 = ifast_mul(z11 - z13, 362);
+  const unsigned z5 = ifast_mul(z10 + z12, 473);
+  tmp10 = ifast_mul(z12, 277) - z5;
+  tmp12 = ifast_mul(z10, -669) + z5;
+  const unsigned tmp6 = tmp12 - tmp7, tmp5 = tmp11 - tmp6, tmp4 = tmp10 + tmp5;
+  o[0] = tmp0 + tmp7; o[7] = tmp0 - tmp7; o[1] = tmp1 + tmp6; o[6] = tmp1 - tmp6;
+  o[2] = tmp2 + tmp5; o[5] = tmp2 - tmp5; o[4] = tmp3 + tmp4; o[3] = tmp3 - tmp4;
+}
+
+// jpeg_idct_ifast with its multiplier table (jddctmgr.c: quantval * aanscales descaled to IFAST_SCALE_BITS, int),
+// image i's at mtab + i * qstride.  Shape of k_idct_islow.  The all-zero shortcuts give the general path's values.
+__global__ void __launch_bounds__(IDCT_BLOCKS * 8) k_idct_ifast(const int16_t *__restrict__ coef, const int *__restrict__ mtab, int qstride,
+                                                                uint8_t *__restrict__ out, int wib, int hib, long long nblocks)
+{
+  __shared__ int4 s_coef[IDCT_BLOCKS * 8];
+  __shared__ int s_ws[IDCT_BLOCKS * IDCT_WS];
+  const int lb = threadIdx.x >> 3, lane = threadIdx.x & 7;
+  const long long blk = (long long)blockIdx.x * IDCT_BLOCKS + lb;
+  const bool valid = blk < nblocks;
+  const long long per = (long long)wib * hib;
+  const long long img = valid ? blk / per : 0;
+  s_coef[threadIdx.x] = valid ? reinterpret_cast<const int4 *>(coef)[blk * 8 + lane] : make_int4(0, 0, 0, 0);
+  __syncwarp();
+  {
+    const int16_t *c = reinterpret_cast<const int16_t *>(s_coef + lb * 8) + lane;
+    const int *q = mtab + img * qstride + lane;
+    unsigned d[8], o[8];
+#pragma unroll
+    for (int r = 0; r < 8; r++) d[r] = (unsigned)(int)c[r * 8] * (unsigned)__ldg(q + r * 8);
+    ifast_1d(d, o);
+    int *ws = s_ws + lb * IDCT_WS + lane;
+#pragma unroll
+    for (int r = 0; r < 8; r++) ws[r * 9] = (int)o[r];
+  }
+  __syncwarp();
+  {
+    const int *ws = s_ws + lb * IDCT_WS + lane * 9;
+    unsigned d[8], o[8];
+#pragma unroll
+    for (int k = 0; k < 8; k++) d[k] = (unsigned)ws[k];
+    ifast_1d(d, o);
+    unsigned s[8];
+#pragma unroll
+    for (int k = 0; k < 8; k++) s[k] = idct_range_limit((int)o[k] >> 5);        // IDESCALE(x, PASS1_BITS + 3)
+    if (valid) {
+      const long long rem = blk - img * per;
+      const int by = (int)(rem / wib), bx = (int)(rem - (long long)by * wib);
+      uint8_t *dst = out + ((img * hib + by) * 8 + lane) * ((long long)wib * 8) + bx * 8;
+      *reinterpret_cast<uint2 *>(dst) = make_uint2(s[0] | s[1] << 8 | s[2] << 16 | s[3] << 24, s[4] | s[5] << 8 | s[6] << 16 | s[7] << 24);
+    }
+  }
+}
+
+// one 8-point pass of jpeg_idct_float (jidctflt.c:72-237) in the reference's operation order (the file is compiled
+// with -fmad=false, so every product and sum is rounded on its own, as FAST_FLOAT float arithmetic is); z5: the
+// centring term pass 2 adds to the DC input (0 in pass 1)
+__device__ __forceinline__ void float_1d(const float d[8], float z5, float o[8])
+{
+  const float c1414 = (float)1.414213562, c1847 = (float)1.847759065, c1082 = (float)1.082392200, c2613 = (float)2.613125930;
+  const float a = d[0] + z5;
+  float tmp10 = a + d[4], tmp11 = a - d[4];
+  float tmp13 = d[2] + d[6], tmp12 = (d[2] - d[6]) * c1414 - tmp13;
+  const float tmp0 = tmp10 + tmp13, tmp3 = tmp10 - tmp13, tmp1 = tmp11 + tmp12, tmp2 = tmp11 - tmp12;
+  const float z13 = d[5] + d[3], z10 = d[5] - d[3], z11 = d[1] + d[7], z12 = d[1] - d[7];
+  const float tmp7 = z11 + z13;
+  tmp11 = (z11 - z13) * c1414;
+  const float zz = (z10 + z12) * c1847;
+  tmp10 = zz - z12 * c1082;
+  tmp12 = zz - z10 * c2613;
+  const float tmp6 = tmp12 - tmp7, tmp5 = tmp11 - tmp6, tmp4 = tmp10 - tmp5;
+  o[0] = tmp0 + tmp7; o[7] = tmp0 - tmp7; o[1] = tmp1 + tmp6; o[6] = tmp1 - tmp6;
+  o[2] = tmp2 + tmp5; o[5] = tmp2 - tmp5; o[3] = tmp3 + tmp4; o[4] = tmp3 - tmp4;
+}
+
+// sample_range_limit[(int)x & RANGE_MASK] (jdmaster.c prepare_range_limit_table): 0 .. 255 as they are, 256 .. 639 are
+// 255, 640 .. 1023 are 0.  (int) of a float beyond the int range is INT_MIN on x86 and saturates here; both land on 0.
+__device__ __forceinline__ unsigned float_range_limit(float x)
+{
+  const int j = (int)x & 1023;
+  return j < 256 ? j : j < 640 ? 255 : 0;
+}
+
+// jpeg_idct_float with its multiplier table (quantval * aanscalefactor[row] * aanscalefactor[col] in double, stored as
+// float), image i's at mtab + i * qstride.  Shape of k_idct_islow.  The all-zero column shortcut gives the general
+// path's values (x + 0 and x - 0 are x).
+__global__ void __launch_bounds__(IDCT_BLOCKS * 8) k_idct_float(const int16_t *__restrict__ coef, const float *__restrict__ mtab, int qstride,
+                                                                uint8_t *__restrict__ out, int wib, int hib, long long nblocks)
+{
+  __shared__ int4 s_coef[IDCT_BLOCKS * 8];
+  __shared__ float s_ws[IDCT_BLOCKS * IDCT_WS];
+  const int lb = threadIdx.x >> 3, lane = threadIdx.x & 7;
+  const long long blk = (long long)blockIdx.x * IDCT_BLOCKS + lb;
+  const bool valid = blk < nblocks;
+  const long long per = (long long)wib * hib;
+  const long long img = valid ? blk / per : 0;
+  s_coef[threadIdx.x] = valid ? reinterpret_cast<const int4 *>(coef)[blk * 8 + lane] : make_int4(0, 0, 0, 0);
+  __syncwarp();
+  {
+    const int16_t *c = reinterpret_cast<const int16_t *>(s_coef + lb * 8) + lane;
+    const float *q = mtab + img * qstride + lane;
+    float d[8], o[8];
+#pragma unroll
+    for (int r = 0; r < 8; r++) d[r] = (float)c[r * 8] * (__ldg(q + r * 8) * 0.125f);
+    float_1d(d, 0.f, o);
+    float *ws = s_ws + lb * IDCT_WS + lane;
+#pragma unroll
+    for (int r = 0; r < 8; r++) ws[r * 9] = o[r];
+  }
+  __syncwarp();
+  {
+    const float *ws = s_ws + lb * IDCT_WS + lane * 9;
+    float d[8], o[8];
+#pragma unroll
+    for (int k = 0; k < 8; k++) d[k] = ws[k];
+    float_1d(d, 128.5f, o);
+    unsigned s[8];
+#pragma unroll
+    for (int k = 0; k < 8; k++) s[k] = float_range_limit(o[k]);
+    if (valid) {
+      const long long rem = blk - img * per;
+      const int by = (int)(rem / wib), bx = (int)(rem - (long long)by * wib);
+      uint8_t *dst = out + ((img * hib + by) * 8 + lane) * ((long long)wib * 8) + bx * 8;
+      *reinterpret_cast<uint2 *>(dst) = make_uint2(s[0] | s[1] << 8 | s[2] << 16 | s[3] << 24, s[4] | s[5] << 8 | s[6] << 16 | s[7] << 24);
+    }
+  }
+}
+
+void launch_idct_opts(int size, int method, const int16_t *coef, const void *tab, int qstride, uint8_t *out, int wib, int hib, int n, cudaStream_t s)
+{
+  const long long nblocks = (long long)n * wib * hib;
+  const unsigned grid8 = (unsigned)((nblocks + IDCT_BLOCKS - 1) / IDCT_BLOCKS);
+  const uint16_t *q = static_cast<const uint16_t *>(tab);
+  if (size == 1) { k_idct_red<1><<<(unsigned)((nblocks + 255) / 256), 256, 0, s>>>(coef, q, qstride, out, wib, hib, nblocks); LAUNCHED(); }
+  else if (size == 2) { k_idct_red<2><<<grid8, IDCT_BLOCKS * 8, 0, s>>>(coef, q, qstride, out, wib, hib, nblocks); LAUNCHED(); }
+  else if (size == 4) { k_idct_red<4><<<grid8, IDCT_BLOCKS * 8, 0, s>>>(coef, q, qstride, out, wib, hib, nblocks); LAUNCHED(); }
+  else if (method == 1) { k_idct_ifast<<<grid8, IDCT_BLOCKS * 8, 0, s>>>(coef, static_cast<const int *>(tab), qstride, out, wib, hib, nblocks); LAUNCHED(); }
+  else if (method == 2) { k_idct_float<<<grid8, IDCT_BLOCKS * 8, 0, s>>>(coef, static_cast<const float *>(tab), qstride, out, wib, hib, nblocks); LAUNCHED(); }
+  else launch_idct_islow(coef, q, qstride, out, wib, hib, n, s);
+}
+
+// one output sample of a component plane (dw x dh real samples) at pixel (x, y): fullsize, replication by hr x vr
+// (h2v1_upsample, h2v2_upsample, int_upsample and what the merged upsampler does to chroma, jdmerge.c), or the fancy
+// filters of upsample4 evaluated for one pixel
+__device__ __forceinline__ int up_one(const uint8_t *__restrict__ p, int pitch, int dw, int dh, int hr, int vr, bool fancy, int x, int y)
+{
+  if (hr == 1 && vr == 1) return __ldg(p + (long long)y * pitch + x);
+  if (!fancy) return up_at(p, pitch, dw, dh, vr == 2 ? y >> 1 : y, hr == 2 ? x >> 1 : x);
+  if (vr == 1) {                                          // h2v1_fancy_upsample
+    const int c = x >> 1, a = up_at(p, pitch, dw, dh, y, c);
+    return (x & 1) ? (3 * a + up_at(p, pitch, dw, dh, y, c + 1) + 2) >> 2 : (3 * a + up_at(p, pitch, dw, dh, y, c - 1) + 1) >> 2;
+  }
+  const int r = y >> 1, r1 = (y & 1) ? r + 1 : r - 1;
+  if (hr == 1) return (3 * up_at(p, pitch, dw, dh, r, x) + up_at(p, pitch, dw, dh, r1, x) + ((y & 1) ? 2 : 1)) >> 2;   // h1v2_fancy_upsample
+  const int c = x >> 1, cn = (x & 1) ? c + 1 : c - 1;     // h2v2_fancy_upsample
+  const int s0 = 3 * up_at(p, pitch, dw, dh, r, c) + up_at(p, pitch, dw, dh, r1, c), s1 = 3 * up_at(p, pitch, dw, dh, r, cn) + up_at(p, pitch, dw, dh, r1, cn);
+  return (3 * s0 + s1 + ((x & 1) ? 7 : 8)) >> 4;
+}
+
+// Sample planes -> pixels in the requested layout, one thread per pixel: each used component upsampled by up_one, then
+// the deconverter jinit_color_deconverter picks (jdcolor.c:760-930, jdcolext.c): grayscale_convert, ycc_rgb_convert,
+// null_convert / rgb_rgb_convert, gray_rgb_convert or rgb_gray_convert, into o.ps bytes with R, G, B at o.off[0..2]
+// and 0xFF at o.off[3] where the pixel has a fourth byte.
+__global__ void __launch_bounds__(256) k_upsample_opts(UpsOpt o, uint8_t *__restrict__ pix, long long row_pitch, long long image_stride, int W, int H)
+{
+  const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y, img = blockIdx.z;
+  if (x >= W || y >= H) return;
+  int v[3] = {0, 0, 0};
+#pragma unroll
+  for (int c = 0; c < 3; c++)
+    if (c < o.nin) v[c] = up_one(o.plane[c] + img * o.stride[c], o.pitch[c], o.dw[c], o.dh[c], o.hr[c], o.vr[c], o.fancy[c] != 0, x, y);
+  uint8_t *d = pix + img * image_stride + (long long)y * row_pitch + (long long)x * o.ps;
+  int r, g, b;
+  switch (o.conv) {
+  case UPS_GRAY: d[0] = (uint8_t)v[0]; return;
+  case UPS_RGB_GRAY: d[0] = (uint8_t)((19595 * v[0] + 38470 * v[1] + 7471 * v[2] + 32768) >> 16); return;
+  case UPS_YCC_RGB: {
+    const int u = v[1] - 128, w = v[2] - 128;
+    r = min(max(v[0] + ((91881 * w + 32768) >> 16), 0), 255);
+    g = min(max(v[0] + ((-22554 * u + 32768 - 46802 * w) >> 16), 0), 255);
+    b = min(max(v[0] + ((116130 * u + 32768) >> 16), 0), 255);
+    break;
+  }
+  case UPS_GRAY_RGB: r = g = b = v[0]; break;
+  default: r = v[0]; g = v[1]; b = v[2]; break;          // UPS_COPY3
+  }
+  d[o.off[0]] = (uint8_t)r; d[o.off[1]] = (uint8_t)g; d[o.off[2]] = (uint8_t)b;
+  if (o.ps == 4) d[o.off[3]] = 0xFF;
+}
+
+void launch_upsample_opts(const UpsOpt &o, uint8_t *pix, size_t row_pitch, size_t image_stride, int W, int H, int n, cudaStream_t s)
+{
+  const dim3 cta(64, 4), grid((unsigned)((W + 63) / 64), (unsigned)((H + 3) / 4), (unsigned)n);
+  k_upsample_opts<<<grid, cta, 0, s>>>(o, pix, (long long)row_pitch, (long long)image_stride, W, H); LAUNCHED();
+}
+
 }  // namespace b200

@@ -258,6 +258,21 @@ void launch_idct_islow(const int16_t *coef, const uint16_t *quant, int qstride, 
 int launch_upsample_color(int hx, int vx, int nc, const uint8_t *const *planes, const int *pitch, const long long *stride, int dw, int dh, bool ycc,
                           uint8_t *pix, size_t row_pitch, size_t image_stride, int W, int H, int n, cudaStream_t s);
 
+// decompression with options.  IDCT of one component whose DCT_scaled_size is `size`: 1, 2, 4 -> k_idct_red<size>
+// (tab: the uint16 quantization tables), 8 -> by method: 0 islow (tab as for 1 .. 4), 1 k_idct_ifast (tab: int
+// multiplier tables), 2 k_idct_float (tab: float multiplier tables); image i's table at tab + i * qstride entries.
+// out: [n][hib * size][wib * size] samples.
+void launch_idct_opts(int size, int method, const int16_t *coef, const void *tab, int qstride, uint8_t *out, int wib, int hib, int n, cudaStream_t s);
+// k_upsample_opts: per used component (nin of them) image 0's plane, pitch / stride in bytes, dw x dh real samples,
+// the replication factors hr x vr (1 or 2) after IDCT scaling, and fancy (the smoothing filter instead of
+// replication); conv the colour conversion (UPS_* of decode.cuh); ps bytes per pixel with R, G, B (or the one gray byte) at off[0..2] and
+// 0xFF at off[3] when ps is 4.
+struct UpsOpt {
+  const uint8_t *plane[3]; int pitch[3]; long long stride[3]; int dw[3], dh[3], hr[3], vr[3], fancy[3];
+  int nin, conv, ps, off[4];
+};
+void launch_upsample_opts(const UpsOpt &o, uint8_t *pix, size_t row_pitch, size_t image_stride, int W, int H, int n, cudaStream_t s);
+
 extern unsigned long long g_kernel_launches;
 
 }  // namespace b200

@@ -258,6 +258,99 @@ extern "C" int b200jpeg_decompress_output(const b200jpeg_source_info *src, int *
   return B200JPEG_OK;
 }
 
+extern "C" b200jpeg_decompress_options b200jpeg_default_decompress_options(void)
+{
+  b200jpeg_decompress_options o;
+  o.scale_num = 1; o.scale_denom = 1; o.dct_method = B200JPEG_DCT_ISLOW; o.do_fancy_upsampling = 1; o.out_color_space = -1;
+  return o;
+}
+
+namespace b200 {
+
+// jpeg_calc_output_dimensions (jdmaster.c:96-370), the method choice of jddctmgr.c start_pass, jinit_upsampler
+// (jdsample.c:421-530) and jinit_color_deconverter (jdcolor.c:760-930) for one source and one set of options
+int plan_decompress(const b200jpeg_source_info &s, const b200jpeg_decompress_options &o, DecPlan &p)
+{
+  p = DecPlan();
+  const int nc = s.num_components, jcs = s.jpeg_color_space;
+  if (nc < 1 || nc > 4) return bad(B200JPEG_ERR_PARAM, "bad argument");
+  if (o.scale_num < 1 || o.scale_denom < 1) { set_error("scale %d/%d: scale_num and scale_denom must be positive", o.scale_num, o.scale_denom); return B200JPEG_ERR_PARAM; }
+  if (o.dct_method < B200JPEG_DCT_ISLOW || o.dct_method > B200JPEG_DCT_FLOAT) { set_error("dct_method %d is not JDCT_ISLOW, JDCT_IFAST or JDCT_FLOAT", o.dct_method); return B200JPEG_ERR_PARAM; }
+  // the block size jpeg_core_output_dimensions picks: the least k with scale_num * 8 <= scale_denom * k, at most 16
+  int k = 16;
+  for (int t = 1; t < 16; t++) if ((long long)o.scale_num * 8 <= (long long)o.scale_denom * t) { k = t; break; }
+  if (k != 1 && k != 2 && k != 4 && k != 8) {
+    set_error("scale %d/%d gives an IDCT block size of %d: only sizes 1, 2, 4 and 8 (1/8, 1/4, 1/2, 1/1) are decoded on the device", o.scale_num, o.scale_denom, k);
+    return B200JPEG_ERR_UNSUPPORTED;
+  }
+  p.k = k; p.method = o.dct_method;
+  // out_color_space and the deconverter
+  const int def = jcs == B200JPEG_CS_GRAYSCALE ? B200JPEG_CS_GRAYSCALE : jcs == B200JPEG_CS_YCbCr || jcs == B200JPEG_CS_RGB ? B200JPEG_CS_RGB : B200JPEG_CS_CMYK;
+  const int ocs = o.out_color_space == -1 ? def : o.out_color_space;
+  if (ocs < 0 || ocs > B200JPEG_CS_RGB565) { set_error("out_color_space %d is not a J_COLOR_SPACE", o.out_color_space); return B200JPEG_ERR_PARAM; }
+  const bool refuse = ocs == B200JPEG_CS_RGB565 || ((ocs == B200JPEG_CS_CMYK || ocs == B200JPEG_CS_YCCK) && o.out_color_space != -1);
+  if (refuse) { set_error("out_color_space %d (RGB565, CMYK or YCCK output) is not on the device path", ocs); return B200JPEG_ERR_UNSUPPORTED; }
+  p.out_cs = ocs;
+  bool conv_ok = true;
+  if (ocs == B200JPEG_CS_GRAYSCALE) {
+    p.out_nc = 1; p.ps = 1; p.nin = 1;
+    if (jcs == B200JPEG_CS_GRAYSCALE || jcs == B200JPEG_CS_YCbCr) { p.conv = UPS_GRAY; for (int c = 1; c < nc; c++) p.needed[c] = false; }
+    else if (jcs == B200JPEG_CS_RGB) { p.conv = UPS_RGB_GRAY; p.nin = 3; }
+    else conv_ok = false;
+  } else if (B200JPEG_CS_IS_RGB(ocs)) {
+    p.out_nc = p.ps = B200JPEG_CS_PIXELSIZE(ocs);
+    const int f = B200JPEG_CS_FIRST(ocs), bf = B200JPEG_CS_BLUE_FIRST(ocs);
+    p.off[0] = f + (bf ? 2 : 0); p.off[1] = f + 1; p.off[2] = f + (bf ? 0 : 2); p.off[3] = f ? 0 : 3;
+    if (jcs == B200JPEG_CS_YCbCr) { p.conv = UPS_YCC_RGB; p.nin = 3; }
+    else if (jcs == B200JPEG_CS_GRAYSCALE) { p.conv = UPS_GRAY_RGB; p.nin = 1; }
+    else if (jcs == B200JPEG_CS_RGB) { p.conv = UPS_COPY3; p.nin = 3; }
+    else conv_ok = false;
+  } else if (nc == 4 && ocs == B200JPEG_CS_CMYK) {         // the default of a CMYK / YCCK file (the batch refuses those)
+    p.out_nc = p.ps = 4; p.nin = 0;
+  } else if (ocs == jcs) {                                  // null_convert to the file's own space
+    p.out_nc = p.ps = nc; p.nin = nc; p.conv = nc == 1 ? UPS_GRAY : UPS_COPY3;
+    p.off[0] = 0; p.off[1] = 1; p.off[2] = 2;
+  } else conv_ok = false;
+  if (!conv_ok) return bad(B200JPEG_ERR_PARAM, "Unsupported color conversion request");   // JERR_CONVERSION_NOTIMPL
+  // output size, and per component the IDCT size (chroma scaled up through the IDCT while that divides evenly) and
+  // the downsampled size after scaling
+  int mh = 1, mv = 1;
+  for (int c = 0; c < nc; c++) { mh = std::max(mh, s.h_samp_factor[c]); mv = std::max(mv, s.v_samp_factor[c]); }
+  const long long W = s.image_width, H = s.image_height;
+  p.out_w = (int)((W * k + 7) / 8); p.out_h = (int)((H * k + 7) / 8);
+  const bool do_fancy = o.do_fancy_upsampling && k > 1;
+  for (int c = 0; c < nc; c++) {
+    const int h = s.h_samp_factor[c], v = s.v_samp_factor[c];
+    int ss = k;
+    while (ss < 8 && (mh * k) % (h * ss * 2) == 0 && (mv * k) % (v * ss * 2) == 0) ss *= 2;
+    p.ssize[c] = ss;
+    p.dw[c] = (int)((W * h * ss + mh * 8 - 1) / (mh * 8)); p.dh[c] = (int)((H * v * ss + mv * 8 - 1) / (mv * 8));
+    const int hin = h * ss / k, vin = v * ss / k;
+    if (!hin || !vin || mh % hin || mv % vin || mh / hin > 2 || mv / vin > 2) { set_error("component %d: upsampling by %d x %d is not on the device path", c, mh / std::max(hin, 1), mv / std::max(vin, 1)); return B200JPEG_ERR_UNSUPPORTED; }
+    p.hr[c] = mh / hin; p.vr[c] = mv / vin;
+    // fancy: h2v1 / h2v2 need downsampled_width > 2, h1v2 does not; fullsize and int_upsample have no filter
+    p.fancy[c] = do_fancy && (p.hr[c] == 2 ? p.dw[c] > 2 : p.vr[c] == 2);
+  }
+  p.is_default = k == 8 && p.method == B200JPEG_DCT_ISLOW && o.do_fancy_upsampling && ocs == def;
+  return B200JPEG_OK;
+}
+
+}  // namespace b200
+
+extern "C" int b200jpeg_decompress_output_opts(const b200jpeg_source_info *src, const b200jpeg_decompress_options *opts,
+                                               int *width, int *height, int *color_space, int *components)
+{
+  if (!src || !opts || src->num_components < 1) return bad(B200JPEG_ERR_PARAM, "bad argument");
+  DecPlan p;
+  const int rc = plan_decompress(*src, *opts, p);
+  if (rc) return rc;
+  if (width) *width = p.out_w;
+  if (height) *height = p.out_h;
+  if (color_space) *color_space = p.out_cs;
+  if (components) *components = p.out_nc;
+  return B200JPEG_OK;
+}
+
 namespace b200 {
 
 // The descriptors of a batch of sequential files (see decode.cuh).  The unstuffed words go to alloc(bound) first.

@@ -405,7 +405,35 @@ def recompress():
     print("wrote", len(cases), "decompress cases,", len(rec), "recompress cases")
 
 
+def decompress_options():
+    """tests/golden/decompress_options_golden.json: for every (source, options) of tests/decompress_options_cases.py the
+    md5 of the source, the fields jpeg_calc_output_dimensions sets and the md5 of the pixels the reference decodes with
+    those options (build/librefdecopt.so), and the reference's message for each refused colour pair."""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import decompress_options_cases as O
+    if not O.have_reference():
+        sys.exit("build/librefdecopt.so is missing: run __graft_entry__.build() with the reference build under oracle/_ref/")
+    cases = []
+    for cid, sid, scale, dct, fancy, cs in O.cases():
+        src, _ = O.source(sid)
+        px, info, msg = O.ref_decompress(src, O.opts_tuple(scale, dct, fancy, cs))
+        if px is None:
+            sys.exit(f"{cid}: the reference refuses it: {msg}")
+        nc = info[6]
+        cases.append({"id": cid, "src_md5": O.md5(src), "pix_md5": O.md5(px), "shape": list(px.shape), "out_color_space": info[3],
+                      "components": [info[7 + 3 * c:10 + 3 * c] for c in range(nc)], "warnings": info[5]})
+    refused = []
+    for sid, cs in O.REFUSED_PAIRS:
+        _, _, msg = O.ref_decompress(O.source(sid)[0], (1, 1, 0, 1, cs), header_only=True)
+        refused.append({"source": sid, "out_color_space": cs, "message": msg})
+    json.dump({"generator": "tools/make_golden.py --decompress-options", "reference": "mozilla/mozjpeg 5.0.0 (C path, WITH_SIMD=0), oracle/_ref",
+               "cases": cases, "refused_pairs": refused}, open(os.path.join(GOLD, "decompress_options_golden.json"), "w"), indent=0)
+    print("wrote", len(cases), "cases,", len(refused), "refused pairs")
+
+
 def main():
+    if "--decompress-options" in sys.argv:
+        return decompress_options()
     if "--recompress" in sys.argv:
         return recompress()
     if "--transform" in sys.argv:

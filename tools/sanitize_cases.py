@@ -80,5 +80,10 @@ n += len(enc.read_coefficients([srcs[0][:sc.data_offset + sc.data_size] + bytes(
 # recompression (IDCT, upsampling + colour conversion, then the pixel encode): 4:2:0 at a ragged size
 rag = enc.encode_batch(mj.params_from_switches(["-revert", "-quality", "90"], 203, 131), np.stack([synth_image(11, 203, 131), synth_image(12, 203, 131)]))
 n += len(enc.recompress(mj.params_for_jpeg_input(["-baseline", "-quality", "75", "-sample", "2x2"], rag[0]), rag))
+# decompression with options: the reduced IDCTs (1x1, 2x2, 4x4), ifast and float, plain upsampling, EXT_* layouts
+for kw in (dict(scale=(1, 8)), dict(scale=(1, 4), dct="fast", fancy=False), dict(scale=(1, 2), dct="float", colorspace="bgrx"),
+           dict(dct="fast", colorspace="gray"), dict(fancy=False, colorspace="xrgb")):
+    n += len(enc.decompress(rag, **kw))
+    n += len(enc.recompress(mj.params_for_jpeg_input(["-baseline", "-quality", "75"], rag[0], **kw), rag, **kw))
 print("sanitize cases done:", n, "files, kernel launches", enc.kernel_launches())
 enc.close()
