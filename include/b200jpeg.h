@@ -296,6 +296,26 @@ int  b200jpeg_encoder_set_stream(b200jpeg_encoder *enc, void *cuda_stream);
  * intermediate HBM arenas are sized for one chunk.  0 = automatic (about 1.6 M
  * 8x8 blocks per chunk, i.e. 8 images of 3840x2160 4:2:0). */
 int  b200jpeg_encoder_set_chunk_images(b200jpeg_encoder *enc, int images_per_chunk);
+/* Progressive decode (off by default): with on != 0 the decode entry points
+ * (b200jpeg_decode_coefs_batch, b200jpeg_transcode_batch[_transform],
+ * b200jpeg_decompress_batch[_opts], b200jpeg_recompress_batch[_opts]) take
+ * progressive Huffman (SOF2) files at 8 and 12 bits as well, and a batch may mix
+ * them with sequential files of one geometry.  It is opt-in because the
+ * documented contract of those entry points is "SOF2 -> B200JPEG_ERR_UNSUPPORTED,
+ * decode it yourself", and because the AC refinement scans are decoded serially
+ * per restart segment: one warp walks each segment's blocks in order, so without
+ * restart markers the time of a refinement scan grows with the image's block
+ * count: about 1 s (q75) to 3 s (q90) for a 3840x2160 4:2:0 image of mozjpeg's
+ * default profile on an H100 (DESIGN.md section 8), shared by the images decoded
+ * beside it, and a very large image without restarts holds one warp for longer.
+ * With it on, a progressive file is refused with B200JPEG_ERR_BAD_SOURCE for
+ * what the reference stops on (JERR_BAD_PROGRESSION) and also for what it only
+ * warns on: an AC scan before its component's DC scan, an Ah that is not the
+ * coefficient's current point transform, a second first scan of a coefficient,
+ * a refinement symbol of size other than 1 and a coefficient past its scan's
+ * band.  The pixel routes refuse, with B200JPEG_ERR_UNSUPPORTED, an incomplete
+ * progression that the reference decompressor would block-smooth. */
+int  b200jpeg_encoder_set_progressive_decode(b200jpeg_encoder *enc, int on);
 /* Images per chunk the last batch was processed with (= images per kernel launch). */
 int  b200jpeg_last_chunk_images(const b200jpeg_encoder *enc);
 /* Consecutive chunks rotate over `n_streams` (1 to 4, default 2; B200JPEG_STREAMS in the environment) compute
@@ -402,7 +422,8 @@ int  b200jpeg_encode_yuv_batch(b200jpeg_encoder *enc, const b200jpeg_params *p,
  * non-interleaved ones; restart intervals): replaces jpeg_read_coefficients (jdtrans.c:47-124) for a batch of files of
  * one geometry (size, precision, components and sampling); Huffman tables, quantization tables, restart interval and
  * scan layout may differ per file.  Progressive (SOF2) files are B200JPEG_ERR_UNSUPPORTED: pass their coefficients
- * to b200jpeg_encode_batch_coefs instead.  Corrupt entropy-coded data (an invalid code, too few bits for a segment's
+ * to b200jpeg_encode_batch_coefs instead, or turn b200jpeg_encoder_set_progressive_decode on, which decodes them
+ * here too (first scans in the speculative decode, then DC refinements, then AC refinements serially per segment).  Corrupt entropy-coded data (an invalid code, too few bits for a segment's
  * MCUs, a wrong RSTn, an unexpected marker) is B200JPEG_ERR_BAD_SOURCE naming the first such image; the reference only
  * warns there and fills the gap.  Bytes after a segment's last MCU are ignored, like the reference does.
  *
@@ -444,7 +465,9 @@ int  b200jpeg_last_decode_sync(const b200jpeg_encoder *enc, int *max_cta_rounds,
  *
  * Accepted: SOF0 / SOF1, 8 bits, one component, or three with component 0 at the largest sampling factors (1 or 2 each
  * way) over 1x1 chroma (4:4:4, 4:2:2, 4:4:0, 4:2:0).  12-bit, 4-component, progressive files and every other sampling
- * layout are B200JPEG_ERR_UNSUPPORTED naming the first such image, before any device work.
+ * layout are B200JPEG_ERR_UNSUPPORTED naming the first such image, before any device work.  With
+ * b200jpeg_encoder_set_progressive_decode on, SOF2 files of that kind are accepted unless the reference would
+ * block-smooth them (smoothing_ok, jdcoefct.c: an incomplete progression), which is B200JPEG_ERR_UNSUPPORTED.
  *
  * b200jpeg_decompress_batch writes image i's rows (image_width * components bytes, see b200jpeg_decompress_output) to
  * pixels + i * image_stride, row_pitch bytes apart, in host or device memory (pixels_on_device).  The batch is

@@ -47,6 +47,11 @@ class Encoder:
         """Images per pipeline chunk (0 = automatic)."""
         A.check(_lib.b200jpeg_encoder_set_chunk_images(self._h, n), "set_chunk_images")
 
+    def set_progressive_decode(self, on: bool) -> None:
+        """Decode progressive (SOF2) files too in read_coefficients, transcode_files(_transform), decompress(_ptr) and
+        recompress (off by default: those refuse SOF2 files, see b200jpeg_encoder_set_progressive_decode)."""
+        A.check(_lib.b200jpeg_encoder_set_progressive_decode(self._h, 1 if on else 0), "set_progressive_decode")
+
     def chunk_images(self) -> int:
         """Images per chunk (= per kernel launch) of the last batch."""
         return int(_lib.b200jpeg_last_chunk_images(self._h))

@@ -144,7 +144,7 @@ EXPORTS = [
     "b200jpeg_set_linear_quality", "b200jpeg_set_quality", "b200jpeg_default_qtables",
     "b200jpeg_simple_progression", "b200jpeg_enable_lossless", "b200jpeg_std_huff_tables", "b200jpeg_std_quant_tbl",
     "b200jpeg_validate", "b200jpeg_total_passes", "b200jpeg_yuv_plane_dims",
-    "b200jpeg_encoder_create", "b200jpeg_encoder_destroy", "b200jpeg_encoder_set_stream", "b200jpeg_encoder_set_chunk_images", "b200jpeg_last_chunk_images", "b200jpeg_encoder_set_streams", "b200jpeg_encode_batch",
+    "b200jpeg_encoder_create", "b200jpeg_encoder_destroy", "b200jpeg_encoder_set_stream", "b200jpeg_encoder_set_chunk_images", "b200jpeg_encoder_set_progressive_decode", "b200jpeg_last_chunk_images", "b200jpeg_encoder_set_streams", "b200jpeg_encode_batch",
     "b200jpeg_encode_batch_device_only", "b200jpeg_encode_batch_raw", "b200jpeg_encode_batch_coefs", "b200jpeg_encode_yuv_batch",
     "b200jpeg_encode_batch_qtables", "b200jpeg_encode_batch_raw_qtables", "b200jpeg_encode_batch_coefs_qtables", "b200jpeg_get_output", "b200jpeg_last_scan_bytes",
     "b200jpeg_kernel_launches", "b200jpeg_last_stage_times", "b200jpeg_debug_get_coefs",
@@ -192,6 +192,7 @@ def load() -> C.CDLL:
     lib.b200jpeg_encoder_destroy.argtypes = [C.c_void_p]; lib.b200jpeg_encoder_destroy.restype = None
     lib.b200jpeg_encoder_set_stream.argtypes = [C.c_void_p, C.c_void_p]; lib.b200jpeg_encoder_set_stream.restype = C.c_int
     lib.b200jpeg_encoder_set_chunk_images.argtypes = [C.c_void_p, C.c_int]; lib.b200jpeg_encoder_set_chunk_images.restype = C.c_int
+    lib.b200jpeg_encoder_set_progressive_decode.argtypes = [C.c_void_p, C.c_int]; lib.b200jpeg_encoder_set_progressive_decode.restype = C.c_int
     lib.b200jpeg_last_chunk_images.argtypes = [C.c_void_p]; lib.b200jpeg_last_chunk_images.restype = C.c_int
     lib.b200jpeg_encoder_set_streams.argtypes = [C.c_void_p, C.c_int]; lib.b200jpeg_encoder_set_streams.restype = C.c_int
     lib.b200jpeg_encode_batch.argtypes = [C.c_void_p, P, C.c_void_p, C.c_int, C.c_size_t, C.c_size_t, C.c_int]; lib.b200jpeg_encode_batch.restype = C.c_int

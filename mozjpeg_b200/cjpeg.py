@@ -460,7 +460,12 @@ def main(argv: Sequence[str] = None) -> int:
         if not all(d[:1] == b"\xff" for d in data):
             print("all input files of one call must have the same format", file=sys.stderr)
             return 2
-        out = Encoder(0).recompress(params_for_jpeg_input(switches, data[0]), data)
+        enc = Encoder(0)
+        enc.set_progressive_decode(True)      # the reference's cjpeg reads progressive JPEG input too
+        try:
+            out = enc.recompress(params_for_jpeg_input(switches, data[0]), data)
+        finally:
+            enc.close()
         for f, jpg in zip(files, out):
             # a JPEG input named x.jpg must not be overwritten by its own output
             name = outfile if (outfile and len(files) == 1) else f.rsplit(".", 1)[0] + ".out.jpg"

@@ -103,6 +103,7 @@ struct b200jpeg_encoder {
   int chunk = 0;                    // images per chunk of the last batch
   int last_chunk_i0 = 0, last_chunk_n = 0, last_chunk_slot = 0;   // the chunk whose intermediates are still in the arenas
   int chunk_images_override = 0;    // 0 = automatic
+  bool progressive_decode = false;  // decode SOF2 files too (b200jpeg_encoder_set_progressive_decode)
   bool keep_plain = false;
   // device arenas sized for ONE chunk; two of them so that consecutive chunks can run on two
   // streams and fill each other's latency-bound phases (serial table construction, trellis chains)
@@ -142,14 +143,16 @@ struct b200jpeg_encoder {
   PinBuf h_dec_words, h_dec_stat;
   DevBuf d_dec_words, d_dec_segs, d_dec_scans, d_dec_tabs, d_dec_out, d_dec_rec, d_dec_pre, d_dec_tsum, d_dec_dcd, d_dec_planes, d_dec_stat;
   size_t dec_plane_off[4] = {0, 0, 0, 0};
-  cudaEvent_t dec_ev[7] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+  cudaEvent_t dec_ev[9] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};   // [7], [8]: refinements
   int dec_rounds = 0; long long dec_redone = 0;
+  bool dec_prog = false;            // the last decode had a progressive file: its stage times include the refinements
+  bool dec_ms_prog = false;         // some chunk of the last decompress had one: dec_ms holds refinement times
   // decompression to pixels (b200jpeg_decompress_batch / b200jpeg_recompress_batch): one chunk's sample planes and
   // quantization tables, the whole batch's pixels where the caller gave no device buffer, the stage times summed over
   // the chunks, and per image the source's COM / APPn segments a recompress copies into its file
   DevBuf d_dec_samples, d_dec_quant, d_dec_pixels, d_dec_mtab;   // d_dec_mtab: ifast / float multiplier tables
   cudaEvent_t pix_ev[3] = {nullptr, nullptr, nullptr};
-  float dec_ms[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  float dec_ms[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};   // the six decode stages, idct, upsample_color, the two refinements
   std::vector<std::vector<uint8_t>> dec_markers;
   const std::vector<std::vector<uint8_t>> *copy_markers = nullptr;   // of the batch being encoded, or nullptr
   CoefXform xform{};                            // the coefficient import's block mapping in the current batch (all zero: a copy)
@@ -1626,30 +1629,41 @@ static uint32_t *dec_words_alloc(void *ctx, size_t words)
   return e->h_dec_words.reserve(words * 4) ? nullptr : e->h_dec_words.as<uint32_t>();
 }
 
-static const char *const kDecStages[6] = {"dec_h2d", "dec_sync", "dec_fix", "dec_scan", "dec_write", "dec_dc"};
+static const char *const kDecStages[8] = {"dec_h2d", "dec_sync", "dec_fix", "dec_scan", "dec_write", "dec_dc", "dec_dc_refine", "dec_ac_refine"};
 
-// the decode stages of the last decode, appended to the stage times
+// the decode stages of the last decode, appended to the stage times (the refinements after a progressive decode)
 static void add_decode_stage_times(b200jpeg_encoder *e)
 {
-  for (int k = 0; k < 6; k++) {
+  for (int k = 0; k < (e->dec_prog ? 8 : 6); k++) {
     float ms = 0.f; cudaEventElapsedTime(&ms, e->dec_ev[k], e->dec_ev[k + 1]);
     e->stage_names.push_back(kDecStages[k]); e->stage_ms.push_back(ms); e->stage_calls.push_back(1);
   }
 }
 
-// Entropy decode of n sequential files into e->d_dec_planes (jpeg_read_coefficients for the batch).
+// the decode stage times of the last decode, added to e->dec_ms
+static void sum_decode_stage_times(b200jpeg_encoder *e)
+{
+  for (int k = 0; k < (e->dec_prog ? 8 : 6); k++) { float ms = 0.f; cudaEventElapsedTime(&ms, e->dec_ev[k], e->dec_ev[k + 1]); e->dec_ms[k < 6 ? k : k + 2] += ms; }
+}
+
+// Entropy decode of n files into e->d_dec_planes (jpeg_read_coefficients for the batch): the first scans through the
+// speculative decode, then every DC refinement, then the AC refinement levels in order.
 // first: the batch index of files[0], for the messages.
 static int decode_files(b200jpeg_encoder *e, const uint8_t *const *files, const size_t *sizes, int n, int first = 0)
 {
   if (!e || !files || !sizes || n <= 0) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
   CU(cudaSetDevice(e->device));
   DecBatch &b = e->dec;
+  b.progressive = e->progressive_decode;
   int rc = build_decode_batch(files, sizes, n, b, dec_words_alloc, e, first);
   if (rc) return rc;
+  e->dec_prog = false;
+  for (int i = 0; i < n; i++) e->dec_prog |= b.info[i].sof == 0xC2;
+  const size_t nseg_all = b.segs.size() + b.dcr_segs.size() + b.acr_segs.size();
   size_t total = 0;
   for (int c = 0; c < b.nc; c++) { e->dec_plane_off[c] = total; total += ((size_t)n * b.wib[c] * b.hib[c] * 128 + 255) & ~(size_t)255; }
   const long long ntiles = (b.nsub + 1023) / 1024;
-  if ((rc = e->d_dec_words.reserve(b.nwords * 4 + 16)) || (rc = e->d_dec_segs.reserve(b.segs.size() * sizeof(DecSeg))) ||
+  if ((rc = e->d_dec_words.reserve(b.nwords * 4 + 16)) || (rc = e->d_dec_segs.reserve(nseg_all * sizeof(DecSeg))) ||
       (rc = e->d_dec_scans.reserve(b.scans.size() * sizeof(DecScan))) || (rc = e->d_dec_tabs.reserve(b.tabs.size() * sizeof(DecTable))) ||
       (rc = e->d_dec_out.reserve(sizeof(DecOut))) || (rc = e->d_dec_rec.reserve((size_t)b.nsub * sizeof(DecRec))) ||
       (rc = e->d_dec_pre.reserve((size_t)b.nsub * 4)) || (rc = e->d_dec_tsum.reserve((size_t)ntiles * 8)) ||
@@ -1665,6 +1679,9 @@ static int decode_files(b200jpeg_encoder *e, const uint8_t *const *files, const 
   CU(cudaEventRecord(e->dec_ev[0], s));
   CU(cudaMemcpyAsync(e->d_dec_words.p, e->h_dec_words.p, b.nwords * 4, cudaMemcpyHostToDevice, s));
   CU(cudaMemcpyAsync(e->d_dec_segs.p, b.segs.data(), b.segs.size() * sizeof(DecSeg), cudaMemcpyHostToDevice, s));
+  DecSeg *d_dcr = e->d_dec_segs.as<DecSeg>() + b.segs.size(), *d_acr = d_dcr + b.dcr_segs.size();
+  if (!b.dcr_segs.empty()) CU(cudaMemcpyAsync(d_dcr, b.dcr_segs.data(), b.dcr_segs.size() * sizeof(DecSeg), cudaMemcpyHostToDevice, s));
+  if (!b.acr_segs.empty()) CU(cudaMemcpyAsync(d_acr, b.acr_segs.data(), b.acr_segs.size() * sizeof(DecSeg), cudaMemcpyHostToDevice, s));
   CU(cudaMemcpyAsync(e->d_dec_scans.p, b.scans.data(), b.scans.size() * sizeof(DecScan), cudaMemcpyHostToDevice, s));
   CU(cudaMemcpyAsync(e->d_dec_tabs.p, b.tabs.data(), b.tabs.size() * sizeof(DecTable), cudaMemcpyHostToDevice, s));
   CU(cudaMemcpyAsync(e->d_dec_out.p, &o, sizeof o, cudaMemcpyHostToDevice, s));
@@ -1674,14 +1691,21 @@ static int decode_files(b200jpeg_encoder *e, const uint8_t *const *files, const 
                 e->d_dec_rec.as<DecRec>(), e->d_dec_pre.as<uint32_t>(), e->d_dec_tsum.as<unsigned long long>(), e->d_dec_dcd.as<int>(), e->d_dec_out.as<DecOut>(),
                 reinterpret_cast<uint32_t *>(stat), reinterpret_cast<int *>(stat + rounds_off), reinterpret_cast<unsigned long long *>(stat + rounds_off + 8),
                 e->dec_ev + 1, s);
+  if (e->dec_prog)
+    launch_decode_refine(e->d_dec_words.as<uint32_t>(), d_dcr, (int)b.dcr_segs.size(), b.dcr_blocks, d_acr, b.acr_level.data(), (int)b.acr_level.size() - 1,
+                         e->d_dec_scans.as<DecScan>(), e->d_dec_tabs.as<DecTable>(), e->d_dec_out.as<DecOut>(), reinterpret_cast<uint32_t *>(stat), e->dec_ev + 7, s);
   CU(cudaGetLastError());
   CU(cudaMemcpyAsync(e->h_dec_stat.p, stat, stat_bytes, cudaMemcpyDeviceToHost, s));
   CU(cudaStreamSynchronize(s));
   const uint8_t *hs = e->h_dec_stat.as<uint8_t>();
   e->dec_rounds = *reinterpret_cast<const int *>(hs + rounds_off);
   e->dec_redone = (long long)*reinterpret_cast<const unsigned long long *>(hs + rounds_off + 8);
-  for (int i = 0; i < n; i++)
-    if (reinterpret_cast<const uint32_t *>(hs)[i]) { set_error("image %d: corrupt entropy-coded data (an invalid Huffman code, or too few bits for a segment's MCUs)", first + i); return B200JPEG_ERR_BAD_SOURCE; }
+  for (int i = 0; i < n; i++) {
+    const uint32_t st = reinterpret_cast<const uint32_t *>(hs)[i];
+    if (st & 1) { set_error("image %d: corrupt entropy-coded data (an invalid Huffman code, or too few bits for a segment's MCUs)", first + i); return B200JPEG_ERR_BAD_SOURCE; }
+    if (st & 2) { set_error("image %d: corrupt entropy-coded data (a coefficient past the end of its scan's spectral band)", first + i); return B200JPEG_ERR_BAD_SOURCE; }
+    if (st & 4) { set_error("image %d: corrupt entropy-coded data (an AC refinement symbol whose size is not 1)", first + i); return B200JPEG_ERR_BAD_SOURCE; }
+  }
   return B200JPEG_OK;
 }
 
@@ -1764,12 +1788,13 @@ static int transcode_files(b200jpeg_encoder *e, const b200jpeg_params *p, const 
   return B200JPEG_OK;
 }
 
-// A source b200jpeg_decompress_batch takes: sequential, 8-bit, gray or three components with component 0 at the
+// A source b200jpeg_decompress_batch takes: sequential (or, with progressive decode on, progressive without the block
+// smoothing a default decompress object would apply), 8-bit, gray or three components with component 0 at the
 // largest factors (1 or 2 each way) over 1x1 chroma; everything else is refused, never approximated.
-static int check_decompress_source(const b200jpeg_source_info &s, int i)
+static int check_decompress_source(const b200jpeg_source_info &s, int i, bool progressive)
 {
   const char *why = nullptr;
-  if (s.sof == 0xC2) why = "progressive (SOF2) source: only sequential files are decoded to pixels";
+  if (s.sof == 0xC2 && !progressive) why = "progressive (SOF2) source: only sequential files are decoded to pixels";
   else if (s.data_precision != 8) why = "12-bit source: only 8-bit files are decoded to pixels";
   else if (s.num_components != 1 && s.num_components != 3) why = "4-component (CMYK / YCCK) source: only gray and 3-component files are decoded to pixels";
   else if (s.num_components == 3 && (s.h_samp_factor[0] > 2 || s.v_samp_factor[0] > 2 || s.h_samp_factor[1] != 1 || s.v_samp_factor[1] != 1 ||
@@ -1778,6 +1803,14 @@ static int check_decompress_source(const b200jpeg_source_info &s, int i)
   if (why) { set_error("image %d: %s", i, why); return B200JPEG_ERR_UNSUPPORTED; }
   for (int c = 0; c < s.num_components; c++)
     if (!s.comp_quant_present[c]) { set_error("image %d: Quantization table 0x%02x was not defined", i, s.quant_tbl_no[c]); return B200JPEG_ERR_BAD_SOURCE; }
+  if (s.sof == 0xC2) {
+    int cb[4][64];
+    if (int rc = check_progression(s, cb)) { std::string m = b200jpeg_last_error(); set_error("image %d: %s", i, m.c_str()); return rc; }
+    if (smoothing_applies(s, cb)) {
+      set_error("image %d: incomplete progression: the reference decompressor applies block smoothing to it (do_block_smoothing), which is not on the device path", i);
+      return B200JPEG_ERR_UNSUPPORTED;
+    }
+  }
   return B200JPEG_OK;
 }
 
@@ -1851,7 +1884,7 @@ static int idct_upsample_opts(b200jpeg_encoder *e, const DecPlan &plan, int nk, 
   CU(cudaEventRecord(e->pix_ev[2], s));
   CU(cudaGetLastError());
   CU(cudaStreamSynchronize(s));
-  for (int k = 0; k < 6; k++) { float ms = 0.f; cudaEventElapsedTime(&ms, e->dec_ev[k], e->dec_ev[k + 1]); e->dec_ms[k] += ms; }
+  sum_decode_stage_times(e);
   for (int k = 0; k < 2; k++) { float ms = 0.f; cudaEventElapsedTime(&ms, e->pix_ev[k], e->pix_ev[k + 1]); e->dec_ms[6 + k] += ms; }
   return B200JPEG_OK;
 }
@@ -1871,7 +1904,7 @@ static int decompress_files(b200jpeg_encoder *e, const uint8_t *const *files, co
       if (!files[i]) { set_error("image %d: no file", i); return B200JPEG_ERR_PARAM; }
       int rc = b200jpeg_parse_source(files[i], sizes[i], &s);
       if (rc) { std::string m = b200jpeg_last_error(); set_error("image %d: %s", i, m.c_str()); return rc; }
-      if ((rc = check_decompress_source(s, i))) return rc;
+      if ((rc = check_decompress_source(s, i, e->progressive_decode))) return rc;
       if (i == 0) s0 = s;
       bool same = s.image_width == s0.image_width && s.image_height == s0.image_height && s.num_components == s0.num_components;
       for (int c = 0; same && c < s.num_components; c++) same = s.h_samp_factor[c] == s0.h_samp_factor[c] && s.v_samp_factor[c] == s0.v_samp_factor[c];
@@ -1889,6 +1922,7 @@ static int decompress_files(b200jpeg_encoder *e, const uint8_t *const *files, co
   CU(cudaSetDevice(e->device));
   for (cudaEvent_t &ev : e->pix_ev) if (!ev) CU(cudaEventCreate(&ev));
   for (float &m : e->dec_ms) m = 0.f;
+  e->dec_ms_prog = false;
   e->dec.want_markers = want_markers;
   if (want_markers) e->dec_markers.assign(n, std::vector<uint8_t>());
   // chunks of about 1.6 M blocks (8 images of 3840x2160 4:2:0, 300 MB of coefficient and sample planes)
@@ -1902,6 +1936,7 @@ static int decompress_files(b200jpeg_encoder *e, const uint8_t *const *files, co
     const int nk = std::min(C, n - i0);
     int rc = decode_files(e, files + i0, sizes + i0, nk, i0);
     if (rc) return rc;
+    e->dec_ms_prog |= e->dec_prog;
     const DecBatch &b = e->dec;
     if (want_markers) for (int i = 0; i < nk; i++) e->dec_markers[i0 + i].swap(e->dec.markers[i]);
     if (!def) { if ((rc = idct_upsample_opts(e, plan, nk, pix + (size_t)i0 * image_stride, row_pitch, image_stride, qt, mt))) return rc; continue; }
@@ -1927,7 +1962,7 @@ static int decompress_files(b200jpeg_encoder *e, const uint8_t *const *files, co
     CU(cudaEventRecord(e->pix_ev[2], s));
     CU(cudaGetLastError());
     CU(cudaStreamSynchronize(s));
-    for (int k = 0; k < 6; k++) { float ms = 0.f; cudaEventElapsedTime(&ms, e->dec_ev[k], e->dec_ev[k + 1]); e->dec_ms[k] += ms; }
+    sum_decode_stage_times(e);
     for (int k = 0; k < 2; k++) { float ms = 0.f; cudaEventElapsedTime(&ms, e->pix_ev[k], e->pix_ev[k + 1]); e->dec_ms[6 + k] += ms; }
   }
   return B200JPEG_OK;
@@ -1937,7 +1972,8 @@ static int decompress_files(b200jpeg_encoder *e, const uint8_t *const *files, co
 static void add_decompress_stage_times(b200jpeg_encoder *e)
 {
   static const char *const extra[2] = {"idct", "upsample_color"};
-  for (int k = 0; k < 8; k++) { e->stage_names.push_back(k < 6 ? kDecStages[k] : extra[k - 6]); e->stage_ms.push_back(e->dec_ms[k]); e->stage_calls.push_back(1); }
+  for (int k = 0; k < (e->dec_ms_prog ? 8 : 6); k++) { e->stage_names.push_back(kDecStages[k]); e->stage_ms.push_back(e->dec_ms[k < 6 ? k : k + 2]); e->stage_calls.push_back(1); }
+  for (int k = 0; k < 2; k++) { e->stage_names.push_back(extra[k]); e->stage_ms.push_back(e->dec_ms[6 + k]); e->stage_calls.push_back(1); }
 }
 
 // b200jpeg_decompress_batch (opts nullptr) and b200jpeg_decompress_batch_opts
@@ -2155,6 +2191,13 @@ int b200jpeg_encoder_set_chunk_images(b200jpeg_encoder *e, int images_per_chunk)
 {
   if (!e || images_per_chunk < 0) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
   e->chunk_images_override = images_per_chunk;
+  return B200JPEG_OK;
+}
+
+int b200jpeg_encoder_set_progressive_decode(b200jpeg_encoder *e, int on)
+{
+  if (!e) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
+  e->progressive_decode = on != 0;
   return B200JPEG_OK;
 }
 

@@ -14,12 +14,24 @@ void lossless_start(const b200jpeg_params *in, b200jpeg_params *out);
 
 // jpeg_make_d_derived_tbl with its validation (source.cpp); -1 for a table the reference refuses
 int derive_dec_table(const b200jpeg_huff_tbl &h, bool is_dc, DecTable *out);
-// the host half of the device decode of a batch of sequential files (source.cpp): parsed headers, one geometry,
-// scan / segment descriptors, derived tables; the unstuffed segments go to the nwords words alloc(ctx, bound) returned
+// start_pass_phuff_decoder's checks over every scan of a progressive file (jdphuff.c:91-144), with its warnings
+// (JWRN_BOGUS_PROGRESSION) and a repeated first scan of a coefficient refused as well; coef_bits: [component][k], the
+// point transform of the last scan that coded k (-1: none).  Messages name the scan, not the image.
+int check_progression(const b200jpeg_source_info &s, int coef_bits[4][64]);
+// smoothing_ok (jdcoefct.c:359-421) once the whole file is read: a decompress object at its defaults smooths the blocks
+bool smoothing_applies(const b200jpeg_source_info &s, const int coef_bits[4][64]);
+// the host half of the device decode of a batch of files (source.cpp): parsed headers, one geometry, scan / segment
+// descriptors, derived tables; the unstuffed segments go to the nwords words alloc(ctx, bound) returned.  segs: the
+// segments of first scans (the speculative decode); dcr_segs: DC refinement segments (dcr_blocks blocks in all);
+// acr_segs: AC refinement segments, level L (the L-th AC refinement scan of each image component) at
+// [acr_level[L], acr_level[L + 1])
 struct DecBatch {
   std::vector<b200jpeg_source_info> info;
-  std::vector<DecScan> scans; std::vector<DecSeg> segs; std::vector<DecTable> tabs;
-  long long nsub = 0, nblocks = 0; unsigned long long nwords = 0;
+  std::vector<DecScan> scans; std::vector<DecSeg> segs, dcr_segs, acr_segs; std::vector<DecTable> tabs;
+  std::vector<int> acr_level;
+  long long nsub = 0, nblocks = 0, dcr_blocks = 0; unsigned long long nwords = 0;
+  // progressive: take SOF2 files (else they are refused as before)
+  bool progressive = false;
   int W = 0, H = 0, nc = 0, precision = 8;
   int wib[4] = {0, 0, 0, 0}, hib[4] = {0, 0, 0, 0}, h[4] = {0, 0, 0, 0}, v[4] = {0, 0, 0, 0};
   // want_markers: also collect each file's COM / APPn segments as cjpeg copies them from a JPEG input (raw segments,

@@ -4004,8 +4004,9 @@ void launch_stuff(const uint32_t *bitbuf, size_t bitbuf_stride_words, const unsi
 
 namespace b200 {
 
-// ================================================================ sequential Huffman decode (jpeg_read_coefficients)
-// Speculative decode with self-synchronisation over DEC_SUB_BITS-bit subsequences of every restart segment (decode.cuh).
+// ================================================================ Huffman decode (jpeg_read_coefficients)
+// Speculative decode with self-synchronisation over DEC_SUB_BITS-bit subsequences of every restart segment of every
+// first scan (sequential, DC first, AC first; decode.cuh).
 // A subsequence's record holds the (position, state) its last decode started from and where it stopped.  Every
 // segment's first subsequence starts exact; any other is right once its start equals its predecessor's stop.
 
@@ -4150,9 +4151,34 @@ __device__ __forceinline__ int16_t *dec_block(const DecOut &o, const DecScan &sc
   return o.plane[c] + (((long long)sc.img * o.hib[c] + row) * o.wib[c] + col) * 64;
 }
 
+// the blocks subsequence j writes (k_dec_write), from (pos, st) to the first block start at or past bit b
+template <bool PROG>
+__device__ __forceinline__ void dec_write_blocks(const uint32_t *w, const DecSeg &g, const DecScan &sc, const DecTable *tabs, uint32_t pos, uint32_t st,
+                                                 uint32_t b, long long blk, long long need, const DecOut &o, int *dcd, uint32_t *status)
+{
+  bool skip = (st & 127) != 0 && st != DEC_DEAD;         // the block in progress belongs to the predecessor
+  int16_t *dst = nullptr;
+  while (st != DEC_DEAD && blk < need) {
+    if ((st & 127) == 0) {                                // a block starts here
+      if (pos >= b) break;
+      dst = dec_block(o, sc, g.mcu0 + blk / sc.nb, (int)(st >> 7));
+    }
+    int zz, val, done;
+    st = dec_step<PROG>(w, g.nbits, pos, st, sc, tabs, zz, val, done);
+    if (st == DEC_DEAD) break;
+    if (!skip) {
+      if (zz == 0) dcd[g.blk0 + blk] = val;
+      else if (PROG && zz > sc.Se) atomicOr(&status[sc.img], 2u);
+      else if (zz > 0 && dst) dst[c_zz[zz]] = PROG ? (int16_t)((unsigned)val << sc.Al) : (int16_t)val;
+    }
+    if (done) { blk += done; skip = false; }
+  }
+}
+
 // one thread per subsequence: decode again from the synchronised start and write the AC coefficients of every block
 // that starts inside the subsequence (finishing the last one past its end) into the planes (zeroed before), the DC
-// differences into dcd; the segment's last subsequence checks that the segment holds all its MCUs
+// differences into dcd; the segment's last subsequence checks that the segment holds all its MCUs.  AC first values
+// are stored shifted by Al; one past a band that ends before 63 (it would land in another scan's band) sets status 2.
 __global__ void __launch_bounds__(128) k_dec_write(const uint32_t *__restrict__ words, const DecSeg *__restrict__ segs, int nsegs,
                                                    const DecScan *__restrict__ scans, const DecTable *__restrict__ tabs,
                                                    const DecRec *__restrict__ rec, long long nsub, const uint32_t *__restrict__ pre,
@@ -4167,30 +4193,16 @@ __global__ void __launch_bounds__(128) k_dec_write(const uint32_t *__restrict__ 
   const DecRec r = rec[j];
   const long long need = (long long)g.nmcu * sc.nb;
   const unsigned long long seg_base = dec_prefix(pre, tsum, g.sub0);
-  long long blk = (long long)(dec_prefix(pre, tsum, j) - seg_base);
+  const long long blk = (long long)(dec_prefix(pre, tsum, j) - seg_base);
   if (j == g.sub0 + g.nsub - 1 && blk + (long long)r.count < need) atomicOr(&status[sc.img], 1u);
   const uint32_t b = min((uint32_t)(j - g.sub0 + 1) * DEC_SUB_BITS, g.nbits);
-  uint32_t pos = r.in_pos, st = r.in_st;
-  bool skip = (st & 127) != 0 && st != DEC_DEAD;         // the block in progress belongs to the predecessor
-  int16_t *dst = nullptr;
-  while (st != DEC_DEAD && blk < need) {
-    if ((st & 127) == 0) {                                // a block starts here
-      if (pos >= b) break;
-      dst = dec_block(*o, sc, g.mcu0 + blk / sc.nb, (int)(st >> 7));
-    }
-    int zz, val; bool done;
-    st = dec_step(w, g.nbits, pos, st, sc, tabs, zz, val, done);
-    if (st == DEC_DEAD) break;
-    if (!skip) {
-      if (zz == 0) dcd[g.blk0 + blk] = val;
-      else if (zz > 0 && dst) dst[c_zz[zz]] = (int16_t)val;
-    }
-    if (done) { blk++; skip = false; }
-  }
+  if (sc.kind == DEC_SEQ) dec_write_blocks<false>(w, g, sc, tabs, r.in_pos, r.in_st, b, blk, need, *o, dcd, status);
+  else dec_write_blocks<true>(w, g, sc, tabs, r.in_pos, r.in_st, b, blk, need, *o, dcd, status);
 }
 
 // one warp per (segment, scan component): DC values = running sum of the differences over the component's blocks in
-// scan order, dummy blocks included, reset at the segment start (decode_mcu: int accumulation, JCOEF store)
+// scan order, dummy blocks included, reset at the segment start (decode_mcu: int accumulation, JCOEF store of the
+// sum shifted by Al)
 __global__ void __launch_bounds__(128) k_dec_dc(const DecSeg *__restrict__ segs, int nsegs, const DecScan *__restrict__ scans,
                                                 const int *__restrict__ dcd, const DecOut *__restrict__ o)
 {
@@ -4200,7 +4212,7 @@ __global__ void __launch_bounds__(128) k_dec_dc(const DecSeg *__restrict__ segs,
   const DecSeg g = segs[gw >> 2];
   const int k = (int)(gw & 3);
   const DecScan &sc = scans[g.scan];
-  if (k >= sc.ncomp) return;
+  if (k >= sc.ncomp || sc.kind == DEC_AC_FIRST) return;
   const int cnt = sc.cnt[k], first = sc.first[k];
   const long long total = (long long)g.nmcu * cnt;
   unsigned carry = 0;
@@ -4211,9 +4223,151 @@ __global__ void __launch_bounds__(128) k_dec_dc(const DecSeg *__restrict__ segs,
     unsigned x = v;
     for (int of = 1; of < 32; of <<= 1) { const unsigned y = __shfl_up_sync(0xffffffffu, x, of); if (lane >= of) x += y; }
     const unsigned s = x + carry;
-    if (e < total) { int16_t *dst = dec_block(*o, sc, g.mcu0 + m, slot); if (dst) dst[0] = (int16_t)s; }
+    if (e < total) { int16_t *dst = dec_block(*o, sc, g.mcu0 + m, slot); if (dst) dst[0] = (int16_t)(s << sc.Al); }
     carry = __shfl_sync(0xffffffffu, s, 31);
   }
+}
+
+// ---------------------------------------------------------------- successive-approximation refinement scans
+
+// one thread per block of every DC refinement segment (decode_mcu_DC_refine, jdphuff.c:443-489): block j of a segment
+// ORs bit j of the segment, at 1 << Al, into its DC.  Refinements of different Al touch different bits, so every DC
+// refinement scan runs in this one launch; the OR goes through the 32-bit word holding coefficients 0 and 1.  A
+// segment with fewer bits than blocks sets status 1.
+__global__ void __launch_bounds__(128) k_dec_dc_refine(const uint32_t *__restrict__ words, const DecSeg *__restrict__ segs, int nsegs,
+                                                       const DecScan *__restrict__ scans, long long nblocks, const DecOut *__restrict__ o,
+                                                       uint32_t *__restrict__ status)
+{
+  const long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= nblocks) return;
+  int lo = 0, hi = nsegs - 1;
+  while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (segs[mid].blk0 <= j) lo = mid; else hi = mid - 1; }
+  const DecSeg g = segs[lo];
+  const DecScan &sc = scans[g.scan];
+  const long long b = j - g.blk0;
+  if (b >= (long long)g.nbits) { if (b == (long long)g.nbits) atomicOr(&status[sc.img], 1u); return; }
+  if (!((dec_bswap(words[g.word0 + (b >> 5)]) >> (31 - (b & 31))) & 1u)) return;
+  int16_t *dst = dec_block(*o, sc, g.mcu0 + b / sc.nb, (int)(b % sc.nb));
+  if (dst) atomicOr(reinterpret_cast<unsigned *>(dst), (1u << sc.Al) & 0xFFFFu);
+}
+
+// the zigzag index of each natural position (the inverse of c_zz)
+__constant__ uint8_t c_unzz[64] = {
+   0,  1,  5,  6, 14, 15, 27, 28,  2,  4,  7, 13, 16, 26, 29, 42,  3,  8, 12, 17, 25, 30, 41, 43,  9, 11, 18, 24, 31, 40, 44, 53,
+  10, 19, 23, 32, 39, 45, 52, 54, 20, 22, 33, 38, 46, 51, 55, 60, 21, 34, 37, 47, 50, 56, 59, 61, 35, 36, 48, 49, 57, 58, 62, 63};
+
+// n (<= 64) bits at pos, MSB first, into the low bits
+__device__ __forceinline__ unsigned long long dec_bits(const uint32_t *w, uint32_t pos, int n)
+{
+  unsigned long long x = 0;
+  while (n > 0) { const int c = n < 24 ? n : 24; x = (x << c) | (dec_window(w, pos) >> (32 - c)); pos += c; n -= c; }
+  return x;
+}
+
+// bits (MSB first: the first bit for the lowest set bit of mask) spread over the set bits of mask
+__device__ __forceinline__ unsigned long long dec_deposit(unsigned long long mask, unsigned long long bits, int n)
+{
+  unsigned long long r = 0;
+  for (int i = n - 1; i >= 0; i--) { const unsigned long long lowest = mask & (0ull - mask); if ((bits >> i) & 1ull) r |= lowest; mask ^= lowest; }
+  return r;
+}
+
+// One warp per AC refinement segment of one level (decode_mcu_AC_refine, jdphuff.c:497-640), its blocks in order: the
+// bits a block takes depend on which coefficients of its band are already nonzero, so a segment is decoded serially.
+// Each block's 128 bytes come in one coalesced load (the next block's is in flight meanwhile); a ballot gives the
+// band's nonzero mask in zigzag order; every lane runs the same symbol decode, walking the correction bits over the
+// mask's set bits; the lanes then write the changed coefficients back.  Status: 1 for an invalid code or too few bits,
+// 2 for a new coefficient past a band that ends before 63, 4 for a symbol of size other than 1.
+__global__ void __launch_bounds__(128) k_dec_ac_refine(const uint32_t *__restrict__ words, const DecSeg *__restrict__ segs, int nsegs,
+                                                       const DecScan *__restrict__ scans, const DecTable *__restrict__ tabs,
+                                                       const DecOut *__restrict__ o, uint32_t *__restrict__ status)
+{
+  const int gw = (int)(((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+  const int lane = threadIdx.x & 31;
+  if (gw >= nsegs) return;
+  const DecSeg g = segs[gw];
+  const DecScan &sc = scans[g.scan];
+  const DecTable &t = tabs[sc.tac[0]];
+  const uint32_t *w = words + g.word0;
+  const int Ss = sc.Ss, Se = sc.Se, p1 = 1 << sc.Al, m1 = -p1;
+  const unsigned long long band = (Se == 63 ? ~0ull : (1ull << (Se + 1)) - 1) & ~((1ull << Ss) - 1);
+  const int z0 = c_unzz[2 * lane], z1 = c_unzz[2 * lane + 1], n0 = c_zz[lane], n1 = c_zz[lane + 32];
+  const long long need = g.nmcu;
+  uint32_t pos = 0, eobrun = 0, err = 0;
+  unsigned *blk = need ? reinterpret_cast<unsigned *>(dec_block(*o, sc, g.mcu0, 0)) : nullptr;
+  unsigned nxt = blk ? blk[lane] : 0u;
+  for (long long b = 0; b < need && !err; b++) {
+    unsigned *cur = blk;
+    const unsigned word = nxt;
+    if (b + 1 < need) { blk = reinterpret_cast<unsigned *>(dec_block(*o, sc, g.mcu0 + b + 1, 0)); nxt = blk[lane]; }
+    const int16_t c0 = (int16_t)(word & 0xFFFFu), c1 = (int16_t)(word >> 16);
+    // the nonzero coefficients of the band as a zigzag mask: lane l looks up zigzag indices l and l + 32
+    const unsigned q0 = __shfl_sync(0xffffffffu, word, n0 >> 1), q1 = __shfl_sync(0xffffffffu, word, n1 >> 1);
+    const unsigned long long zmask = ((unsigned long long)__ballot_sync(0xffffffffu, ((n0 & 1) ? q0 >> 16 : q0 & 0xFFFFu) != 0) |
+                                      (unsigned long long)__ballot_sync(0xffffffffu, ((n1 & 1) ? q1 >> 16 : q1 & 0xFFFFu) != 0) << 32) & band;
+    unsigned long long inc = 0, newnz = 0, newneg = 0;
+    int k = Ss;
+    if (eobrun == 0) {
+      for (; k <= Se; k++) {
+        int sym;
+        const uint32_t win = dec_window(w, pos);
+        const int len = dec_symbol(win, t, sym);
+        if (!len || pos + (uint32_t)len > g.nbits) { err = 1; break; }
+        pos += len;
+        int r = sym >> 4, s = sym & 15;
+        bool neg = false;
+        if (s) {
+          if (s != 1) { err = 4; break; }
+          if (pos + 1 > g.nbits) { err = 1; break; }
+          neg = !((dec_window(w, pos) >> 31) & 1u); pos++;
+        } else if (r != 15) {
+          if (pos + (uint32_t)r > g.nbits) { err = 1; break; }
+          eobrun = (1u << r) + (r ? (uint32_t)dec_bits(w, pos, r) : 0u); pos += r;
+          break;
+        }
+        // the (r + 1)-th zero at or after k is the target; the nonzero ones before it take a correction bit each
+        unsigned long long zeros = ~zmask & band & ~((1ull << k) - 1);
+        for (int i = 0; i < r && zeros; i++) zeros &= zeros - 1;
+        const int target = zeros ? __ffsll((long long)zeros) - 1 : Se + 1;
+        const unsigned long long before = zmask & ~((1ull << k) - 1) & (target >= 64 ? ~0ull : (1ull << target) - 1);
+        const int nc = __popcll(before);
+        if (pos + (uint32_t)nc > g.nbits) { err = 1; break; }
+        inc |= dec_deposit(before, dec_bits(w, pos, nc), nc); pos += nc;
+        k = target;
+        if (s) {
+          if (k > Se && Se < 63) { err = 2; break; }
+          const int z = k > 63 ? 63 : k;
+          newnz |= 1ull << z; if (neg) newneg |= 1ull << z; else newneg &= ~(1ull << z);
+        }
+      }
+    }
+    if (!err && eobrun > 0) {
+      const unsigned long long rest = zmask & (k >= 64 ? 0ull : ~((1ull << k) - 1));
+      const int nc = __popcll(rest);
+      if (pos + (uint32_t)nc > g.nbits) err = 1;
+      else { inc |= dec_deposit(rest, dec_bits(w, pos, nc), nc); pos += nc; eobrun--; }
+    }
+    if (err || !(inc | newnz)) continue;
+    int v0 = c0, v1 = c1;
+    if ((newnz >> z0) & 1) v0 = ((newneg >> z0) & 1) ? m1 : p1;
+    else if (((inc >> z0) & 1) && !(v0 & p1)) v0 += v0 >= 0 ? p1 : m1;
+    if ((newnz >> z1) & 1) v1 = ((newneg >> z1) & 1) ? m1 : p1;
+    else if (((inc >> z1) & 1) && !(v1 & p1)) v1 += v1 >= 0 ? p1 : m1;
+    cur[lane] = (unsigned)(uint16_t)v0 | (unsigned)(uint16_t)v1 << 16;
+  }
+  if (err && lane == 0) atomicOr(&status[sc.img], (uint32_t)err);
+}
+
+void launch_decode_refine(const uint32_t *words, const DecSeg *dcr, int ndcr, long long dcr_blocks, const DecSeg *acr, const int *acr_level, int nlevels,
+                          const DecScan *scans, const DecTable *tabs, const DecOut *o, uint32_t *status, cudaEvent_t *marks, cudaStream_t s)
+{
+  if (ndcr) { k_dec_dc_refine<<<(unsigned)((dcr_blocks + 127) / 128), 128, 0, s>>>(words, dcr, ndcr, scans, dcr_blocks, o, status); LAUNCHED(); }
+  cudaEventRecord(marks[0], s);
+  for (int l = 0; l < nlevels; l++) {
+    const int n = acr_level[l + 1] - acr_level[l];
+    if (n) { k_dec_ac_refine<<<(unsigned)((n * 32 + 127) / 128), 128, 0, s>>>(words, acr + acr_level[l], n, scans, tabs, o, status); LAUNCHED(); }
+  }
+  cudaEventRecord(marks[1], s);
 }
 
 void launch_decode(const uint32_t *words, const DecSeg *segs, int nsegs, const DecScan *scans, const DecTable *tabs, long long nsub,

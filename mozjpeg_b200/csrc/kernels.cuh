@@ -240,13 +240,21 @@ void launch_lossless_encode(const Geom &g, const ScanDesc &sd, const uint16_t *d
 struct AlSearch { ScanDesc sd[24]; int first, per_al, nband, al_max, nscans_total; };
 void launch_select_al(const Geom &g, const AlSearch &as, const DevHuff *tabs_scan, const uint32_t *scan_size, int n, int *best_al, cudaStream_t s);
 
-// sequential Huffman decode (decode.cuh): k_dec_sync, k_dec_fix, the block-count scan, k_dec_write, k_dec_dc on the
-// batch's descriptors; rec: nsub records, pre: nsub words, tsum: ceil(nsub / 1024) words, dcd: one int per block of
-// every scan (dummy blocks included); o: the destination in device memory; the planes are zeroed by the caller; status[img] bit 0 = corrupt data;
+// Huffman decode of the first scans (decode.cuh): k_dec_sync, k_dec_fix, the block-count scan, k_dec_write, k_dec_dc on
+// the batch's descriptors; rec: nsub records, pre: nsub words, tsum: ceil(nsub / 1024) words, dcd: one int per block of
+// every scan (dummy blocks included); o: the destination in device memory; the planes are zeroed by the caller; status[img] bit 0 = corrupt data, bit 1 = a
+// coefficient past its band;
 // max_rounds / redone: synchronisation work (zeroed by the caller); marks: 6 events recorded around the stages
 void launch_decode(const uint32_t *words, const DecSeg *segs, int nsegs, const DecScan *scans, const DecTable *tabs, long long nsub,
                    DecRec *rec, uint32_t *pre, unsigned long long *tsum, int *dcd, const DecOut *o, uint32_t *status,
                    int *max_rounds, unsigned long long *redone, cudaEvent_t *marks, cudaStream_t s);
+
+// the refinement scans of progressive files, after launch_decode: k_dec_dc_refine over the dcr_blocks blocks of the ndcr
+// DC refinement segments, then k_dec_ac_refine once per level over AC refinement segments [acr_level[l],
+// acr_level[l + 1]) (acr_level: host memory); status[img]: bit 0 corrupt data or too few bits, bit 1 a coefficient past
+// its band, bit 2 a refinement symbol of size other than 1; marks: 2 events recorded behind the two stages
+void launch_decode_refine(const uint32_t *words, const DecSeg *dcr, int ndcr, long long dcr_blocks, const DecSeg *acr, const int *acr_level, int nlevels,
+                          const DecScan *scans, const DecTable *tabs, const DecOut *o, uint32_t *status, cudaEvent_t *marks, cudaStream_t s);
 
 // decompression to pixels behind the entropy decode (jpeg_read_scanlines of a default decompress object, 8-bit).
 // k_idct_islow: coef [n][hib][wib][64] natural order -> out [n][hib * 8][wib * 8] samples, dequantized with image i's

@@ -353,19 +353,60 @@ extern "C" int b200jpeg_decompress_output_opts(const b200jpeg_source_info *src, 
 
 namespace b200 {
 
-// The descriptors of a batch of sequential files (see decode.cuh).  The unstuffed words go to alloc(bound) first.
+int check_progression(const b200jpeg_source_info &s, int coef_bits[4][64])
+{
+  for (int c = 0; c < 4; c++) for (int k = 0; k < 64; k++) coef_bits[c][k] = -1;
+  for (int n = 0; n < s.num_scans; n++) {
+    const b200jpeg_source_scan &sc = s.scans[n];
+    const bool dc = sc.Ss == 0;
+    bool bad = dc ? sc.Se != 0 : (sc.Ss > sc.Se || sc.Se >= 64 || sc.comps_in_scan != 1);
+    if ((sc.Ah != 0 && sc.Al != sc.Ah - 1) || sc.Al > 13) bad = true;
+    if (bad) { set_error("scan %d: bad progression parameters Ss=%d Se=%d Ah=%d Al=%d", n, sc.Ss, sc.Se, sc.Ah, sc.Al); return B200JPEG_ERR_BAD_SOURCE; }   // JERR_BAD_PROGRESSION
+    for (int i = 0; i < sc.comps_in_scan; i++) {
+      int *cb = coef_bits[sc.component_index[i]];
+      if (!dc && cb[0] < 0) { set_error("scan %d: bogus progression: AC scan of component %d before its DC scan", n, sc.component_index[i]); return B200JPEG_ERR_BAD_SOURCE; }
+      for (int k = sc.Ss; k <= sc.Se; k++) {
+        if (sc.Ah != (cb[k] < 0 ? 0 : cb[k])) { set_error("scan %d: bogus progression: Ah=%d for coefficient %d of component %d, which holds %d", n, sc.Ah, k, sc.component_index[i], cb[k]); return B200JPEG_ERR_BAD_SOURCE; }
+        if (sc.Ah == 0 && cb[k] >= 0) { set_error("scan %d: bogus progression: a second first scan of coefficient %d of component %d", n, k, sc.component_index[i]); return B200JPEG_ERR_BAD_SOURCE; }
+        cb[k] = sc.Al;
+      }
+    }
+  }
+  return B200JPEG_OK;
+}
+
+bool smoothing_applies(const b200jpeg_source_info &s, const int coef_bits[4][64])
+{
+  static const int kPos[10] = {0, 1, 8, 16, 9, 2, 3, 10, 17, 24};      // Q00_POS .. Q30_POS
+  if (s.sof != 0xC2) return false;
+  bool useful = false;
+  for (int c = 0; c < s.num_components; c++) {
+    if (!s.comp_quant_present[c]) return false;
+    for (int i = 0; i < 10; i++) if (!s.comp_quant[c][kPos[i]]) return false;
+    if (coef_bits[c][0] < 0) return false;
+    for (int k = 1; k < 10; k++) if (coef_bits[c][k] != 0) useful = true;
+  }
+  return useful;
+}
+
+// The descriptors of a batch of files (see decode.cuh).  The unstuffed words go to alloc(bound) first.
 int build_decode_batch(const uint8_t *const *files, const size_t *sizes, int n, DecBatch &b, uint32_t *(*alloc)(void *, size_t), void *ctx, int first)
 {
   if (b.want_markers) b.markers.resize(n);
-  b.info.resize(n); b.scans.clear(); b.segs.clear(); b.tabs.clear();
-  b.nsub = 0; b.nblocks = 0;
+  b.info.resize(n); b.scans.clear(); b.segs.clear(); b.dcr_segs.clear(); b.acr_segs.clear(); b.tabs.clear();
+  b.nsub = 0; b.nblocks = 0; b.dcr_blocks = 0;
+  std::vector<std::vector<DecSeg>> acr;                // AC refinement segments by level
   size_t bound = 0;
   for (int i = 0; i < n; i++) {
     if (!files[i]) { set_error("image %d: no file", first + i); return B200JPEG_ERR_PARAM; }
     b200jpeg_source_info &s = b.info[i];
     int rc = parse_source(files[i], sizes[i], &s, b.want_markers ? &b.markers[i] : nullptr);
     if (rc) { std::string m = b200jpeg_last_error(); set_error("image %d: %s", first + i, m.c_str()); return rc; }
-    if (s.sof == 0xC2) { set_error("image %d: progressive (SOF2) source: the device decode takes sequential files; pass its coefficients instead", first + i); return B200JPEG_ERR_UNSUPPORTED; }
+    if (s.sof == 0xC2 && !b.progressive) { set_error("image %d: progressive (SOF2) source: the device decode takes sequential files; pass its coefficients instead", first + i); return B200JPEG_ERR_UNSUPPORTED; }
+    if (s.sof == 0xC2) {
+      int cb[4][64];
+      if ((rc = check_progression(s, cb))) { std::string m = b200jpeg_last_error(); set_error("image %d: %s", first + i, m.c_str()); return rc; }
+    }
     const b200jpeg_source_info &s0 = b.info[0];
     bool same = s.image_width == s0.image_width && s.image_height == s0.image_height && s.data_precision == s0.data_precision && s.num_components == s0.num_components;
     for (int c = 0; same && c < s.num_components; c++) same = s.h_samp_factor[c] == s0.h_samp_factor[c] && s.v_samp_factor[c] == s0.v_samp_factor[c];
@@ -404,28 +445,34 @@ int build_decode_batch(const uint8_t *const *files, const size_t *sizes, int n, 
       b.tabs.push_back(t); tix[pool * 2 + dc] = (int)b.tabs.size() - 1;
       return (int)b.tabs.size() - 1;
     };
-    int scanned[4] = {0, 0, 0, 0};
+    int scanned[4] = {0, 0, 0, 0}, ac_refines[4] = {0, 0, 0, 0};
+    const bool prog = s.sof == 0xC2;
     for (int k = 0; k < s.num_scans; k++) {
       const b200jpeg_source_scan &ss = s.scans[k];
-      if (ss.Ss != 0 || ss.Se != 63 || ss.Ah != 0 || ss.Al != 0) { set_error("image %d: scan %d is not a sequential scan (Ss=%d Se=%d Ah=%d Al=%d)", first + i, k, ss.Ss, ss.Se, ss.Ah, ss.Al); return B200JPEG_ERR_BAD_SOURCE; }
+      if (!prog && (ss.Ss != 0 || ss.Se != 63 || ss.Ah != 0 || ss.Al != 0)) { set_error("image %d: scan %d is not a sequential scan (Ss=%d Se=%d Ah=%d Al=%d)", first + i, k, ss.Ss, ss.Se, ss.Ah, ss.Al); return B200JPEG_ERR_BAD_SOURCE; }
       DecScan sc; memset(&sc, 0, sizeof sc);
       sc.img = i; sc.ncomp = ss.comps_in_scan;
+      sc.kind = !prog ? DEC_SEQ : ss.Ss == 0 ? (ss.Ah ? DEC_DC_REFINE : DEC_DC_FIRST) : (ss.Ah ? DEC_AC_REFINE : DEC_AC_FIRST);
+      sc.Ss = ss.Ss; sc.Se = ss.Se; sc.Al = ss.Al;
+      const bool need_dc = sc.kind == DEC_SEQ || sc.kind == DEC_DC_FIRST, need_ac = sc.kind == DEC_SEQ || sc.kind >= DEC_AC_FIRST;
       const long long mcus = scan_mcus(ss);
       sc.per_row = sc.ncomp == 1 ? b.wib[ss.component_index[0]] : (b.W + hmax * 8 - 1) / (hmax * 8);
       int slot = 0;
       for (int j = 0; j < sc.ncomp; j++) {
         const int c = ss.component_index[j];
-        if (scanned[c]++) { set_error("image %d: component %d appears in two sequential scans", first + i, c); return B200JPEG_ERR_UNSUPPORTED; }
+        if (!prog && scanned[c]++) { set_error("image %d: component %d appears in two sequential scans", first + i, c); return B200JPEG_ERR_UNSUPPORTED; }
         const int hh = sc.ncomp == 1 ? 1 : b.h[c], vv = sc.ncomp == 1 ? 1 : b.v[c];
         sc.ci[j] = c; sc.first[j] = slot; sc.cnt[j] = hh * vv; sc.mx[c] = hh; sc.my[c] = vv;
         if (slot + hh * vv > 10) { set_error("image %d: scan %d has more than 10 blocks per MCU", first + i, k); return B200JPEG_ERR_BAD_SOURCE; }   // JERR_BAD_MCU_SIZE
-        const int td = table(ss.dc_huff[j], true), ta = table(ss.ac_huff[j], false);
+        const int td = need_dc ? table(ss.dc_huff[j], true) : 0, ta = need_ac ? table(ss.ac_huff[j], false) : 0;
         for (int y = 0; y < vv; y++)
           for (int x = 0; x < hh; x++, slot++) { sc.comp[slot] = (int8_t)c; sc.dx[slot] = (int8_t)x; sc.dy[slot] = (int8_t)y; sc.tdc[slot] = (int16_t)td; sc.tac[slot] = (int16_t)ta; }
       }
       sc.nb = slot;
       const int scan_idx = (int)b.scans.size();
       b.scans.push_back(sc);
+      const int level = sc.kind == DEC_AC_REFINE ? ac_refines[sc.ci[0]]++ : 0;
+      if (level >= (int)acr.size()) acr.resize(level + 1);
       // restart segments: unstuff into the upload buffer, one word-aligned stream per segment
       const int ri = ss.restart_interval;
       const long long nseg = ri ? (mcus + ri - 1) / ri : 1;
@@ -455,16 +502,24 @@ int build_decode_batch(const uint8_t *const *files, const size_t *sizes, int n, 
         DecSeg g;
         g.word0 = wpos; g.nbits = (uint32_t)(cnt * 8); g.scan = scan_idx;
         g.mcu0 = (int)(sg * (ri ? ri : 0)); g.nmcu = (int)(ri ? std::min<long long>(ri, mcus - sg * ri) : mcus);
-        g.sub0 = b.nsub; g.nsub = std::max(1, (int)((g.nbits + DEC_SUB_BITS - 1) / DEC_SUB_BITS));
-        g.blk0 = b.nblocks;
-        b.nsub += g.nsub; b.nblocks += (long long)g.nmcu * sc.nb;
-        b.segs.push_back(g);
+        g.sub0 = 0; g.nsub = 0; g.blk0 = 0;
+        if (sc.kind == DEC_DC_REFINE) { g.blk0 = b.dcr_blocks; b.dcr_blocks += (long long)g.nmcu * sc.nb; b.dcr_segs.push_back(g); }
+        else if (sc.kind == DEC_AC_REFINE) acr[level].push_back(g);
+        else {
+          g.sub0 = b.nsub; g.nsub = std::max(1, (int)((g.nbits + DEC_SUB_BITS - 1) / DEC_SUB_BITS));
+          g.blk0 = b.nblocks;
+          b.nsub += g.nsub;
+          if (sc.kind != DEC_AC_FIRST) b.nblocks += (long long)g.nmcu * sc.nb;      // the DC differences
+          b.segs.push_back(g);
+        }
         wpos += words;
         if (cnt >= (1u << 29)) { set_error("image %d: a restart segment of 512 MB or more", first + i); return B200JPEG_ERR_UNSUPPORTED; }
       }
       // anything after the last segment's MCUs (further RSTn included) is ignored, like the reference
     }
   }
+  b.acr_level.assign(1, 0);
+  for (const std::vector<DecSeg> &l : acr) { b.acr_segs.insert(b.acr_segs.end(), l.begin(), l.end()); b.acr_level.push_back((int)b.acr_segs.size()); }
   b.nwords = wpos;
   return B200JPEG_OK;
 }

@@ -114,6 +114,7 @@ def main(argv: Sequence[str] = None) -> int:
     with open(files[0], "rb") as f:
         src = f.read()
     enc = Encoder(0)
+    enc.set_progressive_decode(True)          # the reference's djpeg reads progressive files too
     try:
         px = enc.decompress([src], **opts)[0]
     finally:

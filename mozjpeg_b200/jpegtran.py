@@ -319,8 +319,9 @@ def _same_except_quant(a: SourceInfo, b: SourceInfo) -> bool:
 def transcode(encoder, sources: Sequence[bytes], coef_planes: Optional[Sequence[Sequence]], switches: Sequence[str]) -> List[bytes]:
     """``jpegtran <switches>`` on same-shaped source files: sources[i] is the original file, coef_planes[ci] an
     (N, height_in_blocks, width_in_blocks, 64) int16 array of its quantized coefficients (natural order), or None:
-    the sources' entropy-coded data is then decoded on the device (sequential Huffman files; a progressive source
-    raises ValueError, pass its planes instead).
+    the sources' entropy-coded data is then decoded on the device (sequential Huffman files, and progressive ones
+    when the encoder's progressive decode is on; otherwise a progressive source raises ValueError, pass its planes
+    instead).
     Every source keeps its own quantization tables (its DQT); everything else jpeg_copy_critical_parameters takes
     from a source must match the first one, else ValueError names the first source that differs."""
     infos = [parse_header(s) for s in sources]
@@ -357,7 +358,7 @@ def transcode(encoder, sources: Sequence[bytes], coef_planes: Optional[Sequence[
 
 def main(argv: Sequence[str] = None) -> int:
     """``python -m mozjpeg_b200.jpegtran [switches] [-outfile name] file.jpg`` - jpegtran's command line on the device
-    path, from the file's bytes (sequential Huffman sources)."""
+    path, from the file's bytes (sequential and progressive Huffman sources, as the reference's jpegtran reads both)."""
     import sys
     from . import Encoder
     args = list(sys.argv[1:] if argv is None else argv)
@@ -392,6 +393,7 @@ def main(argv: Sequence[str] = None) -> int:
         print(f"jpegtran: {e}", file=sys.stderr)          # jpegtran.c:679-682
         return 1
     enc = Encoder(0)
+    enc.set_progressive_decode(True)
     try:
         out = transcode(enc, [src], None, switches)[0]
     finally:

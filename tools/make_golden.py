@@ -431,7 +431,48 @@ def decompress_options():
     print("wrote", len(cases), "cases,", len(refused), "refused pairs")
 
 
+# jpegtran switch sets the progressive goldens record
+PROGRESSIVE_JPEGTRAN = [[], ["-optimize"], ["-progressive"], ["-rotate", "90"], ["-crop", "48x32+9+5"]]
+
+
+def progressive():
+    """tests/golden/progressive_golden.json: for every source of tests/progressive_cases.py the md5 of the file, of the
+    reference's jpeg_read_coefficients planes, of its jpegtran output for each PROGRESSIVE_JPEGTRAN switch set and of
+    its default decompression (build/librefdec.so), or the reference's refusal of the file, and whether that
+    decompression block-smooths it (build/librefsmooth.so, tests/refsmooth.c)."""
+    import subprocess
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import progressive_cases as P
+    import recompress_cases as R
+    if not R.have_reference():
+        sys.exit("build/librefdec.so is missing: run __graft_entry__.build() with the reference build under oracle/_ref/")
+    cases = []
+    for sid, src in P.all_sources():
+        rec = {"id": sid, "src_md5": P.md5(src)}
+        try:
+            rec["coef_md5"] = P.md5_planes(O.ref_read_coefs(src)["coefs"])
+        except Exception as e:                                  # noqa: BLE001 (the reference's refusal is the record)
+            rec["coef_error"] = str(e).splitlines()[0] if str(e) else type(e).__name__
+        tran = {}
+        for sw in PROGRESSIVE_JPEGTRAN:
+            r = subprocess.run([os.path.join(O.REF_DIR, "jpegtran"), *sw], input=src, capture_output=True)
+            tran[" ".join(sw)] = P.md5(r.stdout) if r.returncode in (0, 2) else None       # 2: written with warnings
+        rec["jpegtran"] = tran
+        try:
+            px, _ = R.ref_decompress(src)
+            rec["pix_md5"] = P.md5(px)
+        except RuntimeError:
+            rec["pix_md5"] = None
+        rec["ref_smooths"] = P.ref_smooths(src)
+        cases.append(rec)
+    json.dump({"generator": "tools/make_golden.py --progressive", "reference": "mozilla/mozjpeg 5.0.0 (C path, WITH_SIMD=0), oracle/_ref",
+               "jpegtran_switches": PROGRESSIVE_JPEGTRAN, "cases": cases}, open(os.path.join(GOLD, "progressive_golden.json"), "w"), indent=0)
+    print("wrote", len(cases), "progressive cases")
+
+
 def main():
+    if "--progressive" in sys.argv:
+        return progressive()
     if "--decompress-options" in sys.argv:
         return decompress_options()
     if "--recompress" in sys.argv:

@@ -85,5 +85,19 @@ for kw in (dict(scale=(1, 8)), dict(scale=(1, 4), dct="fast", fancy=False), dict
            dict(dct="fast", colorspace="gray"), dict(fancy=False, colorspace="xrgb")):
     n += len(enc.decompress(rag, **kw))
     n += len(enc.recompress(mj.params_for_jpeg_input(["-baseline", "-quality", "75"], rag[0], **kw), rag, **kw))
+# progressive decode: the default profile (scan search, successive approximation), the standard script with restarts,
+# mixed with sequential files, through the coefficient, transcode and pixel routes; then a truncated refinement scan
+enc.set_progressive_decode(True)
+prog = enc.encode_batch(mj.params_from_switches(["-quality", "75"], w, h), img)
+prog_rst = enc.encode_batch(mj.params_from_switches(["-revert", "-progressive", "-restart", "1"], w, h), img)
+n += len(enc.read_coefficients(prog + prog_rst + srcs))
+n += len(T.transcode(enc, prog, None, ["-rotate", "90"]))
+n += len(enc.decompress(prog_rst, scale=(1, 4)))
+last = T.parse_source(prog[0]).scans[-1]
+try:
+    enc.read_coefficients([prog[0][:last.data_offset + last.data_size // 2]])
+except mj.B200JpegError as e:
+    assert e.code == mj._abi.ERR_BAD_SOURCE, e
+enc.set_progressive_decode(False)
 print("sanitize cases done:", n, "files, kernel launches", enc.kernel_launches())
 enc.close()
