@@ -103,6 +103,7 @@ template <bool PROG>
 DEC_HD uint32_t dec_step(const uint32_t *w, uint32_t nbits, uint32_t &pos, uint32_t st, const DecScan &sc, const DecTable *tabs,
                          int &zz, int &val, int &done)
 {
+  zz = -1; val = 0; done = 0;                             // a dead stream completes no block
   int k = (int)(st & 127), slot = (int)(st >> 7);
   const bool acf = PROG && sc.kind == DEC_AC_FIRST;
   if (acf && k == 0) k = sc.Ss;
@@ -119,7 +120,7 @@ DEC_HD uint32_t dec_step(const uint32_t *w, uint32_t nbits, uint32_t &pos, uint3
   int v = 0;
   if (s) v = x < (1 << (s - 1)) ? x + (int)(~0u << s) + 1 : x;   // HUFF_EXTEND (jdhuff.c:483-490)
   pos += (uint32_t)(len + extra);
-  zz = -1; val = v; done = 0;
+  val = v;
   if (k == 0) { zz = 0; k = PROG && sc.kind == DEC_DC_FIRST ? 64 : 1; }
   else if (s) { k += r; zz = k > 63 ? 63 : k; k++; }
   else if (r == 15) k += 16;
