@@ -80,12 +80,12 @@ using namespace b200;
 struct Arena {
   b200::DevBuf d_planes;             // input smoothing: the pre-pass's component planes
   b200::DevBuf d_coef[4], d_raw[4], d_plain[4], d_hist, d_tabs_trellis, d_rec, d_srec, d_splits, d_best_al, d_qimg, d_qsum, d_eo, d_es;
-  b200::DevBuf d_blk_bits, d_tile_bits, d_tile_base, d_seg_corr, d_mark, d_stuff_lb, d_blk_aux, d_blk_run, d_blk_mask, d_total_bits, d_bitbuf;
+  b200::DevBuf d_blk_bits, d_slot, d_tile_bits, d_tile_base, d_seg_corr, d_mark, d_stuff_lb, d_blk_aux, d_blk_run, d_blk_mask, d_total_bits, d_bitbuf;
   b200::DevBuf d_sym, d_dcq;         // sequential scans after the trellis: symbol records + dense DC values (SymOut, kernels.cuh)
   b200::DevBuf d_diff;               // lossless scans: the differences of the scan being coded (launch_lossless_diff)
   b200::Geom g;                      // the plan's geometry with this arena's coefficient pointers
   void release() {
-    b200::DevBuf *db[] = {&d_planes, &d_hist, &d_tabs_trellis, &d_rec, &d_srec, &d_splits, &d_best_al, &d_qimg, &d_qsum, &d_eo, &d_es, &d_blk_bits, &d_tile_bits, &d_tile_base, &d_seg_corr, &d_mark, &d_stuff_lb, &d_blk_aux, &d_blk_run, &d_blk_mask, &d_total_bits, &d_bitbuf, &d_sym, &d_dcq, &d_diff};
+    b200::DevBuf *db[] = {&d_planes, &d_hist, &d_tabs_trellis, &d_rec, &d_srec, &d_splits, &d_best_al, &d_qimg, &d_qsum, &d_eo, &d_es, &d_blk_bits, &d_slot, &d_tile_bits, &d_tile_base, &d_seg_corr, &d_mark, &d_stuff_lb, &d_blk_aux, &d_blk_run, &d_blk_mask, &d_total_bits, &d_bitbuf, &d_sym, &d_dcq, &d_diff};
     for (b200::DevBuf *b : db) b->release();
     for (int i = 0; i < 4; i++) { d_coef[i].release(); d_raw[i].release(); d_plain[i].release(); }
   }
@@ -456,6 +456,13 @@ static size_t smooth_plane_bytes(const Geom &g)
 
 // Sequential scans behind the default trellis (one round over 1..63 by k_trellis_ac3): the entropy stages read the symbol
 // records the trellis back-track leaves instead of the coefficient planes.  B200JPEG_SYMREC=0 keeps them on the planes.
+// code slots for the sequential scans (k_block_bits_seq / k_encode_seq): not at 12 bits, where most blocks are longer
+// than a slot, so that packing them from slots saves nothing and filling the slots costs the bit-count pass (DESIGN §5)
+static bool use_slots(const Plan &pl, const b200jpeg_params *p)
+{
+  return !pl.progressive && !pl.lossless && p->data_precision == 8;
+}
+
 static bool use_symrec(const Plan &pl, const b200jpeg_params *p)
 {
   static const bool off = getenv("B200JPEG_SYMREC") && getenv("B200JPEG_SYMREC")[0] == '0';
@@ -508,6 +515,7 @@ static int prepare_batch(b200jpeg_encoder *e, int n_total, int chunk, bool host_
     }
     if (pl.lossless) { if ((rc = a.d_diff.reserve((size_t)n * pl.max_scan_blocks * g.nc * 2))) return rc; }
     if ((rc = a.d_blk_bits.reserve((size_t)n * pl.max_scan_blocks * 4))) return rc;
+    if (use_slots(pl, p)) { if ((rc = a.d_slot.reserve((size_t)n * pl.max_scan_blocks * sizeof(SeqSlot)))) return rc; }
     if (pl.progressive) { if ((rc = a.d_blk_aux.reserve((size_t)n * pl.max_scan_blocks * 4))) return rc; if ((rc = a.d_blk_run.reserve((size_t)n * pl.max_scan_blocks * 4))) return rc; if ((rc = a.d_blk_mask.reserve((size_t)n * pl.max_scan_blocks * 24))) return rc; }
     if ((rc = a.d_total_bits.reserve((size_t)n * 8))) return rc;
     if ((rc = a.d_tile_bits.reserve((size_t)n * ((pl.max_scan_blocks + 255) / 256) * 4))) return rc;
@@ -822,6 +830,7 @@ static int run_pipeline(b200jpeg_encoder *e, const ChunkIO &io, Timer &tm)
   const DcRec *nz_rec = (pl.trellis && !pl.progressive && !symrec) ? A.d_rec.as<DcRec>() : nullptr;
   const uint8_t *sym = symrec ? A.d_sym.as<uint8_t>() : nullptr;
   const int16_t *dcq = symrec ? A.d_dcq.as<int16_t>() : nullptr;
+  SeqSlot *slot = use_slots(pl, p) ? A.d_slot.as<SeqSlot>() : nullptr;
   for (size_t j = 0; j < pl.order.size(); j++) {
     const int si = pl.order[j];
     ScanDesc sd = pl.scans[si];
@@ -865,7 +874,7 @@ static int run_pipeline(b200jpeg_encoder *e, const ChunkIO &io, Timer &tm)
     } else { tabs = e->d_tabs_fixed.as<DevHuff>(); tstride = 0; }
     const size_t mark_words = (e->bitbuf_words_per_image * 4 / 8 + 64) / 4;
     tm.mark("block_bits");
-    launch_block_bits(g, sd, nz_rec, sym, dcq, rl, tabs, tstride, pl.progressive, A.d_blk_bits.as<uint32_t>(), A.d_tile_bits.as<uint32_t>(), aux, run_e, pm, status, n, s);
+    launch_block_bits(g, sd, nz_rec, sym, dcq, rl, tabs, tstride, pl.progressive, A.d_blk_bits.as<uint32_t>(), A.d_tile_bits.as<uint32_t>(), slot, aux, run_e, pm, status, n, s);
     tm.mark("scan_layout");
     launch_scan_layout(sd, A.d_blk_bits.as<uint32_t>(), A.d_tile_bits.as<uint32_t>(), A.d_tile_base.as<unsigned long long>(),
                        A.d_seg_corr.as<uint32_t>(), pl.max_scan_blocks, A.d_total_bits.as<unsigned long long>(),
@@ -873,7 +882,7 @@ static int run_pipeline(b200jpeg_encoder *e, const ChunkIO &io, Timer &tm)
     tm.mark("encode");
     launch_zero_stream(A.d_bitbuf.as<uint32_t>(), e->bitbuf_words_per_image, A.d_total_bits.as<unsigned long long>(), n, s);
     if (sd.ri) CU(cudaMemsetAsync(A.d_mark.p, 0, mark_words * 4 * n, s));
-    launch_encode(g, sd, nz_rec, sym, dcq, rl, tabs, tstride, pl.progressive, A.d_blk_bits.as<uint32_t>(), A.d_tile_bits.as<uint32_t>(), A.d_tile_base.as<unsigned long long>(),
+    launch_encode(g, sd, nz_rec, sym, dcq, rl, tabs, tstride, pl.progressive, A.d_blk_bits.as<uint32_t>(), A.d_tile_bits.as<uint32_t>(), slot, A.d_tile_base.as<unsigned long long>(),
                   A.d_seg_corr.as<uint32_t>(), pl.max_scan_blocks, aux, run_e, pm,
                   A.d_bitbuf.as<uint32_t>(), e->bitbuf_words_per_image, A.d_mark.as<uint32_t>(), mark_words, status, n, s);
     tm.mark("stuff");

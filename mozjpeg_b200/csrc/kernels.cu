@@ -2949,6 +2949,36 @@ struct CountSink {
   __device__ void ac(int sym, int nb, int) { int s = asz[sym]; if (!s) bad = 1; bits += s + nb; }
 };
 
+// CountSink of the sequential scans, which also keeps the block's last SEQ_SLOT_BITS bits: code and value bits in
+// stream order, right-aligned in a[] (a[0] most significant).  Only a block of at most SEQ_SLOT_BITS bits stores them;
+// the packer walks a longer one again.
+struct SlotSink {
+  const uint16_t *dco, *aco; const uint8_t *dsz, *asz; unsigned bits; int bad;
+  unsigned a[SEQ_SLOT_WORDS];
+  __device__ void put(unsigned v, int n) {                    // v < 2^n, n <= 32: one funnel shift per word
+#pragma unroll
+    for (int i = 0; i < SEQ_SLOT_WORDS - 1; i++) a[i] = __funnelshift_lc(a[i + 1], a[i], n);
+    a[SEQ_SLOT_WORDS - 1] = __funnelshift_lc(__funnelshift_lc(0u, v, 32 - n), a[SEQ_SLOT_WORDS - 1], n);
+    bits += n;
+  }
+  __device__ void dc(int nb, int v) { const int s = dsz[nb]; if (!s) bad = 1; put((unsigned)dco[nb] << nb | ((unsigned)v & ((1u << nb) - 1u)), s + nb); }
+  __device__ void ac(int sym, int nb, int v) { const int s = asz[sym]; if (!s) bad = 1; put((unsigned)aco[sym] << nb | ((unsigned)v & ((1u << nb) - 1u)), s + nb); }
+  // the slot: the bit string left-aligned, first bit = bit 31 of word 0 (bits <= SEQ_SLOT_BITS)
+  __device__ SeqSlot slot() const {
+    const int sh = SEQ_SLOT_BITS - (int)bits;
+#if SEQ_SLOT_BITS > 64
+    unsigned long long h = (unsigned long long)a[0] << 32 | a[1], l = (unsigned long long)a[2] << 32 | a[3];
+    if (sh >= 64) { h = sh < 128 ? l << (sh - 64) : 0ull; l = 0; }
+    else if (sh) { h = (h << sh) | (l >> (64 - sh)); l <<= sh; }
+    return make_uint4((unsigned)(h >> 32), (unsigned)h, (unsigned)(l >> 32), (unsigned)l);
+#else
+    unsigned long long l = (unsigned long long)a[0] << 32 | a[1];
+    l = sh < 64 ? l << sh : 0ull;
+    return make_uint2((unsigned)(l >> 32), (unsigned)l);
+#endif
+  }
+};
+
 // sum of v over the CTA (256 threads), result valid in thread 0
 __device__ __forceinline__ unsigned cta_sum_256(unsigned v, unsigned *ws /* [8] shared */)
 {
@@ -2976,34 +3006,42 @@ __device__ __forceinline__ unsigned cta_excl_scan_256(unsigned v, unsigned *ws /
 }
 
 // One tile = the 256 blocks of one CTA; tile_bits[img][tile] = bits the tile emits; blk_bits[img][t] = bits
-// the tile's blocks before t emit (exclusive prefix inside the tile).
+// the tile's blocks before t emit (exclusive prefix inside the tile); slot[img][t] = block t's bit string when it
+// has at most SEQ_SLOT_BITS bits (not written otherwise; SLOTS = false: no slots, the packer walks every block).
+template <bool SLOTS>
 __global__ void __launch_bounds__(256) k_block_bits_seq(Geom g, ScanDesc sd, const DcRec *__restrict__ nz_rec, const uint8_t *__restrict__ sym, const int16_t *__restrict__ dcq,
                                                         RecLayout rl, const DevHuff *__restrict__ tabs, size_t stride,
-                                                        uint32_t *__restrict__ blk_bits, uint32_t *__restrict__ tile_bits, uint32_t *__restrict__ status)
+                                                        uint32_t *__restrict__ blk_bits, uint32_t *__restrict__ tile_bits, SeqSlot *__restrict__ slot,
+                                                        uint32_t *__restrict__ status)
 {
   __shared__ ScanTables st;
   __shared__ unsigned ws[8];
   int img = blockIdx.y;
-  load_scan_tables(st, tabs, stride, img, g, sd, false);
+  load_scan_tables(st, tabs, stride, img, g, sd, SLOTS);
   __syncthreads();
   long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   unsigned bits = 0;
-  if (t < sd.nblocks && sym) {
-    const CompGeom &c = g.c[sd.ci[sd.k_comp[(int)(t % sd.bim)]]];
-    CountSink sink{st.size[c.dc_tbl], st.size[4 + c.ac_tbl], 0u, 0};
-    walk_seq_rec(g, sd, sym, dcq, rl, img, t, sink);
-    if (sink.bad) atomicOr(&status[img], 2u);
-    bits = sink.bits;
-  } else if (t < sd.nblocks) {
+  if (t < sd.nblocks) {
     int sci, k; long long mcu;
-    const int16_t *blk = block_ptr(g, sd, img, t, sci, mcu, k);
-    int last = prev_dc(g, sd, img, t, sci, mcu, k);
+    const int16_t *blk = nullptr; int last = 0;
+    if (sym) sci = sd.k_comp[(int)(t % sd.bim)];
+    else { blk = block_ptr(g, sd, img, t, sci, mcu, k); last = prev_dc(g, sd, img, t, sci, mcu, k); }
     const CompGeom &c = g.c[sd.ci[sci]];
-    CountSink sink{st.size[c.dc_tbl], st.size[4 + c.ac_tbl], 0u, 0};
-    if (SEQ_SPARSE_STATS && nz_rec) walk_seq_sparse(blk, block_nzmask(g, sd, nz_rec, rl, img, sci, mcu, k), last, sink);
-    else walk_seq_block(blk, last, sink);
-    if (sink.bad) atomicOr(&status[img], 2u);
-    bits = sink.bits;
+    auto walk = [&](auto &sink) {
+      if (sym) walk_seq_rec(g, sd, sym, dcq, rl, img, t, sink);
+      else if (SEQ_SPARSE_STATS && nz_rec) walk_seq_sparse(blk, block_nzmask(g, sd, nz_rec, rl, img, sci, mcu, k), last, sink);
+      else walk_seq_block(blk, last, sink);
+      if (sink.bad) atomicOr(&status[img], 2u);
+      bits = sink.bits;
+    };
+    if constexpr (SLOTS) {
+      SlotSink sink{st.code[c.dc_tbl], st.code[4 + c.ac_tbl], st.size[c.dc_tbl], st.size[4 + c.ac_tbl], 0u, 0, {}};
+      walk(sink);
+      if (bits <= SEQ_SLOT_BITS) slot[(size_t)img * sd.nblocks + t] = sink.slot();
+    } else {
+      CountSink sink{st.size[c.dc_tbl], st.size[4 + c.ac_tbl], 0u, 0};
+      walk(sink);
+    }
   }
   unsigned tot;
   const unsigned pre = cta_excl_scan_256(bits, ws, tot);
@@ -3104,31 +3142,91 @@ struct BitSinkQ : BitSink {
   __device__ void ac(int sym, int nb, int v) { const unsigned e = acs[sym]; put(((e & 0xFFFFu) << nb) | ((unsigned)v & ((1u << nb) - 1u)), (int)(e >> 16) + nb); }
 };
 
+// 32 bits of a slot (SEQ_SLOT_WORDS words, bit string left-aligned) seen from a word that starts k bits into the block
+// (k < 0: the block starts -k bits into the word)
+__device__ __forceinline__ unsigned slot_window(const uint32_t *__restrict__ s, int k)
+{
+  if (k < 0) return s[0] >> -k;
+  const int i = k >> 5;
+  const unsigned a = i < SEQ_SLOT_WORDS ? s[i] : 0u, b = i + 1 < SEQ_SLOT_WORDS ? s[i + 1] : 0u;
+  return __funnelshift_l(b, a, k & 31);
+}
+
+// One CTA per tile of 256 blocks.  A block of at most SEQ_SLOT_BITS bits that does not end a restart segment (a slot
+// block) is copied from the slot k_block_bits_seq stored: output word w is built by the slot block holding bit 32w,
+// from its bits and those of the tile's blocks that follow it inside the word.  A word that lies wholly in the tile's
+// slot blocks is written with a plain store; every other one (the tile's edge words, words shared with a fallback
+// block or a restart marker) gets this CTA's part with atomicOr, into the stream k_zero_stream cleared.  The other
+// (fallback) blocks walk their record or coefficients again, as encode_one_block (jchuff.c:563-661) does, into
+// BitSinkQ, whose atomicOr only ever lands on words that no plain store writes.
 __global__ void __launch_bounds__(256) k_encode_seq(Geom g, ScanDesc sd, const DcRec *__restrict__ rec, const uint8_t *__restrict__ sym, const int16_t *__restrict__ dcq,
                                                     RecLayout rl, const DevHuff *__restrict__ tabs, size_t stride,
-                                                    const uint32_t *__restrict__ blk_bits, const uint32_t *__restrict__ tile_bits /* per-tile totals: not read here */,
-                                                    const unsigned long long *__restrict__ tile_base,
+                                                    const uint32_t *__restrict__ blk_bits, const uint32_t *__restrict__ tile_bits,
+                                                    const SeqSlot *__restrict__ slot, const unsigned long long *__restrict__ tile_base,
                                                     const uint32_t *__restrict__ seg_corr, long long seg_stride,
                                                     uint32_t *__restrict__ bitbuf, size_t bitbuf_stride_words,
                                                     uint32_t *__restrict__ mark, size_t mark_stride_words, const uint32_t *__restrict__ status)
 {
   __shared__ ScanTables st;
   __shared__ uint32_t acs[4][256];
-  int img = blockIdx.y;
-  load_scan_tables(st, tabs, stride, img, g, sd, true);
-  __syncthreads();
-  for (int i = 0; i < sd.ncomps; i++) {
-    const int sl = g.c[sd.ci[i]].ac_tbl;
-    for (int k = threadIdx.x; k < 256; k += blockDim.x) acs[sl][k] = (uint32_t)st.code[4 + sl][k] | (uint32_t)st.size[4 + sl][k] << 16;
-  }
-  __syncthreads();
+  __shared__ SeqSlot s_slot[256];
+  __shared__ unsigned s_off[257];           // bit offsets from the tile's first word; s_off[nt] = the last block's end
+  __shared__ uint8_t s_fb[256];             // fallback block
+  const int img = blockIdx.y;
   if (status[img] & ~1u) return;            // an earlier stage flagged this image (overflow / bad coefficient)
-  long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const int j = threadIdx.x;
+  const long long t0 = (long long)blockIdx.x * 256, t = t0 + j;
+  const int nt = (int)min(256LL, sd.nblocks - t0);
+  const long long seglen = (long long)sd.ri * sd.bim;
   const unsigned long long tb = tile_base[(size_t)img * gridDim.x + blockIdx.x];
+  const unsigned long long base = (tb + (sd.ri ? seg_corr[(size_t)img * seg_stride + t0 / seglen] : 0u)) >> 5;  // first word
   uint32_t *gbuf = bitbuf + (size_t)img * bitbuf_stride_words;
-  if (t < sd.nblocks) {
-    unsigned long long off = tb + blk_bits[(size_t)img * sd.nblocks + t];
-    if (sd.ri) off += seg_corr[(size_t)img * seg_stride + t / ((long long)sd.ri * sd.bim)];
+  unsigned long long off = 0;
+  unsigned len = 0;
+  bool fb = false;
+  if (j < nt) {
+    const uint32_t *pre = blk_bits + (size_t)img * sd.nblocks;
+    const unsigned p = pre[t];
+    len = (j + 1 < nt ? pre[t + 1] : tile_bits[(size_t)img * gridDim.x + blockIdx.x]) - p;
+    off = tb + p;
+    if (sd.ri) off += seg_corr[(size_t)img * seg_stride + t / seglen];
+    fb = !slot || len > SEQ_SLOT_BITS || (sd.ri && (t + 1) % seglen == 0 && t + 1 < sd.nblocks);
+    if (!fb) s_slot[j] = slot[(size_t)img * sd.nblocks + t];
+    s_off[j] = (unsigned)(off - base * 32);
+    s_fb[j] = fb;
+    if (j == nt - 1) s_off[nt] = s_off[j] + len;
+  }
+  if (__syncthreads_or(fb)) {               // table staging only for a tile that has fallback blocks
+    load_scan_tables(st, tabs, stride, img, g, sd, true);
+    __syncthreads();
+    for (int i = 0; i < sd.ncomps; i++) {
+      const int sl = g.c[sd.ci[i]].ac_tbl;
+      for (int k = threadIdx.x; k < 256; k += blockDim.x) acs[sl][k] = (uint32_t)st.code[4 + sl][k] | (uint32_t)st.size[4 + sl][k] << 16;
+    }
+    __syncthreads();
+  }
+  if (j >= nt) return;
+  if (!fb) {
+    const unsigned o = s_off[j];
+    // the words this block builds: those whose first bit it holds, and the word it starts in when that word's first
+    // bit is no slot block's of this tile (the tile's first block, or the block after a fallback one)
+    const unsigned w_lo = (o & 31) && (j == 0 || s_fb[j - 1]) ? o >> 5 : (o + 31) >> 5;
+    for (unsigned w = w_lo; w * 32 < o + len; w++) {
+      const unsigned W = w * 32;
+      unsigned word = 0;
+      bool whole = o <= W;                  // every bit of the word is a slot block's of this tile
+      int m = j;
+      for (; m < nt && s_off[m] < W + 32; m++) {
+        if (s_fb[m]) { whole = false; continue; }
+        word |= slot_window(reinterpret_cast<const uint32_t *>(&s_slot[m]), (int)(W - s_off[m]));
+      }
+      if (m == nt && s_off[nt] < W + 32) whole = false;
+      if (whole) gbuf[base + w] = word;
+      else if (word) atomicOr(&gbuf[base + w], word);
+    }
+    return;
+  }
+  {
     const CompGeom &c = g.c[sd.ci[sd.k_comp[(int)(t % sd.bim)]]];
     BitSinkQ sink;
     sink.buf = gbuf; sink.widx = off >> 5; sink.acc = 0; sink.nacc = (int)(off & 31);
@@ -3769,11 +3867,12 @@ void launch_gather_prog(const Geom &g, const ScanDesc &sd, const uint32_t *aux, 
 }
 
 void launch_block_bits(const Geom &g, const ScanDesc &sd, const DcRec *nz_rec, const uint8_t *sym, const int16_t *dcq, const RecLayout &rl, const DevHuff *tabs, size_t stride, int progressive,
-                       uint32_t *blk_bits, uint32_t *tile_bits, const uint32_t *blk_aux, const uint32_t *run_e, const unsigned long long *pm, uint32_t *status, int n, cudaStream_t s)
+                       uint32_t *blk_bits, uint32_t *tile_bits, SeqSlot *slot, const uint32_t *blk_aux, const uint32_t *run_e, const unsigned long long *pm, uint32_t *status, int n, cudaStream_t s)
 {
   dim3 grid((unsigned)((sd.nblocks + 255) / 256), n);
   if (progressive) k_block_bits_prog<<<grid, 256, 0, s>>>(g, sd, tabs, stride, blk_aux, run_e, pm, blk_bits, tile_bits, status);
-  else k_block_bits_seq<<<grid, 256, 0, s>>>(g, sd, nz_rec, sym, dcq, rl, tabs, stride, blk_bits, tile_bits, status);
+  else if (slot) k_block_bits_seq<true><<<grid, 256, 0, s>>>(g, sd, nz_rec, sym, dcq, rl, tabs, stride, blk_bits, tile_bits, slot, status);
+  else k_block_bits_seq<false><<<grid, 256, 0, s>>>(g, sd, nz_rec, sym, dcq, rl, tabs, stride, blk_bits, tile_bits, nullptr, status);
   LAUNCHED();
 }
 void launch_scan_layout(const ScanDesc &sd, const uint32_t *blk_bits, const uint32_t *tile_bits, unsigned long long *tile_base,
@@ -3804,13 +3903,13 @@ void launch_zero_stream(uint32_t *bitbuf, size_t stride_words, const unsigned lo
   k_zero_stream<<<grid, 256, 0, s>>>(bitbuf, stride_words, total_bits); LAUNCHED();
 }
 void launch_encode(const Geom &g, const ScanDesc &sd, const DcRec *nz_rec, const uint8_t *sym, const int16_t *dcq, const RecLayout &rl, const DevHuff *tabs, size_t stride, int progressive,
-                   const uint32_t *blk_bits, const uint32_t *tile_bits, const unsigned long long *tile_base, const uint32_t *seg_corr, long long seg_stride,
+                   const uint32_t *blk_bits, const uint32_t *tile_bits, const SeqSlot *slot, const unsigned long long *tile_base, const uint32_t *seg_corr, long long seg_stride,
                    const uint32_t *blk_aux, const uint32_t *run_e, const unsigned long long *pm,
                    uint32_t *bitbuf, size_t bitbuf_stride_words, uint32_t *mark, size_t mark_stride_words, const uint32_t *status, int n, cudaStream_t s)
 {
   dim3 grid((unsigned)((sd.nblocks + 255) / 256), n);
   if (progressive) k_encode_prog<<<grid, 256, 0, s>>>(g, sd, tabs, stride, blk_aux, run_e, pm, blk_bits, tile_bits, tile_base, seg_corr, seg_stride, bitbuf, bitbuf_stride_words, mark, mark_stride_words, status);
-  else k_encode_seq<<<grid, 256, 0, s>>>(g, sd, nz_rec, sym, dcq, rl, tabs, stride, blk_bits, tile_bits, tile_base, seg_corr, seg_stride, bitbuf, bitbuf_stride_words, mark, mark_stride_words, status);
+  else k_encode_seq<<<grid, 256, 0, s>>>(g, sd, nz_rec, sym, dcq, rl, tabs, stride, blk_bits, tile_bits, slot, tile_base, seg_corr, seg_stride, bitbuf, bitbuf_stride_words, mark, mark_stride_words, status);
   LAUNCHED();
 }
 // =====================================================================

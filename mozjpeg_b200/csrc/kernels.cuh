@@ -201,9 +201,25 @@ void launch_gather_seq_dc(const Geom &g, const ScanDesc &sd, const int16_t *dcq,
 // unsigned long long [3][n][nblocks] (written here, read by the three symbol walks of the scan)
 void launch_prog_prepare(const Geom &g, const ScanDesc &sd, uint32_t *aux, uint32_t *run_e, unsigned long long *pm, int *tile_last, int *tile_first, int n, cudaStream_t s);
 void launch_gather_prog(const Geom &g, const ScanDesc &sd, const uint32_t *aux, const uint32_t *run_e, const unsigned long long *pm, uint32_t *hist, uint32_t *status, int n, cudaStream_t s);
+// Code slots of the sequential scans: k_block_bits_seq stores the bit string of every block of at most SEQ_SLOT_BITS bits
+// (code and value bits, left-aligned), k_encode_seq copies it into the stream.  One slot per scan block,
+// [n][max_scan_blocks].  (H100, cfg2 and cfg4 q90: DESIGN §3 has the bits-per-block histogram the width comes from.)
+#ifndef SEQ_SLOT_BITS
+#define SEQ_SLOT_BITS 128
+#endif
+#define SEQ_SLOT_WORDS (SEQ_SLOT_BITS / 32)
+#if SEQ_SLOT_BITS == 128
+typedef uint4 SeqSlot;
+#elif SEQ_SLOT_BITS == 64
+typedef uint2 SeqSlot;
+#else
+#error "SEQ_SLOT_BITS is 64 or 128"
+#endif
 // sym / dcq (here and in launch_encode): the symbol records and dense DC values of sequential scans after the trellis, or nullptr
+// slot (here and in launch_encode): the code slots of a sequential scan, or nullptr: every block is walked again by the
+// packer; not used by progressive scans
 void launch_block_bits(const Geom &g, const ScanDesc &sd, const DcRec *nz_rec, const uint8_t *sym, const int16_t *dcq, const RecLayout &rl, const DevHuff *tabs, size_t tabs_image_stride, int progressive,
-                       uint32_t *blk_bits, uint32_t *tile_bits, const uint32_t *blk_aux, const uint32_t *run_e, const unsigned long long *pm, uint32_t *status, int n, cudaStream_t s);
+                       uint32_t *blk_bits, uint32_t *tile_bits, SeqSlot *slot, const uint32_t *blk_aux, const uint32_t *run_e, const unsigned long long *pm, uint32_t *status, int n, cudaStream_t s);
 // tile_base[img][tile] / seg_corr[img][segment] / total_bits[img] from the tile sums (and the restart interval)
 void launch_scan_layout(const ScanDesc &sd, const uint32_t *blk_bits, const uint32_t *tile_bits, unsigned long long *tile_base,
                         uint32_t *seg_corr, long long seg_stride, unsigned long long *total_bits, size_t capacity_bits,
@@ -213,7 +229,7 @@ void launch_zero_stream(uint32_t *bitbuf, size_t bitbuf_image_stride_words, cons
 // mark: bitmap over the unstuffed bytes of each image (restart markers' 0xFF), only touched when sd.ri != 0
 // nz_rec: the side records holding every block's final non-zero positions (trellis on, sequential scans), or nullptr
 void launch_encode(const Geom &g, const ScanDesc &sd, const DcRec *nz_rec, const uint8_t *sym, const int16_t *dcq, const RecLayout &rl, const DevHuff *tabs, size_t tabs_image_stride, int progressive,
-                   const uint32_t *blk_bits, const uint32_t *tile_bits, const unsigned long long *tile_base, const uint32_t *seg_corr, long long seg_stride,
+                   const uint32_t *blk_bits, const uint32_t *tile_bits, const SeqSlot *slot, const unsigned long long *tile_base, const uint32_t *seg_corr, long long seg_stride,
                    const uint32_t *blk_aux, const uint32_t *run_e, const unsigned long long *pm,
                    uint32_t *bitbuf, size_t bitbuf_image_stride_words, uint32_t *mark, size_t mark_stride_words, const uint32_t *status, int n, cudaStream_t s);
 // byte stuffing of every scan in one pass with a decoupled look-back (k_stuff): out[img][out_start[img] ...], scan_size,
