@@ -454,8 +454,6 @@ static size_t smooth_plane_bytes(const Geom &g)
   return t;
 }
 
-// Sequential scans behind the default trellis (one round over 1..63 by k_trellis_ac3): the entropy stages read the symbol
-// records the trellis back-track leaves instead of the coefficient planes.  B200JPEG_SYMREC=0 keeps them on the planes.
 // code slots for the sequential scans (k_block_bits_seq / k_encode_seq): not at 12 bits, where most blocks are longer
 // than a slot, so that packing them from slots saves nothing and filling the slots costs the bit-count pass (DESIGN §5)
 static bool use_slots(const Plan &pl, const b200jpeg_params *p)
@@ -463,11 +461,12 @@ static bool use_slots(const Plan &pl, const b200jpeg_params *p)
   return !pl.progressive && !pl.lossless && p->data_precision == 8;
 }
 
+// Sequential scans behind the default trellis (one round over 1..63 by k_trellis_ac3): the entropy stages read the symbol
+// records the trellis back-track leaves instead of the coefficient planes.
 static bool use_symrec(const Plan &pl, const b200jpeg_params *p)
 {
-  static const bool off = getenv("B200JPEG_SYMREC") && getenv("B200JPEG_SYMREC")[0] == '0';
   const bool generic_rounds = p->use_scans_in_trellis || p->trellis_num_loops > 1 || p->trellis_q_opt || p->trellis_eob_opt;
-  return !off && pl.trellis && !pl.progressive && !generic_rounds;
+  return pl.trellis && !pl.progressive && !generic_rounds;
 }
 
 // Buffers and constants of one batch of n_total images processed in chunks of `chunk`.
@@ -654,7 +653,7 @@ static int run_pipeline(b200jpeg_encoder *e, const ChunkIO &io, Timer &tm)
   // ---- pass 0 data path: colour/downsample/FDCT/quantize (compress_first_pass) ----
   RecLayout rl; memset(&rl, 0, sizeof rl);
   for (int ci = 0; ci < g.nc; ci++) { rl.comp_off[ci] = rl.per_image; rl.per_image += (long long)g.c[ci].wib * g.c[ci].hib; }
-  rl.sym_hi = (long long)n * rl.per_image * (SYMREC_BYTES / 2);      // second plane of the symbol records (SYMREC_SPLIT)
+  rl.sym_hi = (long long)n * rl.per_image * (SYMREC_BYTES / 2);      // second plane of the symbol records (kernels.cuh)
   tm.mark("forward");
   // the fast quantizer / DC-trellis forms serve a launch only if every table set allows them for the launch's components
   int qfast = 1;
@@ -865,7 +864,7 @@ static int run_pipeline(b200jpeg_encoder *e, const ChunkIO &io, Timer &tm)
         if (!symstats) CU(cudaMemsetAsync(A.d_hist.p, 0, hist_bytes, s));
         if (pl.progressive) launch_gather_prog(g, sd, aux, run_e, pm, A.d_hist.as<uint32_t>(), status, n, s);
         else if (symstats) launch_gather_seq_dc(g, sd, dcq, rl, A.d_hist.as<uint32_t>(), status, n, s);      // the AC counts are there already
-        else launch_gather_seq(g, sd, nz_rec, sym, dcq, rl, A.d_hist.as<uint32_t>(), status, n, s);
+        else launch_gather_seq(g, sd, sym, dcq, rl, A.d_hist.as<uint32_t>(), status, n, s);
         tm.mark("scan_tables");
         SlotMasks masks; memset(&masks, 0, sizeof masks); masks.period = 1; masks.m[0] = scan_slot_mask(pl, sd);
         launch_gen_tables(A.d_hist.as<uint32_t>(), tset, tstride, masks, n, s);
@@ -874,7 +873,8 @@ static int run_pipeline(b200jpeg_encoder *e, const ChunkIO &io, Timer &tm)
     } else { tabs = e->d_tabs_fixed.as<DevHuff>(); tstride = 0; }
     const size_t mark_words = (e->bitbuf_words_per_image * 4 / 8 + 64) / 4;
     tm.mark("block_bits");
-    launch_block_bits(g, sd, nz_rec, sym, dcq, rl, tabs, tstride, pl.progressive, A.d_blk_bits.as<uint32_t>(), A.d_tile_bits.as<uint32_t>(), slot, aux, run_e, pm, status, n, s);
+    if (pl.progressive) launch_block_bits_prog(g, sd, tabs, tstride, aux, run_e, pm, A.d_blk_bits.as<uint32_t>(), A.d_tile_bits.as<uint32_t>(), status, n, s);
+    else launch_block_bits_seq(g, sd, sym, dcq, rl, tabs, tstride, A.d_blk_bits.as<uint32_t>(), A.d_tile_bits.as<uint32_t>(), slot, status, n, s);
     tm.mark("scan_layout");
     launch_scan_layout(sd, A.d_blk_bits.as<uint32_t>(), A.d_tile_bits.as<uint32_t>(), A.d_tile_base.as<unsigned long long>(),
                        A.d_seg_corr.as<uint32_t>(), pl.max_scan_blocks, A.d_total_bits.as<unsigned long long>(),
@@ -882,9 +882,12 @@ static int run_pipeline(b200jpeg_encoder *e, const ChunkIO &io, Timer &tm)
     tm.mark("encode");
     launch_zero_stream(A.d_bitbuf.as<uint32_t>(), e->bitbuf_words_per_image, A.d_total_bits.as<unsigned long long>(), n, s);
     if (sd.ri) CU(cudaMemsetAsync(A.d_mark.p, 0, mark_words * 4 * n, s));
-    launch_encode(g, sd, nz_rec, sym, dcq, rl, tabs, tstride, pl.progressive, A.d_blk_bits.as<uint32_t>(), A.d_tile_bits.as<uint32_t>(), slot, A.d_tile_base.as<unsigned long long>(),
-                  A.d_seg_corr.as<uint32_t>(), pl.max_scan_blocks, aux, run_e, pm,
-                  A.d_bitbuf.as<uint32_t>(), e->bitbuf_words_per_image, A.d_mark.as<uint32_t>(), mark_words, status, n, s);
+    if (pl.progressive)
+      launch_encode_prog(g, sd, tabs, tstride, aux, run_e, pm, A.d_blk_bits.as<uint32_t>(), A.d_tile_bits.as<uint32_t>(), A.d_tile_base.as<unsigned long long>(),
+                         A.d_seg_corr.as<uint32_t>(), pl.max_scan_blocks, A.d_bitbuf.as<uint32_t>(), e->bitbuf_words_per_image, A.d_mark.as<uint32_t>(), mark_words, status, n, s);
+    else
+      launch_encode_seq(g, sd, nz_rec, sym, dcq, rl, tabs, tstride, A.d_blk_bits.as<uint32_t>(), A.d_tile_bits.as<uint32_t>(), slot, A.d_tile_base.as<unsigned long long>(),
+                        A.d_seg_corr.as<uint32_t>(), pl.max_scan_blocks, A.d_bitbuf.as<uint32_t>(), e->bitbuf_words_per_image, A.d_mark.as<uint32_t>(), mark_words, status, n, s);
     tm.mark("stuff");
     CU(cudaMemsetAsync(A.d_stuff_lb.p, 0, stuff_lookback_bytes(e->bitbuf_words_per_image, n), s));
     launch_stuff(A.d_bitbuf.as<uint32_t>(), e->bitbuf_words_per_image, A.d_total_bits.as<unsigned long long>(), A.d_stuff_lb.p,

@@ -27,9 +27,6 @@ __constant__ uint8_t c_izz[64] = {
 // the same table by column: byte r of c_izz_col[j] = zigzag position of natural index 8r + j (one 8-byte load per lane
 // instead of eight byte loads at lane-dependent constant addresses, which the constant cache serialises)
 __constant__ unsigned long long c_izz_col[8] = {0x2315140a09030200ull, 0x242216130b080401ull, 0x30252117120c0705ull, 0x312f262018110d06ull, 0x39322e271f19100eull, 0x3a38332d281e1a0full, 0x3e3b37342c291d1bull, 0x3f3d3c36352b2a1cull};
-#ifndef FWD_KZ_PACKED
-#define FWD_KZ_PACKED 1
-#endif
 #define ZZ_LIST \
   X(0,0) X(1,1) X(2,8) X(3,16) X(4,9) X(5,2) X(6,3) X(7,10) X(8,17) X(9,24) X(10,32) X(11,25) X(12,18) X(13,11) X(14,4) X(15,5) \
   X(16,12) X(17,19) X(18,26) X(19,33) X(20,40) X(21,48) X(22,41) X(23,34) X(24,27) X(25,20) X(26,13) X(27,6) X(28,7) X(29,14) X(30,21) X(31,28) \
@@ -485,9 +482,6 @@ __device__ __forceinline__ int quant_fast(int x, uint2 k, int L, int dering)
 
 
 // DCTM: 0 = JDCT_ISLOW, 1 = JDCT_IFAST, 2 = JDCT_FLOAT (1 and 2: 8-bit only in this kernel; 12-bit: k_forward)
-#ifndef FWD_MASK_SQ
-#define FWD_MASK_SQ 1
-#endif
 #ifndef FWD_MIN_CTAS
 #define FWD_MIN_CTAS 6
 #endif
@@ -775,13 +769,7 @@ __global__ void __launch_bounds__(128, FWD_MIN_CTAS) k_forward_tile(Geom g, cons
   // zigzag positions of this lane's 8 coefficients (natural index 8r + jc)
   int kz[8];
 #pragma unroll
-  for (int r = 0; r < 8; r++) {
-#if FWD_KZ_PACKED
-    kz[r] = (int)((c_izz_col[jc] >> (8 * r)) & 63);
-#else
-    kz[r] = c_izz[8 * r + jc];
-#endif
-  }
+  for (int r = 0; r < 8; r++) kz[r] = (int)((c_izz_col[jc] >> (8 * r)) & 63);
 #pragma unroll 1
   for (int b = tid >> 3; b < NB; b += 16) {
     const wtype *w = sW + b * 72 + jc;
@@ -846,9 +834,9 @@ __global__ void __launch_bounds__(128, FWD_MIN_CTAS) k_forward_tile(Geom g, cons
       sR[b * 64 + k] = (int16_t)dd[r];
       // the trellis derives its entries from the RAW coefficient (qval = (|x| + q/2) / q, jcdctmgr.c:1136); with the
       // integer DCT that is the plain-quantized value, with the float DCT it can differ from quantize_float's result
-      if (!(FWD_MASK_SQ && DCTM == 0)) {
+      if (DCTM != 0) {
         bool nzv = qv != 0;
-        if (DCTM != 0 && rec) { const int dq = (int)qt->q[g.c[ci].qt][nat].d; nzv = abs(dd[r]) >= dq - dq / 2; }
+        if (rec) { const int dq = (int)qt->q[g.c[ci].qt][nat].d; nzv = abs(dd[r]) >= dq - dq / 2; }
         if (nzv && nat != 0) { if (k < 32) mlo |= 1u << k; else mhi |= 1u << (k - 32); }
       }
     }
@@ -860,7 +848,7 @@ __global__ void __launch_bounds__(128, FWD_MIN_CTAS) k_forward_tile(Geom g, cons
       int16_t *ww = blk16 + jc;
 #pragma unroll
       for (int r = 0; r < 8; r++) ww[8 * r] = (int16_t)dd[r];
-      if (FWD_MASK_SQ && DCTM == 0) {
+      if (DCTM == 0) {
         // integer DCT: the mask is "which of the block's 64 staged (zigzag-ordered) values are non-zero"; lane j tests
         // the 8 values at positions 8j..8j+7 (two per 32-bit word) and stores its byte of the 64-bit mask
         __syncwarp();
@@ -876,10 +864,10 @@ __global__ void __launch_bounds__(128, FWD_MIN_CTAS) k_forward_tile(Geom g, cons
         if (j == 0) m8 &= ~1u;                                   // position 0 is the DC value
         reinterpret_cast<uint8_t *>(&sMask[b])[j] = (uint8_t)m8;
       } else {
-      mlo |= __shfl_xor_sync(0xffffffffu, mlo, 1); mhi |= __shfl_xor_sync(0xffffffffu, mhi, 1);
-      mlo |= __shfl_xor_sync(0xffffffffu, mlo, 2); mhi |= __shfl_xor_sync(0xffffffffu, mhi, 2);
-      mlo |= __shfl_xor_sync(0xffffffffu, mlo, 4); mhi |= __shfl_xor_sync(0xffffffffu, mhi, 4);
-      if (j == 0) sMask[b] = make_uint2(mlo, mhi);
+        mlo |= __shfl_xor_sync(0xffffffffu, mlo, 1); mhi |= __shfl_xor_sync(0xffffffffu, mhi, 1);
+        mlo |= __shfl_xor_sync(0xffffffffu, mlo, 2); mhi |= __shfl_xor_sync(0xffffffffu, mhi, 2);
+        mlo |= __shfl_xor_sync(0xffffffffu, mlo, 4); mhi |= __shfl_xor_sync(0xffffffffu, mhi, 4);
+        if (j == 0) sMask[b] = make_uint2(mlo, mhi);
       }
     }
   }
@@ -928,7 +916,7 @@ __global__ void __launch_bounds__(128, FWD_MIN_CTAS) k_forward_tile(Geom g, cons
         const int16_t *q = sQ + b * 64;
         fs.dcq[ridx] = q[0];
         unsigned long long m;
-        if (FWD_MASK_SQ && DCTM == 0) m = rr.nzmask;
+        if (DCTM == 0) m = rr.nzmask;
         else {
           m = 0;
 #pragma unroll
@@ -1028,10 +1016,9 @@ static EncodeTiledFn tensor_map_encoder()
 // which the kernel addresses as image 0.
 static int make_pixel_tensor_map(const Geom &g, const uint8_t *src, int n, int ic, int tile_rows, CUtensorMap *tm)
 {
-  static const bool off = getenv("B200JPEG_NO_TMA") != nullptr;     // A/B aid
   memset(tm, 0, sizeof *tm);
   EncodeTiledFn enc = tensor_map_encoder();
-  if (off || !enc || g.raw_in || !src || g.in_comps != ic || g.px_swap || g.px_first || g.max_coef_bits != 10) return 0;
+  if (!enc || g.raw_in || !src || g.in_comps != ic || g.px_swap || g.px_first || g.max_coef_bits != 10) return 0;
   if (g.image_stride == 0) n = 1;
   if (((size_t)src & 15) || (g.row_pitch & 15) || (n > 1 && (g.image_stride & 15))) return 0;
   const cuuint64_t dims[3] = {(cuuint64_t)g.W * ic, (cuuint64_t)g.H, (cuuint64_t)n};
@@ -1236,9 +1223,8 @@ bool forward_tiled(const Geom &g, int dct_method)
 {
   const bool ycc = g.nc == 3 && (g.raw_in || (g.cs_mode == 0 && (g.in_comps == 3 || g.in_comps == 4))) && g.c[0].h == g.hmax && g.c[0].v == g.vmax &&
                    g.c[1].h == 1 && g.c[1].v == 1 && g.c[2].h == 1 && g.c[2].v == 1 && g.hmax <= 2 && g.vmax <= 2;
-  static const bool force_generic = getenv("B200JPEG_GENERIC_FORWARD") != nullptr;   // A/B switch for debugging
   // (12-bit samples with the fast / float DCT: the one-thread-per-block kernel only)
-  return !force_generic && ((forward_gray(g) && g.hmax == 1 && g.vmax == 1) || ycc) && !(g.max_coef_bits == 14 && dct_method != 0);
+  return ((forward_gray(g) && g.hmax == 1 && g.vmax == 1) || ycc) && !(g.max_coef_bits == 14 && dct_method != 0);
 }
 void launch_forward(const Geom &g, const uint8_t *src, const QuantTables *qt, int qfast, int dct_method, int dering, DcRec *rec, const RecLayout &rl, int keep_raw,
                     const FwdStats &fs, int n, cudaStream_t s)
@@ -1366,8 +1352,6 @@ void launch_dummy(const Geom &g, int n, cudaStream_t s)
 // =====================================================================
 // scan-order block addressing (compress_output, jccoefct.c:498-553)
 // =====================================================================
-struct BlockRef { const int16_t *blk; int sci; int mcu; int k; };
-
 __device__ __forceinline__ const int16_t *block_ptr(const Geom &g, const ScanDesc &sd, int img, long long t, int &sci, long long &mcu, int &k)
 {
   mcu = t / sd.bim; k = (int)(t - mcu * sd.bim);
@@ -1393,14 +1377,14 @@ __device__ __forceinline__ int prev_dc(const Geom &g, const ScanDesc &sd, int im
 // Walks one block the way encode_one_block (jchuff.c:563-661) / htest_one_block
 // (jchuff.c:812-878) do, calling sink.dc(nbits, valuebits) and
 // sink.ac(symbol, nbits, valuebits) in stream order.
-// ld(v): the block's v-th group of 8 zigzag-ordered coefficients (16 bytes)
-template <class Sink, class Load>
-__device__ __forceinline__ void walk_seq_chunks(Load ld, int last_dc, Sink &sink)
+template <class Sink>
+__device__ __forceinline__ void walk_seq_block(const int16_t *__restrict__ blk, int last_dc, Sink &sink)
 {
+  const uint4 *b4 = reinterpret_cast<const uint4 *>(blk);
   int r = 0;
 #pragma unroll
   for (int v = 0; v < 8; v++) {
-    uint4 q = ld(v);
+    uint4 q = b4[v];
     unsigned w[4] = {q.x, q.y, q.z, q.w};
 #pragma unroll
     for (int j = 0; j < 8; j++) {
@@ -1424,21 +1408,7 @@ __device__ __forceinline__ void walk_seq_chunks(Load ld, int last_dc, Sink &sink
   }
   if (r > 0) sink.ac(0, 0, 0);
 }
-template <class Sink>
-__device__ __forceinline__ void walk_seq_block(const int16_t *__restrict__ blk, int last_dc, Sink &sink)
-{
-  const uint4 *b4 = reinterpret_cast<const uint4 *>(blk);
-  walk_seq_chunks([&](int v) { return b4[v]; }, last_dc, sink);
-}
 
-#ifndef SEQ_SPARSE_ENC
-#define SEQ_SPARSE_ENC 1
-#endif
-// the same sparse walk in the statistics and bit-count kernels: measured slower than the dense 16-byte loads there
-// (0.61 / 0.62 vs 0.53 / 0.57 ms per 64 4K images), so off
-#ifndef SEQ_SPARSE_STATS
-#define SEQ_SPARSE_STATS 0
-#endif
 // Zigzag positions of a scan-order block's non-zero AC coefficients, from the side records (the AC trellis leaves the
 // final ones there); dummy blocks have none.
 __device__ __forceinline__ unsigned long long block_nzmask(const Geom &g, const ScanDesc &sd, const DcRec *__restrict__ rec, const RecLayout &rl,
@@ -1451,7 +1421,9 @@ __device__ __forceinline__ unsigned long long block_nzmask(const Geom &g, const 
   const long long row = mrow * mh + sd.k_y[k]; const int col = mcol * mw + sd.k_x[k];
   return (row < c.hib && col < c.wib) ? rec[(size_t)img * rl.per_image + rl.comp_off[ci] + (size_t)row * c.wib + col].nzmask : 0ull;
 }
-// walk_seq_block for a block whose non-zero positions are known: touches only those coefficients
+// walk_seq_block for a block whose non-zero positions are known: touches only those coefficients.  Used by the packer
+// only: in the statistics and bit-count kernels it measured slower than the dense 16-byte loads (0.61 / 0.62 vs 0.53 /
+// 0.57 ms per 64 4K images)
 template <class Sink>
 __device__ __forceinline__ void walk_seq_sparse(const int16_t *__restrict__ blk, unsigned long long mask, int last_dc, Sink &sink)
 {
@@ -1545,13 +1517,8 @@ __device__ __forceinline__ void walk_seq_rec(const Geom &g, const ScanDesc &sd, 
   const int16_t *dimg = dcq + (size_t)img * rl.per_image;
   const bool real = row < c.hib && col < c.wib;
   const size_t ridx = (size_t)img * rl.per_image + rl.comp_off[ci] + (real ? (size_t)row * c.wib + col : (size_t)0);
-#if SYMREC_SPLIT
   const uint4 *r4 = reinterpret_cast<const uint4 *>(sym + ridx * (SYMREC_BYTES / 2));
   const uint4 *r4hi = reinterpret_cast<const uint4 *>(sym + (size_t)rl.sym_hi + ridx * (SYMREC_BYTES / 2)) - 4;      // words 16..31 = pieces 4..7
-#else
-  const uint4 *r4 = reinterpret_cast<const uint4 *>(sym + ridx * SYMREC_BYTES);
-  const uint4 *r4hi = r4;
-#endif
   uint4 q0 = make_uint4(1u, 0u, 0u, 0u);                       // a dummy block: one entry, EOB
   if (real) q0 = r4[0];
   emit_dc(dense_dc(c, dimg + rl.comp_off[ci], row, col), prev_dc_dense(g, sd, dimg, rl, sp), sink);
@@ -1588,17 +1555,9 @@ __device__ __forceinline__ void walk_seq_rec(const Geom &g, const ScanDesc &sd, 
 // ---------------------------------------------------------------------
 // statistics pass (encode_mcu_gather, jchuff.c:886-915)
 // ---------------------------------------------------------------------
-// shared-memory histogram increment (warp-aggregating the atomics per counter was measured slower).  A few symbols
-// (EOB, 0x01, 0x11, 0x02) make up most of a scan, so the lanes of a warp mostly hit the same few counters; keeping
-// GATHER_COPIES copies of the histograms per CTA (a thread uses copy lane mod copies) is a build-time option; the
-// per-scan kernels' copies are 8 KB each, so more copies cost occupancy there.  Default 1 (not re-measured on H100).
-#ifndef GATHER_COPIES
-#define GATHER_COPIES 1
-#endif
-#ifndef GATHER_COPIES_SCAN
-#define GATHER_COPIES_SCAN 1
-#endif
-// blocks per CTA = GATHER_TILES * 256: zeroing and flushing the copies is paid once per CTA
+// shared-memory histogram increment (warp-aggregating the atomics per counter was measured slower).  One histogram copy
+// per CTA: the per-scan kernels' histograms are 8 KB each, so more copies would cost occupancy there.
+// blocks per CTA = GATHER_TILES * 256: zeroing and flushing the histograms is paid once per CTA
 #ifndef GATHER_TILES
 #define GATHER_TILES 4
 #endif
@@ -1612,23 +1571,20 @@ struct HistSink {
   __device__ void ac(int sym, int nb, int) { if (nb > maxbits) bad = 1; hist_inc(&ac_hist[sym]); }
 };
 
-// nz_rec: the side records holding every block's final non-zero positions (after the AC trellis), or nullptr: the walk
-// then touches only those coefficients (and the 32-byte sectors they sit in) instead of the whole 128-byte block
-__global__ void __launch_bounds__(256) k_gather_seq(Geom g, ScanDesc sd, const DcRec *__restrict__ nz_rec, const uint8_t *__restrict__ sym, const int16_t *__restrict__ dcq,
+__global__ void __launch_bounds__(256) k_gather_seq(Geom g, ScanDesc sd, const uint8_t *__restrict__ sym, const int16_t *__restrict__ dcq,
                                                     RecLayout rl, uint32_t *__restrict__ hist, uint32_t *__restrict__ status)
 {
-  __shared__ unsigned sh[GATHER_COPIES_SCAN][HIST_SLOTS * HIST_BINS];
+  __shared__ unsigned sh[HIST_SLOTS * HIST_BINS];
   int img = blockIdx.y;
-  for (int i = threadIdx.x; i < GATHER_COPIES_SCAN * HIST_SLOTS * HIST_BINS; i += blockDim.x) (&sh[0][0])[i] = 0;
+  for (int i = threadIdx.x; i < HIST_SLOTS * HIST_BINS; i += blockDim.x) sh[i] = 0;
   __syncthreads();
 #pragma unroll 1
   for (int tile = 0; tile < GATHER_TILES; tile++) {
     long long t = ((long long)blockIdx.x * GATHER_TILES + tile) * blockDim.x + threadIdx.x;
     if (t >= sd.nblocks) break;
-    unsigned *mine = sh[threadIdx.x % GATHER_COPIES_SCAN];
     if (sym) {                                         // symbol records (a scan script with several sequential scans: per-scan counts)
       const CompGeom &c = g.c[sd.ci[sd.k_comp[(int)(t % sd.bim)]]];
-      HistSink sink{mine + c.dc_tbl * HIST_BINS, mine + (4 + c.ac_tbl) * HIST_BINS, 0, g.max_coef_bits};
+      HistSink sink{sh + c.dc_tbl * HIST_BINS, sh + (4 + c.ac_tbl) * HIST_BINS, 0, g.max_coef_bits};
       walk_seq_rec(g, sd, sym, dcq, rl, img, t, sink);
       if (sink.bad) atomicOr(&status[img], 2u);
       continue;
@@ -1637,57 +1593,34 @@ __global__ void __launch_bounds__(256) k_gather_seq(Geom g, ScanDesc sd, const D
     const int16_t *blk = block_ptr(g, sd, img, t, sci, mcu, k);
     int last = prev_dc(g, sd, img, t, sci, mcu, k);
     const CompGeom &c = g.c[sd.ci[sci]];
-    HistSink sink{mine + c.dc_tbl * HIST_BINS, mine + (4 + c.ac_tbl) * HIST_BINS, 0, g.max_coef_bits};
-    if (SEQ_SPARSE_STATS && nz_rec) walk_seq_sparse(blk, block_nzmask(g, sd, nz_rec, rl, img, sci, mcu, k), last, sink);
-    else walk_seq_block(blk, last, sink);
+    HistSink sink{sh + c.dc_tbl * HIST_BINS, sh + (4 + c.ac_tbl) * HIST_BINS, 0, g.max_coef_bits};
+    walk_seq_block(blk, last, sink);
     if (sink.bad) atomicOr(&status[img], 2u);          // JERR_BAD_DCT_COEF
   }
   __syncthreads();
   uint32_t *gh = hist + (size_t)img * HIST_SLOTS * HIST_BINS;
   for (int i = threadIdx.x; i < HIST_SLOTS * HIST_BINS; i += blockDim.x) {
-    unsigned v = 0;
-#pragma unroll
-    for (int cp = 0; cp < GATHER_COPIES_SCAN; cp++) v += sh[cp][i];
+    const unsigned v = sh[i];
     if (v) atomicAdd(&gh[i], v);
   }
 }
 // Trellis-phase statistics: every component as its own non-interleaved scan
 // (jcmaster.c:443-467), all components of all images in one launch;
 // histogram set index = img*nc + ci.
-// GATHER_STAGE: the CTA's 256 blocks arrive through shared memory -- 16-byte pieces in the order they lie in memory (8
-// consecutive lanes fetch one block's 128 bytes: 4 lines per request instead of 32), stored with the piece index XORed
-// by the block's low bits so that the per-thread read-back of whole blocks is conflict-free.
-#ifndef GATHER_STAGE
-#define GATHER_STAGE 0
-#endif
 __global__ void __launch_bounds__(256) k_gather_comp(Geom g, RestartSpec rs, uint32_t *__restrict__ hist, uint32_t *__restrict__ status)
 {
-  __shared__ unsigned sh[GATHER_COPIES][2 * HIST_BINS];
-  __shared__ __align__(16) uint4 stg[GATHER_STAGE ? 256 * 8 : 1];
+  __shared__ unsigned sh[2 * HIST_BINS];
   const int ci = blockIdx.y % g.nc, img = blockIdx.y / g.nc;
   const CompGeom &c = g.c[ci];
   long long nblk = (long long)c.wib * c.hib;
   if ((long long)blockIdx.x * GATHER_TILES * blockDim.x >= nblk) return;
-  for (int i = threadIdx.x; i < GATHER_COPIES * 2 * HIST_BINS; i += blockDim.x) (&sh[0][0])[i] = 0;
+  for (int i = threadIdx.x; i < 2 * HIST_BINS; i += blockDim.x) sh[i] = 0;
   __syncthreads();
   const int16_t *base = c.coef + (size_t)img * c.blocks_per_image * 64;
 #pragma unroll 1
   for (int tile = 0; tile < GATHER_TILES; tile++) {
     const long long t0 = ((long long)blockIdx.x * GATHER_TILES + tile) * blockDim.x;
     if (t0 >= nblk) break;
-    if (GATHER_STAGE) {
-      if (tile) __syncthreads();                             // the previous tile's blocks have been read
-#pragma unroll
-      for (int i = 0; i < 8; i++) {
-        const int q = i * 256 + threadIdx.x, bq = q >> 3, part = q & 7;
-        const long long tb = t0 + bq;
-        if (tb < nblk) {
-          const int rowb = (int)(tb / c.wib), colb = (int)(tb - (long long)rowb * c.wib);
-          stg[bq * 8 + (part ^ (bq & 7))] = reinterpret_cast<const uint4 *>(base + ((size_t)rowb * c.wpad + colb) * 64)[part];
-        }
-      }
-      __syncthreads();
-    }
     const long long t = t0 + threadIdx.x;
     if (t < nblk) {
       int row = (int)(t / c.wib), col = (int)(t - (long long)row * c.wib);
@@ -1695,19 +1628,15 @@ __global__ void __launch_bounds__(256) k_gather_comp(Geom g, RestartSpec rs, uin
       int last = 0;
       const long long ri = rs.in_rows > 0 ? min((long long)rs.in_rows * c.wib, 65535LL) : rs.interval;      // per_scan_setup, jcmaster.c:594-599
       if (t > 0 && !(ri && t % ri == 0)) { int pr = col > 0 ? row : row - 1, pc = col > 0 ? col - 1 : c.wib - 1; last = base[((size_t)pr * c.wpad + pc) * 64]; }
-      unsigned *mine = sh[threadIdx.x % GATHER_COPIES];
-      HistSink sink{mine, mine + HIST_BINS, 0, g.max_coef_bits};
-      if (GATHER_STAGE) { const uint4 *mb = stg + threadIdx.x * 8; const int sw = threadIdx.x & 7; walk_seq_chunks([&](int v) { return mb[v ^ sw]; }, last, sink); }
-      else walk_seq_block(blk, last, sink);
+      HistSink sink{sh, sh + HIST_BINS, 0, g.max_coef_bits};
+      walk_seq_block(blk, last, sink);
       if (sink.bad) atomicOr(&status[img], 2u);
     }
   }
   __syncthreads();
   uint32_t *gh = hist + ((size_t)img * g.nc + ci) * HIST_SLOTS * HIST_BINS;
   for (int i = threadIdx.x; i < HIST_BINS; i += blockDim.x) {
-    unsigned d = 0, a = 0;
-#pragma unroll
-    for (int cp = 0; cp < GATHER_COPIES; cp++) { d += sh[cp][i]; a += sh[cp][HIST_BINS + i]; }
+    const unsigned d = sh[i], a = sh[HIST_BINS + i];
     if (d) atomicAdd(&gh[c.dc_tbl * HIST_BINS + i], d);
     if (a) atomicAdd(&gh[(4 + c.ac_tbl) * HIST_BINS + i], a);
   }
@@ -1760,10 +1689,10 @@ void launch_gather_comp_dc(const Geom &g, const RestartSpec &rs, const int16_t *
   LAUNCHED();
 }
 
-void launch_gather_seq(const Geom &g, const ScanDesc &sd, const DcRec *nz_rec, const uint8_t *sym, const int16_t *dcq, const RecLayout &rl, uint32_t *hist, uint32_t *status, int n, cudaStream_t s)
+void launch_gather_seq(const Geom &g, const ScanDesc &sd, const uint8_t *sym, const int16_t *dcq, const RecLayout &rl, uint32_t *hist, uint32_t *status, int n, cudaStream_t s)
 {
   dim3 grid((unsigned)((sd.nblocks + 256 * GATHER_TILES - 1) / (256 * GATHER_TILES)), n);
-  k_gather_seq<<<grid, 256, 0, s>>>(g, sd, nz_rec, sym, dcq, rl, hist, status);
+  k_gather_seq<<<grid, 256, 0, s>>>(g, sd, sym, dcq, rl, hist, status);
   LAUNCHED();
 }
 
@@ -2297,10 +2226,6 @@ __device__ __forceinline__ float u2f_exact(unsigned v) { return __uint_as_float(
 //    5-8 thousand and stalled on instruction fetch), registers ~50, shared memory 12 bytes per list slot and thread.
 // =====================================================================
 #define T3_THREADS 128
-#ifndef SYMREC_DIRECT
-#define SYMREC_DIRECT 0
-#endif
-static_assert(!(SYMREC_DIRECT && SYMREC_SPLIT), "the direct-store A/B aid writes whole 128-byte slots");
 // resident CTAs per SM the compiler must allow for the <= 8 entries class, and for the 9..15 entries class.  H100, cfg2:
 // 6 (80 registers, no spills) ran the AC stage in 9.84-9.87 ms against 10.06-10.13 at 8 (64 registers, 18 / 20 bytes of
 // spill stores / loads); an earlier GPU measured 12 slower than 8
@@ -2558,8 +2483,7 @@ k_trellis_ac3(Geom g, const TrellisConsts *__restrict__ tc, const DevHuff *__res
         return fm;
       };
       if (!so.sym) {
-        const unsigned long long fm = write_block(last);
-        if (SEQ_SPARSE_ENC) rec[rbase + lin].nzmask = fm;
+        rec[rbase + lin].nzmask = write_block(last);
       } else {
         // sequential scans follow: the back-track leaves the block's AC symbols as a record (header word: number of
         // entries, bit 7 = more than SYMREC_SLOTS; entry = symbol | value bits << 16, LAST symbol of the stream first --
@@ -2569,12 +2493,7 @@ k_trellis_ac3(Geom g, const TrellisConsts *__restrict__ tc, const DevHuff *__res
         // entropy stages when the record overflowed.
         unsigned *scr = reinterpret_cast<unsigned *>(myrec);
         int ns = 0;
-#if SYMREC_DIRECT
-        unsigned *gout = reinterpret_cast<unsigned *>(so.sym + (rbase + lin) * SYMREC_BYTES);      // A/B: entries straight to global memory
-        auto put_sym = [&](unsigned e) { if (ns < SYMREC_SLOTS) gout[ns + 1] = e; ns++; };
-#else
         auto put_sym = [&](unsigned e) { if (ns < SYMREC_SLOTS) scr[((ns + 1) >> 1) * (T3_THREADS * 2) + ((ns + 1) & 1)] = e; ns++; };
-#endif
         const int last0 = last;
         unsigned w = last ? myew[(last - 1) * T3_THREADS] : 0u;
         if (last == 0 || (w & 0xFCu) != (63u << 2)) { put_sym(0u); if (so.hist) atomicAdd(&shist[160], 1u); }      // EOB
@@ -2590,18 +2509,11 @@ k_trellis_ac3(Geom g, const TrellisConsts *__restrict__ tc, const DevHuff *__res
           if (so.hist) { atomicAdd(&shist[(run & 15) * 10 + nb - 1], 1u); if (run >> 4) atomicAdd(&shist[161], (unsigned)(run >> 4)); }
           last = pr; w = wn;
         }
-#if SYMREC_DIRECT
-        gout[0] = ns > SYMREC_SLOTS ? 0x80u : (unsigned)ns; (void)scr;
-#else
         scr[0] = ns > SYMREC_SLOTS ? 0x80u : (unsigned)ns;
         // whole 32-byte sectors leave (the words past the last entry are whatever the list held)
         const int nw = 1 + min(ns, SYMREC_SLOTS);
-#if SYMREC_SPLIT
         uint4 *dlo = reinterpret_cast<uint4 *>(so.sym + (rbase + lin) * (SYMREC_BYTES / 2));
         uint4 *dhi = reinterpret_cast<uint4 *>(so.sym + (size_t)rl.sym_hi + (rbase + lin) * (SYMREC_BYTES / 2)) - 4;
-#else
-        uint4 *dlo = reinterpret_cast<uint4 *>(so.sym + (rbase + lin) * SYMREC_BYTES), *dhi = dlo;
-#endif
         for (int v = 0; 4 * v < nw; v += 2) {
           const uint2 a = myrec[(2 * v) * T3_THREADS], b = myrec[(2 * v + 1) * T3_THREADS];
           const uint2 c2 = myrec[(2 * v + 2) * T3_THREADS], d2 = myrec[(2 * v + 3) * T3_THREADS];
@@ -2609,7 +2521,6 @@ k_trellis_ac3(Geom g, const TrellisConsts *__restrict__ tc, const DevHuff *__res
           dst[v] = make_uint4(a.x, a.y, b.x, b.y);
           dst[v + 1] = make_uint4(c2.x, c2.y, d2.x, d2.y);
         }
-#endif
         if (so.dcq_ac) so.dcq[rbase + lin] = (int16_t)dc_q;          // no DC trellis behind this kernel: the plain-quantized DC is final
         if (so.keep_coef || ns > SYMREC_SLOTS) write_block(last0);
       }
@@ -2949,8 +2860,8 @@ struct CountSink {
   __device__ void ac(int sym, int nb, int) { int s = asz[sym]; if (!s) bad = 1; bits += s + nb; }
 };
 
-// CountSink of the sequential scans, which also keeps the block's last SEQ_SLOT_BITS bits: code and value bits in
-// stream order, right-aligned in a[] (a[0] most significant).  Only a block of at most SEQ_SLOT_BITS bits stores them;
+// CountSink of the sequential scans, which also keeps the block's last 128 bits: code and value bits in stream
+// order, right-aligned in a[] (a[0] most significant).  Only a block of at most 128 bits stores them;
 // the packer walks a longer one again.
 struct SlotSink {
   const uint16_t *dco, *aco; const uint8_t *dsz, *asz; unsigned bits; int bad;
@@ -2963,32 +2874,15 @@ struct SlotSink {
   }
   __device__ void dc(int nb, int v) { const int s = dsz[nb]; if (!s) bad = 1; put((unsigned)dco[nb] << nb | ((unsigned)v & ((1u << nb) - 1u)), s + nb); }
   __device__ void ac(int sym, int nb, int v) { const int s = asz[sym]; if (!s) bad = 1; put((unsigned)aco[sym] << nb | ((unsigned)v & ((1u << nb) - 1u)), s + nb); }
-  // the slot: the bit string left-aligned, first bit = bit 31 of word 0 (bits <= SEQ_SLOT_BITS)
+  // the slot: the bit string left-aligned, first bit = bit 31 of word 0 (bits <= 128)
   __device__ SeqSlot slot() const {
-    const int sh = SEQ_SLOT_BITS - (int)bits;
-#if SEQ_SLOT_BITS > 64
+    const int sh = 128 - (int)bits;
     unsigned long long h = (unsigned long long)a[0] << 32 | a[1], l = (unsigned long long)a[2] << 32 | a[3];
     if (sh >= 64) { h = sh < 128 ? l << (sh - 64) : 0ull; l = 0; }
     else if (sh) { h = (h << sh) | (l >> (64 - sh)); l <<= sh; }
     return make_uint4((unsigned)(h >> 32), (unsigned)h, (unsigned)(l >> 32), (unsigned)l);
-#else
-    unsigned long long l = (unsigned long long)a[0] << 32 | a[1];
-    l = sh < 64 ? l << sh : 0ull;
-    return make_uint2((unsigned)(l >> 32), (unsigned)l);
-#endif
   }
 };
-
-// sum of v over the CTA (256 threads), result valid in thread 0
-__device__ __forceinline__ unsigned cta_sum_256(unsigned v, unsigned *ws /* [8] shared */)
-{
-  for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  if ((threadIdx.x & 31) == 0) ws[threadIdx.x >> 5] = v;
-  __syncthreads();
-  unsigned r = 0;
-  if (threadIdx.x == 0) for (int i = 0; i < 8; i++) r += ws[i];
-  return r;
-}
 
 // exclusive prefix of v inside the CTA (256 threads) and the CTA total (valid in all threads)
 __device__ __forceinline__ unsigned cta_excl_scan_256(unsigned v, unsigned *ws /* [9] shared */, unsigned &total)
@@ -3007,9 +2901,9 @@ __device__ __forceinline__ unsigned cta_excl_scan_256(unsigned v, unsigned *ws /
 
 // One tile = the 256 blocks of one CTA; tile_bits[img][tile] = bits the tile emits; blk_bits[img][t] = bits
 // the tile's blocks before t emit (exclusive prefix inside the tile); slot[img][t] = block t's bit string when it
-// has at most SEQ_SLOT_BITS bits (not written otherwise; SLOTS = false: no slots, the packer walks every block).
+// has at most 128 bits (not written otherwise; SLOTS = false: no slots, the packer walks every block).
 template <bool SLOTS>
-__global__ void __launch_bounds__(256) k_block_bits_seq(Geom g, ScanDesc sd, const DcRec *__restrict__ nz_rec, const uint8_t *__restrict__ sym, const int16_t *__restrict__ dcq,
+__global__ void __launch_bounds__(256) k_block_bits_seq(Geom g, ScanDesc sd, const uint8_t *__restrict__ sym, const int16_t *__restrict__ dcq,
                                                         RecLayout rl, const DevHuff *__restrict__ tabs, size_t stride,
                                                         uint32_t *__restrict__ blk_bits, uint32_t *__restrict__ tile_bits, SeqSlot *__restrict__ slot,
                                                         uint32_t *__restrict__ status)
@@ -3029,7 +2923,6 @@ __global__ void __launch_bounds__(256) k_block_bits_seq(Geom g, ScanDesc sd, con
     const CompGeom &c = g.c[sd.ci[sci]];
     auto walk = [&](auto &sink) {
       if (sym) walk_seq_rec(g, sd, sym, dcq, rl, img, t, sink);
-      else if (SEQ_SPARSE_STATS && nz_rec) walk_seq_sparse(blk, block_nzmask(g, sd, nz_rec, rl, img, sci, mcu, k), last, sink);
       else walk_seq_block(blk, last, sink);
       if (sink.bad) atomicOr(&status[img], 2u);
       bits = sink.bits;
@@ -3037,7 +2930,7 @@ __global__ void __launch_bounds__(256) k_block_bits_seq(Geom g, ScanDesc sd, con
     if constexpr (SLOTS) {
       SlotSink sink{st.code[c.dc_tbl], st.code[4 + c.ac_tbl], st.size[c.dc_tbl], st.size[4 + c.ac_tbl], 0u, 0, {}};
       walk(sink);
-      if (bits <= SEQ_SLOT_BITS) slot[(size_t)img * sd.nblocks + t] = sink.slot();
+      if (bits <= 128) slot[(size_t)img * sd.nblocks + t] = sink.slot();
     } else {
       CountSink sink{st.size[c.dc_tbl], st.size[4 + c.ac_tbl], 0u, 0};
       walk(sink);
@@ -3152,7 +3045,7 @@ __device__ __forceinline__ unsigned slot_window(const uint32_t *__restrict__ s, 
   return __funnelshift_l(b, a, k & 31);
 }
 
-// One CTA per tile of 256 blocks.  A block of at most SEQ_SLOT_BITS bits that does not end a restart segment (a slot
+// One CTA per tile of 256 blocks.  A block of at most 128 bits that does not end a restart segment (a slot
 // block) is copied from the slot k_block_bits_seq stored: output word w is built by the slot block holding bit 32w,
 // from its bits and those of the tile's blocks that follow it inside the word.  A word that lies wholly in the tile's
 // slot blocks is written with a plain store; every other one (the tile's edge words, words shared with a fallback
@@ -3190,7 +3083,7 @@ __global__ void __launch_bounds__(256) k_encode_seq(Geom g, ScanDesc sd, const D
     len = (j + 1 < nt ? pre[t + 1] : tile_bits[(size_t)img * gridDim.x + blockIdx.x]) - p;
     off = tb + p;
     if (sd.ri) off += seg_corr[(size_t)img * seg_stride + t / seglen];
-    fb = !slot || len > SEQ_SLOT_BITS || (sd.ri && (t + 1) % seglen == 0 && t + 1 < sd.nblocks);
+    fb = !slot || len > 128 || (sd.ri && (t + 1) % seglen == 0 && t + 1 < sd.nblocks);
     if (!fb) s_slot[j] = slot[(size_t)img * sd.nblocks + t];
     s_off[j] = (unsigned)(off - base * 32);
     s_fb[j] = fb;
@@ -3237,7 +3130,7 @@ __global__ void __launch_bounds__(256) k_encode_seq(Geom g, ScanDesc sd, const D
       int sci, k; long long mcu;
       const int16_t *blk = block_ptr(g, sd, img, t, sci, mcu, k);
       int last = prev_dc(g, sd, img, t, sci, mcu, k);
-      if (SEQ_SPARSE_ENC && rec) walk_seq_sparse(blk, block_nzmask(g, sd, rec, rl, img, sci, mcu, k), last, sink);
+      if (rec) walk_seq_sparse(blk, block_nzmask(g, sd, rec, rl, img, sci, mcu, k), last, sink);
       else walk_seq_block(blk, last, sink);
     }
     if (sd.ri) emit_restart_marker(sink, sd, t, mark + (size_t)img * mark_stride_words);
@@ -3705,10 +3598,10 @@ struct BitSinkP : BitSink {
 __global__ void __launch_bounds__(256) k_gather_prog(Geom g, ScanDesc sd, const uint32_t *__restrict__ aux, const uint32_t *__restrict__ run_e,
                                                      const unsigned long long *__restrict__ pm, uint32_t *__restrict__ hist, uint32_t *__restrict__ status)
 {
-  __shared__ unsigned sh[GATHER_COPIES_SCAN][HIST_SLOTS * HIST_BINS];
+  __shared__ unsigned sh[HIST_SLOTS * HIST_BINS];
   int img = blockIdx.y;
   const int Al = sd.al_img ? sd.al_img[img] : sd.Al;     // scan search: this scan's Al is the image's best Al so far (jcmaster.c:477-488)
-  for (int i = threadIdx.x; i < GATHER_COPIES_SCAN * HIST_SLOTS * HIST_BINS; i += blockDim.x) (&sh[0][0])[i] = 0;
+  for (int i = threadIdx.x; i < HIST_SLOTS * HIST_BINS; i += blockDim.x) sh[i] = 0;
   __syncthreads();
 #pragma unroll 1
   for (int tile = 0; tile < GATHER_TILES; tile++) {
@@ -3718,8 +3611,7 @@ __global__ void __launch_bounds__(256) k_gather_prog(Geom g, ScanDesc sd, const 
     const int16_t *blk = block_ptr(g, sd, img, t, sci, mcu, k);
     int last = prev_dc_shifted(g, sd, Al, img, t, sci, mcu, k);
     const CompGeom &c = g.c[sd.ci[sci]];
-    unsigned *mine = sh[threadIdx.x % GATHER_COPIES_SCAN];
-    HistSinkP sink{mine + c.dc_tbl * HIST_BINS, mine + (4 + c.ac_tbl) * HIST_BINS, 0, g.max_coef_bits};
+    HistSinkP sink{sh + c.dc_tbl * HIST_BINS, sh + (4 + c.ac_tbl) * HIST_BINS, 0, g.max_coef_bits};
     unsigned a = 0, re = 0; unsigned long long ev = 0, one = 0, bit = 0;
     if (sd.Ss) load_prog_aux(sd, aux, run_e, pm, img, t, a, re, ev, one, bit);
     walk_prog_block(blk, sd, Al, last, a, re, ev, one, bit, sink);
@@ -3728,9 +3620,7 @@ __global__ void __launch_bounds__(256) k_gather_prog(Geom g, ScanDesc sd, const 
   __syncthreads();
   uint32_t *gh = hist + (size_t)img * HIST_SLOTS * HIST_BINS;
   for (int i = threadIdx.x; i < HIST_SLOTS * HIST_BINS; i += blockDim.x) {
-    unsigned v = 0;
-#pragma unroll
-    for (int cp = 0; cp < GATHER_COPIES_SCAN; cp++) v += sh[cp][i];
+    const unsigned v = sh[i];
     if (v) atomicAdd(&gh[i], v);
   }
 }
@@ -3866,13 +3756,19 @@ void launch_gather_prog(const Geom &g, const ScanDesc &sd, const uint32_t *aux, 
   k_gather_prog<<<grid, 256, 0, s>>>(g, sd, aux, run_e, pm, hist, status); LAUNCHED();
 }
 
-void launch_block_bits(const Geom &g, const ScanDesc &sd, const DcRec *nz_rec, const uint8_t *sym, const int16_t *dcq, const RecLayout &rl, const DevHuff *tabs, size_t stride, int progressive,
-                       uint32_t *blk_bits, uint32_t *tile_bits, SeqSlot *slot, const uint32_t *blk_aux, const uint32_t *run_e, const unsigned long long *pm, uint32_t *status, int n, cudaStream_t s)
+void launch_block_bits_seq(const Geom &g, const ScanDesc &sd, const uint8_t *sym, const int16_t *dcq, const RecLayout &rl, const DevHuff *tabs, size_t stride,
+                           uint32_t *blk_bits, uint32_t *tile_bits, SeqSlot *slot, uint32_t *status, int n, cudaStream_t s)
 {
   dim3 grid((unsigned)((sd.nblocks + 255) / 256), n);
-  if (progressive) k_block_bits_prog<<<grid, 256, 0, s>>>(g, sd, tabs, stride, blk_aux, run_e, pm, blk_bits, tile_bits, status);
-  else if (slot) k_block_bits_seq<true><<<grid, 256, 0, s>>>(g, sd, nz_rec, sym, dcq, rl, tabs, stride, blk_bits, tile_bits, slot, status);
-  else k_block_bits_seq<false><<<grid, 256, 0, s>>>(g, sd, nz_rec, sym, dcq, rl, tabs, stride, blk_bits, tile_bits, nullptr, status);
+  if (slot) k_block_bits_seq<true><<<grid, 256, 0, s>>>(g, sd, sym, dcq, rl, tabs, stride, blk_bits, tile_bits, slot, status);
+  else k_block_bits_seq<false><<<grid, 256, 0, s>>>(g, sd, sym, dcq, rl, tabs, stride, blk_bits, tile_bits, nullptr, status);
+  LAUNCHED();
+}
+void launch_block_bits_prog(const Geom &g, const ScanDesc &sd, const DevHuff *tabs, size_t stride, const uint32_t *blk_aux, const uint32_t *run_e, const unsigned long long *pm,
+                            uint32_t *blk_bits, uint32_t *tile_bits, uint32_t *status, int n, cudaStream_t s)
+{
+  dim3 grid((unsigned)((sd.nblocks + 255) / 256), n);
+  k_block_bits_prog<<<grid, 256, 0, s>>>(g, sd, tabs, stride, blk_aux, run_e, pm, blk_bits, tile_bits, status);
   LAUNCHED();
 }
 void launch_scan_layout(const ScanDesc &sd, const uint32_t *blk_bits, const uint32_t *tile_bits, unsigned long long *tile_base,
@@ -3902,14 +3798,20 @@ void launch_zero_stream(uint32_t *bitbuf, size_t stride_words, const unsigned lo
   dim3 grid((unsigned)((stride_words / 4 + 1023) / 1024), n);
   k_zero_stream<<<grid, 256, 0, s>>>(bitbuf, stride_words, total_bits); LAUNCHED();
 }
-void launch_encode(const Geom &g, const ScanDesc &sd, const DcRec *nz_rec, const uint8_t *sym, const int16_t *dcq, const RecLayout &rl, const DevHuff *tabs, size_t stride, int progressive,
-                   const uint32_t *blk_bits, const uint32_t *tile_bits, const SeqSlot *slot, const unsigned long long *tile_base, const uint32_t *seg_corr, long long seg_stride,
-                   const uint32_t *blk_aux, const uint32_t *run_e, const unsigned long long *pm,
-                   uint32_t *bitbuf, size_t bitbuf_stride_words, uint32_t *mark, size_t mark_stride_words, const uint32_t *status, int n, cudaStream_t s)
+void launch_encode_seq(const Geom &g, const ScanDesc &sd, const DcRec *nz_rec, const uint8_t *sym, const int16_t *dcq, const RecLayout &rl, const DevHuff *tabs, size_t stride,
+                       const uint32_t *blk_bits, const uint32_t *tile_bits, const SeqSlot *slot, const unsigned long long *tile_base, const uint32_t *seg_corr, long long seg_stride,
+                       uint32_t *bitbuf, size_t bitbuf_stride_words, uint32_t *mark, size_t mark_stride_words, const uint32_t *status, int n, cudaStream_t s)
 {
   dim3 grid((unsigned)((sd.nblocks + 255) / 256), n);
-  if (progressive) k_encode_prog<<<grid, 256, 0, s>>>(g, sd, tabs, stride, blk_aux, run_e, pm, blk_bits, tile_bits, tile_base, seg_corr, seg_stride, bitbuf, bitbuf_stride_words, mark, mark_stride_words, status);
-  else k_encode_seq<<<grid, 256, 0, s>>>(g, sd, nz_rec, sym, dcq, rl, tabs, stride, blk_bits, tile_bits, slot, tile_base, seg_corr, seg_stride, bitbuf, bitbuf_stride_words, mark, mark_stride_words, status);
+  k_encode_seq<<<grid, 256, 0, s>>>(g, sd, nz_rec, sym, dcq, rl, tabs, stride, blk_bits, tile_bits, slot, tile_base, seg_corr, seg_stride, bitbuf, bitbuf_stride_words, mark, mark_stride_words, status);
+  LAUNCHED();
+}
+void launch_encode_prog(const Geom &g, const ScanDesc &sd, const DevHuff *tabs, size_t stride, const uint32_t *blk_aux, const uint32_t *run_e, const unsigned long long *pm,
+                        const uint32_t *blk_bits, const uint32_t *tile_bits, const unsigned long long *tile_base, const uint32_t *seg_corr, long long seg_stride,
+                        uint32_t *bitbuf, size_t bitbuf_stride_words, uint32_t *mark, size_t mark_stride_words, const uint32_t *status, int n, cudaStream_t s)
+{
+  dim3 grid((unsigned)((sd.nblocks + 255) / 256), n);
+  k_encode_prog<<<grid, 256, 0, s>>>(g, sd, tabs, stride, blk_aux, run_e, pm, blk_bits, tile_bits, tile_base, seg_corr, seg_stride, bitbuf, bitbuf_stride_words, mark, mark_stride_words, status);
   LAUNCHED();
 }
 // =====================================================================

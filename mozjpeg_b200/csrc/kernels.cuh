@@ -114,7 +114,7 @@ static_assert(sizeof(DevHuff) == 17 + 256 + 1 + 12 + 2 + 512 + 256, "DevHuff lay
 struct DcRec { float lambda_dc; int16_t raw_dc; uint8_t nz; uint8_t pad; unsigned long long nzmask; };
 static_assert(sizeof(DcRec) == 16, "DcRec layout");
 // where component ci's records start inside an image's record array
-// sym_hi: byte offset of the symbol records' second plane (SYMREC_SPLIT below) = images in the chunk * per_image * 64
+// sym_hi: byte offset of the symbol records' second plane (see SYMREC_BYTES below) = images in the chunk * per_image * 64
 struct RecLayout { long long per_image; long long comp_off[4]; long long sym_hi; };
 // which of the 8 table slots to (re)build for set i: m[i % period]
 struct SlotMasks { uint32_t m[4]; int period; };
@@ -126,13 +126,10 @@ struct SlotMasks { uint32_t m[4]; int period; };
 // the final DC values; `hist` (or nullptr) receives the blocks' AC symbol counts, [img][HIST_SLOTS][HIST_BINS].
 #define SYMREC_BYTES 128
 #define SYMREC_SLOTS 31
-// SYMREC_SPLIT: a record lives in two 64-byte halves, words 0..15 in plane 0 and words 16..31 in plane 1 (both indexed like
-// the side records), instead of one 128-byte slot: the readers fetch the header and the first entries of every block, and
-// L2 fills whole 128-byte lines -- with one slot per line the bit-count and packing kernels moved 26 / 28 MB per 4K image
-// for ~8 MB of entries; with two blocks per line the second plane is touched only by blocks of 16 and more symbols.
-#ifndef SYMREC_SPLIT
-#define SYMREC_SPLIT 1
-#endif
+// A record lives in two 64-byte halves, words 0..15 in plane 0 and words 16..31 in plane 1 (both indexed like the side
+// records): the readers fetch the header and the first entries of every block, and L2 fills whole 128-byte lines, so
+// the second plane is touched only by blocks of 16 and more symbols (one 128-byte record per line moved 26 / 28 MB per
+// 4K image through the bit-count and packing kernels for ~8 MB of entries).
 // keep_coef: also rewrite the coefficient planes (the debug tap reads them); otherwise only blocks whose record overflowed
 // get their coefficients written back, and the planes keep the plain-quantized values elsewhere.
 // dcq_ac: the AC trellis fills dcq with the plain-quantized DC values (no DC trellis will follow and write the final ones).
@@ -167,9 +164,9 @@ void launch_dummy(const Geom &g, int n, cudaStream_t s);
 void launch_gather_comp(const Geom &g, const RestartSpec &rs, uint32_t *hist, uint32_t *status, int n, cudaStream_t s);
 // the DC half of the trellis-phase statistics from the dense DC values (the AC half came from the forward kernel)
 void launch_gather_comp_dc(const Geom &g, const RestartSpec &rs, const int16_t *dcq, const RecLayout &rl, uint32_t *hist, uint32_t *status, int n, cudaStream_t s);
-// nz_rec (here and in launch_block_bits / launch_encode): the side records holding every block's final non-zero positions
-// (trellis on, sequential scans), or nullptr
-void launch_gather_seq(const Geom &g, const ScanDesc &sd, const DcRec *nz_rec, const uint8_t *sym, const int16_t *dcq, const RecLayout &rl, uint32_t *hist, uint32_t *status, int n, cudaStream_t s);
+// sym / dcq (here, in launch_block_bits_seq and in launch_encode_seq): the symbol records and dense DC values of
+// sequential scans after the trellis, or nullptr
+void launch_gather_seq(const Geom &g, const ScanDesc &sd, const uint8_t *sym, const int16_t *dcq, const RecLayout &rl, uint32_t *hist, uint32_t *status, int n, cudaStream_t s);
 void launch_seed_hist(uint32_t *hist, int slot, int n, cudaStream_t s);
 void launch_gen_tables(const uint32_t *hist, DevHuff *tabs, size_t tabs_set_stride, const SlotMasks &masks, int nsets, cudaStream_t s);
 // AC trellis of the default option set: launch_trellis_sort sorts the side records by non-zero count (srec: 16 bytes
@@ -201,37 +198,33 @@ void launch_gather_seq_dc(const Geom &g, const ScanDesc &sd, const int16_t *dcq,
 // unsigned long long [3][n][nblocks] (written here, read by the three symbol walks of the scan)
 void launch_prog_prepare(const Geom &g, const ScanDesc &sd, uint32_t *aux, uint32_t *run_e, unsigned long long *pm, int *tile_last, int *tile_first, int n, cudaStream_t s);
 void launch_gather_prog(const Geom &g, const ScanDesc &sd, const uint32_t *aux, const uint32_t *run_e, const unsigned long long *pm, uint32_t *hist, uint32_t *status, int n, cudaStream_t s);
-// Code slots of the sequential scans: k_block_bits_seq stores the bit string of every block of at most SEQ_SLOT_BITS bits
+// Code slots of the sequential scans: k_block_bits_seq stores the bit string of every block of at most 128 bits
 // (code and value bits, left-aligned), k_encode_seq copies it into the stream.  One slot per scan block,
 // [n][max_scan_blocks].  (H100, cfg2 and cfg4 q90: DESIGN §3 has the bits-per-block histogram the width comes from.)
-#ifndef SEQ_SLOT_BITS
-#define SEQ_SLOT_BITS 128
-#endif
-#define SEQ_SLOT_WORDS (SEQ_SLOT_BITS / 32)
-#if SEQ_SLOT_BITS == 128
+#define SEQ_SLOT_WORDS 4
 typedef uint4 SeqSlot;
-#elif SEQ_SLOT_BITS == 64
-typedef uint2 SeqSlot;
-#else
-#error "SEQ_SLOT_BITS is 64 or 128"
-#endif
-// sym / dcq (here and in launch_encode): the symbol records and dense DC values of sequential scans after the trellis, or nullptr
-// slot (here and in launch_encode): the code slots of a sequential scan, or nullptr: every block is walked again by the
-// packer; not used by progressive scans
-void launch_block_bits(const Geom &g, const ScanDesc &sd, const DcRec *nz_rec, const uint8_t *sym, const int16_t *dcq, const RecLayout &rl, const DevHuff *tabs, size_t tabs_image_stride, int progressive,
-                       uint32_t *blk_bits, uint32_t *tile_bits, SeqSlot *slot, const uint32_t *blk_aux, const uint32_t *run_e, const unsigned long long *pm, uint32_t *status, int n, cudaStream_t s);
+// slot (here and in launch_encode_seq): the code slots of a sequential scan, or nullptr: every block is walked again by
+// the packer
+void launch_block_bits_seq(const Geom &g, const ScanDesc &sd, const uint8_t *sym, const int16_t *dcq, const RecLayout &rl, const DevHuff *tabs, size_t tabs_image_stride,
+                           uint32_t *blk_bits, uint32_t *tile_bits, SeqSlot *slot, uint32_t *status, int n, cudaStream_t s);
+void launch_block_bits_prog(const Geom &g, const ScanDesc &sd, const DevHuff *tabs, size_t tabs_image_stride, const uint32_t *blk_aux, const uint32_t *run_e, const unsigned long long *pm,
+                            uint32_t *blk_bits, uint32_t *tile_bits, uint32_t *status, int n, cudaStream_t s);
 // tile_base[img][tile] / seg_corr[img][segment] / total_bits[img] from the tile sums (and the restart interval)
 void launch_scan_layout(const ScanDesc &sd, const uint32_t *blk_bits, const uint32_t *tile_bits, unsigned long long *tile_base,
                         uint32_t *seg_corr, long long seg_stride, unsigned long long *total_bits, size_t capacity_bits,
                         uint32_t *status, int n, cudaStream_t s);
 // clears the part of every image's word stream that the scan laid out by launch_scan_layout will occupy
 void launch_zero_stream(uint32_t *bitbuf, size_t bitbuf_image_stride_words, const unsigned long long *total_bits, int n, cudaStream_t s);
-// mark: bitmap over the unstuffed bytes of each image (restart markers' 0xFF), only touched when sd.ri != 0
-// nz_rec: the side records holding every block's final non-zero positions (trellis on, sequential scans), or nullptr
-void launch_encode(const Geom &g, const ScanDesc &sd, const DcRec *nz_rec, const uint8_t *sym, const int16_t *dcq, const RecLayout &rl, const DevHuff *tabs, size_t tabs_image_stride, int progressive,
-                   const uint32_t *blk_bits, const uint32_t *tile_bits, const SeqSlot *slot, const unsigned long long *tile_base, const uint32_t *seg_corr, long long seg_stride,
-                   const uint32_t *blk_aux, const uint32_t *run_e, const unsigned long long *pm,
-                   uint32_t *bitbuf, size_t bitbuf_image_stride_words, uint32_t *mark, size_t mark_stride_words, const uint32_t *status, int n, cudaStream_t s);
+// mark (here and in launch_encode_prog): bitmap over the unstuffed bytes of each image (restart markers' 0xFF), only
+// touched when sd.ri != 0
+// nz_rec: the side records holding every block's final non-zero positions (trellis on, no symbol records), or nullptr:
+// the fallback blocks' walk then touches only those coefficients
+void launch_encode_seq(const Geom &g, const ScanDesc &sd, const DcRec *nz_rec, const uint8_t *sym, const int16_t *dcq, const RecLayout &rl, const DevHuff *tabs, size_t tabs_image_stride,
+                       const uint32_t *blk_bits, const uint32_t *tile_bits, const SeqSlot *slot, const unsigned long long *tile_base, const uint32_t *seg_corr, long long seg_stride,
+                       uint32_t *bitbuf, size_t bitbuf_image_stride_words, uint32_t *mark, size_t mark_stride_words, const uint32_t *status, int n, cudaStream_t s);
+void launch_encode_prog(const Geom &g, const ScanDesc &sd, const DevHuff *tabs, size_t tabs_image_stride, const uint32_t *blk_aux, const uint32_t *run_e, const unsigned long long *pm,
+                        const uint32_t *blk_bits, const uint32_t *tile_bits, const unsigned long long *tile_base, const uint32_t *seg_corr, long long seg_stride,
+                        uint32_t *bitbuf, size_t bitbuf_image_stride_words, uint32_t *mark, size_t mark_stride_words, const uint32_t *status, int n, cudaStream_t s);
 // byte stuffing of every scan in one pass with a decoupled look-back (k_stuff): out[img][out_start[img] ...], scan_size,
 // out_next.  lookback: stuff_lookback_bytes() of look-back state (a descriptor per tile, a ticket per image), all zero
 // before each launch.

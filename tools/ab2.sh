@@ -1,6 +1,6 @@
 #!/bin/bash
 # Development aid, runs on the GPU box: stage times of the default pipeline for a list of "variant[,ENV=VAL...]" specs.
-#   tools/ab2.sh main main,B200JPEG_TRELLIS_V1=1 c4      (variants built by tools/build_variant.sh)
+#   tools/ab2.sh main unroll2 main      (variants built by tools/build_variant.sh, here: unroll2 -DT3_PRED_UNROLL=2)
 # BENCH_ARGS overrides the bench arguments (default: 64 images of 3840x2160, baseline + trellis).
 export B200JPEG_BENCH_CACHE=/dev/shm
 ARGS=${BENCH_ARGS:---batch 64 --steps 3 --warmup 3}
