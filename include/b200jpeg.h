@@ -514,6 +514,41 @@ int  b200jpeg_decompress_batch_opts(b200jpeg_encoder *enc, const b200jpeg_decomp
 int  b200jpeg_recompress_batch_opts(b200jpeg_encoder *enc, const b200jpeg_decompress_options *opts, const b200jpeg_params *p,
                                     const uint8_t *const *files, const size_t *sizes, int n_images);
 
+/*
+ * One decode, several renditions (a rendition ladder: sizes and qualities of the same sources).  The same sources and
+ * source checks as b200jpeg_decompress_batch_opts (one geometry; sequential files, or progressive ones with progressive
+ * decode on).  The files are parsed, uploaded and entropy-decoded once per chunk, whatever n_renditions is; behind each
+ * chunk's decode come the IDCT and upsampling / colour conversion of every distinct option set.  Rungs whose
+ * b200jpeg_decompress_options are identical share one pixel stage.  Rendition r of image i is byte for byte what the
+ * single-rendition call makes with opts[r] (and params[r]), including the default route for default options.
+ *
+ * b200jpeg_decompress_renditions writes the pixels of b200jpeg_decompress_batch_opts(opts[r]) to
+ *   pixels[r] + i * image_stride[r], rows row_pitch[r] apart, in host or device memory (pixels_on_device).
+ * b200jpeg_recompress_renditions encodes rung r from its pixels with params[r] as b200jpeg_recompress_batch_opts does
+ *   (with the sources' COM / APPn segments); file i of rung r is b200jpeg_get_output(enc, r * n_images + i).  All
+ *   n_renditions * n_images files stay readable until the next call, and b200jpeg_last_scan_bytes is their total.
+ *
+ * Refusals come before any device work, write no output, and leave the encoder usable (b200jpeg_get_output then has
+ * nothing to return).  Source problems are the single call's "image i: ..." codes and messages.  A rung's own
+ * problems are the single call's code with the message prefixed "rendition r: ": a scale whose block size is not 1, 2,
+ * 4 or 8, an unsupported out_color_space, params[r] failing b200jpeg_validate, and params[r] not describing the rung's
+ * decoded size, colour space and components (b200jpeg_decompress_output_opts).  n_renditions < 1 and NULL arrays are
+ * B200JPEG_ERR_PARAM.
+ *
+ * HBM: besides one chunk's decode, for each distinct option set its whole batch of pixels (rows of
+ * width * components bytes rounded up to 4, times height, times n_images), as b200jpeg_recompress_batch holds one; the
+ * device-memory form of b200jpeg_decompress_renditions writes into the caller's buffers instead.
+ * b200jpeg_last_stage_times afterwards: the dec_* stages once, idct and upsample_color summed over the distinct option
+ * sets, and each encode stage summed over the rungs.
+ */
+int  b200jpeg_decompress_renditions(b200jpeg_encoder *enc, int n_renditions, const b200jpeg_decompress_options *opts,
+                                    const uint8_t *const *files, const size_t *sizes, int n_images,
+                                    void *const *pixels, int pixels_on_device,
+                                    const size_t *row_pitch, const size_t *image_stride);
+int  b200jpeg_recompress_renditions(b200jpeg_encoder *enc, int n_renditions, const b200jpeg_decompress_options *opts,
+                                    const b200jpeg_params *params,
+                                    const uint8_t *const *files, const size_t *sizes, int n_images);
+
 /* b200jpeg_encode_batch, but stops after the entropy-coded bytes are in HBM: no device->host
  * copy, no host-side file assembly.  Used to time the device pipeline alone. */
 int  b200jpeg_encode_batch_device_only(b200jpeg_encoder *enc, const b200jpeg_params *p,

@@ -18,6 +18,9 @@ from .cjpeg import decompress_options, params_for_jpeg_input, params_from_switch
 
 _lib = A.load()          # raises ImportError with build instructions if missing
 
+# the keywords of decompress_options, which a rendition's option dict may use
+RENDITION_OPTIONS = ("scale", "dct", "fancy", "colorspace")
+
 __all__ = ["Encoder", "Params", "params_from_switches", "read_ppm", "cjpeg", "tj3_params", "quality_tables", "yuv_plane_dims", "B200JpegError"]
 
 
@@ -225,6 +228,71 @@ class Encoder:
             o = decompress_options(**opts)
             A.check(_lib.b200jpeg_recompress_batch_opts(self._h, C.byref(o), C.byref(p), ptrs, sizes, len(bufs)), "recompress_batch_opts")
         return [self.get_output(i) for i in range(len(bufs))]
+
+    # -- renditions: one decode, several outputs -------------------------------------------------------------------
+    @staticmethod
+    def _rendition_options(renditions) -> "C.Array":
+        """b200jpeg_decompress_options for each rung from decompress's keywords; ValueError before any library call for an
+        empty list, a rung that is not a dict or an unknown keyword"""
+        rungs = list(renditions)
+        if not rungs:
+            raise ValueError("no renditions")
+        for r, kw in enumerate(rungs):
+            if not isinstance(kw, dict):
+                raise ValueError(f"rendition {r}: options must be a dict of decompress keywords, not {type(kw).__name__}")
+            unknown = sorted(set(kw) - set(RENDITION_OPTIONS))
+            if unknown:
+                raise ValueError(f"rendition {r}: unknown option {unknown[0]!r} (the options are {', '.join(RENDITION_OPTIONS)})")
+        return (A.DecompressOptions * len(rungs))(*[decompress_options(**kw) for kw in rungs])
+
+    def decompress_renditions(self, files: Sequence[bytes], renditions: Sequence[dict]) -> List[np.ndarray]:
+        """b200jpeg_decompress_renditions: the files decoded once and rendered with each option dict of ``renditions``
+        (decompress's keywords; {} is a default decompress object).  Returns per rendition what decompress(files,
+        **renditions[r]) returns: an (N, H, W, C) uint8 array, (N, H, W) for one output component."""
+        renditions = list(renditions)
+        opts = self._rendition_options(renditions)
+        info = _parse_first(files)
+        shapes = []
+        for r, kw in enumerate(renditions):
+            try:
+                shapes.append(decompress_output(info, **kw))
+            except B200JpegError as e:
+                raise B200JpegError(e.code, "decompress_renditions", f"rendition {r}: ") from None
+        bufs, ptrs, sizes = self._files(files)
+        outs = [np.empty((len(bufs), h, w, nc), dtype=np.uint8) for w, h, _, nc in shapes]
+        k = len(outs)
+        A.check(_lib.b200jpeg_decompress_renditions(self._h, k, opts, ptrs, sizes, len(bufs), (C.c_void_p * k)(*[o.ctypes.data for o in outs]), 0,
+                                                    (C.c_size_t * k)(*[o.strides[1] for o in outs]), (C.c_size_t * k)(*[o.strides[0] for o in outs])),
+                "decompress_renditions")
+        return [o[..., 0] if o.shape[3] == 1 else o for o in outs]
+
+    def decompress_renditions_ptr(self, files: Sequence[bytes], renditions: Sequence[dict], ptrs: Sequence[int],
+                                  row_pitch: Sequence[int], image_stride: Sequence[int]) -> None:
+        """Raw-pointer form of decompress_renditions: rendition r's pixels go to device memory at ptrs[r] (rows
+        row_pitch[r] bytes apart, images image_stride[r] apart) and stay there."""
+        opts = self._rendition_options(renditions)
+        k = len(opts)
+        if not (len(ptrs) == len(row_pitch) == len(image_stride) == k):
+            raise ValueError(f"{k} renditions need {k} pointers, row pitches and image strides")
+        bufs, fptrs, sizes = self._files(files)
+        A.check(_lib.b200jpeg_decompress_renditions(self._h, k, opts, fptrs, sizes, len(bufs), (C.c_void_p * k)(*ptrs), 1,
+                                                    (C.c_size_t * k)(*row_pitch), (C.c_size_t * k)(*image_stride)), "decompress_renditions")
+
+    def recompress_renditions(self, files: Sequence[bytes], renditions) -> List[List[bytes]]:
+        """b200jpeg_recompress_renditions: the files decoded once, and per rendition (params, option dict) recompressed
+        as recompress(params, files, **options) does (params_for_jpeg_input(switches, file, **options) builds params).
+        Returns out[r][i], the file of rendition r for source i."""
+        rungs = list(renditions)
+        for r, rung in enumerate(rungs):
+            if not (isinstance(rung, (tuple, list)) and len(rung) == 2 and isinstance(rung[0], Params)):
+                raise ValueError(f"rendition {r}: expected a (params, options dict) pair")
+        opts = self._rendition_options([kw for _, kw in rungs])
+        k = len(rungs)
+        params = (Params * k)(*[p for p, _ in rungs])
+        bufs, ptrs, sizes = self._files(files)
+        n = len(bufs)
+        A.check(_lib.b200jpeg_recompress_renditions(self._h, k, opts, params, ptrs, sizes, n), "recompress_renditions")
+        return [[self.get_output(r * n + i) for i in range(n)] for r in range(k)]
 
     def last_decode_sync(self):
         """(most rounds a CTA of the speculative decoder needed, subsequences the cross-CTA pass decoded again)."""

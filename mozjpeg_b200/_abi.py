@@ -154,6 +154,7 @@ EXPORTS = [
     "b200jpeg_transform_setup", "b200jpeg_transcode_batch_transform", "b200jpeg_encode_batch_coefs_transform",
     "b200jpeg_decompress_batch", "b200jpeg_recompress_batch", "b200jpeg_decompress_output",
     "b200jpeg_default_decompress_options", "b200jpeg_decompress_output_opts", "b200jpeg_decompress_batch_opts", "b200jpeg_recompress_batch_opts",
+    "b200jpeg_decompress_renditions", "b200jpeg_recompress_renditions",
 ]
 
 _lib = None
@@ -230,6 +231,8 @@ def load() -> C.CDLL:
     lib.b200jpeg_decompress_output_opts.argtypes = [C.POINTER(SourceInfo), PO, PI, PI, PI, PI]; lib.b200jpeg_decompress_output_opts.restype = C.c_int
     lib.b200jpeg_decompress_batch_opts.argtypes = [C.c_void_p, PO, PB, PS, C.c_int, C.c_void_p, C.c_int, C.c_size_t, C.c_size_t]; lib.b200jpeg_decompress_batch_opts.restype = C.c_int
     lib.b200jpeg_recompress_batch_opts.argtypes = [C.c_void_p, PO, P, PB, PS, C.c_int]; lib.b200jpeg_recompress_batch_opts.restype = C.c_int
+    lib.b200jpeg_decompress_renditions.argtypes = [C.c_void_p, C.c_int, PO, PB, PS, C.c_int, PB, C.c_int, PS, PS]; lib.b200jpeg_decompress_renditions.restype = C.c_int
+    lib.b200jpeg_recompress_renditions.argtypes = [C.c_void_p, C.c_int, PO, P, PB, PS, C.c_int]; lib.b200jpeg_recompress_renditions.restype = C.c_int
     lib.b200jpeg_last_error.argtypes = []; lib.b200jpeg_last_error.restype = C.c_char_p
     lib.b200jpeg_version.argtypes = []; lib.b200jpeg_version.restype = C.c_char_p
     _lib = lib
@@ -237,9 +240,9 @@ def load() -> C.CDLL:
 
 
 class B200JpegError(RuntimeError):
-    def __init__(self, code: int, where: str):
+    def __init__(self, code: int, where: str, prefix: str = ""):
         msg = load().b200jpeg_last_error().decode("utf-8", "replace")
-        super().__init__(f"{where}: error {code}: {msg}")
+        super().__init__(f"{where}: error {code}: {prefix}{msg}")
         self.code = code
 
 

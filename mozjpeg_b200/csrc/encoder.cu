@@ -6,11 +6,13 @@
 #include "b200jpeg.h"
 #include "internal.h"
 #include "kernels.cuh"
+#include <climits>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <map>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -151,10 +153,14 @@ struct b200jpeg_encoder {
   // quantization tables, the whole batch's pixels where the caller gave no device buffer, the stage times summed over
   // the chunks, and per image the source's COM / APPn segments a recompress copies into its file
   DevBuf d_dec_samples, d_dec_quant, d_dec_pixels, d_dec_mtab;   // d_dec_mtab: ifast / float multiplier tables
-  cudaEvent_t pix_ev[3] = {nullptr, nullptr, nullptr};
+  std::vector<cudaEvent_t> pix_ev;   // per pixel output of a chunk: before the IDCT, before the upsampling, after it
   float dec_ms[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};   // the six decode stages, idct, upsample_color, the two refinements
   std::vector<std::vector<uint8_t>> dec_markers;
   const std::vector<std::vector<uint8_t>> *copy_markers = nullptr;   // of the batch being encoded, or nullptr
+  // renditions (b200jpeg_decompress_renditions / b200jpeg_recompress_renditions): the whole batch's pixels of each
+  // distinct option set, and the files of every rung but the last (the next rung's encode reuses the file arenas)
+  std::vector<DevBuf> d_rend_pixels;
+  std::vector<uint8_t> rend_files;
   CoefXform xform{};                            // the coefficient import's block mapping in the current batch (all zero: a copy)
 };
 
@@ -1846,35 +1852,92 @@ static void method_table(int method, const uint16_t *q, uint32_t *out)
   }
 }
 
-// the IDCT and upsampling / colour conversion stages of one decoded chunk (e->dec) for a non-default plan: each
-// needed component through the IDCT of its DCT_scaled_size into a plane of wib * size samples a row, then
-// k_upsample_opts into the pixels.  qt / mt: host staging for the tables.
+// the sample planes of one chunk's pixel stage for `plan`: per needed component nk images of hib x wib blocks of
+// ssize x ssize samples; off[c]: where component c's plane starts.  Returns the bytes of all of them.
+static size_t sample_plane_layout(const DecBatch &b, const DecPlan &plan, int nk, size_t off[4])
+{
+  size_t total = 0;
+  for (int c = 0; c < 4; c++) off[c] = 0;
+  for (int c = 0; c < b.nc; c++) {
+    if (!plan.needed[c]) continue;
+    off[c] = total; total += ((size_t)nk * b.hib[c] * b.wib[c] * plan.ssize[c] * plan.ssize[c] + 255) & ~(size_t)255;
+  }
+  return total;
+}
+
+// the device buffers one chunk's pixel stage for `plan` uses: sample planes, dequantization tables and, for the ifast
+// and float IDCTs at full size, multiplier tables.  A chunk's pixel stages are enqueued back to back, so every plan is
+// reserved for before the first is enqueued: no buffer is reallocated under a queued kernel.
+static int reserve_pixel_stage(b200jpeg_encoder *e, const DecPlan &plan, int nk)
+{
+  const DecBatch &b = e->dec;
+  size_t off[4];
+  bool need_mt = false;
+  for (int c = 0; c < b.nc; c++) need_mt |= plan.needed[c] && plan.ssize[c] == 8 && plan.method != B200JPEG_DCT_ISLOW;
+  int rc;
+  if ((rc = e->d_dec_samples.reserve(sample_plane_layout(b, plan, nk, off))) || (rc = e->d_dec_quant.reserve((size_t)nk * b.nc * 128)) ||
+      (need_mt && (rc = e->d_dec_mtab.reserve((size_t)nk * b.nc * 256)))) return rc;
+  return B200JPEG_OK;
+}
+
+// the tables each image of the decoded chunk latched, [nk][nc][64], into e->d_dec_quant (qt: host staging)
+static int upload_chunk_quant(b200jpeg_encoder *e, int nk, std::vector<uint16_t> &qt)
+{
+  const DecBatch &b = e->dec;
+  const int nc = b.nc;
+  qt.resize((size_t)nk * nc * 64);
+  for (int i = 0; i < nk; i++)
+    for (int c = 0; c < nc; c++) memcpy(&qt[((size_t)i * nc + c) * 64], b.info[i].comp_quant[c], 128);
+  CU(cudaMemcpyAsync(e->d_dec_quant.p, qt.data(), qt.size() * 2, cudaMemcpyHostToDevice, e->stream));
+  return B200JPEG_OK;
+}
+
+// the default plan's IDCT and upsampling / colour conversion of one decoded chunk: jpeg_idct_islow per component into
+// planes of wib * 8 samples a row, then the fancy upsampling and default colour conversion into the pixels
+static int idct_upsample_default(b200jpeg_encoder *e, int nk, uint8_t *pix, size_t row_pitch, size_t image_stride, const cudaEvent_t *ev)
+{
+  const DecBatch &b = e->dec;
+  const int nc = b.nc, W = b.W, H = b.H;
+  const int hx = nc == 3 ? b.h[0] : 1, vx = nc == 3 ? b.v[0] : 1;
+  cudaStream_t s = e->stream;
+  size_t off[4];
+  sample_plane_layout(b, DecPlan(), nk, off);
+  CU(cudaEventRecord(ev[0], s));
+  const uint8_t *planes[4] = {nullptr, nullptr, nullptr, nullptr}; int pitch[4] = {0, 0, 0, 0}; long long stride[4] = {0, 0, 0, 0};
+  for (int c = 0; c < nc; c++) {
+    uint8_t *dst = e->d_dec_samples.as<uint8_t>() + off[c];
+    launch_idct_islow(reinterpret_cast<const int16_t *>(e->d_dec_planes.as<uint8_t>() + e->dec_plane_off[c]), e->d_dec_quant.as<uint16_t>() + c * 64, nc * 64,
+                      dst, b.wib[c], b.hib[c], nk, s);
+    planes[c] = dst; pitch[c] = b.wib[c] * 8; stride[c] = (long long)b.hib[c] * 8 * pitch[c];
+  }
+  CU(cudaEventRecord(ev[1], s));
+  const int dw = div_up(W, hx), dh = div_up(H, vx);                    // downsampled_width / _height of the chroma (jdmaster.c)
+  if (launch_upsample_color(hx, vx, nc, planes, pitch, stride, dw, dh, nc == 3 && b.info[0].jpeg_color_space != B200JPEG_CS_RGB,
+                            pix, row_pitch, image_stride, W, H, nk, s)) { set_error("no upsampling kernel for %dx%d sampling of %d components", hx, vx, nc); return B200JPEG_ERR_UNSUPPORTED; }
+  CU(cudaEventRecord(ev[2], s));
+  CU(cudaGetLastError());
+  return B200JPEG_OK;
+}
+
+// the IDCT and upsampling / colour conversion stages of one decoded chunk for a non-default plan: each needed
+// component through the IDCT of its DCT_scaled_size into a plane of wib * size samples a row, then k_upsample_opts
+// into the pixels.  qt: the chunk's tables as upload_chunk_quant staged them; mt: host staging for the multipliers.
 static int idct_upsample_opts(b200jpeg_encoder *e, const DecPlan &plan, int nk, uint8_t *pix, size_t row_pitch, size_t image_stride,
-                              std::vector<uint16_t> &qt, std::vector<uint32_t> &mt)
+                              const std::vector<uint16_t> &qt, std::vector<uint32_t> &mt, const cudaEvent_t *ev)
 {
   const DecBatch &b = e->dec;
   const int nc = b.nc;
   cudaStream_t s = e->stream;
-  size_t off[4] = {0, 0, 0, 0}, total = 0;
+  size_t off[4];
+  sample_plane_layout(b, plan, nk, off);
   bool need_mt = false;
-  for (int c = 0; c < nc; c++) {
-    if (!plan.needed[c]) continue;
-    off[c] = total; total += ((size_t)nk * b.hib[c] * b.wib[c] * plan.ssize[c] * plan.ssize[c] + 255) & ~(size_t)255;
-    need_mt |= plan.ssize[c] == 8 && plan.method != B200JPEG_DCT_ISLOW;
-  }
-  int rc;
-  if ((rc = e->d_dec_samples.reserve(total)) || (rc = e->d_dec_quant.reserve((size_t)nk * nc * 128)) ||
-      (need_mt && (rc = e->d_dec_mtab.reserve((size_t)nk * nc * 256)))) return rc;
-  qt.resize((size_t)nk * nc * 64);
-  for (int i = 0; i < nk; i++)
-    for (int c = 0; c < nc; c++) memcpy(&qt[((size_t)i * nc + c) * 64], b.info[i].comp_quant[c], 128);
-  CU(cudaMemcpyAsync(e->d_dec_quant.p, qt.data(), qt.size() * 2, cudaMemcpyHostToDevice, s));
+  for (int c = 0; c < nc; c++) need_mt |= plan.needed[c] && plan.ssize[c] == 8 && plan.method != B200JPEG_DCT_ISLOW;
   if (need_mt) {
     mt.resize((size_t)nk * nc * 64);
     for (size_t t = 0; t < (size_t)nk * nc; t++) method_table(plan.method, &qt[t * 64], &mt[t * 64]);
     CU(cudaMemcpyAsync(e->d_dec_mtab.p, mt.data(), mt.size() * 4, cudaMemcpyHostToDevice, s));
   }
-  CU(cudaEventRecord(e->pix_ev[0], s));
+  CU(cudaEventRecord(ev[0], s));
   UpsOpt u;
   memset(&u, 0, sizeof u);
   for (int c = 0; c < nc; c++) {
@@ -1889,24 +1952,37 @@ static int idct_upsample_opts(b200jpeg_encoder *e, const DecPlan &plan, int nk, 
       u.dw[c] = plan.dw[c]; u.dh[c] = plan.dh[c]; u.hr[c] = plan.hr[c]; u.vr[c] = plan.vr[c]; u.fancy[c] = plan.fancy[c];
     }
   }
-  CU(cudaEventRecord(e->pix_ev[1], s));
+  CU(cudaEventRecord(ev[1], s));
   u.nin = plan.nin; u.conv = plan.conv; u.ps = plan.ps;
   for (int k = 0; k < 4; k++) u.off[k] = plan.off[k];
   launch_upsample_opts(u, pix, row_pitch, image_stride, plan.out_w, plan.out_h, nk, s);
-  CU(cudaEventRecord(e->pix_ev[2], s));
+  CU(cudaEventRecord(ev[2], s));
   CU(cudaGetLastError());
-  CU(cudaStreamSynchronize(s));
-  sum_decode_stage_times(e);
-  for (int k = 0; k < 2; k++) { float ms = 0.f; cudaEventElapsedTime(&ms, e->pix_ev[k], e->pix_ev[k + 1]); e->dec_ms[6 + k] += ms; }
   return B200JPEG_OK;
 }
 
-// jpeg_read_scanlines for a batch of files: entropy decode, IDCT and upsampling / colour conversion chunk by chunk
-// (the coefficient and sample planes are one chunk's), into pixels on the device.
-// opts: the decompress object's options (nullptr: its defaults); options that give what the defaults give take the
-// default route.
-static int decompress_files(b200jpeg_encoder *e, const uint8_t *const *files, const size_t *sizes, int n, uint8_t *pix, size_t row_pitch, size_t image_stride,
-                            bool want_markers, const b200jpeg_decompress_options *opts = nullptr)
+// Pixels for one DecPlan from the decoded chunk (e->dec, e->d_dec_planes, its tables in e->d_dec_quant) into (pix,
+// row_pitch, image_stride): the default plan through launch_idct_islow and launch_upsample_color, every other plan
+// through idct_upsample_opts.  It only enqueues on e->stream, with events ev[0..2] around the IDCT and around the
+// upsampling / colour conversion; the caller reserves (reserve_pixel_stage), synchronises and adds the times.
+static int chunk_pixels(b200jpeg_encoder *e, const DecPlan &plan, int nk, uint8_t *pix, size_t row_pitch, size_t image_stride,
+                        const std::vector<uint16_t> &qt, std::vector<uint32_t> &mt, const cudaEvent_t *ev)
+{
+  return plan.is_default ? idct_upsample_default(e, nk, pix, row_pitch, image_stride, ev)
+                         : idct_upsample_opts(e, plan, nk, pix, row_pitch, image_stride, qt, mt, ev);
+}
+
+// One pixel output of a decompress: the decompress object's options (nullptr: its defaults) and where image i's rows
+// go on the device (pix + i * image_stride, row_pitch bytes apart).
+struct PixTarget {
+  const b200jpeg_decompress_options *opts; uint8_t *pix; size_t row_pitch, image_stride;
+};
+
+// jpeg_read_scanlines for a batch of files, to one or more targets: the entropy decode chunk by chunk (the coefficient
+// and sample planes are one chunk's), and behind each chunk's decode the IDCT and upsampling / colour conversion of
+// every target, enqueued together and synchronised once.  Options that give what the defaults give take the default
+// route.
+static int decompress_files(b200jpeg_encoder *e, const uint8_t *const *files, const size_t *sizes, int n, const PixTarget *tg, int ntg, bool want_markers)
 {
   // every refusal comes before any device work
   b200jpeg_source_info s0;
@@ -1926,13 +2002,16 @@ static int decompress_files(b200jpeg_encoder *e, const uint8_t *const *files, co
   }
   const int W = s0.image_width, H = s0.image_height, nc = s0.num_components;
   const int hx = nc == 3 ? s0.h_samp_factor[0] : 1, vx = nc == 3 ? s0.v_samp_factor[0] : 1;
-  DecPlan plan;
-  if (opts) { int rc = plan_decompress(s0, *opts, plan); if (rc) return rc; }
-  const bool def = plan.is_default;
-  const int OW = def ? W : plan.out_w, OH = def ? H : plan.out_h, onc = def ? nc : plan.out_nc;
-  if (row_pitch < (size_t)OW * onc || (n > 1 && image_stride < row_pitch * (size_t)(OH - 1) + (size_t)OW * onc)) { set_error("row_pitch or image_stride smaller than the decoded image (%dx%d, %d components)", OW, OH, onc); return B200JPEG_ERR_PARAM; }
+  std::vector<DecPlan> plans(ntg);
+  for (int t = 0; t < ntg; t++) {
+    DecPlan &plan = plans[t];
+    if (tg[t].opts) { int rc = plan_decompress(s0, *tg[t].opts, plan); if (rc) return rc; }
+    const bool def = plan.is_default;
+    const int OW = def ? W : plan.out_w, OH = def ? H : plan.out_h, onc = def ? nc : plan.out_nc;
+    if (tg[t].row_pitch < (size_t)OW * onc || (n > 1 && tg[t].image_stride < tg[t].row_pitch * (size_t)(OH - 1) + (size_t)OW * onc)) { set_error("row_pitch or image_stride smaller than the decoded image (%dx%d, %d components)", OW, OH, onc); return B200JPEG_ERR_PARAM; }
+  }
   CU(cudaSetDevice(e->device));
-  for (cudaEvent_t &ev : e->pix_ev) if (!ev) CU(cudaEventCreate(&ev));
+  while (e->pix_ev.size() < (size_t)ntg * 3) { cudaEvent_t ev; CU(cudaEventCreate(&ev)); e->pix_ev.push_back(ev); }
   for (float &m : e->dec_ms) m = 0.f;
   e->dec_ms_prog = false;
   e->dec.want_markers = want_markers;
@@ -1941,7 +2020,6 @@ static int decompress_files(b200jpeg_encoder *e, const uint8_t *const *files, co
   long long per = 0;
   for (int c = 0; c < nc; c++) per += (long long)div_up((long long)W * s0.h_samp_factor[c], (nc == 3 ? hx : s0.h_samp_factor[0]) * 8) * div_up((long long)H * s0.v_samp_factor[c], (nc == 3 ? vx : s0.v_samp_factor[0]) * 8);
   const int C = std::min(n, e->chunk_images_override > 0 ? e->chunk_images_override : (int)std::max(1LL, 1600000LL / std::max(1LL, per)));
-  cudaStream_t s = e->stream;
   std::vector<uint16_t> qt;
   std::vector<uint32_t> mt;
   for (int i0 = 0; i0 < n; i0 += C) {
@@ -1949,33 +2027,15 @@ static int decompress_files(b200jpeg_encoder *e, const uint8_t *const *files, co
     int rc = decode_files(e, files + i0, sizes + i0, nk, i0);
     if (rc) return rc;
     e->dec_ms_prog |= e->dec_prog;
-    const DecBatch &b = e->dec;
     if (want_markers) for (int i = 0; i < nk; i++) e->dec_markers[i0 + i].swap(e->dec.markers[i]);
-    if (!def) { if ((rc = idct_upsample_opts(e, plan, nk, pix + (size_t)i0 * image_stride, row_pitch, image_stride, qt, mt))) return rc; continue; }
-    size_t off[4] = {0, 0, 0, 0}, total = 0;
-    for (int c = 0; c < nc; c++) { off[c] = total; total += ((size_t)nk * b.hib[c] * b.wib[c] * 64 + 255) & ~(size_t)255; }
-    if ((rc = e->d_dec_samples.reserve(total)) || (rc = e->d_dec_quant.reserve((size_t)nk * nc * 128))) return rc;
-    qt.resize((size_t)nk * nc * 64);
-    for (int i = 0; i < nk; i++)
-      for (int c = 0; c < nc; c++) memcpy(&qt[((size_t)i * nc + c) * 64], b.info[i].comp_quant[c], 128);
-    CU(cudaMemcpyAsync(e->d_dec_quant.p, qt.data(), qt.size() * 2, cudaMemcpyHostToDevice, s));
-    CU(cudaEventRecord(e->pix_ev[0], s));
-    const uint8_t *planes[4] = {nullptr, nullptr, nullptr, nullptr}; int pitch[4] = {0, 0, 0, 0}; long long stride[4] = {0, 0, 0, 0};
-    for (int c = 0; c < nc; c++) {
-      uint8_t *dst = e->d_dec_samples.as<uint8_t>() + off[c];
-      launch_idct_islow(reinterpret_cast<const int16_t *>(e->d_dec_planes.as<uint8_t>() + e->dec_plane_off[c]), e->d_dec_quant.as<uint16_t>() + c * 64, nc * 64,
-                        dst, b.wib[c], b.hib[c], nk, s);
-      planes[c] = dst; pitch[c] = b.wib[c] * 8; stride[c] = (long long)b.hib[c] * 8 * pitch[c];
-    }
-    CU(cudaEventRecord(e->pix_ev[1], s));
-    const int dw = div_up(W, hx), dh = div_up(H, vx);                    // downsampled_width / _height of the chroma (jdmaster.c)
-    if (launch_upsample_color(hx, vx, nc, planes, pitch, stride, dw, dh, nc == 3 && s0.jpeg_color_space != B200JPEG_CS_RGB,
-                              pix + (size_t)i0 * image_stride, row_pitch, image_stride, W, H, nk, s)) { set_error("no upsampling kernel for %dx%d sampling of %d components", hx, vx, nc); return B200JPEG_ERR_UNSUPPORTED; }
-    CU(cudaEventRecord(e->pix_ev[2], s));
-    CU(cudaGetLastError());
-    CU(cudaStreamSynchronize(s));
+    for (int t = 0; t < ntg; t++) if ((rc = reserve_pixel_stage(e, plans[t], nk))) return rc;
+    if ((rc = upload_chunk_quant(e, nk, qt))) return rc;
+    for (int t = 0; t < ntg; t++)
+      if ((rc = chunk_pixels(e, plans[t], nk, tg[t].pix + (size_t)i0 * tg[t].image_stride, tg[t].row_pitch, tg[t].image_stride, qt, mt, &e->pix_ev[(size_t)t * 3]))) return rc;
+    CU(cudaStreamSynchronize(e->stream));
     sum_decode_stage_times(e);
-    for (int k = 0; k < 2; k++) { float ms = 0.f; cudaEventElapsedTime(&ms, e->pix_ev[k], e->pix_ev[k + 1]); e->dec_ms[6 + k] += ms; }
+    for (int t = 0; t < ntg; t++)
+      for (int k = 0; k < 2; k++) { float ms = 0.f; cudaEventElapsedTime(&ms, e->pix_ev[(size_t)t * 3 + k], e->pix_ev[(size_t)t * 3 + k + 1]); e->dec_ms[6 + k] += ms; }
   }
   return B200JPEG_OK;
 }
@@ -2009,13 +2069,15 @@ static int decompress_batch(b200jpeg_encoder *e, const b200jpeg_decompress_optio
     CU(cudaSetDevice(e->device));
     if ((rc = e->d_dec_pixels.reserve(ds * (size_t)n_images))) return rc;
     dst = e->d_dec_pixels.as<uint8_t>();
-    rc = decompress_files(e, files, sizes, n_images, dst, dp, ds, false, opts);
+    const PixTarget t = {opts, dst, dp, ds};
+    rc = decompress_files(e, files, sizes, n_images, &t, 1, false);
     if (rc) return rc;
     for (int i = 0; i < n_images; i++)
       CU(cudaMemcpy2DAsync(static_cast<uint8_t *>(pixels) + (size_t)i * image_stride, row_pitch, dst + (size_t)i * ds, dp, row, rows, cudaMemcpyDeviceToHost, e->stream));
     CU(cudaStreamSynchronize(e->stream));
   } else {
-    int rc = decompress_files(e, files, sizes, n_images, dst, dp, ds, false, opts);
+    const PixTarget t = {opts, dst, dp, ds};
+    int rc = decompress_files(e, files, sizes, n_images, &t, 1, false);
     if (rc) return rc;
   }
   e->pending_marks = 0;
@@ -2048,8 +2110,149 @@ static int recompress_batch(b200jpeg_encoder *e, const b200jpeg_decompress_optio
   }
   CU(cudaSetDevice(e->device));
   if ((rc = e->d_dec_pixels.reserve(stride * (size_t)n_images))) return rc;
-  if ((rc = decompress_files(e, files, sizes, n_images, e->d_dec_pixels.as<uint8_t>(), pitch, stride, true, opts))) return rc;
+  const PixTarget t = {opts, e->d_dec_pixels.as<uint8_t>(), pitch, stride};
+  if ((rc = decompress_files(e, files, sizes, n_images, &t, 1, true))) return rc;
   if ((rc = encode_common(e, p, e->d_dec_pixels.p, 1, pitch, stride, n_images, false, nullptr, nullptr, &e->dec_markers))) return rc;
+  add_decompress_stage_times(e);
+  return B200JPEG_OK;
+}
+
+// The rungs of a rendition call, checked against image 0 before any device work: each rung's decoded size, colour space
+// and components (b200jpeg_decompress_output_opts), and the distinct option sets (set[r]: rung r's set; first[k]: the
+// first rung of set k).  A rung's refusal keeps its code, the message names the rung.
+struct Rungs {
+  std::vector<int> set, first, w, h, cs, nc;
+};
+static int check_rungs(int n_renditions, const b200jpeg_decompress_options *opts, const uint8_t *const *files, const size_t *sizes, Rungs &g)
+{
+  if (!files[0]) { set_error("image 0: no file"); return B200JPEG_ERR_PARAM; }
+  std::unique_ptr<b200jpeg_source_info> s(new b200jpeg_source_info);
+  int rc = b200jpeg_parse_source(files[0], sizes[0], s.get());
+  if (rc) { std::string m = b200jpeg_last_error(); set_error("image 0: %s", m.c_str()); return rc; }
+  g = Rungs();
+  for (int r = 0; r < n_renditions; r++) {
+    int w = 0, h = 0, cs = 0, nc = 0;
+    if ((rc = b200jpeg_decompress_output_opts(s.get(), &opts[r], &w, &h, &cs, &nc))) { std::string m = b200jpeg_last_error(); set_error("rendition %d: %s", r, m.c_str()); return rc; }
+    g.w.push_back(w); g.h.push_back(h); g.cs.push_back(cs); g.nc.push_back(nc);
+    const b200jpeg_decompress_options &o = opts[r];
+    int k = 0;
+    for (; k < (int)g.first.size(); k++) {
+      const b200jpeg_decompress_options &f = opts[g.first[k]];
+      if (f.scale_num == o.scale_num && f.scale_denom == o.scale_denom && f.dct_method == o.dct_method &&
+          f.do_fancy_upsampling == o.do_fancy_upsampling && f.out_color_space == o.out_color_space) break;
+    }
+    if (k == (int)g.first.size()) g.first.push_back(r);
+    g.set.push_back(k);
+  }
+  return B200JPEG_OK;
+}
+
+// one device buffer per distinct option set for the whole batch's pixels, rows padded to 4 bytes as recompress_batch's
+static int reserve_rendition_pixels(b200jpeg_encoder *e, const Rungs &g, int n_images, std::vector<PixTarget> &tg)
+{
+  const int K = (int)g.first.size();
+  if ((int)e->d_rend_pixels.size() < K) e->d_rend_pixels.resize(K);
+  tg.resize(K);
+  for (int k = 0; k < K; k++) {
+    const int r = g.first[k];
+    const size_t pitch = ((size_t)g.w[r] * g.nc[r] + 3) & ~(size_t)3, stride = pitch * (size_t)g.h[r];
+    if (int rc = e->d_rend_pixels[k].reserve(stride * (size_t)n_images)) return rc;
+    tg[k] = PixTarget{nullptr, e->d_rend_pixels[k].as<uint8_t>(), pitch, stride};
+  }
+  return B200JPEG_OK;
+}
+
+// b200jpeg_decompress_renditions: one decode per chunk, one pixel stage per distinct option set, and the rungs that
+// share a set copied from the first of them
+static int decompress_renditions(b200jpeg_encoder *e, int n_renditions, const b200jpeg_decompress_options *opts, const uint8_t *const *files,
+                                 const size_t *sizes, int n_images, void *const *pixels, int pixels_on_device, const size_t *row_pitch,
+                                 const size_t *image_stride)
+{
+  if (!e || n_renditions < 1 || !opts || !files || !sizes || n_images <= 0 || !pixels || !row_pitch || !image_stride) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
+  Rungs g;
+  int rc = check_rungs(n_renditions, opts, files, sizes, g);
+  if (rc) return rc;
+  for (int r = 0; r < n_renditions; r++) {
+    const size_t row = (size_t)g.w[r] * g.nc[r];
+    if (!pixels[r] || row_pitch[r] < row || (n_images > 1 && image_stride[r] < row_pitch[r] * (size_t)(g.h[r] - 1) + row)) {
+      set_error("rendition %d: no pixel buffer, or row_pitch or image_stride smaller than the decoded image (%dx%d, %d components)", r, g.w[r], g.h[r], g.nc[r]);
+      return B200JPEG_ERR_PARAM;
+    }
+  }
+  CU(cudaSetDevice(e->device));
+  std::vector<PixTarget> tg;
+  if (pixels_on_device) {
+    // the first rung of each set receives its pixels where the single call would write them
+    for (int r : g.first) tg.push_back(PixTarget{nullptr, static_cast<uint8_t *>(pixels[r]), row_pitch[r], image_stride[r]});
+  } else if ((rc = reserve_rendition_pixels(e, g, n_images, tg))) return rc;
+  for (int k = 0; k < (int)tg.size(); k++) tg[k].opts = &opts[g.first[k]];
+  if ((rc = decompress_files(e, files, sizes, n_images, tg.data(), (int)tg.size(), false))) return rc;
+  for (int r = 0; r < n_renditions; r++) {
+    const PixTarget &t = tg[g.set[r]];
+    if (pixels_on_device && r == g.first[g.set[r]]) continue;
+    for (int i = 0; i < n_images; i++)
+      CU(cudaMemcpy2DAsync(static_cast<uint8_t *>(pixels[r]) + (size_t)i * image_stride[r], row_pitch[r], t.pix + (size_t)i * t.image_stride, t.row_pitch,
+                           (size_t)g.w[r] * g.nc[r], g.h[r], pixels_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, e->stream));
+  }
+  CU(cudaStreamSynchronize(e->stream));
+  e->pending_marks = 0;
+  e->stage_names.clear(); e->stage_ms.clear(); e->stage_calls.clear();
+  add_decompress_stage_times(e);
+  return B200JPEG_OK;
+}
+
+// b200jpeg_recompress_renditions: the pixels of each distinct option set as decompress_renditions makes them, then per
+// rung recompress_batch's encode of the whole batch from its set's pixels
+static int recompress_renditions(b200jpeg_encoder *e, int n_renditions, const b200jpeg_decompress_options *opts, const b200jpeg_params *params,
+                                 const uint8_t *const *files, const size_t *sizes, int n_images)
+{
+  if (!e || n_renditions < 1 || !opts || !params || !files || !sizes || n_images <= 0) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
+  if ((long long)n_renditions * n_images > INT_MAX) { set_error("%d renditions of %d images are more outputs than b200jpeg_get_output indexes", n_renditions, n_images); return B200JPEG_ERR_PARAM; }
+  Rungs g;
+  int rc = check_rungs(n_renditions, opts, files, sizes, g);
+  if (rc) return rc;
+  for (int r = 0; r < n_renditions; r++) {
+    const b200jpeg_params *p = &params[r];
+    if ((rc = b200jpeg_validate(p))) { std::string m = b200jpeg_last_error(); set_error("rendition %d: %s", r, m.c_str()); return rc; }
+    if (p->data_precision != 8) { set_error("rendition %d: the sources decode to 8-bit samples, the parameter block has data_precision %d", r, p->data_precision); return B200JPEG_ERR_PARAM; }
+    if (g.w[r] != p->image_width || g.h[r] != p->image_height || g.cs[r] != p->in_color_space || g.nc[r] != p->input_components) {
+      set_error("rendition %d: the sources decode to %dx%d pixels of %d samples in colour space %d, the parameter block describes %dx%d of %d in %d (see b200jpeg_decompress_output_opts)",
+                r, g.w[r], g.h[r], g.nc[r], g.cs[r], p->image_width, p->image_height, p->input_components, p->in_color_space);
+      return B200JPEG_ERR_PARAM;
+    }
+  }
+  CU(cudaSetDevice(e->device));
+  std::vector<PixTarget> tg;
+  if ((rc = reserve_rendition_pixels(e, g, n_images, tg))) return rc;
+  for (int k = 0; k < (int)tg.size(); k++) tg[k].opts = &opts[g.first[k]];
+  if ((rc = decompress_files(e, files, sizes, n_images, tg.data(), (int)tg.size(), true))) return rc;
+  // encode rung by rung; a rung's files move to e->rend_files before the next rung's encode reuses the file arenas
+  std::vector<std::pair<size_t, size_t>> kept;          // (offset in rend_files, size) of the files of rungs 0 .. R-2
+  std::vector<const char *> names; std::vector<float> ms; std::vector<int> calls;
+  size_t scan_bytes = 0;
+  e->rend_files.clear();
+  for (int r = 0; r < n_renditions; r++) {
+    const PixTarget &t = tg[g.set[r]];
+    if ((rc = encode_common(e, &params[r], t.pix, 1, t.row_pitch, t.image_stride, n_images, false, nullptr, nullptr, &e->dec_markers))) return rc;
+    scan_bytes += e->last_scan_bytes;
+    for (size_t k = 0; k < e->stage_names.size(); k++) {
+      size_t j = 0;
+      while (j < names.size() && strcmp(names[j], e->stage_names[k])) j++;
+      if (j == names.size()) { names.push_back(e->stage_names[k]); ms.push_back(0.f); calls.push_back(0); }
+      ms[j] += e->stage_ms[k]; calls[j] += e->stage_calls[k];
+    }
+    if (r + 1 == n_renditions) break;
+    for (int i = 0; i < n_images; i++) {
+      kept.emplace_back(e->rend_files.size(), e->files[i].second);
+      e->rend_files.insert(e->rend_files.end(), e->files[i].first, e->files[i].first + e->files[i].second);
+    }
+  }
+  std::vector<std::pair<uint8_t *, size_t>> last(e->files);
+  e->files.clear();
+  for (const std::pair<size_t, size_t> &f : kept) e->files.emplace_back(e->rend_files.data() + f.first, f.second);
+  e->files.insert(e->files.end(), last.begin(), last.end());
+  e->last_scan_bytes = scan_bytes;
+  e->stage_names = names; e->stage_ms = ms; e->stage_calls = calls;
   add_decompress_stage_times(e);
   return B200JPEG_OK;
 }
@@ -2081,6 +2284,23 @@ int b200jpeg_recompress_batch_opts(b200jpeg_encoder *e, const b200jpeg_decompres
 {
   if (!opts) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
   return b200::recompress_batch(e, opts, p, files, sizes, n_images);
+}
+
+int b200jpeg_decompress_renditions(b200jpeg_encoder *e, int n_renditions, const b200jpeg_decompress_options *opts, const uint8_t *const *files,
+                                   const size_t *sizes, int n_images, void *const *pixels, int pixels_on_device,
+                                   const size_t *row_pitch, const size_t *image_stride)
+{
+  if (e) e->files.clear();                       // a refused call leaves no outputs behind
+  return b200::decompress_renditions(e, n_renditions, opts, files, sizes, n_images, pixels, pixels_on_device, row_pitch, image_stride);
+}
+
+int b200jpeg_recompress_renditions(b200jpeg_encoder *e, int n_renditions, const b200jpeg_decompress_options *opts, const b200jpeg_params *params,
+                                   const uint8_t *const *files, const size_t *sizes, int n_images)
+{
+  if (e) e->files.clear();
+  const int rc = b200::recompress_renditions(e, n_renditions, opts, params, files, sizes, n_images);
+  if (rc && e) e->files.clear();
+  return rc;
 }
 
 int b200jpeg_decode_coefs_batch(b200jpeg_encoder *e, const uint8_t *const *files, const size_t *sizes, int n_images,
@@ -2173,6 +2393,7 @@ void b200jpeg_encoder_destroy(b200jpeg_encoder *e)
   DevBuf *dd[] = {&e->d_dec_words, &e->d_dec_segs, &e->d_dec_scans, &e->d_dec_tabs, &e->d_dec_out, &e->d_dec_rec, &e->d_dec_pre, &e->d_dec_tsum, &e->d_dec_dcd, &e->d_dec_planes, &e->d_dec_stat,
                   &e->d_dec_samples, &e->d_dec_quant, &e->d_dec_pixels, &e->d_dec_mtab};
   for (DevBuf *b : dd) b->release();
+  for (DevBuf &b : e->d_rend_pixels) b.release();
   for (cudaEvent_t ev : e->dec_ev) if (ev) cudaEventDestroy(ev);
   for (cudaEvent_t ev : e->pix_ev) if (ev) cudaEventDestroy(ev);
   PinBuf *pb[] = {&e->h_qt, &e->h_tc, &e->h_fixed, &e->h_status, &e->h_out_pos, &e->h_scan_size, &e->h_tabs, &e->h_stage, &e->h_best_al, &e->h_qinit, &e->h_qimg, &e->h_qset, &e->h_dec_words, &e->h_dec_stat};
