@@ -82,12 +82,14 @@ using namespace b200;
 struct Arena {
   b200::DevBuf d_planes;             // input smoothing: the pre-pass's component planes
   b200::DevBuf d_coef[4], d_raw[4], d_plain[4], d_hist, d_tabs_trellis, d_rec, d_srec, d_splits, d_best_al, d_qimg, d_qsum, d_eo, d_es;
-  b200::DevBuf d_blk_bits, d_slot, d_tile_bits, d_tile_base, d_seg_corr, d_mark, d_stuff_lb, d_blk_aux, d_blk_run, d_blk_mask, d_total_bits, d_bitbuf;
+  b200::DevBuf d_slot, d_blk_aux, d_blk_run, d_blk_mask;
+  b200::DevBuf d_stream;             // the scans' coded stream (ScanStream, kernels.cuh)
   b200::DevBuf d_sym, d_dcq;         // sequential scans after the trellis: symbol records + dense DC values (SymOut, kernels.cuh)
   b200::DevBuf d_diff;               // lossless scans: the differences of the scan being coded (launch_lossless_diff)
   b200::Geom g;                      // the plan's geometry with this arena's coefficient pointers
+  b200::ScanStream ss;               // the buffers inside d_stream (status: the chunk's)
   void release() {
-    b200::DevBuf *db[] = {&d_planes, &d_hist, &d_tabs_trellis, &d_rec, &d_srec, &d_splits, &d_best_al, &d_qimg, &d_qsum, &d_eo, &d_es, &d_blk_bits, &d_slot, &d_tile_bits, &d_tile_base, &d_seg_corr, &d_mark, &d_stuff_lb, &d_blk_aux, &d_blk_run, &d_blk_mask, &d_total_bits, &d_bitbuf, &d_sym, &d_dcq, &d_diff};
+    b200::DevBuf *db[] = {&d_planes, &d_hist, &d_tabs_trellis, &d_rec, &d_srec, &d_splits, &d_best_al, &d_qimg, &d_qsum, &d_eo, &d_es, &d_slot, &d_blk_aux, &d_blk_run, &d_blk_mask, &d_stream, &d_sym, &d_dcq, &d_diff};
     for (b200::DevBuf *b : db) b->release();
     for (int i = 0; i < 4; i++) { d_coef[i].release(); d_raw[i].release(); d_plain[i].release(); }
   }
@@ -519,18 +521,10 @@ static int prepare_batch(b200jpeg_encoder *e, int n_total, int chunk, bool host_
       if ((rc = a.d_es.reserve((size_t)n * pl.sum_real_blocks * 16))) return rc;
     }
     if (pl.lossless) { if ((rc = a.d_diff.reserve((size_t)n * pl.max_scan_blocks * g.nc * 2))) return rc; }
-    if ((rc = a.d_blk_bits.reserve((size_t)n * pl.max_scan_blocks * 4))) return rc;
     if (use_slots(pl, p)) { if ((rc = a.d_slot.reserve((size_t)n * pl.max_scan_blocks * sizeof(SeqSlot)))) return rc; }
     if (pl.progressive) { if ((rc = a.d_blk_aux.reserve((size_t)n * pl.max_scan_blocks * 4))) return rc; if ((rc = a.d_blk_run.reserve((size_t)n * pl.max_scan_blocks * 4))) return rc; if ((rc = a.d_blk_mask.reserve((size_t)n * pl.max_scan_blocks * 24))) return rc; }
-    if ((rc = a.d_total_bits.reserve((size_t)n * 8))) return rc;
-    if ((rc = a.d_tile_bits.reserve((size_t)n * ((pl.max_scan_blocks + 255) / 256) * 4))) return rc;
-    if ((rc = a.d_tile_base.reserve((size_t)n * ((pl.max_scan_blocks + 255) / 256) * 8))) return rc;
-    if (pl.restarts) {
-      if ((rc = a.d_seg_corr.reserve((size_t)n * pl.max_scan_blocks * 4))) return rc;       // worst case: one block per segment
-      if ((rc = a.d_mark.reserve((size_t)n * (cap / 8 + 64)))) return rc;
-    }
-    if ((rc = a.d_bitbuf.reserve(cap * n))) return rc;
-    if ((rc = a.d_stuff_lb.reserve(stuff_lookback_bytes(e->bitbuf_words_per_image, n)))) return rc;
+    if ((rc = a.d_stream.reserve(scan_stream_bytes(pl.max_scan_blocks, e->bitbuf_words_per_image, pl.restarts, n)))) return rc;
+    a.ss = scan_stream_at(a.d_stream.p, pl.max_scan_blocks, e->bitbuf_words_per_image, pl.restarts, n);
   }
   // whole batch
   if (host_pixels) { if ((rc = e->d_src.reserve(src_bytes))) return rc; }
@@ -590,6 +584,22 @@ static int prepare_batch(b200jpeg_encoder *e, int n_total, int chunk, bool host_
   return B200JPEG_OK;
 }
 
+// What every scan does once its coder has counted the bits of its blocks into ss: lay the scan out, clear its stream,
+// run the coder's packer (pack), and stuff the bytes into the scan's place j in the chunk's output.
+template <class Pack>
+static void scan_tail(b200jpeg_encoder *e, const ChunkIO &io, Timer &tm, const ScanDesc &sd, const ScanStream &ss, size_t j, int si, Pack pack)
+{
+  const int n = io.n;
+  tm.mark("scan_layout");
+  launch_scan_layout(sd, ss, n, tm.s);
+  tm.mark("encode");
+  launch_zero_stream(sd, ss, n, tm.s);
+  pack();
+  tm.mark("stuff");
+  launch_stuff(sd, ss, io.out, e->out_cap_per_image, e->out_cap_per_image, io.out_pos + j * n, io.out_pos + (j + 1) * n,
+               io.scan_size + (size_t)si * n, n, tm.s);
+}
+
 // The lossless pipeline for one chunk: per scan, differences + category counts -> optimal DC tables (one set per scan,
 // finish_pass_gather, jclhuff.c:531-556) -> bits per MCU -> layout -> packing -> byte stuffing.
 static int run_lossless(b200jpeg_encoder *e, const ChunkIO &io, Timer &tm)
@@ -601,7 +611,7 @@ static int run_lossless(b200jpeg_encoder *e, const ChunkIO &io, Timer &tm)
   const int nscans = (int)pl.scans.size();
   const size_t hist_bytes = (size_t)n * HIST_SLOTS * HIST_BINS * 4;
   const size_t tabset = sizeof(DevHuff) * HIST_SLOTS, tstride = tabset * nscans;
-  const size_t mark_words = (e->bitbuf_words_per_image * 4 / 8 + 64) / 4;
+  ScanStream ss = A.ss; ss.status = io.status;
   for (size_t j = 0; j < pl.order.size(); j++) {
     const int si = pl.order[j];
     const ScanDesc &sd = pl.scans[si];
@@ -614,22 +624,8 @@ static int run_lossless(b200jpeg_encoder *e, const ChunkIO &io, Timer &tm)
     for (int i = 0; i < sd.ncomps; i++) masks.m[0] |= 1u << g.c[sd.ci[i]].dc_tbl;
     launch_gen_tables(A.d_hist.as<uint32_t>(), tset, tstride, masks, n, s);
     tm.mark("block_bits");
-    launch_lossless_bits(g, sd, A.d_diff.as<uint16_t>(), tset, tstride, A.d_blk_bits.as<uint32_t>(), A.d_tile_bits.as<uint32_t>(), io.status, n, s);
-    tm.mark("scan_layout");
-    launch_scan_layout(sd, A.d_blk_bits.as<uint32_t>(), A.d_tile_bits.as<uint32_t>(), A.d_tile_base.as<unsigned long long>(),
-                       A.d_seg_corr.as<uint32_t>(), pl.max_scan_blocks, A.d_total_bits.as<unsigned long long>(),
-                       (size_t)e->bitbuf_words_per_image * 32, io.status, n, s);
-    tm.mark("encode");
-    launch_zero_stream(A.d_bitbuf.as<uint32_t>(), e->bitbuf_words_per_image, A.d_total_bits.as<unsigned long long>(), n, s);
-    if (sd.ri) CU(cudaMemsetAsync(A.d_mark.p, 0, mark_words * 4 * n, s));
-    launch_lossless_encode(g, sd, A.d_diff.as<uint16_t>(), tset, tstride, A.d_blk_bits.as<uint32_t>(), A.d_tile_base.as<unsigned long long>(),
-                           A.d_seg_corr.as<uint32_t>(), pl.max_scan_blocks, A.d_bitbuf.as<uint32_t>(), e->bitbuf_words_per_image,
-                           A.d_mark.as<uint32_t>(), mark_words, io.status, n, s);
-    tm.mark("stuff");
-    CU(cudaMemsetAsync(A.d_stuff_lb.p, 0, stuff_lookback_bytes(e->bitbuf_words_per_image, n), s));
-    launch_stuff(A.d_bitbuf.as<uint32_t>(), e->bitbuf_words_per_image, A.d_total_bits.as<unsigned long long>(), A.d_stuff_lb.p,
-                 io.out, e->out_cap_per_image, e->out_cap_per_image, io.out_pos + j * n, io.out_pos + (j + 1) * n,
-                 io.scan_size + (size_t)si * n, io.status, sd.ri ? A.d_mark.as<uint32_t>() : nullptr, mark_words, n, s);
+    launch_lossless_bits(g, sd, A.d_diff.as<uint16_t>(), tset, tstride, ss, n, s);
+    scan_tail(e, io, tm, sd, ss, j, si, [&] { launch_lossless_encode(g, sd, A.d_diff.as<uint16_t>(), tset, tstride, ss, n, s); });
   }
   tm.mark("end");
   CU(cudaGetLastError());
@@ -764,7 +760,7 @@ static int run_pipeline(b200jpeg_encoder *e, const ChunkIO &io, Timer &tm)
         tm.mark("trellis_stats");
         CU(cudaMemsetAsync(A.d_hist.p, 0, hist_bytes, s));
         launch_seed_hist(A.d_hist.as<uint32_t>(), 4 + gr.c[ci].ac_tbl, n, s);
-        launch_prog_prepare(gr, ts, A.d_blk_aux.as<uint32_t>(), A.d_blk_run.as<uint32_t>(), A.d_blk_mask.as<unsigned long long>(), A.d_tile_bits.as<int>(), A.d_tile_base.as<int>(), n, s);
+        launch_prog_prepare(gr, ts, A.d_blk_aux.as<uint32_t>(), A.d_blk_run.as<uint32_t>(), A.d_blk_mask.as<unsigned long long>(), A.ss, n, s);
         launch_gather_prog(gr, ts, A.d_blk_aux.as<uint32_t>(), A.d_blk_run.as<uint32_t>(), A.d_blk_mask.as<unsigned long long>(), A.d_hist.as<uint32_t>(), status, n, s);
         tm.mark("trellis_tables");
         SlotMasks masks; memset(&masks, 0, sizeof masks); masks.period = 1; masks.m[0] = 1u << (4 + gr.c[ci].ac_tbl);
@@ -831,8 +827,7 @@ static int run_pipeline(b200jpeg_encoder *e, const ChunkIO &io, Timer &tm)
   //      scans are coded (the reference codes them one by one into memory buffers, jcmaster.c:668-674); the two
   //      frequency-split groups are coded at each image's best Al, chosen on the device in between. ----
   int *best_al = A.d_best_al.as<int>();                       // [2][n]: luma, chroma
-  // sequential scans after the trellis: the side records hold every block's final non-zero positions
-  const DcRec *nz_rec = (pl.trellis && !pl.progressive && !symrec) ? A.d_rec.as<DcRec>() : nullptr;
+  ScanStream ss = A.ss; ss.status = status;
   const uint8_t *sym = symrec ? A.d_sym.as<uint8_t>() : nullptr;
   const int16_t *dcq = symrec ? A.d_dcq.as<int16_t>() : nullptr;
   SeqSlot *slot = use_slots(pl, p) ? A.d_slot.as<SeqSlot>() : nullptr;
@@ -861,7 +856,7 @@ static int run_pipeline(b200jpeg_encoder *e, const ChunkIO &io, Timer &tm)
     const bool dc_refine = pl.progressive && sd.Ss == 0 && sd.Ah != 0;
     uint32_t *aux = A.d_blk_aux.as<uint32_t>(), *run_e = A.d_blk_run.as<uint32_t>();
     unsigned long long *pm = A.d_blk_mask.as<unsigned long long>();
-    if (pl.progressive && sd.Ss != 0) { tm.mark("eobrun_runs"); launch_prog_prepare(g, sd, aux, run_e, pm, A.d_tile_bits.as<int>(), A.d_tile_base.as<int>(), n, s); }
+    if (pl.progressive && sd.Ss != 0) { tm.mark("eobrun_runs"); launch_prog_prepare(g, sd, aux, run_e, pm, ss, n, s); }
     if (pl.optimize) {
       DevHuff *tset = io.tabs_scan + (size_t)si * HIST_SLOTS;                              // [img][scan][8]
       tstride = tabset * nscans;
@@ -877,28 +872,14 @@ static int run_pipeline(b200jpeg_encoder *e, const ChunkIO &io, Timer &tm)
       }
       tabs = tset;
     } else { tabs = e->d_tabs_fixed.as<DevHuff>(); tstride = 0; }
-    const size_t mark_words = (e->bitbuf_words_per_image * 4 / 8 + 64) / 4;
     tm.mark("block_bits");
-    if (pl.progressive) launch_block_bits_prog(g, sd, tabs, tstride, aux, run_e, pm, A.d_blk_bits.as<uint32_t>(), A.d_tile_bits.as<uint32_t>(), status, n, s);
-    else launch_block_bits_seq(g, sd, sym, dcq, rl, tabs, tstride, A.d_blk_bits.as<uint32_t>(), A.d_tile_bits.as<uint32_t>(), slot, status, n, s);
-    tm.mark("scan_layout");
-    launch_scan_layout(sd, A.d_blk_bits.as<uint32_t>(), A.d_tile_bits.as<uint32_t>(), A.d_tile_base.as<unsigned long long>(),
-                       A.d_seg_corr.as<uint32_t>(), pl.max_scan_blocks, A.d_total_bits.as<unsigned long long>(),
-                       (size_t)e->bitbuf_words_per_image * 32, status, n, s);
-    tm.mark("encode");
-    launch_zero_stream(A.d_bitbuf.as<uint32_t>(), e->bitbuf_words_per_image, A.d_total_bits.as<unsigned long long>(), n, s);
-    if (sd.ri) CU(cudaMemsetAsync(A.d_mark.p, 0, mark_words * 4 * n, s));
-    if (pl.progressive)
-      launch_encode_prog(g, sd, tabs, tstride, aux, run_e, pm, A.d_blk_bits.as<uint32_t>(), A.d_tile_bits.as<uint32_t>(), A.d_tile_base.as<unsigned long long>(),
-                         A.d_seg_corr.as<uint32_t>(), pl.max_scan_blocks, A.d_bitbuf.as<uint32_t>(), e->bitbuf_words_per_image, A.d_mark.as<uint32_t>(), mark_words, status, n, s);
-    else
-      launch_encode_seq(g, sd, nz_rec, sym, dcq, rl, tabs, tstride, A.d_blk_bits.as<uint32_t>(), A.d_tile_bits.as<uint32_t>(), slot, A.d_tile_base.as<unsigned long long>(),
-                        A.d_seg_corr.as<uint32_t>(), pl.max_scan_blocks, A.d_bitbuf.as<uint32_t>(), e->bitbuf_words_per_image, A.d_mark.as<uint32_t>(), mark_words, status, n, s);
-    tm.mark("stuff");
-    CU(cudaMemsetAsync(A.d_stuff_lb.p, 0, stuff_lookback_bytes(e->bitbuf_words_per_image, n), s));
-    launch_stuff(A.d_bitbuf.as<uint32_t>(), e->bitbuf_words_per_image, A.d_total_bits.as<unsigned long long>(), A.d_stuff_lb.p,
-                 io.out, e->out_cap_per_image, e->out_cap_per_image, io.out_pos + j * n, io.out_pos + (j + 1) * n,
-                 io.scan_size + (size_t)si * n, status, sd.ri ? A.d_mark.as<uint32_t>() : nullptr, mark_words, n, s);
+    if (pl.progressive) {
+      launch_block_bits_prog(g, sd, tabs, tstride, aux, run_e, pm, ss, n, s);
+      scan_tail(e, io, tm, sd, ss, j, si, [&] { launch_encode_prog(g, sd, tabs, tstride, aux, run_e, pm, ss, n, s); });
+    } else {
+      launch_block_bits_seq(g, sd, sym, dcq, rl, tabs, tstride, slot, ss, n, s);
+      scan_tail(e, io, tm, sd, ss, j, si, [&] { launch_encode_seq(g, sd, sym, dcq, rl, tabs, tstride, slot, ss, n, s); });
+    }
   }
   if (pl.search) CU(cudaMemcpyAsync(io.best_al, best_al, (size_t)n * 2 * sizeof(int), cudaMemcpyDeviceToDevice, s));   // kept per chunk for the host
   tm.mark("end");

@@ -1409,49 +1409,6 @@ __device__ __forceinline__ void walk_seq_block(const int16_t *__restrict__ blk, 
   if (r > 0) sink.ac(0, 0, 0);
 }
 
-// Zigzag positions of a scan-order block's non-zero AC coefficients, from the side records (the AC trellis leaves the
-// final ones there); dummy blocks have none.
-__device__ __forceinline__ unsigned long long block_nzmask(const Geom &g, const ScanDesc &sd, const DcRec *__restrict__ rec, const RecLayout &rl,
-                                                           int img, int sci, long long mcu, int k)
-{
-  const int ci = sd.ci[sci];
-  const CompGeom &c = g.c[ci];
-  const long long mrow = mcu / sd.per_row; const int mcol = (int)(mcu - mrow * sd.per_row);
-  const int mh = sd.ncomps == 1 ? 1 : c.v, mw = sd.ncomps == 1 ? 1 : c.h;
-  const long long row = mrow * mh + sd.k_y[k]; const int col = mcol * mw + sd.k_x[k];
-  return (row < c.hib && col < c.wib) ? rec[(size_t)img * rl.per_image + rl.comp_off[ci] + (size_t)row * c.wib + col].nzmask : 0ull;
-}
-// walk_seq_block for a block whose non-zero positions are known: touches only those coefficients.  Used by the packer
-// only: in the statistics and bit-count kernels it measured slower than the dense 16-byte loads (0.61 / 0.62 vs 0.53 /
-// 0.57 ms per 64 4K images)
-template <class Sink>
-__device__ __forceinline__ void walk_seq_sparse(const int16_t *__restrict__ blk, unsigned long long mask, int last_dc, Sink &sink)
-{
-  if (mask & 0xFFFF0000ull) asm volatile("prefetch.global.L1 [%0];" :: "l"(blk + 16));
-  if (mask & 0xFFFF00000000ull) asm volatile("prefetch.global.L1 [%0];" :: "l"(blk + 32));
-  if (mask >> 48) asm volatile("prefetch.global.L1 [%0];" :: "l"(blk + 48));
-  {
-    int temp = (int)blk[0] - last_dc, temp2 = temp;
-    if (temp < 0) { temp = -temp; temp2--; }
-    sink.dc(nbits_of(temp), temp2);
-  }
-  int prev = 0;
-  while (mask) {
-    const int pos = __ffsll((long long)mask) - 1;
-    mask &= mask - 1;
-    const int val = blk[pos];
-    if (val == 0) continue;                              // a superset mask is fine
-    int r = pos - prev - 1; prev = pos;
-    while (r > 15) { sink.ac(0xF0, 0, 0); r -= 16; }
-    int temp = val, temp2 = val;
-    if (temp < 0) { temp = -temp; temp2--; }
-    const int nb = nbits_of(temp);
-    sink.ac((r << 4) + nb, nb, temp2);
-  }
-  if (prev != 63) sink.ac(0, 0, 0);
-}
-
-
 // ---------------------------------------------------------------------
 // Sequential scans after the AC trellis: the blocks' symbols come from the records the trellis back-track left (SymOut,
 // kernels.cuh) and the DC values from the dense array the DC trellis wrote -- the 128-byte coefficient blocks are not read.
@@ -3052,7 +3009,7 @@ __device__ __forceinline__ unsigned slot_window(const uint32_t *__restrict__ s, 
 // block or a restart marker) gets this CTA's part with atomicOr, into the stream k_zero_stream cleared.  The other
 // (fallback) blocks walk their record or coefficients again, as encode_one_block (jchuff.c:563-661) does, into
 // BitSinkQ, whose atomicOr only ever lands on words that no plain store writes.
-__global__ void __launch_bounds__(256) k_encode_seq(Geom g, ScanDesc sd, const DcRec *__restrict__ rec, const uint8_t *__restrict__ sym, const int16_t *__restrict__ dcq,
+__global__ void __launch_bounds__(256) k_encode_seq(Geom g, ScanDesc sd, const uint8_t *__restrict__ sym, const int16_t *__restrict__ dcq,
                                                     RecLayout rl, const DevHuff *__restrict__ tabs, size_t stride,
                                                     const uint32_t *__restrict__ blk_bits, const uint32_t *__restrict__ tile_bits,
                                                     const SeqSlot *__restrict__ slot, const unsigned long long *__restrict__ tile_base,
@@ -3129,9 +3086,7 @@ __global__ void __launch_bounds__(256) k_encode_seq(Geom g, ScanDesc sd, const D
     else {
       int sci, k; long long mcu;
       const int16_t *blk = block_ptr(g, sd, img, t, sci, mcu, k);
-      int last = prev_dc(g, sd, img, t, sci, mcu, k);
-      if (rec) walk_seq_sparse(blk, block_nzmask(g, sd, rec, rl, img, sci, mcu, k), last, sink);
-      else walk_seq_block(blk, last, sink);
+      walk_seq_block(blk, prev_dc(g, sd, img, t, sci, mcu, k), sink);
     }
     if (sd.ri) emit_restart_marker(sink, sd, t, mark + (size_t)img * mark_stride_words);
     sink.finish();
@@ -3658,8 +3613,7 @@ __global__ void __launch_bounds__(256) k_block_bits_prog(Geom g, ScanDesc sd, co
 __global__ void __launch_bounds__(256) k_encode_prog(Geom g, ScanDesc sd, const DevHuff *__restrict__ tabs, size_t stride,
                                                      const uint32_t *__restrict__ aux, const uint32_t *__restrict__ run_e,
                                                      const unsigned long long *__restrict__ pm,
-                                                     const uint32_t *__restrict__ blk_bits, const uint32_t *__restrict__ tile_bits /* per-tile totals: not read here */,
-                                                     const unsigned long long *__restrict__ tile_base,
+                                                     const uint32_t *__restrict__ blk_bits, const unsigned long long *__restrict__ tile_base,
                                                      const uint32_t *__restrict__ seg_corr, long long seg_stride,
                                                      uint32_t *__restrict__ bitbuf, size_t bitbuf_stride_words,
                                                      uint32_t *__restrict__ mark, size_t mark_stride_words, const uint32_t *__restrict__ status)
@@ -3740,9 +3694,10 @@ void launch_select_al(const Geom &g, const AlSearch &as, const DevHuff *tabs_sca
   LAUNCHED();
 }
 
-void launch_prog_prepare(const Geom &g, const ScanDesc &sd, uint32_t *aux, uint32_t *run_e, unsigned long long *pm, int *tile_last, int *tile_first, int n, cudaStream_t s)
+void launch_prog_prepare(const Geom &g, const ScanDesc &sd, uint32_t *aux, uint32_t *run_e, unsigned long long *pm, const ScanStream &ss, int n, cudaStream_t s)
 {
   if (sd.Ss == 0) return;
+  int *tile_last = reinterpret_cast<int *>(ss.tile_bits), *tile_first = reinterpret_cast<int *>(ss.tile_base);
   dim3 grid((unsigned)((sd.nblocks + 255) / 256), n);
   k_prog_flags<<<grid, 256, 0, s>>>(g, sd, aux, run_e, pm, tile_last, tile_first); LAUNCHED();
   if (sd.Ah == 0) {
@@ -3757,26 +3712,24 @@ void launch_gather_prog(const Geom &g, const ScanDesc &sd, const uint32_t *aux, 
 }
 
 void launch_block_bits_seq(const Geom &g, const ScanDesc &sd, const uint8_t *sym, const int16_t *dcq, const RecLayout &rl, const DevHuff *tabs, size_t stride,
-                           uint32_t *blk_bits, uint32_t *tile_bits, SeqSlot *slot, uint32_t *status, int n, cudaStream_t s)
+                           SeqSlot *slot, const ScanStream &ss, int n, cudaStream_t s)
 {
   dim3 grid((unsigned)((sd.nblocks + 255) / 256), n);
-  if (slot) k_block_bits_seq<true><<<grid, 256, 0, s>>>(g, sd, sym, dcq, rl, tabs, stride, blk_bits, tile_bits, slot, status);
-  else k_block_bits_seq<false><<<grid, 256, 0, s>>>(g, sd, sym, dcq, rl, tabs, stride, blk_bits, tile_bits, nullptr, status);
+  if (slot) k_block_bits_seq<true><<<grid, 256, 0, s>>>(g, sd, sym, dcq, rl, tabs, stride, ss.blk_bits, ss.tile_bits, slot, ss.status);
+  else k_block_bits_seq<false><<<grid, 256, 0, s>>>(g, sd, sym, dcq, rl, tabs, stride, ss.blk_bits, ss.tile_bits, nullptr, ss.status);
   LAUNCHED();
 }
 void launch_block_bits_prog(const Geom &g, const ScanDesc &sd, const DevHuff *tabs, size_t stride, const uint32_t *blk_aux, const uint32_t *run_e, const unsigned long long *pm,
-                            uint32_t *blk_bits, uint32_t *tile_bits, uint32_t *status, int n, cudaStream_t s)
+                            const ScanStream &ss, int n, cudaStream_t s)
 {
   dim3 grid((unsigned)((sd.nblocks + 255) / 256), n);
-  k_block_bits_prog<<<grid, 256, 0, s>>>(g, sd, tabs, stride, blk_aux, run_e, pm, blk_bits, tile_bits, status);
+  k_block_bits_prog<<<grid, 256, 0, s>>>(g, sd, tabs, stride, blk_aux, run_e, pm, ss.blk_bits, ss.tile_bits, ss.status);
   LAUNCHED();
 }
-void launch_scan_layout(const ScanDesc &sd, const uint32_t *blk_bits, const uint32_t *tile_bits, unsigned long long *tile_base,
-                        uint32_t *seg_corr, long long seg_stride, unsigned long long *total_bits, size_t capacity_bits,
-                        uint32_t *status, int n, cudaStream_t s)
+void launch_scan_layout(const ScanDesc &sd, const ScanStream &ss, int n, cudaStream_t s)
 {
   const int ntiles = (int)((sd.nblocks + 255) / 256);
-  k_scan_layout<<<n, 256, 0, s>>>(sd, blk_bits, tile_bits, ntiles, tile_base, seg_corr, seg_stride, total_bits, capacity_bits, status);
+  k_scan_layout<<<n, 256, 0, s>>>(sd, ss.blk_bits, ss.tile_bits, ntiles, ss.tile_base, ss.seg_corr, ss.seg_stride, ss.total_bits, ss.bitbuf_words * 32, ss.status);
   LAUNCHED();
 }
 // the packers OR their bits into a zeroed word stream: only the words the scan will occupy (total_bits is known since
@@ -3793,25 +3746,26 @@ __global__ void __launch_bounds__(256) k_zero_stream(uint32_t *__restrict__ bitb
     if (q < need && q < stride4) dst[q] = make_uint4(0, 0, 0, 0);
   }
 }
-void launch_zero_stream(uint32_t *bitbuf, size_t stride_words, const unsigned long long *total_bits, int n, cudaStream_t s)
+void launch_zero_stream(const ScanDesc &sd, const ScanStream &ss, int n, cudaStream_t s)
 {
-  dim3 grid((unsigned)((stride_words / 4 + 1023) / 1024), n);
-  k_zero_stream<<<grid, 256, 0, s>>>(bitbuf, stride_words, total_bits); LAUNCHED();
+  dim3 grid((unsigned)((ss.bitbuf_words / 4 + 1023) / 1024), n);
+  k_zero_stream<<<grid, 256, 0, s>>>(ss.bitbuf, ss.bitbuf_words, ss.total_bits); LAUNCHED();
+  if (sd.ri) cudaMemsetAsync(ss.mark, 0, ss.mark_words * 4 * n, s);
 }
-void launch_encode_seq(const Geom &g, const ScanDesc &sd, const DcRec *nz_rec, const uint8_t *sym, const int16_t *dcq, const RecLayout &rl, const DevHuff *tabs, size_t stride,
-                       const uint32_t *blk_bits, const uint32_t *tile_bits, const SeqSlot *slot, const unsigned long long *tile_base, const uint32_t *seg_corr, long long seg_stride,
-                       uint32_t *bitbuf, size_t bitbuf_stride_words, uint32_t *mark, size_t mark_stride_words, const uint32_t *status, int n, cudaStream_t s)
+void launch_encode_seq(const Geom &g, const ScanDesc &sd, const uint8_t *sym, const int16_t *dcq, const RecLayout &rl, const DevHuff *tabs, size_t stride,
+                       const SeqSlot *slot, const ScanStream &ss, int n, cudaStream_t s)
 {
   dim3 grid((unsigned)((sd.nblocks + 255) / 256), n);
-  k_encode_seq<<<grid, 256, 0, s>>>(g, sd, nz_rec, sym, dcq, rl, tabs, stride, blk_bits, tile_bits, slot, tile_base, seg_corr, seg_stride, bitbuf, bitbuf_stride_words, mark, mark_stride_words, status);
+  k_encode_seq<<<grid, 256, 0, s>>>(g, sd, sym, dcq, rl, tabs, stride, ss.blk_bits, ss.tile_bits, slot, ss.tile_base, ss.seg_corr, ss.seg_stride,
+                                    ss.bitbuf, ss.bitbuf_words, ss.mark, ss.mark_words, ss.status);
   LAUNCHED();
 }
 void launch_encode_prog(const Geom &g, const ScanDesc &sd, const DevHuff *tabs, size_t stride, const uint32_t *blk_aux, const uint32_t *run_e, const unsigned long long *pm,
-                        const uint32_t *blk_bits, const uint32_t *tile_bits, const unsigned long long *tile_base, const uint32_t *seg_corr, long long seg_stride,
-                        uint32_t *bitbuf, size_t bitbuf_stride_words, uint32_t *mark, size_t mark_stride_words, const uint32_t *status, int n, cudaStream_t s)
+                        const ScanStream &ss, int n, cudaStream_t s)
 {
   dim3 grid((unsigned)((sd.nblocks + 255) / 256), n);
-  k_encode_prog<<<grid, 256, 0, s>>>(g, sd, tabs, stride, blk_aux, run_e, pm, blk_bits, tile_bits, tile_base, seg_corr, seg_stride, bitbuf, bitbuf_stride_words, mark, mark_stride_words, status);
+  k_encode_prog<<<grid, 256, 0, s>>>(g, sd, tabs, stride, blk_aux, run_e, pm, ss.blk_bits, ss.tile_base, ss.seg_corr, ss.seg_stride,
+                                     ss.bitbuf, ss.bitbuf_words, ss.mark, ss.mark_words, ss.status);
   LAUNCHED();
 }
 // =====================================================================
@@ -3973,32 +3927,66 @@ void launch_lossless_diff(const Geom &g, const ScanDesc &sd, int precision, cons
   LAUNCHED();
 }
 void launch_lossless_bits(const Geom &g, const ScanDesc &sd, const uint16_t *diff, const DevHuff *tabs, size_t stride,
-                          uint32_t *blk_bits, uint32_t *tile_bits, uint32_t *status, int n, cudaStream_t s)
+                          const ScanStream &ss, int n, cudaStream_t s)
 {
   dim3 grid((unsigned)(((long long)g.W * g.H + 255) / 256), n);
-  k_lossless_bits<<<grid, 256, 0, s>>>(g, sd, diff, tabs, stride, blk_bits, tile_bits, status);
+  k_lossless_bits<<<grid, 256, 0, s>>>(g, sd, diff, tabs, stride, ss.blk_bits, ss.tile_bits, ss.status);
   LAUNCHED();
 }
 void launch_lossless_encode(const Geom &g, const ScanDesc &sd, const uint16_t *diff, const DevHuff *tabs, size_t stride,
-                            const uint32_t *blk_bits, const unsigned long long *tile_base, const uint32_t *seg_corr, long long seg_stride,
-                            uint32_t *bitbuf, size_t bitbuf_stride_words, uint32_t *mark, size_t mark_stride_words, const uint32_t *status, int n, cudaStream_t s)
+                            const ScanStream &ss, int n, cudaStream_t s)
 {
   dim3 grid((unsigned)(((long long)g.W * g.H + 255) / 256), n);
-  k_lossless_encode<<<grid, 256, 0, s>>>(g, sd, diff, tabs, stride, blk_bits, tile_base, seg_corr, seg_stride, bitbuf, bitbuf_stride_words, mark, mark_stride_words, status);
+  k_lossless_encode<<<grid, 256, 0, s>>>(g, sd, diff, tabs, stride, ss.blk_bits, ss.tile_base, ss.seg_corr, ss.seg_stride,
+                                         ss.bitbuf, ss.bitbuf_words, ss.mark, ss.mark_words, ss.status);
   LAUNCHED();
 }
 
-size_t stuff_tiles(size_t bitbuf_stride_words) { return (bitbuf_stride_words + STUFF_TILE_WORDS - 1) / STUFF_TILE_WORDS; }
-size_t stuff_lookback_bytes(size_t bitbuf_stride_words, int n) { return (size_t)n * 8 + (size_t)n * stuff_tiles(bitbuf_stride_words) * 8; }
-void launch_stuff(const uint32_t *bitbuf, size_t bitbuf_stride_words, const unsigned long long *total_bits, void *lookback,
-                  uint8_t *out, size_t out_stride, size_t out_capacity, const unsigned long long *out_start, unsigned long long *out_next,
-                  uint32_t *scan_size, uint32_t *status, const uint32_t *mark, size_t mark_stride_words, int n, cudaStream_t s)
+static size_t stuff_tiles(size_t bitbuf_words) { return (bitbuf_words + STUFF_TILE_WORDS - 1) / STUFF_TILE_WORDS; }
+void launch_stuff(const ScanDesc &sd, const ScanStream &ss, uint8_t *out, size_t out_stride, size_t out_capacity,
+                  const unsigned long long *out_start, unsigned long long *out_next, uint32_t *scan_size, int n, cudaStream_t s)
 {
-  dim3 grid((unsigned)stuff_tiles(bitbuf_stride_words), n);
-  unsigned long long *desc = static_cast<unsigned long long *>(lookback);
+  dim3 grid((unsigned)stuff_tiles(ss.bitbuf_words), n);
+  unsigned long long *desc = static_cast<unsigned long long *>(ss.lookback);
   uint32_t *ticket = reinterpret_cast<uint32_t *>(desc + (size_t)n * grid.x);
-  k_stuff<<<grid, STUFF_THREADS, 0, s>>>(bitbuf, bitbuf_stride_words, total_bits, desc, ticket, out, out_stride, out_capacity, out_start, out_next, scan_size, status, mark, mark_stride_words);
+  cudaMemsetAsync(ss.lookback, 0, (size_t)n * (grid.x + 1) * 8, s);
+  k_stuff<<<grid, STUFF_THREADS, 0, s>>>(ss.bitbuf, ss.bitbuf_words, ss.total_bits, desc, ticket, out, out_stride, out_capacity, out_start, out_next, scan_size,
+                                         ss.status, sd.ri ? ss.mark : nullptr, ss.mark_words);
   LAUNCHED();
+}
+
+// The ScanStream's buffers one after the other, each on a 256-byte boundary (bitbuf is read in 16-byte pieces), and
+// their total size in `bytes`; base == nullptr: the size only
+static ScanStream scan_stream_carve(char *base, long long max_scan_blocks, size_t bitbuf_words, bool restarts, int n, size_t &bytes)
+{
+  const size_t blocks = (size_t)n * max_scan_blocks, tiles = (size_t)n * ((max_scan_blocks + 255) / 256);
+  bytes = 0;
+  auto take = [&](size_t b) { const size_t at = bytes; bytes += (b + 255) & ~(size_t)255; return base ? base + at : nullptr; };
+  ScanStream ss;
+  ss.blk_bits = reinterpret_cast<uint32_t *>(take(blocks * 4));
+  ss.tile_bits = reinterpret_cast<uint32_t *>(take(tiles * 4));
+  ss.tile_base = reinterpret_cast<unsigned long long *>(take(tiles * 8));
+  ss.seg_stride = max_scan_blocks;                                                  // worst case: one block per segment
+  ss.seg_corr = restarts ? reinterpret_cast<uint32_t *>(take(blocks * 4)) : nullptr;
+  ss.total_bits = reinterpret_cast<unsigned long long *>(take((size_t)n * 8));
+  ss.bitbuf_words = bitbuf_words;
+  ss.bitbuf = reinterpret_cast<uint32_t *>(take((size_t)n * bitbuf_words * 4));
+  ss.mark_words = bitbuf_words / 8 + 16;                                            // a bit per stream byte, and 64 bytes
+  ss.mark = restarts ? reinterpret_cast<uint32_t *>(take((size_t)n * ss.mark_words * 4)) : nullptr;
+  ss.lookback = take((size_t)n * (stuff_tiles(bitbuf_words) + 1) * 8);             // launch_stuff's descriptors + tickets
+  ss.status = nullptr;
+  return ss;
+}
+size_t scan_stream_bytes(long long max_scan_blocks, size_t bitbuf_words, bool restarts, int n)
+{
+  size_t bytes;
+  scan_stream_carve(nullptr, max_scan_blocks, bitbuf_words, restarts, n, bytes);
+  return bytes;
+}
+ScanStream scan_stream_at(void *base, long long max_scan_blocks, size_t bitbuf_words, bool restarts, int n)
+{
+  size_t bytes;
+  return scan_stream_carve(static_cast<char *>(base), max_scan_blocks, bitbuf_words, restarts, n, bytes);
 }
 
 }  // namespace b200

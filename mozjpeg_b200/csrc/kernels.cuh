@@ -194,56 +194,77 @@ void launch_trellis_dc(const Geom &g, const TrellisConsts *tc, const DevHuff *ta
 // DC statistics of a sequential scan from the dense DC array (+ the EOB of every dummy block): with the AC counts the
 // trellis back-track left in `hist`, the scan's complete statistics (encode_mcu_gather, jchuff.c:886-915)
 void launch_gather_seq_dc(const Geom &g, const ScanDesc &sd, const int16_t *dcq, const RecLayout &rl, uint32_t *hist, uint32_t *status, int n, cudaStream_t s);
-// tile_last / tile_first: int [n][ceil(nblocks/256)] scratch; pm: the blocks' event masks of this AC scan,
-// unsigned long long [3][n][nblocks] (written here, read by the three symbol walks of the scan)
-void launch_prog_prepare(const Geom &g, const ScanDesc &sd, uint32_t *aux, uint32_t *run_e, unsigned long long *pm, int *tile_last, int *tile_first, int n, cudaStream_t s);
+// The coded stream of one scan: the buffers the three scan coders (sequential, progressive, lossless) share, indexed
+// by the image inside the launch.  Every scan runs its coder's bit-count launch (launch_block_bits_seq / _prog,
+// launch_lossless_bits), then launch_scan_layout, launch_zero_stream, its coder's packer (launch_encode_seq / _prog,
+// launch_lossless_encode) and launch_stuff.  A tile is the 256 blocks (lossless: MCUs) of one bit-count / packer CTA.
+//   blk_bits   [n][sd.nblocks]    bits the tile's blocks before block t emit (exclusive prefix inside the tile)
+//   tile_bits  [n][tiles]         bits each tile emits (tiles = ceil(sd.nblocks / 256))
+//   tile_base  [n][tiles]         bits the scan emits before each tile
+//   seg_corr   [n][seg_stride]    restart intervals only: padding + marker bits inserted before each restart segment
+//   total_bits [n]                bits of the whole unstuffed scan
+//   bitbuf     [n][bitbuf_words]  the unstuffed big-endian bit stream
+//   mark       [n][mark_words]    restart intervals only: bitmap over bitbuf's bytes, bit set = the 0xFF of a restart
+//                                 marker (not stuffed)
+//   lookback                      the stuffer's look-back state: a 64-bit descriptor per 4096-byte tile of bitbuf and a
+//                                 ticket per image
+//   status     [n]                bits 2 (bad coefficient / missing Huffman code) and 4 (bitbuf too small, the host
+//                                 retries) make the packers and the stuffer skip the image
+struct ScanStream {
+  uint32_t *blk_bits, *tile_bits; unsigned long long *tile_base;
+  uint32_t *seg_corr; long long seg_stride;
+  unsigned long long *total_bits;
+  uint32_t *bitbuf; size_t bitbuf_words;
+  uint32_t *mark; size_t mark_words;
+  void *lookback;
+  uint32_t *status;
+};
+// One device allocation of scan_stream_bytes() holds the ScanStream of up to n images whose scans have at most
+// max_scan_blocks blocks and bitbuf_words stream words each (seg_corr and mark only with restarts); scan_stream_at lays
+// its buffers out from base, status left to the caller.
+size_t scan_stream_bytes(long long max_scan_blocks, size_t bitbuf_words, bool restarts, int n);
+ScanStream scan_stream_at(void *base, long long max_scan_blocks, size_t bitbuf_words, bool restarts, int n);
+
+// pm: the blocks' event masks of this AC scan, unsigned long long [3][n][nblocks] (written here, read by the three symbol
+// walks of the scan); ss.tile_bits and ss.tile_base serve as int [n][tiles] scratch
+void launch_prog_prepare(const Geom &g, const ScanDesc &sd, uint32_t *aux, uint32_t *run_e, unsigned long long *pm, const ScanStream &ss, int n, cudaStream_t s);
 void launch_gather_prog(const Geom &g, const ScanDesc &sd, const uint32_t *aux, const uint32_t *run_e, const unsigned long long *pm, uint32_t *hist, uint32_t *status, int n, cudaStream_t s);
 // Code slots of the sequential scans: k_block_bits_seq stores the bit string of every block of at most 128 bits
 // (code and value bits, left-aligned), k_encode_seq copies it into the stream.  One slot per scan block,
 // [n][max_scan_blocks].  (H100, cfg2 and cfg4 q90: DESIGN §3 has the bits-per-block histogram the width comes from.)
 #define SEQ_SLOT_WORDS 4
 typedef uint4 SeqSlot;
-// slot (here and in launch_encode_seq): the code slots of a sequential scan, or nullptr: every block is walked again by
-// the packer
+// The stages of a scan's coded stream (ScanStream above).  Bit counts: ss.blk_bits, ss.tile_bits (and the slots, given
+// one) from the blocks; slot (here and in launch_encode_seq): the code slots of a sequential scan, or nullptr: every
+// block is walked again by the packer
 void launch_block_bits_seq(const Geom &g, const ScanDesc &sd, const uint8_t *sym, const int16_t *dcq, const RecLayout &rl, const DevHuff *tabs, size_t tabs_image_stride,
-                           uint32_t *blk_bits, uint32_t *tile_bits, SeqSlot *slot, uint32_t *status, int n, cudaStream_t s);
+                           SeqSlot *slot, const ScanStream &ss, int n, cudaStream_t s);
 void launch_block_bits_prog(const Geom &g, const ScanDesc &sd, const DevHuff *tabs, size_t tabs_image_stride, const uint32_t *blk_aux, const uint32_t *run_e, const unsigned long long *pm,
-                            uint32_t *blk_bits, uint32_t *tile_bits, uint32_t *status, int n, cudaStream_t s);
-// tile_base[img][tile] / seg_corr[img][segment] / total_bits[img] from the tile sums (and the restart interval)
-void launch_scan_layout(const ScanDesc &sd, const uint32_t *blk_bits, const uint32_t *tile_bits, unsigned long long *tile_base,
-                        uint32_t *seg_corr, long long seg_stride, unsigned long long *total_bits, size_t capacity_bits,
-                        uint32_t *status, int n, cudaStream_t s);
-// clears the part of every image's word stream that the scan laid out by launch_scan_layout will occupy
-void launch_zero_stream(uint32_t *bitbuf, size_t bitbuf_image_stride_words, const unsigned long long *total_bits, int n, cudaStream_t s);
-// mark (here and in launch_encode_prog): bitmap over the unstuffed bytes of each image (restart markers' 0xFF), only
-// touched when sd.ri != 0
-// nz_rec: the side records holding every block's final non-zero positions (trellis on, no symbol records), or nullptr:
-// the fallback blocks' walk then touches only those coefficients
-void launch_encode_seq(const Geom &g, const ScanDesc &sd, const DcRec *nz_rec, const uint8_t *sym, const int16_t *dcq, const RecLayout &rl, const DevHuff *tabs, size_t tabs_image_stride,
-                       const uint32_t *blk_bits, const uint32_t *tile_bits, const SeqSlot *slot, const unsigned long long *tile_base, const uint32_t *seg_corr, long long seg_stride,
-                       uint32_t *bitbuf, size_t bitbuf_image_stride_words, uint32_t *mark, size_t mark_stride_words, const uint32_t *status, int n, cudaStream_t s);
+                            const ScanStream &ss, int n, cudaStream_t s);
+// ss.tile_base, ss.seg_corr, ss.total_bits from the bit counts (and the restart interval); flags a scan that does not
+// fit in bitbuf
+void launch_scan_layout(const ScanDesc &sd, const ScanStream &ss, int n, cudaStream_t s);
+// clears the part of every image's bitbuf that the scan will occupy, and the marker bitmap when sd.ri != 0
+void launch_zero_stream(const ScanDesc &sd, const ScanStream &ss, int n, cudaStream_t s);
+// packers: every block's bits into ss.bitbuf at its offset, restart markers into ss.mark
+void launch_encode_seq(const Geom &g, const ScanDesc &sd, const uint8_t *sym, const int16_t *dcq, const RecLayout &rl, const DevHuff *tabs, size_t tabs_image_stride,
+                       const SeqSlot *slot, const ScanStream &ss, int n, cudaStream_t s);
 void launch_encode_prog(const Geom &g, const ScanDesc &sd, const DevHuff *tabs, size_t tabs_image_stride, const uint32_t *blk_aux, const uint32_t *run_e, const unsigned long long *pm,
-                        const uint32_t *blk_bits, const uint32_t *tile_bits, const unsigned long long *tile_base, const uint32_t *seg_corr, long long seg_stride,
-                        uint32_t *bitbuf, size_t bitbuf_image_stride_words, uint32_t *mark, size_t mark_stride_words, const uint32_t *status, int n, cudaStream_t s);
-// byte stuffing of every scan in one pass with a decoupled look-back (k_stuff): out[img][out_start[img] ...], scan_size,
-// out_next.  lookback: stuff_lookback_bytes() of look-back state (a descriptor per tile, a ticket per image), all zero
-// before each launch.
-size_t stuff_tiles(size_t bitbuf_image_stride_words);
-size_t stuff_lookback_bytes(size_t bitbuf_image_stride_words, int n);
-void launch_stuff(const uint32_t *bitbuf, size_t bitbuf_image_stride_words, const unsigned long long *total_bits, void *lookback,
-                  uint8_t *out, size_t out_image_stride, size_t out_capacity, const unsigned long long *out_start, unsigned long long *out_next,
-                  uint32_t *scan_size, uint32_t *status, const uint32_t *mark, size_t mark_stride_words, int n, cudaStream_t s);
+                        const ScanStream &ss, int n, cudaStream_t s);
+// byte stuffing of every scan in one pass with a decoupled look-back (k_stuff), after clearing ss.lookback:
+// out[img][out_start[img] ...], scan_size, out_next
+void launch_stuff(const ScanDesc &sd, const ScanStream &ss, uint8_t *out, size_t out_image_stride, size_t out_capacity,
+                  const unsigned long long *out_start, unsigned long long *out_next, uint32_t *scan_size, int n, cudaStream_t s);
 
 // lossless (SOF3) scans: sd.ncomps components of one sample per MCU, sd.nblocks = W*H MCUs, sd.Ss the predictor, sd.Al
 // the point transform, sd.ri the restart interval in MCUs (whole rows).  diff: [n][sd.ncomps][W*H] uint16 differences
-// (mod 2^16); hist: the categories per DC table, [img][HIST_SLOTS][HIST_BINS] (zeroed by the caller).  The bit counts,
-// layout, packing and stuffing follow the sequential scans' stages (launch_scan_layout, launch_zero_stream, launch_stuff).
+// (mod 2^16); hist: the categories per DC table, [img][HIST_SLOTS][HIST_BINS] (zeroed by the caller).  The bit counts
+// and the packer write the scan's ScanStream like the sequential scans' stages.
 void launch_lossless_diff(const Geom &g, const ScanDesc &sd, int precision, const uint8_t *src, uint16_t *diff, uint32_t *hist, int n, cudaStream_t s);
 void launch_lossless_bits(const Geom &g, const ScanDesc &sd, const uint16_t *diff, const DevHuff *tabs, size_t tabs_image_stride,
-                          uint32_t *blk_bits, uint32_t *tile_bits, uint32_t *status, int n, cudaStream_t s);
+                          const ScanStream &ss, int n, cudaStream_t s);
 void launch_lossless_encode(const Geom &g, const ScanDesc &sd, const uint16_t *diff, const DevHuff *tabs, size_t tabs_image_stride,
-                            const uint32_t *blk_bits, const unsigned long long *tile_base, const uint32_t *seg_corr, long long seg_stride,
-                            uint32_t *bitbuf, size_t bitbuf_image_stride_words, uint32_t *mark, size_t mark_stride_words, const uint32_t *status, int n, cudaStream_t s);
+                            const ScanStream &ss, int n, cudaStream_t s);
 
 // scan search: per-image best point transform of one Al-search group (see k_select_al)
 struct AlSearch { ScanDesc sd[24]; int first, per_al, nband, al_max, nscans_total; };

@@ -601,7 +601,7 @@ def noise_ramps(seed, w, h):
 
 
 # (id, seed, width, height, gray, quality, walk, restart): walk "symrec" (default trellis), "loops", "scans_in_trellis",
-# "q_opt", "eob_opt" (generic trellis rounds: the sparse walk) or "notrellis" (dense planes)
+# "q_opt", "eob_opt" (generic trellis rounds: final coefficient planes) or "notrellis" (plain-quantized planes)
 PIXEL_CASES = [
     ("gray_q95_symrec", 3, 256, 136, True, 95, "symrec", None),
     ("gray_q100_symrec_rst", 4, 256, 96, True, 100, "symrec", "4B"),
@@ -639,7 +639,7 @@ def pixel_image(pid):
 
 def pixel_walk(pid):
     walk = PIXEL[pid][6]
-    return {"symrec": "symrec", "notrellis": "dense"}.get(walk, "sparse")
+    return {"symrec": "symrec", "notrellis": "dense"}.get(walk, "generic_rounds")
 
 
 @functools.lru_cache(maxsize=None)
@@ -661,7 +661,7 @@ WALK_CLASSES = {
     "dense": set(ALL_CLASSES),
     "dense12": set(TWELVE_CLASSES),
     "symrec": _PIXEL_REACHED,
-    "sparse": _PIXEL_REACHED | {"rst_1block_segments", "tile_256_fb"},
+    "generic_rounds": _PIXEL_REACHED | {"rst_1block_segments", "tile_256_fb"},
 }
 
 
