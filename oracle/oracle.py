@@ -289,6 +289,35 @@ def ref_read_coefs(jpeg: bytes) -> Dict[str, object]:
     return {"coefs": arrs, "qt": np.array(qt, dtype=np.uint16).reshape(4, 64)[:nc.value]}
 
 
+_refshim_tree = None
+
+
+def ref_read_coefs_warn(jpeg: bytes):
+    """jpeg_read_coefficients via the reference decoder, with its warnings counted: (planes or None where the
+    reference stops with an error, warnings emitted).  Runs build/librefshim.so, which build() compiles from this
+    tree's refshim.c against the reference library (oracle/_ref/ can hold a driver built from an older refshim.c)."""
+    global _refshim_tree
+    if _refshim_tree is None:
+        path = os.path.join(_ROOT, "build", "librefshim.so")
+        if not os.path.exists(path):
+            raise RuntimeError("build/librefshim.so is missing: run build() where oracle/_ref is built")
+        _refshim_tree = C.CDLL(path)
+    fn = _refshim_tree.refshim_read_coefs_warn
+    fn.argtypes = [C.c_char_p, C.c_ulong, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_uint16),
+                   C.POINTER(C.POINTER(C.c_int16)), C.POINTER(C.c_int)]
+    fn.restype = C.c_int
+    nc = C.c_int(0); wib = (C.c_int * 4)(); hib = (C.c_int * 4)(); warn = C.c_int(0)
+    if fn(jpeg, len(jpeg), C.byref(nc), wib, hib, None, None, C.byref(warn)) != 0:
+        return None, warn.value
+    arrs = [np.zeros((hib[i], wib[i], 64), dtype=np.int16) for i in range(nc.value)]
+    ptrs = (C.POINTER(C.c_int16) * 4)()
+    for i, a in enumerate(arrs):
+        ptrs[i] = a.ctypes.data_as(C.POINTER(C.c_int16))
+    if fn(jpeg, len(jpeg), C.byref(nc), wib, hib, None, ptrs, C.byref(warn)) != 0:
+        return None, warn.value
+    return arrs, warn.value
+
+
 def _ref_cjpeg_pixels(pixels: np.ndarray, switches: Sequence[str]) -> bytes:
     """The reference's cjpeg binary on an in-memory 8-bit image (written out as a PGM/PPM first)."""
     import tempfile

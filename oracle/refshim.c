@@ -271,6 +271,49 @@ int refshim_read_coefs(const unsigned char *jpg, unsigned long size, int *ncomp,
   return 0;
 }
 
+/*
+ * refshim_read_coefs with the number of warnings the reference emitted on the way (corrupt data it decoded anyway:
+ * premature end of a segment, an invalid Huffman code, extraneous bytes before a marker, ...) in *warnings.  Returns
+ * -1 where the reference stops with an error; *warnings then counts the warnings before it.
+ */
+static int warn_count;
+static void count_emit(j_common_ptr c, int lvl) { (void)c; if (lvl < 0) warn_count++; }
+
+int refshim_read_coefs_warn(const unsigned char *jpg, unsigned long size, int *ncomp,
+                            int *wib, int *hib, unsigned short *qt, short **coefs, int *warnings)
+{
+  struct jpeg_decompress_struct d;
+  struct my_err jerr;
+  jvirt_barray_ptr *arrs;
+  int ci;
+  warn_count = 0;
+  d.err = jpeg_std_error(&jerr.pub);
+  jerr.pub.error_exit = my_exit;
+  jerr.pub.emit_message = count_emit;
+  if (setjmp(jerr.jb)) { jpeg_destroy_decompress(&d); *warnings = warn_count; return -1; }
+  jpeg_create_decompress(&d);
+  jpeg_mem_src(&d, jpg, size);
+  jpeg_read_header(&d, TRUE);
+  arrs = jpeg_read_coefficients(&d);
+  *ncomp = d.num_components;
+  for (ci = 0; ci < d.num_components; ci++) {
+    jpeg_component_info *c = &d.comp_info[ci];
+    int r, i;
+    wib[ci] = c->width_in_blocks; hib[ci] = c->height_in_blocks;
+    if (qt && c->quant_table) for (i = 0; i < 64; i++) qt[ci * 64 + i] = c->quant_table->quantval[i];
+    if (coefs && coefs[ci]) {
+      for (r = 0; r < (int)c->height_in_blocks; r++) {
+        JBLOCKARRAY b = (*d.mem->access_virt_barray)((j_common_ptr)&d, arrs[ci], r, 1, FALSE);
+        memcpy(coefs[ci] + (size_t)r * c->width_in_blocks * 64, b[0], (size_t)c->width_in_blocks * 64 * sizeof(short));
+      }
+    }
+  }
+  jpeg_finish_decompress(&d);
+  jpeg_destroy_decompress(&d);
+  *warnings = warn_count;
+  return 0;
+}
+
 /* Direct access to reference internals used as per-stage oracles. */
 extern void jpeg_fdct_islow(int *data);
 void refshim_fdct_islow(int *data) { jpeg_fdct_islow(data); }
