@@ -549,6 +549,37 @@ int  b200jpeg_recompress_renditions(b200jpeg_encoder *enc, int n_renditions, con
                                     const b200jpeg_params *params,
                                     const uint8_t *const *files, const size_t *sizes, int n_images);
 
+/*
+ * Batches of mixed geometry: the rendition calls without the one-geometry rule.  Size, sampling layout, colour space,
+ * component count (1 or 3), tables, restart intervals and sequential / progressive coding may differ from file to file;
+ * each file must pass the single calls' source checks.  Image i of rung r is byte for byte what
+ * b200jpeg_decompress_batch_opts(opts[r]) makes of that file alone, and for the recompress what
+ * b200jpeg_recompress_batch_opts(opts[r], params[r * n_images + i]) makes (with its COM / APPn segments).  Each output's
+ * size is b200jpeg_decompress_output_opts of its own source.
+ *
+ * The files are decoded in chunks of about 1.6 M blocks, whole images in input order (an image larger than that is a
+ * chunk of its own; b200jpeg_encoder_set_chunk_images sets an image count instead).  A chunk costs one entropy decode
+ * and, per distinct option set, one IDCT launch per component slot and IDCT size present and one upsampling / colour
+ * conversion launch, however many geometries it holds.
+ *
+ * b200jpeg_decompress_mixed writes image i of rung r to pixels[r * n_images + i], rows row_pitch[r * n_images + i]
+ *   apart, in host or device memory (pixels_on_device).
+ * b200jpeg_recompress_mixed encodes image i of rung r with params[r * n_images + i]; the images of one rung whose
+ *   parameter blocks are identical are encoded together.  Its file is b200jpeg_get_output(enc, r * n_images + i).
+ *
+ * Refusals come before any device work, write no output, leave the encoder usable and keep the single calls' codes:
+ * source problems "image i: ...", a rung's options refused for image 0 "rendition r: ...", for a later image
+ * "rendition r, image i: ...", and a parameter block that fails b200jpeg_validate or does not describe image i's
+ * decoded size, colour space and components "rendition r, image i: ...".  HBM: as the rendition calls, with each
+ * distinct option set's whole batch of pixels.
+ */
+int  b200jpeg_decompress_mixed(b200jpeg_encoder *enc, int n_renditions, const b200jpeg_decompress_options *opts,
+                               const uint8_t *const *files, const size_t *sizes, int n_images,
+                               void *const *pixels, int pixels_on_device, const size_t *row_pitch);
+int  b200jpeg_recompress_mixed(b200jpeg_encoder *enc, int n_renditions, const b200jpeg_decompress_options *opts,
+                               const b200jpeg_params *params,
+                               const uint8_t *const *files, const size_t *sizes, int n_images);
+
 /* b200jpeg_encode_batch, but stops after the entropy-coded bytes are in HBM: no device->host
  * copy, no host-side file assembly.  Used to time the device pipeline alone. */
 int  b200jpeg_encode_batch_device_only(b200jpeg_encoder *enc, const b200jpeg_params *p,

@@ -294,6 +294,95 @@ class Encoder:
         A.check(_lib.b200jpeg_recompress_renditions(self._h, k, opts, params, ptrs, sizes, n), "recompress_renditions")
         return [[self.get_output(r * n + i) for i in range(n)] for r in range(k)]
 
+    # -- batches of mixed geometry ---------------------------------------------------------------------------------
+    @staticmethod
+    def _mixed_shapes(bufs, renditions):
+        """[r][i]: (width, height, components) of file i decoded with rung r's options, None where the library will refuse
+        the file or the options (the call then gets no buffer there and returns the library's own refusal)"""
+        out = [[None] * len(bufs) for _ in renditions]
+        for i, b in enumerate(bufs):
+            info = A.SourceInfo()
+            if _lib.b200jpeg_parse_source(b, len(b), C.byref(info)):
+                continue
+            for r, kw in enumerate(renditions):
+                try:
+                    w, h, _, nc = decompress_output(info, **kw)
+                    out[r][i] = (w, h, nc)
+                except B200JpegError:
+                    pass
+        return out
+
+    def decompress_mixed(self, files: Sequence[bytes], renditions: Optional[Sequence[dict]] = None) -> List[List[np.ndarray]]:
+        """b200jpeg_decompress_mixed: files of any mix of sizes, sampling layouts, colour spaces, gray and colour,
+        sequential and progressive, decoded in one call and rendered with each option dict of ``renditions``
+        (decompress's keywords; None is one rung of a default decompress object).  Returns out[r][i], what
+        decompress([files[i]], **renditions[r])[0] returns: an (H, W, C) uint8 array, (H, W) for one output component."""
+        renditions = [{}] if renditions is None else list(renditions)
+        opts = self._rendition_options(renditions)
+        bufs, ptrs, sizes = self._files(files)
+        n, k = len(bufs), len(renditions)
+        outs = [[None if s is None else np.empty((s[1], s[0], s[2]), np.uint8) for s in row] for row in self._mixed_shapes(bufs, renditions)]
+        flat = [o for row in outs for o in row]
+        A.check(_lib.b200jpeg_decompress_mixed(self._h, k, opts, ptrs, sizes, n, (C.c_void_p * (k * n))(*[None if o is None else o.ctypes.data for o in flat]), 0,
+                                               (C.c_size_t * (k * n))(*[0 if o is None else o.strides[0] for o in flat])), "decompress_mixed")
+        return [[o[..., 0] if o.shape[2] == 1 else o for o in row] for row in outs]
+
+    def decompress_mixed_ptr(self, files: Sequence[bytes], renditions: Optional[Sequence[dict]], ptrs: Sequence[int], row_pitch: Sequence[int]) -> None:
+        """Raw-pointer form of decompress_mixed: image i of rung r goes to device memory at ptrs[r * N + i], rows
+        row_pitch[r * N + i] bytes apart, and stays there (sizes from decompress_output of each file)."""
+        renditions = [{}] if renditions is None else list(renditions)
+        opts = self._rendition_options(renditions)
+        bufs, fptrs, sizes = self._files(files)
+        n, k = len(bufs), len(renditions)
+        if not (len(ptrs) == len(row_pitch) == k * n):
+            raise ValueError(f"{k} renditions of {n} images need {k * n} pointers and row pitches")
+        A.check(_lib.b200jpeg_decompress_mixed(self._h, k, opts, fptrs, sizes, n, (C.c_void_p * (k * n))(*ptrs), 1, (C.c_size_t * (k * n))(*row_pitch)),
+                "decompress_mixed")
+
+    def recompress_mixed_params(self, files: Sequence[bytes], rungs) -> List[List[bytes]]:
+        """b200jpeg_recompress_mixed with explicit parameter blocks: rungs[r] is (params, options dict), params a list of
+        one Params per file (params_for_jpeg_input(switches, files[i], **options) builds them).  Returns out[r][i], what
+        recompress(params[i], [files[i]], **options) returns for that file alone."""
+        rungs = list(rungs)
+        n = len(files)
+        for r, rung in enumerate(rungs):
+            if not (isinstance(rung, (tuple, list)) and len(rung) == 2 and isinstance(rung[1], dict)):
+                raise ValueError(f"rendition {r}: expected a (list of params, options dict) pair")
+            if len(rung[0]) != n or not all(isinstance(p, Params) for p in rung[0]):
+                raise ValueError(f"rendition {r}: expected {n} Params, one per file")
+        opts = self._rendition_options([kw for _, kw in rungs])
+        k = len(rungs)
+        params = (Params * (k * n))(*[p for ps, _ in rungs for p in ps])
+        bufs, ptrs, sizes = self._files(files)
+        A.check(_lib.b200jpeg_recompress_mixed(self._h, k, opts, params, ptrs, sizes, n), "recompress_mixed")
+        return [[self.get_output(r * n + i) for i in range(n)] for r in range(k)]
+
+    def recompress_mixed(self, files: Sequence[bytes], rungs) -> List[List[bytes]]:
+        """cjpeg with JPEG input over files of mixed geometry, several rungs in one call: rungs[r] is (cjpeg switches,
+        options dict) and file i of rung r is encoded with params_for_jpeg_input(switches, files[i], **options).
+        Returns out[r][i]."""
+        rungs = list(rungs)
+        for r, rung in enumerate(rungs):
+            if not (isinstance(rung, (tuple, list)) and len(rung) == 2 and isinstance(rung[1], dict) and isinstance(rung[0], (tuple, list))
+                    and all(isinstance(x, str) for x in rung[0])):
+                raise ValueError(f"rendition {r}: expected a (cjpeg switches, options dict) pair")
+        self._rendition_options([kw for _, kw in rungs])
+        built, failed = [], None
+        for sw, kw in rungs:
+            ps = []
+            for f in files:
+                try:
+                    ps.append(params_for_jpeg_input(list(sw), bytes(f), **kw))
+                except B200JpegError as e:
+                    # a file or option the library refuses: it names the image and rung itself
+                    failed = failed or e
+                    ps.append(Params())
+            built.append((ps, kw))
+        out = self.recompress_mixed_params(files, built)
+        if failed is not None:
+            raise failed
+        return out
+
     def last_decode_sync(self):
         """(most rounds a CTA of the speculative decoder needed, subsequences the cross-CTA pass decoded again)."""
         r = C.c_int(0); q = C.c_longlong(0)

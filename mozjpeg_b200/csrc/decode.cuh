@@ -43,6 +43,8 @@ struct DecScan {
   int8_t comp[10], dx[10], dy[10];   // per MCU slot: image component, block offset inside the MCU
   int16_t tdc[10], tac[10];          // per MCU slot: DecTable index of its DC / AC table
   int mx[4], my[4];            // per image component: blocks per MCU across / down (1, 1 in a non-interleaved scan)
+  long long base[4];           // per image component: first block of the image in the component's plane
+  int wib[4], hib[4];          // per image component: its blocks across / down
 };
 
 // one restart segment (the whole scan without restarts)
@@ -59,8 +61,9 @@ struct DecSeg {
 // per subsequence: the (position, state) its last decode started from and ended at, and the blocks it completed
 struct DecRec { uint32_t in_pos, out_pos; uint32_t in_st, out_st; uint32_t count; uint32_t pad; };
 
-// destination planes: [n][hib][wib][64] int16 per component, natural order
-struct DecOut { int16_t *plane[4]; int wib[4], hib[4]; };
+// destination planes, one per component: each image's [hib][wib][64] int16 blocks, natural order, from the block
+// DecScan::base gives (the per-image geometry is the scan's)
+struct DecOut { int16_t *plane[4]; };
 
 DEC_HD uint32_t dec_bswap(uint32_t x)
 {

@@ -11,6 +11,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <array>
 #include <map>
 #include <memory>
 #include <string>
@@ -142,7 +143,8 @@ struct b200jpeg_encoder {
   int st_state = 0, st_next_row = 0;
   b200jpeg_params st_params;
   // device entropy decode (b200jpeg_decode_coefs_batch / b200jpeg_transcode_batch): descriptors of the last batch, the
-  // upload buffer of its unstuffed segments, and the decoded planes ([n][hib][wib][64] per component, natural order)
+  // upload buffer of its unstuffed segments, and the decoded planes (per component, each image's [hib][wib][64] blocks
+  // in turn, natural order)
   b200::DecBatch dec;
   PinBuf h_dec_words, h_dec_stat;
   DevBuf d_dec_words, d_dec_segs, d_dec_scans, d_dec_tabs, d_dec_out, d_dec_rec, d_dec_pre, d_dec_tsum, d_dec_dcd, d_dec_planes, d_dec_stat;
@@ -163,6 +165,9 @@ struct b200jpeg_encoder {
   // distinct option set, and the files of every rung but the last (the next rung's encode reuses the file arenas)
   std::vector<DevBuf> d_rend_pixels;
   std::vector<uint8_t> rend_files;
+  // batches of mixed geometry (b200jpeg_decompress_mixed / b200jpeg_recompress_mixed): one chunk's pixel-stage
+  // descriptors and work tables (IdctImg, UpsImg)
+  DevBuf d_mix_meta;
   CoefXform xform{};                            // the coefficient import's block mapping in the current batch (all zero: a copy)
 };
 
@@ -1647,20 +1652,21 @@ static void sum_decode_stage_times(b200jpeg_encoder *e)
 
 // Entropy decode of n files into e->d_dec_planes (jpeg_read_coefficients for the batch): the first scans through the
 // speculative decode, then every DC refinement, then the AC refinement levels in order.
-// first: the batch index of files[0], for the messages.
-static int decode_files(b200jpeg_encoder *e, const uint8_t *const *files, const size_t *sizes, int n, int first = 0)
+// first: the batch index of files[0], for the messages; mixed: the files may differ in geometry (DecBatch::mixed).
+static int decode_files(b200jpeg_encoder *e, const uint8_t *const *files, const size_t *sizes, int n, int first = 0, bool mixed = false)
 {
   if (!e || !files || !sizes || n <= 0) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
   CU(cudaSetDevice(e->device));
   DecBatch &b = e->dec;
   b.progressive = e->progressive_decode;
+  b.mixed = mixed;
   int rc = build_decode_batch(files, sizes, n, b, dec_words_alloc, e, first);
   if (rc) return rc;
   e->dec_prog = false;
   for (int i = 0; i < n; i++) e->dec_prog |= b.info[i].sof == 0xC2;
   const size_t nseg_all = b.segs.size() + b.dcr_segs.size() + b.acr_segs.size();
   size_t total = 0;
-  for (int c = 0; c < b.nc; c++) { e->dec_plane_off[c] = total; total += ((size_t)n * b.wib[c] * b.hib[c] * 128 + 255) & ~(size_t)255; }
+  for (int c = 0; c < 4; c++) { e->dec_plane_off[c] = total; total += ((size_t)b.plane_blocks[c] * 128 + 255) & ~(size_t)255; }
   const long long ntiles = (b.nsub + 1023) / 1024;
   if ((rc = e->d_dec_words.reserve(b.nwords * 4 + 16)) || (rc = e->d_dec_segs.reserve(nseg_all * sizeof(DecSeg))) ||
       (rc = e->d_dec_scans.reserve(b.scans.size() * sizeof(DecScan))) || (rc = e->d_dec_tabs.reserve(b.tabs.size() * sizeof(DecTable))) ||
@@ -1671,7 +1677,7 @@ static int decode_files(b200jpeg_encoder *e, const uint8_t *const *files, const 
     return rc;
   for (cudaEvent_t &ev : e->dec_ev) if (!ev) CU(cudaEventCreate(&ev));
   DecOut o; memset(&o, 0, sizeof o);
-  for (int c = 0; c < b.nc; c++) { o.plane[c] = reinterpret_cast<int16_t *>(e->d_dec_planes.as<uint8_t>() + e->dec_plane_off[c]); o.wib[c] = b.wib[c]; o.hib[c] = b.hib[c]; }
+  for (int c = 0; c < 4; c++) if (b.plane_blocks[c]) o.plane[c] = reinterpret_cast<int16_t *>(e->d_dec_planes.as<uint8_t>() + e->dec_plane_off[c]);
   cudaStream_t s = e->stream;
   uint8_t *stat = e->d_dec_stat.as<uint8_t>();          // [n] status words, max rounds (int), resynchronised subsequences (u64)
   const size_t rounds_off = ((size_t)n * 4 + 7) & ~(size_t)7, stat_bytes = rounds_off + 16;
@@ -1755,12 +1761,13 @@ static int transcode_files(b200jpeg_encoder *e, const b200jpeg_params *p, const 
   int rc = decode_files(e, files, sizes, n_images);
   if (rc) return rc;
   const DecBatch &b = e->dec;
+  const DecGeom &g0 = b.geom[0];
   // -grayscale keeps the first component of a 3-component source; every other destination has the source's components
-  const bool comps_ok = p->num_components == b.nc || (t && t->force_grayscale && p->num_components == 1);
-  if (!comps_ok) { set_error("the parameter block has %d components, the sources %d", p->num_components, b.nc); return B200JPEG_ERR_PARAM; }
+  const bool comps_ok = p->num_components == g0.nc || (t && t->force_grayscale && p->num_components == 1);
+  if (!comps_ok) { set_error("the parameter block has %d components, the sources %d", p->num_components, g0.nc); return B200JPEG_ERR_PARAM; }
   if (t) {
     for (int c = 0; c < p->num_components; c++)
-      if (t->src_wib[c] != b.wib[c] || t->src_hib[c] != b.hib[c]) { set_error("the sources' component %d has %dx%d blocks, the transform description %dx%d", c, b.wib[c], b.hib[c], t->src_wib[c], t->src_hib[c]); return B200JPEG_ERR_PARAM; }
+      if (t->src_wib[c] != g0.wib[c] || t->src_hib[c] != g0.hib[c]) { set_error("the sources' component %d has %dx%d blocks, the transform description %dx%d", c, g0.wib[c], g0.hib[c], t->src_wib[c], t->src_hib[c]); return B200JPEG_ERR_PARAM; }
   }
   // each image's quantization tables: what its components latched, in the slots p assigns them; in the source's
   // orientation (p's are transposed back), encode_coefs_xform transposes them with the blocks
@@ -1777,8 +1784,8 @@ static int transcode_files(b200jpeg_encoder *e, const b200jpeg_params *p, const 
   }
   int16_t *planes[4]; size_t pitch[4], stride[4];
   for (int c = 0; c < 4; c++) {
-    planes[c] = c < b.nc ? reinterpret_cast<int16_t *>(e->d_dec_planes.as<uint8_t>() + e->dec_plane_off[c]) : nullptr;
-    pitch[c] = c < b.nc ? (size_t)b.wib[c] : 0; stride[c] = c < b.nc ? (size_t)b.wib[c] * b.hib[c] : 0;
+    planes[c] = c < g0.nc ? reinterpret_cast<int16_t *>(e->d_dec_planes.as<uint8_t>() + e->dec_plane_off[c]) : nullptr;
+    pitch[c] = c < g0.nc ? (size_t)g0.wib[c] : 0; stride[c] = c < g0.nc ? (size_t)g0.wib[c] * g0.hib[c] : 0;
   }
   rc = t ? encode_coefs_xform(e, p, t, planes, 1, pitch, stride, qt.data(), n_images)
          : b200jpeg_encode_batch_coefs_qtables(e, p, planes, 1, pitch, stride, qt.data(), n_images);
@@ -1835,7 +1842,7 @@ static void method_table(int method, const uint16_t *q, uint32_t *out)
 
 // the sample planes of one chunk's pixel stage for `plan`: per needed component nk images of hib x wib blocks of
 // ssize x ssize samples; off[c]: where component c's plane starts.  Returns the bytes of all of them.
-static size_t sample_plane_layout(const DecBatch &b, const DecPlan &plan, int nk, size_t off[4])
+static size_t sample_plane_layout(const DecGeom &b, const DecPlan &plan, int nk, size_t off[4])
 {
   size_t total = 0;
   for (int c = 0; c < 4; c++) off[c] = 0;
@@ -1851,7 +1858,7 @@ static size_t sample_plane_layout(const DecBatch &b, const DecPlan &plan, int nk
 // reserved for before the first is enqueued: no buffer is reallocated under a queued kernel.
 static int reserve_pixel_stage(b200jpeg_encoder *e, const DecPlan &plan, int nk)
 {
-  const DecBatch &b = e->dec;
+  const DecGeom &b = e->dec.geom[0];
   size_t off[4];
   bool need_mt = false;
   for (int c = 0; c < b.nc; c++) need_mt |= plan.needed[c] && plan.ssize[c] == 8 && plan.method != B200JPEG_DCT_ISLOW;
@@ -1865,7 +1872,7 @@ static int reserve_pixel_stage(b200jpeg_encoder *e, const DecPlan &plan, int nk)
 static int upload_chunk_quant(b200jpeg_encoder *e, int nk, std::vector<uint16_t> &qt)
 {
   const DecBatch &b = e->dec;
-  const int nc = b.nc;
+  const int nc = b.geom[0].nc;
   qt.resize((size_t)nk * nc * 64);
   for (int i = 0; i < nk; i++)
     for (int c = 0; c < nc; c++) memcpy(&qt[((size_t)i * nc + c) * 64], b.info[i].comp_quant[c], 128);
@@ -1877,7 +1884,7 @@ static int upload_chunk_quant(b200jpeg_encoder *e, int nk, std::vector<uint16_t>
 // planes of wib * 8 samples a row, then the fancy upsampling and default colour conversion into the pixels
 static int idct_upsample_default(b200jpeg_encoder *e, int nk, uint8_t *pix, size_t row_pitch, size_t image_stride, const cudaEvent_t *ev)
 {
-  const DecBatch &b = e->dec;
+  const DecGeom &b = e->dec.geom[0];
   const int nc = b.nc, W = b.W, H = b.H;
   const int hx = nc == 3 ? b.h[0] : 1, vx = nc == 3 ? b.v[0] : 1;
   cudaStream_t s = e->stream;
@@ -1893,7 +1900,7 @@ static int idct_upsample_default(b200jpeg_encoder *e, int nk, uint8_t *pix, size
   }
   CU(cudaEventRecord(ev[1], s));
   const int dw = div_up(W, hx), dh = div_up(H, vx);                    // downsampled_width / _height of the chroma (jdmaster.c)
-  if (launch_upsample_color(hx, vx, nc, planes, pitch, stride, dw, dh, nc == 3 && b.info[0].jpeg_color_space != B200JPEG_CS_RGB,
+  if (launch_upsample_color(hx, vx, nc, planes, pitch, stride, dw, dh, nc == 3 && e->dec.info[0].jpeg_color_space != B200JPEG_CS_RGB,
                             pix, row_pitch, image_stride, W, H, nk, s)) { set_error("no upsampling kernel for %dx%d sampling of %d components", hx, vx, nc); return B200JPEG_ERR_UNSUPPORTED; }
   CU(cudaEventRecord(ev[2], s));
   CU(cudaGetLastError());
@@ -1906,7 +1913,7 @@ static int idct_upsample_default(b200jpeg_encoder *e, int nk, uint8_t *pix, size
 static int idct_upsample_opts(b200jpeg_encoder *e, const DecPlan &plan, int nk, uint8_t *pix, size_t row_pitch, size_t image_stride,
                               const std::vector<uint16_t> &qt, std::vector<uint32_t> &mt, const cudaEvent_t *ev)
 {
-  const DecBatch &b = e->dec;
+  const DecGeom &b = e->dec.geom[0];
   const int nc = b.nc;
   cudaStream_t s = e->stream;
   size_t off[4];
@@ -2182,6 +2189,17 @@ static int decompress_renditions(b200jpeg_encoder *e, int n_renditions, const b2
   return B200JPEG_OK;
 }
 
+// the stage times of the last encode added into (names, ms, calls)
+static void merge_stage_times(const b200jpeg_encoder *e, std::vector<const char *> &names, std::vector<float> &ms, std::vector<int> &calls)
+{
+  for (size_t k = 0; k < e->stage_names.size(); k++) {
+    size_t j = 0;
+    while (j < names.size() && strcmp(names[j], e->stage_names[k])) j++;
+    if (j == names.size()) { names.push_back(e->stage_names[k]); ms.push_back(0.f); calls.push_back(0); }
+    ms[j] += e->stage_ms[k]; calls[j] += e->stage_calls[k];
+  }
+}
+
 // b200jpeg_recompress_renditions: the pixels of each distinct option set as decompress_renditions makes them, then per
 // rung recompress_batch's encode of the whole batch from its set's pixels
 static int recompress_renditions(b200jpeg_encoder *e, int n_renditions, const b200jpeg_decompress_options *opts, const b200jpeg_params *params,
@@ -2216,12 +2234,7 @@ static int recompress_renditions(b200jpeg_encoder *e, int n_renditions, const b2
     const PixTarget &t = tg[g.set[r]];
     if ((rc = encode_common(e, &params[r], t.pix, 1, t.row_pitch, t.image_stride, n_images, false, nullptr, nullptr, &e->dec_markers))) return rc;
     scan_bytes += e->last_scan_bytes;
-    for (size_t k = 0; k < e->stage_names.size(); k++) {
-      size_t j = 0;
-      while (j < names.size() && strcmp(names[j], e->stage_names[k])) j++;
-      if (j == names.size()) { names.push_back(e->stage_names[k]); ms.push_back(0.f); calls.push_back(0); }
-      ms[j] += e->stage_ms[k]; calls[j] += e->stage_calls[k];
-    }
+    merge_stage_times(e, names, ms, calls);
     if (r + 1 == n_renditions) break;
     for (int i = 0; i < n_images; i++) {
       kept.emplace_back(e->rend_files.size(), e->files[i].second);
@@ -2232,6 +2245,411 @@ static int recompress_renditions(b200jpeg_encoder *e, int n_renditions, const b2
   e->files.clear();
   for (const std::pair<size_t, size_t> &f : kept) e->files.emplace_back(e->rend_files.data() + f.first, f.second);
   e->files.insert(e->files.end(), last.begin(), last.end());
+  e->last_scan_bytes = scan_bytes;
+  e->stage_names = names; e->stage_ms = ms; e->stage_calls = calls;
+  add_decompress_stage_times(e);
+  return B200JPEG_OK;
+}
+
+// ---------------------------------------------------------------------------------- batches of mixed geometry
+// (b200jpeg_decompress_mixed / b200jpeg_recompress_mixed): the rendition calls without the one-geometry rule.  The
+// entropy decode takes the files as they come (DecBatch::mixed); the pixel stage runs the IDCT and upsampling kernels
+// in their ragged form, driven by a work table, so a chunk costs the same launches whatever the mix of sizes.
+
+// What the mixed calls know before any device work: each source's header and coefficient blocks, the distinct option
+// sets of the rungs (set[r]: rung r's; first[k]: the first rung of set k) and each set's plan for each image.
+struct MixedSrc {
+  std::vector<b200jpeg_source_info> info;
+  std::vector<long long> blocks;
+  std::vector<int> set, first;
+  std::vector<std::vector<DecPlan>> plan;              // [set][image]
+};
+
+static int check_mixed(b200jpeg_encoder *e, int n_renditions, const b200jpeg_decompress_options *opts, const uint8_t *const *files,
+                       const size_t *sizes, int n, MixedSrc &m)
+{
+  m = MixedSrc();
+  m.info.resize(n); m.blocks.assign(n, 0);
+  for (int i = 0; i < n; i++) {
+    if (!files[i]) { set_error("image %d: no file", i); return B200JPEG_ERR_PARAM; }
+    b200jpeg_source_info &s = m.info[i];
+    int rc = b200jpeg_parse_source(files[i], sizes[i], &s);
+    if (rc) { std::string msg = b200jpeg_last_error(); set_error("image %d: %s", i, msg.c_str()); return rc; }
+    if ((rc = check_decompress_source(s, i, e->progressive_decode))) return rc;
+    int hmax = 1, vmax = 1;
+    for (int c = 0; c < s.num_components; c++) { hmax = std::max(hmax, s.h_samp_factor[c]); vmax = std::max(vmax, s.v_samp_factor[c]); }
+    for (int c = 0; c < s.num_components; c++)
+      m.blocks[i] += (long long)div_up((long long)s.image_width * s.h_samp_factor[c], hmax * 8) * div_up((long long)s.image_height * s.v_samp_factor[c], vmax * 8);
+  }
+  for (int r = 0; r < n_renditions; r++) {
+    const b200jpeg_decompress_options &o = opts[r];
+    int k = 0;
+    for (; k < (int)m.first.size(); k++) {
+      const b200jpeg_decompress_options &f = opts[m.first[k]];
+      if (f.scale_num == o.scale_num && f.scale_denom == o.scale_denom && f.dct_method == o.dct_method &&
+          f.do_fancy_upsampling == o.do_fancy_upsampling && f.out_color_space == o.out_color_space) break;
+    }
+    if (k == (int)m.first.size()) {
+      m.first.push_back(r);
+      m.plan.emplace_back(n);
+      for (int i = 0; i < n; i++)
+        if (int rc = plan_decompress(m.info[i], o, m.plan[k][i])) {
+          std::string msg = b200jpeg_last_error();
+          if (i == 0) set_error("rendition %d: %s", r, msg.c_str()); else set_error("rendition %d, image %d: %s", r, i, msg.c_str());
+          return rc;
+        }
+    }
+    m.set.push_back(k);
+  }
+  return B200JPEG_OK;
+}
+
+// The chunks of a mixed batch: images in order until a chunk holds about 1.6 M blocks (an image larger than that is a
+// chunk of its own), or b200jpeg_encoder_set_chunk_images images.  Returns the first image of each chunk and n.
+static std::vector<int> mixed_chunks(const b200jpeg_encoder *e, const std::vector<long long> &blocks)
+{
+  const int n = (int)blocks.size();
+  std::vector<int> start(1, 0);
+  long long acc = 0;
+  for (int i = 0; i < n; i++) {
+    const bool full = e->chunk_images_override > 0 ? i - start.back() == e->chunk_images_override : acc > 0 && acc + blocks[i] > 1600000LL;
+    if (full) { start.push_back(i); acc = 0; }
+    acc += blocks[i];
+  }
+  start.push_back(n);
+  return start;
+}
+
+// where image i of a pixel output goes
+struct MixedOut { uint8_t *pix; size_t row_pitch; };
+
+// One option set's pixel stage of a mixed chunk, staged on the host: the IDCT launches (one per component slot and
+// IDCT size present among the images), the upsampling launch, and the bytes of their descriptors and work tables.
+struct MixLaunch { int c, size; size_t desc, work; unsigned ncta; };
+struct MixStage {
+  std::vector<uint8_t> meta;
+  std::vector<MixLaunch> idct;
+  size_t ups_desc = 0, ups_work = 0; unsigned ups_cta = 0;
+  bool need_mt = false;
+};
+
+template <class T> static size_t meta_put(std::vector<uint8_t> &m, const T *p, size_t count)
+{
+  const size_t off = (m.size() + 15) & ~(size_t)15;
+  m.resize(off + count * sizeof(T));
+  if (count) memcpy(m.data() + off, p, count * sizeof(T));
+  return off;
+}
+
+// the bytes of one set's sample planes in a chunk (images [i0, i0 + nk)); soff[i][c]: where image i's plane c starts
+static size_t mixed_sample_layout(const DecBatch &b, const std::vector<DecPlan> &plan, int i0, int nk, std::vector<std::array<size_t, 3>> &soff)
+{
+  size_t total = 0;
+  soff.assign(nk, std::array<size_t, 3>{0, 0, 0});
+  for (int i = 0; i < nk; i++) {
+    const DecGeom &g = b.geom[i]; const DecPlan &p = plan[i0 + i];
+    for (int c = 0; c < g.nc; c++) {
+      if (!p.needed[c]) continue;
+      soff[i][c] = total; total += ((size_t)g.wib[c] * g.hib[c] * p.ssize[c] * p.ssize[c] + 255) & ~(size_t)255;
+    }
+  }
+  return total;
+}
+
+static void stage_mixed(const b200jpeg_encoder *e, const std::vector<DecPlan> &plan, int i0, int nk, int qs, const MixedOut *out, uint8_t *samples, MixStage &st)
+{
+  const DecBatch &b = e->dec;
+  std::vector<std::array<size_t, 3>> soff;
+  mixed_sample_layout(b, plan, i0, nk, soff);
+  st = MixStage();
+  std::vector<IdctImg> d; std::vector<uint32_t> w;
+  for (int c = 0; c < 3; c++)
+    for (int size = 1; size <= 8; size *= 2) {
+      d.clear(); w.clear();
+      const int bpc = idct_blocks_per_cta(size);
+      for (int i = 0; i < nk; i++) {
+        const DecGeom &g = b.geom[i]; const DecPlan &p = plan[i0 + i];
+        if (c >= g.nc || !p.needed[c] || p.ssize[c] != size) continue;
+        st.need_mt |= size == 8 && p.method != B200JPEG_DCT_ISLOW;
+        IdctImg im;
+        im.coef = g.base[c]; im.out = (long long)soff[i][c]; im.wib = g.wib[c]; im.hib = g.hib[c]; im.tab = (i * qs + c) * 64; im.cta0 = (int)w.size();
+        const long long ncta = ((long long)g.wib[c] * g.hib[c] + bpc - 1) / bpc;
+        w.insert(w.end(), (size_t)ncta, (uint32_t)d.size());
+        d.push_back(im);
+      }
+      if (d.empty()) continue;
+      MixLaunch l;
+      l.c = c; l.size = size; l.ncta = (unsigned)w.size();
+      l.desc = meta_put(st.meta, d.data(), d.size()); l.work = meta_put(st.meta, w.data(), w.size());
+      st.idct.push_back(l);
+    }
+  std::vector<UpsImg> u; w.clear();
+  for (int i = 0; i < nk; i++) {
+    const DecGeom &g = b.geom[i]; const DecPlan &p = plan[i0 + i];
+    UpsImg im; memset(&im, 0, sizeof im);
+    for (int c = 0; c < 3 && c < g.nc; c++) {
+      if (!p.needed[c]) continue;
+      im.o.plane[c] = samples + soff[i][c]; im.o.pitch[c] = g.wib[c] * p.ssize[c]; im.o.stride[c] = 0;
+      im.o.dw[c] = p.dw[c]; im.o.dh[c] = p.dh[c]; im.o.hr[c] = p.hr[c]; im.o.vr[c] = p.vr[c]; im.o.fancy[c] = p.fancy[c];
+    }
+    im.o.nin = p.nin; im.o.conv = p.conv; im.o.ps = p.ps;
+    for (int k = 0; k < 4; k++) im.o.off[k] = p.off[k];
+    im.pix = out[i].pix; im.row_pitch = (long long)out[i].row_pitch; im.W = p.out_w; im.H = p.out_h;
+    im.gx = div_up(p.out_w, 64); im.cta0 = (int)w.size();
+    w.insert(w.end(), (size_t)im.gx * div_up(p.out_h, 4), (uint32_t)u.size());
+    u.push_back(im);
+  }
+  st.ups_cta = (unsigned)w.size();
+  st.ups_desc = meta_put(st.meta, u.data(), u.size()); st.ups_work = meta_put(st.meta, w.data(), w.size());
+}
+
+// whether images [i0, i0 + nk) of a set's outputs lie one image stride apart at one row pitch (stride: that stride)
+static bool evenly_spaced(const std::vector<MixedOut> &o, int i0, int nk, size_t &stride)
+{
+  stride = nk > 1 ? (size_t)(o[i0 + 1].pix - o[i0].pix) : 0;
+  for (int i = 1; i < nk; i++)
+    if (o[i0 + i].pix < o[i0].pix || o[i0 + i].pix != o[i0].pix + (size_t)i * stride || o[i0 + i].row_pitch != o[i0].row_pitch) return false;
+  return true;
+}
+
+// jpeg_read_scanlines for a batch of mixed geometry, to every option set's outputs (out[k][i]): per chunk the entropy
+// decode, then each set's pixel stage, enqueued together and synchronised once.  A chunk of one geometry (size,
+// sampling, components, RGB-coded or not) whose outputs are evenly spaced takes the one-geometry route (chunk_pixels),
+// faster in its upsampling (DESIGN §12); every other chunk the ragged one.
+static int mixed_files(b200jpeg_encoder *e, const uint8_t *const *files, const size_t *sizes, int n, const MixedSrc &m,
+                       const std::vector<std::vector<MixedOut>> &out, bool want_markers)
+{
+  const int K = (int)m.first.size();
+  while (e->pix_ev.size() < (size_t)K * 3) { cudaEvent_t ev; CU(cudaEventCreate(&ev)); e->pix_ev.push_back(ev); }
+  for (float &ms : e->dec_ms) ms = 0.f;
+  e->dec_ms_prog = false;
+  e->dec.want_markers = want_markers;
+  if (want_markers) e->dec_markers.assign(n, std::vector<uint8_t>());
+  const std::vector<int> start = mixed_chunks(e, m.blocks);
+  e->chunk = 0;
+  std::vector<uint16_t> qt; std::vector<uint32_t> mt; std::vector<MixStage> st(K);
+  std::vector<std::array<size_t, 3>> soff;
+  cudaStream_t s = e->stream;
+  for (size_t ch = 0; ch + 1 < start.size(); ch++) {
+    const int i0 = start[ch], nk = start[ch + 1] - i0;
+    e->chunk = std::max(e->chunk, nk);
+    int rc = decode_files(e, files + i0, sizes + i0, nk, i0, true);
+    if (rc) return rc;
+    e->dec_ms_prog |= e->dec_prog;
+    if (want_markers) for (int i = 0; i < nk; i++) e->dec_markers[i0 + i].swap(e->dec.markers[i]);
+    const DecGeom &g0 = e->dec.geom[0];
+    bool one = true;
+    int qs = 1;                                          // components per image in the chunk's table layout [nk][qs][64]
+    for (int i = 0; i < nk; i++) {
+      const DecGeom &g = e->dec.geom[i];
+      qs = std::max(qs, g.nc);
+      one &= g.W == g0.W && g.H == g0.H && g.nc == g0.nc &&
+             (e->dec.info[i].jpeg_color_space == B200JPEG_CS_RGB) == (e->dec.info[0].jpeg_color_space == B200JPEG_CS_RGB);
+      for (int c = 0; c < g.nc; c++) one &= g.h[c] == g0.h[c] && g.v[c] == g0.v[c];
+    }
+    std::vector<size_t> stride(K, 0);
+    std::vector<char> uniform(K, 0);
+    for (int k = 0; k < K; k++) uniform[k] = one && evenly_spaced(out[k], i0, nk, stride[k]);
+    // every buffer the chunk's pixel stages use is reserved before the first is enqueued
+    size_t samples = 0, meta = 0;
+    for (int k = 0; k < K; k++)
+      if (uniform[k]) { if ((rc = reserve_pixel_stage(e, m.plan[k][i0], nk))) return rc; }
+      else samples = std::max(samples, mixed_sample_layout(e->dec, m.plan[k], i0, nk, soff));
+    if ((rc = e->d_dec_samples.reserve(samples)) || (rc = e->d_dec_quant.reserve((size_t)nk * qs * 128)) || (rc = e->d_dec_mtab.reserve((size_t)nk * qs * 256))) return rc;
+    for (int k = 0; k < K; k++)
+      if (!uniform[k]) { stage_mixed(e, m.plan[k], i0, nk, qs, out[k].data() + i0, e->d_dec_samples.as<uint8_t>(), st[k]); meta = std::max(meta, st[k].meta.size()); }
+    if ((rc = e->d_mix_meta.reserve(meta))) return rc;
+    qt.assign((size_t)nk * qs * 64, 0);
+    for (int i = 0; i < nk; i++)
+      for (int c = 0; c < e->dec.geom[i].nc; c++) memcpy(&qt[((size_t)i * qs + c) * 64], e->dec.info[i].comp_quant[c], 128);
+    CU(cudaMemcpyAsync(e->d_dec_quant.p, qt.data(), qt.size() * 2, cudaMemcpyHostToDevice, s));
+    const int16_t *coef[3];
+    for (int c = 0; c < 3; c++) coef[c] = reinterpret_cast<const int16_t *>(e->d_dec_planes.as<uint8_t>() + e->dec_plane_off[c]);
+    for (int k = 0; k < K; k++) {
+      const MixStage &g = st[k];
+      const int method = m.plan[k][i0].method;
+      const cudaEvent_t *ev = &e->pix_ev[(size_t)k * 3];
+      if (uniform[k]) {
+        const MixedOut &o = out[k][i0];
+        if ((rc = chunk_pixels(e, m.plan[k][i0], nk, o.pix, o.row_pitch, stride[k], qt, mt, ev))) return rc;
+        continue;
+      }
+      // stream order keeps these uploads behind the previous set's kernels, which read the same buffers
+      if (g.need_mt) {
+        mt.resize(qt.size());
+        for (size_t t = 0; t < (size_t)nk * qs; t++) method_table(method, &qt[t * 64], &mt[t * 64]);
+        CU(cudaMemcpyAsync(e->d_dec_mtab.p, mt.data(), mt.size() * 4, cudaMemcpyHostToDevice, s));
+      }
+      CU(cudaMemcpyAsync(e->d_mix_meta.p, g.meta.data(), g.meta.size(), cudaMemcpyHostToDevice, s));
+      const uint8_t *meta_d = e->d_mix_meta.as<uint8_t>();
+      CU(cudaEventRecord(ev[0], s));
+      for (const MixLaunch &l : g.idct) {
+        const bool by_method = l.size == 8 && method != B200JPEG_DCT_ISLOW;
+        const void *tab = by_method ? static_cast<const void *>(e->d_dec_mtab.as<uint32_t>()) : static_cast<const void *>(e->d_dec_quant.as<uint16_t>());
+        launch_idct_ragged(l.size, method, coef[l.c], tab, e->d_dec_samples.as<uint8_t>(), reinterpret_cast<const uint32_t *>(meta_d + l.work),
+                           reinterpret_cast<const IdctImg *>(meta_d + l.desc), l.ncta, s);
+      }
+      CU(cudaEventRecord(ev[1], s));
+      launch_upsample_ragged(reinterpret_cast<const uint32_t *>(meta_d + g.ups_work), reinterpret_cast<const UpsImg *>(meta_d + g.ups_desc), g.ups_cta, s);
+      CU(cudaEventRecord(ev[2], s));
+      CU(cudaGetLastError());
+    }
+    CU(cudaStreamSynchronize(s));
+    sum_decode_stage_times(e);
+    for (int k = 0; k < K; k++)
+      for (int j = 0; j < 2; j++) { float ms = 0.f; cudaEventElapsedTime(&ms, e->pix_ev[(size_t)k * 3 + j], e->pix_ev[(size_t)k * 3 + j + 1]); e->dec_ms[6 + j] += ms; }
+  }
+  return B200JPEG_OK;
+}
+
+// each set's pixels for the whole batch in one device buffer, image i at off[k][i], rows pitch[k][i] apart (the
+// decoded row padded to 4 bytes, as recompress_batch's); order[k]: the images in buffer order
+struct MixedPix { std::vector<std::vector<size_t>> off, pitch; };
+static int reserve_mixed_pixels(b200jpeg_encoder *e, const MixedSrc &m, const std::vector<std::vector<int>> &order, MixedPix &mp,
+                                std::vector<std::vector<MixedOut>> &out)
+{
+  const int K = (int)m.first.size(), n = (int)m.info.size();
+  if ((int)e->d_rend_pixels.size() < K) e->d_rend_pixels.resize(K);
+  mp.off.assign(K, std::vector<size_t>(n)); mp.pitch.assign(K, std::vector<size_t>(n));
+  out.assign(K, std::vector<MixedOut>(n));
+  for (int k = 0; k < K; k++) {
+    size_t total = 0;
+    for (int i : order[k]) {
+      const DecPlan &p = m.plan[k][i];
+      mp.pitch[k][i] = ((size_t)p.out_w * p.out_nc + 3) & ~(size_t)3; mp.off[k][i] = total; total += mp.pitch[k][i] * p.out_h;
+    }
+    if (int rc = e->d_rend_pixels[k].reserve(total)) return rc;
+    for (int i = 0; i < n; i++) out[k][i] = MixedOut{e->d_rend_pixels[k].as<uint8_t>() + mp.off[k][i], mp.pitch[k][i]};
+  }
+  return B200JPEG_OK;
+}
+
+// b200jpeg_decompress_mixed: one decode per chunk, one ragged pixel stage per distinct option set, the rungs that share
+// a set copied from the first of them
+static int decompress_mixed(b200jpeg_encoder *e, int n_renditions, const b200jpeg_decompress_options *opts, const uint8_t *const *files,
+                            const size_t *sizes, int n_images, void *const *pixels, int pixels_on_device, const size_t *row_pitch)
+{
+  if (!e || n_renditions < 1 || !opts || !files || !sizes || n_images <= 0 || !pixels || !row_pitch) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
+  if ((long long)n_renditions * n_images > INT_MAX) { set_error("%d renditions of %d images are more outputs than one call indexes", n_renditions, n_images); return B200JPEG_ERR_PARAM; }
+  const int n = n_images;
+  MixedSrc m;
+  int rc = check_mixed(e, n_renditions, opts, files, sizes, n, m);
+  if (rc) return rc;
+  for (int r = 0; r < n_renditions; r++)
+    for (int i = 0; i < n; i++) {
+      const DecPlan &p = m.plan[m.set[r]][i];
+      const size_t j = (size_t)r * n + i;
+      if (!pixels[j] || row_pitch[j] < (size_t)p.out_w * p.out_nc) {
+        set_error("rendition %d, image %d: no pixel buffer, or row_pitch smaller than the decoded row (%dx%d, %d components)", r, i, p.out_w, p.out_h, p.out_nc);
+        return B200JPEG_ERR_PARAM;
+      }
+    }
+  CU(cudaSetDevice(e->device));
+  const int K = (int)m.first.size();
+  std::vector<std::vector<MixedOut>> out(K, std::vector<MixedOut>(n));
+  if (pixels_on_device) {
+    // the first rung of each set receives its pixels where the caller wants them
+    for (int k = 0; k < K; k++)
+      for (int i = 0; i < n; i++) { const size_t j = (size_t)m.first[k] * n + i; out[k][i] = MixedOut{static_cast<uint8_t *>(pixels[j]), row_pitch[j]}; }
+  } else {
+    std::vector<std::vector<int>> order(K, std::vector<int>(n));
+    for (int k = 0; k < K; k++) for (int i = 0; i < n; i++) order[k][i] = i;
+    MixedPix mp;
+    if ((rc = reserve_mixed_pixels(e, m, order, mp, out))) return rc;
+  }
+  if ((rc = mixed_files(e, files, sizes, n, m, out, false))) return rc;
+  for (int r = 0; r < n_renditions; r++) {
+    const int k = m.set[r];
+    if (pixels_on_device && r == m.first[k]) continue;
+    for (int i = 0; i < n; i++) {
+      const DecPlan &p = m.plan[k][i];
+      const size_t j = (size_t)r * n + i;
+      CU(cudaMemcpy2DAsync(pixels[j], row_pitch[j], out[k][i].pix, out[k][i].row_pitch, (size_t)p.out_w * p.out_nc, p.out_h,
+                           pixels_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, e->stream));
+    }
+  }
+  CU(cudaStreamSynchronize(e->stream));
+  e->pending_marks = 0;
+  e->stage_names.clear(); e->stage_ms.clear(); e->stage_calls.clear();
+  add_decompress_stage_times(e);
+  return B200JPEG_OK;
+}
+
+// b200jpeg_recompress_mixed: the pixels of each distinct option set as decompress_mixed makes them, then per rung one
+// encode per group of images with identical parameter blocks (same decoded size, so one pitch and stride), from the
+// group's images laid out one after another; outputs back in input order
+static int recompress_mixed(b200jpeg_encoder *e, int n_renditions, const b200jpeg_decompress_options *opts, const b200jpeg_params *params,
+                            const uint8_t *const *files, const size_t *sizes, int n_images)
+{
+  if (!e || n_renditions < 1 || !opts || !params || !files || !sizes || n_images <= 0) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
+  if ((long long)n_renditions * n_images > INT_MAX) { set_error("%d renditions of %d images are more outputs than b200jpeg_get_output indexes", n_renditions, n_images); return B200JPEG_ERR_PARAM; }
+  const int n = n_images;
+  MixedSrc m;
+  int rc = check_mixed(e, n_renditions, opts, files, sizes, n, m);
+  if (rc) return rc;
+  // group[r][i]: the first image of rung r whose parameter block equals image i's
+  std::vector<std::vector<int>> group(n_renditions, std::vector<int>(n));
+  for (int r = 0; r < n_renditions; r++)
+    for (int i = 0; i < n; i++) {
+      const b200jpeg_params *p = &params[(size_t)r * n + i];
+      const DecPlan &pl = m.plan[m.set[r]][i];
+      if ((rc = b200jpeg_validate(p))) { std::string msg = b200jpeg_last_error(); set_error("rendition %d, image %d: %s", r, i, msg.c_str()); return rc; }
+      if (p->data_precision != 8) { set_error("rendition %d, image %d: the source decodes to 8-bit samples, the parameter block has data_precision %d", r, i, p->data_precision); return B200JPEG_ERR_PARAM; }
+      if (pl.out_w != p->image_width || pl.out_h != p->image_height || pl.out_cs != p->in_color_space || pl.out_nc != p->input_components) {
+        set_error("rendition %d, image %d: the source decodes to %dx%d pixels of %d samples in colour space %d, the parameter block describes %dx%d of %d in %d (see b200jpeg_decompress_output_opts)",
+                  r, i, pl.out_w, pl.out_h, pl.out_nc, pl.out_cs, p->image_width, p->image_height, p->input_components, p->in_color_space);
+        return B200JPEG_ERR_PARAM;
+      }
+      int g = 0;
+      while (g < i && !(group[r][g] == g && !memcmp(&params[(size_t)r * n + g], p, sizeof *p))) g++;
+      group[r][i] = g;
+    }
+  CU(cudaSetDevice(e->device));
+  // each set's buffer holds the images group by group as its first rung forms them, so that rung encodes in place
+  const int K = (int)m.first.size();
+  std::vector<std::vector<int>> order(K);
+  for (int k = 0; k < K; k++) {
+    const std::vector<int> &gr = group[m.first[k]];
+    for (int g = 0; g < n; g++) if (gr[g] == g) for (int i = g; i < n; i++) if (gr[i] == g) order[k].push_back(i);
+  }
+  MixedPix mp;
+  std::vector<std::vector<MixedOut>> out;
+  if ((rc = reserve_mixed_pixels(e, m, order, mp, out))) return rc;
+  if ((rc = mixed_files(e, files, sizes, n, m, out, true))) return rc;
+  std::vector<std::pair<size_t, size_t>> kept((size_t)n_renditions * n);     // (offset in rend_files, size) per output
+  std::vector<const char *> names; std::vector<float> ms; std::vector<int> calls;
+  std::vector<std::vector<uint8_t>> markers;
+  size_t scan_bytes = 0;
+  e->rend_files.clear();
+  for (int r = 0; r < n_renditions; r++) {
+    const int k = m.set[r];
+    for (int g = 0; g < n; g++) {
+      if (group[r][g] != g) continue;
+      std::vector<int> mem;
+      for (int i = g; i < n; i++) if (group[r][i] == g) mem.push_back(i);
+      const size_t pitch = mp.pitch[k][g], stride = pitch * (size_t)m.plan[k][g].out_h;
+      bool in_place = true;
+      for (size_t j = 1; j < mem.size(); j++) in_place &= mp.off[k][mem[j]] == mp.off[k][mem[0]] + j * stride;
+      const uint8_t *src = out[k][mem[0]].pix;
+      if (!in_place) {                                 // another rung's grouping: gather the group's images
+        if ((rc = e->d_dec_pixels.reserve(stride * mem.size()))) return rc;
+        for (size_t j = 0; j < mem.size(); j++)
+          CU(cudaMemcpyAsync(e->d_dec_pixels.as<uint8_t>() + j * stride, out[k][mem[j]].pix, stride, cudaMemcpyDeviceToDevice, e->stream));
+        src = e->d_dec_pixels.as<uint8_t>();
+      }
+      markers.resize(mem.size());
+      for (size_t j = 0; j < mem.size(); j++) markers[j] = e->dec_markers[mem[j]];
+      if ((rc = encode_common(e, &params[(size_t)r * n + g], src, 1, pitch, stride, (int)mem.size(), false, nullptr, nullptr, &markers))) return rc;
+      scan_bytes += e->last_scan_bytes;
+      merge_stage_times(e, names, ms, calls);
+      for (size_t j = 0; j < mem.size(); j++) {
+        kept[(size_t)r * n + mem[j]] = std::make_pair(e->rend_files.size(), e->files[j].second);
+        e->rend_files.insert(e->rend_files.end(), e->files[j].first, e->files[j].first + e->files[j].second);
+      }
+    }
+  }
+  e->files.clear();
+  for (const std::pair<size_t, size_t> &f : kept) e->files.emplace_back(e->rend_files.data() + f.first, f.second);
   e->last_scan_bytes = scan_bytes;
   e->stage_names = names; e->stage_ms = ms; e->stage_calls = calls;
   add_decompress_stage_times(e);
@@ -2275,6 +2693,22 @@ int b200jpeg_decompress_renditions(b200jpeg_encoder *e, int n_renditions, const 
   return b200::decompress_renditions(e, n_renditions, opts, files, sizes, n_images, pixels, pixels_on_device, row_pitch, image_stride);
 }
 
+int b200jpeg_decompress_mixed(b200jpeg_encoder *e, int n_renditions, const b200jpeg_decompress_options *opts, const uint8_t *const *files,
+                              const size_t *sizes, int n_images, void *const *pixels, int pixels_on_device, const size_t *row_pitch)
+{
+  if (e) e->files.clear();
+  return b200::decompress_mixed(e, n_renditions, opts, files, sizes, n_images, pixels, pixels_on_device, row_pitch);
+}
+
+int b200jpeg_recompress_mixed(b200jpeg_encoder *e, int n_renditions, const b200jpeg_decompress_options *opts, const b200jpeg_params *params,
+                              const uint8_t *const *files, const size_t *sizes, int n_images)
+{
+  if (e) e->files.clear();
+  const int rc = b200::recompress_mixed(e, n_renditions, opts, params, files, sizes, n_images);
+  if (rc && e) e->files.clear();
+  return rc;
+}
+
 int b200jpeg_recompress_renditions(b200jpeg_encoder *e, int n_renditions, const b200jpeg_decompress_options *opts, const b200jpeg_params *params,
                                    const uint8_t *const *files, const size_t *sizes, int n_images)
 {
@@ -2291,7 +2725,7 @@ int b200jpeg_decode_coefs_batch(b200jpeg_encoder *e, const uint8_t *const *files
   e->dec.want_markers = false;
   int rc = decode_files(e, files, sizes, n_images);
   if (rc) return rc;
-  const DecBatch &b = e->dec;
+  const DecGeom &b = e->dec.geom[0];
   for (int c = 0; c < b.nc; c++) {
     const size_t wib = (size_t)b.wib[c], hib = (size_t)b.hib[c];
     if (!planes[c] || row_pitch_blocks[c] < wib || (n_images > 1 && image_stride_blocks[c] < row_pitch_blocks[c] * (hib - 1) + wib)) {

@@ -20,11 +20,19 @@ int derive_dec_table(const b200jpeg_huff_tbl &h, bool is_dc, DecTable *out);
 int check_progression(const b200jpeg_source_info &s, int coef_bits[4][64]);
 // smoothing_ok (jdcoefct.c:359-421) once the whole file is read: a decompress object at its defaults smooths the blocks
 bool smoothing_applies(const b200jpeg_source_info &s, const int coef_bits[4][64]);
-// the host half of the device decode of a batch of files (source.cpp): parsed headers, one geometry, scan / segment
-// descriptors, derived tables; the unstuffed segments go to the nwords words alloc(ctx, bound) returned.  segs: the
-// segments of first scans (the speculative decode); dcr_segs: DC refinement segments (dcr_blocks blocks in all);
+// one image's geometry (jdinput.c initial_setup): size, components, sampling factors, blocks across / down per
+// component, and base[c]: where its blocks start in the batch's plane of component c (in blocks)
+struct DecGeom {
+  int W = 0, H = 0, nc = 0;
+  int wib[4] = {0, 0, 0, 0}, hib[4] = {0, 0, 0, 0}, h[4] = {0, 0, 0, 0}, v[4] = {0, 0, 0, 0};
+  long long base[4] = {0, 0, 0, 0};
+};
+// the host half of the device decode of a batch of files (source.cpp): parsed headers, per-image geometry, scan /
+// segment descriptors, derived tables; the unstuffed segments go to the nwords words alloc(ctx, bound) returned.  segs:
+// the segments of first scans (the speculative decode); dcr_segs: DC refinement segments (dcr_blocks blocks in all);
 // acr_segs: AC refinement segments, level L (the L-th AC refinement scan of each image component) at
-// [acr_level[L], acr_level[L + 1])
+// [acr_level[L], acr_level[L + 1]).  Component c of every image lies in one plane of plane_blocks[c] blocks, the
+// images' ranges one after another in batch order; a one-geometry batch is [n][hib][wib] blocks per component.
 struct DecBatch {
   std::vector<b200jpeg_source_info> info;
   std::vector<DecScan> scans; std::vector<DecSeg> segs, dcr_segs, acr_segs; std::vector<DecTable> tabs;
@@ -32,8 +40,12 @@ struct DecBatch {
   long long nsub = 0, nblocks = 0, dcr_blocks = 0; unsigned long long nwords = 0;
   // progressive: take SOF2 files (else they are refused as before)
   bool progressive = false;
-  int W = 0, H = 0, nc = 0, precision = 8;
-  int wib[4] = {0, 0, 0, 0}, hib[4] = {0, 0, 0, 0}, h[4] = {0, 0, 0, 0}, v[4] = {0, 0, 0, 0};
+  // mixed: take files of different geometry (else a file whose size, precision, components or sampling differ from
+  // image 0's is refused)
+  bool mixed = false;
+  int precision = 8;
+  std::vector<DecGeom> geom;
+  long long plane_blocks[4] = {0, 0, 0, 0};
   // want_markers: also collect each file's COM / APPn segments as cjpeg copies them from a JPEG input (raw segments,
   // file order; see parse_source)
   bool want_markers = false;

@@ -4136,8 +4136,8 @@ __device__ __forceinline__ int16_t *dec_block(const DecOut &o, const DecScan &sc
 {
   const int c = sc.comp[slot];
   const long long col = (mcu % sc.per_row) * sc.mx[c] + sc.dx[slot], row = (mcu / sc.per_row) * sc.my[c] + sc.dy[slot];
-  if (col >= o.wib[c] || row >= o.hib[c]) return nullptr;          // a dummy block of an interleaved scan
-  return o.plane[c] + (((long long)sc.img * o.hib[c] + row) * o.wib[c] + col) * 64;
+  if (col >= sc.wib[c] || row >= sc.hib[c]) return nullptr;        // a dummy block of an interleaved scan
+  return o.plane[c] + (sc.base[c] + row * sc.wib[c] + col) * 64;
 }
 
 // the blocks subsequence j writes (k_dec_write), from (pos, st) to the first block start at or past bit b
@@ -4394,6 +4394,35 @@ __device__ __forceinline__ int idct_range_limit(int x)
 #define IDCT_BLOCKS 32           // blocks per CTA of k_idct_islow (8 lanes each)
 #define IDCT_WS 73               // ints per block of its workspace: 8 rows of 9, and one more so that blocks start in different banks
 
+// Where block lb of this CTA of an IDCT kernel lies, for output blocks of N x N samples: its index in the coefficient
+// plane, its table's offset, the byte offset of its first sample row and the row pitch.  One-geometry form (RAGGED
+// false): the plane holds [n][hib][wib] blocks, image i's table at i * qstride, the samples [n][hib * N][wib * N].
+// Ragged form: work[blockIdx.x] names the image (imgs[]) the CTA works on; each image's blocks are padded to whole
+// CTAs of BPC blocks, so a CTA never spans two images.
+struct IdctAt { bool valid; long long blk, q, o, pitch; };
+template <bool RAGGED, int BPC, int N>
+__device__ __forceinline__ IdctAt idct_at(int lb, int wib, int hib, long long nblocks, int qstride, const uint32_t *__restrict__ work,
+                                          const IdctImg *__restrict__ imgs)
+{
+  IdctAt a;
+  if (!RAGGED) {
+    a.blk = (long long)blockIdx.x * BPC + lb;
+    a.valid = a.blk < nblocks;
+    const long long per = (long long)wib * hib, img = a.valid ? a.blk / per : 0, rem = a.blk - img * per;
+    const int by = (int)(rem / wib), bx = (int)(rem - (long long)by * wib);
+    a.q = img * qstride; a.pitch = (long long)wib * N;
+    a.o = ((img * hib + by) * N) * a.pitch + bx * N;
+  } else {
+    const IdctImg d = imgs[work[blockIdx.x]];
+    const long long b = (long long)(blockIdx.x - d.cta0) * BPC + lb;
+    a.valid = b < (long long)d.wib * d.hib;
+    const int by = (int)(b / d.wib), bx = (int)(b - (long long)by * d.wib);
+    a.blk = d.coef + b; a.q = d.tab; a.pitch = (long long)d.wib * N;
+    a.o = d.out + (long long)by * N * a.pitch + bx * N;
+  }
+  return a;
+}
+
 // jpeg_idct_islow (jidctint.c:171-419, 8-bit: CONST_BITS 13, PASS1_BITS 2) with the dequantization of jddctmgr.c:
 // 134-146 (ISLOW_MULT_TYPE is a short: the table entries are taken as int16).  Eight lanes per block: each loads one
 // 16-byte row of the JBLOCK, transforms one column into the int workspace (pass 1), then one row into eight samples
@@ -4402,22 +4431,22 @@ __device__ __forceinline__ int idct_range_limit(int x)
 // 16-bit coefficients under a 16-bit table; pass 2 needs bits 18..27 of its sums only, which 32-bit arithmetic keeps.
 // coef: [nblocks][64] natural order ([n][hib][wib] blocks); quant: image i's table at quant + i * qstride;
 // out: [n][hib * 8][wib * 8] samples.
+template <bool RAGGED>
 __global__ void __launch_bounds__(IDCT_BLOCKS * 8) k_idct_islow(const int16_t *__restrict__ coef, const uint16_t *__restrict__ quant, int qstride,
-                                                                uint8_t *__restrict__ out, int wib, int hib, long long nblocks)
+                                                                uint8_t *__restrict__ out, int wib, int hib, long long nblocks,
+                                                                const uint32_t *__restrict__ work, const IdctImg *__restrict__ imgs)
 {
   __shared__ int4 s_coef[IDCT_BLOCKS * 8];
   __shared__ int s_ws[IDCT_BLOCKS * IDCT_WS];
   const int lb = threadIdx.x >> 3, lane = threadIdx.x & 7;
-  const long long blk = (long long)blockIdx.x * IDCT_BLOCKS + lb;
-  const bool valid = blk < nblocks;
-  const long long per = (long long)wib * hib;
-  const long long img = valid ? blk / per : 0;
-  s_coef[threadIdx.x] = valid ? reinterpret_cast<const int4 *>(coef)[blk * 8 + lane] : make_int4(0, 0, 0, 0);
+  const IdctAt at = idct_at<RAGGED, IDCT_BLOCKS, 8>(lb, wib, hib, nblocks, qstride, work, imgs);
+  const bool valid = at.valid;
+  s_coef[threadIdx.x] = valid ? reinterpret_cast<const int4 *>(coef)[at.blk * 8 + lane] : make_int4(0, 0, 0, 0);
   __syncwarp();
   // pass 1: column `lane`
   {
     const int16_t *c = reinterpret_cast<const int16_t *>(s_coef + lb * 8) + lane;
-    const uint16_t *q = quant + img * qstride + lane;
+    const uint16_t *q = quant + at.q + lane;
     long long d[8];
 #pragma unroll
     for (int r = 0; r < 8; r++) d[r] = (long long)c[r * 8] * (int16_t)q[r * 8];
@@ -4467,9 +4496,7 @@ __global__ void __launch_bounds__(IDCT_BLOCKS * 8) k_idct_islow(const int16_t *_
     const unsigned o2 = idct_range_limit((int)((tmp12 + tmp1 + rnd) >> 18)), o5 = idct_range_limit((int)((tmp12 - tmp1 + rnd) >> 18));
     const unsigned o3 = idct_range_limit((int)((tmp13 + tmp0 + rnd) >> 18)), o4 = idct_range_limit((int)((tmp13 - tmp0 + rnd) >> 18));
     if (valid) {
-      const long long rem = blk - img * per;
-      const int by = (int)(rem / wib), bx = (int)(rem - (long long)by * wib);
-      uint8_t *dst = out + ((img * hib + by) * 8 + lane) * ((long long)wib * 8) + bx * 8;
+      uint8_t *dst = out + at.o + lane * at.pitch;
       *reinterpret_cast<uint2 *>(dst) = make_uint2(o0 | o1 << 8 | o2 << 16 | o3 << 24, o4 | o5 << 8 | o6 << 16 | o7 << 24);
     }
   }
@@ -4478,7 +4505,7 @@ __global__ void __launch_bounds__(IDCT_BLOCKS * 8) k_idct_islow(const int16_t *_
 void launch_idct_islow(const int16_t *coef, const uint16_t *quant, int qstride, uint8_t *out, int wib, int hib, int n, cudaStream_t s)
 {
   const long long nblocks = (long long)n * wib * hib;
-  k_idct_islow<<<(unsigned)((nblocks + IDCT_BLOCKS - 1) / IDCT_BLOCKS), IDCT_BLOCKS * 8, 0, s>>>(coef, quant, qstride, out, wib, hib, nblocks); LAUNCHED();
+  k_idct_islow<false><<<(unsigned)((nblocks + IDCT_BLOCKS - 1) / IDCT_BLOCKS), IDCT_BLOCKS * 8, 0, s>>>(coef, quant, qstride, out, wib, hib, nblocks, nullptr, nullptr); LAUNCHED();
 }
 
 // the sample of a chroma plane at (row, col), both clamped to the real downsampled samples: the row above the first is
@@ -4592,32 +4619,29 @@ int launch_upsample_color(int hx, int vx, int nc, const uint8_t *const *planes, 
 // dq << (CONST_BITS + 1 or 2) is dq << PASS1_BITS, truncated to int the same way; pass 2: both are DESCALE(w0, 5)), so
 // there is no branch.  N = 1: one thread per block reads the DC term only.
 // out: [n][hib * N][wib * N] samples.
-template <int N>
+template <int N, bool RAGGED>
 __global__ void __launch_bounds__(IDCT_BLOCKS * 8) k_idct_red(const int16_t *__restrict__ coef, const uint16_t *__restrict__ quant, int qstride,
-                                                              uint8_t *__restrict__ out, int wib, int hib, long long nblocks)
+                                                              uint8_t *__restrict__ out, int wib, int hib, long long nblocks,
+                                                              const uint32_t *__restrict__ work, const IdctImg *__restrict__ imgs)
 {
-  const long long per = (long long)wib * hib;
   if (N == 1) {
-    const long long blk = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (blk >= nblocks) return;
-    const long long img = blk / per, rem = blk - img * per;
-    const int by = (int)(rem / wib), bx = (int)(rem - (long long)by * wib);
-    const int dq = (int)__ldg(coef + blk * 64) * (int)__ldg(quant + img * qstride);
-    out[(img * hib + by) * (long long)wib + bx] = (uint8_t)idct_range_limit((int)(((long long)dq + 4) >> 3));
+    const IdctAt at = idct_at<RAGGED, 256, 1>(threadIdx.x, wib, hib, nblocks, qstride, work, imgs);
+    if (!at.valid) return;
+    const int dq = (int)__ldg(coef + at.blk * 64) * (int)__ldg(quant + at.q);
+    out[at.o] = (uint8_t)idct_range_limit((int)(((long long)dq + 4) >> 3));
     return;
   }
   __shared__ int4 s_coef[IDCT_BLOCKS * 8];
   __shared__ int s_ws[IDCT_BLOCKS * IDCT_WS];
   const int lb = threadIdx.x >> 3, lane = threadIdx.x & 7;
-  const long long blk = (long long)blockIdx.x * IDCT_BLOCKS + lb;
-  const bool valid = blk < nblocks;
-  const long long img = valid ? blk / per : 0;
-  s_coef[threadIdx.x] = valid ? reinterpret_cast<const int4 *>(coef)[blk * 8 + lane] : make_int4(0, 0, 0, 0);
+  const IdctAt at = idct_at<RAGGED, IDCT_BLOCKS, N>(lb, wib, hib, nblocks, qstride, work, imgs);
+  const bool valid = at.valid;
+  s_coef[threadIdx.x] = valid ? reinterpret_cast<const int4 *>(coef)[at.blk * 8 + lane] : make_int4(0, 0, 0, 0);
   __syncwarp();
   const bool col_used = N == 4 ? lane != 4 : (lane & 1) || lane == 0;
   if (col_used) {                                         // pass 1: column `lane` -> ws rows 0 .. N-1
     const int16_t *c = reinterpret_cast<const int16_t *>(s_coef + lb * 8) + lane;
-    const uint16_t *q = quant + img * qstride + lane;
+    const uint16_t *q = quant + at.q + lane;
     long long d[8];
 #pragma unroll
     for (int r = 0; r < 8; r++) d[r] = (N == 4 && r == 4) || (N == 2 && (r == 2 || r == 4 || r == 6)) ? 0 : (long long)((int)c[r * 8] * (int)q[r * 8]);
@@ -4637,9 +4661,7 @@ __global__ void __launch_bounds__(IDCT_BLOCKS * 8) k_idct_red(const int16_t *__r
   __syncwarp();
   if (valid && lane < N) {                                // pass 2: row `lane`
     const int *w = s_ws + lb * IDCT_WS + lane * 9;
-    const long long rem = blk - img * per;
-    const int by = (int)(rem / wib), bx = (int)(rem - (long long)by * wib);
-    uint8_t *dst = out + ((img * hib + by) * N + lane) * ((long long)wib * N) + bx * N;
+    uint8_t *dst = out + at.o + lane * at.pitch;
     if (N == 4) {
       const long long t0 = (long long)w[0] * 16384, t2 = (long long)w[2] * 15137 + (long long)w[6] * -6270;
       const long long tmp10 = t0 + t2, tmp12 = t0 - t2;
@@ -4687,21 +4709,21 @@ __device__ __forceinline__ void ifast_1d(const unsigned d[8], unsigned o[8])
 
 // jpeg_idct_ifast with its multiplier table (jddctmgr.c: quantval * aanscales descaled to IFAST_SCALE_BITS, int),
 // image i's at mtab + i * qstride.  Shape of k_idct_islow.  The all-zero shortcuts give the general path's values.
+template <bool RAGGED>
 __global__ void __launch_bounds__(IDCT_BLOCKS * 8) k_idct_ifast(const int16_t *__restrict__ coef, const int *__restrict__ mtab, int qstride,
-                                                                uint8_t *__restrict__ out, int wib, int hib, long long nblocks)
+                                                                uint8_t *__restrict__ out, int wib, int hib, long long nblocks,
+                                                                const uint32_t *__restrict__ work, const IdctImg *__restrict__ imgs)
 {
   __shared__ int4 s_coef[IDCT_BLOCKS * 8];
   __shared__ int s_ws[IDCT_BLOCKS * IDCT_WS];
   const int lb = threadIdx.x >> 3, lane = threadIdx.x & 7;
-  const long long blk = (long long)blockIdx.x * IDCT_BLOCKS + lb;
-  const bool valid = blk < nblocks;
-  const long long per = (long long)wib * hib;
-  const long long img = valid ? blk / per : 0;
-  s_coef[threadIdx.x] = valid ? reinterpret_cast<const int4 *>(coef)[blk * 8 + lane] : make_int4(0, 0, 0, 0);
+  const IdctAt at = idct_at<RAGGED, IDCT_BLOCKS, 8>(lb, wib, hib, nblocks, qstride, work, imgs);
+  const bool valid = at.valid;
+  s_coef[threadIdx.x] = valid ? reinterpret_cast<const int4 *>(coef)[at.blk * 8 + lane] : make_int4(0, 0, 0, 0);
   __syncwarp();
   {
     const int16_t *c = reinterpret_cast<const int16_t *>(s_coef + lb * 8) + lane;
-    const int *q = mtab + img * qstride + lane;
+    const int *q = mtab + at.q + lane;
     unsigned d[8], o[8];
 #pragma unroll
     for (int r = 0; r < 8; r++) d[r] = (unsigned)(int)c[r * 8] * (unsigned)__ldg(q + r * 8);
@@ -4721,9 +4743,7 @@ __global__ void __launch_bounds__(IDCT_BLOCKS * 8) k_idct_ifast(const int16_t *_
 #pragma unroll
     for (int k = 0; k < 8; k++) s[k] = idct_range_limit((int)o[k] >> 5);        // IDESCALE(x, PASS1_BITS + 3)
     if (valid) {
-      const long long rem = blk - img * per;
-      const int by = (int)(rem / wib), bx = (int)(rem - (long long)by * wib);
-      uint8_t *dst = out + ((img * hib + by) * 8 + lane) * ((long long)wib * 8) + bx * 8;
+      uint8_t *dst = out + at.o + lane * at.pitch;
       *reinterpret_cast<uint2 *>(dst) = make_uint2(s[0] | s[1] << 8 | s[2] << 16 | s[3] << 24, s[4] | s[5] << 8 | s[6] << 16 | s[7] << 24);
     }
   }
@@ -4761,21 +4781,21 @@ __device__ __forceinline__ unsigned float_range_limit(float x)
 // jpeg_idct_float with its multiplier table (quantval * aanscalefactor[row] * aanscalefactor[col] in double, stored as
 // float), image i's at mtab + i * qstride.  Shape of k_idct_islow.  The all-zero column shortcut gives the general
 // path's values (x + 0 and x - 0 are x).
+template <bool RAGGED>
 __global__ void __launch_bounds__(IDCT_BLOCKS * 8) k_idct_float(const int16_t *__restrict__ coef, const float *__restrict__ mtab, int qstride,
-                                                                uint8_t *__restrict__ out, int wib, int hib, long long nblocks)
+                                                                uint8_t *__restrict__ out, int wib, int hib, long long nblocks,
+                                                                const uint32_t *__restrict__ work, const IdctImg *__restrict__ imgs)
 {
   __shared__ int4 s_coef[IDCT_BLOCKS * 8];
   __shared__ float s_ws[IDCT_BLOCKS * IDCT_WS];
   const int lb = threadIdx.x >> 3, lane = threadIdx.x & 7;
-  const long long blk = (long long)blockIdx.x * IDCT_BLOCKS + lb;
-  const bool valid = blk < nblocks;
-  const long long per = (long long)wib * hib;
-  const long long img = valid ? blk / per : 0;
-  s_coef[threadIdx.x] = valid ? reinterpret_cast<const int4 *>(coef)[blk * 8 + lane] : make_int4(0, 0, 0, 0);
+  const IdctAt at = idct_at<RAGGED, IDCT_BLOCKS, 8>(lb, wib, hib, nblocks, qstride, work, imgs);
+  const bool valid = at.valid;
+  s_coef[threadIdx.x] = valid ? reinterpret_cast<const int4 *>(coef)[at.blk * 8 + lane] : make_int4(0, 0, 0, 0);
   __syncwarp();
   {
     const int16_t *c = reinterpret_cast<const int16_t *>(s_coef + lb * 8) + lane;
-    const float *q = mtab + img * qstride + lane;
+    const float *q = mtab + at.q + lane;
     float d[8], o[8];
 #pragma unroll
     for (int r = 0; r < 8; r++) d[r] = (float)c[r * 8] * (__ldg(q + r * 8) * 0.125f);
@@ -4795,9 +4815,7 @@ __global__ void __launch_bounds__(IDCT_BLOCKS * 8) k_idct_float(const int16_t *_
 #pragma unroll
     for (int k = 0; k < 8; k++) s[k] = float_range_limit(o[k]);
     if (valid) {
-      const long long rem = blk - img * per;
-      const int by = (int)(rem / wib), bx = (int)(rem - (long long)by * wib);
-      uint8_t *dst = out + ((img * hib + by) * 8 + lane) * ((long long)wib * 8) + bx * 8;
+      uint8_t *dst = out + at.o + lane * at.pitch;
       *reinterpret_cast<uint2 *>(dst) = make_uint2(s[0] | s[1] << 8 | s[2] << 16 | s[3] << 24, s[4] | s[5] << 8 | s[6] << 16 | s[7] << 24);
     }
   }
@@ -4808,12 +4826,26 @@ void launch_idct_opts(int size, int method, const int16_t *coef, const void *tab
   const long long nblocks = (long long)n * wib * hib;
   const unsigned grid8 = (unsigned)((nblocks + IDCT_BLOCKS - 1) / IDCT_BLOCKS);
   const uint16_t *q = static_cast<const uint16_t *>(tab);
-  if (size == 1) { k_idct_red<1><<<(unsigned)((nblocks + 255) / 256), 256, 0, s>>>(coef, q, qstride, out, wib, hib, nblocks); LAUNCHED(); }
-  else if (size == 2) { k_idct_red<2><<<grid8, IDCT_BLOCKS * 8, 0, s>>>(coef, q, qstride, out, wib, hib, nblocks); LAUNCHED(); }
-  else if (size == 4) { k_idct_red<4><<<grid8, IDCT_BLOCKS * 8, 0, s>>>(coef, q, qstride, out, wib, hib, nblocks); LAUNCHED(); }
-  else if (method == 1) { k_idct_ifast<<<grid8, IDCT_BLOCKS * 8, 0, s>>>(coef, static_cast<const int *>(tab), qstride, out, wib, hib, nblocks); LAUNCHED(); }
-  else if (method == 2) { k_idct_float<<<grid8, IDCT_BLOCKS * 8, 0, s>>>(coef, static_cast<const float *>(tab), qstride, out, wib, hib, nblocks); LAUNCHED(); }
+  if (size == 1) { k_idct_red<1, false><<<(unsigned)((nblocks + 255) / 256), 256, 0, s>>>(coef, q, qstride, out, wib, hib, nblocks, nullptr, nullptr); LAUNCHED(); }
+  else if (size == 2) { k_idct_red<2, false><<<grid8, IDCT_BLOCKS * 8, 0, s>>>(coef, q, qstride, out, wib, hib, nblocks, nullptr, nullptr); LAUNCHED(); }
+  else if (size == 4) { k_idct_red<4, false><<<grid8, IDCT_BLOCKS * 8, 0, s>>>(coef, q, qstride, out, wib, hib, nblocks, nullptr, nullptr); LAUNCHED(); }
+  else if (method == 1) { k_idct_ifast<false><<<grid8, IDCT_BLOCKS * 8, 0, s>>>(coef, static_cast<const int *>(tab), qstride, out, wib, hib, nblocks, nullptr, nullptr); LAUNCHED(); }
+  else if (method == 2) { k_idct_float<false><<<grid8, IDCT_BLOCKS * 8, 0, s>>>(coef, static_cast<const float *>(tab), qstride, out, wib, hib, nblocks, nullptr, nullptr); LAUNCHED(); }
   else launch_idct_islow(coef, q, qstride, out, wib, hib, n, s);
+}
+
+int idct_blocks_per_cta(int size) { return size == 1 ? 256 : IDCT_BLOCKS; }
+
+void launch_idct_ragged(int size, int method, const int16_t *coef, const void *tab, uint8_t *out, const uint32_t *work, const IdctImg *imgs,
+                        unsigned ncta, cudaStream_t s)
+{
+  const uint16_t *q = static_cast<const uint16_t *>(tab);
+  if (size == 1) { k_idct_red<1, true><<<ncta, 256, 0, s>>>(coef, q, 0, out, 0, 0, 0, work, imgs); LAUNCHED(); }
+  else if (size == 2) { k_idct_red<2, true><<<ncta, IDCT_BLOCKS * 8, 0, s>>>(coef, q, 0, out, 0, 0, 0, work, imgs); LAUNCHED(); }
+  else if (size == 4) { k_idct_red<4, true><<<ncta, IDCT_BLOCKS * 8, 0, s>>>(coef, q, 0, out, 0, 0, 0, work, imgs); LAUNCHED(); }
+  else if (method == 1) { k_idct_ifast<true><<<ncta, IDCT_BLOCKS * 8, 0, s>>>(coef, static_cast<const int *>(tab), 0, out, 0, 0, 0, work, imgs); LAUNCHED(); }
+  else if (method == 2) { k_idct_float<true><<<ncta, IDCT_BLOCKS * 8, 0, s>>>(coef, static_cast<const float *>(tab), 0, out, 0, 0, 0, work, imgs); LAUNCHED(); }
+  else { k_idct_islow<true><<<ncta, IDCT_BLOCKS * 8, 0, s>>>(coef, q, 0, out, 0, 0, 0, work, imgs); LAUNCHED(); }
 }
 
 // one output sample of a component plane (dw x dh real samples) at pixel (x, y): fullsize, replication by hr x vr
@@ -4838,15 +4870,13 @@ __device__ __forceinline__ int up_one(const uint8_t *__restrict__ p, int pitch, 
 // the deconverter jinit_color_deconverter picks (jdcolor.c:760-930, jdcolext.c): grayscale_convert, ycc_rgb_convert,
 // null_convert / rgb_rgb_convert, gray_rgb_convert or rgb_gray_convert, into o.ps bytes with R, G, B at o.off[0..2]
 // and 0xFF at o.off[3] where the pixel has a fourth byte.
-__global__ void __launch_bounds__(256) k_upsample_opts(UpsOpt o, uint8_t *__restrict__ pix, long long row_pitch, long long image_stride, int W, int H)
+__device__ __forceinline__ void upsample_pixel(const UpsOpt &o, long long img, uint8_t *__restrict__ row, int x, int y)
 {
-  const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y, img = blockIdx.z;
-  if (x >= W || y >= H) return;
   int v[3] = {0, 0, 0};
 #pragma unroll
   for (int c = 0; c < 3; c++)
     if (c < o.nin) v[c] = up_one(o.plane[c] + img * o.stride[c], o.pitch[c], o.dw[c], o.dh[c], o.hr[c], o.vr[c], o.fancy[c] != 0, x, y);
-  uint8_t *d = pix + img * image_stride + (long long)y * row_pitch + (long long)x * o.ps;
+  uint8_t *d = row + (long long)x * o.ps;
   int r, g, b;
   switch (o.conv) {
   case UPS_GRAY: d[0] = (uint8_t)v[0]; return;
@@ -4865,10 +4895,38 @@ __global__ void __launch_bounds__(256) k_upsample_opts(UpsOpt o, uint8_t *__rest
   if (o.ps == 4) d[o.off[3]] = 0xFF;
 }
 
+__global__ void __launch_bounds__(256) k_upsample_opts(UpsOpt o, uint8_t *__restrict__ pix, long long row_pitch, long long image_stride, int W, int H)
+{
+  const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y, img = blockIdx.z;
+  if (x >= W || y >= H) return;
+  upsample_pixel(o, img, pix + img * image_stride + (long long)y * row_pitch, x, y);
+}
+
+// k_upsample_opts over images of different geometry and conversion: work[blockIdx.x] names the image (imgs[]) whose
+// 64 x 4 pixel tile the CTA makes, tile blockIdx.x - cta0 of its gx tiles a row; the image's sample planes are its own
+// (UpsOpt::stride unused).  The descriptor is staged in shared memory once per CTA.
+__global__ void __launch_bounds__(256) k_upsample_ragged(const uint32_t *__restrict__ work, const UpsImg *__restrict__ imgs)
+{
+  static_assert(sizeof(UpsImg) % 4 == 0 && sizeof(UpsImg) / 4 <= 256, "UpsImg is staged one word per thread");
+  __shared__ UpsImg d;
+  const int tid = threadIdx.y * blockDim.x + threadIdx.x;
+  if (tid < (int)(sizeof(UpsImg) / 4)) reinterpret_cast<uint32_t *>(&d)[tid] = reinterpret_cast<const uint32_t *>(imgs + work[blockIdx.x])[tid];
+  __syncthreads();
+  const int t = (int)blockIdx.x - d.cta0, ty = t / d.gx;
+  const int x = (t - ty * d.gx) * 64 + threadIdx.x, y = ty * 4 + threadIdx.y;
+  if (x >= d.W || y >= d.H) return;
+  upsample_pixel(d.o, 0, d.pix + (long long)y * d.row_pitch, x, y);
+}
+
 void launch_upsample_opts(const UpsOpt &o, uint8_t *pix, size_t row_pitch, size_t image_stride, int W, int H, int n, cudaStream_t s)
 {
   const dim3 cta(64, 4), grid((unsigned)((W + 63) / 64), (unsigned)((H + 3) / 4), (unsigned)n);
   k_upsample_opts<<<grid, cta, 0, s>>>(o, pix, (long long)row_pitch, (long long)image_stride, W, H); LAUNCHED();
+}
+
+void launch_upsample_ragged(const uint32_t *work, const UpsImg *imgs, unsigned ncta, cudaStream_t s)
+{
+  k_upsample_ragged<<<ncta, dim3(64, 4), 0, s>>>(work, imgs); LAUNCHED();
 }
 
 }  // namespace b200

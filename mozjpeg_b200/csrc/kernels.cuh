@@ -311,6 +311,19 @@ struct UpsOpt {
 };
 void launch_upsample_opts(const UpsOpt &o, uint8_t *pix, size_t row_pitch, size_t image_stride, int W, int H, int n, cudaStream_t s);
 
+// The pixel stage of a chunk whose images differ in geometry: the same kernels driven by a work table, one 4-byte image
+// index per CTA, and a descriptor per image.  An IDCT image: wib x hib blocks from block `coef` of the coefficient
+// plane, its table at `tab` entries, its samples at byte `out`, wib * size a row; cta0: its first CTA, its blocks
+// padded to whole CTAs of idct_blocks_per_cta(size) blocks.  size and method as for launch_idct_opts.
+struct IdctImg { long long coef, out; int wib, hib, tab, cta0; };
+int idct_blocks_per_cta(int size);
+void launch_idct_ragged(int size, int method, const int16_t *coef, const void *tab, uint8_t *out, const uint32_t *work, const IdctImg *imgs,
+                        unsigned ncta, cudaStream_t s);
+// An upsampling / colour conversion image: its UpsOpt (planes of its own; stride unused), W x H pixels at pix,
+// row_pitch bytes apart; cta0: its first CTA, gx: its 64 x 4 pixel tiles a row.
+struct UpsImg { UpsOpt o; uint8_t *pix; long long row_pitch; int W, H, cta0, gx; };
+void launch_upsample_ragged(const uint32_t *work, const UpsImg *imgs, unsigned ncta, cudaStream_t s);
+
 extern unsigned long long g_kernel_launches;
 
 }  // namespace b200

@@ -410,25 +410,43 @@ int build_decode_batch(const uint8_t *const *files, const size_t *sizes, int n, 
     const b200jpeg_source_info &s0 = b.info[0];
     bool same = s.image_width == s0.image_width && s.image_height == s0.image_height && s.data_precision == s0.data_precision && s.num_components == s0.num_components;
     for (int c = 0; same && c < s.num_components; c++) same = s.h_samp_factor[c] == s0.h_samp_factor[c] && s.v_samp_factor[c] == s0.v_samp_factor[c];
-    if (!same) { set_error("image %d: geometry (size, precision, components, sampling) differs from image 0", first + i); return B200JPEG_ERR_PARAM; }
+    if (!same && !b.mixed) { set_error("image %d: geometry (size, precision, components, sampling) differs from image 0", first + i); return B200JPEG_ERR_PARAM; }
   }
-  const b200jpeg_source_info &s0 = b.info[0];
-  b.W = s0.image_width; b.H = s0.image_height; b.nc = s0.num_components; b.precision = s0.data_precision;
-  int hmax = 1, vmax = 1;
-  for (int c = 0; c < b.nc; c++) { hmax = std::max(hmax, s0.h_samp_factor[c]); vmax = std::max(vmax, s0.v_samp_factor[c]); }
-  for (int c = 0; c < b.nc; c++) {
-    b.h[c] = s0.h_samp_factor[c]; b.v[c] = s0.v_samp_factor[c];
-    b.wib[c] = (int)(((long long)b.W * b.h[c] + hmax * 8 - 1) / (hmax * 8));      // jdinput.c initial_setup
-    b.hib[c] = (int)(((long long)b.H * b.v[c] + vmax * 8 - 1) / (vmax * 8));
+  b.precision = b.info[0].data_precision;
+  b.geom.assign(n, DecGeom());
+  for (long long &pb : b.plane_blocks) pb = 0;
+  for (int i = 0; i < n; i++) {
+    const b200jpeg_source_info &s = b.info[i];
+    DecGeom &g = b.geom[i];
+    g.W = s.image_width; g.H = s.image_height; g.nc = s.num_components;
+    int hmax = 1, vmax = 1;
+    for (int c = 0; c < g.nc; c++) { hmax = std::max(hmax, s.h_samp_factor[c]); vmax = std::max(vmax, s.v_samp_factor[c]); }
+    for (int c = 0; c < g.nc; c++) {
+      g.h[c] = s.h_samp_factor[c]; g.v[c] = s.v_samp_factor[c];
+      g.wib[c] = (int)(((long long)g.W * g.h[c] + hmax * 8 - 1) / (hmax * 8));      // jdinput.c initial_setup
+      g.hib[c] = (int)(((long long)g.H * g.v[c] + vmax * 8 - 1) / (vmax * 8));
+      g.base[c] = b.plane_blocks[c]; b.plane_blocks[c] += (long long)g.wib[c] * g.hib[c];
+    }
   }
-  auto scan_mcus = [&](const b200jpeg_source_scan &ss) -> long long {
-    if (ss.comps_in_scan == 1) return (long long)b.wib[ss.component_index[0]] * b.hib[ss.component_index[0]];
-    return (long long)((b.W + hmax * 8 - 1) / (hmax * 8)) * ((b.H + vmax * 8 - 1) / (vmax * 8));
+  // MCUs of a scan of image i, and MCUs per MCU row
+  auto mcu_row = [&](int i, const b200jpeg_source_scan &ss) -> long long {
+    const DecGeom &g = b.geom[i];
+    if (ss.comps_in_scan == 1) return g.wib[ss.component_index[0]];
+    int hmax = 1;
+    for (int c = 0; c < g.nc; c++) hmax = std::max(hmax, g.h[c]);
+    return (g.W + hmax * 8 - 1) / (hmax * 8);
+  };
+  auto scan_mcus = [&](int i, const b200jpeg_source_scan &ss) -> long long {
+    const DecGeom &g = b.geom[i];
+    if (ss.comps_in_scan == 1) return (long long)g.wib[ss.component_index[0]] * g.hib[ss.component_index[0]];
+    int vmax = 1;
+    for (int c = 0; c < g.nc; c++) vmax = std::max(vmax, g.v[c]);
+    return mcu_row(i, ss) * ((g.H + vmax * 8 - 1) / (vmax * 8));
   };
   for (int i = 0; i < n; i++)
     for (int k = 0; k < b.info[i].num_scans; k++) {
       const b200jpeg_source_scan &ss = b.info[i].scans[k];
-      const long long ri = ss.restart_interval, nseg = ri ? (scan_mcus(ss) + ri - 1) / ri : 1;
+      const long long ri = ss.restart_interval, nseg = ri ? (scan_mcus(i, ss) + ri - 1) / ri : 1;
       bound += ss.data_size + 16 * (size_t)nseg + 16;      // each segment: its bytes, up to 3 pad bytes, 2 zero words
     }
   uint32_t *out = alloc(ctx, bound / 4 + 4);
@@ -436,6 +454,7 @@ int build_decode_batch(const uint8_t *const *files, const size_t *sizes, int n, 
   unsigned long long wpos = 0;
   for (int i = 0; i < n; i++) {
     const b200jpeg_source_info &s = b.info[i];
+    const DecGeom &gm = b.geom[i];
     const uint8_t *d = files[i];
     std::map<int, int> tix;                          // pool index * 2 + is_dc -> DecTable index
     auto table = [&](int pool, bool dc) -> int {
@@ -455,13 +474,14 @@ int build_decode_batch(const uint8_t *const *files, const size_t *sizes, int n, 
       sc.kind = !prog ? DEC_SEQ : ss.Ss == 0 ? (ss.Ah ? DEC_DC_REFINE : DEC_DC_FIRST) : (ss.Ah ? DEC_AC_REFINE : DEC_AC_FIRST);
       sc.Ss = ss.Ss; sc.Se = ss.Se; sc.Al = ss.Al;
       const bool need_dc = sc.kind == DEC_SEQ || sc.kind == DEC_DC_FIRST, need_ac = sc.kind == DEC_SEQ || sc.kind >= DEC_AC_FIRST;
-      const long long mcus = scan_mcus(ss);
-      sc.per_row = sc.ncomp == 1 ? b.wib[ss.component_index[0]] : (b.W + hmax * 8 - 1) / (hmax * 8);
+      const long long mcus = scan_mcus(i, ss);
+      sc.per_row = (int)mcu_row(i, ss);
+      for (int c = 0; c < gm.nc; c++) { sc.base[c] = gm.base[c]; sc.wib[c] = gm.wib[c]; sc.hib[c] = gm.hib[c]; }
       int slot = 0;
       for (int j = 0; j < sc.ncomp; j++) {
         const int c = ss.component_index[j];
         if (!prog && scanned[c]++) { set_error("image %d: component %d appears in two sequential scans", first + i, c); return B200JPEG_ERR_UNSUPPORTED; }
-        const int hh = sc.ncomp == 1 ? 1 : b.h[c], vv = sc.ncomp == 1 ? 1 : b.v[c];
+        const int hh = sc.ncomp == 1 ? 1 : gm.h[c], vv = sc.ncomp == 1 ? 1 : gm.v[c];
         sc.ci[j] = c; sc.first[j] = slot; sc.cnt[j] = hh * vv; sc.mx[c] = hh; sc.my[c] = vv;
         if (slot + hh * vv > 10) { set_error("image %d: scan %d has more than 10 blocks per MCU", first + i, k); return B200JPEG_ERR_BAD_SOURCE; }   // JERR_BAD_MCU_SIZE
         const int td = need_dc ? table(ss.dc_huff[j], true) : 0, ta = need_ac ? table(ss.ac_huff[j], false) : 0;
