@@ -515,6 +515,66 @@ int  b200jpeg_recompress_batch_opts(b200jpeg_encoder *enc, const b200jpeg_decomp
                                     const uint8_t *const *files, const size_t *sizes, int n_images);
 
 /*
+ * Decompression to YUV planes: replaces tj3DecompressToYUVPlanes8 (turbojpeg.c:2032-2195; jpeg_read_raw_data with
+ * TurboJPEG's plane layout) for a batch of files of one geometry (size, components, sampling).  Of the options only
+ * these apply, the others must keep b200jpeg_default_decompress_options' values, else B200JPEG_ERR_PARAM:
+ *   scale_num / scale_denom: one of TurboJPEG's scaling factors (n/8 for n = 1 .. 16, in lowest terms; others are
+ *     B200JPEG_ERR_PARAM "Unsupported scaling factor").  The IDCT block size is 8 * num / denom; only 1/8, 1/4, 1/2 and
+ *     1/1 are on the device, the others are B200JPEG_ERR_UNSUPPORTED.
+ *   dct_method: B200JPEG_DCT_ISLOW, or B200JPEG_DCT_IFAST (TJPARAM_FASTDCT); FLOAT is B200JPEG_ERR_PARAM.
+ * Sources: gray, and 3-component files whose sampling getSubsamp names (turbojpeg.c:400-479: 4:4:4, 4:2:2, 4:2:0,
+ * 4:4:0, 4:1:1, 4:4:1 and the non-standard 4:2:2, 4:4:0 and 4:4:4 spellings), RGB-coded files included (their planes
+ * are R, G and B).  Refused with the reference's text, before any device work and naming the image: other sampling
+ * ("Could not determine subsampling level of JPEG image") and 4 components ("JPEG image must have 3 or fewer
+ * components"), B200JPEG_ERR_PARAM; 12-bit files ("Unsupported JPEG data precision 12", B200JPEG_ERR_PARAM, as the
+ * 8-bit function refuses them).  Progressive files follow b200jpeg_encoder_set_progressive_decode, with the pixel
+ * routes' refusal of block-smoothed progressions; corrupt data is B200JPEG_ERR_BAD_SOURCE (TurboJPEG returns -1 on
+ * that warning).
+ *
+ * Plane ci of image i goes to planes[ci] + i * plane_stride[ci], b200jpeg_decompress_yuv_dims' pw x ph samples, rows
+ * plane_pitch[ci] bytes apart, in host or device memory (planes_on_device).  A plane holds component ci's IDCT output
+ * (iw = width_in_blocks * k by ih = height_in_blocks * k samples) cropped to pw x ph.  Where pw > iw or ph > ih (luma
+ * at 1/8 of a 2x2-sampled file with odd block counts, 4:1:1 at 1/4, ...) the reference copies bytes of its temporary
+ * buffer that depend on its heap layout (stale rows of the previous iMCU row, bytes past the end of a row): those
+ * columns iw .. pw-1 and rows ih .. ph-1 are not written here.  Nor are the bytes between pw and the pitch and between
+ * images.  A plane pitch below pw or a stride below one plane is B200JPEG_ERR_PARAM.
+ * For TJSAMP_420 below 1/1 every component runs luma's IDCT size, as TurboJPEG forces it (chroma stays subsampled); at
+ * 1/2 with IFAST the chroma IDCT (jpeg_idct_4x4) reads the ifast multiplier table libjpeg built before the override,
+ * exactly as the reference does.  Chunks as b200jpeg_decompress_batch; host planes come through one compact device
+ * staging buffer.  Stage times: the dec_* stages and idct.
+ */
+enum { B200JPEG_TJSAMP_444 = 0, B200JPEG_TJSAMP_422 = 1, B200JPEG_TJSAMP_420 = 2, B200JPEG_TJSAMP_GRAY = 3, B200JPEG_TJSAMP_440 = 4,
+       B200JPEG_TJSAMP_411 = 5, B200JPEG_TJSAMP_441 = 6 };
+int  b200jpeg_decompress_yuv_batch(b200jpeg_encoder *enc, const b200jpeg_decompress_options *opts, const uint8_t *const *files,
+                                   const size_t *sizes, int n_images, uint8_t *const *planes, int planes_on_device,
+                                   const size_t *plane_pitch, const size_t *plane_stride);
+/* Host only: plane ci's size, pw = tj3YUVPlaneWidth(ci, output_width, subsamp) by ph = tj3YUVPlaneHeight(ci,
+ * output_height, subsamp), and the TJSAMP_* of the source, for these options; otherwise the batch's refusals of the
+ * options, the sampling, the component count and the scale (without the image prefix), and B200JPEG_ERR_PARAM for ci
+ * outside the components. */
+int  b200jpeg_decompress_yuv_dims(const b200jpeg_source_info *src, const b200jpeg_decompress_options *opts, int ci,
+                                  int *width, int *height, int *subsamp);
+
+/*
+ * YUV decoding: replaces tj3DecodeYUVPlanes8 (turbojpeg.c:2418-2556), the upsampling and colour conversion of a
+ * decompress without the JPEG stages, for a batch of `n_images` images sharing `p`: the same parameter block
+ * b200jpeg_encode_yuv_batch takes for the pixel format and TJSAMP_* (tj3_params), so that the two calls are inverse on
+ * one description.  Plane ci of image i is read from planes[ci] + i * plane_stride[ci], b200jpeg_yuv_plane_dims
+ * samples, rows plane_pitch[ci] bytes apart; pixels go to pixels + i * image_stride, rows row_pitch bytes apart, in
+ * in_color_space's layout (GRAYSCALE or the RGB family; 0xFF in the fourth byte of 4-byte formats).  Host or device
+ * memory on either side (planes_on_device, pixels_on_device); the call returns when the pixels are written.
+ * As the reference with do_fancy_upsampling off: chroma is replicated (the merged upsampler for 4:2:0 and 4:2:2,
+ * int_upsample for 4:4:0, 4:1:1 and 4:4:1, which give the same pixels), a gray pixel format reads luma only, gray planes
+ * to the RGB family replicate it; only the first image_height rows are made (rows_to_go).  Refused with
+ * B200JPEG_ERR_PARAM: CMYK pixels ("Cannot decode YUV images into packed-pixel CMYK images."), a parameter block whose
+ * colour space and sampling name no TJSAMP_* ("TJPARAM_SUBSAMP must be specified"), precision other than 8, and pitches
+ * or strides below a plane or an image.  Bottom-up rows are not offered.  Stage time: yuv_to_pixels.
+ */
+int  b200jpeg_decode_yuv_batch(b200jpeg_encoder *enc, const b200jpeg_params *p, const uint8_t *const *planes, int planes_on_device,
+                               const size_t *plane_pitch, const size_t *plane_stride, void *pixels, int pixels_on_device,
+                               size_t row_pitch, size_t image_stride, int n_images);
+
+/*
  * One decode, several renditions (a rendition ladder: sizes and qualities of the same sources).  The same sources and
  * source checks as b200jpeg_decompress_batch_opts (one geometry; sequential files, or progressive ones with progressive
  * decode on).  The files are parsed, uploaded and entropy-decoded once per chunk, whatever n_renditions is; behind each

@@ -21,7 +21,8 @@ _lib = A.load()          # raises ImportError with build instructions if missing
 # the keywords of decompress_options, which a rendition's option dict may use
 RENDITION_OPTIONS = ("scale", "dct", "fancy", "colorspace")
 
-__all__ = ["Encoder", "Params", "params_from_switches", "read_ppm", "cjpeg", "tj3_params", "quality_tables", "yuv_plane_dims", "B200JpegError"]
+__all__ = ["Encoder", "Params", "params_from_switches", "read_ppm", "cjpeg", "tj3_params", "quality_tables", "yuv_plane_dims", "decompress_yuv_dims",
+           "yuv_packed_layout", "B200JpegError"]
 
 
 class Encoder:
@@ -229,6 +230,35 @@ class Encoder:
             A.check(_lib.b200jpeg_recompress_batch_opts(self._h, C.byref(o), C.byref(p), ptrs, sizes, len(bufs)), "recompress_batch_opts")
         return [self.get_output(i) for i in range(len(bufs))]
 
+    # -- decompression to YUV planes (tj3DecompressToYUVPlanes8) ------------------------------------------------------
+    def decompress_yuv(self, files: Sequence[bytes], **opts) -> List[List[np.ndarray]]:
+        """tj3DecompressToYUVPlanes8 for same-geometry files, on the device (b200jpeg_decompress_yuv_batch): per image
+        the list of its (ph, pw) uint8 planes, sizes from decompress_yuv_dims.  Keyword options: scale=(num, denom) (a
+        TurboJPEG scaling factor; 1/8, 1/4, 1/2, 1/1 on the device), dct="int" | "fast" (TJPARAM_FASTDCT).  Columns
+        past the IDCT output (iw) and rows past it (ih), which the reference fills from its heap, are left zero."""
+        try:
+            _, dims = decompress_yuv_dims(_parse_first(files), **opts)
+        except A.B200JpegError as e:
+            raise A.B200JpegError(e.code, "decompress_yuv_batch", "image 0: ") from None
+        bufs, ptrs, sizes = self._files(files)
+        n = len(bufs)
+        planes = [np.zeros((n, ph, pw), dtype=np.uint8) for pw, ph in dims]
+        k = len(planes)
+        o = decompress_options(**opts)
+        A.check(_lib.b200jpeg_decompress_yuv_batch(self._h, C.byref(o), ptrs, sizes, n, (C.c_void_p * k)(*[q.ctypes.data for q in planes]), 0,
+                                                   (C.c_size_t * k)(*[q.strides[1] for q in planes]),
+                                                   (C.c_size_t * k)(*[q.strides[0] for q in planes])), "decompress_yuv_batch")
+        return [[q[i] for q in planes] for i in range(n)]
+
+    def decompress_yuv_ptr(self, files: Sequence[bytes], ptrs: Sequence[int], pitch: Sequence[int], stride: Sequence[int], **opts) -> None:
+        """Raw-pointer form of decompress_yuv: plane ci of image i goes to device memory at ptrs[ci] + i * stride[ci],
+        rows pitch[ci] bytes apart."""
+        bufs, fp, sizes = self._files(files)
+        k = len(ptrs)
+        o = decompress_options(**opts)
+        A.check(_lib.b200jpeg_decompress_yuv_batch(self._h, C.byref(o), fp, sizes, len(bufs), (C.c_void_p * k)(*ptrs), 1,
+                                                   (C.c_size_t * k)(*pitch), (C.c_size_t * k)(*stride)), "decompress_yuv_batch")
+
     # -- renditions: one decode, several outputs -------------------------------------------------------------------
     @staticmethod
     def _rendition_options(renditions) -> "C.Array":
@@ -429,6 +459,32 @@ class Encoder:
                                                (C.c_void_p * k)(*planes), int(planes_on_device), (C.c_size_t * k)(*plane_pitch),
                                                (C.c_size_t * k)(*plane_stride), n), "encode_yuv_batch")
 
+    # -- YUV decoding (tj3DecodeYUVPlanes8) ---------------------------------
+    def decode_yuv(self, p: Params, planes) -> np.ndarray:
+        """The inverse of encode_yuv_batch on the same ``p`` (tj3_params for the pixel format and subsampling):
+        planes[i] is image i's list of (ph, pw) uint8 planes (one per component of p, sizes from yuv_plane_dims) ->
+        an (N, H, W, C) uint8 array of pixels (C = 1 for a gray pixel format), as tj3DecodeYUVPlanes8 makes them."""
+        n = len(planes)
+        k = p.num_components
+        arrs = [np.ascontiguousarray(np.stack([planes[i][ci] for i in range(n)]), dtype=np.uint8) for ci in range(k)]
+        for ci, a in enumerate(arrs):
+            if a.shape[1:] != yuv_plane_dims(p, ci)[::-1]:
+                raise ValueError(f"plane {ci} is {a.shape[2]}x{a.shape[1]}, the parameter block's is {yuv_plane_dims(p, ci)}")
+        ps = 1 if p.in_color_space == A.CS_GRAYSCALE else p.input_components
+        out = np.empty((n, p.image_height, p.image_width, ps), dtype=np.uint8)
+        self.decode_yuv_ptr(p, [a.ctypes.data for a in arrs], False, [a.strides[1] for a in arrs], [a.strides[0] for a in arrs],
+                            out.ctypes.data, False, out.strides[1], out.strides[0], n)
+        return out
+
+    def decode_yuv_ptr(self, p: Params, planes: Sequence[int], planes_on_device: bool, plane_pitch: Sequence[int], plane_stride: Sequence[int],
+                       ptr: int, pixels_on_device: bool, row_pitch: int, image_stride: int, n: int) -> None:
+        """Raw-pointer form of decode_yuv (device tensors, pinned host buffers): planes[ci] is image 0's plane of
+        component ci, plane_pitch / plane_stride / row_pitch / image_stride in bytes."""
+        k = len(planes)
+        A.check(_lib.b200jpeg_decode_yuv_batch(self._h, C.byref(p), (C.c_void_p * k)(*planes), int(planes_on_device), (C.c_size_t * k)(*plane_pitch),
+                                               (C.c_size_t * k)(*plane_stride), ptr, int(pixels_on_device), row_pitch, image_stride, n),
+                "decode_yuv_batch")
+
     def get_output(self, i: int) -> bytes:
         d = C.POINTER(C.c_uint8)(); n = C.c_size_t(0)
         A.check(_lib.b200jpeg_get_output(self._h, i, C.byref(d), C.byref(n)), "get_output")
@@ -570,6 +626,38 @@ def yuv_plane_dims(p: Params, ci: int):
     w = C.c_int(0); h = C.c_int(0)
     A.check(_lib.b200jpeg_yuv_plane_dims(C.byref(p), ci, C.byref(w), C.byref(h)), "yuv_plane_dims")
     return w.value, h.value
+
+
+# TJSAMP_* names in enum order (turbojpeg.h), as tj3_params takes them
+TJSAMP_NAMES = ("444", "422", "420", "gray", "440", "411", "441")
+
+
+def decompress_yuv_dims(info: "A.SourceInfo", **opts):
+    """(subsampling name, [(pw, ph) per plane]) of a source decompressed to YUV planes with the keyword options of
+    Encoder.decompress_yuv (b200jpeg_decompress_yuv_dims): getSubsamp's TJSAMP_* and tj3YUVPlaneWidth / Height."""
+    o = decompress_options(**opts)
+    w = C.c_int(0); h = C.c_int(0); ss = C.c_int(0)
+    A.check(_lib.b200jpeg_decompress_yuv_dims(C.byref(info), C.byref(o), 0, C.byref(w), C.byref(h), C.byref(ss)), "decompress_yuv_dims")
+    dims = []
+    for ci in range(1 if ss.value == 3 else 3):
+        A.check(_lib.b200jpeg_decompress_yuv_dims(C.byref(info), C.byref(o), ci, C.byref(w), C.byref(h), None), "decompress_yuv_dims")
+        dims.append((w.value, h.value))
+    return TJSAMP_NAMES[ss.value], dims
+
+
+def yuv_packed_layout(dims, align: int = 1):
+    """The unified YUV buffer of tj3DecompressToYUV8 / tj3DecodeYUV8 / tj3EncodeYUV8 for planes of sizes dims
+    [(pw, ph), ...]: (offsets, pitches, total bytes).  Each plane's rows are PAD(pw, align) bytes apart and the planes
+    follow each other (total = tj3YUVBufSize); align must be a power of two.  Pass offsets and pitches, with the
+    buffer's address added, to the planes' ptr / pitch arguments."""
+    if align < 1 or align & (align - 1):
+        raise ValueError(f"align must be a power of two, not {align}")
+    offsets, pitches, total = [], [], 0
+    for pw, ph in dims:
+        pitch = -(-pw // align) * align
+        offsets.append(total); pitches.append(pitch)
+        total += pitch * ph
+    return offsets, pitches, total
 
 
 def quality_tables(p: Params, qualities: Sequence[int], force_baseline: bool = True) -> np.ndarray:

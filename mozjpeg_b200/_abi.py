@@ -155,6 +155,7 @@ EXPORTS = [
     "b200jpeg_decompress_batch", "b200jpeg_recompress_batch", "b200jpeg_decompress_output",
     "b200jpeg_default_decompress_options", "b200jpeg_decompress_output_opts", "b200jpeg_decompress_batch_opts", "b200jpeg_recompress_batch_opts",
     "b200jpeg_decompress_renditions", "b200jpeg_recompress_renditions", "b200jpeg_decompress_mixed", "b200jpeg_recompress_mixed",
+    "b200jpeg_decompress_yuv_batch", "b200jpeg_decompress_yuv_dims", "b200jpeg_decode_yuv_batch",
 ]
 
 _lib = None
@@ -235,6 +236,10 @@ def load() -> C.CDLL:
     lib.b200jpeg_recompress_renditions.argtypes = [C.c_void_p, C.c_int, PO, P, PB, PS, C.c_int]; lib.b200jpeg_recompress_renditions.restype = C.c_int
     lib.b200jpeg_decompress_mixed.argtypes = [C.c_void_p, C.c_int, PO, PB, PS, C.c_int, PB, C.c_int, PS]; lib.b200jpeg_decompress_mixed.restype = C.c_int
     lib.b200jpeg_recompress_mixed.argtypes = [C.c_void_p, C.c_int, PO, P, PB, PS, C.c_int]; lib.b200jpeg_recompress_mixed.restype = C.c_int
+    lib.b200jpeg_decompress_yuv_batch.argtypes = [C.c_void_p, PO, PB, PS, C.c_int, PB, C.c_int, PS, PS]; lib.b200jpeg_decompress_yuv_batch.restype = C.c_int
+    lib.b200jpeg_decompress_yuv_dims.argtypes = [C.POINTER(SourceInfo), PO, C.c_int, PI, PI, PI]; lib.b200jpeg_decompress_yuv_dims.restype = C.c_int
+    lib.b200jpeg_decode_yuv_batch.argtypes = [C.c_void_p, P, PB, C.c_int, PS, PS, C.c_void_p, C.c_int, C.c_size_t, C.c_size_t, C.c_int]
+    lib.b200jpeg_decode_yuv_batch.restype = C.c_int
     lib.b200jpeg_last_error.argtypes = []; lib.b200jpeg_last_error.restype = C.c_char_p
     lib.b200jpeg_version.argtypes = []; lib.b200jpeg_version.restype = C.c_char_p
     _lib = lib

@@ -1794,6 +1794,23 @@ static int transcode_files(b200jpeg_encoder *e, const b200jpeg_params *p, const 
   return B200JPEG_OK;
 }
 
+// what every decode to samples needs of a source beyond its layout: each component's table defined and, for a
+// progressive file, a valid progression the reference would not block-smooth
+static int check_tables_progression(const b200jpeg_source_info &s, int i)
+{
+  for (int c = 0; c < s.num_components; c++)
+    if (!s.comp_quant_present[c]) { set_error("image %d: Quantization table 0x%02x was not defined", i, s.quant_tbl_no[c]); return B200JPEG_ERR_BAD_SOURCE; }
+  if (s.sof == 0xC2) {
+    int cb[4][64];
+    if (int rc = check_progression(s, cb)) { std::string m = b200jpeg_last_error(); set_error("image %d: %s", i, m.c_str()); return rc; }
+    if (smoothing_applies(s, cb)) {
+      set_error("image %d: incomplete progression: the reference decompressor applies block smoothing to it (do_block_smoothing), which is not on the device path", i);
+      return B200JPEG_ERR_UNSUPPORTED;
+    }
+  }
+  return B200JPEG_OK;
+}
+
 // A source b200jpeg_decompress_batch takes: sequential (or, with progressive decode on, progressive without the block
 // smoothing a default decompress object would apply), 8-bit, gray or three components with component 0 at the
 // largest factors (1 or 2 each way) over 1x1 chroma; everything else is refused, never approximated.
@@ -1807,17 +1824,7 @@ static int check_decompress_source(const b200jpeg_source_info &s, int i, bool pr
                                      s.h_samp_factor[2] != 1 || s.v_samp_factor[2] != 1))
     why = "sampling layout other than 4:4:4, 4:2:2, 4:4:0 or 4:2:0 (the reference's int_upsample and 2:1 non-fancy cases are not on the device)";
   if (why) { set_error("image %d: %s", i, why); return B200JPEG_ERR_UNSUPPORTED; }
-  for (int c = 0; c < s.num_components; c++)
-    if (!s.comp_quant_present[c]) { set_error("image %d: Quantization table 0x%02x was not defined", i, s.quant_tbl_no[c]); return B200JPEG_ERR_BAD_SOURCE; }
-  if (s.sof == 0xC2) {
-    int cb[4][64];
-    if (int rc = check_progression(s, cb)) { std::string m = b200jpeg_last_error(); set_error("image %d: %s", i, m.c_str()); return rc; }
-    if (smoothing_applies(s, cb)) {
-      set_error("image %d: incomplete progression: the reference decompressor applies block smoothing to it (do_block_smoothing), which is not on the device path", i);
-      return B200JPEG_ERR_UNSUPPORTED;
-    }
-  }
-  return B200JPEG_OK;
+  return check_tables_progression(s, i);
 }
 
 // the multiplier tables of jddctmgr.c start_pass for the ifast and float IDCTs, from one quantization table
@@ -2071,6 +2078,177 @@ static int decompress_batch(b200jpeg_encoder *e, const b200jpeg_decompress_optio
   e->pending_marks = 0;
   e->stage_names.clear(); e->stage_ms.clear(); e->stage_calls.clear();
   add_decompress_stage_times(e);
+  return B200JPEG_OK;
+}
+
+// b200jpeg_decompress_yuv_batch: the entropy decode chunk by chunk, then per component the IDCT that
+// tj3DecompressToYUVPlanes8 runs, stored straight into the planes (device planes), or into a compact staging buffer of
+// the batch's written samples copied out with one cudaMemcpy2DAsync per plane and image (host planes)
+static int decompress_yuv(b200jpeg_encoder *e, const b200jpeg_decompress_options *opts, const uint8_t *const *files, const size_t *sizes, int n,
+                          uint8_t *const *planes, int planes_on_device, const size_t *plane_pitch, const size_t *plane_stride)
+{
+  if (!e || !opts || !files || !sizes || !planes || !plane_pitch || !plane_stride || n <= 0) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
+  // every refusal comes before any device work
+  YuvPlan plan;
+  b200jpeg_source_info s0;
+  {
+    static thread_local b200jpeg_source_info s;
+    for (int i = 0; i < n; i++) {
+      if (!files[i]) { set_error("image %d: no file", i); return B200JPEG_ERR_PARAM; }
+      int rc = b200jpeg_parse_source(files[i], sizes[i], &s);
+      YuvPlan pi;
+      if (!rc) rc = plan_yuv(s, *opts, pi);
+      if (!rc && s.data_precision != 8) { set_error("Unsupported JPEG data precision %d", s.data_precision); rc = B200JPEG_ERR_PARAM; }   // JERR_BAD_PRECISION
+      if (!rc && s.sof == 0xC2 && !e->progressive_decode) { set_error("progressive (SOF2) source: only sequential files are decoded to planes unless progressive decode is on"); rc = B200JPEG_ERR_UNSUPPORTED; }
+      if (rc) { std::string m = b200jpeg_last_error(); set_error("image %d: %s", i, m.c_str()); return rc; }
+      if ((rc = check_tables_progression(s, i))) return rc;
+      if (i == 0) { s0 = s; plan = pi; }
+      bool same = s.image_width == s0.image_width && s.image_height == s0.image_height && s.num_components == s0.num_components;
+      for (int c = 0; same && c < s.num_components; c++) same = s.h_samp_factor[c] == s0.h_samp_factor[c] && s.v_samp_factor[c] == s0.v_samp_factor[c];
+      if (!same) { set_error("image %d: geometry (size, components, sampling) differs from image 0", i); return B200JPEG_ERR_PARAM; }
+    }
+  }
+  const int nc = plan.nc;
+  int cw[3], ch[3];                                        // the samples written: the IDCT output inside the plane
+  for (int c = 0; c < nc; c++) {
+    cw[c] = std::min(plan.iw[c], plan.pw[c]); ch[c] = std::min(plan.ih[c], plan.ph[c]);
+    if (!planes[c]) { set_error("plane %d: no destination", c); return B200JPEG_ERR_PARAM; }
+    if (plane_pitch[c] < (size_t)plan.pw[c] || (n > 1 && plane_stride[c] < plane_pitch[c] * (size_t)(plan.ph[c] - 1) + (size_t)plan.pw[c])) {
+      set_error("plane %d: pitch %zu or stride %zu smaller than the plane (%dx%d)", c, plane_pitch[c], plane_stride[c], plan.pw[c], plan.ph[c]);
+      return B200JPEG_ERR_PARAM;
+    }
+  }
+  CU(cudaSetDevice(e->device));
+  uint8_t *dst[3]; size_t dp[3], ds[3];
+  if (planes_on_device) {
+    for (int c = 0; c < nc; c++) { dst[c] = planes[c]; dp[c] = plane_pitch[c]; ds[c] = plane_stride[c]; }
+  } else {
+    size_t off[3], total = 0;
+    for (int c = 0; c < nc; c++) { dp[c] = (size_t)cw[c]; ds[c] = dp[c] * ch[c]; off[c] = total; total += (ds[c] * n + 255) & ~(size_t)255; }
+    if (int rc = e->d_dec_pixels.reserve(total)) return rc;
+    for (int c = 0; c < nc; c++) dst[c] = e->d_dec_pixels.as<uint8_t>() + off[c];
+  }
+  while (e->pix_ev.size() < 2) { cudaEvent_t ev; CU(cudaEventCreate(&ev)); e->pix_ev.push_back(ev); }
+  for (float &m : e->dec_ms) m = 0.f;
+  e->dec_ms_prog = false;
+  e->dec.want_markers = false;
+  // chunks of about 1.6 M blocks, as decompress_files
+  long long per = 0;
+  for (int c = 0; c < nc; c++) per += (long long)(plan.iw[c] / plan.k) * (plan.ih[c] / plan.k);
+  const int C = std::min(n, e->chunk_images_override > 0 ? e->chunk_images_override : (int)std::max(1LL, 1600000LL / std::max(1LL, per)));
+  e->chunk = C;
+  // the ifast multiplier tables: for the 8x8 ifast IDCT, and for 4:2:0 chroma at 1/2 under IFAST
+  bool need_mt = plan.k == 8 && plan.method == B200JPEG_DCT_IFAST;
+  for (int c = 0; c < nc; c++) need_mt |= plan.int_table[c];
+  std::vector<uint16_t> qt;
+  std::vector<uint32_t> mt;
+  cudaStream_t s = e->stream;
+  for (int i0 = 0; i0 < n; i0 += C) {
+    const int nk = std::min(C, n - i0);
+    int rc = decode_files(e, files + i0, sizes + i0, nk, i0);
+    if (rc) return rc;
+    e->dec_ms_prog |= e->dec_prog;
+    if ((rc = e->d_dec_quant.reserve((size_t)nk * nc * 128)) || (need_mt && (rc = e->d_dec_mtab.reserve((size_t)nk * nc * 256)))) return rc;
+    if ((rc = upload_chunk_quant(e, nk, qt))) return rc;
+    if (need_mt) {
+      mt.resize((size_t)nk * nc * 64);
+      for (size_t t = 0; t < (size_t)nk * nc; t++) method_table(B200JPEG_DCT_IFAST, &qt[t * 64], &mt[t * 64]);
+      CU(cudaMemcpyAsync(e->d_dec_mtab.p, mt.data(), mt.size() * 4, cudaMemcpyHostToDevice, s));
+    }
+    const DecGeom &g = e->dec.geom[0];
+    CU(cudaEventRecord(e->pix_ev[0], s));
+    for (int c = 0; c < nc; c++) {
+      const bool by_mt = (plan.k == 8 && plan.method == B200JPEG_DCT_IFAST) || plan.int_table[c];
+      const void *tab = by_mt ? static_cast<const void *>(e->d_dec_mtab.as<uint32_t>() + c * 64) : static_cast<const void *>(e->d_dec_quant.as<uint16_t>() + c * 64);
+      const IdctDst d = {(long long)dp[c], (long long)ds[c], cw[c], ch[c]};
+      launch_idct_plane(plan.k, plan.method, plan.int_table[c], reinterpret_cast<const int16_t *>(e->d_dec_planes.as<uint8_t>() + e->dec_plane_off[c]), tab, nc * 64,
+                        dst[c] + (size_t)i0 * ds[c], d, g.wib[c], g.hib[c], nk, s);
+    }
+    CU(cudaEventRecord(e->pix_ev[1], s));
+    CU(cudaGetLastError());
+    CU(cudaStreamSynchronize(s));
+    sum_decode_stage_times(e);
+    float ms = 0.f; cudaEventElapsedTime(&ms, e->pix_ev[0], e->pix_ev[1]); e->dec_ms[6] += ms;
+  }
+  if (!planes_on_device) {
+    for (int i = 0; i < n; i++)
+      for (int c = 0; c < nc; c++)
+        if (cw[c] > 0 && ch[c] > 0)
+          CU(cudaMemcpy2DAsync(planes[c] + (size_t)i * plane_stride[c], plane_pitch[c], dst[c] + (size_t)i * ds[c], dp[c], cw[c], ch[c], cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+  }
+  e->pending_marks = 0;
+  e->stage_names.clear(); e->stage_ms.clear(); e->stage_calls.clear();
+  for (int k = 0; k < (e->dec_ms_prog ? 8 : 6); k++) { e->stage_names.push_back(kDecStages[k]); e->stage_ms.push_back(e->dec_ms[k < 6 ? k : k + 2]); e->stage_calls.push_back(1); }
+  e->stage_names.push_back("idct"); e->stage_ms.push_back(e->dec_ms[6]); e->stage_calls.push_back(1);
+  return B200JPEG_OK;
+}
+
+// b200jpeg_decode_yuv_batch: host planes are staged into one compact device buffer (one cudaMemcpy2DAsync per plane
+// and image), host pixels come back through one (one copy per image); then a single k_yuv_to_pixels launch
+static int decode_yuv(b200jpeg_encoder *e, const b200jpeg_params *p, const uint8_t *const *planes, int planes_on_device, const size_t *plane_pitch,
+                      const size_t *plane_stride, void *pixels, int pixels_on_device, size_t row_pitch, size_t image_stride, int n)
+{
+  if (!e || !p || !planes || !plane_pitch || !plane_stride || !pixels || n <= 0 || p->image_width <= 0 || p->image_height <= 0) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
+  if (p->data_precision != 8) { set_error("data_precision %d: YUV planes are decoded at 8 bits", p->data_precision); return B200JPEG_ERR_PARAM; }
+  const int cs = p->in_color_space, nc = p->num_components, W = p->image_width, H = p->image_height;
+  if (cs == B200JPEG_CS_CMYK) { set_error("Cannot decode YUV images into packed-pixel CMYK images."); return B200JPEG_ERR_PARAM; }
+  if (cs != B200JPEG_CS_GRAYSCALE && !B200JPEG_CS_IS_RGB(cs)) { set_error("in_color_space %d is not a TurboJPEG pixel format", cs); return B200JPEG_ERR_PARAM; }
+  // the TJSAMP_* the planes are in: gray, or YCbCr with component 0 at 1, 2 or 4 each way (as tj3_params sets them) over 1x1 chroma
+  const b200jpeg_component_info *ci = p->comp_info;
+  const int h0 = ci[0].h_samp_factor, v0 = ci[0].v_samp_factor;
+  bool known = (nc == 1 && p->jpeg_color_space == B200JPEG_CS_GRAYSCALE) ||
+               (nc == 3 && p->jpeg_color_space == B200JPEG_CS_YCbCr && ci[1].h_samp_factor == 1 && ci[1].v_samp_factor == 1 && ci[2].h_samp_factor == 1 &&
+                ci[2].v_samp_factor == 1 && ((h0 == 1 && v0 == 1) || (h0 == 2 && v0 == 1) || (h0 == 2 && v0 == 2) || (h0 == 1 && v0 == 2) || (h0 == 4 && v0 == 1) || (h0 == 1 && v0 == 4)));
+  if (!known) { set_error("TJPARAM_SUBSAMP must be specified (the parameter block's components and sampling name no TJSAMP_* layout)"); return B200JPEG_ERR_PARAM; }
+  const int ps = cs == B200JPEG_CS_GRAYSCALE ? 1 : B200JPEG_CS_PIXELSIZE(cs);
+  if (row_pitch < (size_t)W * ps || (n > 1 && image_stride < row_pitch * (size_t)(H - 1) + (size_t)W * ps)) { set_error("row_pitch or image_stride smaller than the image (%dx%d, %d bytes a pixel)", W, H, ps); return B200JPEG_ERR_PARAM; }
+  YuvPix d; memset(&d, 0, sizeof d);
+  d.ps = ps; d.hs = h0 == 4 ? 2 : h0 - 1; d.vs = v0 == 4 ? 2 : v0 - 1;
+  d.conv = cs == B200JPEG_CS_GRAYSCALE ? UPS_GRAY : nc == 1 ? UPS_GRAY_RGB : UPS_YCC_RGB;
+  if (ps > 1) {
+    const int f = B200JPEG_CS_FIRST(cs), bf = B200JPEG_CS_BLUE_FIRST(cs);
+    d.off[0] = f + (bf ? 2 : 0); d.off[1] = f + 1; d.off[2] = f + (bf ? 0 : 2); d.off[3] = f ? 0 : 3;
+  }
+  const int nread = d.conv == UPS_YCC_RGB ? 3 : 1;           // a gray pixel format reads luma only
+  int pw[3], ph[3];
+  for (int c = 0; c < nread; c++) {
+    b200jpeg_yuv_plane_dims(p, c, &pw[c], &ph[c]);
+    if (!planes[c]) { set_error("plane %d: no source", c); return B200JPEG_ERR_PARAM; }
+    if (plane_pitch[c] < (size_t)pw[c] || (n > 1 && plane_stride[c] < plane_pitch[c] * (size_t)(ph[c] - 1) + (size_t)pw[c])) {
+      set_error("plane %d: pitch %zu or stride %zu smaller than the plane (%dx%d)", c, plane_pitch[c], plane_stride[c], pw[c], ph[c]);
+      return B200JPEG_ERR_PARAM;
+    }
+  }
+  CU(cudaSetDevice(e->device));
+  cudaStream_t s = e->stream;
+  size_t off[3], total = 0;
+  for (int c = 0; c < nread; c++) { off[c] = total; total += ((size_t)pw[c] * ph[c] * n + 255) & ~(size_t)255; }
+  int rc;
+  if (!planes_on_device && (rc = e->d_dec_samples.reserve(total))) return rc;
+  const size_t dp = ((size_t)W * ps + 3) & ~(size_t)3, ds = dp * H;
+  if (!pixels_on_device && (rc = e->d_dec_pixels.reserve(ds * (size_t)n))) return rc;
+  while (e->pix_ev.size() < 2) { cudaEvent_t ev; CU(cudaEventCreate(&ev)); e->pix_ev.push_back(ev); }
+  for (int c = 0; c < nread; c++) {
+    if (planes_on_device) { d.plane[c] = planes[c]; d.pitch[c] = (long long)plane_pitch[c]; d.stride[c] = (long long)plane_stride[c]; continue; }
+    uint8_t *st = e->d_dec_samples.as<uint8_t>() + off[c];
+    d.plane[c] = st; d.pitch[c] = pw[c]; d.stride[c] = (long long)pw[c] * ph[c];
+    for (int i = 0; i < n; i++)
+      CU(cudaMemcpy2DAsync(st + (size_t)i * d.stride[c], pw[c], planes[c] + (size_t)i * plane_stride[c], plane_pitch[c], pw[c], ph[c], cudaMemcpyHostToDevice, s));
+  }
+  uint8_t *pix = pixels_on_device ? static_cast<uint8_t *>(pixels) : e->d_dec_pixels.as<uint8_t>();
+  CU(cudaEventRecord(e->pix_ev[0], s));
+  launch_yuv_to_pixels(d, pix, pixels_on_device ? row_pitch : dp, pixels_on_device ? image_stride : ds, W, H, n, s);
+  CU(cudaEventRecord(e->pix_ev[1], s));
+  CU(cudaGetLastError());
+  if (!pixels_on_device)
+    for (int i = 0; i < n; i++)
+      CU(cudaMemcpy2DAsync(static_cast<uint8_t *>(pixels) + (size_t)i * image_stride, row_pitch, pix + (size_t)i * ds, dp, (size_t)W * ps, H, cudaMemcpyDeviceToHost, s));
+  CU(cudaStreamSynchronize(s));
+  float ms = 0.f; cudaEventElapsedTime(&ms, e->pix_ev[0], e->pix_ev[1]);
+  e->pending_marks = 0;
+  e->stage_names.clear(); e->stage_ms.clear(); e->stage_calls.clear();
+  e->stage_names.push_back("yuv_to_pixels"); e->stage_ms.push_back(ms); e->stage_calls.push_back(1);
   return B200JPEG_OK;
 }
 
@@ -2671,6 +2849,20 @@ int b200jpeg_decompress_batch_opts(b200jpeg_encoder *e, const b200jpeg_decompres
 {
   if (!opts) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
   return b200::decompress_batch(e, opts, files, sizes, n_images, pixels, pixels_on_device, row_pitch, image_stride);
+}
+
+int b200jpeg_decompress_yuv_batch(b200jpeg_encoder *e, const b200jpeg_decompress_options *opts, const uint8_t *const *files,
+                                  const size_t *sizes, int n_images, uint8_t *const *planes, int planes_on_device,
+                                  const size_t *plane_pitch, const size_t *plane_stride)
+{
+  return b200::decompress_yuv(e, opts, files, sizes, n_images, planes, planes_on_device, plane_pitch, plane_stride);
+}
+
+int b200jpeg_decode_yuv_batch(b200jpeg_encoder *e, const b200jpeg_params *p, const uint8_t *const *planes, int planes_on_device,
+                              const size_t *plane_pitch, const size_t *plane_stride, void *pixels, int pixels_on_device,
+                              size_t row_pitch, size_t image_stride, int n_images)
+{
+  return b200::decode_yuv(e, p, planes, planes_on_device, plane_pitch, plane_stride, pixels, pixels_on_device, row_pitch, image_stride, n_images);
 }
 
 int b200jpeg_recompress_batch(b200jpeg_encoder *e, const b200jpeg_params *p, const uint8_t *const *files, const size_t *sizes, int n_images)

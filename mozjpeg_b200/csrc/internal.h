@@ -66,4 +66,15 @@ struct DecPlan {
   bool is_default = true;
 };
 int plan_decompress(const b200jpeg_source_info &s, const b200jpeg_decompress_options &o, DecPlan &p);
+
+// What tj3DecompressToYUVPlanes8 (turbojpeg.c:2032-2195) decides for one source and one set of options (source.cpp):
+// the TJSAMP_* getSubsamp assigns, the IDCT block size k every component runs (TurboJPEG overrides libjpeg's chroma
+// scaling for TJSAMP_420), the IDCT method (B200JPEG_DCT_ISLOW or _IFAST), and per component the plane pw x ph, the
+// IDCT output iw x ih and whether its table is the ifast multiplier table read by jpeg_idct_4x4 (int_table).
+struct YuvPlan {
+  int subsamp = -1, k = 8, method = 0, nc = 0, out_w = 0, out_h = 0;
+  int pw[3] = {0, 0, 0}, ph[3] = {0, 0, 0}, iw[3] = {0, 0, 0}, ih[3] = {0, 0, 0};
+  bool int_table[3] = {false, false, false};
+};
+int plan_yuv(const b200jpeg_source_info &s, const b200jpeg_decompress_options &o, YuvPlan &p);
 }

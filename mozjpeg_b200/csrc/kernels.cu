@@ -4399,10 +4399,12 @@ __device__ __forceinline__ int idct_range_limit(int x)
 // false): the plane holds [n][hib][wib] blocks, image i's table at i * qstride, the samples [n][hib * N][wib * N].
 // Ragged form: work[blockIdx.x] names the image (imgs[]) the CTA works on; each image's blocks are padded to whole
 // CTAs of BPC blocks, so a CTA never spans two images.
-struct IdctAt { bool valid; long long blk, q, o, pitch; };
-template <bool RAGGED, int BPC, int N>
+// PLANE form (one geometry): the samples go to pd's plane, image i's at i * pd.stride, rows pd.pitch apart; x0 / y0:
+// the block's first column and row there, for the clipping to pd.cw x pd.ch.
+struct IdctAt { bool valid; long long blk, q, o, pitch; int x0, y0; };
+template <bool RAGGED, int BPC, int N, bool PLANE = false>
 __device__ __forceinline__ IdctAt idct_at(int lb, int wib, int hib, long long nblocks, int qstride, const uint32_t *__restrict__ work,
-                                          const IdctImg *__restrict__ imgs)
+                                          const IdctImg *__restrict__ imgs, const IdctDst &pd = IdctDst())
 {
   IdctAt a;
   if (!RAGGED) {
@@ -4412,6 +4414,7 @@ __device__ __forceinline__ IdctAt idct_at(int lb, int wib, int hib, long long nb
     const int by = (int)(rem / wib), bx = (int)(rem - (long long)by * wib);
     a.q = img * qstride; a.pitch = (long long)wib * N;
     a.o = ((img * hib + by) * N) * a.pitch + bx * N;
+    if (PLANE) { a.pitch = pd.pitch; a.o = img * pd.stride + (long long)by * N * pd.pitch + bx * N; a.x0 = bx * N; a.y0 = by * N; }
   } else {
     const IdctImg d = imgs[work[blockIdx.x]];
     const long long b = (long long)(blockIdx.x - d.cta0) * BPC + lb;
@@ -4423,6 +4426,23 @@ __device__ __forceinline__ IdctAt idct_at(int lb, int wib, int hib, long long nb
   return a;
 }
 
+// the PLANE store of one sample row of a block: its N samples, packed little-endian in lo and hi, clipped to the first n
+// (none for n <= 0); whole aligned rows as one store
+template <int N>
+__device__ __forceinline__ void store_row_clipped(uint8_t *dst, unsigned lo, unsigned hi, int n)
+{
+  if (n >= N && (reinterpret_cast<uintptr_t>(dst) & (N - 1)) == 0) {
+    if (N == 8) *reinterpret_cast<uint2 *>(dst) = make_uint2(lo, hi);
+    else if (N == 4) *reinterpret_cast<uint32_t *>(dst) = lo;
+    else if (N == 2) *reinterpret_cast<uint16_t *>(dst) = (uint16_t)lo;
+    else *dst = (uint8_t)lo;
+    return;
+  }
+#pragma unroll
+  for (int k = 0; k < N; k++)
+    if (k < n) dst[k] = (uint8_t)((k < 4 ? lo : hi) >> (8 * (k & 3)));
+}
+
 // jpeg_idct_islow (jidctint.c:171-419, 8-bit: CONST_BITS 13, PASS1_BITS 2) with the dequantization of jddctmgr.c:
 // 134-146 (ISLOW_MULT_TYPE is a short: the table entries are taken as int16).  Eight lanes per block: each loads one
 // 16-byte row of the JBLOCK, transforms one column into the int workspace (pass 1), then one row into eight samples
@@ -4430,16 +4450,17 @@ __device__ __forceinline__ IdctAt idct_at(int lb, int wib, int hib, long long nb
 // butterfly gives, so there is no branch.  Pass 1 keeps the reference's 64-bit intermediates (JLONG): a file may carry
 // 16-bit coefficients under a 16-bit table; pass 2 needs bits 18..27 of its sums only, which 32-bit arithmetic keeps.
 // coef: [nblocks][64] natural order ([n][hib][wib] blocks); quant: image i's table at quant + i * qstride;
-// out: [n][hib * 8][wib * 8] samples.
-template <bool RAGGED>
+// out: [n][hib * 8][wib * 8] samples, or with PLANE pd's plane (idct_at).
+template <bool RAGGED, bool PLANE = false>
 __global__ void __launch_bounds__(IDCT_BLOCKS * 8) k_idct_islow(const int16_t *__restrict__ coef, const uint16_t *__restrict__ quant, int qstride,
                                                                 uint8_t *__restrict__ out, int wib, int hib, long long nblocks,
-                                                                const uint32_t *__restrict__ work, const IdctImg *__restrict__ imgs)
+                                                                const uint32_t *__restrict__ work, const IdctImg *__restrict__ imgs,
+                                                                IdctDst pd = IdctDst())
 {
   __shared__ int4 s_coef[IDCT_BLOCKS * 8];
   __shared__ int s_ws[IDCT_BLOCKS * IDCT_WS];
   const int lb = threadIdx.x >> 3, lane = threadIdx.x & 7;
-  const IdctAt at = idct_at<RAGGED, IDCT_BLOCKS, 8>(lb, wib, hib, nblocks, qstride, work, imgs);
+  const IdctAt at = idct_at<RAGGED, IDCT_BLOCKS, 8, PLANE>(lb, wib, hib, nblocks, qstride, work, imgs, pd);
   const bool valid = at.valid;
   s_coef[threadIdx.x] = valid ? reinterpret_cast<const int4 *>(coef)[at.blk * 8 + lane] : make_int4(0, 0, 0, 0);
   __syncwarp();
@@ -4497,7 +4518,9 @@ __global__ void __launch_bounds__(IDCT_BLOCKS * 8) k_idct_islow(const int16_t *_
     const unsigned o3 = idct_range_limit((int)((tmp13 + tmp0 + rnd) >> 18)), o4 = idct_range_limit((int)((tmp13 - tmp0 + rnd) >> 18));
     if (valid) {
       uint8_t *dst = out + at.o + lane * at.pitch;
-      *reinterpret_cast<uint2 *>(dst) = make_uint2(o0 | o1 << 8 | o2 << 16 | o3 << 24, o4 | o5 << 8 | o6 << 16 | o7 << 24);
+      const unsigned lo = o0 | o1 << 8 | o2 << 16 | o3 << 24, hi = o4 | o5 << 8 | o6 << 16 | o7 << 24;
+      if (!PLANE) *reinterpret_cast<uint2 *>(dst) = make_uint2(lo, hi);
+      else if (at.y0 + lane < pd.ch) store_row_clipped<8>(dst, lo, hi, pd.cw - at.x0);
     }
   }
 }
@@ -4618,15 +4641,18 @@ int launch_upsample_color(int hx, int vx, int nc, const uint8_t *const *planes, 
 // The reference's shortcuts for all-zero AC columns and rows give what the general path gives (pass 1: DESCALE of
 // dq << (CONST_BITS + 1 or 2) is dq << PASS1_BITS, truncated to int the same way; pass 2: both are DESCALE(w0, 5)), so
 // there is no branch.  N = 1: one thread per block reads the DC term only.
-// out: [n][hib * N][wib * N] samples.
-template <int N, bool RAGGED>
-__global__ void __launch_bounds__(IDCT_BLOCKS * 8) k_idct_red(const int16_t *__restrict__ coef, const uint16_t *__restrict__ quant, int qstride,
+// out: [n][hib * N][wib * N] samples, or with PLANE pd's plane (idct_at).  T: the table entries' type, uint16_t, or int
+// for the ifast multiplier table a TJSAMP_420 chroma component reads at 1/2 (products wrap modulo 2^32 as the
+// reference's int arithmetic does).
+template <int N, bool RAGGED, bool PLANE = false, typename T = uint16_t>
+__global__ void __launch_bounds__(IDCT_BLOCKS * 8) k_idct_red(const int16_t *__restrict__ coef, const T *__restrict__ quant, int qstride,
                                                               uint8_t *__restrict__ out, int wib, int hib, long long nblocks,
-                                                              const uint32_t *__restrict__ work, const IdctImg *__restrict__ imgs)
+                                                              const uint32_t *__restrict__ work, const IdctImg *__restrict__ imgs,
+                                                              IdctDst pd = IdctDst())
 {
   if (N == 1) {
-    const IdctAt at = idct_at<RAGGED, 256, 1>(threadIdx.x, wib, hib, nblocks, qstride, work, imgs);
-    if (!at.valid) return;
+    const IdctAt at = idct_at<RAGGED, 256, 1, PLANE>(threadIdx.x, wib, hib, nblocks, qstride, work, imgs, pd);
+    if (!at.valid || (PLANE && (at.x0 >= pd.cw || at.y0 >= pd.ch))) return;
     const int dq = (int)__ldg(coef + at.blk * 64) * (int)__ldg(quant + at.q);
     out[at.o] = (uint8_t)idct_range_limit((int)(((long long)dq + 4) >> 3));
     return;
@@ -4634,14 +4660,14 @@ __global__ void __launch_bounds__(IDCT_BLOCKS * 8) k_idct_red(const int16_t *__r
   __shared__ int4 s_coef[IDCT_BLOCKS * 8];
   __shared__ int s_ws[IDCT_BLOCKS * IDCT_WS];
   const int lb = threadIdx.x >> 3, lane = threadIdx.x & 7;
-  const IdctAt at = idct_at<RAGGED, IDCT_BLOCKS, N>(lb, wib, hib, nblocks, qstride, work, imgs);
+  const IdctAt at = idct_at<RAGGED, IDCT_BLOCKS, N, PLANE>(lb, wib, hib, nblocks, qstride, work, imgs, pd);
   const bool valid = at.valid;
   s_coef[threadIdx.x] = valid ? reinterpret_cast<const int4 *>(coef)[at.blk * 8 + lane] : make_int4(0, 0, 0, 0);
   __syncwarp();
   const bool col_used = N == 4 ? lane != 4 : (lane & 1) || lane == 0;
   if (col_used) {                                         // pass 1: column `lane` -> ws rows 0 .. N-1
     const int16_t *c = reinterpret_cast<const int16_t *>(s_coef + lb * 8) + lane;
-    const uint16_t *q = quant + at.q + lane;
+    const T *q = quant + at.q + lane;
     long long d[8];
 #pragma unroll
     for (int r = 0; r < 8; r++) d[r] = (N == 4 && r == 4) || (N == 2 && (r == 2 || r == 4 || r == 6)) ? 0 : (long long)((int)c[r * 8] * (int)q[r * 8]);
@@ -4659,7 +4685,7 @@ __global__ void __launch_bounds__(IDCT_BLOCKS * 8) k_idct_red(const int16_t *__r
     }
   }
   __syncwarp();
-  if (valid && lane < N) {                                // pass 2: row `lane`
+  if (valid && lane < N && (!PLANE || at.y0 + lane < pd.ch)) {   // pass 2: row `lane`
     const int *w = s_ws + lb * IDCT_WS + lane * 9;
     uint8_t *dst = out + at.o + lane * at.pitch;
     if (N == 4) {
@@ -4671,13 +4697,15 @@ __global__ void __launch_bounds__(IDCT_BLOCKS * 8) k_idct_red(const int16_t *__r
       const long long rnd = 1LL << 18;
       const unsigned s0 = idct_range_limit((int)((tmp10 + o2 + rnd) >> 19)), s3 = idct_range_limit((int)((tmp10 - o2 + rnd) >> 19));
       const unsigned s1 = idct_range_limit((int)((tmp12 + o0 + rnd) >> 19)), s2 = idct_range_limit((int)((tmp12 - o0 + rnd) >> 19));
-      *reinterpret_cast<uint32_t *>(dst) = s0 | s1 << 8 | s2 << 16 | s3 << 24;
+      if (!PLANE) *reinterpret_cast<uint32_t *>(dst) = s0 | s1 << 8 | s2 << 16 | s3 << 24;
+      else store_row_clipped<4>(dst, s0 | s1 << 8 | s2 << 16 | s3 << 24, 0, pd.cw - at.x0);
     } else {
       const long long tmp10 = (long long)w[0] * 32768;
       const long long o0 = (long long)w[7] * -5906 + (long long)w[5] * 6967 + (long long)w[3] * -10426 + (long long)w[1] * 29692;
       const long long rnd = 1LL << 19;
       const unsigned s0 = idct_range_limit((int)((tmp10 + o0 + rnd) >> 20)), s1 = idct_range_limit((int)((tmp10 - o0 + rnd) >> 20));
-      *reinterpret_cast<uint16_t *>(dst) = (uint16_t)(s0 | s1 << 8);
+      if (!PLANE) *reinterpret_cast<uint16_t *>(dst) = (uint16_t)(s0 | s1 << 8);
+      else store_row_clipped<2>(dst, s0 | s1 << 8, 0, pd.cw - at.x0);
     }
   }
 }
@@ -4709,15 +4737,16 @@ __device__ __forceinline__ void ifast_1d(const unsigned d[8], unsigned o[8])
 
 // jpeg_idct_ifast with its multiplier table (jddctmgr.c: quantval * aanscales descaled to IFAST_SCALE_BITS, int),
 // image i's at mtab + i * qstride.  Shape of k_idct_islow.  The all-zero shortcuts give the general path's values.
-template <bool RAGGED>
+template <bool RAGGED, bool PLANE = false>
 __global__ void __launch_bounds__(IDCT_BLOCKS * 8) k_idct_ifast(const int16_t *__restrict__ coef, const int *__restrict__ mtab, int qstride,
                                                                 uint8_t *__restrict__ out, int wib, int hib, long long nblocks,
-                                                                const uint32_t *__restrict__ work, const IdctImg *__restrict__ imgs)
+                                                                const uint32_t *__restrict__ work, const IdctImg *__restrict__ imgs,
+                                                                IdctDst pd = IdctDst())
 {
   __shared__ int4 s_coef[IDCT_BLOCKS * 8];
   __shared__ int s_ws[IDCT_BLOCKS * IDCT_WS];
   const int lb = threadIdx.x >> 3, lane = threadIdx.x & 7;
-  const IdctAt at = idct_at<RAGGED, IDCT_BLOCKS, 8>(lb, wib, hib, nblocks, qstride, work, imgs);
+  const IdctAt at = idct_at<RAGGED, IDCT_BLOCKS, 8, PLANE>(lb, wib, hib, nblocks, qstride, work, imgs, pd);
   const bool valid = at.valid;
   s_coef[threadIdx.x] = valid ? reinterpret_cast<const int4 *>(coef)[at.blk * 8 + lane] : make_int4(0, 0, 0, 0);
   __syncwarp();
@@ -4744,7 +4773,9 @@ __global__ void __launch_bounds__(IDCT_BLOCKS * 8) k_idct_ifast(const int16_t *_
     for (int k = 0; k < 8; k++) s[k] = idct_range_limit((int)o[k] >> 5);        // IDESCALE(x, PASS1_BITS + 3)
     if (valid) {
       uint8_t *dst = out + at.o + lane * at.pitch;
-      *reinterpret_cast<uint2 *>(dst) = make_uint2(s[0] | s[1] << 8 | s[2] << 16 | s[3] << 24, s[4] | s[5] << 8 | s[6] << 16 | s[7] << 24);
+      const unsigned lo = s[0] | s[1] << 8 | s[2] << 16 | s[3] << 24, hi = s[4] | s[5] << 8 | s[6] << 16 | s[7] << 24;
+      if (!PLANE) *reinterpret_cast<uint2 *>(dst) = make_uint2(lo, hi);
+      else if (at.y0 + lane < pd.ch) store_row_clipped<8>(dst, lo, hi, pd.cw - at.x0);
     }
   }
 }
@@ -4927,6 +4958,52 @@ void launch_upsample_opts(const UpsOpt &o, uint8_t *pix, size_t row_pitch, size_
 void launch_upsample_ragged(const uint32_t *work, const UpsImg *imgs, unsigned ncta, cudaStream_t s)
 {
   k_upsample_ragged<<<ncta, dim3(64, 4), 0, s>>>(work, imgs); LAUNCHED();
+}
+
+// tj3DecodeYUVPlanes8 with do_fancy_upsampling off: the merged upsampler (4:2:0, 4:2:2 to the RGB family) and
+// int_upsample (4:4:0, 4:1:1, 4:4:1) both replicate chroma, so each pixel reads one luma and one sample of each chroma
+// plane, then ycc_rgb_convert (jdcolor.c, SCALEBITS 16; the merged upsampler's tables give the same values),
+// gray_rgb_convert or grayscale_convert.  One thread per pixel; rows past H are never made (rows_to_go).  It shares no
+// code with k_upsample_opts, so that kernel and the pixel routes built on it stay as they are.
+__global__ void __launch_bounds__(256) k_yuv_to_pixels(YuvPix d, uint8_t *__restrict__ pix, long long row_pitch, long long image_stride, int W, int H)
+{
+  const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
+  const long long img = blockIdx.z;
+  if (x >= W || y >= H) return;
+  const int l = __ldg(d.plane[0] + img * d.stride[0] + (long long)y * d.pitch[0] + x);
+  uint8_t *o = pix + img * image_stride + (long long)y * row_pitch + (long long)x * d.ps;
+  if (d.conv == UPS_GRAY) { o[0] = (uint8_t)l; return; }
+  int r = l, g = l, b = l;
+  if (d.conv == UPS_YCC_RGB) {
+    const long long cy = y >> d.vs, cx = x >> d.hs;
+    const int u = __ldg(d.plane[1] + img * d.stride[1] + cy * d.pitch[1] + cx) - 128;
+    const int w = __ldg(d.plane[2] + img * d.stride[2] + cy * d.pitch[2] + cx) - 128;
+    r = min(max(l + ((91881 * w + 32768) >> 16), 0), 255);
+    g = min(max(l + ((-22554 * u + 32768 - 46802 * w) >> 16), 0), 255);
+    b = min(max(l + ((116130 * u + 32768) >> 16), 0), 255);
+  }
+  o[d.off[0]] = (uint8_t)r; o[d.off[1]] = (uint8_t)g; o[d.off[2]] = (uint8_t)b;
+  if (d.ps == 4) o[d.off[3]] = 0xFF;
+}
+
+void launch_yuv_to_pixels(const YuvPix &d, uint8_t *pix, size_t row_pitch, size_t image_stride, int W, int H, int n, cudaStream_t s)
+{
+  const dim3 cta(64, 4), grid((unsigned)((W + 63) / 64), (unsigned)((H + 3) / 4), (unsigned)n);
+  k_yuv_to_pixels<<<grid, cta, 0, s>>>(d, pix, (long long)row_pitch, (long long)image_stride, W, H); LAUNCHED();
+}
+
+void launch_idct_plane(int size, int method, bool int_table, const int16_t *coef, const void *tab, int qstride, uint8_t *out, const IdctDst &d,
+                       int wib, int hib, int n, cudaStream_t s)
+{
+  const long long nblocks = (long long)n * wib * hib;
+  const unsigned grid8 = (unsigned)((nblocks + IDCT_BLOCKS - 1) / IDCT_BLOCKS);
+  const uint16_t *q = static_cast<const uint16_t *>(tab);
+  if (size == 1) { k_idct_red<1, false, true><<<(unsigned)((nblocks + 255) / 256), 256, 0, s>>>(coef, q, qstride, out, wib, hib, nblocks, nullptr, nullptr, d); LAUNCHED(); }
+  else if (size == 2) { k_idct_red<2, false, true><<<grid8, IDCT_BLOCKS * 8, 0, s>>>(coef, q, qstride, out, wib, hib, nblocks, nullptr, nullptr, d); LAUNCHED(); }
+  else if (size == 4 && int_table) { k_idct_red<4, false, true, int><<<grid8, IDCT_BLOCKS * 8, 0, s>>>(coef, static_cast<const int *>(tab), qstride, out, wib, hib, nblocks, nullptr, nullptr, d); LAUNCHED(); }
+  else if (size == 4) { k_idct_red<4, false, true><<<grid8, IDCT_BLOCKS * 8, 0, s>>>(coef, q, qstride, out, wib, hib, nblocks, nullptr, nullptr, d); LAUNCHED(); }
+  else if (method == 1) { k_idct_ifast<false, true><<<grid8, IDCT_BLOCKS * 8, 0, s>>>(coef, static_cast<const int *>(tab), qstride, out, wib, hib, nblocks, nullptr, nullptr, d); LAUNCHED(); }
+  else { k_idct_islow<false, true><<<grid8, IDCT_BLOCKS * 8, 0, s>>>(coef, q, qstride, out, wib, hib, nblocks, nullptr, nullptr, d); LAUNCHED(); }
 }
 
 }  // namespace b200

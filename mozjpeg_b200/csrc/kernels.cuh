@@ -324,6 +324,20 @@ void launch_idct_ragged(int size, int method, const int16_t *coef, const void *t
 struct UpsImg { UpsOpt o; uint8_t *pix; long long row_pitch; int W, H, cta0, gx; };
 void launch_upsample_ragged(const uint32_t *work, const UpsImg *imgs, unsigned ncta, cudaStream_t s);
 
+// Decompression to YUV planes (jpeg_read_raw_data): the IDCT kernels above with their PLANE store, which writes image
+// i's samples straight into out + i * stride, rows `pitch` bytes apart, clipped to the first cw columns and ch rows.
+// size as for launch_idct_opts, method 0 (islow) or 1 (ifast: tab as for launch_idct_opts); int_table: size 4 reading an int table (tab as for method 1) the way
+// jpeg_idct_4x4 reads its islow table, which is what a TJSAMP_420 chroma component gets at 1/2 with JDCT_IFAST.
+struct IdctDst { long long pitch, stride; int cw, ch; };
+// Decoding YUV planes to pixels (tj3DecodeYUVPlanes8, do_fancy_upsampling off): pixel (x, y) of image i from luma
+// sample (x, y) and chroma sample (x >> hs, y >> vs) of image i's planes (plane[c] + i * stride[c], pitch[c] bytes a
+// row); conv UPS_GRAY (luma only), UPS_GRAY_RGB or UPS_YCC_RGB; ps bytes a pixel with R, G, B at off[0..2] and 0xFF at
+// off[3] when ps is 4.
+struct YuvPix { const uint8_t *plane[3]; long long pitch[3], stride[3]; int hs, vs, conv, ps, off[4]; };
+void launch_yuv_to_pixels(const YuvPix &d, uint8_t *pix, size_t row_pitch, size_t image_stride, int W, int H, int n, cudaStream_t s);
+void launch_idct_plane(int size, int method, bool int_table, const int16_t *coef, const void *tab, int qstride, uint8_t *out, const IdctDst &d,
+                       int wib, int hib, int n, cudaStream_t s);
+
 extern unsigned long long g_kernel_launches;
 
 }  // namespace b200

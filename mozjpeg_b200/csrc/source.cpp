@@ -335,7 +335,101 @@ int plan_decompress(const b200jpeg_source_info &s, const b200jpeg_decompress_opt
   return B200JPEG_OK;
 }
 
+// TJSAMP_* geometry (turbojpeg.h tjMCUWidth / tjMCUHeight): 444, 422, 420, GRAY, 440, 411, 441
+static const int kTjMcuW[7] = {8, 16, 16, 8, 8, 32, 8}, kTjMcuH[7] = {8, 8, 16, 8, 16, 8, 32};
+
+// getSubsamp (turbojpeg.c:400-479), including its non-standard 4:2:2, 4:4:0 and 4:4:4 spellings; -1 for TJSAMP_UNKNOWN
+static int tj_subsamp(const b200jpeg_source_info &s)
+{
+  const int nc = s.num_components;
+  const bool cmyk = s.jpeg_color_space == B200JPEG_CS_YCCK || s.jpeg_color_space == B200JPEG_CS_CMYK;
+  if (nc == 1 && s.jpeg_color_space == B200JPEG_CS_GRAYSCALE) return B200JPEG_TJSAMP_GRAY;
+  int r = -1;
+  for (int i = 0; i < 7; i++) {
+    if (i == B200JPEG_TJSAMP_GRAY) continue;
+    if (nc != 3 && !(cmyk && nc == 4)) continue;
+    const int h0 = s.h_samp_factor[0], v0 = s.v_samp_factor[0];
+    if (h0 == kTjMcuW[i] / 8 && v0 == kTjMcuH[i] / 8) {
+      int match = 0;
+      for (int k = 1; k < nc; k++) {
+        const int href = cmyk && k == 3 ? kTjMcuW[i] / 8 : 1, vref = cmyk && k == 3 ? kTjMcuH[i] / 8 : 1;
+        match += s.h_samp_factor[k] == href && s.v_samp_factor[k] == vref;
+      }
+      if (match == nc - 1) return i;
+    }
+    if (h0 == 2 && v0 == 2 && (i == B200JPEG_TJSAMP_422 || i == B200JPEG_TJSAMP_440)) {
+      int match = 0;
+      for (int k = 1; k < nc; k++) {
+        const int href = cmyk && k == 3 ? 2 : kTjMcuH[i] / 8, vref = cmyk && k == 3 ? 2 : kTjMcuW[i] / 8;
+        match += s.h_samp_factor[k] == href && s.v_samp_factor[k] == vref;
+      }
+      if (match == nc - 1) return i;
+    }
+    // the reference's `break` here leaves only its component loop, so a later layout may still claim the file
+    if (h0 * v0 <= 10 / 3 && i == B200JPEG_TJSAMP_444) {
+      int match = 0;
+      for (int k = 1; k < nc; k++) {
+        match += s.h_samp_factor[k] == h0 && s.v_samp_factor[k] == v0;
+        if (match == nc - 1) { r = i; break; }
+      }
+    }
+  }
+  return r;
+}
+
+// tj3YUVPlaneWidth / tj3YUVPlaneHeight (turbojpeg.c:1051-1110)
+static int tj_plane_w(int ci, int w, int ss) { const int pw = (w + kTjMcuW[ss] / 8 - 1) / (kTjMcuW[ss] / 8) * (kTjMcuW[ss] / 8); return ci == 0 ? pw : pw * 8 / kTjMcuW[ss]; }
+static int tj_plane_h(int ci, int h, int ss) { const int ph = (h + kTjMcuH[ss] / 8 - 1) / (kTjMcuH[ss] / 8) * (kTjMcuH[ss] / 8); return ci == 0 ? ph : ph * 8 / kTjMcuH[ss]; }
+
+int plan_yuv(const b200jpeg_source_info &s, const b200jpeg_decompress_options &o, YuvPlan &p)
+{
+  p = YuvPlan();
+  static const int kTjScale[16][2] = {{2, 1}, {15, 8}, {7, 4}, {13, 8}, {3, 2}, {11, 8}, {5, 4}, {9, 8}, {1, 1}, {7, 8}, {3, 4}, {5, 8}, {1, 2}, {3, 8}, {1, 4}, {1, 8}};
+  bool tj_scale = false;
+  for (const int *f : kTjScale) tj_scale |= o.scale_num == f[0] && o.scale_denom == f[1];
+  if (!tj_scale) { set_error("scale %d/%d: Unsupported scaling factor (TurboJPEG's factors are n/8 for n = 1 .. 16, in lowest terms)", o.scale_num, o.scale_denom); return B200JPEG_ERR_PARAM; }
+  if (o.dct_method != B200JPEG_DCT_ISLOW && o.dct_method != B200JPEG_DCT_IFAST) { set_error("dct_method %d: TurboJPEG decompresses to YUV with JDCT_ISLOW or JDCT_IFAST (TJPARAM_FASTDCT) only", o.dct_method); return B200JPEG_ERR_PARAM; }
+  if (o.do_fancy_upsampling != 1 || o.out_color_space != -1) { set_error("do_fancy_upsampling %d, out_color_space %d: decompression to YUV planes has no upsampling or colour conversion, so both must keep their defaults (1, -1)", o.do_fancy_upsampling, o.out_color_space); return B200JPEG_ERR_PARAM; }
+  const int nc = s.num_components;
+  p.subsamp = tj_subsamp(s);
+  if (p.subsamp < 0) return bad(B200JPEG_ERR_PARAM, "Could not determine subsampling level of JPEG image");
+  if (nc > 3) return bad(B200JPEG_ERR_PARAM, "JPEG image must have 3 or fewer components");
+  const int k = 8 * o.scale_num / o.scale_denom;
+  if (k != 1 && k != 2 && k != 4 && k != 8) {
+    set_error("scale %d/%d gives an IDCT block size of %d: only sizes 1, 2, 4 and 8 (1/8, 1/4, 1/2, 1/1) are decoded on the device", o.scale_num, o.scale_denom, k);
+    return B200JPEG_ERR_UNSUPPORTED;
+  }
+  p.k = k; p.method = o.dct_method; p.nc = nc;
+  const long long W = s.image_width, H = s.image_height;
+  p.out_w = (int)((W * k + 7) / 8); p.out_h = (int)((H * k + 7) / 8);       // jpeg_calc_output_dimensions
+  int mh = 1, mv = 1;
+  for (int c = 0; c < nc; c++) { mh = std::max(mh, s.h_samp_factor[c]); mv = std::max(mv, s.v_samp_factor[c]); }
+  for (int c = 0; c < nc; c++) {
+    const long long wib = (W * s.h_samp_factor[c] + mh * 8 - 1) / (mh * 8), hib = (H * s.v_samp_factor[c] + mv * 8 - 1) / (mv * 8);
+    p.iw[c] = (int)(wib * k); p.ih[c] = (int)(hib * k);
+    p.pw[c] = tj_plane_w(c, p.out_w, p.subsamp); p.ph[c] = tj_plane_h(c, p.out_h, p.subsamp);
+    // libjpeg doubles a 4:2:0 chroma IDCT below 1/1 and builds its table for that size; TurboJPEG then runs luma's
+    // IDCT on it, so at 1/2 jpeg_idct_4x4 reads the table start_pass built for an 8x8 IDCT of dct_method
+    p.int_table[c] = c > 0 && p.subsamp == B200JPEG_TJSAMP_420 && k == 4 && o.dct_method == B200JPEG_DCT_IFAST;
+  }
+  return B200JPEG_OK;
+}
+
 }  // namespace b200
+
+extern "C" int b200jpeg_decompress_yuv_dims(const b200jpeg_source_info *src, const b200jpeg_decompress_options *opts, int ci,
+                                            int *width, int *height, int *subsamp)
+{
+  if (!src || !opts || src->num_components < 1) return bad(B200JPEG_ERR_PARAM, "bad argument");
+  YuvPlan p;
+  const int rc = plan_yuv(*src, *opts, p);
+  if (rc) return rc;
+  if (ci < 0 || ci >= p.nc) { set_error("component %d: the source has %d", ci, p.nc); return B200JPEG_ERR_PARAM; }
+  if (width) *width = p.pw[ci];
+  if (height) *height = p.ph[ci];
+  if (subsamp) *subsamp = p.subsamp;
+  return B200JPEG_OK;
+}
 
 extern "C" int b200jpeg_decompress_output_opts(const b200jpeg_source_info *src, const b200jpeg_decompress_options *opts,
                                                int *width, int *height, int *color_space, int *components)

@@ -10,7 +10,7 @@ Inputs are either the reference's own test image (testimages/testorig.ppm,
 copied to tests/golden/ as a data fixture) or synthetic images generated from
 a seed by oracle.synth_image (SURVEY 8d).
 """
-import hashlib, json, os, shutil, sys
+import ctypes as C, hashlib, json, os, shutil, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import numpy as np
@@ -335,6 +335,50 @@ def yuv():
     print("wrote", len(cases), "YUV cases;", sum("error" in c for c in cases), "refusals")
 
 
+def yuv_decode():
+    """tests/golden/yuv_decode_golden.json: the reference's tj3DecompressToYUVPlanes8 (oracle/_ref/libturbojpeg_ref.so
+    through ctypes) on every (source, scale, dct) of tests/yuv_decode_cases.py: the TJSAMP_*, each plane's size and the
+    md5 of its defined samples (yuv_decode_cases.defined), or the reference's refusal."""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import yuv_decode_cases as Y
+    import mozjpeg_b200 as mj
+    from mozjpeg_b200 import _abi as A
+    ref = Y.RefTJ()
+    cases = []
+    for cid, sid, scale, dct in Y.cases():
+        src = Y.source(sid)
+        ss, planes, err = ref.decompress_planes(src, scale, dct)
+        c = {"id": cid, "src_md5": hashlib.md5(src).hexdigest()}
+        if err is not None:
+            c["error"] = err
+        else:
+            info = A.SourceInfo()
+            A.check(mj._lib.b200jpeg_parse_source(src, len(src), C.byref(info)), "parse_source")
+            _, dims = Y.plan(info, scale)
+            c["subsamp"] = Y.SUBSAMPS[ss]
+            c["dims"] = [list(p.shape[::-1]) for p in planes]
+            c["md5"] = [Y.md5(Y.defined(p, *d)) for p, d in zip(planes, dims)]
+        cases.append(c)
+    recompress = []
+    for sid, scale, dct in Y.RECOMPRESS:
+        src = Y.source(sid)
+        info = A.SourceInfo()
+        A.check(mj._lib.b200jpeg_parse_source(src, len(src), C.byref(info)), "parse_source")
+        _, dims = Y.plan(info, scale)
+        assert all(iw >= pw and ih >= ph for pw, ph, iw, ih in dims), (sid, scale, "planes not fully defined")
+        out = ref.recompress(src, scale, dct)
+        recompress.append({"id": Y.case_id(sid, scale, dct), "md5": hashlib.md5(out).hexdigest(), "size": len(out)})
+    decode = []
+    for did, ss, (w, h), pf, pad in Y.decode_cases():
+        px, err = ref.decode_pixels(Y.decode_planes(ss, w, h), ss, w, h, pf, pad)
+        decode.append({"id": did, "error": err} if err is not None else {"id": did, "md5": Y.md5(px), "shape": list(px.shape)})
+    ref.close()
+    json.dump({"generator": "tools/make_golden.py --yuv-decode", "reference": "mozilla/mozjpeg 5.0.0 (C path, WITH_SIMD=0), oracle/_ref",
+               "cases": cases, "recompress": recompress, "decode": decode}, open(os.path.join(GOLD, "yuv_decode_golden.json"), "w"), indent=0)
+    print("wrote", len(cases), "YUV decompress cases;", sum("error" in c for c in cases), "refusals;", len(recompress), "recompress;",
+          len(decode), "decode cases,", sum("error" in c for c in decode), "refused")
+
+
 def decode():
     """tests/golden/decode_golden.json: for every source of tests/decode_cases.py, the md5 of the file and of the
     reference's jpeg_read_coefficients planes for it (oracle/_ref/librefshim.so through ctypes)."""
@@ -481,6 +525,8 @@ def main():
         return transform()
     if "--decode" in sys.argv:
         return decode()
+    if "--yuv-decode" in sys.argv:
+        return yuv_decode()
     if "--yuv" in sys.argv:
         return yuv()
     if "--lossless" in sys.argv:
