@@ -492,9 +492,10 @@ int  b200jpeg_decompress_output(const b200jpeg_source_info *src, int *width, int
  * EXT_* output orders), sample for sample, on the sources b200jpeg_decompress_batch accepts (same checks, same
  * messages).
  *   scale_num / scale_denom: as jpeg_core_output_dimensions buckets them into a block size k (1/5 is k = 2); k must be
- *     1, 2, 4 or 8 (1/8, 1/4, 1/2, 1/1), other k are B200JPEG_ERR_UNSUPPORTED.  Output: ceil(W k / 8) x ceil(H k / 8).
- *   dct_method: B200JPEG_DCT_*, for components whose DCT_scaled_size is 8 (jddctmgr.c); smaller sizes use
- *     jidctred.c's IDCTs whatever the method.
+ *     1, 2, 4 or 8 (1/8, 1/4, 1/2, 1/1) unless all_scales, other k are B200JPEG_ERR_UNSUPPORTED.  Output:
+ *     ceil(W k / 8) x ceil(H k / 8).
+ *   dct_method: B200JPEG_DCT_*, for components whose DCT_scaled_size is 8 (jddctmgr.c); sizes 1, 2 and 4 use
+ *     jidctred.c's IDCTs and the other sizes jidctint.c's scaled IDCTs, whatever the method.
  *   do_fancy_upsampling: 0 replicates chroma (and the merged upsampler, which gives the same pixels).
  *   out_color_space: -1 for what default_decompress_parms picks; else GRAYSCALE, RGB, EXT_*, or YCbCr from a YCbCr
  *     file.  Pairs the reference refuses are B200JPEG_ERR_PARAM "Unsupported color conversion request"; CMYK, YCCK
@@ -502,7 +503,10 @@ int  b200jpeg_decompress_output(const b200jpeg_source_info *src, int *width, int
  * The default options give b200jpeg_decompress_batch's and b200jpeg_recompress_batch's route and bytes.
  */
 #define B200JPEG_CS_RGB565 16
-typedef struct { int scale_num, scale_denom, dct_method, do_fancy_upsampling, out_color_space; } b200jpeg_decompress_options;
+/*   all_scales: 0 (the default) refuses the block sizes above; 1 decodes every block size jpeg_core_output_dimensions
+ *     picks (1 .. 16, every scale_num / scale_denom) with jidctint.c's scaled IDCTs, sample for sample.  A C
+ *     initialiser of the first five fields leaves it 0. */
+typedef struct { int scale_num, scale_denom, dct_method, do_fancy_upsampling, out_color_space, all_scales; } b200jpeg_decompress_options;
 b200jpeg_decompress_options b200jpeg_default_decompress_options(void);
 /* jpeg_calc_output_dimensions + out_color_components for these options: B200JPEG_ERR_* as the batch would refuse. */
 int  b200jpeg_decompress_output_opts(const b200jpeg_source_info *src, const b200jpeg_decompress_options *opts,
@@ -520,7 +524,8 @@ int  b200jpeg_recompress_batch_opts(b200jpeg_encoder *enc, const b200jpeg_decomp
  * these apply, the others must keep b200jpeg_default_decompress_options' values, else B200JPEG_ERR_PARAM:
  *   scale_num / scale_denom: one of TurboJPEG's scaling factors (n/8 for n = 1 .. 16, in lowest terms; others are
  *     B200JPEG_ERR_PARAM "Unsupported scaling factor").  The IDCT block size is 8 * num / denom; only 1/8, 1/4, 1/2 and
- *     1/1 are on the device, the others are B200JPEG_ERR_UNSUPPORTED.
+ *     1/1 are on the device unless all_scales, the others are B200JPEG_ERR_UNSUPPORTED.
+ *   all_scales: as for b200jpeg_decompress_batch_opts; with it every factor above is decoded.
  *   dct_method: B200JPEG_DCT_ISLOW, or B200JPEG_DCT_IFAST (TJPARAM_FASTDCT); FLOAT is B200JPEG_ERR_PARAM.
  * Sources: gray, and 3-component files whose sampling getSubsamp names (turbojpeg.c:400-479: 4:4:4, 4:2:2, 4:2:0,
  * 4:4:0, 4:1:1, 4:4:1 and the non-standard 4:2:2, 4:4:0 and 4:4:4 spellings), RGB-coded files included (their planes

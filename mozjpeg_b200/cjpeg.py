@@ -339,7 +339,7 @@ def params_for_jpeg_input(switches: Sequence[str], jpeg: bytes, **opts) -> A.Par
     """cjpeg's cinfo at jpeg_start_compress for a JPEG input file: rdjpeg.c's start_input_jpeg takes the image size,
     in_color_space (the decompressor's out_color_space) and input_components from the source (data_precision is 8 for
     every source the device decodes), then jpeg_default_colorspace and the second switch pass run as for any input.
-    Keyword options (decompress_options: scale, dct, fancy, colorspace) describe a rendition decoded with them, for
+    Keyword options (decompress_options: scale, dct, fancy, colorspace, all_scales) describe a rendition decoded with them, for
     Encoder.recompress with the same options; without them the decompress defaults."""
     lib = A.load()
     info = A.SourceInfo()
@@ -359,10 +359,10 @@ COLOR_SPACES = {"gray": 1, "grayscale": 1, "rgb": 2, "ycbcr": 3, "cmyk": 4, "ycc
                 "xbgr": 10, "xrgb": 11, "rgba": 12, "bgra": 13, "abgr": 14, "argb": 15, "rgb565": 16}
 
 
-def decompress_options(scale=(1, 1), dct: str = "int", fancy: bool = True, colorspace=None) -> A.DecompressOptions:
+def decompress_options(scale=(1, 1), dct: str = "int", fancy: bool = True, colorspace=None, all_scales: bool = False) -> A.DecompressOptions:
     """b200jpeg_decompress_options from keywords: scale=(scale_num, scale_denom), dct "int" | "fast" | "float"
     (JDCT_ISLOW / IFAST / FLOAT), fancy (do_fancy_upsampling), colorspace None (the decompressor's default), a
-    B200JPEG_CS_* number or a name of COLOR_SPACES."""
+    B200JPEG_CS_* number or a name of COLOR_SPACES, all_scales (decode every scale, not only 1/8, 1/4, 1/2 and 1/1)."""
     if dct not in DCT_METHODS:
         raise ValueError(f"dct must be one of {sorted(DCT_METHODS)}, not {dct!r}")
     if colorspace is None:
@@ -374,7 +374,7 @@ def decompress_options(scale=(1, 1), dct: str = "int", fancy: bool = True, color
     else:
         cs = int(colorspace)
     num, denom = scale
-    return A.DecompressOptions(int(num), int(denom), DCT_METHODS[dct], int(bool(fancy)), cs)
+    return A.DecompressOptions(int(num), int(denom), DCT_METHODS[dct], int(bool(fancy)), cs, int(bool(all_scales)))
 
 
 def read_pnm(data: bytes):

@@ -2011,10 +2011,18 @@ static int decompress_files(b200jpeg_encoder *e, const uint8_t *const *files, co
   e->dec_ms_prog = false;
   e->dec.want_markers = want_markers;
   if (want_markers) e->dec_markers.assign(n, std::vector<uint8_t>());
-  // chunks of about 1.6 M blocks (8 images of 3840x2160 4:2:0, 300 MB of coefficient and sample planes)
+  // chunks of about 1.6 M blocks (8 images of 3840x2160 4:2:0, 300 MB of coefficient and sample planes); a block whose
+  // IDCT writes more than 8 x 8 samples counts as ssize^2 / 64 blocks, so the sample planes stay that size (DESIGN §14)
   long long per = 0;
-  for (int c = 0; c < nc; c++) per += (long long)div_up((long long)W * s0.h_samp_factor[c], (nc == 3 ? hx : s0.h_samp_factor[0]) * 8) * div_up((long long)H * s0.v_samp_factor[c], (nc == 3 ? vx : s0.v_samp_factor[0]) * 8);
+  for (int t = 0; t < ntg; t++) {
+    long long pt = 0;
+    for (int c = 0; c < nc; c++)
+      pt += (long long)div_up((long long)W * s0.h_samp_factor[c], (nc == 3 ? hx : s0.h_samp_factor[0]) * 8) * div_up((long long)H * s0.v_samp_factor[c], (nc == 3 ? vx : s0.v_samp_factor[0]) * 8) *
+            std::max(64, plans[t].ssize[c] * plans[t].ssize[c]) / 64;
+    per = std::max(per, pt);
+  }
   const int C = std::min(n, e->chunk_images_override > 0 ? e->chunk_images_override : (int)std::max(1LL, 1600000LL / std::max(1LL, per)));
+  e->chunk = C;
   std::vector<uint16_t> qt;
   std::vector<uint32_t> mt;
   for (int i0 = 0; i0 < n; i0 += C) {
@@ -2305,7 +2313,7 @@ static int check_rungs(int n_renditions, const b200jpeg_decompress_options *opts
     for (; k < (int)g.first.size(); k++) {
       const b200jpeg_decompress_options &f = opts[g.first[k]];
       if (f.scale_num == o.scale_num && f.scale_denom == o.scale_denom && f.dct_method == o.dct_method &&
-          f.do_fancy_upsampling == o.do_fancy_upsampling && f.out_color_space == o.out_color_space) break;
+          f.do_fancy_upsampling == o.do_fancy_upsampling && f.out_color_space == o.out_color_space && f.all_scales == o.all_scales) break;
     }
     if (k == (int)g.first.size()) g.first.push_back(r);
     g.set.push_back(k);
@@ -2465,7 +2473,7 @@ static int check_mixed(b200jpeg_encoder *e, int n_renditions, const b200jpeg_dec
     for (; k < (int)m.first.size(); k++) {
       const b200jpeg_decompress_options &f = opts[m.first[k]];
       if (f.scale_num == o.scale_num && f.scale_denom == o.scale_denom && f.dct_method == o.dct_method &&
-          f.do_fancy_upsampling == o.do_fancy_upsampling && f.out_color_space == o.out_color_space) break;
+          f.do_fancy_upsampling == o.do_fancy_upsampling && f.out_color_space == o.out_color_space && f.all_scales == o.all_scales) break;
     }
     if (k == (int)m.first.size()) {
       m.first.push_back(r);
@@ -2478,6 +2486,20 @@ static int check_mixed(b200jpeg_encoder *e, int n_renditions, const b200jpeg_dec
         }
     }
     m.set.push_back(k);
+  }
+  // the chunk weight of an image: its blocks, those whose IDCT writes more than 8 x 8 samples counted as ssize^2 / 64
+  // blocks under the largest of the sets' plans, so a chunk's sample planes stay the size they have at 1/1 (DESIGN §14)
+  for (int i = 0; i < n; i++) {
+    const b200jpeg_source_info &s = m.info[i];
+    int hmax = 1, vmax = 1;
+    for (int c = 0; c < s.num_components; c++) { hmax = std::max(hmax, s.h_samp_factor[c]); vmax = std::max(vmax, s.v_samp_factor[c]); }
+    for (const std::vector<DecPlan> &pl : m.plan) {
+      long long w = 0;
+      for (int c = 0; c < s.num_components; c++)
+        w += (long long)div_up((long long)s.image_width * s.h_samp_factor[c], hmax * 8) * div_up((long long)s.image_height * s.v_samp_factor[c], vmax * 8) *
+             std::max(64, pl[i].ssize[c] * pl[i].ssize[c]) / 64;
+      m.blocks[i] = std::max(m.blocks[i], w);
+    }
   }
   return B200JPEG_OK;
 }
@@ -2542,7 +2564,7 @@ static void stage_mixed(const b200jpeg_encoder *e, const std::vector<DecPlan> &p
   st = MixStage();
   std::vector<IdctImg> d; std::vector<uint32_t> w;
   for (int c = 0; c < 3; c++)
-    for (int size = 1; size <= 8; size *= 2) {
+    for (int size = 1; size <= 16; size++) {
       d.clear(); w.clear();
       const int bpc = idct_blocks_per_cta(size);
       for (int i = 0; i < nk; i++) {

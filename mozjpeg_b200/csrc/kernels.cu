@@ -4710,6 +4710,79 @@ __global__ void __launch_bounds__(IDCT_BLOCKS * 8) k_idct_red(const int16_t *__r
   }
 }
 
+#include "idct_scaled.inc"
+
+// workspace ints per block of k_idct_scaled: rows of 9 (8 used), 8 rows below N = 8 else N, and one more so that
+// blocks start in different banks
+template <int N> __host__ __device__ constexpr int idct_scaled_ws() { return (N < 8 ? 8 : N) * 9 + 1; }
+
+// jpeg_idct_3x3 .. jpeg_idct_16x16 but 4 and 8 (jidctint.c:427-2625; the passes as idct_scaled.inc folds them) with
+// the islow-style table (entries taken as unsigned 16-bit values, as k_idct_red takes them).  Eight lanes per block:
+// lane r loads coefficient row r; pass 1 runs lanes 0 .. M-1 over columns (M = N below 8, reading rows 0 .. N-1 only,
+// else 8) into N workspace rows, in 64 bits as the reference's JLONG; pass 2 gives lane l rows l, l + 8 (N > 8), each
+// from M workspace values, and stores its N samples byte by byte (rows of N samples at a pitch of wib * N bytes are
+// not word-aligned for odd N).  out: [n][hib * N][wib * N] samples, or with PLANE pd's plane clipped to pd.cw x pd.ch.
+template <int N, bool RAGGED, bool PLANE = false>
+__global__ void __launch_bounds__(IDCT_BLOCKS * 8) k_idct_scaled(const int16_t *__restrict__ coef, const uint16_t *__restrict__ quant, int qstride,
+                                                                 uint8_t *__restrict__ out, int wib, int hib, long long nblocks,
+                                                                 const uint32_t *__restrict__ work, const IdctImg *__restrict__ imgs,
+                                                                 IdctDst pd = IdctDst())
+{
+  constexpr int M = N < 8 ? N : 8, WS = idct_scaled_ws<N>();
+  __shared__ int4 s_coef[IDCT_BLOCKS * 8];
+  __shared__ int s_ws[IDCT_BLOCKS * WS];
+  const int lb = threadIdx.x >> 3, lane = threadIdx.x & 7;
+  const IdctAt at = idct_at<RAGGED, IDCT_BLOCKS, N, PLANE>(lb, wib, hib, nblocks, qstride, work, imgs, pd);
+  const bool valid = at.valid;
+  s_coef[threadIdx.x] = valid && lane < M ? reinterpret_cast<const int4 *>(coef)[at.blk * 8 + lane] : make_int4(0, 0, 0, 0);
+  __syncwarp();
+  if (lane < M) {                                          // pass 1: column `lane` -> ws rows 0 .. N-1
+    const int16_t *c = reinterpret_cast<const int16_t *>(s_coef + lb * 8) + lane;
+    const uint16_t *q = quant + at.q + lane;
+    long long d[M];
+#pragma unroll
+    for (int r = 0; r < M; r++) d[r] = (long long)((int)c[r * 8] * (int)q[r * 8]);
+    int o[N];
+    idct_scaled_p1<N>(d, o);
+    int *ws = s_ws + lb * WS + lane;
+#pragma unroll
+    for (int r = 0; r < N; r++) ws[r * 9] = o[r];
+  }
+  __syncwarp();
+#pragma unroll
+  for (int r0 = 0; r0 < N; r0 += 8) {                      // pass 2: row r0 + lane
+    const int r = r0 + lane;
+    if (!valid || r >= N || (PLANE && at.y0 + r >= pd.ch)) continue;
+    const int *w = s_ws + lb * WS + r * 9;
+    unsigned d[M], o[N];
+#pragma unroll
+    for (int k = 0; k < M; k++) d[k] = (unsigned)w[k];
+    idct_scaled_p2<N>(d, o);
+    uint8_t *dst = out + at.o + r * at.pitch;
+    const int n = PLANE ? pd.cw - at.x0 : N;
+#pragma unroll
+    for (int x = 0; x < N; x++)
+      if (x < n) dst[x] = (uint8_t)idct_range_limit((int)o[x]);
+  }
+}
+
+// k_idct_scaled's instances, by N
+template <bool RAGGED, bool PLANE>
+static void launch_idct_scaled(int size, const int16_t *coef, const uint16_t *q, int qstride, uint8_t *out, int wib, int hib, long long nblocks,
+                               unsigned grid, const uint32_t *work, const IdctImg *imgs, const IdctDst &d, cudaStream_t s)
+{
+  switch (size) {
+#define IDCT_SCALED_CASE(NN) \
+    case NN: k_idct_scaled<NN, RAGGED, PLANE><<<grid, IDCT_BLOCKS * 8, 0, s>>>(coef, q, qstride, out, wib, hib, nblocks, work, imgs, d); LAUNCHED(); break;
+    IDCT_SCALED_CASE(3) IDCT_SCALED_CASE(5) IDCT_SCALED_CASE(6) IDCT_SCALED_CASE(7) IDCT_SCALED_CASE(9) IDCT_SCALED_CASE(10)
+    IDCT_SCALED_CASE(11) IDCT_SCALED_CASE(12) IDCT_SCALED_CASE(13) IDCT_SCALED_CASE(14) IDCT_SCALED_CASE(15) IDCT_SCALED_CASE(16)
+#undef IDCT_SCALED_CASE
+    default: break;
+  }
+}
+
+bool idct_size_scaled(int size) { return size >= 3 && size <= 16 && size != 4 && size != 8; }
+
 // MULTIPLY of jidctfst.c (8-bit: CONST_BITS 8, no rounding): the int times a JLONG constant in 64 bits, shifted, and
 // truncated back to DCTELEM (int)
 __device__ __forceinline__ unsigned ifast_mul(unsigned v, int c)
@@ -4860,6 +4933,7 @@ void launch_idct_opts(int size, int method, const int16_t *coef, const void *tab
   if (size == 1) { k_idct_red<1, false><<<(unsigned)((nblocks + 255) / 256), 256, 0, s>>>(coef, q, qstride, out, wib, hib, nblocks, nullptr, nullptr); LAUNCHED(); }
   else if (size == 2) { k_idct_red<2, false><<<grid8, IDCT_BLOCKS * 8, 0, s>>>(coef, q, qstride, out, wib, hib, nblocks, nullptr, nullptr); LAUNCHED(); }
   else if (size == 4) { k_idct_red<4, false><<<grid8, IDCT_BLOCKS * 8, 0, s>>>(coef, q, qstride, out, wib, hib, nblocks, nullptr, nullptr); LAUNCHED(); }
+  else if (idct_size_scaled(size)) launch_idct_scaled<false, false>(size, coef, q, qstride, out, wib, hib, nblocks, grid8, nullptr, nullptr, IdctDst(), s);
   else if (method == 1) { k_idct_ifast<false><<<grid8, IDCT_BLOCKS * 8, 0, s>>>(coef, static_cast<const int *>(tab), qstride, out, wib, hib, nblocks, nullptr, nullptr); LAUNCHED(); }
   else if (method == 2) { k_idct_float<false><<<grid8, IDCT_BLOCKS * 8, 0, s>>>(coef, static_cast<const float *>(tab), qstride, out, wib, hib, nblocks, nullptr, nullptr); LAUNCHED(); }
   else launch_idct_islow(coef, q, qstride, out, wib, hib, n, s);
@@ -4874,6 +4948,7 @@ void launch_idct_ragged(int size, int method, const int16_t *coef, const void *t
   if (size == 1) { k_idct_red<1, true><<<ncta, 256, 0, s>>>(coef, q, 0, out, 0, 0, 0, work, imgs); LAUNCHED(); }
   else if (size == 2) { k_idct_red<2, true><<<ncta, IDCT_BLOCKS * 8, 0, s>>>(coef, q, 0, out, 0, 0, 0, work, imgs); LAUNCHED(); }
   else if (size == 4) { k_idct_red<4, true><<<ncta, IDCT_BLOCKS * 8, 0, s>>>(coef, q, 0, out, 0, 0, 0, work, imgs); LAUNCHED(); }
+  else if (idct_size_scaled(size)) launch_idct_scaled<true, false>(size, coef, q, 0, out, 0, 0, 0, ncta, work, imgs, IdctDst(), s);
   else if (method == 1) { k_idct_ifast<true><<<ncta, IDCT_BLOCKS * 8, 0, s>>>(coef, static_cast<const int *>(tab), 0, out, 0, 0, 0, work, imgs); LAUNCHED(); }
   else if (method == 2) { k_idct_float<true><<<ncta, IDCT_BLOCKS * 8, 0, s>>>(coef, static_cast<const float *>(tab), 0, out, 0, 0, 0, work, imgs); LAUNCHED(); }
   else { k_idct_islow<true><<<ncta, IDCT_BLOCKS * 8, 0, s>>>(coef, q, 0, out, 0, 0, 0, work, imgs); LAUNCHED(); }
@@ -5002,6 +5077,7 @@ void launch_idct_plane(int size, int method, bool int_table, const int16_t *coef
   else if (size == 2) { k_idct_red<2, false, true><<<grid8, IDCT_BLOCKS * 8, 0, s>>>(coef, q, qstride, out, wib, hib, nblocks, nullptr, nullptr, d); LAUNCHED(); }
   else if (size == 4 && int_table) { k_idct_red<4, false, true, int><<<grid8, IDCT_BLOCKS * 8, 0, s>>>(coef, static_cast<const int *>(tab), qstride, out, wib, hib, nblocks, nullptr, nullptr, d); LAUNCHED(); }
   else if (size == 4) { k_idct_red<4, false, true><<<grid8, IDCT_BLOCKS * 8, 0, s>>>(coef, q, qstride, out, wib, hib, nblocks, nullptr, nullptr, d); LAUNCHED(); }
+  else if (idct_size_scaled(size)) launch_idct_scaled<false, true>(size, coef, q, qstride, out, wib, hib, nblocks, grid8, nullptr, nullptr, d, s);
   else if (method == 1) { k_idct_ifast<false, true><<<grid8, IDCT_BLOCKS * 8, 0, s>>>(coef, static_cast<const int *>(tab), qstride, out, wib, hib, nblocks, nullptr, nullptr, d); LAUNCHED(); }
   else { k_idct_islow<false, true><<<grid8, IDCT_BLOCKS * 8, 0, s>>>(coef, q, qstride, out, wib, hib, nblocks, nullptr, nullptr, d); LAUNCHED(); }
 }

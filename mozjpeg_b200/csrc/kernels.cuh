@@ -298,8 +298,9 @@ int launch_upsample_color(int hx, int vx, int nc, const uint8_t *const *planes, 
 
 // decompression with options.  IDCT of one component whose DCT_scaled_size is `size`: 1, 2, 4 -> k_idct_red<size>
 // (tab: the uint16 quantization tables), 8 -> by method: 0 islow (tab as for 1 .. 4), 1 k_idct_ifast (tab: int
-// multiplier tables), 2 k_idct_float (tab: float multiplier tables); image i's table at tab + i * qstride entries.
-// out: [n][hib * size][wib * size] samples.
+// multiplier tables), 2 k_idct_float (tab: float multiplier tables); 3, 5, 6, 7 and 9 .. 16 -> k_idct_scaled<size>
+// whatever the method (tab as for 1 .. 4: jddctmgr.c gives those sizes the islow-style table); image i's table at
+// tab + i * qstride entries.  out: [n][hib * size][wib * size] samples.
 void launch_idct_opts(int size, int method, const int16_t *coef, const void *tab, int qstride, uint8_t *out, int wib, int hib, int n, cudaStream_t s);
 // k_upsample_opts: per used component (nin of them) image 0's plane, pitch / stride in bytes, dw x dh real samples,
 // the replication factors hr x vr (1 or 2) after IDCT scaling, and fancy (the smoothing filter instead of

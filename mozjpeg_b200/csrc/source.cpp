@@ -261,7 +261,7 @@ extern "C" int b200jpeg_decompress_output(const b200jpeg_source_info *src, int *
 extern "C" b200jpeg_decompress_options b200jpeg_default_decompress_options(void)
 {
   b200jpeg_decompress_options o;
-  o.scale_num = 1; o.scale_denom = 1; o.dct_method = B200JPEG_DCT_ISLOW; o.do_fancy_upsampling = 1; o.out_color_space = -1;
+  o.scale_num = 1; o.scale_denom = 1; o.dct_method = B200JPEG_DCT_ISLOW; o.do_fancy_upsampling = 1; o.out_color_space = -1; o.all_scales = 0;
   return o;
 }
 
@@ -279,7 +279,7 @@ int plan_decompress(const b200jpeg_source_info &s, const b200jpeg_decompress_opt
   // the block size jpeg_core_output_dimensions picks: the least k with scale_num * 8 <= scale_denom * k, at most 16
   int k = 16;
   for (int t = 1; t < 16; t++) if ((long long)o.scale_num * 8 <= (long long)o.scale_denom * t) { k = t; break; }
-  if (k != 1 && k != 2 && k != 4 && k != 8) {
+  if (!o.all_scales && k != 1 && k != 2 && k != 4 && k != 8) {
     set_error("scale %d/%d gives an IDCT block size of %d: only sizes 1, 2, 4 and 8 (1/8, 1/4, 1/2, 1/1) are decoded on the device", o.scale_num, o.scale_denom, k);
     return B200JPEG_ERR_UNSUPPORTED;
   }
@@ -395,7 +395,7 @@ int plan_yuv(const b200jpeg_source_info &s, const b200jpeg_decompress_options &o
   if (p.subsamp < 0) return bad(B200JPEG_ERR_PARAM, "Could not determine subsampling level of JPEG image");
   if (nc > 3) return bad(B200JPEG_ERR_PARAM, "JPEG image must have 3 or fewer components");
   const int k = 8 * o.scale_num / o.scale_denom;
-  if (k != 1 && k != 2 && k != 4 && k != 8) {
+  if (!o.all_scales && k != 1 && k != 2 && k != 4 && k != 8) {
     set_error("scale %d/%d gives an IDCT block size of %d: only sizes 1, 2, 4 and 8 (1/8, 1/4, 1/2, 1/1) are decoded on the device", o.scale_num, o.scale_denom, k);
     return B200JPEG_ERR_UNSUPPORTED;
   }

@@ -1,8 +1,8 @@
 """``python -m mozjpeg_b200.djpeg`` -- the reference's djpeg command line on the device path, for the switches that set
 decompress options (djpeg.c parse_switches, with its abbreviations) and PPM / PGM output framed as wrppm.c writes it:
 
-  -scale M/N            scale_num / scale_denom (the block sizes 1, 2, 4 and 8: 1/8, 1/4, 1/2, 1/1, and fractions that
-                        fall into them)
+  -scale M/N            scale_num / scale_denom: every fraction, bucketed into the block sizes 1 .. 16 as the reference
+                        does (main() passes all_scales=True)
   -dct int|fast|float   dct_method
   -nosmooth             do_fancy_upsampling = FALSE
   -fast                 JDCT_IFAST and no fancy upsampling (the quantization settings it also makes need -colors)
@@ -116,7 +116,7 @@ def main(argv: Sequence[str] = None) -> int:
     enc = Encoder(0)
     enc.set_progressive_decode(True)          # the reference's djpeg reads progressive files too
     try:
-        px = enc.decompress([src], **opts)[0]
+        px = enc.decompress([src], all_scales=True, **opts)[0]
     finally:
         enc.close()
     out = ppm_bytes(px)

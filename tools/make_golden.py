@@ -475,6 +475,45 @@ def decompress_options():
     print("wrote", len(cases), "cases,", len(refused), "refused pairs")
 
 
+def idct_scaling():
+    """tests/golden/idct_scaling_golden.json: for every (source, options) of tests/idct_scaling_cases.py what
+    --decompress-options records (build/librefdecopt.so), and the reference's tj3DecompressToYUVPlanes8 planes
+    (oracle/_ref/libturbojpeg_ref.so) of every YUV source at the TurboJPEG factors whose block sizes are new."""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import decompress_options_cases as O
+    import idct_scaling_cases as S
+    import yuv_decode_cases as Y
+    import mozjpeg_b200 as mj
+    from mozjpeg_b200 import _abi as A
+    if not O.have_reference():
+        sys.exit("build/librefdecopt.so is missing: run __graft_entry__.build() with the reference build under oracle/_ref/")
+    cases = []
+    for cid, sid, scale, dct, fancy, cs in S.cases():
+        src, _ = O.source(sid)
+        px, info, msg = O.ref_decompress(src, O.opts_tuple(scale, dct, fancy, cs))
+        if px is None:
+            sys.exit(f"{cid}: the reference refuses it: {msg}")
+        nc = info[6]
+        cases.append({"id": cid, "src_md5": O.md5(src), "pix_md5": O.md5(px), "shape": list(px.shape), "out_color_space": info[3],
+                      "components": [info[7 + 3 * c:10 + 3 * c] for c in range(nc)], "warnings": info[5]})
+    ref = Y.RefTJ()
+    yuv = []
+    for sid, scale, dct in S.YUV_CASES:
+        src = Y.source(sid)
+        ss, planes, err = ref.decompress_planes(src, scale, dct)
+        if err is not None:
+            sys.exit(f"{sid} {scale} {dct}: the reference refuses it: {err}")
+        info = A.SourceInfo()
+        A.check(mj._lib.b200jpeg_parse_source(src, len(src), C.byref(info)), "parse_source")
+        _, dims = Y.plan(info, scale)
+        yuv.append({"id": Y.case_id(sid, scale, dct), "src_md5": hashlib.md5(src).hexdigest(), "subsamp": Y.SUBSAMPS[ss],
+                    "dims": [list(p.shape[::-1]) for p in planes], "md5": [Y.md5(Y.defined(p, *d)) for p, d in zip(planes, dims)]})
+    ref.close()
+    json.dump({"generator": "tools/make_golden.py --idct-scaling", "reference": "mozilla/mozjpeg 5.0.0 (C path, WITH_SIMD=0), oracle/_ref",
+               "cases": cases, "yuv": yuv}, open(os.path.join(GOLD, "idct_scaling_golden.json"), "w"), indent=0)
+    print("wrote", len(cases), "cases,", len(yuv), "YUV cases")
+
+
 # jpegtran switch sets the progressive goldens record
 PROGRESSIVE_JPEGTRAN = [[], ["-optimize"], ["-progressive"], ["-rotate", "90"], ["-crop", "48x32+9+5"]]
 
@@ -517,6 +556,8 @@ def progressive():
 def main():
     if "--progressive" in sys.argv:
         return progressive()
+    if "--idct-scaling" in sys.argv:
+        return idct_scaling()
     if "--decompress-options" in sys.argv:
         return decompress_options()
     if "--recompress" in sys.argv:

@@ -85,6 +85,14 @@ for kw in (dict(scale=(1, 8)), dict(scale=(1, 4), dct="fast", fancy=False), dict
            dict(dct="fast", colorspace="gray"), dict(fancy=False, colorspace="xrgb")):
     n += len(enc.decompress(rag, **kw))
     n += len(enc.recompress(mj.params_for_jpeg_input(["-baseline", "-quality", "75"], rag[0], **kw), rag, **kw))
+# every scale (all_scales): the scaled IDCTs of jidctint.c, one small ragged size per N, in the one-geometry form, the
+# ragged form (a mixed batch of two geometries) and the PLANE form (YUV planes clipped at odd widths)
+NEW = (3, 5, 6, 7, 9, 10, 11, 12, 13, 14, 15, 16)
+for k in NEW:
+    n += len(enc.decompress(rag, scale=(k, 8), all_scales=True))
+n += len(enc.decompress_mixed([rag[0], srcs[0]], [dict(scale=(k, 8), all_scales=True) for k in NEW])[0])
+for f in ((3, 8), (5, 8), (3, 4), (7, 8), (9, 8), (5, 4), (11, 8), (3, 2), (13, 8), (7, 4), (15, 8), (2, 1)):
+    n += len(enc.decompress_yuv(rag, scale=f, all_scales=True))
 # progressive decode: the default profile (scan search, successive approximation), the standard script with restarts,
 # mixed with sequential files, through the coefficient, transcode and pixel routes; then a truncated refinement scan
 enc.set_progressive_decode(True)
