@@ -1875,14 +1875,14 @@ static int reserve_pixel_stage(b200jpeg_encoder *e, const DecPlan &plan, int nk)
   return B200JPEG_OK;
 }
 
-// the tables each image of the decoded chunk latched, [nk][nc][64], into e->d_dec_quant (qt: host staging)
-static int upload_chunk_quant(b200jpeg_encoder *e, int nk, std::vector<uint16_t> &qt)
+// the tables each image of the decoded chunk latched, [nk][qs][64] (qs: the most components of an image; slots past
+// an image's components are zero), into e->d_dec_quant (qt: host staging)
+static int upload_chunk_quant(b200jpeg_encoder *e, int nk, int qs, std::vector<uint16_t> &qt)
 {
   const DecBatch &b = e->dec;
-  const int nc = b.geom[0].nc;
-  qt.resize((size_t)nk * nc * 64);
+  qt.assign((size_t)nk * qs * 64, 0);
   for (int i = 0; i < nk; i++)
-    for (int c = 0; c < nc; c++) memcpy(&qt[((size_t)i * nc + c) * 64], b.info[i].comp_quant[c], 128);
+    for (int c = 0; c < b.geom[i].nc; c++) memcpy(&qt[((size_t)i * qs + c) * 64], b.info[i].comp_quant[c], 128);
   CU(cudaMemcpyAsync(e->d_dec_quant.p, qt.data(), qt.size() * 2, cudaMemcpyHostToDevice, e->stream));
   return B200JPEG_OK;
 }
@@ -1967,126 +1967,30 @@ static int chunk_pixels(b200jpeg_encoder *e, const DecPlan &plan, int nk, uint8_
                          : idct_upsample_opts(e, plan, nk, pix, row_pitch, image_stride, qt, mt, ev);
 }
 
-// One pixel output of a decompress: the decompress object's options (nullptr: its defaults) and where image i's rows
-// go on the device (pix + i * image_stride, row_pitch bytes apart).
-struct PixTarget {
-  const b200jpeg_decompress_options *opts; uint8_t *pix; size_t row_pitch, image_stride;
-};
-
-// jpeg_read_scanlines for a batch of files, to one or more targets: the entropy decode chunk by chunk (the coefficient
-// and sample planes are one chunk's), and behind each chunk's decode the IDCT and upsampling / colour conversion of
-// every target, enqueued together and synchronised once.  Options that give what the defaults give take the default
-// route.
-static int decompress_files(b200jpeg_encoder *e, const uint8_t *const *files, const size_t *sizes, int n, const PixTarget *tg, int ntg, bool want_markers)
+// The chunks of a batch: images in order until a chunk weighs about 1.6 M blocks (8 images of 3840x2160 4:2:0, 300 MB
+// of coefficient and sample planes; an image heavier than that is a chunk of its own), or b200jpeg_encoder_set_chunk_images
+// images.  Returns the first image of each chunk and n.
+static std::vector<int> mixed_chunks(const b200jpeg_encoder *e, const std::vector<long long> &blocks)
 {
-  // every refusal comes before any device work
-  b200jpeg_source_info s0;
-  {
-    static thread_local b200jpeg_source_info s;
-    for (int i = 0; i < n; i++) {
-      if (!files[i]) { set_error("image %d: no file", i); return B200JPEG_ERR_PARAM; }
-      int rc = b200jpeg_parse_source(files[i], sizes[i], &s);
-      if (rc) { std::string m = b200jpeg_last_error(); set_error("image %d: %s", i, m.c_str()); return rc; }
-      if ((rc = check_decompress_source(s, i, e->progressive_decode))) return rc;
-      if (i == 0) s0 = s;
-      bool same = s.image_width == s0.image_width && s.image_height == s0.image_height && s.num_components == s0.num_components;
-      for (int c = 0; same && c < s.num_components; c++) same = s.h_samp_factor[c] == s0.h_samp_factor[c] && s.v_samp_factor[c] == s0.v_samp_factor[c];
-      if (same && s.num_components == 3) same = (s.jpeg_color_space == B200JPEG_CS_RGB) == (s0.jpeg_color_space == B200JPEG_CS_RGB);
-      if (!same) { set_error("image %d: geometry (size, components, sampling, colour space) differs from image 0", i); return B200JPEG_ERR_PARAM; }
-    }
+  const int n = (int)blocks.size();
+  std::vector<int> start(1, 0);
+  long long acc = 0;
+  for (int i = 0; i < n; i++) {
+    const bool full = e->chunk_images_override > 0 ? i - start.back() == e->chunk_images_override : acc > 0 && acc + blocks[i] > 1600000LL;
+    if (full) { start.push_back(i); acc = 0; }
+    acc += blocks[i];
   }
-  const int W = s0.image_width, H = s0.image_height, nc = s0.num_components;
-  const int hx = nc == 3 ? s0.h_samp_factor[0] : 1, vx = nc == 3 ? s0.v_samp_factor[0] : 1;
-  std::vector<DecPlan> plans(ntg);
-  for (int t = 0; t < ntg; t++) {
-    DecPlan &plan = plans[t];
-    if (tg[t].opts) { int rc = plan_decompress(s0, *tg[t].opts, plan); if (rc) return rc; }
-    const bool def = plan.is_default;
-    const int OW = def ? W : plan.out_w, OH = def ? H : plan.out_h, onc = def ? nc : plan.out_nc;
-    if (tg[t].row_pitch < (size_t)OW * onc || (n > 1 && tg[t].image_stride < tg[t].row_pitch * (size_t)(OH - 1) + (size_t)OW * onc)) { set_error("row_pitch or image_stride smaller than the decoded image (%dx%d, %d components)", OW, OH, onc); return B200JPEG_ERR_PARAM; }
-  }
-  CU(cudaSetDevice(e->device));
-  while (e->pix_ev.size() < (size_t)ntg * 3) { cudaEvent_t ev; CU(cudaEventCreate(&ev)); e->pix_ev.push_back(ev); }
-  for (float &m : e->dec_ms) m = 0.f;
-  e->dec_ms_prog = false;
-  e->dec.want_markers = want_markers;
-  if (want_markers) e->dec_markers.assign(n, std::vector<uint8_t>());
-  // chunks of about 1.6 M blocks (8 images of 3840x2160 4:2:0, 300 MB of coefficient and sample planes); a block whose
-  // IDCT writes more than 8 x 8 samples counts as ssize^2 / 64 blocks, so the sample planes stay that size (DESIGN §14)
-  long long per = 0;
-  for (int t = 0; t < ntg; t++) {
-    long long pt = 0;
-    for (int c = 0; c < nc; c++)
-      pt += (long long)div_up((long long)W * s0.h_samp_factor[c], (nc == 3 ? hx : s0.h_samp_factor[0]) * 8) * div_up((long long)H * s0.v_samp_factor[c], (nc == 3 ? vx : s0.v_samp_factor[0]) * 8) *
-            std::max(64, plans[t].ssize[c] * plans[t].ssize[c]) / 64;
-    per = std::max(per, pt);
-  }
-  const int C = std::min(n, e->chunk_images_override > 0 ? e->chunk_images_override : (int)std::max(1LL, 1600000LL / std::max(1LL, per)));
-  e->chunk = C;
-  std::vector<uint16_t> qt;
-  std::vector<uint32_t> mt;
-  for (int i0 = 0; i0 < n; i0 += C) {
-    const int nk = std::min(C, n - i0);
-    int rc = decode_files(e, files + i0, sizes + i0, nk, i0);
-    if (rc) return rc;
-    e->dec_ms_prog |= e->dec_prog;
-    if (want_markers) for (int i = 0; i < nk; i++) e->dec_markers[i0 + i].swap(e->dec.markers[i]);
-    for (int t = 0; t < ntg; t++) if ((rc = reserve_pixel_stage(e, plans[t], nk))) return rc;
-    if ((rc = upload_chunk_quant(e, nk, qt))) return rc;
-    for (int t = 0; t < ntg; t++)
-      if ((rc = chunk_pixels(e, plans[t], nk, tg[t].pix + (size_t)i0 * tg[t].image_stride, tg[t].row_pitch, tg[t].image_stride, qt, mt, &e->pix_ev[(size_t)t * 3]))) return rc;
-    CU(cudaStreamSynchronize(e->stream));
-    sum_decode_stage_times(e);
-    for (int t = 0; t < ntg; t++)
-      for (int k = 0; k < 2; k++) { float ms = 0.f; cudaEventElapsedTime(&ms, e->pix_ev[(size_t)t * 3 + k], e->pix_ev[(size_t)t * 3 + k + 1]); e->dec_ms[6 + k] += ms; }
-  }
-  return B200JPEG_OK;
+  start.push_back(n);
+  return start;
 }
 
-// the stages of the last decompress, appended to the stage times
-static void add_decompress_stage_times(b200jpeg_encoder *e)
+// the stages of the last decompress, appended to the stage times: the decode's, then the first `pixel` of "idct" and
+// "upsample_color"
+static void add_decompress_stage_times(b200jpeg_encoder *e, int pixel = 2)
 {
   static const char *const extra[2] = {"idct", "upsample_color"};
   for (int k = 0; k < (e->dec_ms_prog ? 8 : 6); k++) { e->stage_names.push_back(kDecStages[k]); e->stage_ms.push_back(e->dec_ms[k < 6 ? k : k + 2]); e->stage_calls.push_back(1); }
-  for (int k = 0; k < 2; k++) { e->stage_names.push_back(extra[k]); e->stage_ms.push_back(e->dec_ms[6 + k]); e->stage_calls.push_back(1); }
-}
-
-// b200jpeg_decompress_batch (opts nullptr) and b200jpeg_decompress_batch_opts
-static int decompress_batch(b200jpeg_encoder *e, const b200jpeg_decompress_options *opts, const uint8_t *const *files, const size_t *sizes, int n_images,
-                            void *pixels, int pixels_on_device, size_t row_pitch, size_t image_stride)
-{
-  if (!e || !files || !sizes || !pixels || n_images <= 0) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
-  uint8_t *dst = static_cast<uint8_t *>(pixels);
-  size_t dp = row_pitch, ds = image_stride;
-  if (!pixels_on_device) {
-    // decode into a buffer of the batch's size on the device, then copy the rows out
-    b200jpeg_source_info *s = new b200jpeg_source_info;
-    int rc = b200jpeg_parse_source(files[0], files[0] ? sizes[0] : 0, s);
-    int ow = 0, oh = 0, ocs = 0, onc = 0;
-    if (!rc) rc = opts ? b200jpeg_decompress_output_opts(s, opts, &ow, &oh, &ocs, &onc) : b200jpeg_decompress_output(s, &ow, &oh, &ocs, &onc);
-    const size_t row = rc ? 0 : (size_t)ow * onc, rows = rc ? 0 : (size_t)oh;
-    delete s;
-    if (rc) { std::string m = b200jpeg_last_error(); set_error("image 0: %s", m.c_str()); return rc; }
-    if (row_pitch < row || (n_images > 1 && image_stride < row_pitch * (rows - 1) + row)) { set_error("row_pitch or image_stride smaller than the decoded image"); return B200JPEG_ERR_PARAM; }
-    dp = (row + 3) & ~(size_t)3; ds = dp * rows;
-    CU(cudaSetDevice(e->device));
-    if ((rc = e->d_dec_pixels.reserve(ds * (size_t)n_images))) return rc;
-    dst = e->d_dec_pixels.as<uint8_t>();
-    const PixTarget t = {opts, dst, dp, ds};
-    rc = decompress_files(e, files, sizes, n_images, &t, 1, false);
-    if (rc) return rc;
-    for (int i = 0; i < n_images; i++)
-      CU(cudaMemcpy2DAsync(static_cast<uint8_t *>(pixels) + (size_t)i * image_stride, row_pitch, dst + (size_t)i * ds, dp, row, rows, cudaMemcpyDeviceToHost, e->stream));
-    CU(cudaStreamSynchronize(e->stream));
-  } else {
-    const PixTarget t = {opts, dst, dp, ds};
-    int rc = decompress_files(e, files, sizes, n_images, &t, 1, false);
-    if (rc) return rc;
-  }
-  e->pending_marks = 0;
-  e->stage_names.clear(); e->stage_ms.clear(); e->stage_calls.clear();
-  add_decompress_stage_times(e);
-  return B200JPEG_OK;
+  for (int k = 0; k < pixel; k++) { e->stage_names.push_back(extra[k]); e->stage_ms.push_back(e->dec_ms[6 + k]); e->stage_calls.push_back(1); }
 }
 
 // b200jpeg_decompress_yuv_batch: the entropy decode chunk by chunk, then per component the IDCT that
@@ -2140,24 +2044,24 @@ static int decompress_yuv(b200jpeg_encoder *e, const b200jpeg_decompress_options
   for (float &m : e->dec_ms) m = 0.f;
   e->dec_ms_prog = false;
   e->dec.want_markers = false;
-  // chunks of about 1.6 M blocks, as decompress_files
   long long per = 0;
   for (int c = 0; c < nc; c++) per += (long long)(plan.iw[c] / plan.k) * (plan.ih[c] / plan.k);
-  const int C = std::min(n, e->chunk_images_override > 0 ? e->chunk_images_override : (int)std::max(1LL, 1600000LL / std::max(1LL, per)));
-  e->chunk = C;
+  const std::vector<int> start = mixed_chunks(e, std::vector<long long>(n, per));
+  e->chunk = 0;
   // the ifast multiplier tables: for the 8x8 ifast IDCT, and for 4:2:0 chroma at 1/2 under IFAST
   bool need_mt = plan.k == 8 && plan.method == B200JPEG_DCT_IFAST;
   for (int c = 0; c < nc; c++) need_mt |= plan.int_table[c];
   std::vector<uint16_t> qt;
   std::vector<uint32_t> mt;
   cudaStream_t s = e->stream;
-  for (int i0 = 0; i0 < n; i0 += C) {
-    const int nk = std::min(C, n - i0);
+  for (size_t j = 0; j + 1 < start.size(); j++) {
+    const int i0 = start[j], nk = start[j + 1] - i0;
+    e->chunk = std::max(e->chunk, nk);
     int rc = decode_files(e, files + i0, sizes + i0, nk, i0);
     if (rc) return rc;
     e->dec_ms_prog |= e->dec_prog;
     if ((rc = e->d_dec_quant.reserve((size_t)nk * nc * 128)) || (need_mt && (rc = e->d_dec_mtab.reserve((size_t)nk * nc * 256)))) return rc;
-    if ((rc = upload_chunk_quant(e, nk, qt))) return rc;
+    if ((rc = upload_chunk_quant(e, nk, nc, qt))) return rc;
     if (need_mt) {
       mt.resize((size_t)nk * nc * 64);
       for (size_t t = 0; t < (size_t)nk * nc; t++) method_table(B200JPEG_DCT_IFAST, &qt[t * 64], &mt[t * 64]);
@@ -2187,8 +2091,7 @@ static int decompress_yuv(b200jpeg_encoder *e, const b200jpeg_decompress_options
   }
   e->pending_marks = 0;
   e->stage_names.clear(); e->stage_ms.clear(); e->stage_calls.clear();
-  for (int k = 0; k < (e->dec_ms_prog ? 8 : 6); k++) { e->stage_names.push_back(kDecStages[k]); e->stage_ms.push_back(e->dec_ms[k < 6 ? k : k + 2]); e->stage_calls.push_back(1); }
-  e->stage_names.push_back("idct"); e->stage_ms.push_back(e->dec_ms[6]); e->stage_calls.push_back(1);
+  add_decompress_stage_times(e, 1);
   return B200JPEG_OK;
 }
 
@@ -2260,121 +2163,6 @@ static int decode_yuv(b200jpeg_encoder *e, const b200jpeg_params *p, const uint8
   return B200JPEG_OK;
 }
 
-// b200jpeg_recompress_batch (opts nullptr) and b200jpeg_recompress_batch_opts
-static int recompress_batch(b200jpeg_encoder *e, const b200jpeg_decompress_options *opts, const b200jpeg_params *p, const uint8_t *const *files,
-                            const size_t *sizes, int n_images)
-{
-  if (!e || !p || !files || !sizes || n_images <= 0) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
-  int rc = b200jpeg_validate(p);
-  if (rc) return rc;
-  if (p->data_precision != 8) { set_error("the sources decode to 8-bit samples, the parameter block has data_precision %d", p->data_precision); return B200JPEG_ERR_PARAM; }
-  const size_t pitch = ((size_t)p->image_width * p->input_components + 3) & ~(size_t)3, stride = pitch * (size_t)p->image_height;
-  {
-    b200jpeg_source_info *s = new b200jpeg_source_info;
-    int w = 0, h = 0, cs = 0, nc = 0;
-    rc = files[0] ? b200jpeg_parse_source(files[0], sizes[0], s) : B200JPEG_OK;
-    if (!rc && files[0]) rc = opts ? b200jpeg_decompress_output_opts(s, opts, &w, &h, &cs, &nc) : b200jpeg_decompress_output(s, &w, &h, &cs, &nc);
-    delete s;
-    if (rc) { std::string m = b200jpeg_last_error(); set_error("image 0: %s", m.c_str()); return rc; }
-    if (files[0] && (w != p->image_width || h != p->image_height || cs != p->in_color_space || nc != p->input_components)) {
-      set_error("the sources decode to %dx%d pixels of %d samples in colour space %d, the parameter block describes %dx%d of %d in %d (see b200jpeg_decompress_output)",
-                w, h, nc, cs, p->image_width, p->image_height, p->input_components, p->in_color_space);
-      return B200JPEG_ERR_PARAM;
-    }
-  }
-  CU(cudaSetDevice(e->device));
-  if ((rc = e->d_dec_pixels.reserve(stride * (size_t)n_images))) return rc;
-  const PixTarget t = {opts, e->d_dec_pixels.as<uint8_t>(), pitch, stride};
-  if ((rc = decompress_files(e, files, sizes, n_images, &t, 1, true))) return rc;
-  if ((rc = encode_common(e, p, e->d_dec_pixels.p, 1, pitch, stride, n_images, false, nullptr, nullptr, &e->dec_markers))) return rc;
-  add_decompress_stage_times(e);
-  return B200JPEG_OK;
-}
-
-// The rungs of a rendition call, checked against image 0 before any device work: each rung's decoded size, colour space
-// and components (b200jpeg_decompress_output_opts), and the distinct option sets (set[r]: rung r's set; first[k]: the
-// first rung of set k).  A rung's refusal keeps its code, the message names the rung.
-struct Rungs {
-  std::vector<int> set, first, w, h, cs, nc;
-};
-static int check_rungs(int n_renditions, const b200jpeg_decompress_options *opts, const uint8_t *const *files, const size_t *sizes, Rungs &g)
-{
-  if (!files[0]) { set_error("image 0: no file"); return B200JPEG_ERR_PARAM; }
-  std::unique_ptr<b200jpeg_source_info> s(new b200jpeg_source_info);
-  int rc = b200jpeg_parse_source(files[0], sizes[0], s.get());
-  if (rc) { std::string m = b200jpeg_last_error(); set_error("image 0: %s", m.c_str()); return rc; }
-  g = Rungs();
-  for (int r = 0; r < n_renditions; r++) {
-    int w = 0, h = 0, cs = 0, nc = 0;
-    if ((rc = b200jpeg_decompress_output_opts(s.get(), &opts[r], &w, &h, &cs, &nc))) { std::string m = b200jpeg_last_error(); set_error("rendition %d: %s", r, m.c_str()); return rc; }
-    g.w.push_back(w); g.h.push_back(h); g.cs.push_back(cs); g.nc.push_back(nc);
-    const b200jpeg_decompress_options &o = opts[r];
-    int k = 0;
-    for (; k < (int)g.first.size(); k++) {
-      const b200jpeg_decompress_options &f = opts[g.first[k]];
-      if (f.scale_num == o.scale_num && f.scale_denom == o.scale_denom && f.dct_method == o.dct_method &&
-          f.do_fancy_upsampling == o.do_fancy_upsampling && f.out_color_space == o.out_color_space && f.all_scales == o.all_scales) break;
-    }
-    if (k == (int)g.first.size()) g.first.push_back(r);
-    g.set.push_back(k);
-  }
-  return B200JPEG_OK;
-}
-
-// one device buffer per distinct option set for the whole batch's pixels, rows padded to 4 bytes as recompress_batch's
-static int reserve_rendition_pixels(b200jpeg_encoder *e, const Rungs &g, int n_images, std::vector<PixTarget> &tg)
-{
-  const int K = (int)g.first.size();
-  if ((int)e->d_rend_pixels.size() < K) e->d_rend_pixels.resize(K);
-  tg.resize(K);
-  for (int k = 0; k < K; k++) {
-    const int r = g.first[k];
-    const size_t pitch = ((size_t)g.w[r] * g.nc[r] + 3) & ~(size_t)3, stride = pitch * (size_t)g.h[r];
-    if (int rc = e->d_rend_pixels[k].reserve(stride * (size_t)n_images)) return rc;
-    tg[k] = PixTarget{nullptr, e->d_rend_pixels[k].as<uint8_t>(), pitch, stride};
-  }
-  return B200JPEG_OK;
-}
-
-// b200jpeg_decompress_renditions: one decode per chunk, one pixel stage per distinct option set, and the rungs that
-// share a set copied from the first of them
-static int decompress_renditions(b200jpeg_encoder *e, int n_renditions, const b200jpeg_decompress_options *opts, const uint8_t *const *files,
-                                 const size_t *sizes, int n_images, void *const *pixels, int pixels_on_device, const size_t *row_pitch,
-                                 const size_t *image_stride)
-{
-  if (!e || n_renditions < 1 || !opts || !files || !sizes || n_images <= 0 || !pixels || !row_pitch || !image_stride) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
-  Rungs g;
-  int rc = check_rungs(n_renditions, opts, files, sizes, g);
-  if (rc) return rc;
-  for (int r = 0; r < n_renditions; r++) {
-    const size_t row = (size_t)g.w[r] * g.nc[r];
-    if (!pixels[r] || row_pitch[r] < row || (n_images > 1 && image_stride[r] < row_pitch[r] * (size_t)(g.h[r] - 1) + row)) {
-      set_error("rendition %d: no pixel buffer, or row_pitch or image_stride smaller than the decoded image (%dx%d, %d components)", r, g.w[r], g.h[r], g.nc[r]);
-      return B200JPEG_ERR_PARAM;
-    }
-  }
-  CU(cudaSetDevice(e->device));
-  std::vector<PixTarget> tg;
-  if (pixels_on_device) {
-    // the first rung of each set receives its pixels where the single call would write them
-    for (int r : g.first) tg.push_back(PixTarget{nullptr, static_cast<uint8_t *>(pixels[r]), row_pitch[r], image_stride[r]});
-  } else if ((rc = reserve_rendition_pixels(e, g, n_images, tg))) return rc;
-  for (int k = 0; k < (int)tg.size(); k++) tg[k].opts = &opts[g.first[k]];
-  if ((rc = decompress_files(e, files, sizes, n_images, tg.data(), (int)tg.size(), false))) return rc;
-  for (int r = 0; r < n_renditions; r++) {
-    const PixTarget &t = tg[g.set[r]];
-    if (pixels_on_device && r == g.first[g.set[r]]) continue;
-    for (int i = 0; i < n_images; i++)
-      CU(cudaMemcpy2DAsync(static_cast<uint8_t *>(pixels[r]) + (size_t)i * image_stride[r], row_pitch[r], t.pix + (size_t)i * t.image_stride, t.row_pitch,
-                           (size_t)g.w[r] * g.nc[r], g.h[r], pixels_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, e->stream));
-  }
-  CU(cudaStreamSynchronize(e->stream));
-  e->pending_marks = 0;
-  e->stage_names.clear(); e->stage_ms.clear(); e->stage_calls.clear();
-  add_decompress_stage_times(e);
-  return B200JPEG_OK;
-}
-
 // the stage times of the last encode added into (names, ms, calls)
 static void merge_stage_times(const b200jpeg_encoder *e, std::vector<const char *> &names, std::vector<float> &ms, std::vector<int> &calls)
 {
@@ -2386,138 +2174,108 @@ static void merge_stage_times(const b200jpeg_encoder *e, std::vector<const char 
   }
 }
 
-// b200jpeg_recompress_renditions: the pixels of each distinct option set as decompress_renditions makes them, then per
-// rung recompress_batch's encode of the whole batch from its set's pixels
-static int recompress_renditions(b200jpeg_encoder *e, int n_renditions, const b200jpeg_decompress_options *opts, const b200jpeg_params *params,
-                                 const uint8_t *const *files, const size_t *sizes, int n_images)
+// ------------------------------------------------------------------- decompress and recompress from JPEG files
+// Every call that decodes files to pixels (b200jpeg_decompress_batch, _renditions and _mixed, and the recompress forms
+// of each) runs through one checker (plan_rungs), one per-chunk loop (mixed_files) and one chunk rule (mixed_chunks).
+// A single call is one rung; the single and rendition calls also hold every file to image 0's geometry.  The entropy
+// decode takes the files as they come (DecBatch::mixed); the pixel stage of a chunk of one geometry with evenly spaced
+// outputs is the one-geometry route (chunk_pixels), of every other chunk the ragged IDCT and upsampling kernels driven
+// by a work table, so a chunk costs the same launches whatever the mix of sizes.
+//
+// Refusals come before any device work, in this order: the arguments, the sources image by image, the rungs' options,
+// then the output buffers, or each parameter block (b200jpeg_validate, precision, its image's decoded geometry).  The
+// sources come before the parameter blocks because a caller that cannot build an image's block from a refused file
+// passes an empty one and relies on the file's own refusal (Encoder.recompress_mixed).
+
+// A per-rung, per-image array of a call, read as a[r * rung_step + i * image_step]: a mixed call passes one entry per
+// output, a rendition call one per rung (image step 0), a single call one in all (both steps 0).
+template <class T> struct View {
+  const T *a; size_t rung_step, image_step;
+  const T &operator()(int r, int i) const { return a[(size_t)r * rung_step + (size_t)i * image_step]; }
+};
+
+// A decompress or recompress call: its kind, its R rungs' options and its n files.  The kind decides whether the files
+// must share one geometry (single and rendition calls) and how messages name a rung and an image: a single call names
+// neither, a rendition call the rung, a mixed call the rung and the image.
+enum CallKind { SINGLE_CALL, RENDITION_CALL, MIXED_CALL };
+struct Call {
+  CallKind kind; int R, n;
+  const b200jpeg_decompress_options *opts;
+  const uint8_t *const *files; const size_t *sizes;
+};
+
+// the front of a message about image i of rung r (i < 0: about the rung as a whole)
+static std::string where(const Call &c, int r, int i)
 {
-  if (!e || n_renditions < 1 || !opts || !params || !files || !sizes || n_images <= 0) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
-  if ((long long)n_renditions * n_images > INT_MAX) { set_error("%d renditions of %d images are more outputs than b200jpeg_get_output indexes", n_renditions, n_images); return B200JPEG_ERR_PARAM; }
-  Rungs g;
-  int rc = check_rungs(n_renditions, opts, files, sizes, g);
-  if (rc) return rc;
-  for (int r = 0; r < n_renditions; r++) {
-    const b200jpeg_params *p = &params[r];
-    if ((rc = b200jpeg_validate(p))) { std::string m = b200jpeg_last_error(); set_error("rendition %d: %s", r, m.c_str()); return rc; }
-    if (p->data_precision != 8) { set_error("rendition %d: the sources decode to 8-bit samples, the parameter block has data_precision %d", r, p->data_precision); return B200JPEG_ERR_PARAM; }
-    if (g.w[r] != p->image_width || g.h[r] != p->image_height || g.cs[r] != p->in_color_space || g.nc[r] != p->input_components) {
-      set_error("rendition %d: the sources decode to %dx%d pixels of %d samples in colour space %d, the parameter block describes %dx%d of %d in %d (see b200jpeg_decompress_output_opts)",
-                r, g.w[r], g.h[r], g.nc[r], g.cs[r], p->image_width, p->image_height, p->input_components, p->in_color_space);
-      return B200JPEG_ERR_PARAM;
-    }
-  }
-  CU(cudaSetDevice(e->device));
-  std::vector<PixTarget> tg;
-  if ((rc = reserve_rendition_pixels(e, g, n_images, tg))) return rc;
-  for (int k = 0; k < (int)tg.size(); k++) tg[k].opts = &opts[g.first[k]];
-  if ((rc = decompress_files(e, files, sizes, n_images, tg.data(), (int)tg.size(), true))) return rc;
-  // encode rung by rung; a rung's files move to e->rend_files before the next rung's encode reuses the file arenas
-  std::vector<std::pair<size_t, size_t>> kept;          // (offset in rend_files, size) of the files of rungs 0 .. R-2
-  std::vector<const char *> names; std::vector<float> ms; std::vector<int> calls;
-  size_t scan_bytes = 0;
-  e->rend_files.clear();
-  for (int r = 0; r < n_renditions; r++) {
-    const PixTarget &t = tg[g.set[r]];
-    if ((rc = encode_common(e, &params[r], t.pix, 1, t.row_pitch, t.image_stride, n_images, false, nullptr, nullptr, &e->dec_markers))) return rc;
-    scan_bytes += e->last_scan_bytes;
-    merge_stage_times(e, names, ms, calls);
-    if (r + 1 == n_renditions) break;
-    for (int i = 0; i < n_images; i++) {
-      kept.emplace_back(e->rend_files.size(), e->files[i].second);
-      e->rend_files.insert(e->rend_files.end(), e->files[i].first, e->files[i].first + e->files[i].second);
-    }
-  }
-  std::vector<std::pair<uint8_t *, size_t>> last(e->files);
-  e->files.clear();
-  for (const std::pair<size_t, size_t> &f : kept) e->files.emplace_back(e->rend_files.data() + f.first, f.second);
-  e->files.insert(e->files.end(), last.begin(), last.end());
-  e->last_scan_bytes = scan_bytes;
-  e->stage_names = names; e->stage_ms = ms; e->stage_calls = calls;
-  add_decompress_stage_times(e);
-  return B200JPEG_OK;
+  char b[64] = "";
+  if (c.kind == MIXED_CALL && i >= 0) snprintf(b, sizeof b, "rendition %d, image %d: ", r, i);
+  else if (c.kind != SINGLE_CALL) snprintf(b, sizeof b, "rendition %d: ", r);
+  return b;
 }
 
-// ---------------------------------------------------------------------------------- batches of mixed geometry
-// (b200jpeg_decompress_mixed / b200jpeg_recompress_mixed): the rendition calls without the one-geometry rule.  The
-// entropy decode takes the files as they come (DecBatch::mixed); the pixel stage runs the IDCT and upsampling kernels
-// in their ragged form, driven by a work table, so a chunk costs the same launches whatever the mix of sizes.
-
-// What the mixed calls know before any device work: each source's header and coefficient blocks, the distinct option
-// sets of the rungs (set[r]: rung r's; first[k]: the first rung of set k) and each set's plan for each image.
-struct MixedSrc {
-  std::vector<b200jpeg_source_info> info;
-  std::vector<long long> blocks;
+// What a call knows before any device work: each image's chunk weight, the distinct option sets of the rungs (set[r]:
+// rung r's; first[k]: the first rung of set k) and each set's plan for each image.
+struct RungSets {
+  std::vector<long long> weight;
   std::vector<int> set, first;
   std::vector<std::vector<DecPlan>> plan;              // [set][image]
 };
 
-static int check_mixed(b200jpeg_encoder *e, int n_renditions, const b200jpeg_decompress_options *opts, const uint8_t *const *files,
-                       const size_t *sizes, int n, MixedSrc &m)
+// The checks of a call's sources and rung options: each file parsed into one scratch header and checked as
+// b200jpeg_decompress_batch takes it, then each distinct option set planned for it.  A refused option set is reported
+// after every source passed, for the first image it fails on, naming the image only when that is not image 0.
+static int plan_rungs(const b200jpeg_encoder *e, const Call &c, RungSets &m)
 {
-  m = MixedSrc();
-  m.info.resize(n); m.blocks.assign(n, 0);
-  for (int i = 0; i < n; i++) {
-    if (!files[i]) { set_error("image %d: no file", i); return B200JPEG_ERR_PARAM; }
-    b200jpeg_source_info &s = m.info[i];
-    int rc = b200jpeg_parse_source(files[i], sizes[i], &s);
-    if (rc) { std::string msg = b200jpeg_last_error(); set_error("image %d: %s", i, msg.c_str()); return rc; }
-    if ((rc = check_decompress_source(s, i, e->progressive_decode))) return rc;
-    int hmax = 1, vmax = 1;
-    for (int c = 0; c < s.num_components; c++) { hmax = std::max(hmax, s.h_samp_factor[c]); vmax = std::max(vmax, s.v_samp_factor[c]); }
-    for (int c = 0; c < s.num_components; c++)
-      m.blocks[i] += (long long)div_up((long long)s.image_width * s.h_samp_factor[c], hmax * 8) * div_up((long long)s.image_height * s.v_samp_factor[c], vmax * 8);
-  }
-  for (int r = 0; r < n_renditions; r++) {
-    const b200jpeg_decompress_options &o = opts[r];
+  m = RungSets();
+  for (int r = 0; r < c.R; r++) {
+    const b200jpeg_decompress_options &o = c.opts[r];
     int k = 0;
     for (; k < (int)m.first.size(); k++) {
-      const b200jpeg_decompress_options &f = opts[m.first[k]];
+      const b200jpeg_decompress_options &f = c.opts[m.first[k]];
       if (f.scale_num == o.scale_num && f.scale_denom == o.scale_denom && f.dct_method == o.dct_method &&
           f.do_fancy_upsampling == o.do_fancy_upsampling && f.out_color_space == o.out_color_space && f.all_scales == o.all_scales) break;
     }
-    if (k == (int)m.first.size()) {
-      m.first.push_back(r);
-      m.plan.emplace_back(n);
-      for (int i = 0; i < n; i++)
-        if (int rc = plan_decompress(m.info[i], o, m.plan[k][i])) {
-          std::string msg = b200jpeg_last_error();
-          if (i == 0) set_error("rendition %d: %s", r, msg.c_str()); else set_error("rendition %d, image %d: %s", r, i, msg.c_str());
-          return rc;
-        }
-    }
+    if (k == (int)m.first.size()) m.first.push_back(r);
     m.set.push_back(k);
   }
-  // the chunk weight of an image: its blocks, those whose IDCT writes more than 8 x 8 samples counted as ssize^2 / 64
-  // blocks under the largest of the sets' plans, so a chunk's sample planes stay the size they have at 1/1 (DESIGN §14)
-  for (int i = 0; i < n; i++) {
-    const b200jpeg_source_info &s = m.info[i];
+  const int K = (int)m.first.size();
+  m.plan.assign(K, std::vector<DecPlan>(c.n));
+  m.weight.assign(c.n, 0);
+  std::vector<int> bad(K, -1), bad_rc(K, 0);           // per set: the first image whose plan was refused, and the code
+  std::vector<std::string> why(K);
+  static thread_local b200jpeg_source_info s;
+  std::array<int, 12> g0{};
+  for (int i = 0; i < c.n; i++) {
+    if (!c.files[i]) { set_error("image %d: no file", i); return B200JPEG_ERR_PARAM; }
+    int rc = b200jpeg_parse_source(c.files[i], c.sizes[i], &s);
+    if (rc) { std::string msg = b200jpeg_last_error(); set_error("image %d: %s", i, msg.c_str()); return rc; }
+    if ((rc = check_decompress_source(s, i, e->progressive_decode))) return rc;
+    // the geometry one-geometry calls compare: size, components, sampling factors, and RGB-coded or not
+    const int nc = s.num_components;
+    std::array<int, 12> g{s.image_width, s.image_height, nc, nc == 3 && s.jpeg_color_space == B200JPEG_CS_RGB};
     int hmax = 1, vmax = 1;
-    for (int c = 0; c < s.num_components; c++) { hmax = std::max(hmax, s.h_samp_factor[c]); vmax = std::max(vmax, s.v_samp_factor[c]); }
-    for (const std::vector<DecPlan> &pl : m.plan) {
+    for (int ch = 0; ch < nc; ch++) {
+      g[4 + 2 * ch] = s.h_samp_factor[ch]; g[5 + 2 * ch] = s.v_samp_factor[ch];
+      hmax = std::max(hmax, s.h_samp_factor[ch]); vmax = std::max(vmax, s.v_samp_factor[ch]);
+    }
+    if (i == 0) g0 = g;
+    if (c.kind != MIXED_CALL && g != g0) { set_error("image %d: geometry (size, components, sampling, colour space) differs from image 0", i); return B200JPEG_ERR_PARAM; }
+    // the chunk weight: the image's blocks, those whose IDCT writes more than 8 x 8 samples counted as ssize^2 / 64
+    // blocks under the largest of the sets' plans, so a chunk's sample planes stay the size they have at 1/1 (DESIGN §14)
+    for (int k = 0; k < K; k++) {
+      if (bad[k] >= 0) continue;
+      const DecPlan &p = m.plan[k][i];
+      if ((rc = plan_decompress(s, c.opts[m.first[k]], m.plan[k][i]))) { bad[k] = i; bad_rc[k] = rc; why[k] = b200jpeg_last_error(); continue; }
       long long w = 0;
-      for (int c = 0; c < s.num_components; c++)
-        w += (long long)div_up((long long)s.image_width * s.h_samp_factor[c], hmax * 8) * div_up((long long)s.image_height * s.v_samp_factor[c], vmax * 8) *
-             std::max(64, pl[i].ssize[c] * pl[i].ssize[c]) / 64;
-      m.blocks[i] = std::max(m.blocks[i], w);
+      for (int ch = 0; ch < nc; ch++)
+        w += (long long)div_up((long long)s.image_width * s.h_samp_factor[ch], hmax * 8) * div_up((long long)s.image_height * s.v_samp_factor[ch], vmax * 8) *
+             std::max(64, p.ssize[ch] * p.ssize[ch]) / 64;
+      m.weight[i] = std::max(m.weight[i], w);
     }
   }
+  for (int k = 0; k < K; k++)
+    if (bad[k] >= 0) { set_error("%s%s", where(c, m.first[k], bad[k] ? bad[k] : -1).c_str(), why[k].c_str()); return bad_rc[k]; }
   return B200JPEG_OK;
-}
-
-// The chunks of a mixed batch: images in order until a chunk holds about 1.6 M blocks (an image larger than that is a
-// chunk of its own), or b200jpeg_encoder_set_chunk_images images.  Returns the first image of each chunk and n.
-static std::vector<int> mixed_chunks(const b200jpeg_encoder *e, const std::vector<long long> &blocks)
-{
-  const int n = (int)blocks.size();
-  std::vector<int> start(1, 0);
-  long long acc = 0;
-  for (int i = 0; i < n; i++) {
-    const bool full = e->chunk_images_override > 0 ? i - start.back() == e->chunk_images_override : acc > 0 && acc + blocks[i] > 1600000LL;
-    if (full) { start.push_back(i); acc = 0; }
-    acc += blocks[i];
-  }
-  start.push_back(n);
-  return start;
 }
 
 // where image i of a pixel output goes
@@ -2612,20 +2370,19 @@ static bool evenly_spaced(const std::vector<MixedOut> &o, int i0, int nk, size_t
   return true;
 }
 
-// jpeg_read_scanlines for a batch of mixed geometry, to every option set's outputs (out[k][i]): per chunk the entropy
-// decode, then each set's pixel stage, enqueued together and synchronised once.  A chunk of one geometry (size,
-// sampling, components, RGB-coded or not) whose outputs are evenly spaced takes the one-geometry route (chunk_pixels),
-// faster in its upsampling (DESIGN §12); every other chunk the ragged one.
-static int mixed_files(b200jpeg_encoder *e, const uint8_t *const *files, const size_t *sizes, int n, const MixedSrc &m,
-                       const std::vector<std::vector<MixedOut>> &out, bool want_markers)
+// jpeg_read_scanlines for a call's files, to every option set's outputs (out[k][i]): per chunk the entropy decode, then
+// each set's pixel stage, enqueued together and synchronised once.  A chunk of one geometry (size, sampling,
+// components, RGB-coded or not) whose outputs are evenly spaced takes the one-geometry route (chunk_pixels), faster in
+// its upsampling (DESIGN §12); every other chunk the ragged one.
+static int mixed_files(b200jpeg_encoder *e, const Call &c, const RungSets &m, const std::vector<std::vector<MixedOut>> &out, bool want_markers)
 {
-  const int K = (int)m.first.size();
+  const int K = (int)m.first.size(), n = c.n;
   while (e->pix_ev.size() < (size_t)K * 3) { cudaEvent_t ev; CU(cudaEventCreate(&ev)); e->pix_ev.push_back(ev); }
   for (float &ms : e->dec_ms) ms = 0.f;
   e->dec_ms_prog = false;
   e->dec.want_markers = want_markers;
   if (want_markers) e->dec_markers.assign(n, std::vector<uint8_t>());
-  const std::vector<int> start = mixed_chunks(e, m.blocks);
+  const std::vector<int> start = mixed_chunks(e, m.weight);
   e->chunk = 0;
   std::vector<uint16_t> qt; std::vector<uint32_t> mt; std::vector<MixStage> st(K);
   std::vector<std::array<size_t, 3>> soff;
@@ -2633,7 +2390,7 @@ static int mixed_files(b200jpeg_encoder *e, const uint8_t *const *files, const s
   for (size_t ch = 0; ch + 1 < start.size(); ch++) {
     const int i0 = start[ch], nk = start[ch + 1] - i0;
     e->chunk = std::max(e->chunk, nk);
-    int rc = decode_files(e, files + i0, sizes + i0, nk, i0, true);
+    int rc = decode_files(e, c.files + i0, c.sizes + i0, nk, i0, true);
     if (rc) return rc;
     e->dec_ms_prog |= e->dec_prog;
     if (want_markers) for (int i = 0; i < nk; i++) e->dec_markers[i0 + i].swap(e->dec.markers[i]);
@@ -2659,10 +2416,7 @@ static int mixed_files(b200jpeg_encoder *e, const uint8_t *const *files, const s
     for (int k = 0; k < K; k++)
       if (!uniform[k]) { stage_mixed(e, m.plan[k], i0, nk, qs, out[k].data() + i0, e->d_dec_samples.as<uint8_t>(), st[k]); meta = std::max(meta, st[k].meta.size()); }
     if ((rc = e->d_mix_meta.reserve(meta))) return rc;
-    qt.assign((size_t)nk * qs * 64, 0);
-    for (int i = 0; i < nk; i++)
-      for (int c = 0; c < e->dec.geom[i].nc; c++) memcpy(&qt[((size_t)i * qs + c) * 64], e->dec.info[i].comp_quant[c], 128);
-    CU(cudaMemcpyAsync(e->d_dec_quant.p, qt.data(), qt.size() * 2, cudaMemcpyHostToDevice, s));
+    if ((rc = upload_chunk_quant(e, nk, qs, qt))) return rc;
     const int16_t *coef[3];
     for (int c = 0; c < 3; c++) coef[c] = reinterpret_cast<const int16_t *>(e->d_dec_planes.as<uint8_t>() + e->dec_plane_off[c]);
     for (int k = 0; k < K; k++) {
@@ -2702,70 +2456,68 @@ static int mixed_files(b200jpeg_encoder *e, const uint8_t *const *files, const s
   return B200JPEG_OK;
 }
 
-// each set's pixels for the whole batch in one device buffer, image i at off[k][i], rows pitch[k][i] apart (the
-// decoded row padded to 4 bytes, as recompress_batch's); order[k]: the images in buffer order
-struct MixedPix { std::vector<std::vector<size_t>> off, pitch; };
-static int reserve_mixed_pixels(b200jpeg_encoder *e, const MixedSrc &m, const std::vector<std::vector<int>> &order, MixedPix &mp,
-                                std::vector<std::vector<MixedOut>> &out)
+// each set's pixels for the whole batch in one device buffer, the images in order[k], each row the decoded row padded
+// to 4 bytes (the pitch the encoder reads)
+static int reserve_set_pixels(b200jpeg_encoder *e, const RungSets &m, const std::vector<std::vector<int>> &order, std::vector<std::vector<MixedOut>> &out)
 {
-  const int K = (int)m.first.size(), n = (int)m.info.size();
+  const int K = (int)m.first.size(), n = (int)m.weight.size();
   if ((int)e->d_rend_pixels.size() < K) e->d_rend_pixels.resize(K);
-  mp.off.assign(K, std::vector<size_t>(n)); mp.pitch.assign(K, std::vector<size_t>(n));
   out.assign(K, std::vector<MixedOut>(n));
+  std::vector<size_t> off(n);
   for (int k = 0; k < K; k++) {
     size_t total = 0;
     for (int i : order[k]) {
       const DecPlan &p = m.plan[k][i];
-      mp.pitch[k][i] = ((size_t)p.out_w * p.out_nc + 3) & ~(size_t)3; mp.off[k][i] = total; total += mp.pitch[k][i] * p.out_h;
+      out[k][i].row_pitch = ((size_t)p.out_w * p.out_nc + 3) & ~(size_t)3; off[i] = total; total += out[k][i].row_pitch * p.out_h;
     }
     if (int rc = e->d_rend_pixels[k].reserve(total)) return rc;
-    for (int i = 0; i < n; i++) out[k][i] = MixedOut{e->d_rend_pixels[k].as<uint8_t>() + mp.off[k][i], mp.pitch[k][i]};
+    for (int i = 0; i < n; i++) out[k][i].pix = e->d_rend_pixels[k].as<uint8_t>() + off[i];
   }
   return B200JPEG_OK;
 }
 
-// b200jpeg_decompress_mixed: one decode per chunk, one ragged pixel stage per distinct option set, the rungs that share
-// a set copied from the first of them
-static int decompress_mixed(b200jpeg_encoder *e, int n_renditions, const b200jpeg_decompress_options *opts, const uint8_t *const *files,
-                            const size_t *sizes, int n_images, void *const *pixels, int pixels_on_device, const size_t *row_pitch)
+// The decompress calls: image i of rung r goes to pix(r, i) + i * stride(r, i), rows pitch(r, i) apart.  One decode per
+// chunk and one pixel stage per distinct option set; on the device the first rung of each set receives its pixels in
+// place, every other output is copied from its set's.
+static int decompress_rungs(b200jpeg_encoder *e, const Call &c, View<void *> pix, View<size_t> pitch, View<size_t> stride, int on_device)
 {
-  if (!e || n_renditions < 1 || !opts || !files || !sizes || n_images <= 0 || !pixels || !row_pitch) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
-  if ((long long)n_renditions * n_images > INT_MAX) { set_error("%d renditions of %d images are more outputs than one call indexes", n_renditions, n_images); return B200JPEG_ERR_PARAM; }
-  const int n = n_images;
-  MixedSrc m;
-  int rc = check_mixed(e, n_renditions, opts, files, sizes, n, m);
+  RungSets m;
+  int rc = plan_rungs(e, c, m);
   if (rc) return rc;
-  for (int r = 0; r < n_renditions; r++)
+  const int n = c.n, K = (int)m.first.size();
+  for (int r = 0; r < c.R; r++)
     for (int i = 0; i < n; i++) {
       const DecPlan &p = m.plan[m.set[r]][i];
-      const size_t j = (size_t)r * n + i;
-      if (!pixels[j] || row_pitch[j] < (size_t)p.out_w * p.out_nc) {
+      const size_t row = (size_t)p.out_w * p.out_nc;
+      if (c.kind == MIXED_CALL && (!pix(r, i) || pitch(r, i) < row)) {
         set_error("rendition %d, image %d: no pixel buffer, or row_pitch smaller than the decoded row (%dx%d, %d components)", r, i, p.out_w, p.out_h, p.out_nc);
+        return B200JPEG_ERR_PARAM;
+      }
+      if (c.kind != MIXED_CALL && (!pix(r, i) || pitch(r, i) < row || (n > 1 && stride(r, i) < pitch(r, i) * (size_t)(p.out_h - 1) + row))) {
+        set_error("%s%srow_pitch or image_stride smaller than the decoded image (%dx%d, %d components)", where(c, r, -1).c_str(),
+                  c.kind == RENDITION_CALL ? "no pixel buffer, or " : "", p.out_w, p.out_h, p.out_nc);
         return B200JPEG_ERR_PARAM;
       }
     }
   CU(cudaSetDevice(e->device));
-  const int K = (int)m.first.size();
+  auto dst = [&](int r, int i) { return static_cast<uint8_t *>(pix(r, i)) + (size_t)i * stride(r, i); };
   std::vector<std::vector<MixedOut>> out(K, std::vector<MixedOut>(n));
-  if (pixels_on_device) {
-    // the first rung of each set receives its pixels where the caller wants them
+  if (on_device) {
     for (int k = 0; k < K; k++)
-      for (int i = 0; i < n; i++) { const size_t j = (size_t)m.first[k] * n + i; out[k][i] = MixedOut{static_cast<uint8_t *>(pixels[j]), row_pitch[j]}; }
+      for (int i = 0; i < n; i++) out[k][i] = MixedOut{dst(m.first[k], i), pitch(m.first[k], i)};
   } else {
     std::vector<std::vector<int>> order(K, std::vector<int>(n));
-    for (int k = 0; k < K; k++) for (int i = 0; i < n; i++) order[k][i] = i;
-    MixedPix mp;
-    if ((rc = reserve_mixed_pixels(e, m, order, mp, out))) return rc;
+    for (std::vector<int> &o : order) for (int i = 0; i < n; i++) o[i] = i;
+    if ((rc = reserve_set_pixels(e, m, order, out))) return rc;
   }
-  if ((rc = mixed_files(e, files, sizes, n, m, out, false))) return rc;
-  for (int r = 0; r < n_renditions; r++) {
+  if ((rc = mixed_files(e, c, m, out, false))) return rc;
+  for (int r = 0; r < c.R; r++) {
     const int k = m.set[r];
-    if (pixels_on_device && r == m.first[k]) continue;
+    if (on_device && r == m.first[k]) continue;
     for (int i = 0; i < n; i++) {
       const DecPlan &p = m.plan[k][i];
-      const size_t j = (size_t)r * n + i;
-      CU(cudaMemcpy2DAsync(pixels[j], row_pitch[j], out[k][i].pix, out[k][i].row_pitch, (size_t)p.out_w * p.out_nc, p.out_h,
-                           pixels_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, e->stream));
+      CU(cudaMemcpy2DAsync(dst(r, i), pitch(r, i), out[k][i].pix, out[k][i].row_pitch, (size_t)p.out_w * p.out_nc, p.out_h,
+                           on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, e->stream));
     }
   }
   CU(cudaStreamSynchronize(e->stream));
@@ -2775,33 +2527,38 @@ static int decompress_mixed(b200jpeg_encoder *e, int n_renditions, const b200jpe
   return B200JPEG_OK;
 }
 
-// b200jpeg_recompress_mixed: the pixels of each distinct option set as decompress_mixed makes them, then per rung one
-// encode per group of images with identical parameter blocks (same decoded size, so one pitch and stride), from the
-// group's images laid out one after another; outputs back in input order
-static int recompress_mixed(b200jpeg_encoder *e, int n_renditions, const b200jpeg_decompress_options *opts, const b200jpeg_params *params,
-                            const uint8_t *const *files, const size_t *sizes, int n_images)
+// The recompress calls: image i of rung r is encoded with params(r, i).  The pixels of each distinct option set as
+// decompress_rungs makes them, then per rung one encode per group of images with identical parameter blocks (one
+// decoded size, so one pitch and stride), from the group's images one after another; outputs numbered rung by rung in
+// input order.
+static int recompress_rungs(b200jpeg_encoder *e, const Call &c, View<b200jpeg_params> params)
 {
-  if (!e || n_renditions < 1 || !opts || !params || !files || !sizes || n_images <= 0) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
-  if ((long long)n_renditions * n_images > INT_MAX) { set_error("%d renditions of %d images are more outputs than b200jpeg_get_output indexes", n_renditions, n_images); return B200JPEG_ERR_PARAM; }
-  const int n = n_images;
-  MixedSrc m;
-  int rc = check_mixed(e, n_renditions, opts, files, sizes, n, m);
+  const int n = c.n, R = c.R;
+  const bool mixed = c.kind == MIXED_CALL;
+  RungSets m;
+  int rc = plan_rungs(e, c, m);
   if (rc) return rc;
   // group[r][i]: the first image of rung r whose parameter block equals image i's
-  std::vector<std::vector<int>> group(n_renditions, std::vector<int>(n));
-  for (int r = 0; r < n_renditions; r++)
+  std::vector<std::vector<int>> group(R, std::vector<int>(n));
+  for (int r = 0; r < R; r++)
     for (int i = 0; i < n; i++) {
-      const b200jpeg_params *p = &params[(size_t)r * n + i];
+      const b200jpeg_params *p = &params(r, i);
+      if (i == 0 || params.image_step) {
+        if ((rc = b200jpeg_validate(p))) { std::string msg = b200jpeg_last_error(); set_error("%s%s", where(c, r, i).c_str(), msg.c_str()); return rc; }
+        if (p->data_precision != 8) {
+          set_error("%sthe source%s to 8-bit samples, the parameter block has data_precision %d", where(c, r, i).c_str(), mixed ? " decodes" : "s decode", p->data_precision);
+          return B200JPEG_ERR_PARAM;
+        }
+      }
       const DecPlan &pl = m.plan[m.set[r]][i];
-      if ((rc = b200jpeg_validate(p))) { std::string msg = b200jpeg_last_error(); set_error("rendition %d, image %d: %s", r, i, msg.c_str()); return rc; }
-      if (p->data_precision != 8) { set_error("rendition %d, image %d: the source decodes to 8-bit samples, the parameter block has data_precision %d", r, i, p->data_precision); return B200JPEG_ERR_PARAM; }
       if (pl.out_w != p->image_width || pl.out_h != p->image_height || pl.out_cs != p->in_color_space || pl.out_nc != p->input_components) {
-        set_error("rendition %d, image %d: the source decodes to %dx%d pixels of %d samples in colour space %d, the parameter block describes %dx%d of %d in %d (see b200jpeg_decompress_output_opts)",
-                  r, i, pl.out_w, pl.out_h, pl.out_nc, pl.out_cs, p->image_width, p->image_height, p->input_components, p->in_color_space);
+        set_error("%sthe source%s to %dx%d pixels of %d samples in colour space %d, the parameter block describes %dx%d of %d in %d (see b200jpeg_decompress_output%s)",
+                  where(c, r, i).c_str(), mixed ? " decodes" : "s decode", pl.out_w, pl.out_h, pl.out_nc, pl.out_cs, p->image_width, p->image_height,
+                  p->input_components, p->in_color_space, c.kind == SINGLE_CALL ? "" : "_opts");
         return B200JPEG_ERR_PARAM;
       }
       int g = 0;
-      while (g < i && !(group[r][g] == g && !memcmp(&params[(size_t)r * n + g], p, sizeof *p))) g++;
+      while (g < i && !(group[r][g] == g && (&params(r, g) == p || !memcmp(&params(r, g), p, sizeof *p)))) g++;
       group[r][i] = g;
     }
   CU(cudaSetDevice(e->device));
@@ -2812,24 +2569,28 @@ static int recompress_mixed(b200jpeg_encoder *e, int n_renditions, const b200jpe
     const std::vector<int> &gr = group[m.first[k]];
     for (int g = 0; g < n; g++) if (gr[g] == g) for (int i = g; i < n; i++) if (gr[i] == g) order[k].push_back(i);
   }
-  MixedPix mp;
   std::vector<std::vector<MixedOut>> out;
-  if ((rc = reserve_mixed_pixels(e, m, order, mp, out))) return rc;
-  if ((rc = mixed_files(e, files, sizes, n, m, out, true))) return rc;
-  std::vector<std::pair<size_t, size_t>> kept((size_t)n_renditions * n);     // (offset in rend_files, size) per output
+  if ((rc = reserve_set_pixels(e, m, order, out))) return rc;
+  if ((rc = mixed_files(e, c, m, out, true))) return rc;
+  // a group's files move to e->rend_files when another encode follows and would reuse the file arenas; the last
+  // encode's stay where they are.  kept: per output, (offset in rend_files, size), or (SIZE_MAX, its index in the last
+  // encode).
+  int last = n - 1;
+  while (group[R - 1][last] != last) last--;
+  std::vector<std::pair<size_t, size_t>> kept((size_t)R * n);
   std::vector<const char *> names; std::vector<float> ms; std::vector<int> calls;
   std::vector<std::vector<uint8_t>> markers;
   size_t scan_bytes = 0;
   e->rend_files.clear();
-  for (int r = 0; r < n_renditions; r++) {
+  for (int r = 0; r < R; r++) {
     const int k = m.set[r];
     for (int g = 0; g < n; g++) {
       if (group[r][g] != g) continue;
       std::vector<int> mem;
       for (int i = g; i < n; i++) if (group[r][i] == g) mem.push_back(i);
-      const size_t pitch = mp.pitch[k][g], stride = pitch * (size_t)m.plan[k][g].out_h;
+      const size_t pitch = out[k][g].row_pitch, stride = pitch * (size_t)m.plan[k][g].out_h;
       bool in_place = true;
-      for (size_t j = 1; j < mem.size(); j++) in_place &= mp.off[k][mem[j]] == mp.off[k][mem[0]] + j * stride;
+      for (size_t j = 1; j < mem.size(); j++) in_place &= out[k][mem[j]].pix == out[k][mem[0]].pix + j * stride;
       const uint8_t *src = out[k][mem[0]].pix;
       if (!in_place) {                                 // another rung's grouping: gather the group's images
         if ((rc = e->d_dec_pixels.reserve(stride * mem.size()))) return rc;
@@ -2837,19 +2598,25 @@ static int recompress_mixed(b200jpeg_encoder *e, int n_renditions, const b200jpe
           CU(cudaMemcpyAsync(e->d_dec_pixels.as<uint8_t>() + j * stride, out[k][mem[j]].pix, stride, cudaMemcpyDeviceToDevice, e->stream));
         src = e->d_dec_pixels.as<uint8_t>();
       }
-      markers.resize(mem.size());
-      for (size_t j = 0; j < mem.size(); j++) markers[j] = e->dec_markers[mem[j]];
-      if ((rc = encode_common(e, &params[(size_t)r * n + g], src, 1, pitch, stride, (int)mem.size(), false, nullptr, nullptr, &markers))) return rc;
+      const std::vector<std::vector<uint8_t>> *mk = &e->dec_markers;     // the whole batch in input order
+      if ((int)mem.size() < n) {
+        markers.resize(mem.size());
+        for (size_t j = 0; j < mem.size(); j++) markers[j] = e->dec_markers[mem[j]];
+        mk = &markers;
+      }
+      if ((rc = encode_common(e, &params(r, g), src, 1, pitch, stride, (int)mem.size(), false, nullptr, nullptr, mk))) return rc;
       scan_bytes += e->last_scan_bytes;
       merge_stage_times(e, names, ms, calls);
+      const bool final = r + 1 == R && g == last;
       for (size_t j = 0; j < mem.size(); j++) {
-        kept[(size_t)r * n + mem[j]] = std::make_pair(e->rend_files.size(), e->files[j].second);
-        e->rend_files.insert(e->rend_files.end(), e->files[j].first, e->files[j].first + e->files[j].second);
+        kept[(size_t)r * n + mem[j]] = final ? std::make_pair(SIZE_MAX, j) : std::make_pair(e->rend_files.size(), e->files[j].second);
+        if (!final) e->rend_files.insert(e->rend_files.end(), e->files[j].first, e->files[j].first + e->files[j].second);
       }
     }
   }
+  const std::vector<std::pair<uint8_t *, size_t>> fin(e->files);
   e->files.clear();
-  for (const std::pair<size_t, size_t> &f : kept) e->files.emplace_back(e->rend_files.data() + f.first, f.second);
+  for (const std::pair<size_t, size_t> &f : kept) e->files.push_back(f.first == SIZE_MAX ? fin[f.second] : std::make_pair(e->rend_files.data() + f.first, f.second));
   e->last_scan_bytes = scan_bytes;
   e->stage_names = names; e->stage_ms = ms; e->stage_calls = calls;
   add_decompress_stage_times(e);
@@ -2863,14 +2630,16 @@ extern "C" {
 int b200jpeg_decompress_batch(b200jpeg_encoder *e, const uint8_t *const *files, const size_t *sizes, int n_images,
                               void *pixels, int pixels_on_device, size_t row_pitch, size_t image_stride)
 {
-  return b200::decompress_batch(e, nullptr, files, sizes, n_images, pixels, pixels_on_device, row_pitch, image_stride);
+  const b200jpeg_decompress_options o = b200jpeg_default_decompress_options();
+  return b200jpeg_decompress_batch_opts(e, &o, files, sizes, n_images, pixels, pixels_on_device, row_pitch, image_stride);
 }
 
 int b200jpeg_decompress_batch_opts(b200jpeg_encoder *e, const b200jpeg_decompress_options *opts, const uint8_t *const *files,
                                    const size_t *sizes, int n_images, void *pixels, int pixels_on_device, size_t row_pitch, size_t image_stride)
 {
-  if (!opts) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
-  return b200::decompress_batch(e, opts, files, sizes, n_images, pixels, pixels_on_device, row_pitch, image_stride);
+  if (!e || !opts || !files || !sizes || !pixels || n_images <= 0) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
+  return decompress_rungs(e, Call{SINGLE_CALL, 1, n_images, opts, files, sizes}, View<void *>{&pixels, 0, 0}, View<size_t>{&row_pitch, 0, 0},
+                          View<size_t>{&image_stride, 0, 0}, pixels_on_device);
 }
 
 int b200jpeg_decompress_yuv_batch(b200jpeg_encoder *e, const b200jpeg_decompress_options *opts, const uint8_t *const *files,
@@ -2889,14 +2658,15 @@ int b200jpeg_decode_yuv_batch(b200jpeg_encoder *e, const b200jpeg_params *p, con
 
 int b200jpeg_recompress_batch(b200jpeg_encoder *e, const b200jpeg_params *p, const uint8_t *const *files, const size_t *sizes, int n_images)
 {
-  return b200::recompress_batch(e, nullptr, p, files, sizes, n_images);
+  const b200jpeg_decompress_options o = b200jpeg_default_decompress_options();
+  return b200jpeg_recompress_batch_opts(e, &o, p, files, sizes, n_images);
 }
 
 int b200jpeg_recompress_batch_opts(b200jpeg_encoder *e, const b200jpeg_decompress_options *opts, const b200jpeg_params *p,
                                    const uint8_t *const *files, const size_t *sizes, int n_images)
 {
-  if (!opts) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
-  return b200::recompress_batch(e, opts, p, files, sizes, n_images);
+  if (!e || !opts || !p || !files || !sizes || n_images <= 0) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
+  return recompress_rungs(e, Call{SINGLE_CALL, 1, n_images, opts, files, sizes}, View<b200jpeg_params>{p, 0, 0});
 }
 
 int b200jpeg_decompress_renditions(b200jpeg_encoder *e, int n_renditions, const b200jpeg_decompress_options *opts, const uint8_t *const *files,
@@ -2904,21 +2674,30 @@ int b200jpeg_decompress_renditions(b200jpeg_encoder *e, int n_renditions, const 
                                    const size_t *row_pitch, const size_t *image_stride)
 {
   if (e) e->files.clear();                       // a refused call leaves no outputs behind
-  return b200::decompress_renditions(e, n_renditions, opts, files, sizes, n_images, pixels, pixels_on_device, row_pitch, image_stride);
+  if (!e || n_renditions < 1 || !opts || !files || !sizes || n_images <= 0 || !pixels || !row_pitch || !image_stride) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
+  return decompress_rungs(e, Call{RENDITION_CALL, n_renditions, n_images, opts, files, sizes}, View<void *>{pixels, 1, 0}, View<size_t>{row_pitch, 1, 0},
+                          View<size_t>{image_stride, 1, 0}, pixels_on_device);
 }
 
 int b200jpeg_decompress_mixed(b200jpeg_encoder *e, int n_renditions, const b200jpeg_decompress_options *opts, const uint8_t *const *files,
                               const size_t *sizes, int n_images, void *const *pixels, int pixels_on_device, const size_t *row_pitch)
 {
   if (e) e->files.clear();
-  return b200::decompress_mixed(e, n_renditions, opts, files, sizes, n_images, pixels, pixels_on_device, row_pitch);
+  if (!e || n_renditions < 1 || !opts || !files || !sizes || n_images <= 0 || !pixels || !row_pitch) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
+  if ((long long)n_renditions * n_images > INT_MAX) { set_error("%d renditions of %d images are more outputs than one call indexes", n_renditions, n_images); return B200JPEG_ERR_PARAM; }
+  static const size_t none = 0;                  // each output is placed on its own: no image stride
+  const size_t n = (size_t)n_images;
+  return decompress_rungs(e, Call{MIXED_CALL, n_renditions, n_images, opts, files, sizes}, View<void *>{pixels, n, 1}, View<size_t>{row_pitch, n, 1},
+                          View<size_t>{&none, 0, 0}, pixels_on_device);
 }
 
 int b200jpeg_recompress_mixed(b200jpeg_encoder *e, int n_renditions, const b200jpeg_decompress_options *opts, const b200jpeg_params *params,
                               const uint8_t *const *files, const size_t *sizes, int n_images)
 {
   if (e) e->files.clear();
-  const int rc = b200::recompress_mixed(e, n_renditions, opts, params, files, sizes, n_images);
+  if (!e || n_renditions < 1 || !opts || !params || !files || !sizes || n_images <= 0) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
+  if ((long long)n_renditions * n_images > INT_MAX) { set_error("%d renditions of %d images are more outputs than b200jpeg_get_output indexes", n_renditions, n_images); return B200JPEG_ERR_PARAM; }
+  const int rc = recompress_rungs(e, Call{MIXED_CALL, n_renditions, n_images, opts, files, sizes}, View<b200jpeg_params>{params, (size_t)n_images, 1});
   if (rc && e) e->files.clear();
   return rc;
 }
@@ -2927,7 +2706,9 @@ int b200jpeg_recompress_renditions(b200jpeg_encoder *e, int n_renditions, const 
                                    const uint8_t *const *files, const size_t *sizes, int n_images)
 {
   if (e) e->files.clear();
-  const int rc = b200::recompress_renditions(e, n_renditions, opts, params, files, sizes, n_images);
+  if (!e || n_renditions < 1 || !opts || !params || !files || !sizes || n_images <= 0) { set_error("bad argument"); return B200JPEG_ERR_PARAM; }
+  if ((long long)n_renditions * n_images > INT_MAX) { set_error("%d renditions of %d images are more outputs than b200jpeg_get_output indexes", n_renditions, n_images); return B200JPEG_ERR_PARAM; }
+  const int rc = recompress_rungs(e, Call{RENDITION_CALL, n_renditions, n_images, opts, files, sizes}, View<b200jpeg_params>{params, 1, 0});
   if (rc && e) e->files.clear();
   return rc;
 }

@@ -182,6 +182,19 @@ def test_refusals_name_the_image_and_the_encoder_recovers(built):
         enc.decompress([good], scale=(3, 8))
     with pytest.raises(mj.B200JpegError, match="Unsupported color conversion request"):
         enc.decompress([O.source("gray")[0]], colorspace="ycbcr")
+    # a refused option set reads the same whether the pixels go to host or to device memory
+    import ctypes as C
+    import torch
+    from mozjpeg_b200 import _abi as A
+    _, ptrs, sizes = enc._files([good])
+    o = mj.decompress_options(scale=(3, 8))
+    host, dev = np.empty((136, 200, 3), dtype=np.uint8), torch.empty((136, 200, 3), dtype=torch.uint8, device="cuda")
+    msgs = []
+    for ptr, on_device in ((host.ctypes.data, 0), (dev.data_ptr(), 1)):
+        with pytest.raises(mj.B200JpegError) as e:
+            A.check(A.load().b200jpeg_decompress_batch_opts(enc._h, C.byref(o), ptrs, sizes, 1, ptr, on_device, 600, 600 * 136), "decompress_batch_opts")
+        msgs.append(str(e.value))
+    assert msgs[0] == msgs[1] and "IDCT block size of 3" in msgs[0], msgs
     want = PIX["o_420:1/2:int:fancy:default"]
     assert O.md5(enc.decompress([O.source("o_420")[0]], scale=(1, 2))[0]) == want["pix_md5"]
     enc.close()

@@ -185,10 +185,17 @@ def test_permuting_the_inputs_permutes_the_outputs(encoder):
 def test_a_uniform_batch_gives_the_batch_routes_outputs(encoder):
     import mozjpeg_b200 as mj
     files = [_src("u_420", 227, 149, 30 + k, ["-revert", "-sample", "2x2", "-quality", str(60 + 10 * k)]) for k in range(3)]
+
+    def launches(fn):
+        before = encoder.kernel_launches()
+        got = fn()
+        return got, encoder.kernel_launches() - before
     for kw in [{}, dict(scale=(1, 2), dct="float"), dict(colorspace="gray")]:
-        out = encoder.decompress_mixed(files, [kw])[0]
-        batch = encoder.decompress(files, **kw)
-        assert all(np.array_equal(out[i], batch[i]) for i in range(len(files))), kw
+        out, n_mixed = launches(lambda: encoder.decompress_mixed(files, [kw])[0])
+        rend, n_rend = launches(lambda: encoder.decompress_renditions(files, [kw])[0])
+        batch, n_batch = launches(lambda: encoder.decompress(files, **kw))
+        assert all(np.array_equal(out[i], batch[i]) and np.array_equal(rend[i], batch[i]) for i in range(len(files))), kw
+        assert n_mixed == n_rend == n_batch, (kw, n_mixed, n_rend, n_batch)
     p = mj.params_for_jpeg_input(["-quality", "75"], files[0])
     assert encoder.recompress_mixed(files, [(["-quality", "75"], {})])[0] == encoder.recompress(p, files)
 
