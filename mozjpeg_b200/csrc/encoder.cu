@@ -82,7 +82,7 @@ using namespace b200;
 #define MAX_ARENAS 4
 struct Arena {
   b200::DevBuf d_planes;             // input smoothing: the pre-pass's component planes
-  b200::DevBuf d_coef[4], d_raw[4], d_plain[4], d_hist, d_tabs_trellis, d_rec, d_srec, d_splits, d_best_al, d_qimg, d_qsum, d_eo, d_es;
+  b200::DevBuf d_coef[4], d_raw[4], d_plain[4], d_hist, d_tabs_trellis, d_rec, d_big, d_bigcnt, d_best_al, d_qimg, d_qsum, d_eo, d_es;
   b200::DevBuf d_slot, d_blk_aux, d_blk_run, d_blk_mask;
   b200::DevBuf d_stream;             // the scans' coded stream (ScanStream, kernels.cuh)
   b200::DevBuf d_sym, d_dcq;         // sequential scans after the trellis: symbol records + dense DC values (SymOut, kernels.cuh)
@@ -90,7 +90,7 @@ struct Arena {
   b200::Geom g;                      // the plan's geometry with this arena's coefficient pointers
   b200::ScanStream ss;               // the buffers inside d_stream (status: the chunk's)
   void release() {
-    b200::DevBuf *db[] = {&d_planes, &d_hist, &d_tabs_trellis, &d_rec, &d_srec, &d_splits, &d_best_al, &d_qimg, &d_qsum, &d_eo, &d_es, &d_slot, &d_blk_aux, &d_blk_run, &d_blk_mask, &d_stream, &d_sym, &d_dcq, &d_diff};
+    b200::DevBuf *db[] = {&d_planes, &d_hist, &d_tabs_trellis, &d_rec, &d_big, &d_bigcnt, &d_best_al, &d_qimg, &d_qsum, &d_eo, &d_es, &d_slot, &d_blk_aux, &d_blk_run, &d_blk_mask, &d_stream, &d_sym, &d_dcq, &d_diff};
     for (b200::DevBuf *b : db) b->release();
     for (int i = 0; i < 4; i++) { d_coef[i].release(); d_raw[i].release(); d_plain[i].release(); }
   }
@@ -510,8 +510,8 @@ static int prepare_batch(b200jpeg_encoder *e, int n_total, int chunk, bool host_
     if ((rc = a.d_hist.reserve(hist_bytes * g.nc))) return rc;
     if ((rc = a.d_tabs_trellis.reserve(tabset * 4 * n))) return rc;
     if ((rc = a.d_rec.reserve((size_t)n * pl.sum_real_blocks * sizeof(DcRec)))) return rc;
-    if ((rc = a.d_srec.reserve((size_t)n * pl.sum_real_blocks * 16))) return rc;
-    if ((rc = a.d_splits.reserve((size_t)n * 4 * (4 + 128) * 4))) return rc;      // class boundaries + the sort's counters
+    if ((rc = a.d_big.reserve((size_t)n * pl.sum_real_blocks * 16))) return rc;     // the AC trellis's big-class lists
+    if ((rc = a.d_bigcnt.reserve((size_t)n * 4 * 2 * 4))) return rc;               // and their lengths
     if (use_symrec(pl, p)) {
       if ((rc = a.d_sym.reserve((size_t)n * pl.sum_real_blocks * SYMREC_BYTES))) return rc;
       if ((rc = a.d_dcq.reserve((size_t)n * pl.sum_real_blocks * 2))) return rc;
@@ -773,11 +773,8 @@ static int run_pipeline(b200jpeg_encoder *e, const ChunkIO &io, Timer &tm)
       }
     }
     if (!generic_rounds) {
-      tm.mark("trellis_sort");
-      launch_trellis_sort(gr, A.d_rec.as<DcRec>(), rlr, A.d_srec.p, A.d_splits.as<uint32_t>(), n, s);
       tm.mark("trellis_ac");
-      if (so.hist) CU(cudaMemsetAsync(A.d_hist.p, 0, hist_bytes, s));
-      launch_trellis_ac3(gr, e->d_tc.as<TrellisConsts>(), tset, tabset, A.d_rec.as<DcRec>(), rlr, A.d_srec.p, A.d_splits.as<uint32_t>(), so, n, e->sms, s);
+      launch_trellis_ac3(gr, e->d_tc.as<TrellisConsts>(), tset, tabset, A.d_rec.as<DcRec>(), rlr, A.d_big.p, A.d_bigcnt.as<uint32_t>(), so, n, e->sms, s);
     } else {
       tm.mark("trellis_ac");
       float4 *eo = eobopt ? A.d_eo.as<float4>() : nullptr;

@@ -2092,86 +2092,23 @@ void launch_qopt_update(long long *qsum, uint16_t *qimg, int n, cudaStream_t s)
   LAUNCHED();
 }
 
-// sorted side record of the AC trellis: {norm, block index inside the component, non-zero mask}
+// entry of the AC trellis's big-class lists: {norm, block index inside the component, non-zero mask}
 struct SRec { float norm; uint32_t lin; unsigned long long nzmask; };
 static_assert(sizeof(SRec) == 16, "SRec layout");
-
-// Counting sort of every (image, component)'s side records by their number of non-zero plain-quantized AC values,
-// in decreasing order, so that the 32 blocks a warp of the trellis kernel works on have similar trip counts; four class
-// boundaries per (image, component): [0, s0) more than 32 non-zeros, [s0, s1) mid_max+1..32, [s1, s2) 9..mid_max,
-// [s2, nblk) at most 8.  Spread over several CTAs per (image, component) (one CTA each left most SMs idle behind the
-// luma planes): k_sort_count adds each slice's counts per non-zero count to global counters, k_sort_scatter turns them
-// into class offsets, reserves a range per count and slice with one global atomic each and writes the records.  The
-// order inside a count is arbitrary (it only decides which blocks share a warp).  gcnt / gcur: [n*nc][64], zeroed.
-#define SORT_SLICE 4096
-__global__ void __launch_bounds__(256) k_sort_count(Geom g, const DcRec *__restrict__ rec, RecLayout rl, unsigned *__restrict__ gcnt)
-{
-  __shared__ unsigned cnt[64];
-  const int ci = blockIdx.y % g.nc, img = blockIdx.y / g.nc;
-  const CompGeom &c = g.c[ci];
-  const long long nblk = (long long)c.wib * c.hib, b0 = (long long)blockIdx.x * SORT_SLICE;
-  if (b0 >= nblk) return;
-  const DcRec *r = rec + (size_t)img * rl.per_image + rl.comp_off[ci];
-  if (threadIdx.x < 64) cnt[threadIdx.x] = 0;
-  __syncthreads();
-  const long long b1 = min(nblk, b0 + SORT_SLICE);
-  for (long long b = b0 + threadIdx.x; b < b1; b += blockDim.x) atomicAdd(&cnt[63 - min((int)r[b].nz, 63)], 1u);
-  __syncthreads();
-  if (threadIdx.x < 64 && cnt[threadIdx.x]) atomicAdd(&gcnt[(size_t)blockIdx.y * 64 + threadIdx.x], cnt[threadIdx.x]);
-}
-__global__ void __launch_bounds__(256) k_sort_scatter(Geom g, const DcRec *__restrict__ rec, RecLayout rl, SRec *__restrict__ srec, uint32_t *__restrict__ splits,
-                                                      const unsigned *__restrict__ gcnt, unsigned *__restrict__ gcur, int mid_max)
-{
-  __shared__ unsigned cnt[64], start[64];
-  const int ci = blockIdx.y % g.nc, img = blockIdx.y / g.nc;
-  const CompGeom &c = g.c[ci];
-  const long long nblk = (long long)c.wib * c.hib, b0 = (long long)blockIdx.x * SORT_SLICE;
-  if (b0 >= nblk) return;
-  const DcRec *r = rec + (size_t)img * rl.per_image + rl.comp_off[ci];
-  SRec *p = srec + (size_t)img * rl.per_image + rl.comp_off[ci];
-  if (threadIdx.x < 64) cnt[threadIdx.x] = 0;
-  __syncthreads();
-  const long long b1 = min(nblk, b0 + SORT_SLICE);
-  for (long long b = b0 + threadIdx.x; b < b1; b += blockDim.x) atomicAdd(&cnt[63 - min((int)r[b].nz, 63)], 1u);
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    unsigned a = 0;
-    for (int k = 0; k < 64; k++) { start[k] = a; a += gcnt[(size_t)blockIdx.y * 64 + k]; }
-    if (blockIdx.x == 0) {
-      splits[4 * blockIdx.y] = start[63 - 32]; splits[4 * blockIdx.y + 1] = start[63 - mid_max]; splits[4 * blockIdx.y + 2] = start[63 - 8];
-      splits[4 * blockIdx.y + 3] = (uint32_t)nblk;
-    }
-  }
-  __syncthreads();
-  // this slice's range inside every count's run
-  if (threadIdx.x < 64) { const unsigned mine = cnt[threadIdx.x]; start[threadIdx.x] += mine ? atomicAdd(&gcur[(size_t)blockIdx.y * 64 + threadIdx.x], mine) : 0u; }
-  __syncthreads();
-  for (long long b = b0 + threadIdx.x; b < b1; b += blockDim.x) {
-    const uint4 q = reinterpret_cast<const uint4 *>(r)[b];        // {norm, raw_dc | nz << 16, mask lo, mask hi}
-    const int nz = (int)((q.y >> 16) & 0xFF);
-    const unsigned pos = atomicAdd(&start[63 - min(nz, 63)], 1u);
-    reinterpret_cast<uint4 *>(p)[pos] = make_uint4(q.x, (unsigned)b, q.z, q.w);
-  }
-}
-static void launch_sort2(const Geom &g, const DcRec *rec, const RecLayout &rl, SRec *srec, uint32_t *splits, unsigned *scratch /* [2][n*nc][64] */, int mid_max, int n, cudaStream_t s)
-{
-  long long mb = 0;
-  for (int ci = 0; ci < g.nc; ci++) mb = max(mb, (long long)g.c[ci].wib * g.c[ci].hib);
-  const size_t words = (size_t)n * g.nc * 64;
-  cudaMemsetAsync(scratch, 0, 2 * words * sizeof(unsigned), s);
-  dim3 grid((unsigned)((mb + SORT_SLICE - 1) / SORT_SLICE), n * g.nc);
-  k_sort_count<<<grid, 256, 0, s>>>(g, rec, rl, scratch); LAUNCHED();
-  k_sort_scatter<<<grid, 256, 0, s>>>(g, rec, rl, srec, splits, scratch, scratch + words, mid_max); LAUNCHED();
-}
 
 // exact int -> float for 0 <= v < 2^23 without the conversion unit
 __device__ __forceinline__ float u2f_exact(unsigned v) { return __uint_as_float(0x4B000000u | v) - 8388608.0f; }
 
 // =====================================================================
 // AC trellis (third generation; the first two unrolled the entry x predecessor loops over register-resident lists and
-// are in the history): rolled loops over shared-memory lists, jcdctmgr.c:1121-1222.  One thread per block, blocks in
-// sorted order (k_sort_count / k_sort_scatter), one kernel
-// instantiation per count class; the class only sizes the per-thread lists.
+// are in the history): rolled loops over shared-memory lists, jcdctmgr.c:1121-1222.  One thread per block.  The trellis loops of a warp run
+// as long as the largest plain-quantized non-zero count among its 32 blocks, so the blocks are grouped by that count:
+//  * k_trellis_ac3<15> (the tile kernel) takes a tile of T3_TILE consecutive blocks of one (image, component), counting-
+//    sorts each tile in shared memory by non-zero count, decreasing, runs the blocks with at most 15 entries 128 at a
+//    time and appends the others to the big-class lists of their (image, component) in the tile's sorted order: blocks
+//    with more than 32 entries from the front of the component's range of the list buffer, 16..32 from its back;
+//  * k_trellis_ac3<32> and <64> then run those lists.
+// The class only sizes the per-thread lists.
 //  * phase 1 walks the 63 raw coefficients once (packed fp32x2 conversion / squaring / weighting, scalar prefix chain
 //    in the reference's order) and PUSHES an entry {A[p-1], p | raw << 16} for every position p whose plain-quantized
 //    value is non-zero -- nothing else of the prefix is kept;
@@ -2183,14 +2120,16 @@ __device__ __forceinline__ float u2f_exact(unsigned v) { return __uint_as_float(
 //    5-8 thousand and stalled on instruction fetch), registers ~50, shared memory 12 bytes per list slot and thread.
 // =====================================================================
 #define T3_THREADS 128
-// resident CTAs per SM the compiler must allow for the <= 8 entries class, and for the 9..15 entries class.  H100, cfg2:
-// 6 (80 registers, no spills) ran the AC stage in 9.84-9.87 ms against 10.06-10.13 at 8 (64 registers, 18 / 20 bytes of
-// spill stores / loads); an earlier GPU measured 12 slower than 8
-#ifndef T3_MINB_8
-#define T3_MINB_8 6
-#endif
+// resident CTAs per SM the compiler must allow for the tile kernel.  H100, cfg2 (then two small classes, <= 8 and
+// 9..15 entries): 6 (80 registers, no spills) ran the AC stage in 9.84-9.87 ms against 10.06-10.13 at 8 (64 registers,
+// 18 / 20 bytes of spill stores / loads); an earlier GPU measured 12 slower than 8
 #ifndef T3_MINB_15
 #define T3_MINB_15 6
+#endif
+// blocks per tile, one tile per CTA of the tile kernel (2-byte local indices: at most 65536).  H100, cfg2, AC stage:
+// 256 / 512 / 1024 blocks 10.19 / 9.57-9.59 / 9.11-9.23 ms; CTAs that ran 2-8 tiles each were slower (512: 9.74-11.54)
+#ifndef T3_TILE
+#define T3_TILE 1024
 #endif
 #ifndef T3_PRED_UNROLL
 #define T3_PRED_UNROLL 4       // predecessor loop: iterations in flight (their shared-memory loads are independent); 1 / 2 / 4: 2.56 / 2.49 / 2.44 ms per 64 4K images
@@ -2226,19 +2165,20 @@ __device__ __forceinline__ float t3_dist(const int cand, const int q, const int 
 }
 
 template <int MM>
-__global__ void __launch_bounds__(T3_THREADS, MM <= 8 ? T3_MINB_8 : MM <= 15 ? T3_MINB_15 : MM <= 32 ? 4 : 2)
+__global__ void __launch_bounds__(T3_THREADS, MM <= 15 ? T3_MINB_15 : MM <= 32 ? 4 : 2)
 k_trellis_ac3(Geom g, const TrellisConsts *__restrict__ tc, const DevHuff *__restrict__ tabs, size_t tabs_set_stride,
-              DcRec *__restrict__ rec, RecLayout rl, const SRec *__restrict__ srec, const uint32_t *__restrict__ splits, SymOut so)
+              DcRec *__restrict__ rec, RecLayout rl, SRec *__restrict__ big, unsigned *__restrict__ bigcnt, SymOut so, int tile_ci)
 {
-  const int ci = blockIdx.y % g.nc, img = blockIdx.y / g.nc;
+  static_assert(MM == 15 || MM == 32 || MM == 64, "k_trellis_ac3 classes");
+  // the tile kernel runs one component (tile_ci) per launch, blockIdx.y = image; the big classes all components,
+  // blockIdx.y = image * nc + component.  row: the (image, component)'s table set and list counters
+  const int ci = MM == 15 ? tile_ci : (int)(blockIdx.y % g.nc), img = MM == 15 ? (int)blockIdx.y : (int)(blockIdx.y / g.nc);
+  const int row = img * g.nc + ci;
   const CompGeom &c = g.c[ci];
-  long long lo, hi;
-  {
-    const uint4 sp = reinterpret_cast<const uint4 *>(splits)[blockIdx.y];
-    if (MM == 64) { lo = 0; hi = sp.x; } else if (MM == 32) { lo = sp.x; hi = sp.y; } else if (MM == 15) { lo = sp.y; hi = sp.z; } else { lo = sp.z; hi = sp.w; }
-  }
-  const int nchunks = (int)((hi - lo + T3_THREADS - 1) / T3_THREADS);
-  if ((int)blockIdx.x >= nchunks) return;
+  const long long nblk = (long long)c.wib * c.hib;
+  // tile kernel: tiles of the component; big classes: chunks of 128 list entries ([0] more than 32 entries, [1] 16..32)
+  const long long nwork = MM == 15 ? (nblk + T3_TILE - 1) / T3_TILE : (bigcnt[2 * row + (MM == 64 ? 0 : 1)] + T3_THREADS - 1) / T3_THREADS;
+  if ((long long)blockIdx.x >= nwork) return;
   extern __shared__ __align__(16) unsigned char t3_dyn[];
   T3Smem<MM> &L = *reinterpret_cast<T3Smem<MM> *>(t3_dyn);
   // rate[k][run] (:1163-1175), +inf where the reference skips.  Lanes past their block's last entry run the loops on
@@ -2254,7 +2194,7 @@ k_trellis_ac3(Geom g, const TrellisConsts *__restrict__ tc, const DevHuff *__res
   for (int i = tid; i < 164; i += T3_THREADS) shist[i] = 0;
   uint8_t *acsi = reinterpret_cast<uint8_t *>(t3_dyn);        // table build only
   {
-    const DevHuff *ac = reinterpret_cast<const DevHuff *>(reinterpret_cast<const char *>(tabs) + (size_t)blockIdx.y * tabs_set_stride) + (4 + c.ac_tbl);
+    const DevHuff *ac = reinterpret_cast<const DevHuff *>(reinterpret_cast<const char *>(tabs) + (size_t)row * tabs_set_stride) + (4 + c.ac_tbl);
     for (int i = tid; i < 256; i += T3_THREADS) acsi[i] = ac->size[i];
     const TrellisConsts *tq = qset_of(tc, g, img);             // the image's table set (the other fields are the batch's)
     if (tid < 64) {
@@ -2282,17 +2222,16 @@ k_trellis_ac3(Geom g, const TrellisConsts *__restrict__ tc, const DevHuff *__res
   const char *srate_b = reinterpret_cast<const char *>(srate);
   const float INF = __int_as_float(0x7F800000);
 
-#pragma unroll 1
-  for (int chunk = blockIdx.x; chunk < nchunks; chunk += gridDim.x) {
-    const long long tix = lo + (long long)chunk * T3_THREADS + tid;
-    const bool live = tix < hi;                                // whole warps stay in step (warp reductions below); dead lanes do no memory traffic
-    SRec sr; sr.norm = 0.f; sr.lin = 0; sr.nzmask = 0;
-    if (live) sr = srec[rbase + tix];
-    const unsigned lin = sr.lin;
+  // one block per lane: its record's norm and non-zero mask, its index inside the component.  Whole warps call it
+  // together (warp reductions below); dead lanes do no memory traffic.
+  auto run_block = [&](const bool live, const float rnorm, const unsigned lin, const unsigned long long nzmask) {
     const int by = lin / c.wib, bx = lin - by * c.wib;
     const size_t blk = ((size_t)img * c.hpad + by) * c.wpad + bx;
     const int16_t *raw16 = c.raw + blk * 64;
     int16_t *o16 = c.coef + blk * 64;
+    const unsigned mlo = (unsigned)nzmask, mhi = (unsigned)(nzmask >> 32);
+    const int m = __popc(mlo) + __popc(mhi);
+    const int mmax = __reduce_max_sync(0xffffffffu, m);
     uint4 rv[8];
 #pragma unroll
     for (int v = 0; v < 8; v++) rv[v] = make_uint4(0, 0, 0, 0);
@@ -2302,23 +2241,23 @@ k_trellis_ac3(Geom g, const TrellisConsts *__restrict__ tc, const DevHuff *__res
     unsigned dc_q = 0;
     const bool want_dc = !so.sym || so.keep_coef || so.dcq_ac;
     if (live) {
-      const uint4 *r4 = reinterpret_cast<const uint4 *>(raw16);
+      // (a warp whose 32 blocks have no entry at all -- the tail of a tile's sorted order -- needs neither the raw block,
+      // nor the prefix, nor the search)
+      if (mmax != 0) {
+        const uint4 *r4 = reinterpret_cast<const uint4 *>(raw16);
 #pragma unroll
-      for (int v = 0; v < 8; v++) rv[v] = r4[v];
+        for (int v = 0; v < 8; v++) rv[v] = r4[v];
+      }
       if (want_dc) dc_q = (unsigned)(unsigned short)o16[0];
     }
     // (the record keeps the norm: the DC trellis derives lambda_dc from it, dc_lambda)
     float lambda;
     {
-      const float norm = (float)((double)sr.norm / 63.0);      // :1026-1035
+      const float norm = (float)((double)rnorm / 63.0);        // :1026-1035
       if (use_norm) lambda = (float)(p1 / (p2 + (double)norm)); else lambda = lambda_const;
     }
     // phase 1: accumulated zero distortion, zigzag order, serial fp32 (:1134); entries pushed where the mask says so
-    const unsigned mlo = (unsigned)sr.nzmask, mhi = (unsigned)(sr.nzmask >> 32);
-    const int m = __popc(mlo) + __popc(mhi);
-    const int mmax = __reduce_max_sync(0xffffffffu, m);
     float azd = 0.0f;
-    // (a warp whose 32 blocks have no entry at all -- the tail of the sorted order -- needs neither the prefix nor the search)
     if (mmax != 0) {
       uint2 *push = myrec;
       const float bias = -8421376.0f;   // -(2^23 + 2^15): undoes the exponent trick and the +32768 offset
@@ -2482,6 +2421,78 @@ k_trellis_ac3(Geom g, const TrellisConsts *__restrict__ tc, const DevHuff *__res
         if (so.keep_coef || ns > SYMREC_SLOTS) write_block(last0);
       }
     }
+  };
+
+  if constexpr (MM == 15) {
+    // per tile: a counting sort by non-zero count (key 63 - nz, so decreasing) of 2-byte local indices
+    __shared__ unsigned short sidx[T3_TILE];
+    __shared__ unsigned scnt[64];
+    __shared__ unsigned sbig[4];            // blocks with more than 32 entries, with 16 or more, their offsets in the two lists
+    constexpr int PER = T3_TILE / T3_THREADS;
+    static_assert(PER * T3_THREADS == T3_TILE && T3_TILE <= 65536, "T3_TILE");
+    const DcRec *crec = rec + rbase;
+    const uint4 *crec4 = reinterpret_cast<const uint4 *>(crec);         // {norm, raw_dc | nz << 16, mask lo, mask hi}
+    uint4 *cbig = reinterpret_cast<uint4 *>(big + rbase);
+    {
+      const long long t0 = (long long)blockIdx.x * T3_TILE;
+      const int tn = (int)min((long long)T3_TILE, nblk - t0);
+      if (tid < 64) scnt[tid] = 0;
+      __syncthreads();
+      int key[PER];
+#pragma unroll
+      for (int k = 0; k < PER; k++) {
+        const int j = tid + k * T3_THREADS;
+        key[k] = j < tn ? 63 - min((int)crec[t0 + j].nz, 63) : -1;
+        if (key[k] >= 0) atomicAdd(&scnt[key[k]], 1u);
+      }
+      __syncthreads();
+      if (tid < 32) {
+        // exclusive prefix over the 64 counts, two per lane; the class boundaries sit at keys 31 (nz 32) and 48 (nz 15)
+        const unsigned a = scnt[2 * tid], b = scnt[2 * tid + 1];
+        unsigned incl = a + b;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) { const unsigned v = __shfl_up_sync(0xffffffffu, incl, o); if (tid >= o) incl += v; }
+        const unsigned ex = incl - a - b;
+        scnt[2 * tid] = ex; scnt[2 * tid + 1] = ex + a;
+        const unsigned n64 = __shfl_sync(0xffffffffu, ex + a, 15), nbig = __shfl_sync(0xffffffffu, ex, 24);
+        if (tid == 0) {
+          sbig[0] = n64; sbig[1] = nbig;
+          sbig[2] = n64 ? atomicAdd(&bigcnt[2 * row], n64) : 0u;
+          sbig[3] = nbig > n64 ? atomicAdd(&bigcnt[2 * row + 1], nbig - n64) : 0u;
+        }
+      }
+      __syncthreads();
+#pragma unroll
+      for (int k = 0; k < PER; k++)
+        if (key[k] >= 0) sidx[atomicAdd(&scnt[key[k]], 1u)] = (unsigned short)(tid + k * T3_THREADS);
+      __syncthreads();
+      const int n64 = (int)sbig[0], nbig = (int)sbig[1];
+      const long long o64 = sbig[2], o32 = sbig[3];
+      for (int j = tid; j < nbig; j += T3_THREADS) {
+        const int l = sidx[j];
+        const uint4 q = crec4[t0 + l];
+        cbig[j < n64 ? o64 + j : nblk - 1 - (o32 + (j - n64))] = make_uint4(q.x, (unsigned)(t0 + l), q.z, q.w);
+      }
+#pragma unroll 1
+      for (int r = nbig; r < tn; r += T3_THREADS) {
+        const int j = r + tid;
+        const bool live = j < tn;
+        unsigned lin = 0; uint4 q = make_uint4(0, 0, 0, 0);
+        if (live) { lin = (unsigned)(t0 + sidx[j]); q = crec4[lin]; }
+        run_block(live, __uint_as_float(q.x), lin, (unsigned long long)q.z | (unsigned long long)q.w << 32);
+      }
+    }
+  } else {
+    const long long cnt = bigcnt[2 * row + (MM == 64 ? 0 : 1)];
+    const SRec *lst = big + rbase;
+#pragma unroll 1
+    for (long long chunk = blockIdx.x; chunk < nwork; chunk += gridDim.x) {
+      const long long tix = chunk * T3_THREADS + tid;
+      const bool live = tix < cnt;
+      SRec sr; sr.norm = 0.f; sr.lin = 0; sr.nzmask = 0;
+      if (live) sr = lst[MM == 64 ? tix : nblk - 1 - tix];
+      run_block(live, sr.norm, sr.lin, sr.nzmask);
+    }
   }
   if (so.hist) {
     __syncthreads();
@@ -2493,36 +2504,46 @@ k_trellis_ac3(Geom g, const TrellisConsts *__restrict__ tc, const DevHuff *__res
   }
 }
 
+// zeroes the list counters and, when the trellis counts the scan's AC symbols, the histograms it adds them to (one
+// launch instead of two memset nodes)
+__global__ void __launch_bounds__(256) k_trellis_ac3_reset(uint32_t *__restrict__ bigcnt, int nbig, uint32_t *__restrict__ hist, int nhist)
+{
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < nbig + nhist; i += gridDim.x * blockDim.x) {
+    if (i < nbig) bigcnt[i] = 0u; else hist[i - nbig] = 0u;
+  }
+}
 template <int MM>
 static void launch_t3(dim3 grid, cudaStream_t s, const Geom &g, const TrellisConsts *tc, const DevHuff *tabs, size_t tabs_set_stride,
-                      DcRec *rec, const RecLayout &rl, const SRec *srec, const uint32_t *splits, const SymOut &so)
+                      DcRec *rec, const RecLayout &rl, SRec *big, unsigned *bigcnt, const SymOut &so, int tile_ci)
 {
   // per device: an application may hold encoders on several GPUs in one process, so the opt-in is not cached
   if (sizeof(T3Smem<MM>) + 8192 > 48 * 1024) cudaFuncSetAttribute(k_trellis_ac3<MM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(T3Smem<MM>));
-  k_trellis_ac3<MM><<<grid, T3_THREADS, sizeof(T3Smem<MM>), s>>>(g, tc, tabs, tabs_set_stride, rec, rl, srec, splits, so); LAUNCHED();
-}
-void launch_trellis_sort(const Geom &g, const DcRec *rec, const RecLayout &rl, void *srec, uint32_t *splits, int n, cudaStream_t s)
-{
-  // splits: 4 words per (image, component), followed by the sort's scratch counters (2 x 64 words each)
-  launch_sort2(g, rec, rl, static_cast<SRec *>(srec), splits, splits + (size_t)n * g.nc * 4, 15, n, s);
+  k_trellis_ac3<MM><<<grid, T3_THREADS, sizeof(T3Smem<MM>), s>>>(g, tc, tabs, tabs_set_stride, rec, rl, big, bigcnt, so, tile_ci); LAUNCHED();
 }
 void launch_trellis_ac3(const Geom &g, const TrellisConsts *tc, const DevHuff *tabs, size_t tabs_set_stride,
-                        DcRec *rec, const RecLayout &rl, const void *srec, const uint32_t *splits, const SymOut &so, int n, int sms, cudaStream_t s)
+                        DcRec *rec, const RecLayout &rl, void *big, uint32_t *bigcnt, const SymOut &so, int n, int sms, cudaStream_t s)
 {
+  const int ny = n * g.nc;
+  SRec *bl = static_cast<SRec *>(big);
+  {
+    const int nbig = ny * 2, nhist = so.hist ? n * HIST_SLOTS * HIST_BINS : 0;
+    k_trellis_ac3_reset<<<(nbig + nhist + 255) / 256, 256, 0, s>>>(bigcnt, nbig, so.hist, nhist); LAUNCHED();
+  }
+  // the tile kernel once per component, so that each grid is exactly its component's tiles (a subsampled component
+  // has a quarter of the full-size one's at 4:2:0)
   long long mb = 0;
-  for (int ci = 0; ci < g.nc; ci++) mb = max(mb, (long long)g.c[ci].wib * g.c[ci].hib);
-  const unsigned full = (unsigned)((mb + T3_THREADS - 1) / T3_THREADS);
-  // CTAs loop over their class's chunks: enough of them per (image, component) to fill the device, few enough to amortise the tables
-  unsigned gx = (unsigned)max(1, min((int)full, (sms * 8 * 3 + n * g.nc - 1) / (n * g.nc)));
-  dim3 grid(gx, n * g.nc);
-  const SRec *sr = static_cast<const SRec *>(srec);
-  // largest blocks first: the classes touch disjoint blocks.  The two big-list classes hold 2 / 4 CTAs per SM (96 / 48 KB of
-  // lists): a full-size grid of CTAs that mostly find their class empty costs more there than the few chunks are worth,
-  // so they get 8 / 16 CTAs per (image, component), still one to two waves when the classes are full (high quality settings)
-  launch_t3<64>(dim3(min(gx, 8u), grid.y), s, g, tc, tabs, tabs_set_stride, rec, rl, sr, splits, so);
-  launch_t3<32>(dim3(min(gx, 16u), grid.y), s, g, tc, tabs, tabs_set_stride, rec, rl, sr, splits, so);
-  launch_t3<15>(grid, s, g, tc, tabs, tabs_set_stride, rec, rl, sr, splits, so);
-  launch_t3<8>(grid, s, g, tc, tabs, tabs_set_stride, rec, rl, sr, splits, so);
+  for (int ci = 0; ci < g.nc; ci++) {
+    const long long nb = (long long)g.c[ci].wib * g.c[ci].hib;
+    mb = max(mb, nb);
+    launch_t3<15>(dim3((unsigned)((nb + T3_TILE - 1) / T3_TILE), n), s, g, tc, tabs, tabs_set_stride, rec, rl, bl, bigcnt, so, ci);
+  }
+  // The big classes' CTAs loop over their chunks.  The two hold 2 / 4 CTAs per SM (96 / 48 KB of lists): a full-size grid of CTAs that mostly find their
+  // class empty costs more there than the few chunks are worth, so they get 8 / 16 CTAs per (image, component), still
+  // one to two waves when the classes are full (high quality settings)
+  const int full = (int)((mb + T3_THREADS - 1) / T3_THREADS);
+  const unsigned gx = (unsigned)max(1, min(full, (sms * 8 * 3 + ny - 1) / ny));
+  launch_t3<64>(dim3(min(gx, 8u), ny), s, g, tc, tabs, tabs_set_stride, rec, rl, bl, bigcnt, so, -1);
+  launch_t3<32>(dim3(min(gx, 16u), ny), s, g, tc, tabs, tabs_set_stride, rec, rl, bl, bigcnt, so, -1);
 }
 
 // =====================================================================

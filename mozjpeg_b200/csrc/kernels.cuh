@@ -169,13 +169,13 @@ void launch_gather_comp_dc(const Geom &g, const RestartSpec &rs, const int16_t *
 void launch_gather_seq(const Geom &g, const ScanDesc &sd, const uint8_t *sym, const int16_t *dcq, const RecLayout &rl, uint32_t *hist, uint32_t *status, int n, cudaStream_t s);
 void launch_seed_hist(uint32_t *hist, int slot, int n, cudaStream_t s);
 void launch_gen_tables(const uint32_t *hist, DevHuff *tabs, size_t tabs_set_stride, const SlotMasks &masks, int nsets, cudaStream_t s);
-// AC trellis of the default option set: launch_trellis_sort sorts the side records by non-zero count (srec: 16 bytes
-// per real block; splits: 4 class boundaries per (image, component) followed by 128 words of sorting counters each),
-// then launch_trellis_ac3 runs one class-specific kernel per count class.  The records keep the forward kernel's norm
-// (the DC trellis behind it derives lambda_dc: launch_trellis_dc with lambda_from_norm)
-void launch_trellis_sort(const Geom &g, const DcRec *rec, const RecLayout &rl, void *srec, uint32_t *splits, int n, cudaStream_t s);
+// AC trellis of the default option set: a tile kernel sorts tiles of consecutive blocks by non-zero count in shared
+// memory and runs the blocks with at most 15 entries; the blocks with more go to two lists per (image, component),
+// which two class-specific kernels run (big: 16 bytes per real block, indexed like the side records; bigcnt: 2 list
+// lengths per (image, component); both bigcnt and so.hist, n images' worth, are zeroed here).  The records keep the forward kernel's norm (the DC trellis behind it
+// derives lambda_dc: launch_trellis_dc with lambda_from_norm)
 void launch_trellis_ac3(const Geom &g, const TrellisConsts *tc, const DevHuff *tabs, size_t tabs_set_stride,
-                        DcRec *rec, const RecLayout &rl, const void *srec, const uint32_t *splits, const SymOut &so, int n, int sms, cudaStream_t s);
+                        DcRec *rec, const RecLayout &rl, void *big, uint32_t *bigcnt, const SymOut &so, int n, int sms, cudaStream_t s);
 // use_scans_in_trellis: quantize_trellis restricted to the zigzag band [Ss, Se]
 void launch_trellis_ac_band(const Geom &g, const TrellisConsts *tc, const DevHuff *tabs, size_t tabs_set_stride,
                             DcRec *rec, const RecLayout &rl, int Ss, int Se, const uint16_t *qimg, float4 *eo, int n, cudaStream_t s);
