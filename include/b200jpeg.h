@@ -498,15 +498,23 @@ int  b200jpeg_decompress_output(const b200jpeg_source_info *src, int *width, int
  *     jidctred.c's IDCTs and the other sizes jidctint.c's scaled IDCTs, whatever the method.
  *   do_fancy_upsampling: 0 replicates chroma (and the merged upsampler, which gives the same pixels).
  *   out_color_space: -1 for what default_decompress_parms picks; else GRAYSCALE, RGB, EXT_*, or YCbCr from a YCbCr
- *     file.  Pairs the reference refuses are B200JPEG_ERR_PARAM "Unsupported color conversion request"; CMYK, YCCK
- *     and B200JPEG_CS_RGB565 output are B200JPEG_ERR_UNSUPPORTED.
+ *     file.  Pairs the reference refuses are B200JPEG_ERR_PARAM "Unsupported color conversion request"; CMYK and YCCK
+ *     output without cmyk, and B200JPEG_CS_RGB565 output, are B200JPEG_ERR_UNSUPPORTED.
  * The default options give b200jpeg_decompress_batch's and b200jpeg_recompress_batch's route and bytes.
  */
 #define B200JPEG_CS_RGB565 16
 /*   all_scales: 0 (the default) refuses the block sizes above; 1 decodes every block size jpeg_core_output_dimensions
  *     picks (1 .. 16, every scale_num / scale_denom) with jidctint.c's scaled IDCTs, sample for sample.  A C
- *     initialiser of the first five fields leaves it 0. */
-typedef struct { int scale_num, scale_denom, dct_method, do_fancy_upsampling, out_color_space, all_scales; } b200jpeg_decompress_options;
+ *     initialiser of the first five fields leaves it 0.
+ *   cmyk: 0 (the default) refuses 4-component sources and CMYK / YCCK output as described above.  1 decodes 8-bit
+ *     4-component files (CMYK: Adobe transform 0 or no Adobe marker; YCCK: transform 2) whose every sampling factor is
+ *     1 or 2, to 4 bytes a pixel as jinit_color_deconverter does: CMYK output (the default) is ycck_cmyk_convert of a
+ *     YCCK file and null_convert of a CMYK file, YCCK output of a YCCK file is null_convert.  The other pairs with a
+ *     4-component side (a CMYK / YCCK file to GRAYSCALE, RGB or EXT_*, a CMYK file to YCCK, a 1- or 3-component file to
+ *     CMYK or YCCK) are B200JPEG_ERR_PARAM "Unsupported color conversion request".  A batch, rendition or mixed call
+ *     takes 4-component files only when every rung sets it; the YUV routes ignore it.  A C initialiser of the first
+ *     six fields leaves it 0. */
+typedef struct { int scale_num, scale_denom, dct_method, do_fancy_upsampling, out_color_space, all_scales, cmyk; } b200jpeg_decompress_options;
 b200jpeg_decompress_options b200jpeg_default_decompress_options(void);
 /* jpeg_calc_output_dimensions + out_color_components for these options: B200JPEG_ERR_* as the batch would refuse. */
 int  b200jpeg_decompress_output_opts(const b200jpeg_source_info *src, const b200jpeg_decompress_options *opts,

@@ -19,7 +19,7 @@ from .cjpeg import decompress_options, params_for_jpeg_input, params_from_switch
 _lib = A.load()          # raises ImportError with build instructions if missing
 
 # the keywords of decompress_options, which a rendition's option dict may use
-RENDITION_OPTIONS = ("scale", "dct", "fancy", "colorspace", "all_scales")
+RENDITION_OPTIONS = ("scale", "dct", "fancy", "colorspace", "all_scales", "cmyk")
 
 __all__ = ["Encoder", "Params", "params_from_switches", "read_ppm", "cjpeg", "tj3_params", "quality_tables", "yuv_plane_dims", "decompress_yuv_dims",
            "yuv_packed_layout", "B200JpegError"]
@@ -196,7 +196,9 @@ class Encoder:
     def decompress(self, files: Sequence[bytes], **opts) -> np.ndarray:
         """jpeg_read_scanlines for same-geometry sequential files, on the device: an (N, H, W, C) uint8 array, (N, H,
         W) for one output component.  Keyword options (decompress_options): scale=(num, denom), dct="int" | "fast" |
-        "float", fancy=True, colorspace=None, all_scales=False (True: every scale, not only 1/8 .. 1/1); without them a default decompress object (b200jpeg_decompress_batch)."""
+        "float", fancy=True, colorspace=None, all_scales=False (True: every scale, not only 1/8 .. 1/1), cmyk=False (True:
+        CMYK / YCCK files decode to (N, H, W, 4) CMYK, or YCCK with colorspace="ycck"); without them a default decompress
+        object (b200jpeg_decompress_batch)."""
         o = decompress_options(**opts) if opts else None
         w, h, _, nc = decompress_output(_parse_first(files), **opts)
         bufs, ptrs, sizes = self._files(files)
@@ -278,7 +280,7 @@ class Encoder:
 
     def decompress_renditions(self, files: Sequence[bytes], renditions: Sequence[dict]) -> List[np.ndarray]:
         """b200jpeg_decompress_renditions: the files decoded once and rendered with each option dict of ``renditions``
-        (decompress's keywords, all_scales included; {} is a default decompress object).  Returns per rendition what decompress(files,
+        (decompress's keywords, all_scales and cmyk included; {} is a default decompress object).  Returns per rendition what decompress(files,
         **renditions[r]) returns: an (N, H, W, C) uint8 array, (N, H, W) for one output component."""
         renditions = list(renditions)
         opts = self._rendition_options(renditions)
@@ -312,7 +314,7 @@ class Encoder:
     def recompress_renditions(self, files: Sequence[bytes], renditions) -> List[List[bytes]]:
         """b200jpeg_recompress_renditions: the files decoded once, and per rendition (params, option dict) recompressed
         as recompress(params, files, **options) does (params_for_jpeg_input(switches, file, **options) builds params);
-        the option dicts take decompress's keywords, all_scales included.  Returns out[r][i], the file of rendition r
+        the option dicts take decompress's keywords, all_scales and cmyk included.  Returns out[r][i], the file of rendition r
         for source i."""
         rungs = list(renditions)
         for r, rung in enumerate(rungs):
@@ -347,7 +349,7 @@ class Encoder:
     def decompress_mixed(self, files: Sequence[bytes], renditions: Optional[Sequence[dict]] = None) -> List[List[np.ndarray]]:
         """b200jpeg_decompress_mixed: files of any mix of sizes, sampling layouts, colour spaces, gray and colour,
         sequential and progressive, decoded in one call and rendered with each option dict of ``renditions``
-        (decompress's keywords, all_scales included; None is one rung of a default decompress object).  Returns out[r][i], what
+        (decompress's keywords, all_scales and cmyk included; None is one rung of a default decompress object).  Returns out[r][i], what
         decompress([files[i]], **renditions[r])[0] returns: an (H, W, C) uint8 array, (H, W) for one output component."""
         renditions = [{}] if renditions is None else list(renditions)
         opts = self._rendition_options(renditions)
@@ -374,7 +376,7 @@ class Encoder:
     def recompress_mixed_params(self, files: Sequence[bytes], rungs) -> List[List[bytes]]:
         """b200jpeg_recompress_mixed with explicit parameter blocks: rungs[r] is (params, options dict), params a list of
         one Params per file (params_for_jpeg_input(switches, files[i], **options) builds them; options as decompress's
-        keywords, all_scales included).  Returns out[r][i], what
+        keywords, all_scales and cmyk included).  Returns out[r][i], what
         recompress(params[i], [files[i]], **options) returns for that file alone."""
         rungs = list(rungs)
         n = len(files)
@@ -392,7 +394,7 @@ class Encoder:
 
     def recompress_mixed(self, files: Sequence[bytes], rungs) -> List[List[bytes]]:
         """cjpeg with JPEG input over files of mixed geometry, several rungs in one call: rungs[r] is (cjpeg switches,
-        options dict, decompress's keywords with all_scales among them) and file i of rung r is encoded with
+        options dict, decompress's keywords with all_scales and cmyk among them) and file i of rung r is encoded with
         params_for_jpeg_input(switches, files[i], **options).  Returns out[r][i]."""
         rungs = list(rungs)
         for r, rung in enumerate(rungs):

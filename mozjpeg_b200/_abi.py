@@ -98,9 +98,9 @@ class SourceScan(C.Structure):
 class DecompressOptions(C.Structure):
     """b200jpeg_decompress_options: scale_num / scale_denom, dct_method (B200JPEG_DCT_*), do_fancy_upsampling and
     out_color_space (-1: the decompressor's default), all_scales (1: every block size 1 .. 16; 0, the default: 1, 2, 4
-    and 8 only)."""
+    and 8 only), cmyk (1: decode 4-component CMYK / YCCK files to 4 bytes a pixel; 0, the default: refuse them)."""
     _fields_ = [("scale_num", C.c_int), ("scale_denom", C.c_int), ("dct_method", C.c_int), ("do_fancy_upsampling", C.c_int),
-                ("out_color_space", C.c_int), ("all_scales", C.c_int)]
+                ("out_color_space", C.c_int), ("all_scales", C.c_int), ("cmyk", C.c_int)]
 
 
 class SourceInfo(C.Structure):

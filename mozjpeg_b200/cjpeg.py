@@ -339,7 +339,7 @@ def params_for_jpeg_input(switches: Sequence[str], jpeg: bytes, **opts) -> A.Par
     """cjpeg's cinfo at jpeg_start_compress for a JPEG input file: rdjpeg.c's start_input_jpeg takes the image size,
     in_color_space (the decompressor's out_color_space) and input_components from the source (data_precision is 8 for
     every source the device decodes), then jpeg_default_colorspace and the second switch pass run as for any input.
-    Keyword options (decompress_options: scale, dct, fancy, colorspace, all_scales) describe a rendition decoded with them, for
+    Keyword options (decompress_options: scale, dct, fancy, colorspace, all_scales, cmyk) describe a rendition decoded with them, for
     Encoder.recompress with the same options; without them the decompress defaults."""
     lib = A.load()
     info = A.SourceInfo()
@@ -359,10 +359,12 @@ COLOR_SPACES = {"gray": 1, "grayscale": 1, "rgb": 2, "ycbcr": 3, "cmyk": 4, "ycc
                 "xbgr": 10, "xrgb": 11, "rgba": 12, "bgra": 13, "abgr": 14, "argb": 15, "rgb565": 16}
 
 
-def decompress_options(scale=(1, 1), dct: str = "int", fancy: bool = True, colorspace=None, all_scales: bool = False) -> A.DecompressOptions:
+def decompress_options(scale=(1, 1), dct: str = "int", fancy: bool = True, colorspace=None, all_scales: bool = False,
+                       cmyk: bool = False) -> A.DecompressOptions:
     """b200jpeg_decompress_options from keywords: scale=(scale_num, scale_denom), dct "int" | "fast" | "float"
     (JDCT_ISLOW / IFAST / FLOAT), fancy (do_fancy_upsampling), colorspace None (the decompressor's default), a
-    B200JPEG_CS_* number or a name of COLOR_SPACES, all_scales (decode every scale, not only 1/8, 1/4, 1/2 and 1/1)."""
+    B200JPEG_CS_* number or a name of COLOR_SPACES, all_scales (decode every scale, not only 1/8, 1/4, 1/2 and 1/1),
+    cmyk (decode 4-component CMYK / YCCK files, to 4 bytes a pixel; without it they are refused)."""
     if dct not in DCT_METHODS:
         raise ValueError(f"dct must be one of {sorted(DCT_METHODS)}, not {dct!r}")
     if colorspace is None:
@@ -374,7 +376,7 @@ def decompress_options(scale=(1, 1), dct: str = "int", fancy: bool = True, color
     else:
         cs = int(colorspace)
     num, denom = scale
-    return A.DecompressOptions(int(num), int(denom), DCT_METHODS[dct], int(bool(fancy)), cs, int(bool(all_scales)))
+    return A.DecompressOptions(int(num), int(denom), DCT_METHODS[dct], int(bool(fancy)), cs, int(bool(all_scales)), int(bool(cmyk)))
 
 
 def read_pnm(data: bytes):
@@ -430,7 +432,8 @@ def main(argv: Sequence[str] = None) -> int:
     """``python -m mozjpeg_b200.cjpeg [switches] [-outfile name] file.ppm [more.ppm ...]`` - cjpeg's command line on
     the device path.  Several input files of one size are encoded as one batch (outputs: <input>.jpg).  Input files
     that start with 0xFF are JPEG files (select_file_type, cjpeg.c:145-148): they are decoded and recompressed on the
-    device, and must then all be JPEG files of one geometry."""
+    device, and must then all be JPEG files of one geometry; CMYK and YCCK files are taken too (cmyk=True), as the
+    reference's cjpeg reads them."""
     import sys
     import numpy as np
     from . import Encoder
@@ -463,7 +466,7 @@ def main(argv: Sequence[str] = None) -> int:
         enc = Encoder(0)
         enc.set_progressive_decode(True)      # the reference's cjpeg reads progressive JPEG input too
         try:
-            out = enc.recompress(params_for_jpeg_input(switches, data[0]), data)
+            out = enc.recompress(params_for_jpeg_input(switches, data[0], cmyk=True), data, cmyk=True)
         finally:
             enc.close()
         for f, jpg in zip(files, out):

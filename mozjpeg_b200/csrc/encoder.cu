@@ -1810,13 +1810,17 @@ static int check_tables_progression(const b200jpeg_source_info &s, int i)
 
 // A source b200jpeg_decompress_batch takes: sequential (or, with progressive decode on, progressive without the block
 // smoothing a default decompress object would apply), 8-bit, gray or three components with component 0 at the
-// largest factors (1 or 2 each way) over 1x1 chroma; everything else is refused, never approximated.
-static int check_decompress_source(const b200jpeg_source_info &s, int i, bool progressive)
+// largest factors (1 or 2 each way) over 1x1 chroma, or, when every rung of the call sets cmyk, four components whose
+// every sampling factor is 1 or 2 (a factor of 3 or 4 keeps the 4-component refusal); everything else is refused,
+// never approximated.
+static int check_decompress_source(const b200jpeg_source_info &s, int i, bool progressive, bool cmyk)
 {
+  bool four_ok = cmyk && s.num_components == 4;
+  for (int c = 0; four_ok && c < 4; c++) four_ok = s.h_samp_factor[c] <= 2 && s.v_samp_factor[c] <= 2;
   const char *why = nullptr;
   if (s.sof == 0xC2 && !progressive) why = "progressive (SOF2) source: only sequential files are decoded to pixels";
   else if (s.data_precision != 8) why = "12-bit source: only 8-bit files are decoded to pixels";
-  else if (s.num_components != 1 && s.num_components != 3) why = "4-component (CMYK / YCCK) source: only gray and 3-component files are decoded to pixels";
+  else if (s.num_components != 1 && s.num_components != 3 && !four_ok) why = "4-component (CMYK / YCCK) source: only gray and 3-component files are decoded to pixels";
   else if (s.num_components == 3 && (s.h_samp_factor[0] > 2 || s.v_samp_factor[0] > 2 || s.h_samp_factor[1] != 1 || s.v_samp_factor[1] != 1 ||
                                      s.h_samp_factor[2] != 1 || s.v_samp_factor[2] != 1))
     why = "sampling layout other than 4:4:4, 4:2:2, 4:4:0 or 4:2:0 (the reference's int_upsample and 2:1 non-fancy cases are not on the device)";
@@ -1911,6 +1915,34 @@ static int idct_upsample_default(b200jpeg_encoder *e, int nk, uint8_t *pix, size
   return B200JPEG_OK;
 }
 
+// component c of plan p in an upsampling descriptor: its sample plane (pitch bytes a row, images stride apart) and
+// the plan's size, replication and filter for it
+static void ups_component(UpsOpt4 &u, const DecPlan &p, int c, const uint8_t *plane, int pitch, long long stride)
+{
+  u.plane[c] = plane; u.pitch[c] = pitch; u.stride[c] = stride;
+  u.dw[c] = p.dw[c]; u.dh[c] = p.dh[c]; u.hr[c] = p.hr[c]; u.vr[c] = p.vr[c]; u.fancy[c] = p.fancy[c];
+}
+
+static void ups_conversion(UpsOpt4 &u, const DecPlan &p)
+{
+  u.nin = p.nin; u.conv = p.conv; u.ps = p.ps;
+  for (int k = 0; k < 4; k++) u.off[k] = p.off[k];
+}
+
+// the first three components of a descriptor, for the 1- and 3-component kernels (k_upsample_opts<3>, _ragged<3>)
+static UpsOpt ups_narrow(const UpsOpt4 &a)
+{
+  UpsOpt o;
+  memset(&o, 0, sizeof o);
+  for (int c = 0; c < 3; c++) {
+    o.plane[c] = a.plane[c]; o.pitch[c] = a.pitch[c]; o.stride[c] = a.stride[c];
+    o.dw[c] = a.dw[c]; o.dh[c] = a.dh[c]; o.hr[c] = a.hr[c]; o.vr[c] = a.vr[c]; o.fancy[c] = a.fancy[c];
+  }
+  o.nin = a.nin; o.conv = a.conv; o.ps = a.ps;
+  for (int k = 0; k < 4; k++) o.off[k] = a.off[k];
+  return o;
+}
+
 // the IDCT and upsampling / colour conversion stages of one decoded chunk for a non-default plan: each needed
 // component through the IDCT of its DCT_scaled_size into a plane of wib * size samples a row, then k_upsample_opts
 // into the pixels.  qt: the chunk's tables as upload_chunk_quant staged them; mt: host staging for the multipliers.
@@ -1930,7 +1962,7 @@ static int idct_upsample_opts(b200jpeg_encoder *e, const DecPlan &plan, int nk, 
     CU(cudaMemcpyAsync(e->d_dec_mtab.p, mt.data(), mt.size() * 4, cudaMemcpyHostToDevice, s));
   }
   CU(cudaEventRecord(ev[0], s));
-  UpsOpt u;
+  UpsOpt4 u;
   memset(&u, 0, sizeof u);
   for (int c = 0; c < nc; c++) {
     if (!plan.needed[c]) continue;
@@ -1939,15 +1971,12 @@ static int idct_upsample_opts(b200jpeg_encoder *e, const DecPlan &plan, int nk, 
     const bool by_method = sz == 8 && plan.method != B200JPEG_DCT_ISLOW;
     const void *tab = by_method ? static_cast<const void *>(e->d_dec_mtab.as<uint32_t>() + c * 64) : static_cast<const void *>(e->d_dec_quant.as<uint16_t>() + c * 64);
     launch_idct_opts(sz, plan.method, reinterpret_cast<const int16_t *>(e->d_dec_planes.as<uint8_t>() + e->dec_plane_off[c]), tab, nc * 64, dst, b.wib[c], b.hib[c], nk, s);
-    if (c < 3) {
-      u.plane[c] = dst; u.pitch[c] = b.wib[c] * sz; u.stride[c] = (long long)b.hib[c] * sz * u.pitch[c];
-      u.dw[c] = plan.dw[c]; u.dh[c] = plan.dh[c]; u.hr[c] = plan.hr[c]; u.vr[c] = plan.vr[c]; u.fancy[c] = plan.fancy[c];
-    }
+    ups_component(u, plan, c, dst, b.wib[c] * sz, (long long)b.hib[c] * sz * b.wib[c] * sz);
   }
   CU(cudaEventRecord(ev[1], s));
-  u.nin = plan.nin; u.conv = plan.conv; u.ps = plan.ps;
-  for (int k = 0; k < 4; k++) u.off[k] = plan.off[k];
-  launch_upsample_opts(u, pix, row_pitch, image_stride, plan.out_w, plan.out_h, nk, s);
+  ups_conversion(u, plan);
+  if (plan.nin == 4) launch_upsample_opts(u, pix, row_pitch, image_stride, plan.out_w, plan.out_h, nk, s);
+  else launch_upsample_opts(ups_narrow(u), pix, row_pitch, image_stride, plan.out_w, plan.out_h, nk, s);
   CU(cudaEventRecord(ev[2], s));
   CU(cudaGetLastError());
   return B200JPEG_OK;
@@ -1955,12 +1984,14 @@ static int idct_upsample_opts(b200jpeg_encoder *e, const DecPlan &plan, int nk, 
 
 // Pixels for one DecPlan from the decoded chunk (e->dec, e->d_dec_planes, its tables in e->d_dec_quant) into (pix,
 // row_pitch, image_stride): the default plan through launch_idct_islow and launch_upsample_color, every other plan
-// through idct_upsample_opts.  It only enqueues on e->stream, with events ev[0..2] around the IDCT and around the
-// upsampling / colour conversion; the caller reserves (reserve_pixel_stage), synchronises and adds the times.
+// through idct_upsample_opts.  A 4-component plan takes idct_upsample_opts whatever is_default says: the default
+// route's k_upsample_color has no 4-component instance.  It only enqueues on e->stream, with events ev[0..2] around
+// the IDCT and around the upsampling / colour conversion; the caller reserves (reserve_pixel_stage), synchronises and
+// adds the times.
 static int chunk_pixels(b200jpeg_encoder *e, const DecPlan &plan, int nk, uint8_t *pix, size_t row_pitch, size_t image_stride,
                         const std::vector<uint16_t> &qt, std::vector<uint32_t> &mt, const cudaEvent_t *ev)
 {
-  return plan.is_default ? idct_upsample_default(e, nk, pix, row_pitch, image_stride, ev)
+  return plan.is_default && plan.nin != 4 ? idct_upsample_default(e, nk, pix, row_pitch, image_stride, ev)
                          : idct_upsample_opts(e, plan, nk, pix, row_pitch, image_stride, qt, mt, ev);
 }
 
@@ -2218,6 +2249,13 @@ struct RungSets {
   std::vector<std::vector<DecPlan>> plan;              // [set][image]
 };
 
+// what a one-geometry chunk's single conversion needs its images to share beyond the geometry: RGB-coded or not for
+// three components, YCCK or CMYK for four
+static int conversion_class(const b200jpeg_source_info &s)
+{
+  return (s.num_components == 3 && s.jpeg_color_space == B200JPEG_CS_RGB) || (s.num_components == 4 && s.jpeg_color_space == B200JPEG_CS_YCCK);
+}
+
 // The checks of a call's sources and rung options: each file parsed into one scratch header and checked as
 // b200jpeg_decompress_batch takes it, then each distinct option set planned for it.  A refused option set is reported
 // after every source passed, for the first image it fails on, naming the image only when that is not image 0.
@@ -2230,11 +2268,14 @@ static int plan_rungs(const b200jpeg_encoder *e, const Call &c, RungSets &m)
     for (; k < (int)m.first.size(); k++) {
       const b200jpeg_decompress_options &f = c.opts[m.first[k]];
       if (f.scale_num == o.scale_num && f.scale_denom == o.scale_denom && f.dct_method == o.dct_method &&
-          f.do_fancy_upsampling == o.do_fancy_upsampling && f.out_color_space == o.out_color_space && f.all_scales == o.all_scales) break;
+          f.do_fancy_upsampling == o.do_fancy_upsampling && f.out_color_space == o.out_color_space && f.all_scales == o.all_scales &&
+          f.cmyk == o.cmyk) break;
     }
     if (k == (int)m.first.size()) m.first.push_back(r);
     m.set.push_back(k);
   }
+  bool cmyk = true;                                    // 4-component sources: only when every rung decodes them
+  for (int r = 0; r < c.R; r++) cmyk &= c.opts[r].cmyk != 0;
   const int K = (int)m.first.size();
   m.plan.assign(K, std::vector<DecPlan>(c.n));
   m.weight.assign(c.n, 0);
@@ -2246,10 +2287,10 @@ static int plan_rungs(const b200jpeg_encoder *e, const Call &c, RungSets &m)
     if (!c.files[i]) { set_error("image %d: no file", i); return B200JPEG_ERR_PARAM; }
     int rc = b200jpeg_parse_source(c.files[i], c.sizes[i], &s);
     if (rc) { std::string msg = b200jpeg_last_error(); set_error("image %d: %s", i, msg.c_str()); return rc; }
-    if ((rc = check_decompress_source(s, i, e->progressive_decode))) return rc;
-    // the geometry one-geometry calls compare: size, components, sampling factors, and RGB-coded or not
+    if ((rc = check_decompress_source(s, i, e->progressive_decode, cmyk))) return rc;
+    // the geometry one-geometry calls compare: size, components, sampling factors, and the conversion class
     const int nc = s.num_components;
-    std::array<int, 12> g{s.image_width, s.image_height, nc, nc == 3 && s.jpeg_color_space == B200JPEG_CS_RGB};
+    std::array<int, 12> g{s.image_width, s.image_height, nc, conversion_class(s)};
     int hmax = 1, vmax = 1;
     for (int ch = 0; ch < nc; ch++) {
       g[4 + 2 * ch] = s.h_samp_factor[ch]; g[5 + 2 * ch] = s.v_samp_factor[ch];
@@ -2284,7 +2325,8 @@ struct MixLaunch { int c, size; size_t desc, work; unsigned ncta; };
 struct MixStage {
   std::vector<uint8_t> meta;
   std::vector<MixLaunch> idct;
-  size_t ups_desc = 0, ups_work = 0; unsigned ups_cta = 0;
+  size_t ups_desc = 0, ups_work = 0; unsigned ups_cta = 0;         // 1- and 3-component images
+  size_t ups4_desc = 0, ups4_work = 0; unsigned ups4_cta = 0;      // 4-component images
   bool need_mt = false;
 };
 
@@ -2297,10 +2339,10 @@ template <class T> static size_t meta_put(std::vector<uint8_t> &m, const T *p, s
 }
 
 // the bytes of one set's sample planes in a chunk (images [i0, i0 + nk)); soff[i][c]: where image i's plane c starts
-static size_t mixed_sample_layout(const DecBatch &b, const std::vector<DecPlan> &plan, int i0, int nk, std::vector<std::array<size_t, 3>> &soff)
+static size_t mixed_sample_layout(const DecBatch &b, const std::vector<DecPlan> &plan, int i0, int nk, std::vector<std::array<size_t, 4>> &soff)
 {
   size_t total = 0;
-  soff.assign(nk, std::array<size_t, 3>{0, 0, 0});
+  soff.assign(nk, std::array<size_t, 4>{0, 0, 0, 0});
   for (int i = 0; i < nk; i++) {
     const DecGeom &g = b.geom[i]; const DecPlan &p = plan[i0 + i];
     for (int c = 0; c < g.nc; c++) {
@@ -2314,11 +2356,11 @@ static size_t mixed_sample_layout(const DecBatch &b, const std::vector<DecPlan> 
 static void stage_mixed(const b200jpeg_encoder *e, const std::vector<DecPlan> &plan, int i0, int nk, int qs, const MixedOut *out, uint8_t *samples, MixStage &st)
 {
   const DecBatch &b = e->dec;
-  std::vector<std::array<size_t, 3>> soff;
+  std::vector<std::array<size_t, 4>> soff;
   mixed_sample_layout(b, plan, i0, nk, soff);
   st = MixStage();
   std::vector<IdctImg> d; std::vector<uint32_t> w;
-  for (int c = 0; c < 3; c++)
+  for (int c = 0; c < 4; c++)
     for (int size = 1; size <= 16; size++) {
       d.clear(); w.clear();
       const int bpc = idct_blocks_per_cta(size);
@@ -2338,24 +2380,32 @@ static void stage_mixed(const b200jpeg_encoder *e, const std::vector<DecPlan> &p
       l.desc = meta_put(st.meta, d.data(), d.size()); l.work = meta_put(st.meta, w.data(), w.size());
       st.idct.push_back(l);
     }
-  std::vector<UpsImg> u; w.clear();
+  // the upsampling images, 4-component ones in a table of their own for k_upsample_ragged<4>
+  std::vector<UpsImg> u; std::vector<UpsImg4> u4; std::vector<uint32_t> w4; w.clear();
   for (int i = 0; i < nk; i++) {
     const DecGeom &g = b.geom[i]; const DecPlan &p = plan[i0 + i];
-    UpsImg im; memset(&im, 0, sizeof im);
-    for (int c = 0; c < 3 && c < g.nc; c++) {
-      if (!p.needed[c]) continue;
-      im.o.plane[c] = samples + soff[i][c]; im.o.pitch[c] = g.wib[c] * p.ssize[c]; im.o.stride[c] = 0;
-      im.o.dw[c] = p.dw[c]; im.o.dh[c] = p.dh[c]; im.o.hr[c] = p.hr[c]; im.o.vr[c] = p.vr[c]; im.o.fancy[c] = p.fancy[c];
-    }
-    im.o.nin = p.nin; im.o.conv = p.conv; im.o.ps = p.ps;
-    for (int k = 0; k < 4; k++) im.o.off[k] = p.off[k];
+    UpsImg4 im; memset(&im, 0, sizeof im);
+    for (int c = 0; c < g.nc; c++)
+      if (p.needed[c]) ups_component(im.o, p, c, samples + soff[i][c], g.wib[c] * p.ssize[c], 0);
+    ups_conversion(im.o, p);
     im.pix = out[i].pix; im.row_pitch = (long long)out[i].row_pitch; im.W = p.out_w; im.H = p.out_h;
-    im.gx = div_up(p.out_w, 64); im.cta0 = (int)w.size();
-    w.insert(w.end(), (size_t)im.gx * div_up(p.out_h, 4), (uint32_t)u.size());
-    u.push_back(im);
+    im.gx = div_up(p.out_w, 64);
+    if (p.nin == 4) {
+      im.cta0 = (int)w4.size();
+      w4.insert(w4.end(), (size_t)im.gx * div_up(p.out_h, 4), (uint32_t)u4.size());
+      u4.push_back(im);
+      continue;
+    }
+    UpsImg im3;
+    memset(&im3, 0, sizeof im3);
+    im3.o = ups_narrow(im.o); im3.pix = im.pix; im3.row_pitch = im.row_pitch; im3.W = im.W; im3.H = im.H; im3.gx = im.gx; im3.cta0 = (int)w.size();
+    w.insert(w.end(), (size_t)im3.gx * div_up(p.out_h, 4), (uint32_t)u.size());
+    u.push_back(im3);
   }
   st.ups_cta = (unsigned)w.size();
   st.ups_desc = meta_put(st.meta, u.data(), u.size()); st.ups_work = meta_put(st.meta, w.data(), w.size());
+  st.ups4_cta = (unsigned)w4.size();
+  st.ups4_desc = meta_put(st.meta, u4.data(), u4.size()); st.ups4_work = meta_put(st.meta, w4.data(), w4.size());
 }
 
 // whether images [i0, i0 + nk) of a set's outputs lie one image stride apart at one row pitch (stride: that stride)
@@ -2382,7 +2432,7 @@ static int mixed_files(b200jpeg_encoder *e, const Call &c, const RungSets &m, co
   const std::vector<int> start = mixed_chunks(e, m.weight);
   e->chunk = 0;
   std::vector<uint16_t> qt; std::vector<uint32_t> mt; std::vector<MixStage> st(K);
-  std::vector<std::array<size_t, 3>> soff;
+  std::vector<std::array<size_t, 4>> soff;
   cudaStream_t s = e->stream;
   for (size_t ch = 0; ch + 1 < start.size(); ch++) {
     const int i0 = start[ch], nk = start[ch + 1] - i0;
@@ -2397,8 +2447,7 @@ static int mixed_files(b200jpeg_encoder *e, const Call &c, const RungSets &m, co
     for (int i = 0; i < nk; i++) {
       const DecGeom &g = e->dec.geom[i];
       qs = std::max(qs, g.nc);
-      one &= g.W == g0.W && g.H == g0.H && g.nc == g0.nc &&
-             (e->dec.info[i].jpeg_color_space == B200JPEG_CS_RGB) == (e->dec.info[0].jpeg_color_space == B200JPEG_CS_RGB);
+      one &= g.W == g0.W && g.H == g0.H && g.nc == g0.nc && conversion_class(e->dec.info[i]) == conversion_class(e->dec.info[0]);
       for (int c = 0; c < g.nc; c++) one &= g.h[c] == g0.h[c] && g.v[c] == g0.v[c];
     }
     std::vector<size_t> stride(K, 0);
@@ -2414,8 +2463,8 @@ static int mixed_files(b200jpeg_encoder *e, const Call &c, const RungSets &m, co
       if (!uniform[k]) { stage_mixed(e, m.plan[k], i0, nk, qs, out[k].data() + i0, e->d_dec_samples.as<uint8_t>(), st[k]); meta = std::max(meta, st[k].meta.size()); }
     if ((rc = e->d_mix_meta.reserve(meta))) return rc;
     if ((rc = upload_chunk_quant(e, nk, qs, qt))) return rc;
-    const int16_t *coef[3];
-    for (int c = 0; c < 3; c++) coef[c] = reinterpret_cast<const int16_t *>(e->d_dec_planes.as<uint8_t>() + e->dec_plane_off[c]);
+    const int16_t *coef[4];
+    for (int c = 0; c < 4; c++) coef[c] = reinterpret_cast<const int16_t *>(e->d_dec_planes.as<uint8_t>() + e->dec_plane_off[c]);
     for (int k = 0; k < K; k++) {
       const MixStage &g = st[k];
       const int method = m.plan[k][i0].method;
@@ -2441,7 +2490,8 @@ static int mixed_files(b200jpeg_encoder *e, const Call &c, const RungSets &m, co
                            reinterpret_cast<const IdctImg *>(meta_d + l.desc), l.ncta, s);
       }
       CU(cudaEventRecord(ev[1], s));
-      launch_upsample_ragged(reinterpret_cast<const uint32_t *>(meta_d + g.ups_work), reinterpret_cast<const UpsImg *>(meta_d + g.ups_desc), g.ups_cta, s);
+      if (g.ups_cta) launch_upsample_ragged(reinterpret_cast<const uint32_t *>(meta_d + g.ups_work), reinterpret_cast<const UpsImg *>(meta_d + g.ups_desc), g.ups_cta, s);
+      if (g.ups4_cta) launch_upsample_ragged(reinterpret_cast<const uint32_t *>(meta_d + g.ups4_work), reinterpret_cast<const UpsImg4 *>(meta_d + g.ups4_desc), g.ups4_cta, s);
       CU(cudaEventRecord(ev[2], s));
       CU(cudaGetLastError());
     }

@@ -5022,7 +5022,28 @@ __device__ __forceinline__ void upsample_pixel(const UpsOpt &o, long long img, u
   if (o.ps == 4) d[o.off[3]] = 0xFF;
 }
 
-__global__ void __launch_bounds__(256) k_upsample_opts(UpsOpt o, uint8_t *__restrict__ pix, long long row_pitch, long long image_stride, int W, int H)
+// The 4-component form (UpsOpt4): the four components upsampled by up_one, then ycck_cmyk_convert (jdcolor.c:544-587:
+// C, M and Y are 255 minus the R, G and B of ycc_rgb_convert, range-limited, and K passes through) or null_convert, into
+// 4 bytes stored as one 32-bit word where the pixel's address is a multiple of 4.
+__device__ __forceinline__ void upsample_pixel(const UpsOpt4 &o, long long img, uint8_t *__restrict__ row, int x, int y)
+{
+  int v[4];
+#pragma unroll
+  for (int c = 0; c < 4; c++) v[c] = up_one(o.plane[c] + img * o.stride[c], o.pitch[c], o.dw[c], o.dh[c], o.hr[c], o.vr[c], o.fancy[c] != 0, x, y);
+  if (o.conv == UPS_YCCK_CMYK) {
+    const int l = v[0], u = v[1] - 128, w = v[2] - 128;
+    v[0] = 255 - min(max(l + ((91881 * w + 32768) >> 16), 0), 255);
+    v[1] = 255 - min(max(l + ((-22554 * u + 32768 - 46802 * w) >> 16), 0), 255);
+    v[2] = 255 - min(max(l + ((116130 * u + 32768) >> 16), 0), 255);
+  }
+  uint8_t *d = row + (long long)x * 4;
+  if ((reinterpret_cast<uintptr_t>(d) & 3) == 0) *reinterpret_cast<uint32_t *>(d) = (uint32_t)v[0] | (uint32_t)v[1] << 8 | (uint32_t)v[2] << 16 | (uint32_t)v[3] << 24;
+  else { d[0] = (uint8_t)v[0]; d[1] = (uint8_t)v[1]; d[2] = (uint8_t)v[2]; d[3] = (uint8_t)v[3]; }
+}
+
+// NC: 3 for UpsOpt (1- and 3-component files), 4 for UpsOpt4
+template <int NC>
+__global__ void __launch_bounds__(256) k_upsample_opts(UpsOptN<NC> o, uint8_t *__restrict__ pix, long long row_pitch, long long image_stride, int W, int H)
 {
   const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y, img = blockIdx.z;
   if (x >= W || y >= H) return;
@@ -5032,12 +5053,13 @@ __global__ void __launch_bounds__(256) k_upsample_opts(UpsOpt o, uint8_t *__rest
 // k_upsample_opts over images of different geometry and conversion: work[blockIdx.x] names the image (imgs[]) whose
 // 64 x 4 pixel tile the CTA makes, tile blockIdx.x - cta0 of its gx tiles a row; the image's sample planes are its own
 // (UpsOpt::stride unused).  The descriptor is staged in shared memory once per CTA.
-__global__ void __launch_bounds__(256) k_upsample_ragged(const uint32_t *__restrict__ work, const UpsImg *__restrict__ imgs)
+template <int NC>
+__global__ void __launch_bounds__(256) k_upsample_ragged(const uint32_t *__restrict__ work, const UpsImgN<NC> *__restrict__ imgs)
 {
-  static_assert(sizeof(UpsImg) % 4 == 0 && sizeof(UpsImg) / 4 <= 256, "UpsImg is staged one word per thread");
-  __shared__ UpsImg d;
+  static_assert(sizeof(UpsImgN<NC>) % 4 == 0 && sizeof(UpsImgN<NC>) / 4 <= 256, "UpsImg is staged one word per thread");
+  __shared__ UpsImgN<NC> d;
   const int tid = threadIdx.y * blockDim.x + threadIdx.x;
-  if (tid < (int)(sizeof(UpsImg) / 4)) reinterpret_cast<uint32_t *>(&d)[tid] = reinterpret_cast<const uint32_t *>(imgs + work[blockIdx.x])[tid];
+  if (tid < (int)(sizeof(UpsImgN<NC>) / 4)) reinterpret_cast<uint32_t *>(&d)[tid] = reinterpret_cast<const uint32_t *>(imgs + work[blockIdx.x])[tid];
   __syncthreads();
   const int t = (int)blockIdx.x - d.cta0, ty = t / d.gx;
   const int x = (t - ty * d.gx) * 64 + threadIdx.x, y = ty * 4 + threadIdx.y;
@@ -5045,16 +5067,22 @@ __global__ void __launch_bounds__(256) k_upsample_ragged(const uint32_t *__restr
   upsample_pixel(d.o, 0, d.pix + (long long)y * d.row_pitch, x, y);
 }
 
-void launch_upsample_opts(const UpsOpt &o, uint8_t *pix, size_t row_pitch, size_t image_stride, int W, int H, int n, cudaStream_t s)
+template <int NC>
+void launch_upsample_opts(const UpsOptN<NC> &o, uint8_t *pix, size_t row_pitch, size_t image_stride, int W, int H, int n, cudaStream_t s)
 {
   const dim3 cta(64, 4), grid((unsigned)((W + 63) / 64), (unsigned)((H + 3) / 4), (unsigned)n);
-  k_upsample_opts<<<grid, cta, 0, s>>>(o, pix, (long long)row_pitch, (long long)image_stride, W, H); LAUNCHED();
+  k_upsample_opts<NC><<<grid, cta, 0, s>>>(o, pix, (long long)row_pitch, (long long)image_stride, W, H); LAUNCHED();
 }
+template void launch_upsample_opts<3>(const UpsOpt &, uint8_t *, size_t, size_t, int, int, int, cudaStream_t);
+template void launch_upsample_opts<4>(const UpsOpt4 &, uint8_t *, size_t, size_t, int, int, int, cudaStream_t);
 
-void launch_upsample_ragged(const uint32_t *work, const UpsImg *imgs, unsigned ncta, cudaStream_t s)
+template <int NC>
+void launch_upsample_ragged(const uint32_t *work, const UpsImgN<NC> *imgs, unsigned ncta, cudaStream_t s)
 {
-  k_upsample_ragged<<<ncta, dim3(64, 4), 0, s>>>(work, imgs); LAUNCHED();
+  k_upsample_ragged<NC><<<ncta, dim3(64, 4), 0, s>>>(work, imgs); LAUNCHED();
 }
+template void launch_upsample_ragged<3>(const uint32_t *, const UpsImg *, unsigned, cudaStream_t);
+template void launch_upsample_ragged<4>(const uint32_t *, const UpsImg4 *, unsigned, cudaStream_t);
 
 // tj3DecodeYUVPlanes8 with do_fancy_upsampling off: the merged upsampler (4:2:0, 4:2:2 to the RGB family) and
 // int_upsample (4:4:0, 4:1:1, 4:4:1) both replicate chroma, so each pixel reads one luma and one sample of each chroma

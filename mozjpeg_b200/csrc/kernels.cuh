@@ -302,15 +302,19 @@ int launch_upsample_color(int hx, int vx, int nc, const uint8_t *const *planes, 
 // whatever the method (tab as for 1 .. 4: jddctmgr.c gives those sizes the islow-style table); image i's table at
 // tab + i * qstride entries.  out: [n][hib * size][wib * size] samples.
 void launch_idct_opts(int size, int method, const int16_t *coef, const void *tab, int qstride, uint8_t *out, int wib, int hib, int n, cudaStream_t s);
-// k_upsample_opts: per used component (nin of them) image 0's plane, pitch / stride in bytes, dw x dh real samples,
+// k_upsample_opts<NC>: per used component (nin of them) image 0's plane, pitch / stride in bytes, dw x dh real samples,
 // the replication factors hr x vr (1 or 2) after IDCT scaling, and fancy (the smoothing filter instead of
-// replication); conv the colour conversion (UPS_* of decode.cuh); ps bytes per pixel with R, G, B (or the one gray byte) at off[0..2] and
-// 0xFF at off[3] when ps is 4.
-struct UpsOpt {
-  const uint8_t *plane[3]; int pitch[3]; long long stride[3]; int dw[3], dh[3], hr[3], vr[3], fancy[3];
+// replication); conv the colour conversion (UPS_* of decode.cuh).  NC = 3 (UpsOpt): 1- and 3-component files, ps bytes
+// per pixel with R, G, B (or the one gray byte) at off[0..2] and 0xFF at off[3] when ps is 4.  NC = 4 (UpsOpt4):
+// 4-component files, conv UPS_YCCK_CMYK or UPS_COPY4, 4 bytes a pixel in component order (ps and off unused).
+template <int NC> struct UpsOptN {
+  const uint8_t *plane[NC]; int pitch[NC]; long long stride[NC]; int dw[NC], dh[NC], hr[NC], vr[NC], fancy[NC];
   int nin, conv, ps, off[4];
 };
-void launch_upsample_opts(const UpsOpt &o, uint8_t *pix, size_t row_pitch, size_t image_stride, int W, int H, int n, cudaStream_t s);
+typedef UpsOptN<3> UpsOpt;
+typedef UpsOptN<4> UpsOpt4;
+template <int NC>
+void launch_upsample_opts(const UpsOptN<NC> &o, uint8_t *pix, size_t row_pitch, size_t image_stride, int W, int H, int n, cudaStream_t s);
 
 // The pixel stage of a chunk whose images differ in geometry: the same kernels driven by a work table, one 4-byte image
 // index per CTA, and a descriptor per image.  An IDCT image: wib x hib blocks from block `coef` of the coefficient
@@ -322,8 +326,11 @@ void launch_idct_ragged(int size, int method, const int16_t *coef, const void *t
                         unsigned ncta, cudaStream_t s);
 // An upsampling / colour conversion image: its UpsOpt (planes of its own; stride unused), W x H pixels at pix,
 // row_pitch bytes apart; cta0: its first CTA, gx: its 64 x 4 pixel tiles a row.
-struct UpsImg { UpsOpt o; uint8_t *pix; long long row_pitch; int W, H, cta0, gx; };
-void launch_upsample_ragged(const uint32_t *work, const UpsImg *imgs, unsigned ncta, cudaStream_t s);
+template <int NC> struct UpsImgN { UpsOptN<NC> o; uint8_t *pix; long long row_pitch; int W, H, cta0, gx; };
+typedef UpsImgN<3> UpsImg;
+typedef UpsImgN<4> UpsImg4;
+template <int NC>
+void launch_upsample_ragged(const uint32_t *work, const UpsImgN<NC> *imgs, unsigned ncta, cudaStream_t s);
 
 // Decompression to YUV planes (jpeg_read_raw_data): the IDCT kernels above with their PLANE store, which writes image
 // i's samples straight into out + i * stride, rows `pitch` bytes apart, clipped to the first cw columns and ch rows.

@@ -261,7 +261,7 @@ extern "C" int b200jpeg_decompress_output(const b200jpeg_source_info *src, int *
 extern "C" b200jpeg_decompress_options b200jpeg_default_decompress_options(void)
 {
   b200jpeg_decompress_options o;
-  o.scale_num = 1; o.scale_denom = 1; o.dct_method = B200JPEG_DCT_ISLOW; o.do_fancy_upsampling = 1; o.out_color_space = -1; o.all_scales = 0;
+  o.scale_num = 1; o.scale_denom = 1; o.dct_method = B200JPEG_DCT_ISLOW; o.do_fancy_upsampling = 1; o.out_color_space = -1; o.all_scales = 0; o.cmyk = 0;
   return o;
 }
 
@@ -288,7 +288,7 @@ int plan_decompress(const b200jpeg_source_info &s, const b200jpeg_decompress_opt
   const int def = jcs == B200JPEG_CS_GRAYSCALE ? B200JPEG_CS_GRAYSCALE : jcs == B200JPEG_CS_YCbCr || jcs == B200JPEG_CS_RGB ? B200JPEG_CS_RGB : B200JPEG_CS_CMYK;
   const int ocs = o.out_color_space == -1 ? def : o.out_color_space;
   if (ocs < 0 || ocs > B200JPEG_CS_RGB565) { set_error("out_color_space %d is not a J_COLOR_SPACE", o.out_color_space); return B200JPEG_ERR_PARAM; }
-  const bool refuse = ocs == B200JPEG_CS_RGB565 || ((ocs == B200JPEG_CS_CMYK || ocs == B200JPEG_CS_YCCK) && o.out_color_space != -1);
+  const bool refuse = ocs == B200JPEG_CS_RGB565 || (!o.cmyk && (ocs == B200JPEG_CS_CMYK || ocs == B200JPEG_CS_YCCK) && o.out_color_space != -1);
   if (refuse) { set_error("out_color_space %d (RGB565, CMYK or YCCK output) is not on the device path", ocs); return B200JPEG_ERR_UNSUPPORTED; }
   p.out_cs = ocs;
   bool conv_ok = true;
@@ -305,10 +305,13 @@ int plan_decompress(const b200jpeg_source_info &s, const b200jpeg_decompress_opt
     else if (jcs == B200JPEG_CS_GRAYSCALE) { p.conv = UPS_GRAY_RGB; p.nin = 1; }
     else if (jcs == B200JPEG_CS_RGB) { p.conv = UPS_COPY3; p.nin = 3; }
     else conv_ok = false;
-  } else if (nc == 4 && ocs == B200JPEG_CS_CMYK) {         // the default of a CMYK / YCCK file (the batch refuses those)
-    p.out_nc = p.ps = 4; p.nin = 0;
+  } else if (ocs == B200JPEG_CS_CMYK) {                     // the default of a CMYK / YCCK file (refused without cmyk)
+    p.out_nc = p.ps = 4; p.nin = 4;
+    if (jcs == B200JPEG_CS_YCCK) p.conv = UPS_YCCK_CMYK;
+    else if (jcs == B200JPEG_CS_CMYK) p.conv = UPS_COPY4;
+    else conv_ok = false;
   } else if (ocs == jcs) {                                  // null_convert to the file's own space
-    p.out_nc = p.ps = nc; p.nin = nc; p.conv = nc == 1 ? UPS_GRAY : UPS_COPY3;
+    p.out_nc = p.ps = nc; p.nin = nc; p.conv = nc == 1 ? UPS_GRAY : nc == 4 ? UPS_COPY4 : UPS_COPY3;
     p.off[0] = 0; p.off[1] = 1; p.off[2] = 2;
   } else conv_ok = false;
   if (!conv_ok) return bad(B200JPEG_ERR_PARAM, "Unsupported color conversion request");   // JERR_CONVERSION_NOTIMPL

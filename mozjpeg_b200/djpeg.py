@@ -3,6 +3,7 @@ decompress options (djpeg.c parse_switches, with its abbreviations) and PPM / PG
 
   -scale M/N            scale_num / scale_denom: every fraction, bucketed into the block sizes 1 .. 16 as the reference
                         does (main() passes all_scales=True)
+  CMYK and YCCK files   decoded to CMYK (main() passes cmyk=True) and written as P6 the way wrppm.c's put_cmyk does
   -dct int|fast|float   dct_method
   -nosmooth             do_fancy_upsampling = FALSE
   -fast                 JDCT_IFAST and no fancy upsampling (the quantization settings it also makes need -colors)
@@ -72,8 +73,18 @@ def parse(switches: Sequence[str]) -> dict:
     return o
 
 
+def cmyk_to_rgb(px: np.ndarray) -> np.ndarray:
+    """cmyk.h cmyk_to_rgb, which wrppm.c's put_cmyk applies to CMYK output: R, G, B = C, M, Y * K / 255 + 0.5 in double
+    precision, truncated"""
+    a = np.asarray(px, dtype=np.float64)
+    return (a[..., :3] * a[..., 3:4] / 255.0 + 0.5).astype(np.uint8)
+
+
 def ppm_bytes(px: np.ndarray) -> bytes:
-    """wrppm.c's file for 8-bit samples: P5 for one component, P6 for RGB, then the rows"""
+    """wrppm.c's file for 8-bit samples: P5 for one component, P6 for RGB, P6 of cmyk_to_rgb for CMYK, then the rows"""
+    px = np.asarray(px)
+    if px.ndim == 3 and px.shape[2] == 4:
+        px = cmyk_to_rgb(px)
     px = np.ascontiguousarray(px, dtype=np.uint8)
     h, w = px.shape[:2]
     magic = "P5" if px.ndim == 2 or px.shape[2] == 1 else "P6"
@@ -116,7 +127,7 @@ def main(argv: Sequence[str] = None) -> int:
     enc = Encoder(0)
     enc.set_progressive_decode(True)          # the reference's djpeg reads progressive files too
     try:
-        px = enc.decompress([src], all_scales=True, **opts)[0]
+        px = enc.decompress([src], all_scales=True, cmyk=True, **opts)[0]
     finally:
         enc.close()
     out = ppm_bytes(px)

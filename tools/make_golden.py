@@ -475,6 +475,44 @@ def decompress_options():
     print("wrote", len(cases), "cases,", len(refused), "refused pairs")
 
 
+def cmyk():
+    """tests/golden/cmyk_golden.json: for every (source, options) of tests/cmyk_cases.py the md5 of the source, the fields
+    jpeg_calc_output_dimensions sets and the md5 of the pixels the reference decodes with those options
+    (build/librefdecopt.so, which takes 4 output components), the reference's message for each refused colour pair, and
+    for every recompress case the md5 and size of what the reference's cjpeg writes from the file."""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import cmyk_cases as K
+    import decompress_options_cases as O
+    import recompress_cases as R
+    if not (O.have_reference() and R.have_reference()):
+        sys.exit("build/librefdecopt.so or oracle/_ref/cjpeg is missing: run __graft_entry__.build() with the reference build under oracle/_ref/")
+    sources = [{"id": sid, "md5": K.md5(K.source(sid))} for sid in [c[0] for c in K.SOURCES] + ["cmyk_markers", "ycck_markers"]]
+    cases = []
+    for cid, sid, scale, dct, fancy, cs in K.cases():
+        src = K.source(sid)
+        px, info, msg = O.ref_decompress(src, K.opts_tuple(scale, dct, fancy, cs))
+        if px is None:
+            sys.exit(f"{cid}: the reference refuses it: {msg}")
+        cases.append({"id": cid, "src_md5": K.md5(src), "pix_md5": K.md5(px), "shape": list(px.shape), "out_color_space": info[3],
+                      "jpeg_color_space": info[4], "components": [info[7 + 3 * c:10 + 3 * c] for c in range(info[6])], "warnings": info[5]})
+    refused = []
+    for sid, cs in K.REFUSED_PAIRS:
+        _, _, msg = O.ref_decompress(K.source(sid), (1, 1, 0, 1, cs), header_only=True)
+        refused.append({"source": sid, "out_color_space": cs, "message": msg})
+    rec = []
+    for rid, sid, sw in K.RECOMPRESS:
+        out = R.ref_cjpeg(K.source(sid), sw)
+        rec.append({"id": rid, "source": sid, "switches": sw, "md5": K.md5(out), "size": len(out)})
+    # djpeg's PPM of a YCCK file: the reference's CMYK pixels through wrppm.c put_cmyk (cmyk.h cmyk_to_rgb, in double)
+    px, _, _ = O.ref_decompress(K.source("ycck_420"), (1, 1, 0, 1, -1))
+    rgb = bytes(int(float(v) * float(k) / 255.0 + 0.5) for row in px.tolist() for *cmy, k in row for v in cmy)
+    ppm = {"ycck_420": K.md5(b"P6\n%d %d\n255\n" % (px.shape[1], px.shape[0]) + rgb)}
+    json.dump({"generator": "tools/make_golden.py --cmyk", "reference": "mozilla/mozjpeg 5.0.0 (C path, WITH_SIMD=0), oracle/_ref",
+               "sources": sources, "cases": cases, "refused_pairs": refused, "recompress": rec, "djpeg_ppm": ppm},
+              open(os.path.join(GOLD, "cmyk_golden.json"), "w"), indent=0)
+    print("wrote", len(cases), "cases,", len(refused), "refused pairs,", len(rec), "recompress cases")
+
+
 def idct_scaling():
     """tests/golden/idct_scaling_golden.json: for every (source, options) of tests/idct_scaling_cases.py what
     --decompress-options records (build/librefdecopt.so), and the reference's tj3DecompressToYUVPlanes8 planes
@@ -554,6 +592,8 @@ def progressive():
 
 
 def main():
+    if "--cmyk" in sys.argv:
+        return cmyk()
     if "--progressive" in sys.argv:
         return progressive()
     if "--idct-scaling" in sys.argv:

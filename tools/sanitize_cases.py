@@ -93,6 +93,14 @@ for k in NEW:
 n += len(enc.decompress_mixed([rag[0], srcs[0]], [dict(scale=(k, 8), all_scales=True) for k in NEW])[0])
 for f in ((3, 8), (5, 8), (3, 4), (7, 8), (9, 8), (5, 4), (11, 8), (3, 2), (13, 8), (7, 4), (15, 8), (2, 1)):
     n += len(enc.decompress_yuv(rag, scale=f, all_scales=True))
+# CMYK and YCCK sources (cmyk): k_upsample_opts<4> through the one-geometry form, k_upsample_ragged<4> through a mixed
+# batch with a 3-component file, at ragged sizes with the 2:1 edge rules
+cm = enc.encode_batch(mj.tj3_params(61, 37, subsamp="444", cmyk=True, colorspace=mj._abi.CS_CMYK), np.stack([synth_image(13, 61, 37)[..., [0, 1, 2, 0]]] * 2))
+yk = enc.encode_batch(mj.tj3_params(67, 35, subsamp="420", cmyk=True), np.stack([synth_image(14, 67, 35)[..., [0, 1, 2, 1]]] * 2))
+for f in (cm, yk):
+    n += len(enc.decompress(f, cmyk=True))
+    n += len(enc.decompress(f, scale=(1, 2), dct="fast", fancy=False, cmyk=True))
+n += len(enc.decompress_mixed([cm[0], yk[0], rag[0]], [dict(cmyk=True), dict(scale=(1, 4), cmyk=True)])[0])
 # progressive decode: the default profile (scan search, successive approximation), the standard script with restarts,
 # mixed with sequential files, through the coefficient, transcode and pixel routes; then a truncated refinement scan
 enc.set_progressive_decode(True)
